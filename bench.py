@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- images/s of the ctdet heat-map decode hot path (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One step = one ctdet_decode pass (3x3 peak-NMS + top-K + wh/reg gather + box assembly)
@@ -12,8 +12,10 @@ own 64-image shard, no data-path collective (SURVEY.md section 8e).
 Prints ONE JSON line (rank 0).  `value` = device-resident throughput (CUDA events, max
 over ranks); `e2e` = same metric through the public API with pinned HOST buffers, the
 H2D of the heat/wh/reg batch and the D2H of the detections inside the timed region;
-`roofline` = algorithmic bytes / device time against MEASURED_PEAKS.json;
+`roofline` = algorithmic bytes / device time against MEASURED_PEAKS.json (else the H100 SXM data sheet);
 `cpu_baseline` = the CPU port of the reference path on a bounded sample.
+`--dump-outputs DIR` writes what the last timed step returned, DIR/dets.npy ([64, K, 6] float32: x1, y1, x2,
+y2, score, class), so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -31,8 +33,7 @@ METRIC = "images/sec ctdet 512x512->128x128x80 heatmap decode K=100"
 UNIT = "images/s"
 B_PER_GPU, C, H, W, K = 64, 80, 128, 128, 100
 ALG_BYTES_PER_IMAGE = C * H * W * 4 + K * 4 * 4 + K * 6 * 4   # SURVEY.md section 8d: 5,246,880 B
-N_ROT = 3                                                      # rotating input batches (3 x 352 MB >> 126 MB L2)
-NCU_TRAFFIC_BYTES = 341761536 + 3631360                        # measured DRAM read + write of one launch (profiles/r2)
+N_ROT = 3                                                      # rotating input batches (3 x 352 MB >> 50 MB L2)
 
 
 def workload_config(world):
@@ -106,7 +107,7 @@ def synth(batch, device, seed):
 
 
 class ClockSampler(threading.Thread):
-    """Samples SM clock / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples SM clock / throttle reasons during the timed region through NVML."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -138,14 +139,15 @@ class ClockSampler(threading.Thread):
                     for bit, name in names.items():
                         if r & bit:
                             self.reasons.add(name)
-                if not self.recording:
-                    time.sleep(0.0005)          # back-to-back NVML reads (~50 us each) inside the timed region
+                # sleep between reads, inside the timed region too: a polling loop holds the GIL often enough to
+                # slow the launching thread to the GPU's pace, which starves the GPU and spreads short runs widely
+                time.sleep(0.001 if self.recording else 0.0005)
         except Exception as e:  # no NVML: report that instead of inventing numbers
             self.reasons.add("nvml_unavailable:%s" % type(e).__name__)
             self.alive.set()
 
     def force_sample(self):
-        """One synchronous sample (the driver's 20-step region lasts < 2 ms, shorter than a scheduling quantum)."""
+        """One synchronous sample (a 20-step timed region lasts a few ms: it may hold no periodic sample at all)."""
         self.sample_now = True
         t0 = time.perf_counter()
         while self.sample_now and time.perf_counter() - t0 < 0.05 and self.is_alive():
@@ -164,7 +166,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 def cpu_port_rate(batch, repeats, threads):
@@ -242,7 +244,11 @@ def main():
                     help="pin the rank to its GPU's NUMA node before allocating (default: only when world > 1)")
     ap.add_argument("--no-bind-numa", dest="bind_numa", action="store_false")
     ap.add_argument("--no-secondary", action="store_true", help="skip the per-kernel secondary measurements (N=1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the detections of the last timed step to DIR/dets.npy (float32), rank 0")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1 (the timed region is the steps)")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -301,6 +307,10 @@ def main():
     sampler.force_sample()
     launches = CL.launch_count() - l0
     ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "dets.npy"), dets.float().cpu().numpy())
     sampler.stop_flag = True
     sampler.join(timeout=2)
     t = torch.tensor([ms], device=dev)
@@ -406,9 +416,7 @@ def main():
             "config": workload_config(world),
             "per_rank_ms_per_step": [round(m / args.steps, 5) for m in per_rank_ms],
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": NCU_TRAFFIC_BYTES, "peak_source": peak_src,
-                         "traffic_source": "profiles/r2_select_hot_summary.csv (ncu --set full: "
-                                           "dram__bytes_read.sum + dram__bytes_write.sum, one launch)",
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "kernel": "k_select_hot (the whole decode call is this one launch)",
                          "alg_bytes_per_launch": ALG_BYTES_PER_IMAGE * B_PER_GPU},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
@@ -416,7 +424,7 @@ def main():
                     "h2d_gbs_per_rank": h2d_gbs_per_rank if args.e2e_steps > 0 else None,
                     "h2d_probe_gbs": round(h2d_probe, 2) if args.e2e_steps > 0 else None, "host_binding": numa,
                     "bound_by": "PCIe Gen5 x16 host->device copy of the fp32 heat/wh/reg batch (352 MB per step, "
-                                "pinned, chunked and overlapped with the decode); the decode itself is ~1% of it"},
+                                "pinned, chunked and overlapped with the decode)"},
             "gpu_launches": int(launches),
             "secondary": secondary,
             "clocks": sampler.summary(),

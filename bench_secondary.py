@@ -18,7 +18,7 @@ def _peaks():
         j = json.load(open(p))
         return float(j["hbm_gbs"]), float(j["bf16_tflops"]), "measured"
     except Exception:
-        return 6650.0, 1590.0, "fallback"
+        return 3350.0, 989.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16)"
 
 
 def timeit(fn, iters=20, warm=3):
@@ -177,7 +177,7 @@ def run(dev, batches, K=100, steps=20):
             fn = DCNv2Function(1, 1, 1, 1)
             flops = 2.0 * co * ci * 9 * hh * hh * b
             ms = timeit(lambda: fn(x, off, msk, w, bias), steps)
-            r = _tensor(ms, flops, tf, src, config="DCNv2 forward B=%d %d@%dx%d->%d (tcgen05, 3xTF32)" % (b, ci, hh, hh, co))
+            r = _tensor(ms, flops, tf, src, config="DCNv2 forward B=%d %d@%dx%d->%d (wgmma, 3xTF32)" % (b, ci, hh, hh, co))
             alg = b * ((ci + 27) * hh * hh * 4 + co * hh * hh * 4) + co * ci * 36
             r["hbm_frac"] = round(alg / (ms * 1e-3) / 1e9 / hbm, 4)
             leaves = [t.clone().requires_grad_(True) for t in (x, off, msk, w, bias)]
@@ -187,7 +187,7 @@ def run(dev, batches, K=100, steps=20):
                     t.grad = None
                 fn(*leaves).sum().backward()
             r["fwd_bwd_ms"] = round(timeit(fb, max(5, steps // 4), 2), 5)
-            # the backward alone (tcgen05: column-gradient GEMM + weight-gradient GEMM = twice the forward's flops)
+            # the backward alone (wgmma: column-gradient GEMM + weight-gradient GEMM = twice the forward's flops)
             bwd_ms = max(r["fwd_bwd_ms"] - ms, 1e-6)
             r["backward"] = _tensor(bwd_ms, 2.0 * flops, tf, src,
                                     config="DCNv2 backward (fwd_bwd_ms - forward; dX by 16-byte vector reductions, the other "
@@ -304,8 +304,7 @@ def run_allreduce(dev, world, rank, steps=10):
     return {"grad_allreduce_dla34": {
         "bytes": nbytes, "params": nparam, "buckets": n_buckets, "allreduce_ms": round(ms_ar, 4),
         "bus_bandwidth_gbs": round(busbw, 1),
-        "nvlink_reference": "725 GB/s bus bandwidth of an 8-rank all-reduce at 1 GiB (B200_PROFILING.md); a 78.7 MB "
-                            "message in 4 buckets is latency-dominated",
+        "note": "a 78.7 MB message in 4 buckets is latency-dominated",
         "step_ms_no_exchange": round(ms_none, 4), "step_ms_exchange_after_backward": round(ms_seq, 4),
         "step_ms_overlapped": round(ms_ovl, 4),
         "exposed_exchange_ms": round(ms_ovl - ms_none, 4),

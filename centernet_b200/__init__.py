@@ -1,4 +1,4 @@
-"""centernet_b200 -- B200-native (sm_100a) CenterNet heat-map hot path.
+"""centernet_b200 -- H100-native (sm_90a) CenterNet heat-map hot path.
 
 Host-side mirror of the reference operator interface:
 

@@ -1,10 +1,10 @@
-"""Builds the sm_100a CUDA library and its pybind11 layer IN-TREE.
+"""Builds the sm_90a CUDA library and its pybind11 layer IN-TREE.
 
   centernet_b200/lib/libcenternet_b200.so   <- nvcc, every csrc/*.cu   (the C ABI)
   centernet_b200/_C<ext>.so                 <- g++,  csrc/pybind.cpp    (thin binding)
 
-Run as ``python -m centernet_b200.build`` (add ``--force`` to rebuild).  nvcc
-cross-compiles without a GPU, so this also runs in the CPU-only build container.
+Run as ``python centernet_b200/build.py`` (add ``--force`` to rebuild; the package itself
+cannot be imported before the extension exists).  nvcc cross-compiles without a GPU.
 """
 import glob
 import os
@@ -18,7 +18,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libcenternet_b200.so")
 EXT = os.path.join(HERE, "_C" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-cudart", "static"] + os.environ.get("CNB_NVCC_DEFINES", "").split()
 
 

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the centernet_b200 kernels (sm_100a only).
+// Shared device/host helpers for the centernet_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,8 +9,8 @@
 #include <atomic>
 #include "../../include/centernet_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "centernet_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900 || !defined(__CUDA_ARCH_FEAT_SM90_ALL))
+#error "centernet_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace cnb {
@@ -48,9 +48,9 @@ inline void count_launch(int n = 1) { g_launches.fetch_add((unsigned long long)n
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 inline int num_sms() {
-  int dev = 0, n = 148;
+  int dev = 0, n = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n > 0 ? n : 148;
+  return n > 0 ? n : 132;
 }
 
 // ---------------------------------------------------------------- device side

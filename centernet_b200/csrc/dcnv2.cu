@@ -15,7 +15,7 @@
 //      memory straight from x (gathers hit L1/L2; the column matrix never touches HBM);
 //   3. the chunk is contracted against the matching weight slice [8*KT][Cout_tile] with an 8x4
 //      register tile per thread (fp32 FMA -- bit-compatible accumulation precision with the
-//      reference SGEMM; the tcgen05 path is the next step, see DESIGN.md);
+//      reference SGEMM; the tensor-core path is dcnv2_tc.cu);
 //   4. bias + store, coalesced along pixels.
 // Backward: k_dcn_bwd_data recomputes the sampling per pixel tile, contracts grad_out with W^T
 // chunk by chunk and turns the column gradient into dX (atomicAdd scatter, as the reference),
@@ -516,7 +516,7 @@ using namespace cnb;
 extern "C" {
 
 // No column / ones scratch (the reference's `columns`, `ones`): the workspace holds the weights re-tiled
-// (TF32 hi/lo split, UMMA layout) and a channels-last copy of the input for the tensor-core forward.  Passing workspace == NULL
+// (TF32 hi/lo split, wgmma K-major layout) and a channels-last copy of the input for the tensor-core forward.  Passing workspace == NULL
 // (or too small) to cnb_dcnv2_forward selects the fp32 CUDA-core kernel instead.
 size_t cnb_dcnv2_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw, int stride, int pad, int dil,
                                  int dg) {

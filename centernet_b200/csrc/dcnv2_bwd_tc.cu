@@ -1,11 +1,11 @@
-// DCNv2 backward with both dense contractions on the 5th-generation tensor cores (tcgen05 / UMMA, 3xTF32).
+// DCNv2 backward with both dense contractions on the Hopper tensor cores (wgmma, 3xTF32).
 // Reference: dcn_v2_cuda.c:104-241 (per sample: SGEMM columns = W^T . dY, col2im_coord, col2im, im2col again,
 // SGEMM dW += dY . columns^T, SGEMV dBias) and dcn_v2_im2col_cuda.cu:182-312.
 //
 // The column gradient
 //     dcol[b][p][q = (channel block, tap)][32 ch] = sum_o dY[b][o][p] * W[o][ch][tap]
-// is a plain GEMM (M = pixels, N = Cin*9, K = Cout).  k_dcn_bwd_dcol_tc runs it as a persistent TMA -> UMMA ->
-// TMEM pipeline (both operands arrive pre-split into TF32 hi/lo tiles; no thread touches an operand) and writes
+// is a plain GEMM (M = pixels, N = Cin*9, K = Cout).  k_dcn_bwd_dcol_tc runs it as a persistent TMA -> wgmma
+// pipeline (both operands arrive pre-split into TF32 hi/lo tiles; no thread touches an operand) and writes
 // dcol channels-last, so that everything after it moves whole 128-byte lines:
 //   k_dcn_bwd_offmask   one (tap, 4 pixels) per warp, lane = (pixel, 4-channel quad): reads the dcol line and the
 //                       four bilinear corner lines of the channels-last input, reduces dMask / dOffset over the
@@ -15,7 +15,8 @@
 //   k_dcn_bwd_dx_nchw   adds the channels-last dX into the caller's NCHW gradient
 // The weight gradient dW[o][ch][tap] = sum_{b,p} dY[b][o][p] * col[b][p][ch][tap] is a GEMM with K = pixels:
 // k_dcn_bwd_weight_tc rebuilds the masked column tile in shared memory exactly as the forward sampler does
-// (never in HBM), keeps a [128 rows = 4 chunks x 32 ch] x Cout accumulator in TMEM over its whole pixel range and
+// (never in HBM), keeps a [128 rows = 4 chunks x 32 ch] x (64|128 output channels) accumulator in the registers of two
+// warpgroups over its whole pixel range and
 // writes one partial per CTA; k_dcn_bwd_wreduce adds the partials in a fixed order (deterministic).
 #include <stdlib.h>
 #include "dcnv2_tc.cuh"
@@ -25,12 +26,12 @@ namespace cnb {
 constexpr int BW_STAGES = 3;
 constexpr int BW_STAGE_BYTES = 4 * TC_A_BYTES;     // A hi, A lo, B hi, B lo: 4 x (128 rows x 32 k x 4 B) = 64 KB
 constexpr int BW_TILE_FLOATS = 2 * TC_TP * TC_K;   // one operand tile, hi + lo
-constexpr int BW_THREADS = 192;                    // warps 0-3 epilogue, 4 MMA, 5 TMA
+constexpr int BW_THREADS = (4 * TC_MMA_WGS + 1) * 32;   // warps 0-7 two consumer warpgroups (MMA + epilogue), 8 TMA
 
 struct BwdGeom {
   int KS;      // 32-wide slices of Cout (K of the dcol GEMM)
   int Q;       // chunks (channel block, tap) = nb * 9
-  int RG;      // groups of 4 chunks = 128 UMMA rows
+  int RG;      // groups of 4 chunks = 128 GEMM rows
   int Qp;      // RG * 4: chunk pitch of dcol
   int tiles;   // pixel tiles per image
 };
@@ -91,48 +92,18 @@ __global__ void __launch_bounds__(256) k_bwd_prep_gy(const float *__restrict__ g
   }
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(da), "l"(db), "r"(idesc),
-               "r"(acc) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,"
-      "%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 // ------------------------------------------------------------------ dcol = dY^T . W   (item = image, pixel tile, row group)
 __global__ void __launch_bounds__(BW_THREADS, 1)
 k_dcn_bwd_dcol_tc(const float *__restrict__ gyt, const float *__restrict__ wtt, float *__restrict__ dcol,
                   const DcnShapeTc s, const BwdGeom g, const int n_items) {
   extern __shared__ __align__(128) unsigned char tc_smem[];
-  __shared__ __align__(8) uint64_t full[BW_STAGES], empty[BW_STAGES], tm_full[2], tm_empty[2];
-  __shared__ uint32_t tmem_base;
+  __shared__ __align__(8) uint64_t full[BW_STAGES], empty[BW_STAGES];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
-    for (int i = 0; i < BW_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tm_full[i], 1); mbar_init(&tm_empty[i], TC_EPI_WARPS); }
+    for (int i = 0; i < BW_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TC_MMA_WGS); }
     mbar_fence_init();
   }
-  if (warp == TC_WARP_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base)), "n"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tm = tmem_base;
 
   if (warp == TC_WARP_TMA) {
     if (lane == 0) {
@@ -152,83 +123,49 @@ k_dcn_bwd_dcol_tc(const float *__restrict__ gyt, const float *__restrict__ wtt, 
         }
       }
     }
-  } else if (warp == TC_WARP_MMA) {
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(TC_TP >> 4) << 24);
-      int stage = 0, ph = 0, acc = 0, aph = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        mbar_wait(&tm_empty[acc], (uint32_t)(aph ^ 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d_tmem = tm + (uint32_t)(acc * 128);
-        for (int ks = 0; ks < g.KS; ++ks) {
-          mbar_wait(&full[stage], (uint32_t)ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t ah = smem_u32(tc_smem + (size_t)stage * BW_STAGE_BYTES), al = ah + TC_A_BYTES;
-          const uint32_t bh = al + TC_A_BYTES, bl = bh + TC_A_BYTES;
-#pragma unroll
-          for (int k8 = 0; k8 < TC_K / 8; ++k8) {
-            const uint32_t koff = (uint32_t)k8 * 2u * TC_LBO;
-            const uint64_t dah = tc_desc(ah + koff), dal = tc_desc(al + koff);
-            const uint64_t dbh = tc_desc(bh + koff), dbl = tc_desc(bl + koff);
-            umma_tf32(d_tmem, dal, dbh, idesc, (ks > 0 || k8 > 0) ? 1u : 0u);   // lo * hi  (small terms first)
-            umma_tf32(d_tmem, dah, dbl, idesc, 1u);                             // hi * lo
-            umma_tf32(d_tmem, dah, dbh, idesc, 1u);                             // hi * hi
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == BW_STAGES) { stage = 0; ph ^= 1; }
-        }
-        umma_commit(&tm_full[acc]);
-        if (++acc == 2) { acc = 0; aph ^= 1; }
-      }
-    }
-  } else {
-    // epilogue: TMEM lane = pixel, 32 columns = the 32 channels of one chunk = one 128-byte line of dcol.  A thread
-    // holding a whole line would make every store instruction touch 32 lines (16 bytes each); the warp's 32 x 128 B
-    // block goes through shared memory instead (16-byte chunks XOR-swizzled by the pixel: conflict-free both ways)
-    // and leaves as 8 stores of 4 complete lines.
-    const int qw = warp;
+  } else if (warp < TC_WARP_TMA) {
+    // consumers: warpgroup wgi computes pixels 64 wgi .. 64 wgi + 63 of the tile x the 128 columns (4 chunks x 32 ch)
+    // of the row group, then stores them straight from the registers: per row a thread holds 2 adjacent channels of
+    // every 8, so a warp's store covers 8 pixels x 32 contiguous bytes
+    const int wgi = warp >> 2, wq = warp & 3;
     const long long HWo = (long long)s.Ho * s.Wo;
-    unsigned char *stg = tc_smem + (size_t)BW_STAGES * BW_STAGE_BYTES + (size_t)qw * 4096;
-    const int ej = lane >> 3, ec = lane & 7;
-    int acc = 0, aph = 0;
+    int stage = 0, ph = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
       const int rg = item % g.RG, bt = item / g.RG;
       const int t = bt % g.tiles, b = bt / g.tiles;
       const int ty0 = (t / s.tiles_x) * s.th, tx0 = (t % s.tiles_x) * s.tw;
-      float *dimg = dcol + (long long)b * HWo * g.Qp * TC_CB + (long long)rg * 4 * TC_CB + ec * 4;
-      mbar_wait(&tm_full[acc], (uint32_t)aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t taddr = tm + ((uint32_t)(qw * 32) << 16) + (uint32_t)(acc * 128);
-#pragma unroll 1
-      for (int ql = 0; ql < 4; ++ql) {
-        uint32_t v[32];
-        tmem_ld32(taddr + (uint32_t)(ql * 32), v);
+      float d[64];
 #pragma unroll
-        for (int c = 0; c < 8; ++c)
-          *reinterpret_cast<float4 *>(stg + lane * 128 + ((c ^ (lane & 7)) << 4)) =
-              make_float4(__uint_as_float(v[4 * c]), __uint_as_float(v[4 * c + 1]), __uint_as_float(v[4 * c + 2]),
-                          __uint_as_float(v[4 * c + 3]));
-        __syncwarp();
+      for (int i = 0; i < 64; ++i) d[i] = 0.f;
+      for (int ks = 0; ks < g.KS; ++ks) {
+        mbar_wait(&full[stage], (uint32_t)ph);
+        const uint32_t base = smem_u32(tc_smem + (size_t)stage * BW_STAGE_BYTES);
+        const uint32_t ah = base + (uint32_t)wgi * 8u * TC_SBO, al = ah + TC_A_BYTES;
+        const uint32_t bh = base + 2u * TC_A_BYTES, bl = bh + TC_A_BYTES;
+        wgmma_fence();
 #pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int pl = it * 4 + ej;                       // pixel within the warp's 32
-          const float4 val = *reinterpret_cast<const float4 *>(stg + pl * 128 + ((ec ^ (pl & 7)) << 4));
-          const int pp = qw * 32 + pl;
-          const int ho = ty0 + pp / s.tw, wo = tx0 + pp % s.tw;
-          if (ho < s.Ho && wo < s.Wo)
-            *reinterpret_cast<float4 *>(dimg + ((long long)ho * s.Wo + wo) * g.Qp * TC_CB + ql * TC_CB) = val;
+        for (int k8 = 0; k8 < TC_K / 8; ++k8) {
+          const uint32_t koff = (uint32_t)k8 * 2u * TC_LBO;
+          wgmma_3xtf32<128>(d, tc_desc(ah + koff), tc_desc(al + koff), tc_desc(bh + koff), tc_desc(bl + koff),
+                            (ks > 0 || k8 > 0) ? 1u : 0u);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait_all();
+        if ((tid & 127) == 0) mbar_arrive_tc(&empty[stage]);
+        if (++stage == BW_STAGES) { stage = 0; ph ^= 1; }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive_tc(&tm_empty[acc]);
-      if (++acc == 2) { acc = 0; aph ^= 1; }
+      float *dimg = dcol + (long long)b * HWo * g.Qp * TC_CB + (long long)rg * 4 * TC_CB + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int pp = wgi * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        const int ho = ty0 + pp / s.tw, wo = tx0 + pp % s.tw;
+        if (ho >= s.Ho || wo >= s.Wo) continue;
+        float *dp = dimg + ((long long)ho * s.Wo + wo) * g.Qp * TC_CB;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) *reinterpret_cast<float2 *>(dp + 8 * j) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+      }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == TC_WARP_MMA) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tm), "n"(256));
 }
 
 // ------------------------------------------------------------------ dMask / dOffset (+ the dX scatter)
@@ -589,41 +526,42 @@ __global__ void __launch_bounds__(256) k_dcn_bwd_dx_nchw(const float *__restrict
 }
 
 // ------------------------------------------------------------------ dW = dY . col^T   (K = pixels)
-constexpr int WG_SAMPLERS = 16;
-constexpr int WG_GEOM = 4;                                    // warps 0-3: geometry producers (4 taps x 32 pixels per slice), then epilogue
+constexpr int WG_SAMPLERS = 8;                                // sampler warps, 4 tasks each (2 rounds of 2)
+constexpr int WG_TASKS = 32 / WG_SAMPLERS;
+constexpr int WG_GEOM = 4;                                    // warps 0-3: geometry producers (4 taps x 32 pixels per slice)
 constexpr int WG_MR = 4;                                      // slices of geometry in flight
-constexpr int WG_THREADS = (TC_WARP_S0 + WG_SAMPLERS) * 32;   // warps 0-3 geometry + epilogue, 4 MMA, 5 TMA, 6-21 samplers
+constexpr int WG_WARP_C0 = 4;                                 // warps 4-11: two consumer warpgroups (MMA + epilogue)
+constexpr int WG_WARP_S0 = WG_WARP_C0 + 4 * TC_MMA_WGS;       // warps 12-19: samplers; lane 0 of warp 12 also issues the
+                                                              // dY tile copies (TMA) of each stage it has seen drained
+constexpr int WG_THREADS = (WG_WARP_S0 + WG_SAMPLERS) * 32;   // 640: leaves the consumers 96+ registers
 constexpr uint32_t WG_SBO = 1040;                             // pitch of the A tile's 8-row groups (bank-conflict-free scalar stores)
 constexpr int WG_A_BYTES = (TC_TP / 8) * WG_SBO;              // 16640 per hi / lo tile
-__device__ __forceinline__ uint64_t wg_desc_a(uint32_t addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr >> 4) & 0x3fff);
-  d |= (uint64_t)((TC_LBO >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((WG_SBO >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
+constexpr int WG_STAGES = 3;
 
 struct WgGeom {
-  int co_r;          // Cout rounded up to 16 (UMMA N)
+  int co_r;          // Cout rounded up to 64, or to 128 above 64: a whole number of N tiles
+  int nt;            // output channels per CTA (wgmma N): 64 or 128
+  int n_nt;          // N tiles (CTAs per row group and split)
   int spi;           // 32-pixel slices per image
   int n_slices;      // B * spi
   int splits;        // pixel-range splits (CTAs per row group)
   int stages;
-  int stage_bytes;   // 2 * WG_A_BYTES + 2 * co_r * 128
+  int stage_bytes;   // 2 * WG_A_BYTES + 2 * nt * 128
   unsigned wo_magic; // floor(2^32 / Wo) + 1: p / Wo == umulhi(p, magic) for p < 2^32 / Wo; 0 = divide
 };
 static WgGeom wg_geom(const DcnShapeTc &s, const BwdGeom &g) {
   WgGeom w;
-  w.co_r = (s.Cout + 15) / 16 * 16;
+  w.co_r = s.Cout <= 64 ? 64 : (s.Cout + 127) / 128 * 128;
+  w.nt = w.co_r == 64 ? 64 : 128;
+  w.n_nt = w.co_r / w.nt;
   w.spi = (int)(((long long)s.Ho * s.Wo + TC_K - 1) / TC_K);
   w.n_slices = s.B * w.spi;
-  int splits = num_sms() / g.RG;          // one CTA per SM at most (a CTA owns ~200 KB of shared memory): no second wave
+  int splits = num_sms() / (g.RG * w.n_nt);   // one CTA per SM at most (a CTA owns ~200 KB of shared memory): no second wave
   if (splits > w.n_slices) splits = w.n_slices;
   if (splits < 1) splits = 1;
   w.splits = splits;
-  w.stage_bytes = 2 * WG_A_BYTES + 2 * w.co_r * TC_K * 4;
-  w.stages = w.stage_bytes <= 66048 ? 3 : 2;
+  w.stage_bytes = 2 * WG_A_BYTES + 2 * w.nt * TC_K * 4;
+  w.stages = WG_STAGES;
   w.wo_magic = ((unsigned long long)s.Ho * s.Wo * s.Wo < (1ull << 32)) ? (unsigned)((1ull << 32) / (unsigned)s.Wo + 1) : 0u;
   return w;
 }
@@ -669,50 +607,47 @@ __global__ void __launch_bounds__(256) k_dcn_bwd_bias_reduce(const float *__rest
   if (threadIdx.x == 0) gb[o] += red[0];
 }
 
-// CTA = (row group rg = 4 chunks x 32 channels, split): D[128 rows][Cout] accumulates over the CTA's slices in TMEM.
+// CTA = (row group rg = 4 chunks x 32 channels, N tile, split): D[128 rows][NT output channels] accumulates over the
+// CTA's slices in the registers of two consumer warpgroups (64 rows each).
+template <int NT>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 k_dcn_bwd_weight_tc(const float *__restrict__ xt, const float *__restrict__ offset, const float *__restrict__ mask,
                     const float *__restrict__ gyk, float *__restrict__ wpart, const DcnShapeTc s, const BwdGeom g,
                     const WgGeom wg) {
   extern __shared__ __align__(128) unsigned char tc_smem[];
-  __shared__ __align__(8) uint64_t a_full[3], b_full[3], empty[3], tm_full, m_full[WG_MR], m_empty[WG_MR];
-  __shared__ uint32_t tmem_base;
+  __shared__ __align__(8) uint64_t a_full[WG_STAGES], b_full[WG_STAGES], empty[WG_STAGES], m_full[WG_MR], m_empty[WG_MR];
   __shared__ BwdMetaTc wmeta[WG_MR][128];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int rg = blockIdx.x % g.RG, split = blockIdx.x / g.RG;
+  const int rg = blockIdx.x % g.RG, nti = (blockIdx.x / g.RG) % wg.n_nt, split = blockIdx.x / g.RG / wg.n_nt;
   const int sl0 = (int)((long long)split * wg.n_slices / wg.splits), sl1 = (int)((long long)(split + 1) * wg.n_slices / wg.splits);
   const int KT = s.kh * s.kw;
   const long long HWo = (long long)s.Ho * s.Wo, HW = (long long)s.H * s.W;
   const int Cp = s.nb * TC_CB;
-  const int b_bytes = wg.co_r * TC_K * 4;
+  const int b_bytes = NT * TC_K * 4;                 // the CTA's N tile of one hi or lo dY tile
 
   if (tid == 0) {
-    for (int i = 0; i < 3; ++i) { mbar_init(&a_full[i], WG_SAMPLERS); mbar_init(&b_full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(&tm_full, 1);
+    for (int i = 0; i < WG_STAGES; ++i) {
+      mbar_init(&a_full[i], WG_SAMPLERS);
+      mbar_init(&b_full[i], 1);
+      mbar_init(&empty[i], TC_MMA_WGS);
+    }
     for (int i = 0; i < WG_MR; ++i) { mbar_init(&m_full[i], WG_GEOM); mbar_init(&m_empty[i], WG_SAMPLERS); }
     mbar_fence_init();
   }
-  if (warp == TC_WARP_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base)), "n"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tm = tmem_base;
 
-  if (warp >= TC_WARP_S0) {
+  if (warp >= WG_WARP_S0) {
     // =========================================================== samplers: the masked column tile, rows = channels
     // task = (chunk ql, 4 pixels): lane = (pixel j, channel quad c4) gathers 4 corners x 16 bytes and stores its
     // 4 channels x 1 pixel as scalars -- the 8-row groups of the A tile are pitched WG_SBO = 1040 bytes so that the 32
     // lanes of a store hit 32 different banks.  Warps run free of each other: the geometry comes through a ring, the
-    // tile goes out through the 3-stage A ring.
-    const int sw = warp - TC_WARP_S0;
+    // tile goes out through the 3-stage A ring.  A warp's WG_TASKS tasks run in rounds of two.
+    const int sw = warp - WG_WARP_S0;
     const int j = lane >> 3, c4 = lane & 7;
-    int t_meta[2], t_xc[2];
-    uint32_t t_dst[2];
+    int t_meta[WG_TASKS], t_xc[WG_TASKS];
+    uint32_t t_dst[WG_TASKS];
 #pragma unroll
-    for (int it = 0; it < 2; ++it) {
+    for (int it = 0; it < WG_TASKS; ++it) {
       const int task = sw + it * WG_SAMPLERS;      // chunk ql = task / 8, pixel group pg = task % 8
       const int ql = task >> 3, pg = task & 7;
       const int q = rg * 4 + ql;
@@ -725,99 +660,107 @@ k_dcn_bwd_weight_tc(const float *__restrict__ xt, const float *__restrict__ offs
     const int xs1 = Cp, xs2 = s.W * Cp, xs3 = (s.W + 1) * Cp;
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
     int stage = 0, ph = 0, ms = 0, mph = 0;
-    int b = sl0 / wg.spi, sll = sl0 - b * wg.spi;      // image and slice within the image (of the slice being LOADED)
-    BwdMetaTc mt[2];
-    float4 xc[2][4];
-    // take the geometry of the next slice from the ring and issue its eight corner loads (a corner that is out of range,
-    // or a sample that is outside altogether -- all four flags clear, weights zero -- is simply not loaded)
-    auto load_slice = [&]() {
+    int b = sl0 / wg.spi, sll = sl0 - b * wg.spi;      // image and slice within the image
+    const size_t tile_bytes = (size_t)wg.co_r * TC_K * 4;          // one hi or lo dY tile, all output channels
+    for (int sl = sl0; sl < sl1; ++sl) {
+      // take the geometry of the slice from the ring (a corner that is out of range, or a sample that is outside
+      // altogether -- all four flags clear, weights zero -- is simply not loaded)
       mbar_wait(&m_full[ms], (uint32_t)mph);
+      BwdMetaTc mt[WG_TASKS];
 #pragma unroll
-      for (int it = 0; it < 2; ++it) mt[it] = wmeta[ms][t_meta[it]];
+      for (int it = 0; it < WG_TASKS; ++it) mt[it] = wmeta[ms][t_meta[it]];
       __syncwarp();
       if (lane == 0) mbar_arrive_tc(&m_empty[ms]);
       if (++ms == WG_MR) { ms = 0; mph ^= 1; }
       const float *x_img = xt + (long long)b * HW * Cp;
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int flags = mt[it].packed;
-        const int xo = ((flags >> 7) - (s.W + 1)) * Cp + t_xc[it];
-        xc[it][0] = (flags & 1) ? __ldg(reinterpret_cast<const float4 *>(x_img + xo)) : z4;
-        xc[it][1] = (flags & 2) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs1))) : z4;
-        xc[it][2] = (flags & 4) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs2))) : z4;
-        xc[it][3] = (flags & 8) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs3))) : z4;
-      }
-      if (++sll == wg.spi) { sll = 0; ++b; }
-    };
-    for (int sl = sl0; sl < sl1; ++sl) {
-      load_slice();
-      float4 val[2];
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const float lh = mt[it].lh, lw = mt[it].lw, mm = mt[it].m, hh = 1.f - lh, hw = 1.f - lw;
-        const float w1 = hh * hw * mm, w2 = hh * lw * mm, w3 = lh * hw * mm, w4 = lh * lw * mm;   // as the forward sampler
-        const float4 x1 = xc[it][0], x2 = xc[it][1], x3 = xc[it][2], x4 = xc[it][3];
-        float4 v;
-        v.x = fmaf(w4, x4.x, fmaf(w3, x3.x, fmaf(w2, x2.x, w1 * x1.x)));
-        v.y = fmaf(w4, x4.y, fmaf(w3, x3.y, fmaf(w2, x2.y, w1 * x1.y)));
-        v.z = fmaf(w4, x4.z, fmaf(w3, x3.z, fmaf(w2, x2.z, w1 * x1.z)));
-        v.w = fmaf(w4, x4.w, fmaf(w3, x3.w, fmaf(w2, x2.w, w1 * x1.w)));
-        val[it] = v;
-      }
-      mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
       unsigned char *a_hi = tc_smem + (size_t)stage * wg.stage_bytes;
       unsigned char *a_lo = a_hi + WG_A_BYTES;
 #pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const float4 v = val[it];
-        const float4 h4 = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
-        float *dh = reinterpret_cast<float *>(a_hi + t_dst[it]), *dl = reinterpret_cast<float *>(a_lo + t_dst[it]);
-        dh[0] = h4.x; dh[4] = h4.y; dh[8] = h4.z; dh[12] = h4.w;                          // rows c4*4 + 0..3: 16 bytes apart
-        dl[0] = v.x - h4.x; dl[4] = v.y - h4.y; dl[8] = v.z - h4.z; dl[12] = v.w - h4.w;
+      for (int r = 0; r < WG_TASKS; r += 2) {
+        float4 xc[2][4];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int flags = mt[r + u].packed;
+          const int xo = ((flags >> 7) - (s.W + 1)) * Cp + t_xc[r + u];
+          xc[u][0] = (flags & 1) ? __ldg(reinterpret_cast<const float4 *>(x_img + xo)) : z4;
+          xc[u][1] = (flags & 2) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs1))) : z4;
+          xc[u][2] = (flags & 4) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs2))) : z4;
+          xc[u][3] = (flags & 8) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs3))) : z4;
+        }
+        if (r == 0) {
+          mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
+          if (sw == 0 && lane == 0) {
+            // B operand: rows nti*NT .. nti*NT + NT - 1 of the slice's hi and lo dY tiles (8-row groups are contiguous,
+            // 128 bytes a row)
+            unsigned char *dst = a_hi + 2 * WG_A_BYTES;
+            const unsigned char *src = reinterpret_cast<const unsigned char *>(gyk) + (size_t)sl * 2 * tile_bytes +
+                                       (size_t)nti * NT * TC_K * 4;
+            mbar_expect_tx(&b_full[stage], 2u * (uint32_t)b_bytes);
+            for (uint32_t off = 0; off < (uint32_t)b_bytes; off += 2048u) {
+              bulk_g2s(dst + off, src + off, 2048u, &b_full[stage]);
+              bulk_g2s(dst + b_bytes + off, src + tile_bytes + off, 2048u, &b_full[stage]);
+            }
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const BwdMetaTc &m = mt[r + u];
+          const float lh = m.lh, lw = m.lw, mm = m.m, hh = 1.f - lh, hw = 1.f - lw;
+          const float w1 = hh * hw * mm, w2 = hh * lw * mm, w3 = lh * hw * mm, w4 = lh * lw * mm;   // as the forward sampler
+          const float4 x1 = xc[u][0], x2 = xc[u][1], x3 = xc[u][2], x4 = xc[u][3];
+          float4 v;
+          v.x = fmaf(w4, x4.x, fmaf(w3, x3.x, fmaf(w2, x2.x, w1 * x1.x)));
+          v.y = fmaf(w4, x4.y, fmaf(w3, x3.y, fmaf(w2, x2.y, w1 * x1.y)));
+          v.z = fmaf(w4, x4.z, fmaf(w3, x3.z, fmaf(w2, x2.z, w1 * x1.z)));
+          v.w = fmaf(w4, x4.w, fmaf(w3, x3.w, fmaf(w2, x2.w, w1 * x1.w)));
+          const float4 h4 = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
+          float *dh = reinterpret_cast<float *>(a_hi + t_dst[r + u]), *dl = reinterpret_cast<float *>(a_lo + t_dst[r + u]);
+          dh[0] = h4.x; dh[4] = h4.y; dh[8] = h4.z; dh[12] = h4.w;                          // rows c4*4 + 0..3: 16 bytes apart
+          dl[0] = v.x - h4.x; dl[4] = v.y - h4.y; dl[8] = v.z - h4.z; dl[12] = v.w - h4.w;
+        }
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) mbar_arrive_tc(&a_full[stage]);
       if (++stage == wg.stages) { stage = 0; ph ^= 1; }
+      if (++sll == wg.spi) { sll = 0; ++b; }
     }
-  } else if (warp == TC_WARP_TMA) {
-    if (lane == 0) {
-      int stage = 0, ph = 0;
-      for (int sl = sl0; sl < sl1; ++sl) {
-        mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
-        unsigned char *dst = tc_smem + (size_t)stage * wg.stage_bytes + 2 * WG_A_BYTES;
-        const unsigned char *src = reinterpret_cast<const unsigned char *>(gyk) + (size_t)sl * 2 * b_bytes;
-        mbar_expect_tx(&b_full[stage], 2u * (uint32_t)b_bytes);
-        for (uint32_t off = 0; off < 2u * (uint32_t)b_bytes; off += 2048u) bulk_g2s(dst + off, src + off, 2048u, &b_full[stage]);
-        if (++stage == wg.stages) { stage = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp == TC_WARP_MMA) {
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(wg.co_r >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int stage = 0, ph = 0;
-      for (int sl = sl0; sl < sl1; ++sl) {
-        mbar_wait(&a_full[stage], (uint32_t)ph);
-        mbar_wait(&b_full[stage], (uint32_t)ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t ah = smem_u32(tc_smem + (size_t)stage * wg.stage_bytes), al = ah + WG_A_BYTES;
-        const uint32_t bh = al + WG_A_BYTES, bl = bh + (uint32_t)b_bytes;
+  } else if (warp >= WG_WARP_C0) {
+    // =========================================================== consumers: warpgroup cw accumulates rows 64 cw .. 64 cw + 63
+    const int cw = (warp - WG_WARP_C0) >> 2, wq = warp & 3;
+    float d[NT / 2];
 #pragma unroll
-        for (int k8 = 0; k8 < TC_K / 8; ++k8) {
-          const uint32_t koff = (uint32_t)k8 * 2u * TC_LBO;
-          const uint64_t dah = wg_desc_a(ah + koff), dal = wg_desc_a(al + koff);
-          const uint64_t dbh = tc_desc(bh + koff), dbl = tc_desc(bl + koff);
-          umma_tf32(tm, dal, dbh, idesc, (sl > sl0 || k8 > 0) ? 1u : 0u);
-          umma_tf32(tm, dah, dbl, idesc, 1u);
-          umma_tf32(tm, dah, dbh, idesc, 1u);
-        }
-        umma_commit(&empty[stage]);
-        if (++stage == wg.stages) { stage = 0; ph ^= 1; }
+    for (int i = 0; i < NT / 2; ++i) d[i] = 0.f;
+    int stage = 0, ph = 0;
+    for (int sl = sl0; sl < sl1; ++sl) {
+      mbar_wait(&a_full[stage], (uint32_t)ph);
+      mbar_wait(&b_full[stage], (uint32_t)ph);
+      const uint32_t base = smem_u32(tc_smem + (size_t)stage * wg.stage_bytes);
+      const uint32_t ah = base + (uint32_t)cw * 8u * WG_SBO, al = ah + WG_A_BYTES;
+      const uint32_t bh = base + 2u * WG_A_BYTES, bl = bh + (uint32_t)b_bytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k8 = 0; k8 < TC_K / 8; ++k8) {
+        const uint32_t koff = (uint32_t)k8 * 2u * TC_LBO;
+        wgmma_3xtf32<NT>(d, wg_desc(ah + koff, TC_LBO, WG_SBO), wg_desc(al + koff, TC_LBO, WG_SBO), tc_desc(bh + koff),
+                         tc_desc(bl + koff), (sl > sl0 || k8 > 0) ? 1u : 0u);
       }
-      umma_commit(&tm_full);
+      wgmma_commit();
+      wgmma_wait_all();
+      if (((tid - WG_WARP_C0 * 32) & 127) == 0) mbar_arrive_tc(&empty[stage]);
+      if (++stage == wg.stages) { stage = 0; ph ^= 1; }
+    }
+    // epilogue: wpart[split][rg][row][co_r], columns nti*NT .. nti*NT + NT - 1 (zeros for a CTA without slices)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      float *dst = wpart + (((size_t)split * g.RG + rg) * 128 + row) * wg.co_r + nti * NT + 2 * (lane & 3);
+#pragma unroll
+      for (int jj = 0; jj < NT / 8; ++jj)
+        *reinterpret_cast<float2 *>(dst + 8 * jj) = make_float2(d[4 * jj + 2 * h], d[4 * jj + 2 * h + 1]);
     }
   } else {
-    // =========================================================== warps 0-3 first produce the geometry: 4 taps x 32 pixels of a slice, one
+    // =========================================================== warps 0-3 produce the geometry: 4 taps x 32 pixels of a slice, one
     // entry per thread, WG_MR slices ahead of the samplers (ring in shared memory, mbarrier hand-over); the offsets and
     // mask of the next slice are fetched before the current entry is finished
     const int st = tid;
@@ -878,33 +821,7 @@ k_dcn_bwd_weight_tc(const float *__restrict__ xt, const float *__restrict__ offs
       b = nb_;
       sll = nsl;
     }
-    // epilogue: TMEM lane = row (chunk, channel), columns = output channels -> wpart[split][rg][row][co_r]
-    const int qw = warp;
-    float *dst = wpart + (((size_t)split * g.RG + rg) * 128 + qw * 32 + lane) * wg.co_r;
-    if (sl1 > sl0) {
-      mbar_wait(&tm_full, 0u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    const uint32_t taddr = tm + ((uint32_t)(qw * 32) << 16);
-#pragma unroll 1
-    for (int c0 = 0; c0 < wg.co_r; c0 += 32) {
-      uint32_t v[32];
-      if (sl1 > sl0) {
-        tmem_ld32(taddr + (uint32_t)c0, v);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = 0u;
-      }
-#pragma unroll
-      for (int i = 0; i < 32; i += 4)
-        if (c0 + i < wg.co_r)
-          *reinterpret_cast<float4 *>(dst + c0 + i) = make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]),
-                                                                   __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-    }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == TC_WARP_MMA) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tm), "n"(256));
 }
 
 // gw[o][ch][tap] += sum over splits (ascending) of wpart[split][rg][row][o]
@@ -998,7 +915,7 @@ int dcn_backward_data_tc(const float *input, const float *offset, const float *m
   k_bwd_prep_w<<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtt);
   CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight tiles");
   count_launch();
-  const size_t smem = (size_t)BW_STAGES * BW_STAGE_BYTES + 4 * 4096;     // operand ring + the epilogue warps' staging
+  const size_t smem = (size_t)BW_STAGES * BW_STAGE_BYTES;     // operand ring
   static thread_local int dev_done = -1;
   int dev = 0;
   cudaGetDevice(&dev);
@@ -1014,7 +931,7 @@ int dcn_backward_data_tc(const float *input, const float *offset, const float *m
     const int n_items = nbimg * g.tiles * g.RG;
     const int grid = n_items < num_sms() ? n_items : num_sms();
     k_dcn_bwd_dcol_tc<<<grid, BW_THREADS, smem, stream>>>(gyt, wtt, dcol, s, g, n_items);
-    CNB_CHECK_LAUNCH("cnb_dcnv2_backward column gradient (tcgen05)");
+    CNB_CHECK_LAUNCH("cnb_dcnv2_backward column gradient (wgmma)");
     k_dcn_bwd_offmask<3><<<nbimg * g.tiles, 256, 0, stream>>>(xsrc, offset, mask, dcol, (grad_input && !gather) ? dxt : nullptr,
                                                               grad_offset, grad_mask, gather ? grad_input : nullptr, s, g, b0);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward offset/mask gradient");
@@ -1075,11 +992,16 @@ int dcn_backward_weight_tc(const float *input, const float *offset, const float 
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev_done != dev) {
-    CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * 66048));
+    CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  WG_STAGES * (2 * WG_A_BYTES + 2 * 64 * TC_K * 4)));
+    CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  WG_STAGES * (2 * WG_A_BYTES + 2 * 128 * TC_K * 4)));
     dev_done = dev;
   }
-  k_dcn_bwd_weight_tc<<<g.RG * wg.splits, WG_THREADS, smem, stream>>>(xsrc, offset, mask, gyk, wpart, s, g, wg);
-  CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight gradient (tcgen05)");
+  const unsigned wgrid = (unsigned)(g.RG * wg.n_nt * wg.splits);
+  if (wg.nt == 64) k_dcn_bwd_weight_tc<64><<<wgrid, WG_THREADS, smem, stream>>>(xsrc, offset, mask, gyk, wpart, s, g, wg);
+  else k_dcn_bwd_weight_tc<128><<<wgrid, WG_THREADS, smem, stream>>>(xsrc, offset, mask, gyk, wpart, s, g, wg);
+  CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight gradient (wgmma)");
   const long long total = (long long)g.RG * 128 * wg.co_r;
   k_dcn_bwd_wreduce<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(wpart, grad_weight, s, g, wg);
   CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight gradient reduce");

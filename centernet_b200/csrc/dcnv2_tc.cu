@@ -1,31 +1,30 @@
-// DCNv2 forward with the dense contraction on the 5th-generation tensor cores (tcgen05 / UMMA) -- a
-// persistent, warp-specialised pipeline (reference: dcn_v2_cuda.c:10-102 + dcn_v2_im2col_cuda.cu:118-180).
+// DCNv2 forward with the dense contraction on the Hopper tensor cores (wgmma) -- a persistent,
+// warp-specialised pipeline (reference: dcn_v2_cuda.c:10-102 + dcn_v2_im2col_cuda.cu:118-180).
 //
-//   work item   = (image, 8x16 output-pixel tile [128 pixels = UMMA M], Cout tile of 64|128, K split)
+//   work item   = (image, 8x16 output-pixel tile [128 pixels = 2 x wgmma M], Cout tile of 64|128, K split)
 //   chunk       = 32 input channels x one tap: K = 32 of the contraction; chunks of an item run over
 //                 (channel block OUTER, tap INNER), so the ~40 KB input neighbourhood of a channel block is
 //                 fetched from L2 once and then re-read by all 9 taps x 4 bilinear corners out of L1
 //   sampler warps (16)  build the column tile col[128 px, 32 ch] of a chunk directly in shared memory
 //                 (never in HBM -- the reference writes and re-reads a 37.7 MB column matrix per sample),
-//                 split into TF32 hi/lo, in the canonical no-swizzle K-major UMMA layout; 3-deep ring
+//                 split into TF32 hi/lo, in the canonical no-swizzle K-major layout; 2|3-deep ring
 //   TMA warp      streams the matching pre-split weight tile (hi+lo) with cp.async.bulk (UBLKCP)
-//   MMA warp      one thread issues tcgen05.mma.kind::tf32 (UTCHMMA): D[128, Cout_t] += col . W^T, three MMAs
-//                 per k-step (lo.hi + hi.lo + hi.hi = "3xTF32", fp32-accurate: the reference is an fp32
-//                 SGEMM and plain TF32 misses the 1e-4 bar at K = Cin*9 <= 4608); tcgen05.commit frees the
-//                 ring slot; accumulators live in TMEM, double-buffered across items
-//   epilogue warps (4)  tcgen05.ld the finished accumulator, add the bias and store NCHW while the
-//                 samplers are already on the next item
+//   consumer warpgroups (2)  each issues wgmma.m64nCo_t k8 .tf32 on its 64 rows: D[64, Cout_t] += col . W^T,
+//                 three MMAs per k-step (lo.hi + hi.lo + hi.hi = "3xTF32", fp32-accurate: the reference is an fp32
+//                 SGEMM and plain TF32 misses the 1e-4 bar at K = Cin*9 <= 4608), waits for them and frees the ring
+//                 slot; the accumulator lives in registers, and the same warpgroup adds the bias and stores NCHW
+//                 while the samplers are already filling the ring for the next item
 // Nobody waits on anybody except through mbarriers; the only CTA-wide barriers are at start and end.
 //
 // Sampling: the input is read from a channels-last copy [B][H*W][Cin/32][32] (k_dcn_nhwc; skipped when the
 // caller's tensor already is channels-last).  A warp gather covers 4 pixels x 32 channels with
 // lane = pixel * 8 + quad, so each quarter-warp -- the unit the L1 data pipe serves for 16-byte accesses --
 // reads ONE fully used 128-byte line (4 wavefronts per gather).  Each lane then holds exactly one 16-byte k-chunk of
-// the K-major UMMA tile; the tile's k-chunks are pitched 144 bytes (LBO in the descriptor) instead of 128, which puts
+// the K-major A tile; the tile's k-chunks are pitched 144 bytes (LBO in the descriptor) instead of 128, which puts
 // the eight chunks a quarter-warp stores into eight different bank groups -- conflict-free without a transpose
 // (round 1 transposed across the warp with 16 shuffles; same speed, fewer instructions).
 //
-// Small maps (16x16, 8x8): too few tiles to fill 148 SMs, so the channel blocks of an item are split over
+// Small maps (16x16, 8x8): too few tiles to fill 132 SMs, so the channel blocks of an item are split over
 // several CTAs (split-K); the partial sums go to the workspace and k_dcn_reduce adds them in a fixed order
 // (deterministic, no atomics).
 //
@@ -36,7 +35,7 @@
 
 namespace cnb {
 
-// W[Cout][Cin][KT] -> per (cout tile, channel block bi, tap): hi tile then lo tile, each [co_t][32] in the UMMA
+// W[Cout][Cin][KT] -> per (cout tile, channel block bi, tap): hi tile then lo tile, each [co_t][32] in the K-major
 // layout; k = channel within the block.  Tile index = (cot * nb + bi) * 9 + tap.
 __global__ void __launch_bounds__(256) k_dcn_prep_weights(const float *__restrict__ w, const DcnShapeTc s,
                                                           float *__restrict__ ws) {
@@ -139,8 +138,7 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
   constexpr int B_BYTES = CO_T * TC_K * 4;                  // one hi or lo weight tile
   constexpr int STAGE_BYTES = 2 * FW_A_BYTES + 2 * B_BYTES;
   TapMetaTc *meta = reinterpret_cast<TapMetaTc *>(tc_smem + (size_t)STAGES * STAGE_BYTES);     // [9][128]
-  __shared__ __align__(8) uint64_t a_full[STAGES], b_full[STAGES], empty[STAGES], tm_full[2], tm_empty[2];
-  __shared__ uint32_t tmem_base;
+  __shared__ __align__(8) uint64_t a_full[STAGES], b_full[STAGES], empty[STAGES];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int KT = s.kh * s.kw;
@@ -151,23 +149,11 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&a_full[i], TC_SAMPLERS);
       mbar_init(&b_full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tm_full[i], 1);
-      mbar_init(&tm_empty[i], TC_EPI_WARPS);
+      mbar_init(&empty[i], TC_MMA_WGS);
     }
     mbar_fence_init();
   }
-  if (warp == TC_WARP_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base)),
-                 "n"(2 * CO_T));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tm = tmem_base;
 
   if (warp >= TC_WARP_S0) {
     // =========================================================== samplers: A operand of every chunk
@@ -217,8 +203,12 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
         const float *xb = xbat + (long long)bi * TC_CB;
         for (int tap = 0; tap < TC_NT; ++tap) {
           // warp item = 4 pixels: every lane gathers the 4 corners of its pixel as 16-byte pieces (4 channels);
-          // both of a warp's items (pixels 8w..8w+3 and 8w+4..8w+7) are gathered before either is reduced
-          const int pp0 = sw * 8 + sp, pp1 = pp0 + 4;
+          // a warp fills TC_SAMPLER_ROUNDS 8-pixel row groups, one after the other; both items of a group (pixels
+          // 8r..8r+3 and 8r+4..8r+7) are gathered before either is reduced
+#pragma unroll 1
+          for (int rnd = 0; rnd < TC_SAMPLER_ROUNDS; ++rnd) {
+          const int rgp = sw * TC_SAMPLER_ROUNDS + rnd;
+          const int pp0 = rgp * 8 + sp, pp1 = pp0 + 4;
           const TapMetaTc m0 = meta[tap * TC_TP + pp0], m1 = meta[tap * TC_TP + pp1];
           float4 u0[4], u1[4];
 #pragma unroll
@@ -235,7 +225,7 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
           };
           const float4 v0 = reduce(m0, u0), v1 = reduce(m1, u1);   // (row sp, quad sq) and (row 4 + sp, quad sq)
           // the ring slot must have been drained by the MMAs that last read it
-          mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
+          if (rnd == 0) mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
           unsigned char *a_hi = tc_smem + (size_t)stage * STAGE_BYTES;
           unsigned char *a_lo = a_hi + FW_A_BYTES;
           // each lane already holds one 16-byte k-chunk of the K-major tile: (row, chunk sq).  The k-chunks of the A tile
@@ -244,13 +234,14 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
           {
             const float4 h0 = make_float4(tf32_hi(v0.x), tf32_hi(v0.y), tf32_hi(v0.z), tf32_hi(v0.w));
             const float4 h1 = make_float4(tf32_hi(v1.x), tf32_hi(v1.y), tf32_hi(v1.z), tf32_hi(v1.w));
-            const uint32_t off0 = (uint32_t)sw * FW_SBO + (uint32_t)sq * FW_LBO + (uint32_t)sp * 16u, off1 = off0 + 64u;
+            const uint32_t off0 = (uint32_t)rgp * FW_SBO + (uint32_t)sq * FW_LBO + (uint32_t)sp * 16u, off1 = off0 + 64u;
             *reinterpret_cast<float4 *>(a_hi + off0) = h0;
             *reinterpret_cast<float4 *>(a_lo + off0) = make_float4(v0.x - h0.x, v0.y - h0.y, v0.z - h0.z, v0.w - h0.w);
             *reinterpret_cast<float4 *>(a_hi + off1) = h1;
             *reinterpret_cast<float4 *>(a_lo + off1) = make_float4(v1.x - h1.x, v1.y - h1.y, v1.z - h1.z, v1.w - h1.w);
           }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> async proxy (UMMA reads)
+          }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> async proxy (wgmma reads)
           __syncwarp();
           if (lane == 0) mbar_arrive_tc(&a_full[stage]);
           if (++stage == STAGES) { stage = 0; ph ^= 1; }
@@ -276,102 +267,61 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
         }
       }
     }
-  } else if (warp == TC_WARP_MMA) {
-    // =========================================================== MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(CO_T >> 3) << 17) | ((uint32_t)(TC_TP >> 4) << 24);
-      int stage = 0, ph = 0, acc = 0, aph = 0;
-      for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
-        const ItemTc it = tc_item(s, item);
-        mbar_wait(&tm_empty[acc], (uint32_t)(aph ^ 1));     // the epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d_tmem = tm + (uint32_t)(acc * CO_T);
-        const int n_ch = (it.b1 - it.b0) * TC_NT;
-        for (int ch = 0; ch < n_ch; ++ch) {
-          mbar_wait(&a_full[stage], (uint32_t)ph);
-          mbar_wait(&b_full[stage], (uint32_t)ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t ah = smem_u32(tc_smem + (size_t)stage * STAGE_BYTES), al = ah + FW_A_BYTES;
-          const uint32_t bh = al + FW_A_BYTES, bl = bh + B_BYTES;
-#pragma unroll
-          for (int ks = 0; ks < TC_K / 8; ++ks) {   // one UMMA per 8 k (two 16-byte k-chunks), 3 per step (3xTF32)
-            const uint32_t koff = (uint32_t)ks * 2u * TC_LBO;
-            const uint32_t koff_a = (uint32_t)ks * 2u * FW_LBO;
-            const uint64_t dah = fw_desc_a(ah + koff_a), dal = fw_desc_a(al + koff_a);
-            const uint64_t dbh = tc_desc(bh + koff), dbl = tc_desc(bl + koff);
-            const uint32_t acc0 = (ch > 0 || ks > 0) ? 1u : 0u;
-            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                         "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(dal), "l"(dbh),
-                         "r"(idesc), "r"(acc0) : "memory");      // lo * hi   (small terms first)
-            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                         "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(dah), "l"(dbl),
-                         "r"(idesc), "r"(1u) : "memory");        // hi * lo
-            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                         "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(dah), "l"(dbh),
-                         "r"(idesc), "r"(1u) : "memory");        // hi * hi
-          }
-          // frees the ring slot (A and B) once the MMAs above have read it
-          asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                           smem_u32(&empty[stage])) : "memory");
-          if (++stage == STAGES) { stage = 0; ph ^= 1; }
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                         smem_u32(&tm_full[acc])) : "memory");
-        if (++acc == 2) { acc = 0; aph ^= 1; }
-      }
-    }
   } else {
-    // =========================================================== epilogue: TMEM -> registers -> bias -> global
-    const int q = warp;                 // TMEM lane quarter == warp index (warps 0..3)
-    int acc = 0, aph = 0;
+    // =========================================================== consumers: wgmma over the ring, epilogue from registers
+    const int wgi = warp >> 2, wq = warp & 3;
+    int stage = 0, ph = 0;
     for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
       const ItemTc it = tc_item(s, item);
-      const int pp = q * 32 + lane;
-      const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
-      const bool ok = ho < s.Ho && wo < s.Wo;
-      const long long p = (long long)ho * s.Wo + wo;
-      float *dst = (s.splits > 1 ? part + (long long)it.split * s.B * s.Cout * HWo : y) + (long long)it.b * s.Cout * HWo + p;
-      mbar_wait(&tm_full[acc], (uint32_t)aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t taddr = tm + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * CO_T);
-#pragma unroll 1
-      for (int c32 = 0; c32 < CO_T; c32 += 32) {
-        uint32_t v[32];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,"
-            "%25,%26,%27,%28,%29,%30,%31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr + (uint32_t)c32));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (ok) {
+      float d[CO_T / 2];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int o = it.cot * CO_T + c32 + j;
+      for (int i = 0; i < CO_T / 2; ++i) d[i] = 0.f;
+      const int n_ch = (it.b1 - it.b0) * TC_NT;
+      for (int ch = 0; ch < n_ch; ++ch) {
+        mbar_wait(&a_full[stage], (uint32_t)ph);
+        mbar_wait(&b_full[stage], (uint32_t)ph);
+        const uint32_t base = smem_u32(tc_smem + (size_t)stage * STAGE_BYTES);
+        const uint32_t ah = base + (uint32_t)wgi * 8u * FW_SBO, al = ah + FW_A_BYTES;   // this warpgroup's 64 rows
+        const uint32_t bh = base + 2u * FW_A_BYTES, bl = bh + B_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < TC_K / 8; ++ks) {   // one k8 step = two 16-byte k-chunks
+          const uint32_t koff = (uint32_t)ks * 2u * TC_LBO, koff_a = (uint32_t)ks * 2u * FW_LBO;
+          wgmma_3xtf32<CO_T>(d, fw_desc_a(ah + koff_a), fw_desc_a(al + koff_a), tc_desc(bh + koff), tc_desc(bl + koff),
+                             (ch > 0 || ks > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();          // the slot is read: hand it back to the samplers and the TMA warp
+        if ((tid & 127) == 0) mbar_arrive_tc(&empty[stage]);
+        if (++stage == STAGES) { stage = 0; ph ^= 1; }
+      }
+      // epilogue: d[4j + r] = (row wq*16 + lane/4 + 8*(r/2), column 8j + 2*(lane%4) + r%2) of this warpgroup's 64 rows
+      float *dst = (s.splits > 1 ? part + (long long)it.split * s.B * s.Cout * HWo : y) + (long long)it.b * s.Cout * HWo;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int pp = wgi * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
+        if (ho >= s.Ho || wo >= s.Wo) continue;
+        float *dp = dst + (long long)ho * s.Wo + wo;
+#pragma unroll
+        for (int j = 0; j < CO_T / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int o = it.cot * CO_T + 8 * j + 2 * (lane & 3) + e;
             if (o < s.Cout) {
-              float r = __uint_as_float(v[j]);
+              float r = d[4 * j + 2 * h + e];
               if (s.splits == 1) {
                 if (bias) r += __ldg(bias + o);
                 if (s.epi_scale) r = fmaf(r, __ldg(s.epi_scale + o), __ldg(s.epi_shift + o));
                 if (s.relu) r = fmaxf(r, 0.f);
               }
-              dst[(long long)o * HWo] = r;
+              dp[(long long)o * HWo] = r;
             }
           }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive_tc(&tm_empty[acc]);
-      if (++acc == 2) { acc = 0; aph ^= 1; }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == TC_WARP_MMA) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tm), "n"(2 * CO_T));
 }
 
 size_t dcn_tc_wtiles_bytes(int cin, int cout, int dg) {
@@ -429,7 +379,7 @@ static int launch_fwd(const float *xt, const float *offset, const float *mask, c
   }
   const int grid = s.n_items < num_sms() ? s.n_items : num_sms();
   k_dcn_forward_tc<CO_T, STAGES><<<grid, TC_THREADS, smem, stream>>>(xt, offset, mask, wtiles, bias, output, part, s);
-  CNB_CHECK_LAUNCH("cnb_dcnv2_forward (tcgen05)");
+  CNB_CHECK_LAUNCH("cnb_dcnv2_forward (wgmma)");
   count_launch();
   return CNB_OK;
 }

@@ -1,23 +1,23 @@
-// Shared by the tcgen05 DCNv2 kernels (dcnv2_tc.cu: forward, dcnv2_bwd_tc.cu: backward): the UMMA tile
-// layout (K-major, no swizzle), the instruction descriptor pieces and the shape / work decomposition.
+// Shared by the wgmma DCNv2 kernels (dcnv2_tc.cu: forward, dcnv2_bwd_tc.cu: backward): the shared-memory tile
+// layout (K-major, no swizzle), the wgmma descriptor and instruction wrappers and the shape / work decomposition.
 #pragma once
 #include "common.cuh"
 
 namespace cnb {
 
-constexpr int TC_TP = 128;        // pixels per item (UMMA M)
+constexpr int TC_TP = 128;        // pixels per item (two warpgroups x wgmma M = 64)
 constexpr int TC_CB = 32;         // input channels per chunk = one 128-byte line of the channels-last copy
 constexpr int TC_NT = 9;          // taps (3x3 kernel; fewer taps leave zero weight tiles)
 constexpr int TC_K = TC_CB;       // K per chunk
 constexpr int TC_KC = TC_K / 4;   // 16-byte k-chunks
-constexpr int TC_EPI_WARPS = 4;   // warps 0-3: TMEM lane quarter = warp index
-constexpr int TC_WARP_MMA = 4;
-constexpr int TC_WARP_TMA = 5;
-constexpr int TC_WARP_S0 = 6;     // first sampler warp
-constexpr int TC_SAMPLERS = 16;   // sampler warps: 2 warp items (4 pixels each) per warp and chunk
-constexpr int TC_THREADS = (TC_WARP_S0 + TC_SAMPLERS) * 32;   // 704
+constexpr int TC_MMA_WGS = 2;     // warps 0-7: two consumer warpgroups, warpgroup i owns rows 64i..64i+63 of the tile
+constexpr int TC_WARP_TMA = 8;
+constexpr int TC_WARP_S0 = 9;     // first sampler warp
+constexpr int TC_SAMPLERS = 8;    // sampler warps of the forward: 2 rounds x 2 warp items (4 pixels each) per chunk
+constexpr int TC_SAMPLER_ROUNDS = TC_TP / 8 / TC_SAMPLERS;
+constexpr int TC_THREADS = (TC_WARP_S0 + TC_SAMPLERS) * 32;   // 544: the consumers hold up to 64 accumulators each
 constexpr uint32_t TC_LBO = 128;            // bytes between consecutive k-chunks (one 8 x 16 B core matrix)
-constexpr uint32_t TC_SBO = TC_KC * 128;    // bytes between 8-row groups
+constexpr uint32_t TC_SBO = TC_KC * 128;    // bytes between 8-row groups (1024)
 constexpr int TC_A_BYTES = TC_TP * TC_K * 4;  // 16384 per hi / lo tile
 
 // A tile of the forward sampler: the same K-major core-matrix layout with the k-chunks pitched 144 bytes apart
@@ -50,21 +50,66 @@ struct __align__(16) TapMetaTc {
 __device__ __forceinline__ uint32_t tc_tile_off(int row, int k) {  // byte offset of element (row, k) in a K-major tile
   return (uint32_t)(row >> 3) * TC_SBO + (uint32_t)(k >> 2) * TC_LBO + (uint32_t)(row & 7) * 16u + (uint32_t)(k & 3) * 4u;
 }
-__device__ __forceinline__ uint64_t tc_desc(uint32_t addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr >> 4) & 0x3fff);
-  d |= (uint64_t)((TC_LBO >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((TC_SBO >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell); layout_type 0 = no swizzle
-  return d;
+// sm_90 shared-memory matrix descriptor: start address, leading (k-chunk) and stride (8-row group) byte offsets,
+// base offset 0, layout type 0 = no swizzle
+__device__ __forceinline__ uint64_t wg_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
+  return (uint64_t)((addr >> 4) & 0x3fff) | ((uint64_t)((lbo >> 4) & 0x3fff) << 16) |
+         ((uint64_t)((sbo >> 4) & 0x3fff) << 32);
 }
-__device__ __forceinline__ uint64_t fw_desc_a(uint32_t addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr >> 4) & 0x3fff);
-  d |= (uint64_t)((FW_LBO >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((FW_SBO >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
+__device__ __forceinline__ uint64_t tc_desc(uint32_t addr) { return wg_desc(addr, TC_LBO, TC_SBO); }
+__device__ __forceinline__ uint64_t fw_desc_a(uint32_t addr) { return wg_desc(addr, FW_LBO, FW_SBO); }
+
+// wgmma (warpgroup-wide, asynchronous): D[64 x N] (+)= A[64 x 8] . B[N x 8]^T in TF32, both operands K-major in
+// shared memory, D in registers: d[4j + r] holds row (warp % 4) * 16 + lane / 4 + 8 * (r / 2), column
+// 8j + 2 * (lane % 4) + r % 2.  scale_d == 0 overwrites D.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
+      "%26,%27,%28,%29,%30,%31}"
+      ", %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
+      "%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,"
+      "%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+      ", %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  static_assert(N == 64 || N == 128, "wgmma_tf32: N is 64 or 128");
+  if constexpr (N == 64) wgmma_tf32_n64(d, da, db, scale_d);
+  else wgmma_tf32_n128(d, da, db, scale_d);
+}
+// 3xTF32 step of one 8-wide k slice: lo.hi + hi.lo + hi.hi (small terms first) -- fp32-accurate products
+template <int N>
+__device__ __forceinline__ void wgmma_3xtf32(float (&d)[N / 2], uint64_t dah, uint64_t dal, uint64_t dbh, uint64_t dbl,
+                                             uint32_t scale_d) {
+  wgmma_tf32<N>(d, dal, dbh, scale_d);
+  wgmma_tf32<N>(d, dah, dbl, 1u);
+  wgmma_tf32<N>(d, dah, dbh, 1u);
 }
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 __device__ __forceinline__ void mbar_arrive_tc(uint64_t *bar) {

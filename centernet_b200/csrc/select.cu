@@ -1,4 +1,4 @@
-// Fused 3x3 peak-NMS + exact top-K (score desc, flat index asc) for sm_100a.
+// Fused 3x3 peak-NMS + exact top-K (score desc, flat index asc) for sm_90a.
 //
 // Reference semantics (models/decode.py):
 //   _nms   :9-15     keep = (maxpool3x3(heat) == heat); heat*keep

@@ -15,7 +15,7 @@ constexpr int SEL_HIST_COARSE = 64;      // 64 fine bins each (only the first FI
 constexpr int SEL_MASK_WORDS = 512;     // qualifying-pixel bitmask of one unit
 constexpr int SEL_RW = 4;               // rows per warp work item
 constexpr int SEL_MAX_K = 1024;
-constexpr int SEL_MAX_CTA = 192;        // stage-1 grid limit (one CTA per SM; B200 has 148)
+constexpr int SEL_MAX_CTA = 192;        // stage-1 grid limit (one CTA per SM; H100 has 132)
 constexpr int SEL_FIN_MAX = 8192;       // separate-finalize sort capacity (keys); the fused finalize uses SEL_CAP
 
 struct SelectPlan {

@@ -1,5 +1,5 @@
 """Training-side data parallelism (SURVEY 8e / row E2): one process per GPU, replicas hold full weights, and the
-ONLY exchange per step is a bucketed NCCL all-reduce of the gradients over NVLink 5 / NVSwitch, launched from
+ONLY exchange per step is a bucketed NCCL all-reduce of the gradients over NVLink 4 / NVSwitch, launched from
 autograd hooks while the rest of the backward is still running.
 
 Replaces src/lib/models/data_parallel.py (single process, scatter -> replicate -> parallel_apply -> gather, the

@@ -14,7 +14,7 @@ from torch.autograd import Function
 
 from ._lib import C, f32c, ptr, stream_ptr, workspace
 
-# CNB_DCN_FP32=1 selects the fp32 CUDA-core contraction instead of the tcgen05 (3xTF32) one
+# CNB_DCN_FP32=1 selects the fp32 CUDA-core contraction instead of the wgmma (3xTF32) one
 _FORCE_FP32 = os.environ.get("CNB_DCN_FP32", "0") == "1"
 # CNB_DCN_DETERMINISTIC=1: bit-identical grad_input (cnb_dcnv2_set_deterministic); also on under
 # torch.use_deterministic_algorithms(True)
@@ -31,7 +31,7 @@ _WT_CACHE = {}      # id(weight) -> (weakref to it, its version when tiled, tile
 
 
 def _weight_tiles(weight, dg):
-    """TF32 hi/lo weight tiles in the UMMA layout (cnb_dcnv2_prepare_weights), rebuilt only when the parameter
+    """TF32 hi/lo weight tiles in the wgmma K-major layout (cnb_dcnv2_prepare_weights), rebuilt only when the parameter
     changes: torch bumps `_version` on every in-place update (optimizer step, load_state_dict), and the entry
     is tied to the tensor OBJECT by a weak reference, so a new tensor that happens to reuse the address never
     sees stale tiles."""

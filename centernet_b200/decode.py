@@ -3,7 +3,7 @@
 Every function takes fp32 CUDA tensors (NCHW; heat maps already sigmoided by the
 caller, as in detectors/ctdet.py:31,40), does not mutate its inputs, and returns a new
 fp32 tensor on the same device, enqueued on the current stream.  The work is done by
-the hand-written sm_100a kernels behind ``include/centernet_b200.h``; there is no
+the hand-written sm_90a kernels behind ``include/centernet_b200.h``; there is no
 CPU path (non-CUDA inputs raise NotImplementedError).
 
 Tie order, which the reference leaves to torch.topk, is defined here as

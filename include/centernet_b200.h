@@ -1,5 +1,5 @@
 /*
- * centernet_b200 -- C ABI of the B200-native CenterNet heat-map hot path.
+ * centernet_b200 -- C ABI of the H100-native CenterNet heat-map hot path.
  *
  * This is the drop-in boundary: plain device pointers, explicit sizes and a
  * CUDA stream handle; no torch types.  The reference has two bindings on this
@@ -222,7 +222,7 @@ int cnb_dcnv2_forward(const float *input, const float *offset, const float *mask
                       int dil_h, int dil_w, int deformable_groups,
                       void *workspace, size_t workspace_bytes, void *stream);
 /* Steady-state form of the forward (what the Python module uses): the weight
- * tiles (TF32 hi/lo split, UMMA layout) are built ONCE per weight version into a
+ * tiles (TF32 hi/lo split, wgmma K-major layout) are built ONCE per weight version into a
  * caller-owned buffer of cnb_dcnv2_wtiles_bytes and reused by every call;
  * input_channels_last != 0 says `input` already is [b][h*w][cin] (torch
  * channels_last) so no re-layout pass runs (needs cin/dg % 32 == 0, else the flag

@@ -1,7 +1,7 @@
 """Recipe for oracle/_ref (TEST INFRASTRUCTURE): the reference DCNv2 on the GPU.
 
 Compiles the reference's two THC-free kernel files UNMODIFIED, from where they lie under
-/root/reference, for sm_100a, together with oracle/ref_host.cu (the cuBLAS restatement of the
+/root/reference, for sm_90a, together with oracle/ref_host.cu (the cuBLAS restatement of the
 removed-THC host loop, dcn_v2_cuda.c:61-97,161-231,243-330) into
 
     oracle/_ref/libdcnv2_ref.so
@@ -39,7 +39,7 @@ def build(force=False):
     if not force and available() and all(os.path.getmtime(s) <= os.path.getmtime(LIB) for s in srcs):
         return LIB
     os.makedirs(OUT, exist_ok=True)
-    cmd = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-shared", "-Xcompiler", "-fPIC",
+    cmd = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-shared", "-Xcompiler", "-fPIC",
            "-cudart", "static", "-I" + REF_CUDA] + srcs + ["-lcublas", "-o", LIB]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

@@ -100,7 +100,7 @@ def _raw_backward(x, off, m, w, go, stride, dg, tensor_cores, pad=1, dil=1):
 @pytest.mark.parametrize("B,Ci,H,W,Co,dg,stride", [(2, 64, 40, 48, 64, 1, 1), (3, 96, 17, 23, 40, 1, 1), (2, 128, 16, 16, 272, 1, 1),
                                                     (2, 64, 16, 24, 64, 2, 1), (2, 40, 19, 21, 24, 1, 2)])
 def test_backward_tensor_core_vs_fp32_path(B, Ci, H, W, Co, dg, stride):
-    """cnb_dcnv2_backward with the workspace (tcgen05, 3xTF32) against the same call without it (fp32 CUDA cores) on
+    """cnb_dcnv2_backward with the workspace (wgmma, 3xTF32) against the same call without it (fp32 CUDA cores) on
     shapes the reference-pinned cases do not reach: ragged tiles, channel blocks with padding, Cout > 256 (dW falls
     back to fp32), two deformable groups, stride 2; and the deterministic part of the tensor-core path repeats."""
     x, off, m, w, _ = [t.cuda() for t in make(B, Ci, H, W, Co, dg, stride, seed=11, off_scale=1.5)]
@@ -241,6 +241,12 @@ def test_fused_inference_paths():
         def forward(self, x):
             return self.actf(self.conv(x))
 
+    # conv_offset_mask runs on cuDNN: keep it fp32 so that the NCHW and channels_last inputs get the same offsets
+    with torch.backends.cudnn.flags(enabled=True, allow_tf32=False):
+        _fused_inference_cases(DeformConv, fuse_dcn_bn_relu)
+
+
+def _fused_inference_cases(DeformConv, fuse_dcn_bn_relu):
     for chi, cho, hw in ((64, 64, 40), (128, 256, 16), (24, 40, 9)):
         m = DeformConv(chi, cho).cuda()
         m.conv.conv_offset_mask.weight.data.normal_(0, 0.02); m.conv.conv_offset_mask.bias.data.normal_(0, 0.5)

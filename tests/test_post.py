@@ -51,21 +51,26 @@ def test_oracle_soft_nms_39_and_merge():
         np.testing.assert_array_equal(res[j], g["mg_out_c%d" % j])
 
 
-def test_reference_nms_module_if_built():
-    """Where oracle/_ref holds the compiled reference (build container, GPU box), the oracle is also checked live
-    against it on fresh random lists."""
-    from oracle import build_ref
-    ref = build_ref.load_nms()
-    if ref is None:
-        pytest.skip("oracle/_ref nms module not built")
+SOFT_NMS_LIVE = ((2, 0.5), (1, 0.3), (0, 0.4))      # (method, Nt)
+
+
+def soft_nms_live_boxes(i):
+    """The i-th of three seeded 70-box lists (drawn in order from one generator)."""
     rng = np.random.default_rng(5)
-    for method, Nt in ((2, 0.5), (1, 0.3), (0, 0.4)):
+    for _ in range(i + 1):
         x = rng.uniform(0, 200, 70); y = rng.uniform(0, 200, 70)
         b = np.stack([x, y, x + rng.uniform(10, 90, 70), y + rng.uniform(10, 90, 70), rng.uniform(0, 1, 70)], 1).astype(np.float32)
-        a1, a2 = b.copy(), b.copy()
-        keep = ref.soft_nms(a1, Nt=Nt, method=method)
-        assert O.soft_nms(a2, Nt=Nt, method=method) == len(keep)
-        np.testing.assert_array_equal(a1, a2)
+    return b
+
+
+def test_reference_nms_module_if_built():
+    """The oracle against the reference's compiled soft_nms (oracle/_ref) on seeded random lists; the reference's
+    results are stored in tests/golden/soft_nms_ref.npz (tests/golden/make_golden_soft_nms.py)."""
+    g = golden("soft_nms_ref")
+    for i, (method, Nt) in enumerate(SOFT_NMS_LIVE):
+        a2 = soft_nms_live_boxes(i).copy()
+        assert O.soft_nms(a2, Nt=Nt, method=method) == len(g["keep_%d" % i])
+        np.testing.assert_array_equal(g["boxes_out_%d" % i], a2)
 
 
 # --------------------------------------------------------------------------- GPU: the CUDA path

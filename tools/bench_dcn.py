@@ -1,4 +1,4 @@
-"""Times the DCNv2 forward/backward kernels on dla_34-style layers (B200): tcgen05 (3xTF32) forward vs the
+"""Times the DCNv2 forward/backward kernels on dla_34-style layers (H100): wgmma (3xTF32) forward vs the
 fp32 CUDA-core forward vs torchvision.ops.deform_conv2d (if present), and checks them against each other."""
 import sys, time
 import torch
@@ -19,7 +19,7 @@ def run(B, Cin, H, W, Cout, iters=20):
     def tc(): C.dcnv2_forward(ptr(x), ptr(off), ptr(msk), ptr(w), ptr(bias), ptr(out_tc), B, Cin, H, W, Cout, 3, 3, 1, 1, 1, 1, 1, 1, 1, ptr(ws), ws.numel(), s)
     def fp(): C.dcnv2_forward(ptr(x), ptr(off), ptr(msk), ptr(w), ptr(bias), ptr(out_fp), B, Cin, H, W, Cout, 3, 3, 1, 1, 1, 1, 1, 1, 1, 0, 0, s)
     res = {}
-    for name, fn in (('tcgen05_3xtf32', tc), ('fp32_cuda_core', fp)):
+    for name, fn in (('wgmma_3xtf32', tc), ('fp32_cuda_core', fp)):
         for _ in range(3): fn()
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -39,7 +39,7 @@ def run(B, Cin, H, W, Cout, iters=20):
         err_tv = (out_fp - ref).abs().max().item()
     except Exception as e:
         err_tv = str(e)[:40]
-    # forward + backward through autograd (this library: tcgen05 forward + fp32 backward kernels)
+    # forward + backward through autograd (this library: wgmma forward + fp32 backward kernels)
     try:
         from centernet_b200.dcn_v2_func import DCNv2Function
         from torchvision.ops import deform_conv2d

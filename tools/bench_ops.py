@@ -1,4 +1,4 @@
-"""Times the other hot-path kernels on BASELINE-config geometries (one B200) and prints achieved GB/s against
+"""Times the other hot-path kernels on BASELINE-config geometries (one H100) and prints achieved GB/s against
 their algorithmic bytes (SURVEY.md section 8d): focal(+splat) fwd+bwd, edge aggregation, multi_pose / exct decode."""
 import sys, json
 import torch

@@ -1,5 +1,5 @@
 """One launch (after one warm-up) of every non-decode hot-path kernel at BASELINE-config geometries, for
-`ncu --set full -k regex:k_` captures (profiles/r1_ops_*).  Not a benchmark: numbers under ncu are never bench values."""
+`ncu --set full -k regex:k_` captures.  Not a benchmark: numbers under ncu are never bench values."""
 import sys
 import torch
 sys.path.insert(0, '.')

@@ -28,7 +28,7 @@ for i in range(60):
 e1.record(); torch.cuda.synchronize()
 print("B=%d wb=%s: %.4f ms per call" % (B, os.environ.get("CNB_SELECT_WB", "default"), e0.elapsed_time(e1) / 60))
 lib = ctypes.CDLL(os.path.join(os.path.dirname(centernet_b200.__file__), "lib", "libcenternet_b200.so"))
-n = 148
+n = 132
 full = np.zeros((192, 10), np.uint64)
 assert lib.cnb_debug_select_stats(full.ctypes.data_as(ctypes.c_void_p), 192) == 0
 out = full[:n]
