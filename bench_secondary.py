@@ -193,24 +193,32 @@ def run(dev, batches, K=100, steps=20):
                                     config="DCNv2 backward (fwd_bwd_ms - forward; dX by 16-byte vector reductions, the other "
                                            "four gradients bit-identical run to run)")
             r["fwd_bwd_over_fwd"] = round(r["fwd_bwd_ms"] / ms, 2)
-            try:   # deterministic dX (cnb_dcnv2_set_deterministic): offsets held inside the gather window
-                from centernet_b200._lib import C as _C
-                leaves_d = [t.clone().requires_grad_(True) for t in (x, off.clamp(-1.9, 1.9), msk, w, bias)]
-
-                def fbd():
-                    for t in leaves_d:
-                        t.grad = None
-                    fn(*leaves_d).sum().backward()
-                import centernet_b200.dcn_v2_func as _f
-                prev = _f._DETERMINISTIC
-                _f._DETERMINISTIC = True
+            # deterministic mode (cnb_dcnv2_set_deterministic: fixed-point dX): offsets clamped to +-1.9 px (the
+            # historical case), the layer's free offsets (randn * 2, as the forward is timed) and the same with a
+            # channels_last activation (input and grad_input stay channels-last)
+            xcl = x.contiguous(memory_format=torch.channels_last)
+            for key, xin, oin in (("fwd_bwd_deterministic_ms", x, off.clamp(-1.9, 1.9)),
+                                  ("fwd_bwd_deterministic_free_ms", x, off),
+                                  ("fwd_bwd_deterministic_free_cl_ms", xcl, off)):
                 try:
-                    r["fwd_bwd_deterministic_ms"] = round(timeit(fbd, 3, 1), 5)
-                finally:
-                    _f._DETERMINISTIC = prev
-                    _C.dcnv2_set_deterministic(0)
-            except Exception as e:   # noqa: BLE001
-                r["fwd_bwd_deterministic_ms"] = "failed: %r" % (e,)
+                    from centernet_b200._lib import C as _C
+                    leaves_d = [t.clone().requires_grad_(True) for t in (xin, oin, msk, w, bias)]
+
+                    def fbd(leaves_d=leaves_d):
+                        for t in leaves_d:
+                            t.grad = None
+                        fn(*leaves_d).sum().backward()
+                    import centernet_b200.dcn_v2_func as _f
+                    prev = _f._DETERMINISTIC
+                    _f._DETERMINISTIC = True
+                    try:
+                        r[key] = round(timeit(fbd, 3, 1), 5)
+                    finally:
+                        _f._DETERMINISTIC = prev
+                        _C.dcnv2_set_deterministic(0)
+                except Exception as e:   # noqa: BLE001
+                    r[key] = "failed: %r" % (e,)
+            del xcl
             if have_ref:
                 r["reference_gpu_fwd_ms"] = round(timeit(lambda: ref_gpu.dcn_v2_forward(x, off, msk, w, bias), 5, 2), 5)
                 go = torch.ones(b, co, hh, hh, device=dev)

@@ -370,10 +370,12 @@ k_dcn_bwd_data(const float *__restrict__ x, const float *__restrict__ offset, co
 // grid = (channel chunks, Cout/64, pixel-range splits).  Each CTA keeps a [8*KT][64] tile of dW in
 // registers (9 x 2 per thread), walks its range of (image, pixel-tile) pairs rebuilding the masked
 // column tile, and adds the tile to grad_weight once (atomicAdd: grad_weight accumulates, as in
-// dcn_v2_cuda.c:217-220).
+// dcn_v2_cuda.c:217-220).  wpart != NULL (deterministic mode): the tile is stored as the split's partial
+// wpart[split][o][cin][KT] instead (every element has one writer per split) and k_dcn_bwd_wsum adds the partials.
 __global__ void __launch_bounds__(DCN_THREADS, 1)
 k_dcn_bwd_weight(const float *__restrict__ x, const float *__restrict__ offset, const float *__restrict__ mask,
-                 const float *__restrict__ gy, float *__restrict__ gw, const DcnShape s, int splits) {
+                 const float *__restrict__ gy, float *__restrict__ gw, float *__restrict__ wpart, const DcnShape s,
+                 int splits) {
   extern __shared__ __align__(16) unsigned char dcn_smem[];
   const int KT = s.kh * s.kw;
   constexpr int KC = DCN_CK * DCN_KT_MAX;
@@ -439,9 +441,37 @@ k_dcn_bwd_weight(const float *__restrict__ x, const float *__restrict__ offset, 
   for (int i = 0; i < 9; ++i) {
     const int kk = kg + 8 * i;
     if (kk >= kc) continue;
+    if (wpart) {
+      float *wp = wpart + (long long)blockIdx.z * s.Cout * s.Cin * KT;
+      if (lane < on) wp[((long long)(o0 + lane) * s.Cin + c0) * KT + kk] = acc[i][0];
+      if (lane + 32 < on) wp[((long long)(o0 + lane + 32) * s.Cin + c0) * KT + kk] = acc[i][1];
+      continue;
+    }
     if (lane < on) atomicAdd(gw + ((long long)(o0 + lane) * s.Cin + c0) * KT + kk, acc[i][0]);
     if (lane + 32 < on) atomicAdd(gw + ((long long)(o0 + lane + 32) * s.Cin + c0) * KT + kk, acc[i][1]);
   }
+}
+
+// gw[i] += sum over splits (ascending) of wpart[split][i]
+__global__ void __launch_bounds__(256) k_dcn_bwd_wsum(const float *__restrict__ wpart, float *__restrict__ gw,
+                                                      long long n, int splits) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float acc = 0.f;
+    for (int sp = 0; sp < splits; ++sp) acc += __ldg(wpart + (long long)sp * n + i);
+    gw[i] += acc;
+  }
+}
+
+// pixel-range splits of k_dcn_bwd_weight: about two CTAs per SM
+static int fp32_weight_splits(int b, int cin, int cout, int dg, long long tiles) {
+  const int cpg = cin / dg;
+  const int chunks = dg * ((cpg + DCN_CK - 1) / DCN_CK);
+  const int cot = (cout + 63) / 64;
+  const long long work = (long long)b * tiles;
+  int splits = (int)((2ll * num_sms() + (long long)chunks * cot - 1) / ((long long)chunks * cot));
+  if (splits < 1) splits = 1;
+  if ((long long)splits > work) splits = (int)work;
+  return splits;
 }
 
 // dBias[o] += sum_{b,p} dY[b,o,p]   (dcn_v2_cuda.c:225-230)
@@ -500,11 +530,12 @@ int dcn_forward_tc(const float *input, const float *offset, const float *mask, c
                    const float *bias, float *output, int b, int cin, int h, int w, int cout, int kh, int kw, int sh,
                    int sw, int ph, int pw, int dh, int dw, int dg, void *workspace, cudaStream_t stream);
 size_t dcn_tc_bwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg);
+size_t dcn_tc_bwd_det_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg);
 extern std::atomic<int> g_dcn_deterministic;
 int dcn_backward_data_tc(const float *input, const float *offset, const float *mask, const float *weight,
                          const float *grad_output, float *grad_input, float *grad_offset, float *grad_mask, int b,
                          int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
-                         int dg, void *workspace, cudaStream_t stream, int xt_ready, int layout);
+                         int dg, void *workspace, cudaStream_t stream, int xt_ready, int layout, int det_mode);
 int dcn_backward_weight_tc(const float *input, const float *offset, const float *mask, const float *grad_output,
                            float *grad_weight, float *grad_bias, int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int sw,
                            int ph, int pw, int dh, int dw, int dg, void *workspace, cudaStream_t stream, int xt_ready,
@@ -512,6 +543,22 @@ int dcn_backward_weight_tc(const float *input, const float *offset, const float 
 }
 
 using namespace cnb;
+
+// Workspace of the tensor-core backward (0: not covered).  Deterministic mode appends one region, used first by the
+// fixed-point dX of the data pass and then, for cout > 256, by the per-split partials of the fp32 dW kernel.
+static size_t dcn_bwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int stride, int pad,
+                                      int dil, int dg, bool det) {
+  const size_t base = dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg);
+  if (!base || !det) return base;
+  size_t extra = dcn_tc_bwd_det_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg);
+  if (cout > 256) {
+    const long long ho = (h + 2 * pad - (dil * (kh - 1) + 1)) / stride + 1, wo = (w + 2 * pad - (dil * (kw - 1) + 1)) / stride + 1;
+    const long long tiles = (ho * wo + DCN_TP - 1) / DCN_TP;
+    const size_t wpart = align_up((size_t)fp32_weight_splits(b, cin, cout, dg, tiles) * cout * cin * kh * kw * 4, 256);
+    if (wpart > extra) extra = wpart;
+  }
+  return base + extra;
+}
 
 extern "C" {
 
@@ -534,7 +581,7 @@ size_t cnb_dcnv2_backward_workspace_bytes(int b, int cin, int cout, int h, int w
   if (b <= 0 || h <= 0 || w <= 0 || cin <= 0 || cout <= 0 || dg <= 0 || cin % dg != 0 || kh * kw > DCN_KT_MAX ||
       stride <= 0 || dil <= 0 || pad < 0)
     return 0;
-  return dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg);
+  return dcn_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg, cnb_dcnv2_get_deterministic() != 0);
 }
 
 size_t cnb_dcnv2_wtiles_bytes(int cin, int cout, int kh, int kw, int dg) {
@@ -664,24 +711,28 @@ static int dcnv2_backward_impl(const float *input, const float *offset, const fl
   constexpr int KC = DCN_CK * DCN_KT_MAX;
   int launches = 0;
   // tensor-core path (dcnv2_bwd_tc.cu) when the caller provides the workspace; else the fp32 CUDA-core kernels below
+  const bool det = cnb_dcnv2_get_deterministic() != 0;
   const bool iso = stride_h == stride_w && pad_h == pad_w && dil_h == dil_w;
   const size_t need = (iso && kh * kw <= DCN_KT_MAX)
-                          ? dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride_h, pad_h, dil_h, deformable_groups)
+                          ? dcn_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride_h, pad_h, dil_h, deformable_groups, det)
                           : 0;
   const bool tc = workspace && need > 0 && workspace_bytes >= need && (reinterpret_cast<uintptr_t>(workspace) & 15u) == 0;
+  // deterministic mode is implemented by the tensor-core backward only (the fp32 kernels scatter with atomics)
+  CNB_REQUIRE(!det || tc || !(grad_input || grad_offset || grad_mask || grad_weight), CNB_EUNSUPPORTED,
+              "cnb_dcnv2_backward: deterministic mode (cnb_dcnv2_set_deterministic) needs the tensor-core backward: a "
+              "workspace of cnb_dcnv2_backward_workspace_bytes queried in deterministic mode, at most 9 taps, isotropic "
+              "stride/pad/dilation and images within its 32-bit indexing");
   if (layout) {   // channels-last input / grad_input: tensor-core path only, whole 32-channel blocks, scatter form of dX
     CNB_REQUIRE(tc && cout <= 256, CNB_EUNSUPPORTED, "cnb_dcnv2_backward_ex: channels-last tensors need the tensor-core path "
                 "(workspace of cnb_dcnv2_backward_workspace_bytes, at most 9 taps, isotropic stride/pad/dilation, cout <= 256)");
     CNB_REQUIRE((cin / deformable_groups) % 32 == 0, CNB_EUNSUPPORTED,
                 "cnb_dcnv2_backward_ex: channels-last tensors need cin / deformable_groups to be a multiple of 32");
-    CNB_REQUIRE(!(layout & 2) || !cnb_dcnv2_get_deterministic(), CNB_EUNSUPPORTED,
-                "cnb_dcnv2_backward_ex: a channels-last grad_input is not available in deterministic mode");
     if (!grad_input) layout &= ~2;
   }
   if (tc && (grad_input || grad_offset || grad_mask)) {
     rc = dcn_backward_data_tc(input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask, b, cin, h, w,
                               cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, deformable_groups, workspace,
-                              stream, 0, layout);
+                              stream, 0, layout, det ? 1 : 0);
     if (rc != CNB_OK) return rc;
   } else if (grad_input || grad_offset || grad_mask) {
     const size_t smem = sizeof(BwdMeta) * DCN_KT_MAX * DCN_TP + sizeof(float) * KC * DCN_TP +
@@ -709,17 +760,25 @@ static int dcnv2_backward_impl(const float *input, const float *offset, const fl
     const int cpg = cin / deformable_groups;
     const int chunks = deformable_groups * ((cpg + DCN_CK - 1) / DCN_CK);
     const int cot = (cout + 63) / 64;
-    long long work = (long long)b * tiles;
-    int splits = (int)((2ll * num_sms() + (long long)chunks * cot - 1) / ((long long)chunks * cot));
-    if (splits < 1) splits = 1;
-    if ((long long)splits > work) splits = (int)work;
+    const int splits = fp32_weight_splits(b, cin, cout, deformable_groups, tiles);
     const size_t smem = sizeof(TapMeta) * DCN_KT_MAX * DCN_TP + sizeof(float) * KC * DCN_TP +
                         sizeof(float) * DCN_TP * 65;
+    // deterministic mode (tc here): per-split partials in the region behind the tensor-core workspace
+    float *wpart = det ? reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) +
+                                                   dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride_h, pad_h,
+                                                                              dil_h, deformable_groups))
+                       : nullptr;
     CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((unsigned)chunks, (unsigned)cot, (unsigned)splits);
-    k_dcn_bwd_weight<<<grid, DCN_THREADS, smem, stream>>>(input, offset, mask, grad_output, grad_weight, s, splits);
+    k_dcn_bwd_weight<<<grid, DCN_THREADS, smem, stream>>>(input, offset, mask, grad_output, grad_weight, wpart, s, splits);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight");
     ++launches;
+    if (wpart) {
+      const long long n = (long long)cout * cin * kh * kw;
+      k_dcn_bwd_wsum<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(wpart, grad_weight, n, splits);
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight partials");
+      ++launches;
+    }
   }
   if (grad_bias) {
     k_dcn_bwd_bias<<<cout, 256, 0, stream>>>(grad_output, grad_bias, b, cout, HWo);

@@ -13,6 +13,11 @@
 //                       dX = dcol * mask * corner weight with 16-byte vector reductions (red.global.add.v4.f32:
 //                       a quarter of the reference's per-element atomicAdds, :182-239) into a channels-last dX
 //   k_dcn_bwd_dx_nchw   adds the channels-last dX into the caller's NCHW gradient
+// Deterministic mode (cnb_dcnv2_set_deterministic) keeps the scatter but makes it order-independent: every dX
+// contribution is rounded to a 64-bit fixed-point integer with a per-image power-of-two scale and added with
+// red.global.add.u64 (integer addition is associative: any order, grid or batch split gives the same sum);
+// k_dcn_bwd_dx_fixed then converts the integers back to fp32 into grad_input (NCHW or channels-last).  The
+// scale comes from a bound on |dX| that holds before any contribution is made (see det_scale).
 // The weight gradient dW[o][ch][tap] = sum_{b,p} dY[b][o][p] * col[b][p][ch][tap] is a GEMM with K = pixels:
 // k_dcn_bwd_weight_tc rebuilds the masked column tile in shared memory exactly as the forward sampler does
 // (never in HBM), keeps a [128 rows = 4 chunks x 32 ch] x (64|128 output channels) accumulator in the registers of two
@@ -45,13 +50,26 @@ static BwdGeom bwd_geom(const DcnShapeTc &s) {
   return g;
 }
 
-// W[Cout][Cin][KT] -> per (row group rg, slice ks): [128 rows = (chunk ql, ch)][32 k = output channel], hi then lo
+// Bounds of deterministic mode, as the bits of non-negative floats (integer max of those bits is the float max,
+// NaN > inf > finite, and max is order-free): bnd[ks] = max over rows r of sum_{o in slice ks} |W[o][r]|,
+// bnd[KS + 2b] = max |dY| of image b, bnd[KS + 2b + 1] = max |mask| of image b.
+__device__ __forceinline__ unsigned abs_bits(float v) { return __float_as_uint(v) & 0x7fffffffu; }
+__device__ __forceinline__ unsigned warp_max_u32(unsigned v) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, d));
+  return v;
+}
+
+// W[Cout][Cin][KT] -> per (row group rg, slice ks): [128 rows = (chunk ql, ch)][32 k = output channel], hi then lo.
+// DET: also bnd[ks] (a warp holds one row's 32 output channels of the slice per iteration: lane = k).
+template <bool DET>
 __global__ void __launch_bounds__(256) k_bwd_prep_w(const float *__restrict__ w, const DcnShapeTc s, const BwdGeom g,
-                                                    float *__restrict__ wtt) {
+                                                    float *__restrict__ wtt, unsigned *__restrict__ bnd) {
   const int KT = s.kh * s.kw, cpg = s.Cin / s.dg;
   const int rg = blockIdx.x / g.KS, ks = blockIdx.x - rg * g.KS;
   unsigned char *hi = reinterpret_cast<unsigned char *>(wtt + (size_t)blockIdx.x * BW_TILE_FLOATS);
   unsigned char *lo = hi + TC_A_BYTES;
+  unsigned rmax = 0;
   for (int i = threadIdx.x; i < TC_TP * TC_K; i += blockDim.x) {
     const int k = i & (TC_K - 1), row = i >> 5;
     const int q = rg * 4 + (row >> 5), ch = row & 31;
@@ -63,12 +81,22 @@ __global__ void __launch_bounds__(256) k_bwd_prep_w(const float *__restrict__ w,
     const float h = tf32_hi(v);
     *reinterpret_cast<float *>(hi + tc_tile_off(row, k)) = h;
     *reinterpret_cast<float *>(lo + tc_tile_off(row, k)) = v - h;
+    if (DET) {
+      float sum = fabsf(v);
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
+      rmax = max(rmax, abs_bits(sum));
+    }
   }
+  if (DET && (threadIdx.x & 31) == 0) atomicMax(bnd + ks, rmax);
 }
 
 // dY [B][Cout][HWo] -> per (image, pixel tile, slice ks): [128 px][32 k = output channel], hi then lo.  grid (tiles, KS, B)
+// DET: also the bounds max |dY| and (blocks of slice 0, over the tile's pixels) max |mask| of each image.
+template <bool DET>
 __global__ void __launch_bounds__(256) k_bwd_prep_gy(const float *__restrict__ gy, const DcnShapeTc s, const BwdGeom g,
-                                                     float *__restrict__ gyt) {
+                                                     float *__restrict__ gyt, const float *__restrict__ mask,
+                                                     unsigned *__restrict__ bnd_img) {
   const int t = blockIdx.x, ks = blockIdx.y, b = blockIdx.z;
   const int pp = threadIdx.x & (TC_TP - 1), half = threadIdx.x >> 7;
   const int ho = (t / s.tiles_x) * s.th + pp / s.tw, wo = (t % s.tiles_x) * s.tw + pp % s.tw;
@@ -76,6 +104,7 @@ __global__ void __launch_bounds__(256) k_bwd_prep_gy(const float *__restrict__ g
   const long long HWo = (long long)s.Ho * s.Wo, p = (long long)ho * s.Wo + wo;
   unsigned char *hi = reinterpret_cast<unsigned char *>(gyt + ((size_t)((size_t)b * g.tiles + t) * g.KS + ks) * BW_TILE_FLOATS);
   unsigned char *lo = hi + TC_A_BYTES;
+  unsigned ymax = 0;
 #pragma unroll
   for (int kc = 0; kc < 4; ++kc) {
     const int kq = half * 4 + kc;
@@ -84,12 +113,45 @@ __global__ void __launch_bounds__(256) k_bwd_prep_gy(const float *__restrict__ g
     for (int j = 0; j < 4; ++j) {
       const int o = ks * TC_K + kq * 4 + j;
       v[j] = (ok && o < s.Cout) ? __ldg(gy + ((long long)b * s.Cout + o) * HWo + p) : 0.f;
+      if (DET) ymax = max(ymax, abs_bits(v[j]));
     }
     const float4 h4 = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
     const uint32_t off = tc_tile_off(pp, kq * 4);
     *reinterpret_cast<float4 *>(hi + off) = h4;
     *reinterpret_cast<float4 *>(lo + off) = make_float4(v[0] - h4.x, v[1] - h4.y, v[2] - h4.z, v[3] - h4.w);
   }
+  if (DET) {
+    unsigned mmax = 0;
+    if (ks == 0 && ok) {
+      const float *mp = mask + (long long)b * s.mask_bs + p;
+      for (int c = half; c < s.dg * s.kh * s.kw; c += 2) mmax = max(mmax, abs_bits(__ldg(mp + (long long)c * HWo)));
+    }
+    ymax = warp_max_u32(ymax);
+    mmax = warp_max_u32(mmax);
+    if ((threadIdx.x & 31) == 0) {
+      atomicMax(bnd_img + 2 * b, ymax);
+      if (mmax) atomicMax(bnd_img + 2 * b + 1, mmax);
+    }
+  }
+}
+
+// Scale of image b's fixed-point dX, or 0 when its bounds are not finite.  A dX element collects at most one
+// contribution dcol * mask * w_corner (w_corner <= 1) per sampling point that can reach it: KT * HWo of them, and
+//   |dcol[p][c,tap]| <= sum_o |W[o][c][tap]| * max|dY_b| <= A * Y_b,   A = sum_ks bnd[ks],
+// so |dX| <= KT * HWo * A * Y_b * M_b = bound.  The scale is the power of two with bound * scale < 2^61: one bit
+// below the 2^62 that the int64 sums stay under, as margin for the rounding of dcol (3xTF32), of the float sums
+// behind A and of the products.  Resolution: bound * 2^-61 (64@128^2: KT * HWo = 2^17.2, so 2^-43.8 * A * Y_b * M_b).
+__device__ __forceinline__ double det_scale(const unsigned *__restrict__ bnd, const DcnShapeTc &s, const BwdGeom &g,
+                                            int b) {
+  double a = 0.0;
+  for (int ks = 0; ks < g.KS; ++ks) a += (double)__uint_as_float(bnd[ks]);
+  const double bound = (double)(s.kh * s.kw) * ((double)s.Ho * s.Wo) * a * (double)__uint_as_float(bnd[g.KS + 2 * b]) *
+                       (double)__uint_as_float(bnd[g.KS + 2 * b + 1]);
+  if (!(bound <= 1e300)) return 0.0;   // inf or NaN in dY, W or the mask
+  if (bound == 0.0) return 1.0;        // every contribution is zero
+  int ex;
+  frexp(bound, &ex);                   // bound < 2^ex
+  return ldexp(1.0, 61 - ex);
 }
 
 // ------------------------------------------------------------------ dcol = dY^T . W   (item = image, pixel tile, row group)
@@ -176,24 +238,28 @@ __device__ __forceinline__ float dot4(const float4 a, const float4 b) {
   return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x)));
 }
 
+// dX contribution of one corner in deterministic mode: the fp32 products of the default scatter, each rounded to
+// the nearest multiple of 1/qs (exact power-of-two scaling in double) and added as a two's-complement integer
+__device__ __forceinline__ void red_add_s64(long long *addr, long long v) {
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(addr), "l"(v) : "memory");
+}
+__device__ __forceinline__ void red_fixed4(long long *addr, const float4 dm, float wgt, double qs) {
+  const long long v0 = __double2ll_rn((double)(dm.x * wgt) * qs), v1 = __double2ll_rn((double)(dm.y * wgt) * qs);
+  const long long v2 = __double2ll_rn((double)(dm.z * wgt) * qs), v3 = __double2ll_rn((double)(dm.w * wgt) * qs);
+  if (v0) red_add_s64(addr, v0);
+  if (v1) red_add_s64(addr + 1, v1);
+  if (v2) red_add_s64(addr + 2, v2);
+  if (v3) red_add_s64(addr + 3, v3);
+}
+
 // Geometry of one (tap, pixel): fractional parts, mask and (hl*W + wl + W + 1) << 7 | flags
-// (bit 0-3: corner in range, 4: sampling point inside (-1,H)x(-1,W), 5: pixel inside the output map,
-//  6: "near" -- the top-left corner lies within [-GX_RD, GX_RD + 1] of the pixel's own input position, so the
-//  sample's dX contribution is collected by the deterministic gather (k_dcn_bwd_dx_gather) instead of scattered).
-constexpr int GX_RD = 2;                       // offsets of magnitude < 2 pixels are always near
-constexpr int GX_WIN = 2 * GX_RD + 3;          // candidate output rows / columns per input position
-constexpr int GX_TH = 8, GX_TW = 16;           // input positions per CTA
-constexpr int GX_WH = GX_TH + GX_WIN - 1, GX_WW = GX_TW + GX_WIN - 1;
-constexpr int GX_NC = GX_WIN * GX_WIN * TC_NT; // candidates per position (441)
-constexpr int GX_ROUNDS = (GX_NC + 31) / 32;
-constexpr int GX_LIST = GX_ROUNDS * 32;        // hit list capacity per warp (every candidate a hit)
+// (bit 0-3: corner in range, 4: sampling point inside (-1,H)x(-1,W), 5: pixel inside the output map).
 struct __align__(16) BwdMetaTc {
   float lh, lw, m;
   int packed;
 };
 __device__ __forceinline__ BwdMetaTc bwd_meta(const DcnShapeTc &s, const float *__restrict__ off_img,
-                                              const float *__restrict__ mask_img, int gi, int tap, int ho, int wo,
-                                              bool gather = false) {
+                                              const float *__restrict__ mask_img, int gi, int tap, int ho, int wo) {
   const int KT = s.kh * s.kw;
   const long long HWo = (long long)s.Ho * s.Wo;
   BwdMetaTc mt;
@@ -220,8 +286,6 @@ __device__ __forceinline__ BwdMetaTc bwd_meta(const DcnShapeTc &s, const float *
       if (hl + 1 <= s.H - 1 && wl >= 0) flags |= 4;
       if (hl + 1 <= s.H - 1 && wl + 1 <= s.W - 1) flags |= 8;
       base = hl * s.W + wl + s.W + 1;
-      const int dh_ = hl - (ho * s.sh - s.ph), dw_ = wl - (wo * s.sw - s.pw);
-      if (gather && dh_ >= -GX_RD && dh_ <= GX_RD + 1 && dw_ >= -GX_RD && dw_ <= GX_RD + 1) flags |= 64;
     }
     mt.packed = (base << 7) | flags;
   }
@@ -236,10 +300,10 @@ template <int MINB>
 __global__ void __launch_bounds__(256, MINB)
 k_dcn_bwd_offmask(const float *__restrict__ xt, const float *__restrict__ offset, const float *__restrict__ mask,
                   const float *__restrict__ dcol, float *__restrict__ dxt, float *__restrict__ goff,
-                  float *__restrict__ gmask, float *__restrict__ gx_far, const DcnShapeTc s, const BwdGeom g,
-                  const int b_first) {
+                  float *__restrict__ gmask, long long *__restrict__ dxi, const unsigned *__restrict__ bnd,
+                  const DcnShapeTc s, const BwdGeom g, const int b_first) {
   // dxt != NULL: every sample is scattered into the channels-last dX (16-byte reductions);
-  // gx_far != NULL: near samples are left to k_dcn_bwd_dx_gather, far ones go to the NCHW gradient with scalar atomics
+  // dxi != NULL (deterministic mode): into the fixed-point dX of the batch chunk [bl][HW][Cp] (scale from bnd)
   __shared__ BwdMetaTc meta[TC_NT * TC_TP];
   const int KT = s.kh * s.kw;
   const long long HWo = (long long)s.Ho * s.Wo, HW = (long long)s.H * s.W;
@@ -253,6 +317,8 @@ k_dcn_bwd_offmask(const float *__restrict__ xt, const float *__restrict__ offset
   const float *off_img = offset + (long long)b * s.off_bs, *mask_img = mask + (long long)b * s.mask_bs;
   const float *x_img = xt + (long long)b * HW * Cp + c4 * 4;
   float *dx_img = dxt ? dxt + (long long)b * HW * Cp + c4 * 4 : nullptr;
+  const double qs = dxi ? det_scale(bnd, s, g, b) : 0.0;     // 0: non-finite bounds, k_dcn_bwd_dx_fixed writes NaN
+  long long *dxi_img = qs != 0.0 ? dxi + (long long)bl * HW * Cp + c4 * 4 : nullptr;
   const float *dc_img = dcol + (long long)bl * HWo * g.Qp * TC_CB + c4 * 4;
   float *gmask_img = gmask ? gmask + (long long)b * s.mask_bs : nullptr;
   float *goff_img = goff ? goff + (long long)b * s.off_bs : nullptr;
@@ -263,7 +329,7 @@ k_dcn_bwd_offmask(const float *__restrict__ xt, const float *__restrict__ offset
     __syncthreads();
     for (int idx = threadIdx.x; idx < KT * TC_TP; idx += 256) {
       const int tap = idx >> 7, pp = idx & (TC_TP - 1);
-      meta[idx] = bwd_meta(s, off_img, mask_img, gi, tap, ty0 + (pp >> tws), tx0 + (pp & (s.tw - 1)), gx_far != nullptr);
+      meta[idx] = bwd_meta(s, off_img, mask_img, gi, tap, ty0 + (pp >> tws), tx0 + (pp & (s.tw - 1)));
     }
     __syncthreads();
     const int cb0 = gi * s.cbs_pg;
@@ -300,7 +366,6 @@ k_dcn_bwd_offmask(const float *__restrict__ xt, const float *__restrict__ offset
       const bool f1 = flags & 1, f2 = flags & 2, f3 = flags & 4, f4 = flags & 8;
       const float lh = cur.mt.lh, lw = cur.mt.lw, hh = 1.f - lh, hw = 1.f - lw, m = cur.mt.m;
       const float w1 = hh * hw, w2 = hh * lw, w3 = lh * hw, w4 = lh * lw;
-      const int base = (cur.mt.packed >> 7) - (s.W + 1);
       int xo = cur.xo, dco = cur.dco;
       float am = 0.f, ah = 0.f, aw = 0.f;
 #pragma unroll 1
@@ -335,19 +400,11 @@ k_dcn_bwd_offmask(const float *__restrict__ xt, const float *__restrict__ offset
             if (f2 && w2 != 0.f) red_add_v4(dx_img + (xo + xs1), dm.x * w2, dm.y * w2, dm.z * w2, dm.w * w2);
             if (f3 && w3 != 0.f) red_add_v4(dx_img + (xo + xs2), dm.x * w3, dm.y * w3, dm.z * w3, dm.w * w3);
             if (f4 && w4 != 0.f) red_add_v4(dx_img + (xo + xs3), dm.x * w4, dm.y * w4, dm.z * w4, dm.w * w4);
-          } else if (gx_far && !(flags & 64)) {
-            const int cw = cbi * TC_CB + c4 * 4, cpg = s.Cin / s.dg;     // channel within the group (pad slots skipped)
-            float *gp = gx_far + ((long long)b * s.Cin + gi * cpg + cw) * HW + base;
-            const float dv[4] = {dm.x, dm.y, dm.z, dm.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              if (cw + i >= cpg) break;
-              float *q = gp + (long long)i * HW;
-              if (f1 && w1 != 0.f) atomicAdd(q, dv[i] * w1);
-              if (f2 && w2 != 0.f) atomicAdd(q + 1, dv[i] * w2);
-              if (f3 && w3 != 0.f) atomicAdd(q + s.W, dv[i] * w3);
-              if (f4 && w4 != 0.f) atomicAdd(q + s.W + 1, dv[i] * w4);
-            }
+          } else if (dxi_img) {
+            if (f1 && w1 != 0.f) red_fixed4(dxi_img + xo, dm, w1, qs);
+            if (f2 && w2 != 0.f) red_fixed4(dxi_img + (xo + xs1), dm, w2, qs);
+            if (f3 && w3 != 0.f) red_fixed4(dxi_img + (xo + xs2), dm, w3, qs);
+            if (f4 && w4 != 0.f) red_fixed4(dxi_img + (xo + xs3), dm, w4, qs);
           }
         }
         xo += TC_CB;
@@ -375,130 +432,6 @@ k_dcn_bwd_offmask(const float *__restrict__ xt, const float *__restrict__ offset
   }
 }
 
-// Deterministic dX for the near samples.  CTA = 8 x 16 input positions of one image; it lays the geometry of every
-// output pixel whose near samples can land in the tile (14 x 22 pixels x 9 taps) into shared memory, then one warp per
-// position walks the position's 441 candidates (tap, row, column) 32 at a time in a FIXED order: a lane tests whether
-// one corner of its candidate is this position; the hits are taken in lane order and every lane (= channel) adds
-// weight * dcol of the hit.  No atomics: two runs give the same bits.  The tile is transposed through shared memory
-// and added to the NCHW gradient (which already holds the far samples' scatter).
-template <int NCB>
-__global__ void __launch_bounds__(256)
-k_dcn_bwd_dx_gather(const float *__restrict__ offset, const float *__restrict__ mask, const float *__restrict__ dcol,
-                    float *__restrict__ gx, const DcnShapeTc s, const BwdGeom g, const int b_first, const int ptx,
-                    const int pty) {
-  extern __shared__ __align__(16) unsigned char gx_smem[];
-  BwdMetaTc *meta = reinterpret_cast<BwdMetaTc *>(gx_smem);                                  // [9][14][22]
-  float(*tile)[GX_TH * GX_TW + 1] =
-      reinterpret_cast<float(*)[GX_TH * GX_TW + 1]>(gx_smem + sizeof(BwdMetaTc) * TC_NT * GX_WH * GX_WW);   // [NCB*32][129]
-  float2 *mylist = reinterpret_cast<float2 *>(gx_smem + sizeof(BwdMetaTc) * TC_NT * GX_WH * GX_WW +
-                                              (size_t)NCB * TC_CB * (GX_TH * GX_TW + 1) * 4) + (threadIdx.x >> 5) * GX_LIST;   // per warp
-  const int KT = s.kh * s.kw, cpg = s.Cin / s.dg;
-  const long long HWo = (long long)s.Ho * s.Wo, HW = (long long)s.H * s.W;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int tix = blockIdx.x % ptx, tiy = (blockIdx.x / ptx) % pty, bl = blockIdx.x / (ptx * pty);
-  const int b = b_first + bl;
-  const int y0 = tiy * GX_TH, x0 = tix * GX_TW;
-  const int ho0 = y0 + s.ph - GX_RD - 2, wo0 = x0 + s.pw - GX_RD - 2;     // first output row / column of the window (stride 1)
-  const float *off_img = offset + (long long)b * s.off_bs, *mask_img = mask + (long long)b * s.mask_bs;
-  const float *dc_img = dcol + (long long)bl * HWo * g.Qp * TC_CB + lane;
-
-  // candidate (tap, r, c) of this lane in every round: its index into the geometry window and into dcol
-  int moff[GX_ROUNDS], doff[GX_ROUNDS];
-#pragma unroll
-  for (int rnd = 0; rnd < GX_ROUNDS; ++rnd) {
-    const int cand = rnd * 32 + lane;
-    const int tap = cand / (GX_WIN * GX_WIN), rc = cand - tap * (GX_WIN * GX_WIN);
-    const int r = rc / GX_WIN, c = rc - r * GX_WIN;
-    moff[rnd] = cand < GX_NC ? (tap * GX_WH + r) * GX_WW + c : -1;
-    doff[rnd] = ((r * s.Wo + c) * g.Qp + tap) * TC_CB;
-  }
-
-  for (int gi = 0; gi < s.dg; ++gi) {
-    __syncthreads();
-    for (int idx = tid; idx < TC_NT * GX_WH * GX_WW; idx += 256) {
-      const int tap = idx / (GX_WH * GX_WW), rem = idx - tap * (GX_WH * GX_WW);
-      const int ho = ho0 + rem / GX_WW, wo = wo0 + rem % GX_WW;
-      BwdMetaTc mt;
-      mt.lh = mt.lw = mt.m = 0.f;
-      mt.packed = 0;
-      if (ho >= 0 && wo >= 0 && tap < KT) mt = bwd_meta(s, off_img, mask_img, gi, tap, ho, wo, true);
-      meta[idx] = mt;
-    }
-    __syncthreads();
-    for (int cbg = 0; cbg < s.cbs_pg; cbg += NCB) {
-      const int ncb = min(NCB, s.cbs_pg - cbg);
-      // warp = one row of the position tile
-      for (int px = 0; px < GX_TW; ++px) {
-        const int y = y0 + warp, x = x0 + px;
-        float acc[NCB];
-#pragma unroll
-        for (int cb = 0; cb < NCB; ++cb) acc[cb] = 0.f;
-        if (y < s.H && x < s.W) {
-          const int mbase = warp * GX_WW + px;
-          const int posk = y * s.W + x + s.W + 1;
-          const int dbase = (((ho0 + warp) * s.Wo + wo0 + px) * g.Qp + (gi * s.cbs_pg + cbg) * TC_NT) * TC_CB;
-          // pass 1: the hits of this position, in candidate order, as (weight, dcol offset) pairs
-          int cnt = 0;
-#pragma unroll
-          for (int rnd = 0; rnd < GX_ROUNDS; ++rnd) {
-            float wgt = 0.f;
-            bool hit = false;
-            if (moff[rnd] >= 0) {
-              const BwdMetaTc e = meta[moff[rnd] + mbase];
-              if (e.packed & 64) {
-                const int diff = posk - (e.packed >> 7);
-                const float hh = 1.f - e.lh, hw = 1.f - e.lw;
-                if (diff == 0) { hit = e.packed & 1; wgt = hh * hw; }
-                else if (diff == 1) { hit = e.packed & 2; wgt = hh * e.lw; }
-                else if (diff == s.W) { hit = e.packed & 4; wgt = e.lh * hw; }
-                else if (diff == s.W + 1) { hit = e.packed & 8; wgt = e.lh * e.lw; }
-                wgt *= e.m;
-              }
-            }
-            const unsigned hits = __ballot_sync(0xffffffffu, hit);
-            if (hit) mylist[cnt + __popc(hits & ((1u << lane) - 1u))] = make_float2(wgt, __int_as_float(doff[rnd] + dbase));
-            cnt += __popc(hits);
-          }
-          __syncwarp();
-          // pass 2: eight hits' lines in flight at a time, added in list order (every lane = one channel)
-          for (int i0 = 0; i0 < cnt; i0 += 8) {
-            const int n = min(8, cnt - i0);
-            float2 e[8];
-            float v[8][NCB];
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-              if (k < n) {
-                e[k] = mylist[i0 + k];
-#pragma unroll
-                for (int cb = 0; cb < NCB; ++cb)
-                  if (cb < ncb) v[k][cb] = __ldg(dc_img + (__float_as_int(e[k].y) + cb * TC_NT * TC_CB));
-              }
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-              if (k < n) {
-#pragma unroll
-                for (int cb = 0; cb < NCB; ++cb)
-                  if (cb < ncb) acc[cb] = fmaf(e[k].x, v[k][cb], acc[cb]);
-              }
-          }
-          __syncwarp();
-        }
-#pragma unroll
-        for (int cb = 0; cb < NCB; ++cb) tile[cb * TC_CB + lane][warp * GX_TW + px] = acc[cb];
-      }
-      __syncthreads();
-      // tile[channel][position] -> gx[b][channel][y][x], 16 consecutive x per row
-      for (int i = tid; i < ncb * TC_CB * GX_TH * GX_TW; i += 256) {
-        const int pp = i & (GX_TH * GX_TW - 1), cl = i >> 7;
-        const int cw = cbg * TC_CB + cl;                   // channel within the group
-        const int y = y0 + (pp >> 4), x = x0 + (pp & 15);
-        if (cw < cpg && y < s.H && x < s.W) gx[((long long)b * s.Cin + gi * cpg + cw) * HW + (long long)y * s.W + x] += tile[cl][pp];
-      }
-      __syncthreads();
-    }
-  }
-}
-
 // gx[b][ch][pos] += dxt[b][pos][slot(ch)]   (inverse of k_dcn_nhwc).  grid (pixel blocks of 32, channel blocks of 64, B)
 __global__ void __launch_bounds__(256) k_dcn_bwd_dx_nchw(const float *__restrict__ dxt, float *__restrict__ gx,
                                                          const DcnShapeTc s) {
@@ -515,6 +448,49 @@ __global__ void __launch_bounds__(256) k_dcn_bwd_dx_nchw(const float *__restrict
       const int slot = (gi * s.cbs_pg + within / TC_CB) * TC_CB + within % TC_CB;
       for (int px = pr; px < 32; px += 4)
         tile[c][px] = (p0 + px < HW) ? __ldg(dxt + ((long long)b * HW + p0 + px) * Cp + slot) : 0.f;
+    }
+  }
+  __syncthreads();
+  {
+    const int px = threadIdx.x & 31, cr = threadIdx.x >> 5;
+    for (int c = cr; c < 64; c += 8)
+      if (c0 + c < s.Cin && p0 + px < HW) gx[((long long)b * s.Cin + c0 + c) * HW + p0 + px] += tile[c][px];
+  }
+}
+
+// Deterministic mode: gx[b] += dxi[bl] / scale (fixed point -> fp32) for the images b = b_first + bl of a batch
+// chunk; all NaN for an image whose bounds are not finite.  NCHW: as k_dcn_bwd_dx_nchw, grid (pixel blocks of 32,
+// channel blocks of 64, images).  CL (channels-last grad_input, cin/dg % 32 == 0 so slot == channel): grid
+// (pixel blocks of 32, 1, images), 8 warps x 4 pixels of whole channel lines.
+template <bool CL>
+__global__ void __launch_bounds__(256) k_dcn_bwd_dx_fixed(const long long *__restrict__ dxi,
+                                                          const unsigned *__restrict__ bnd, float *__restrict__ gx,
+                                                          const DcnShapeTc s, const BwdGeom g, const int b_first) {
+  const long long HW = (long long)s.H * s.W;
+  const long long p0 = (long long)blockIdx.x * 32;
+  const int bl = blockIdx.z, b = b_first + bl;
+  const int Cp = s.nb * TC_CB, cpg = s.Cin / s.dg;
+  const double qs = det_scale(bnd, s, g, b);
+  const double inv = qs != 0.0 ? 1.0 / qs : __longlong_as_double(0x7ff8000000000000ll);
+  const long long *src = dxi + (long long)bl * HW * Cp;
+  if (CL) {
+    for (int i = threadIdx.x; i < 32 * Cp; i += 256) {
+      const long long p = p0 + i / Cp;
+      const int ch = i % Cp;
+      if (p < HW) gx[((long long)b * HW + p) * Cp + ch] += (float)((double)__ldg(src + p * Cp + ch) * inv);
+    }
+    return;
+  }
+  __shared__ float tile[64][33];
+  const int c0 = blockIdx.y * 64;
+  {
+    const int c = threadIdx.x & 63, pr = threadIdx.x >> 6;
+    const int ch = c0 + c;
+    if (ch < s.Cin) {
+      const int gi = ch / cpg, within = ch - gi * cpg;
+      const int slot = (gi * s.cbs_pg + within / TC_CB) * TC_CB + within % TC_CB;
+      for (int px = pr; px < 32; px += 4)
+        tile[c][px] = (p0 + px < HW) ? (float)((double)__ldg(src + (p0 + px) * Cp + slot) * inv) : 0.f;
     }
   }
   __syncthreads();
@@ -883,11 +859,22 @@ size_t dcn_tc_bwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh
   return 2 * bw_xt_bytes(s) + bw_wtt_bytes(g) + (data > wgt ? data : wgt);
 }
 
-// dX, dOffset, dMask (each nullable; accumulated into, as cnb_dcnv2_backward documents).
+// Deterministic mode appends [bounds: KS + 2B uint32][fixed-point dX of one batch chunk: bc x HW x Cp int64] to the
+// layout above (whose size and use do not change).
+size_t dcn_tc_bwd_det_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg) {
+  DcnShapeTc s;
+  fill_shape(&s, b, cin, h, w, cout, kh, kw, sh, sh, ph, ph, dh, dh, dg);
+  const BwdGeom g = bwd_geom(s);
+  const int bc = bw_batch_chunk(s, g);
+  return align_up((size_t)(g.KS + 2 * b) * 4, 256) + align_up((size_t)bc * h * w * s.nb * TC_CB * 8, 256);
+}
+
+// dX, dOffset, dMask (each nullable; accumulated into, as cnb_dcnv2_backward documents).  det != 0: dX in fixed point
+// (order-independent), which needs the workspace of dcn_tc_bwd_det_bytes behind the default one.
 int dcn_backward_data_tc(const float *input, const float *offset, const float *mask, const float *weight,
                          const float *grad_output, float *grad_input, float *grad_offset, float *grad_mask, int b,
                          int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
-                         int dg, void *workspace, cudaStream_t stream, int xt_ready, int layout) {
+                         int dg, void *workspace, cudaStream_t stream, int xt_ready, int layout, int det_mode) {
   // layout bit 0: `input` already is channels-last [b][h*w][cin]; bit 1: so is grad_input (both need cin/dg % 32 == 0,
   // checked by the caller): the layout passes and the channels-last scratch copies are skipped
   DcnShapeTc s;
@@ -903,16 +890,24 @@ int dcn_backward_data_tc(const float *input, const float *offset, const float *m
   float *gyt = reinterpret_cast<float *>(wp); wp += align_up((size_t)bc * bw_gyt_bytes_per_image(g), 256);
   float *dcol = reinterpret_cast<float *>(wp);
   const long long HW = (long long)h * w, HWo = (long long)s.Ho * s.Wo;
+  // default: every sample is scattered into a channels-last dX (16-byte vector reductions) and added to grad_input at
+  // the end; deterministic mode: into the fixed-point dX of the batch chunk, converted into grad_input per chunk
+  const bool det = grad_input && det_mode;
+  unsigned *bnd = nullptr;
+  long long *dxi = nullptr;
+  if (det) {
+    char *dp = reinterpret_cast<char *>(workspace) + dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, sh, ph, dh, dg);
+    bnd = reinterpret_cast<unsigned *>(dp);
+    dxi = reinterpret_cast<long long *>(dp + align_up((size_t)(g.KS + 2 * b) * 4, 256));
+    CNB_CUDA(cudaMemsetAsync(bnd, 0, (size_t)(g.KS + 2 * b) * 4, stream));
+  }
 
   int rc = CNB_OK;
   if (!xt_ready && !(layout & 1)) rc = dcn_to_channels_last(input, xt, s, stream);
   if (rc != CNB_OK) return rc;
-  // default: every sample is scattered into a channels-last dX (16-byte vector reductions) and added to grad_input at
-  // the end; deterministic mode (cnb_dcnv2_set_deterministic, stride 1): near samples by the gather, the rest by atomics
-  // straight into grad_input
-  const bool gather = grad_input && sh == 1 && sw == 1 && w >= 2 && g_dcn_deterministic.load(std::memory_order_relaxed) != 0;
-  if (grad_input && !gather && !(layout & 2)) CNB_CUDA(cudaMemsetAsync(dxt, 0, (size_t)b * HW * s.nb * TC_CB * 4, stream));
-  k_bwd_prep_w<<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtt);
+  if (grad_input && !det && !(layout & 2)) CNB_CUDA(cudaMemsetAsync(dxt, 0, (size_t)b * HW * s.nb * TC_CB * 4, stream));
+  if (det) k_bwd_prep_w<true><<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtt, bnd);
+  else k_bwd_prep_w<false><<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtt, nullptr);
   CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight tiles");
   count_launch();
   const size_t smem = (size_t)BW_STAGES * BW_STAGE_BYTES;     // operand ring
@@ -926,36 +921,35 @@ int dcn_backward_data_tc(const float *input, const float *offset, const float *m
   for (int b0 = 0; b0 < b; b0 += bc) {
     const int nbimg = (b - b0 < bc) ? b - b0 : bc;
     dim3 pgrid((unsigned)g.tiles, (unsigned)g.KS, (unsigned)nbimg);
-    k_bwd_prep_gy<<<pgrid, 256, 0, stream>>>(grad_output + (long long)b0 * cout * HWo, s, g, gyt);
+    if (det) {
+      CNB_CUDA(cudaMemsetAsync(dxi, 0, (size_t)nbimg * HW * s.nb * TC_CB * 8, stream));
+      k_bwd_prep_gy<true><<<pgrid, 256, 0, stream>>>(grad_output + (long long)b0 * cout * HWo, s, g, gyt,
+                                                      mask + (long long)b0 * s.mask_bs, bnd + g.KS + 2 * b0);
+    } else {
+      k_bwd_prep_gy<false><<<pgrid, 256, 0, stream>>>(grad_output + (long long)b0 * cout * HWo, s, g, gyt, nullptr, nullptr);
+    }
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward grad_output tiles");
     const int n_items = nbimg * g.tiles * g.RG;
     const int grid = n_items < num_sms() ? n_items : num_sms();
     k_dcn_bwd_dcol_tc<<<grid, BW_THREADS, smem, stream>>>(gyt, wtt, dcol, s, g, n_items);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward column gradient (wgmma)");
-    k_dcn_bwd_offmask<3><<<nbimg * g.tiles, 256, 0, stream>>>(xsrc, offset, mask, dcol, (grad_input && !gather) ? dxt : nullptr,
-                                                              grad_offset, grad_mask, gather ? grad_input : nullptr, s, g, b0);
+    k_dcn_bwd_offmask<3><<<nbimg * g.tiles, 256, 0, stream>>>(xsrc, offset, mask, dcol, (grad_input && !det) ? dxt : nullptr,
+                                                              grad_offset, grad_mask, dxi, bnd, s, g, b0);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward offset/mask gradient");
     count_launch(3);
-    if (gather) {
-      const int ptx = (w + GX_TW - 1) / GX_TW, pty = (h + GX_TH - 1) / GX_TH;
-      const int ncb = s.cbs_pg >= 2 ? 2 : 1;
-      const size_t gsm = sizeof(BwdMetaTc) * TC_NT * GX_WH * GX_WW + (size_t)ncb * TC_CB * (GX_TH * GX_TW + 1) * 4 +
-                         (size_t)8 * GX_LIST * sizeof(float2);
-      static thread_local int gdev_done = -1;
-      if (gdev_done != dev) {
-        CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_dx_gather<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-        CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_dx_gather<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-        gdev_done = dev;
+    if (det) {
+      if (layout & 2) {
+        k_dcn_bwd_dx_fixed<true><<<dim3((unsigned)((HW + 31) / 32), 1u, (unsigned)nbimg), 256, 0, stream>>>(
+            dxi, bnd, grad_input, s, g, b0);
+      } else {
+        dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((cin + 63) / 64), (unsigned)nbimg);
+        k_dcn_bwd_dx_fixed<false><<<tgrid, 256, 0, stream>>>(dxi, bnd, grad_input, s, g, b0);
       }
-      if (ncb == 2)
-        k_dcn_bwd_dx_gather<2><<<nbimg * ptx * pty, 256, gsm, stream>>>(offset, mask, dcol, grad_input, s, g, b0, ptx, pty);
-      else
-        k_dcn_bwd_dx_gather<1><<<nbimg * ptx * pty, 256, gsm, stream>>>(offset, mask, dcol, grad_input, s, g, b0, ptx, pty);
-      CNB_CHECK_LAUNCH("cnb_dcnv2_backward input gradient (gather)");
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward input gradient (fixed point)");
       count_launch();
     }
   }
-  if (grad_input && !gather && !(layout & 2)) {
+  if (grad_input && !det && !(layout & 2)) {
     dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((cin + 63) / 64), (unsigned)b);
     k_dcn_bwd_dx_nchw<<<tgrid, 256, 0, stream>>>(dxt, grad_input, s);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward input gradient");

@@ -75,19 +75,21 @@ __global__ void __launch_bounds__(256) k_gather_feat(const float *__restrict__ f
 }
 
 // grad_feat[b, ch, ind[b, m]] += grad_out[b, m, ch]: the adjoint of the gather (autograd of `feat.gather(1, ind)`,
-// models/utils.py:15).  An index may repeat inside an image, hence the atomic add; grad_feat arrives zero-filled.
+// models/utils.py:15).  An index may repeat inside an image: one thread per (image, channel) plane adds the plane's M
+// values in ascending m, so repeats sum in a fixed order without atomics.  grad_feat arrives zero-filled.
 __global__ void __launch_bounds__(256) k_gather_feat_bwd(const float *__restrict__ grad_out,
                                                          const int64_t *__restrict__ ind,
                                                          float *__restrict__ grad_feat, int B, int C, long long HW,
                                                          int M) {
-  const long long total = (long long)B * M * C;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int ch = (int)(i % C);
-    const long long bm = i / C;
-    const int b = (int)(bm / M);
-    const long long sp = ind[bm];
-    if (sp >= 0 && sp < HW) atomicAdd(grad_feat + ((long long)b * C + ch) * HW + sp, grad_out[i]);
+  const long long planes = (long long)B * C;
+  for (long long pl = blockIdx.x * (long long)blockDim.x + threadIdx.x; pl < planes;
+       pl += (long long)gridDim.x * blockDim.x) {
+    const int b = (int)(pl / C), ch = (int)(pl % C);
+    float *gp = grad_feat + pl * HW;
+    for (int m = 0; m < M; ++m) {
+      const long long sp = __ldg(ind + (long long)b * M + m);
+      if (sp >= 0 && sp < HW) gp[sp] += __ldg(grad_out + ((long long)b * M + m) * C + ch);
+    }
   }
 }
 
@@ -224,8 +226,8 @@ int cnb_gather_feat_backward(const float *grad_out, const int64_t *ind, float *g
                              void *stream) {
   CNB_REQUIRE(grad_out && ind && grad_feat, CNB_EINVAL, "cnb_gather_feat_backward: null pointer");
   CNB_REQUIRE(b > 0 && c > 0 && hw > 0 && m > 0, CNB_EINVAL, "cnb_gather_feat_backward: non-positive dimension");
-  const long long total = (long long)b * m * c;
-  const int grid = (int)((total + 255) / 256 < 65535 ? (total + 255) / 256 : 65535);
+  const long long planes = (long long)b * c;
+  const int grid = (int)((planes + 255) / 256 < 65535 ? (planes + 255) / 256 : 65535);
   k_gather_feat_bwd<<<grid, 256, 0, (cudaStream_t)stream>>>(grad_out, ind, grad_feat, b, c, hw, m);
   CNB_CHECK_LAUNCH("cnb_gather_feat_backward");
   count_launch();

@@ -19,12 +19,19 @@ namespace cnb {
 
 constexpr int FOCAL_THREADS = 256;
 constexpr int MAX_OBJ_PER_PLANE = 128;
+constexpr int FOCAL_MAX_CTAS = 16384;   // grid cap of the loss kernels: one (pos, neg) partial per CTA
+constexpr size_t FOCAL_PART_OFF = 256;  // partials start here in the workspace
 
 struct FocalAcc {       // lives at the start of the workspace, zeroed per call
-  double pos_sum, neg_sum, num_pos;
+  double num_pos;
   unsigned int done;
   unsigned int pad;
 };
+// The per-CTA loss sums are stored, not atomically added: the last CTA adds them in CTA order, so the loss is
+// bit-identical run to run.  num_pos is a count (exact in double) and keeps its atomics.
+__device__ __forceinline__ double2 *focal_partials(FocalAcc *acc) {
+  return reinterpret_cast<double2 *>(reinterpret_cast<char *>(acc) + FOCAL_PART_OFF);
+}
 
 struct Obj { int x, y, r; };
 
@@ -147,36 +154,53 @@ __device__ __forceinline__ Elem focal_elem(float v, float gt, float inv_norm) {
   return e;
 }
 
-__device__ __forceinline__ void block_accumulate(double pos, double neg, double npos, FocalAcc *acc) {
-  __shared__ double red[3][FOCAL_THREADS / 32];
+// the CTA's (pos, neg) sums (fixed shuffle / warp order) -> its partial
+__device__ __forceinline__ void block_accumulate(double pos, double neg, FocalAcc *acc) {
+  __shared__ double red[2][FOCAL_THREADS / 32];
   for (int o = 16; o > 0; o >>= 1) {
     pos += __shfl_xor_sync(0xffffffffu, pos, o);
     neg += __shfl_xor_sync(0xffffffffu, neg, o);
-    npos += __shfl_xor_sync(0xffffffffu, npos, o);
   }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) { red[0][warp] = pos; red[1][warp] = neg; red[2][warp] = npos; }
+  if (lane == 0) { red[0][warp] = pos; red[1][warp] = neg; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    double a = 0, b = 0, c = 0;
-    for (int i = 0; i < FOCAL_THREADS / 32; ++i) { a += red[0][i]; b += red[1][i]; c += red[2][i]; }
-    atomicAdd(&acc->pos_sum, a);
-    atomicAdd(&acc->neg_sum, b);
-    if (npos >= 0) atomicAdd(&acc->num_pos, c);
+    double a = 0, b = 0;
+    for (int i = 0; i < FOCAL_THREADS / 32; ++i) { a += red[0][i]; b += red[1][i]; }
+    focal_partials(acc)[blockIdx.x] = make_double2(a, b);
   }
 }
 
-// The last CTA to finish turns the accumulators into (loss, num_pos): losses.py:59-66.
+// The last CTA to finish adds the partials in CTA order (thread t takes CTAs t, t + 256, ..., then a fixed tree) and
+// turns them into (loss, num_pos): losses.py:59-66.
 __device__ __forceinline__ void finish_loss(FocalAcc *acc, unsigned int total_blocks, float *out2) {
   __shared__ bool last;
+  __shared__ double red[2][FOCAL_THREADS];
   __threadfence();
   if (threadIdx.x == 0) last = (atomicAdd(&acc->done, 1u) == total_blocks - 1);
   __syncthreads();
-  if (last && threadIdx.x == 0) {
-    __threadfence();
-    const double ps = *((volatile double *)&acc->pos_sum), ns = *((volatile double *)&acc->neg_sum);
+  if (!last) return;
+  __threadfence();
+  const double2 *part = focal_partials(acc);
+  double ps = 0.0, ns = 0.0;
+  for (unsigned i = threadIdx.x; i < total_blocks; i += FOCAL_THREADS) {
+    const double2 v = __ldcg(part + i);
+    ps += v.x;
+    ns += v.y;
+  }
+  red[0][threadIdx.x] = ps;
+  red[1][threadIdx.x] = ns;
+  __syncthreads();
+  for (int d = FOCAL_THREADS / 2; d > 0; d >>= 1) {
+    if ((int)threadIdx.x < d) {
+      red[0][threadIdx.x] += red[0][threadIdx.x + d];
+      red[1][threadIdx.x] += red[1][threadIdx.x + d];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
     const double np_ = *((volatile double *)&acc->num_pos);
-    out2[0] = (np_ == 0.0) ? (float)(-ns) : (float)(-(ps + ns) / np_);
+    out2[0] = (np_ == 0.0) ? (float)(-red[1][0]) : (float)(-(red[0][0] + red[1][0]) / np_);
     out2[1] = (float)np_;
   }
 }
@@ -244,7 +268,7 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense(const float *__re
     pos += e.loss_pos; neg += e.loss_neg;
     if (grad) grad[i] = e.grad;
   }
-  block_accumulate(pos, neg, -1.0, acc);
+  block_accumulate(pos, neg, acc);
   finish_loss(acc, gridDim.x, out2);
 }
 
@@ -255,25 +279,28 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
                                                                const int32_t *rad, const uint8_t *valid, int M, int C,
                                                                int H, int W, float grad_scale,
                                                                float *__restrict__ grad, float *__restrict__ hm,
-                                                               FocalAcc *acc, float *out2, int parts) {
-  // one CTA per (image, class plane, band of H / parts rows): more, shorter CTAs fill the last wave better
+                                                               FocalAcc *acc, float *out2, int parts, int B) {
+  // one CTA per (image, class plane, band of H / parts rows): more, shorter CTAs fill the last wave better.  Grids are
+  // capped at FOCAL_MAX_CTAS (one loss partial per CTA): a CTA then takes items blockIdx.x, + gridDim.x, ...
   __shared__ Obj s_obj[MAX_OBJ_PER_PLANE];
   __shared__ ObjTab s_tab[MAX_OBJ_PER_PLANE];
   __shared__ float s_gauss[GAUSS_TAB_FLOATS];
   __shared__ int s_n, s_total;
-  const int plane = blockIdx.x / parts, part = blockIdx.x - plane * parts;
-  const int b = plane / C, c = plane - b * C;
-  const int y_lo = (int)((long long)H * part / parts), y_hi = (int)((long long)H * (part + 1) / parts);
-  const int nobj = gather_objects(cls, cx, cy, rad, valid, b, M, c, H, W, s_obj, &s_n, y_lo, y_hi);
-  if (nobj) build_tables(s_obj, nobj, s_tab, s_gauss, &s_total);
-  const long long base = (long long)plane * H * W;
   float inv_norm = 0.0f;
   if (!WRITE_HM) {
     const double np_ = acc->num_pos;
     inv_norm = grad_scale / (np_ > 0.0 ? (float)np_ : 1.0f);
   }
   double pos = 0, neg = 0;
-  const int HW = H * W;
+  const int n_items = B * C * parts;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+  __syncthreads();   // the previous item's objects and tables are no longer read
+  const int plane = item / parts, part = item - plane * parts;
+  const int b = plane / C, c = plane - b * C;
+  const int y_lo = (int)((long long)H * part / parts), y_hi = (int)((long long)H * (part + 1) / parts);
+  const int nobj = gather_objects(cls, cx, cy, rad, valid, b, M, c, H, W, s_obj, &s_n, y_lo, y_hi);
+  if (nobj) build_tables(s_obj, nobj, s_tab, s_gauss, &s_total);
+  const long long base = (long long)plane * H * W;
   const bool vec = (W % 4 == 0) && ((((uintptr_t)pred | (uintptr_t)grad | (uintptr_t)hm) & 15u) == 0);
   if (vec) {
     // (x, y) of the thread's float4 advance incrementally: no division in the loop (the kernel is issue-bound)
@@ -308,8 +335,9 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
       }
     }
   }
+  }
   if (!WRITE_HM) {
-    block_accumulate(pos, neg, -1.0, acc);
+    block_accumulate(pos, neg, acc);
     finish_loss(acc, gridDim.x, out2);
   }
 }
@@ -325,33 +353,40 @@ __global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ out
   const uint8_t *mask_u8 = reinterpret_cast<const uint8_t *>(mask_);
   const float *mask_f = reinterpret_cast<const float *>(mask_);
   double loss = 0, msum = 0;
+  // pass 0: the sums (strided per thread, fixed tree); pass 1: the gradient, one thread per (image, channel) plane
+  // walking m in ascending order, so repeated indices add up in a fixed order without atomics
   for (int pass = 0; pass < 2; ++pass) {
     const double denom = pass ? (s_tot[1] + 1e-4) : 1.0;
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-      const int d = (int)(i % D);
-      const long long bm = i / D;
-      const int b = (int)(bm / M);
-      const long long sp = ind[bm];
-      if (sp < 0 || sp >= HW) continue;   // torch's gather raises on such an index; never read or write outside the map
-      const float m = (mode == 3) ? mask_f[i] : (float)mask_u8[bm];
-      float pred = output[((long long)b * D + d) * HW + sp];
-      float tgt = target[i];
-      float scale = 1.0f;
-      if (mode == 2) {  // NormRegL1Loss: pred / (target + 1e-4) against 1
-        scale = 1.0f / (tgt + 1e-4f);
-        pred = pred / (tgt + 1e-4f);
-        tgt = tgt * 0.0f + 1.0f;
-      }
-      const float diff = pred * m - tgt * m;
-      if (pass == 0) {
-        const float ad = fabsf(diff);
-        loss += (mode == 1) ? (ad < 1.0f ? 0.5 * (double)ad * ad : (double)ad - 0.5) : (double)ad;
-        msum += (mode == 1) ? ((d == 0) ? (double)m : 0.0) : (double)m;  // RegLoss divides by mask.sum() un-expanded
-      } else if (grad_output) {
-        float g = (diff > 0.0f) ? 1.0f : (diff < 0.0f ? -1.0f : 0.0f);
-        if (mode == 1 && fabsf(diff) < 1.0f) g = diff;
-        g = g * m * scale * grad_scale / (float)denom;
-        if (g != 0.0f) atomicAdd(grad_output + ((long long)b * D + d) * HW + sp, g);
+    const long long n_it = pass ? (long long)B * D : n;
+    for (long long it = threadIdx.x; it < n_it; it += blockDim.x) {
+      if (pass && !grad_output) break;
+      for (int mm = 0; mm < (pass ? M : 1); ++mm) {
+        const long long i = pass ? ((it / D) * M + mm) * D + it % D : it;
+        const int d = (int)(i % D);
+        const long long bm = i / D;
+        const int b = (int)(bm / M);
+        const long long sp = ind[bm];
+        if (sp < 0 || sp >= HW) continue;   // torch's gather raises on such an index; never read or write outside the map
+        const float m = (mode == 3) ? mask_f[i] : (float)mask_u8[bm];
+        float pred = output[((long long)b * D + d) * HW + sp];
+        float tgt = target[i];
+        float scale = 1.0f;
+        if (mode == 2) {  // NormRegL1Loss: pred / (target + 1e-4) against 1
+          scale = 1.0f / (tgt + 1e-4f);
+          pred = pred / (tgt + 1e-4f);
+          tgt = tgt * 0.0f + 1.0f;
+        }
+        const float diff = pred * m - tgt * m;
+        if (pass == 0) {
+          const float ad = fabsf(diff);
+          loss += (mode == 1) ? (ad < 1.0f ? 0.5 * (double)ad * ad : (double)ad - 0.5) : (double)ad;
+          msum += (mode == 1) ? ((d == 0) ? (double)m : 0.0) : (double)m;  // RegLoss divides by mask.sum() un-expanded
+        } else {
+          float g = (diff > 0.0f) ? 1.0f : (diff < 0.0f ? -1.0f : 0.0f);
+          if (mode == 1 && fabsf(diff) < 1.0f) g = diff;
+          g = g * m * scale * grad_scale / (float)denom;
+          if (g != 0.0f) grad_output[((long long)b * D + d) * HW + sp] += g;
+        }
       }
     }
     if (pass == 0) {
@@ -374,9 +409,11 @@ __global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ out
 
 static int focal_grid(long long n4) {
   long long g = (n4 + FOCAL_THREADS - 1) / FOCAL_THREADS;
-  const long long cap = (long long)num_sms() * 8;
+  long long cap = (long long)num_sms() * 8;
+  if (cap > FOCAL_MAX_CTAS) cap = FOCAL_MAX_CTAS;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
+static int splat_grid(long long items) { return (int)(items < FOCAL_MAX_CTAS ? items : FOCAL_MAX_CTAS); }
 
 }  // namespace cnb
 
@@ -392,13 +429,13 @@ static int focal_parts(int h) {
 
 extern "C" {
 
-size_t cnb_focal_workspace_bytes(long long) { return 256; }
+size_t cnb_focal_workspace_bytes(long long) { return FOCAL_PART_OFF + (size_t)FOCAL_MAX_CTAS * sizeof(double2); }
 
 int cnb_focal_loss(const float *pred, const float *gt, long long n, int logits, float grad_scale, float *out2,
                    float *grad, void *workspace, size_t workspace_bytes, void *stream_) {
   CNB_REQUIRE(pred && gt && out2 && workspace, CNB_EINVAL, "cnb_focal_loss: null pointer");
   CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_loss: n=%lld", n);
-  CNB_REQUIRE(workspace_bytes >= sizeof(FocalAcc), CNB_EWORKSPACE, "cnb_focal_loss: workspace too small");
+  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes(n), CNB_EWORKSPACE, "cnb_focal_loss: workspace too small");
   cudaStream_t stream = (cudaStream_t)stream_;
   FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
   CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
@@ -423,8 +460,8 @@ int cnb_splat_gaussian(const int32_t *obj_cls, const int32_t *obj_cx, const int3
   CNB_REQUIRE(m <= MAX_OBJ_PER_PLANE, CNB_EUNSUPPORTED, "cnb_splat_gaussian: at most %d objects per image (got %d)",
               MAX_OBJ_PER_PLANE, m);
   const int parts = focal_parts(h);
-  k_focal_splat<false, true><<<b * c * parts, FOCAL_THREADS, 0, (cudaStream_t)stream_>>>(
-      nullptr, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, m, c, h, w, 0.0f, nullptr, hm, nullptr, nullptr, parts);
+  k_focal_splat<false, true><<<splat_grid((long long)b * c * parts), FOCAL_THREADS, 0, (cudaStream_t)stream_>>>(
+      nullptr, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, m, c, h, w, 0.0f, nullptr, hm, nullptr, nullptr, parts, b);
   CNB_CHECK_LAUNCH("cnb_splat_gaussian");
   count_launch();
   return CNB_OK;
@@ -439,7 +476,8 @@ int cnb_focal_splat_loss(const float *pred, const int32_t *obj_cls, const int32_
   CNB_REQUIRE(b > 0 && m > 0 && c > 0 && h > 0 && w > 0, CNB_EINVAL, "cnb_focal_splat_loss: non-positive dimension");
   CNB_REQUIRE(m <= MAX_OBJ_PER_PLANE, CNB_EUNSUPPORTED, "cnb_focal_splat_loss: at most %d objects per image (got %d)",
               MAX_OBJ_PER_PLANE, m);
-  CNB_REQUIRE(workspace_bytes >= sizeof(FocalAcc), CNB_EWORKSPACE, "cnb_focal_splat_loss: workspace too small");
+  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes((long long)b * c * h * w), CNB_EWORKSPACE,
+              "cnb_focal_splat_loss: workspace too small");
   cudaStream_t stream = (cudaStream_t)stream_;
   FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
   CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
@@ -449,13 +487,13 @@ int cnb_focal_splat_loss(const float *pred, const int32_t *obj_cls, const int32_
   CNB_CHECK_LAUNCH("cnb_focal_splat_loss count");
   const int parts = focal_parts(h);
   if (logits)
-    k_focal_splat<true, false><<<b * c * parts, FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
+    k_focal_splat<true, false><<<splat_grid((long long)b * c * parts), FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
                                                                              obj_valid, m, c, h, w, grad_scale, grad,
-                                                                             nullptr, acc, out2, parts);
+                                                                             nullptr, acc, out2, parts, b);
   else
-    k_focal_splat<false, false><<<b * c * parts, FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
+    k_focal_splat<false, false><<<splat_grid((long long)b * c * parts), FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
                                                                               obj_valid, m, c, h, w, grad_scale, grad,
-                                                                              nullptr, acc, out2, parts);
+                                                                              nullptr, acc, out2, parts, b);
   CNB_CHECK_LAUNCH("cnb_focal_splat_loss");
   count_launch(2);
   return CNB_OK;

@@ -7,6 +7,7 @@ cnb_dcnv2_backward (im2col-free, no `ones`/`columns` scratch).  Non-CUDA tensors
 NotImplementedError exactly like the reference (:23-24, :41-42).
 """
 import os
+import warnings
 import weakref
 
 import torch
@@ -16,9 +17,23 @@ from ._lib import C, f32c, ptr, stream_ptr, workspace
 
 # CNB_DCN_FP32=1 selects the fp32 CUDA-core contraction instead of the wgmma (3xTF32) one
 _FORCE_FP32 = os.environ.get("CNB_DCN_FP32", "0") == "1"
-# CNB_DCN_DETERMINISTIC=1: bit-identical grad_input (cnb_dcnv2_set_deterministic); also on under
+# CNB_DCN_DETERMINISTIC=1: bit-identical gradients run to run (cnb_dcnv2_set_deterministic); also on under
 # torch.use_deterministic_algorithms(True)
 _DETERMINISTIC = os.environ.get("CNB_DCN_DETERMINISTIC", "0") == "1"
+
+
+def _deterministic():
+    return bool(_DETERMINISTIC or torch.are_deterministic_algorithms_enabled())
+
+
+def _alert_not_deterministic(what):
+    """torch's rule for an op without a deterministic implementation: raise, or warn and run under warn_only."""
+    msg = ("%s does not have a deterministic implementation, but deterministic algorithms were requested "
+           "(torch.use_deterministic_algorithms(True) or CNB_DCN_DETERMINISTIC=1)" % what)
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
 
 
 def _out_hw(h, w, kh, kw, stride, padding, dilation):
@@ -107,12 +122,18 @@ class _DCNv2(Function):
         go = f32c(grad_output)
         n, cin, h, wd = [int(v) for v in x.shape]
         cout, _, kh, kw = [int(v) for v in w.shape]
-        # grad_input by the fixed-order gather when the user asked torch for deterministic algorithms (or CNB_DCN_DETERMINISTIC=1)
-        det = bool(_DETERMINISTIC or torch.are_deterministic_algorithms_enabled())
+        # order-independent (fixed-point) grad_input when the user asked torch for deterministic algorithms (or
+        # CNB_DCN_DETERMINISTIC=1); the workspace query below then includes what that mode needs
+        det = _deterministic()
+        if det and (_FORCE_FP32 or C.dcnv2_backward_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding,
+                                                                     dilation, dg) == 0):
+            _alert_not_deterministic("DCNv2 backward on the fp32 path (CNB_DCN_FP32=1, more than 9 taps or an image "
+                                     "beyond the tensor-core kernels' 32-bit indexing)")
+            det = False                 # warn_only: run the fp32 kernels
         C.dcnv2_set_deterministic(int(det))
-        x_cl = ctx.x_cl and not det and not _FORCE_FP32
+        x_cl = ctx.x_cl and not _FORCE_FP32
         if ctx.x_cl and not x_cl:
-            x = x.contiguous()          # the gather (and the fp32 kernels) work on NCHW
+            x = x.contiguous()          # the fp32 kernels work on NCHW
         # zero-filled, accumulated into -- dcn_v2_func.py:44-48 (zeros_like keeps a channels_last input's layout)
         gx = torch.zeros_like(x)
         goff = torch.zeros_like(off)
@@ -216,6 +237,8 @@ class _PSROIPooling(Function):
     def backward(ctx, grad_output):
         if not grad_output.is_cuda:
             raise NotImplementedError("DCNv2PoolingFunction: CUDA tensors only (dcn_v2_func.py:117-118)")
+        if _deterministic():
+            _alert_not_deterministic("DCNv2PoolingFunction backward (atomic scatter)")
         data, rois, offset, cnt = ctx.saved_tensors
         spatial_scale, pooled_size, output_dim, no_trans, group_size, part_size, sample_per_part, trans_std, ct = ctx.cfg
         grad_output = f32c(grad_output)

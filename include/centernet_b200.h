@@ -170,7 +170,9 @@ int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_hea
  *   obj_cls[b,m] i32, obj_cx/obj_cy[b,m] i32 (ct_int), obj_radius[b,m] i32,
  *   obj_valid[b,m] u8 -- exactly the draw_umich_gaussian calls of
  *   datasets/sample/ctdet.py:111-117.  m <= 128 (the reference's max_objs,
- *   datasets/dataset/coco.py:38); larger lists return CNB_EUNSUPPORTED. */
+ *   datasets/dataset/coco.py:38); larger lists return CNB_EUNSUPPORTED.
+ * Both losses are bit-identical run to run: the workspace (cnb_focal_workspace_bytes) holds one partial sum
+ * per CTA, added in CTA order by the last CTA. */
 size_t cnb_focal_workspace_bytes(long long n);
 int cnb_focal_loss(const float *pred, const float *gt, long long n, int logits,
                    float grad_scale, float *out2, float *grad,
@@ -189,7 +191,7 @@ int cnb_focal_splat_loss(const float *pred, const int32_t *obj_cls, const int32_
  * NormRegL1Loss :151-163 (mode 2), RegWeightedL1Loss :165-175 (mode 3; mask is
  * then float [b,m,d]).  output [b,d,h*w], ind [b,m] i64, target [b,m,d].
  * out[0] = loss; grad_output (nullable, [b,d,hw], must be zero-filled) gets
- * d loss/d output * grad_scale. */
+ * d loss/d output * grad_scale; repeated ind entries add up in ascending m (bit-identical run to run). */
 int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, const float *target,
                  int b, int d, int hw, int m, int mode, float grad_scale,
                  float *out1, float *grad_output, void *stream);
@@ -255,7 +257,7 @@ size_t cnb_dcnv2_backward_workspace_bytes(int b, int cin, int cout, int h, int w
 /* The backward for a channels-last pipeline (torch channels_last): input_channels_last / grad_input_channels_last
  * != 0 say the tensor is [b][h*w][cin]; the re-layout pass of the input, the zero-fill and the final NCHW pass of
  * grad_input disappear (grad_input still arrives zero-filled).  Tensor-core path only: needs the workspace,
- * cin / deformable_groups % 32 == 0, cout <= 256, non-deterministic dX; CNB_EUNSUPPORTED otherwise. */
+ * cin / deformable_groups % 32 == 0, cout <= 256; CNB_EUNSUPPORTED otherwise.  Deterministic mode included. */
 int cnb_dcnv2_backward_ex(const float *input, int input_channels_last, const float *offset,
                           const float *mask, const float *weight, const float *grad_output,
                           float *grad_input, int grad_input_channels_last,
@@ -265,10 +267,17 @@ int cnb_dcnv2_backward_ex(const float *input, int input_channels_last, const flo
                           void *workspace, size_t workspace_bytes, void *stream);
 /* grad_offset, grad_mask, grad_weight and grad_bias of the tensor-core backward are bit-identical run to run.
  * grad_input is by default scattered with (vector) atomics like the reference's col2im
- * (dcn_v2_im2col_cuda.cu:182-239), i.e. its last bits depend on the order the adds land.  on != 0 selects a
- * gather instead (stride 1): every input position collects the samples that fall on it in a fixed order, which
- * makes grad_input bit-identical as well as long as no offset moves a sample more than 2 pixels from its tap
- * (those few still go through atomics); it costs about one extra forward.  Process-wide, default off. */
+ * (dcn_v2_im2col_cuda.cu:182-239), i.e. its last bits depend on the order the adds land.  on != 0 (process-wide,
+ * default off) makes all five gradients bit-identical for every configuration the tensor-core backward covers
+ * (any offsets, stride, dilation, taps <= 9, deformable groups, Cout, channels-last tensors) and independent of
+ * the batch size an image is run with: grad_input is summed in 64-bit fixed point (a per-image power-of-two scale
+ * from a bound on |grad_input|, integer adds in any order) and converted to fp32 at the end; an image whose
+ * grad_output, weight or mask holds an inf or NaN gets an all-NaN grad_input.  While the flag is set:
+ *   cnb_dcnv2_backward_workspace_bytes returns the larger size this mode needs (its default-mode value does not
+ *   change), so query it after setting the flag;
+ *   cnb_dcnv2_backward / _ex return CNB_EUNSUPPORTED for what only the fp32 kernels run (no or too small a
+ *   workspace, anisotropic stride/pad/dilation, images beyond the 32-bit in-image indexing);
+ *   cnb_dcnv2_backward_ex accepts a channels-last grad_input. */
 void cnb_dcnv2_set_deterministic(int on);
 int cnb_dcnv2_get_deterministic(void);
 int cnb_dcnv2_backward(const float *input, const float *offset, const float *mask,

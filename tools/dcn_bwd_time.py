@@ -14,6 +14,17 @@ LAYERS = [(16, 64, 128, 128, 64), (16, 128, 64, 64, 128), (16, 256, 32, 32, 256)
 
 
 def run(x, off, m, w, go, tc, want_dx=True):
+    """tc=False: the fp32 CUDA-core path, which has no deterministic mode: the switch is off for that call."""
+    det = C.dcnv2_get_deterministic()
+    if not tc:
+        C.dcnv2_set_deterministic(0)
+    try:
+        return _run(x, off, m, w, go, tc, want_dx)
+    finally:
+        C.dcnv2_set_deterministic(det)
+
+
+def _run(x, off, m, w, go, tc, want_dx):
     B, Ci, H, W = x.shape
     Co = w.shape[0]
     gx = torch.zeros_like(x); goff = torch.zeros_like(off); gm = torch.zeros_like(m)
@@ -57,7 +68,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--layers", type=int, nargs="*", default=None, help="indices into LAYERS (default: all)")
     ap.add_argument("--quick", action="store_true", help="tensor-core path only, one call per layer (for ncu)")
-    ap.add_argument("--deterministic", action="store_true", help="cnb_dcnv2_set_deterministic(1): dX by the gather")
+    ap.add_argument("--deterministic", action="store_true", help="cnb_dcnv2_set_deterministic(1): fixed-point (order-independent) dX")
     ap.add_argument("--off-scale", type=float, default=1.5)
     ap.add_argument("--off-clamp", type=float, default=0.0, help="clamp the offsets to +-this (0 = no clamp)")
     args = ap.parse_args()
@@ -87,7 +98,7 @@ def main():
         t_tc = timeit(lambda: run(x, off, m, w, go, True))
         t_nodx = timeit(lambda: run(x, off, m, w, go, True, False))
         t_cl = float("nan")
-        if not args.deterministic and Ci % 32 == 0:
+        if Ci % 32 == 0:
             xcl = x.contiguous(memory_format=torch.channels_last)
             c = run_cl(xcl, off, m, w, go)
             errs.append("cl-dx %.2e" % (c[0] - r[0]).abs().max().item())
