@@ -242,6 +242,64 @@ def run(dev, batches, K=100, steps=20):
             return r
         guarded("dcnv2_b%d_%dx%d_%dto%d" % (b, hh, hh, ci, co), dcn)
 
+    # ---- float64 DCNv2 (the reference's dcn_v2_double build) on the FP64 tensor cores, next to the reference's own
+    # float64 kernels (oracle/_ref f64) and torchvision in float64
+    try:
+        from oracle import ref_gpu_f64
+        have_ref64 = ref_gpu_f64.available()
+    except Exception:
+        have_ref64 = False
+    for (b, ci, hh, co) in ((16, 64, 128, 64), (16, 256, 32, 256)):
+        def dcn64(b=b, ci=ci, hh=hh, co=co):
+            f64 = torch.float64
+            x = torch.randn(b, ci, hh, hh, device=dev, generator=g, dtype=f64)
+            off = torch.randn(b, 18, hh, hh, device=dev, generator=g, dtype=f64) * 2
+            msk = torch.sigmoid(torch.randn(b, 9, hh, hh, device=dev, generator=g, dtype=f64))
+            w = torch.randn(co, ci, 3, 3, device=dev, generator=g, dtype=f64) / (3 * ci ** 0.5)
+            bias = torch.randn(co, device=dev, generator=g, dtype=f64)
+            fn = DCNv2Function(1, 1, 1, 1)
+            flops = 2.0 * co * ci * 9 * hh * hh * b
+            peak = 67.0     # H100 SXM data sheet, FP64 tensor core
+            ms = timeit(lambda: fn(x, off, msk, w, bias), 5, 2)
+            leaves = [t.clone().requires_grad_(True) for t in (x, off, msk, w, bias)]
+
+            def fb():
+                for t in leaves:
+                    t.grad = None
+                fn(*leaves).sum().backward()
+            fb_ms = timeit(fb, 3, 1)
+            r = {"ms": round(ms, 5), "fwd_bwd_ms": round(fb_ms, 5),
+                 "roofline": {"bound": "tensor", "achieved": round(flops / (ms * 1e-3) / 1e12, 2), "peak": peak,
+                              "unit": "TFLOP/s", "frac": round(flops / (ms * 1e-3) / 1e12 / peak, 4), "flops": int(flops),
+                              "peak_source": "H100 SXM data sheet FP64 tensor core"},
+                 "fwd_bwd_frac_of_fp64_peak": round(3.0 * flops / (fb_ms * 1e-3) / 1e12 / peak, 4),
+                 "config": "DCNv2 float64 B=%d %d@%dx%d->%d (DMMA, bit-reproducible backward)" % (b, ci, hh, hh, co)}
+            if have_ref64:
+                r["reference_gpu_f64_fwd_ms"] = round(timeit(lambda: ref_gpu_f64.dcn_v2_forward(x, off, msk, w, bias),
+                                                             3, 1), 5)
+                go = torch.ones(b, co, hh, hh, device=dev, dtype=f64)
+
+                def rfb():
+                    ref_gpu_f64.dcn_v2_forward(x, off, msk, w, bias)
+                    ref_gpu_f64.dcn_v2_backward(x, off, msk, w, bias, go)
+                r["reference_gpu_f64_fwd_bwd_ms"] = round(timeit(rfb, 2, 1), 5)
+                r["reference_gpu_f64"] = ("oracle/_ref f64: the reference's dcn_v2_im2col_cuda_double.cu compiled "
+                                          "unmodified + cuBLAS DGEMM, one sample at a time")
+            try:
+                from torchvision.ops import deform_conv2d
+                r["torchvision_f64_fwd_ms"] = round(timeit(lambda: deform_conv2d(x, off, w, bias, padding=1, mask=msk),
+                                                           3, 1), 5)
+
+                def tvfb():
+                    for t in leaves:
+                        t.grad = None
+                    deform_conv2d(leaves[0], leaves[1], leaves[3], leaves[4], padding=1, mask=leaves[2]).sum().backward()
+                r["torchvision_f64_fwd_bwd_ms"] = round(timeit(tvfb, 2, 1), 5)
+            except Exception:
+                pass
+            return r
+        guarded("dcnv2_f64_b%d_%dx%d_%dto%d" % (b, hh, hh, ci, co), dcn64)
+
     # ---- the reference's ATen-op decode on CUDA tensors (BASELINE.md section 2 "reference on GPU" bar)
     def ref_decode_gpu():
         from oracle import torch_port

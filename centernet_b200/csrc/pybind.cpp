@@ -101,6 +101,42 @@ PYBIND11_MODULE(_C, m) {
                                      tstd, ptr<void>(stream)),
           "cnb_psroi_pooling_backward");
   });
+  m.def("psroi_pooling_f64_workspace_bytes", &cnb_psroi_pooling_f64_workspace_bytes);
+  m.def("psroi_pooling_forward_f64", [](P data, P rois, P trans, P out, P cnt, int b, int c, int h, int w, int n,
+                                        int ct, int no_trans, double scale, int od, int gs, int ps, int part, int spp,
+                                        double tstd, P stream) {
+    check(cnb_psroi_pooling_forward_f64(ptr<const double>(data), ptr<const double>(rois), ptr<const double>(trans),
+                                        ptr<double>(out), ptr<double>(cnt), b, c, h, w, n, ct, no_trans, scale, od, gs,
+                                        ps, part, spp, tstd, ptr<void>(stream)),
+          "cnb_psroi_pooling_forward_f64");
+  });
+  m.def("psroi_pooling_backward_f64", [](P gout, P data, P rois, P trans, P cnt, P gdata, P gtrans, int b, int c,
+                                         int h, int w, int n, int ct, int no_trans, double scale, int od, int gs,
+                                         int ps, int part, int spp, double tstd, P ws, size_t wsb, P stream) {
+    check(cnb_psroi_pooling_backward_f64(ptr<const double>(gout), ptr<const double>(data), ptr<const double>(rois),
+                                         ptr<const double>(trans), ptr<const double>(cnt), ptr<double>(gdata),
+                                         ptr<double>(gtrans), b, c, h, w, n, ct, no_trans, scale, od, gs, ps, part,
+                                         spp, tstd, ptr<void>(ws), wsb, ptr<void>(stream)),
+          "cnb_psroi_pooling_backward_f64");
+  });
+  m.def("dcnv2_f64_workspace_bytes", &cnb_dcnv2_f64_workspace_bytes);
+  m.def("dcnv2_forward_f64", [](P input, P offset, P mask, P weight, P bias, P output, int b, int cin, int h, int w,
+                                int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int dg,
+                                P stream) {
+    check(cnb_dcnv2_forward_f64(ptr<const double>(input), ptr<const double>(offset), ptr<const double>(mask),
+                                ptr<const double>(weight), ptr<const double>(bias), ptr<double>(output), b, cin, h, w,
+                                cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, ptr<void>(stream)),
+          "cnb_dcnv2_forward_f64");
+  });
+  m.def("dcnv2_backward_f64", [](P input, P offset, P mask, P weight, P gout, P gin, P goff, P gmask, P gw, P gb,
+                                 int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph,
+                                 int pw, int dh, int dw, int dg, P ws, size_t wsb, P stream) {
+    check(cnb_dcnv2_backward_f64(ptr<const double>(input), ptr<const double>(offset), ptr<const double>(mask),
+                                 ptr<const double>(weight), ptr<const double>(gout), ptr<double>(gin),
+                                 ptr<double>(goff), ptr<double>(gmask), ptr<double>(gw), ptr<double>(gb), b, cin, h, w,
+                                 cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, ptr<void>(ws), wsb, ptr<void>(stream)),
+          "cnb_dcnv2_backward_f64");
+  });
   m.def("ddd_decode", [](P heat, P rot, P depth, P dim, P wh, P reg, int b, int c, int h, int w, int k, P dets, P ws,
                          size_t wsb, P stream) {
     check(cnb_ddd_decode(ptr<const float>(heat), ptr<const float>(rot), ptr<const float>(depth),

@@ -56,7 +56,9 @@ class DCN(DCNv2):
 
     def forward(self, input):
         out = self.conv_offset_mask(input)
-        if input.is_cuda and not torch.is_grad_enabled() and self.kernel_size[0] * self.kernel_size[1] <= 9:
+        # inference in fp32 uses the fused kernel; float64 (no fused form) takes the path below
+        if input.is_cuda and not torch.is_grad_enabled() and self.kernel_size[0] * self.kernel_size[1] <= 9 and \
+                input.dtype != torch.float64:
             # inference: chunk / cat / sigmoid (the three lines below) run inside the DCN kernel's sampler
             return dcn_fused_inference(input, out, self.weight, self.bias, self.stride, self.padding, self.dilation,
                                        self.deformable_groups)
@@ -145,7 +147,8 @@ def fuse_dcn_bn_relu(model):
 
         def fused(x, _m=m, _orig=orig):
             c, bn = _m.conv, _m.actf[0]
-            if _m.training or torch.is_grad_enabled() or not x.is_cuda or not bn.track_running_stats:
+            if _m.training or torch.is_grad_enabled() or not x.is_cuda or not bn.track_running_stats or \
+                    x.dtype == torch.float64:
                 return _orig(x)
             scale, shift = fold_bn(bn)
             om = c.conv_offset_mask(x)

@@ -36,6 +36,20 @@ def _alert_not_deterministic(what):
         raise RuntimeError(msg)
 
 
+def _f64c(what, *tensors):
+    """float64 + contiguous views; the reference's typed backend takes no mixed types, so a float tensor of another
+    dtype next to a float64 input is an error rather than a silent cast."""
+    out = []
+    for t in tensors:
+        if t is None:
+            out.append(None)
+            continue
+        if t.dtype != torch.float64:
+            raise RuntimeError("%s: the input is float64, so every tensor must be float64 too (got %s)" % (what, t.dtype))
+        out.append(t.contiguous())
+    return out
+
+
 def _out_hw(h, w, kh, kw, stride, padding, dilation):
     ho = (h + 2 * padding - (dilation * (kh - 1) + 1)) // stride + 1   # dcn_v2_func.py:64-73
     wo = (w + 2 * padding - (dilation * (kw - 1) + 1)) // stride + 1
@@ -69,21 +83,60 @@ def _weight_tiles(weight, dg):
     return wt
 
 
+def _dcn_shapes(x, off, msk, w, stride, padding, dilation, deformable_groups):
+    n, cin, h, wd = [int(v) for v in x.shape]
+    cout, cin_w, kh, kw = [int(v) for v in w.shape]
+    if cin_w != cin:   # dcn_v2_cuda.c:36-38
+        raise RuntimeError("Input shape and kernel channels wont match: (%d vs %d)." % (cin, cin_w))
+    ho, wo = _out_hw(h, wd, kh, kw, stride, padding, dilation)
+    kt = kh * kw
+    if tuple(off.shape) != (n, 2 * kt * deformable_groups, ho, wo) or \
+            tuple(msk.shape) != (n, kt * deformable_groups, ho, wo):
+        raise RuntimeError("DCNv2: offset/mask shape does not match the output grid")
+    return n, cin, h, wd, cout, kh, kw, ho, wo
+
+
+def _dcn_forward_f64(ctx, input, offset, mask, weight, bias, stride, padding, dilation, dg):
+    """float64 (the reference's dcn_v2_double build): DMMA kernels, bit-reproducible backward in every mode."""
+    x, off, msk, w, b = _f64c("DCNv2", input, offset, mask, weight, bias)
+    n, cin, h, wd, cout, kh, kw, ho, wo = _dcn_shapes(x, off, msk, w, stride, padding, dilation, dg)
+    out = torch.empty((n, cout, ho, wo), dtype=torch.float64, device=x.device)
+    C.dcnv2_forward_f64(ptr(x), ptr(off), ptr(msk), ptr(w), ptr(b), ptr(out), n, cin, h, wd, cout, kh, kw, stride,
+                        stride, padding, padding, dilation, dilation, dg, stream_ptr(x))
+    ctx.save_for_backward(x, off, msk, w, b)
+    ctx.f64 = True
+    ctx.cfg = (stride, padding, dilation, dg)
+    return out
+
+
+def _dcn_backward_f64(ctx, grad_output):
+    x, off, msk, w, b = ctx.saved_tensors
+    stride, padding, dilation, dg = ctx.cfg
+    go = grad_output.double().contiguous()
+    n, cin, h, wd = [int(v) for v in x.shape]
+    cout, _, kh, kw = [int(v) for v in w.shape]
+    gx, goff, gmsk, gw = (torch.zeros_like(t) for t in (x, off, msk, w))   # accumulated into (dcn_v2_func.py:44-48)
+    gb = torch.zeros_like(b) if b is not None else None
+    ws = workspace(C.dcnv2_f64_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding, dilation, dg), x.device)
+    C.dcnv2_backward_f64(ptr(x), ptr(off), ptr(msk), ptr(w), ptr(go), ptr(gx), ptr(goff), ptr(gmsk), ptr(gw), ptr(gb),
+                         n, cin, h, wd, cout, kh, kw, stride, stride, padding, padding, dilation, dilation, dg, ptr(ws),
+                         ws.numel(), stream_ptr(x))
+    return gx, goff, gmsk, gw, gb, None, None, None, None
+
+
 class _DCNv2(Function):
     @staticmethod
     def forward(ctx, input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups):
         if not input.is_cuda:
             raise NotImplementedError
+        ctx.f64 = False
+        if input.dtype == torch.float64:   # dtype follows the input, as the reference's typed backend
+            return _dcn_forward_f64(ctx, input, offset, mask, weight, bias, stride, padding, dilation,
+                                    deformable_groups)
         off, msk, w, b = f32c(offset), f32c(mask), f32c(weight), f32c(bias)
-        n, cin, h, wd = [int(v) for v in input.shape]
-        cout, cin_w, kh, kw = [int(v) for v in w.shape]
-        if cin_w != cin:   # dcn_v2_cuda.c:36-38
-            raise RuntimeError("Input shape and kernel channels wont match: (%d vs %d)." % (cin, cin_w))
-        ho, wo = _out_hw(h, wd, kh, kw, stride, padding, dilation)
+        n, cin, h, wd, cout, kh, kw, ho, wo = _dcn_shapes(input, off, msk, w, stride, padding, dilation,
+                                                          deformable_groups)
         kt = kh * kw
-        if tuple(off.shape) != (n, 2 * kt * deformable_groups, ho, wo) or \
-                tuple(msk.shape) != (n, kt * deformable_groups, ho, wo):
-            raise RuntimeError("DCNv2: offset/mask shape does not match the output grid")
         out = torch.empty((n, cout, ho, wo), dtype=torch.float32, device=input.device)
         # a channels_last activation (what cuDNN produces under torch.channels_last) is sampled in place
         nhwc = (not _FORCE_FP32) and kt <= 9 and (cin // deformable_groups) % 32 == 0 and \
@@ -117,6 +170,8 @@ class _DCNv2(Function):
     def backward(ctx, grad_output):
         if not grad_output.is_cuda:
             raise NotImplementedError
+        if ctx.f64:
+            return _dcn_backward_f64(ctx, grad_output)
         x, off, msk, w, b = ctx.saved_tensors
         stride, padding, dilation, dg = ctx.cfg
         go = f32c(grad_output)
@@ -164,6 +219,8 @@ def dcn_fused_inference(input, offset_mask, weight, bias, stride, padding, dilat
     No autograd (use DCNv2Function for training)."""
     if not input.is_cuda:
         raise NotImplementedError
+    if input.dtype == torch.float64:
+        raise NotImplementedError("dcn_fused_inference: float32 only; float64 runs through DCNv2Function")
     n, cin, h, wd = [int(v) for v in input.shape]
     cout, cin_w, kh, kw = [int(v) for v in weight.shape]
     if cin_w != cin:
@@ -205,6 +262,54 @@ class DCNv2Function(object):
     forward = __call__
 
 
+def _psroi_check(rois, offset, no_trans, part_size):
+    if rois.dim() != 2 or rois.shape[1] != 5:
+        raise RuntimeError("DCNv2PoolingFunction: rois must be [n, 5], got %s" % (tuple(rois.shape),))
+    if not no_trans and (offset.dim() != 4 or offset.shape[0] < rois.shape[0] or
+                         tuple(offset.shape[2:]) != (part_size, part_size)):
+        raise RuntimeError("DCNv2PoolingFunction: offset must be [>=n, 2*classes, %d, %d], got %s"
+                           % (part_size, part_size, tuple(offset.shape)))
+
+
+def _psroi_forward_f64(ctx, data, rois, offset, spatial_scale, pooled_size, output_dim, no_trans, group_size,
+                       part_size, sample_per_part, trans_std):
+    """float64 (dcn_v2_psroi_pooling_cuda_double.cu); rois may be float32 or float64 (both hold box corners
+    exactly in float64)."""
+    no_trans = bool(no_trans)
+    if rois.dtype not in (torch.float32, torch.float64):
+        raise RuntimeError("DCNv2PoolingFunction: rois must be float32 or float64, got %s" % (rois.dtype,))
+    data, = _f64c("DCNv2PoolingFunction", data)
+    rois = rois.double().contiguous()
+    if not no_trans:
+        offset, = _f64c("DCNv2PoolingFunction", offset)
+    _psroi_check(rois, offset, no_trans, part_size)
+    n, (b, c, h, w) = int(rois.shape[0]), data.shape
+    out = torch.empty((n, output_dim, pooled_size, pooled_size), dtype=torch.float64, device=data.device)
+    cnt = torch.empty_like(out)
+    ct = 2 if no_trans else int(offset.shape[1])
+    C.psroi_pooling_forward_f64(ptr(data), ptr(rois), 0 if no_trans else ptr(offset), ptr(out), ptr(cnt), b, c, h, w,
+                                n, ct, int(no_trans), float(spatial_scale), output_dim, group_size, pooled_size,
+                                part_size, sample_per_part, float(trans_std), stream_ptr(data))
+    ctx.save_for_backward(data, rois, offset if not no_trans else data.new_empty(0), cnt)
+    ctx.cfg = (spatial_scale, pooled_size, output_dim, no_trans, group_size, part_size, sample_per_part, trans_std, ct)
+    return out
+
+
+def _psroi_backward_f64(ctx, grad_output):
+    data, rois, offset, cnt = ctx.saved_tensors
+    spatial_scale, pooled_size, output_dim, no_trans, group_size, part_size, sample_per_part, trans_std, ct = ctx.cfg
+    go = grad_output.double().contiguous()
+    grad_input = torch.zeros_like(data)
+    grad_offset = None if no_trans else torch.zeros_like(offset)
+    n, (b, c, h, w) = int(rois.shape[0]), data.shape
+    ws = workspace(C.psroi_pooling_f64_workspace_bytes(b, c, h, w), data.device)
+    C.psroi_pooling_backward_f64(ptr(go), ptr(data), ptr(rois), 0 if no_trans else ptr(offset), ptr(cnt),
+                                 ptr(grad_input), 0 if no_trans else ptr(grad_offset), b, c, h, w, n, ct,
+                                 int(no_trans), float(spatial_scale), output_dim, group_size, pooled_size, part_size,
+                                 sample_per_part, float(trans_std), ptr(ws), ws.numel(), stream_ptr(data))
+    return (grad_input, None, grad_offset) + (None,) * 8
+
+
 class _PSROIPooling(Function):
     """dcn_v2_func.py:76-146 as a modern autograd.Function."""
 
@@ -213,15 +318,15 @@ class _PSROIPooling(Function):
                 sample_per_part, trans_std):
         if not data.is_cuda:
             raise NotImplementedError("DCNv2PoolingFunction: CUDA tensors only (dcn_v2_func.py:100-101)")
+        ctx.f64 = data.dtype == torch.float64
+        if ctx.f64:
+            return _psroi_forward_f64(ctx, data, rois, offset, spatial_scale, pooled_size, output_dim, no_trans,
+                                      group_size, part_size, sample_per_part, trans_std)
         data, rois = f32c(data), f32c(rois)
-        if rois.dim() != 2 or rois.shape[1] != 5:
-            raise RuntimeError("DCNv2PoolingFunction: rois must be [n, 5], got %s" % (tuple(rois.shape),))
         no_trans = bool(no_trans)
         if not no_trans:
             offset = f32c(offset)
-            if offset.dim() != 4 or offset.shape[0] < rois.shape[0] or tuple(offset.shape[2:]) != (part_size, part_size):
-                raise RuntimeError("DCNv2PoolingFunction: offset must be [>=n, 2*classes, %d, %d], got %s"
-                                   % (part_size, part_size, tuple(offset.shape)))
+        _psroi_check(rois, offset, no_trans, part_size)
         n, (b, c, h, w) = int(rois.shape[0]), data.shape
         out = torch.empty((n, output_dim, pooled_size, pooled_size), dtype=torch.float32, device=data.device)
         cnt = torch.empty_like(out)
@@ -237,6 +342,8 @@ class _PSROIPooling(Function):
     def backward(ctx, grad_output):
         if not grad_output.is_cuda:
             raise NotImplementedError("DCNv2PoolingFunction: CUDA tensors only (dcn_v2_func.py:117-118)")
+        if ctx.f64:     # bit-reproducible in every mode: no alert
+            return _psroi_backward_f64(ctx, grad_output)
         if _deterministic():
             _alert_not_deterministic("DCNv2PoolingFunction backward (atomic scatter)")
         data, rois, offset, cnt = ctx.saved_tensors

@@ -13,7 +13,7 @@
  *       (dcn_v2_cuda_forward / dcn_v2_cuda_backward / dcn_v2_psroi_pooling_*).
  *
  * Conventions
- *   - every tensor is fp32, NCHW, contiguous, resident on the current device;
+ *   - every tensor is fp32 (double in the *_f64 entry points), NCHW, contiguous, resident on the current device;
  *     index outputs use the reference's dtypes (int64 indices, int32 classes);
  *   - the caller owns every buffer, including the scratch `workspace`
  *     (size from the matching cnb_*_workspace_bytes); the library never calls
@@ -289,6 +289,41 @@ int cnb_dcnv2_backward(const float *input, const float *offset, const float *mas
                        int dil_h, int dil_w, int deformable_groups,
                        void *workspace, size_t workspace_bytes, void *stream);
 
+/* ------------------------------------------------- A10/A11: DCNv2, float64
+ * The reference's second build, _ext.dcn_v2_double (dcn_v2_cuda_double.c, dcn_v2_im2col_cuda_double.cu): the
+ * same layouts and arguments as the fp32 calls above with double tensors, any kernel size, stride, padding,
+ * dilation and deformable_groups dividing cin.  The contractions run on the FP64 tensor cores (DMMA) and no
+ * column buffer is written in the forward.  bias may be NULL.  The backward ACCUMULATES into zero-filled
+ * gradients (grad_bias may be NULL) and needs a workspace of cnb_dcnv2_f64_workspace_bytes (16-byte aligned;
+ * the forward needs none): two 64-bit limbs per grad_input element, one weight-gradient partial per pixel range
+ * (at most 64) and the column gradient dcol = W^T . dY of as many images as fit in 1.5 GiB (at least one), e.g.
+ * about 1.5 GB in all for B = 16 at 64@128x128 -> 64.
+ * Fixed-point contract: all five float64 gradients are bit-identical run to run, whatever the deterministic flag
+ * below says, and grad_input, grad_offset and grad_mask of an image do not depend on the batch it runs in.
+ * grad_input is summed in two 64-bit integer limbs per element: a contribution v becomes v * 2^(e+L) with a
+ * per-image power of two 2^e from the bound |grad_input| <= KT * HWo * max_k sum_co |W[co,k]| * max|grad_output_b|
+ * * max|mask_b| (bound * 2^e < 2^60), split exactly into hi = floor(v * 2^e) (signed, two's complement) and
+ * lo = floor(frac * 2^L) (L = 40 while KT * HWo < 2^24, fewer bits beyond), both added with integer atomics and
+ * converted to double once at the end; the resolution is about bound * 2^-100.  An image with an inf or NaN in
+ * grad_output, weight or its mask gets an all-NaN grad_input.  grad_offset / grad_mask have one writer each, dW
+ * is added over fixed pixel ranges in range order, grad_bias in a fixed tree.  Errors: CNB_EINVAL (null pointer,
+ * bad shape, too small a workspace), checked before any CUDA call. */
+size_t cnb_dcnv2_f64_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw,
+                                     int stride, int pad, int dil, int dg);
+int cnb_dcnv2_forward_f64(const double *input, const double *offset, const double *mask,
+                          const double *weight, const double *bias, double *output,
+                          int b, int cin, int h, int w, int cout, int kh, int kw,
+                          int stride_h, int stride_w, int pad_h, int pad_w,
+                          int dil_h, int dil_w, int deformable_groups, void *stream);
+int cnb_dcnv2_backward_f64(const double *input, const double *offset, const double *mask,
+                           const double *weight, const double *grad_output,
+                           double *grad_input, double *grad_offset, double *grad_mask,
+                           double *grad_weight, double *grad_bias,
+                           int b, int cin, int h, int w, int cout, int kh, int kw,
+                           int stride_h, int stride_w, int pad_h, int pad_w,
+                           int dil_h, int dil_w, int deformable_groups,
+                           void *workspace, size_t workspace_bytes, void *stream);
+
 /* ------------------------------------------- N4: deformable PSROI pooling
  * Replaces dcn_v2_psroi_pooling_cuda_forward / _backward (src/dcn_v2_cuda.h:35-55,
  * src/cuda/dcn_v2_psroi_pooling_cuda.cu:47-255).  data [b,c,h,w]; rois [num_rois,5]
@@ -309,6 +344,27 @@ int cnb_psroi_pooling_backward(const float *grad_out, const float *data, const f
                                int no_trans, float spatial_scale, int output_dim, int group_size,
                                int pooled_size, int part_size, int sample_per_part, float trans_std,
                                void *stream);
+/* float64 (dcn_v2_psroi_pooling_cuda_double.cu): same arguments with double tensors, rois included; with offsets,
+ * output_dim must be a multiple of channels_trans / 2.  The backward is bit-identical run to run: grad_data goes
+ * through the two-limb fixed-point sum of cnb_dcnv2_backward_f64 (one bound, N * pooled^2 * max|grad_out|, for
+ * the whole call; an inf or NaN anywhere in grad_out makes all of grad_data NaN) and each grad_trans element has
+ * one writer that adds its bins' samples in order.  It needs a
+ * workspace of cnb_psroi_pooling_f64_workspace_bytes (16-byte aligned) and accumulates into zero-filled
+ * grad_data / grad_trans. */
+size_t cnb_psroi_pooling_f64_workspace_bytes(int b, int c, int h, int w);
+int cnb_psroi_pooling_forward_f64(const double *data, const double *rois, const double *trans,
+                                  double *out, double *top_count,
+                                  int b, int c, int h, int w, int num_rois, int channels_trans,
+                                  int no_trans, double spatial_scale, int output_dim, int group_size,
+                                  int pooled_size, int part_size, int sample_per_part, double trans_std,
+                                  void *stream);
+int cnb_psroi_pooling_backward_f64(const double *grad_out, const double *data, const double *rois,
+                                   const double *trans, const double *top_count,
+                                   double *grad_data, double *grad_trans,
+                                   int b, int c, int h, int w, int num_rois, int channels_trans,
+                                   int no_trans, double spatial_scale, int output_dim, int group_size,
+                                   int pooled_size, int part_size, int sample_per_part, double trans_std,
+                                   void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------- N2: detection post-processing
  * Device-side replacements of utils/post_process.py:83-114 (ctdet_post_process,
