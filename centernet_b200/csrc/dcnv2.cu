@@ -21,7 +21,7 @@
 // chunk by chunk and turns the column gradient into dX (atomicAdd scatter, as the reference),
 // dOffset and dMask without materialising it; k_dcn_bwd_weight accumulates dW / dBias over a
 // range of pixel tiles in registers and adds them to the (accumulating) outputs once per CTA.
-#include "common.cuh"
+#include "dcnv2_tc.cuh"
 
 namespace cnb {
 
@@ -494,99 +494,126 @@ __global__ void __launch_bounds__(256) k_dcn_bwd_bias(const float *__restrict__ 
   }
 }
 
-static int check_shape(const char *fn, int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph,
-                       int pw, int dh, int dw, int dg, DcnShape *s) {
+// The one validation of every fp32 DCNv2 entry point and workspace query, then the plan of the call (dcnv2_tc.cuh).
+// x_cl / gx_cl: the caller's input / grad_input are channels-last.
+static int dcn_plan(const char *fn, int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph,
+                    int pw, int dh, int dw, int dg, bool det, bool x_cl, bool gx_cl, DcnPlan *p) {
   CNB_REQUIRE(b > 0 && cin > 0 && h > 0 && w > 0 && cout > 0 && kh > 0 && kw > 0, CNB_EINVAL,
               "%s: non-positive dimension", fn);
   CNB_REQUIRE(sh > 0 && sw > 0 && dh > 0 && dw > 0 && ph >= 0 && pw >= 0 && dg > 0, CNB_EINVAL,
               "%s: bad stride/dilation/padding/groups", fn);
   CNB_REQUIRE(cin % dg == 0, CNB_EINVAL, "%s: channels (%d) not divisible by deformable groups (%d)", fn, cin, dg);
-  CNB_REQUIRE(kh * kw <= DCN_KT_MAX, CNB_EUNSUPPORTED, "%s: kernel %dx%d has more than %d taps", fn, kh, kw,
+  CNB_REQUIRE((long long)kh * kw <= DCN_KT_MAX, CNB_EUNSUPPORTED, "%s: kernel %dx%d has more than %d taps", fn, kh, kw,
               DCN_KT_MAX);
-  s->B = b; s->Cin = cin; s->H = h; s->W = w; s->Cout = cout; s->kh = kh; s->kw = kw; s->sh = sh; s->sw = sw;
-  s->ph = ph; s->pw = pw; s->dh = dh; s->dw = dw; s->dg = dg;
-  s->Ho = (h + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1;   // dcn_v2_cuda.c:40-41
-  s->Wo = (w + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-  CNB_REQUIRE(s->Ho > 0 && s->Wo > 0, CNB_EINVAL, "%s: empty output", fn);
-  CNB_REQUIRE((long long)h * w < (1ll << 31) && (long long)s->Ho * s->Wo < (1ll << 31), CNB_EUNSUPPORTED,
+  const int ho = (h + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1;   // dcn_v2_cuda.c:40-41
+  const int wo = (w + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
+  CNB_REQUIRE(ho > 0 && wo > 0, CNB_EINVAL, "%s: empty output", fn);
+  CNB_REQUIRE((long long)h * w < (1ll << 31) && (long long)ho * wo < (1ll << 31), CNB_EUNSUPPORTED,
               "%s: plane too large", fn);
+  fill_shape(&p->s, b, cin, h, w, cout, kh, kw, sh, sw, ph, pw, dh, dw, dg);
+  const bool whole_blocks = (cin / dg) % TC_CB == 0;
+  p->det = det;
+  p->x_cl = x_cl && whole_blocks;
+  p->gx_cl = gx_cl && whole_blocks;
+  p->xt_ready = false;
+  p->fwd_tc = sh == sw && ph == pw && dh == dw;   // and at most 9 taps, checked above
+  p->fp32_dw_splits = fp32_weight_splits(b, cin, cout, dg, ((long long)ho * wo + DCN_TP - 1) / DCN_TP);
+  plan_forward_tc(p);
+  plan_backward_tc(p);
+  return CNB_OK;
+}
+
+// the fp32 kernels' view of the validated shape
+static DcnShape fp32_shape(const DcnShapeTc &t) {
+  return {t.B, t.Cin, t.H, t.W, t.Cout, t.kh, t.kw, t.sh, t.sw, t.ph, t.pw, t.dh, t.dw, t.dg, t.Ho, t.Wo};
+}
+
+// fp32 CUDA-core backward of dX, dOffset, dMask
+static int fp32_backward_data(const DcnShape &s, const float *input, const float *offset, const float *mask,
+                              const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                              float *grad_mask, cudaStream_t stream) {
+  constexpr int KC = DCN_CK * DCN_KT_MAX;
+  const int tiles = (int)(((long long)s.Ho * s.Wo + DCN_TP - 1) / DCN_TP);
+  const size_t smem = sizeof(BwdMeta) * DCN_KT_MAX * DCN_TP + sizeof(float) * KC * DCN_TP +
+                      sizeof(float) * 64 * DCN_TP + sizeof(float) * 64 * (KC + 1) +
+                      3 * sizeof(float) * DCN_KT_MAX * DCN_TP;
+  CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_data, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // small maps: fewer pixel tiles than SMs -> also split the channel chunks over blockIdx.y
+  const int chunks_pg = (s.Cin / s.dg + DCN_CK - 1) / DCN_CK;
+  int csplit = (int)((2ll * num_sms() + (long long)s.B * tiles - 1) / ((long long)s.B * tiles));
+  if (csplit > chunks_pg) csplit = chunks_pg;
+  if (csplit < 1 || (long long)s.B * tiles >= num_sms()) csplit = 1;
+  dim3 dgrid((unsigned)(s.B * tiles), (unsigned)csplit);
+  k_dcn_bwd_data<<<dgrid, DCN_THREADS, smem, stream>>>(input, offset, mask, weight, grad_output, grad_input,
+                                                       grad_offset, grad_mask, s, csplit);
+  CNB_CHECK_LAUNCH("cnb_dcnv2_backward data");
+  count_launch();
+  return CNB_OK;
+}
+
+// fp32 CUDA-core backward of dW; wpart != NULL (deterministic mode): per-split partials, added in split order
+static int fp32_backward_weight(const DcnShape &s, int splits, const float *input, const float *offset,
+                                const float *mask, const float *grad_output, float *grad_weight, float *wpart,
+                                cudaStream_t stream) {
+  constexpr int KC = DCN_CK * DCN_KT_MAX;
+  const int cpg = s.Cin / s.dg;
+  const int chunks = s.dg * ((cpg + DCN_CK - 1) / DCN_CK);
+  const int cot = (s.Cout + 63) / 64;
+  const size_t smem = sizeof(TapMeta) * DCN_KT_MAX * DCN_TP + sizeof(float) * KC * DCN_TP +
+                      sizeof(float) * DCN_TP * 65;
+  CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  dim3 grid((unsigned)chunks, (unsigned)cot, (unsigned)splits);
+  k_dcn_bwd_weight<<<grid, DCN_THREADS, smem, stream>>>(input, offset, mask, grad_output, grad_weight, wpart, s, splits);
+  CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight");
+  count_launch();
+  if (wpart) {
+    const long long n = (long long)s.Cout * s.Cin * s.kh * s.kw;
+    k_dcn_bwd_wsum<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(wpart, grad_weight, n, splits);
+    CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight partials");
+    count_launch();
+  }
   return CNB_OK;
 }
 
 }  // namespace cnb
 
-namespace cnb {
-size_t dcn_tc_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg);
-size_t dcn_tc_fwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg);
-size_t dcn_tc_wtiles_bytes(int cin, int cout, int dg);
-int dcn_prepare_weights_tc(const float *weight, int cin, int cout, int kh, int kw, int dg, float *wtiles,
-                           cudaStream_t stream);
-int dcn_forward_tc_prepared(const float *input, int input_nhwc, const float *offset, const float *mask,
-                            const float *wtiles, const float *bias, float *output, int b, int cin, int h, int w,
-                            int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int dg,
-                            void *workspace, cudaStream_t stream, int fused_offset_mask, const float *epi_scale,
-                            const float *epi_shift, int relu);
-int dcn_forward_tc(const float *input, const float *offset, const float *mask, const float *weight,
-                   const float *bias, float *output, int b, int cin, int h, int w, int cout, int kh, int kw, int sh,
-                   int sw, int ph, int pw, int dh, int dw, int dg, void *workspace, cudaStream_t stream);
-size_t dcn_tc_bwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg);
-size_t dcn_tc_bwd_det_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg);
-extern std::atomic<int> g_dcn_deterministic;
-int dcn_backward_data_tc(const float *input, const float *offset, const float *mask, const float *weight,
-                         const float *grad_output, float *grad_input, float *grad_offset, float *grad_mask, int b,
-                         int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
-                         int dg, void *workspace, cudaStream_t stream, int xt_ready, int layout, int det_mode);
-int dcn_backward_weight_tc(const float *input, const float *offset, const float *mask, const float *grad_output,
-                           float *grad_weight, float *grad_bias, int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int sw,
-                           int ph, int pw, int dh, int dw, int dg, void *workspace, cudaStream_t stream, int xt_ready,
-                           int layout);
-}
-
 using namespace cnb;
-
-// Workspace of the tensor-core backward (0: not covered).  Deterministic mode appends one region, used first by the
-// fixed-point dX of the data pass and then, for cout > 256, by the per-split partials of the fp32 dW kernel.
-static size_t dcn_bwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int stride, int pad,
-                                      int dil, int dg, bool det) {
-  const size_t base = dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg);
-  if (!base || !det) return base;
-  size_t extra = dcn_tc_bwd_det_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg);
-  if (cout > 256) {
-    const long long ho = (h + 2 * pad - (dil * (kh - 1) + 1)) / stride + 1, wo = (w + 2 * pad - (dil * (kw - 1) + 1)) / stride + 1;
-    const long long tiles = (ho * wo + DCN_TP - 1) / DCN_TP;
-    const size_t wpart = align_up((size_t)fp32_weight_splits(b, cin, cout, dg, tiles) * cout * cin * kh * kw * 4, 256);
-    if (wpart > extra) extra = wpart;
-  }
-  return base + extra;
-}
 
 extern "C" {
 
 // No column / ones scratch (the reference's `columns`, `ones`): the workspace holds the weights re-tiled
 // (TF32 hi/lo split, wgmma K-major layout) and a channels-last copy of the input for the tensor-core forward.  Passing workspace == NULL
-// (or too small) to cnb_dcnv2_forward selects the fp32 CUDA-core kernel instead.
+// (or too small) to cnb_dcnv2_forward selects the fp32 CUDA-core kernel instead.  Every query returns 0 for a shape
+// the calls reject.
 size_t cnb_dcnv2_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw, int stride, int pad, int dil,
                                  int dg) {
-  if (b <= 0 || h <= 0 || w <= 0 || cin <= 0 || cout <= 0 || dg <= 0 || cin % dg != 0 || kh * kw > DCN_KT_MAX ||
-      stride <= 0 || dil <= 0 || pad < 0)
+  DcnPlan p;
+  if (dcn_plan("cnb_dcnv2_workspace_bytes", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg, false,
+               false, false, &p) != CNB_OK)
     return 0;
-  return dcn_tc_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg);
+  return p.fwd.bytes;
 }
 
+// Process-wide; every backward call reads it once and hands it down in its plan.
+static std::atomic<int> g_dcn_deterministic{0};
 void cnb_dcnv2_set_deterministic(int on) { g_dcn_deterministic.store(on ? 1 : 0, std::memory_order_relaxed); }
 int cnb_dcnv2_get_deterministic(void) { return g_dcn_deterministic.load(std::memory_order_relaxed); }
 
 size_t cnb_dcnv2_backward_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw, int stride, int pad,
                                           int dil, int dg) {
-  if (b <= 0 || h <= 0 || w <= 0 || cin <= 0 || cout <= 0 || dg <= 0 || cin % dg != 0 || kh * kw > DCN_KT_MAX ||
-      stride <= 0 || dil <= 0 || pad < 0)
+  DcnPlan p;
+  if (dcn_plan("cnb_dcnv2_backward_workspace_bytes", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg,
+               cnb_dcnv2_get_deterministic() != 0, false, false, &p) != CNB_OK || !p.bwd_tc)
     return 0;
-  return dcn_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg, cnb_dcnv2_get_deterministic() != 0);
+  return p.bwd.bytes;
 }
 
 size_t cnb_dcnv2_wtiles_bytes(int cin, int cout, int kh, int kw, int dg) {
-  if (cin <= 0 || cout <= 0 || dg <= 0 || cin % dg != 0 || kh * kw > DCN_KT_MAX) return 0;
-  return dcn_tc_wtiles_bytes(cin, cout, dg);
+  DcnPlan p;   // the weight tiles do not depend on the image: any one the kernel fits in will do
+  if (dcn_plan("cnb_dcnv2_wtiles_bytes", 1, cin, 8, 8, cout, kh, kw, 1, 1, 1, 1, 1, 1, dg, false, false, false, &p) !=
+      CNB_OK)
+    return 0;
+  return p.fwd.wtiles_bytes;
 }
 
 int cnb_dcnv2_prepare_weights(const float *weight, int cin, int cout, int kh, int kw, int deformable_groups,
@@ -595,9 +622,8 @@ int cnb_dcnv2_prepare_weights(const float *weight, int cin, int cout, int kh, in
   CNB_REQUIRE(cin > 0 && cout > 0 && kh > 0 && kw > 0 && deformable_groups > 0 && cin % deformable_groups == 0,
               CNB_EINVAL, "cnb_dcnv2_prepare_weights: bad shape");
   CNB_REQUIRE(kh * kw <= DCN_KT_MAX, CNB_EUNSUPPORTED, "cnb_dcnv2_prepare_weights: more than %d taps", DCN_KT_MAX);
-  CNB_REQUIRE(wtiles_bytes >= dcn_tc_wtiles_bytes(cin, cout, deformable_groups), CNB_EWORKSPACE,
-              "cnb_dcnv2_prepare_weights: buffer %zu < %zu", wtiles_bytes,
-              dcn_tc_wtiles_bytes(cin, cout, deformable_groups));
+  const size_t need = cnb_dcnv2_wtiles_bytes(cin, cout, kh, kw, deformable_groups);
+  CNB_REQUIRE(wtiles_bytes >= need, CNB_EWORKSPACE, "cnb_dcnv2_prepare_weights: buffer %zu < %zu", wtiles_bytes, need);
   CNB_REQUIRE((reinterpret_cast<uintptr_t>(wtiles) & 15u) == 0, CNB_EINVAL,
               "cnb_dcnv2_prepare_weights: buffer must be 16-byte aligned");
   return dcn_prepare_weights_tc(weight, cin, cout, kh, kw, deformable_groups, reinterpret_cast<float *>(wtiles),
@@ -606,10 +632,11 @@ int cnb_dcnv2_prepare_weights(const float *weight, int cin, int cout, int kh, in
 
 size_t cnb_dcnv2_prepared_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw, int stride, int pad,
                                           int dil, int dg) {
-  if (b <= 0 || h <= 0 || w <= 0 || cin <= 0 || cout <= 0 || dg <= 0 || cin % dg != 0 || kh * kw > DCN_KT_MAX ||
-      stride <= 0 || dil <= 0 || pad < 0)
+  DcnPlan p;
+  if (dcn_plan("cnb_dcnv2_prepared_workspace_bytes", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg,
+               false, false, false, &p) != CNB_OK)
     return 0;
-  return dcn_tc_fwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil, dg);
+  return p.fwd.prepared_bytes;
 }
 
 int cnb_dcnv2_forward_prepared(const float *input, int input_channels_last, const float *offset, const float *mask,
@@ -619,21 +646,17 @@ int cnb_dcnv2_forward_prepared(const float *input, int input_channels_last, cons
                                void *stream_) {
   CNB_REQUIRE(input && offset && mask && wtiles && output && workspace, CNB_EINVAL,
               "cnb_dcnv2_forward_prepared: null pointer");
-  DcnShape s;
-  int rc = check_shape("cnb_dcnv2_forward_prepared", b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w,
-                       dil_h, dil_w, deformable_groups, &s);
+  DcnPlan p;
+  int rc = dcn_plan("cnb_dcnv2_forward_prepared", b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h,
+                    dil_w, deformable_groups, false, input_channels_last != 0, false, &p);
   if (rc != CNB_OK) return rc;
-  CNB_REQUIRE(stride_h == stride_w && pad_h == pad_w && dil_h == dil_w, CNB_EUNSUPPORTED,
-              "cnb_dcnv2_forward_prepared: anisotropic stride/pad/dilation");
-  CNB_REQUIRE(workspace_bytes >= dcn_tc_fwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride_h, pad_h, dil_h,
-                                                            deformable_groups),
-              CNB_EWORKSPACE, "cnb_dcnv2_forward_prepared: workspace too small");
+  CNB_REQUIRE(p.fwd_tc, CNB_EUNSUPPORTED, "cnb_dcnv2_forward_prepared: anisotropic stride/pad/dilation");
+  CNB_REQUIRE(workspace_bytes >= p.fwd.prepared_bytes, CNB_EWORKSPACE, "cnb_dcnv2_forward_prepared: workspace too small");
   CNB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15u) == 0 && (reinterpret_cast<uintptr_t>(wtiles) & 15u) == 0 &&
                   (reinterpret_cast<uintptr_t>(input) & 15u) == 0,
               CNB_EINVAL, "cnb_dcnv2_forward_prepared: buffers must be 16-byte aligned");
-  return dcn_forward_tc_prepared(input, input_channels_last, offset, mask, reinterpret_cast<const float *>(wtiles),
-                                 bias, output, b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h,
-                                 dil_w, deformable_groups, workspace, (cudaStream_t)stream_, 0, nullptr, nullptr, 0);
+  return dcn_forward_tc_prepared(p, input, offset, mask, reinterpret_cast<const float *>(wtiles), bias, output,
+                                 workspace, (cudaStream_t)stream_, 0, nullptr, nullptr, 0);
 }
 
 int cnb_dcnv2_forward_fused(const float *input, int input_channels_last, const float *offset_mask, const void *wtiles,
@@ -644,20 +667,16 @@ int cnb_dcnv2_forward_fused(const float *input, int input_channels_last, const f
               "cnb_dcnv2_forward_fused: null pointer");
   CNB_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), CNB_EINVAL,
               "cnb_dcnv2_forward_fused: bn_scale and bn_shift go together");
-  DcnShape s;
-  int rc = check_shape("cnb_dcnv2_forward_fused", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil,
-                       deformable_groups, &s);
+  DcnPlan p;
+  int rc = dcn_plan("cnb_dcnv2_forward_fused", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil,
+                    deformable_groups, false, input_channels_last != 0, false, &p);
   if (rc != CNB_OK) return rc;
-  CNB_REQUIRE(workspace_bytes >= dcn_tc_fwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride, pad, dil,
-                                                            deformable_groups),
-              CNB_EWORKSPACE, "cnb_dcnv2_forward_fused: workspace too small");
+  CNB_REQUIRE(workspace_bytes >= p.fwd.prepared_bytes, CNB_EWORKSPACE, "cnb_dcnv2_forward_fused: workspace too small");
   CNB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15u) == 0 && (reinterpret_cast<uintptr_t>(wtiles) & 15u) == 0 &&
                   (reinterpret_cast<uintptr_t>(input) & 15u) == 0,
               CNB_EINVAL, "cnb_dcnv2_forward_fused: buffers must be 16-byte aligned");
-  return dcn_forward_tc_prepared(input, input_channels_last, offset_mask, nullptr,
-                                 reinterpret_cast<const float *>(wtiles), bias, output, b, cin, h, w, cout, kh, kw, stride,
-                                 stride, pad, pad, dil, dil, deformable_groups, workspace, (cudaStream_t)stream_, 1,
-                                 bn_scale, bn_shift, relu);
+  return dcn_forward_tc_prepared(p, input, offset_mask, nullptr, reinterpret_cast<const float *>(wtiles), bias, output,
+                                 workspace, (cudaStream_t)stream_, 1, bn_scale, bn_shift, relu);
 }
 
 int cnb_dcnv2_forward(const float *input, const float *offset, const float *mask, const float *weight,
@@ -665,18 +684,22 @@ int cnb_dcnv2_forward(const float *input, const float *offset, const float *mask
                       int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int deformable_groups,
                       void *workspace, size_t workspace_bytes, void *stream_) {
   CNB_REQUIRE(input && offset && mask && weight && output, CNB_EINVAL, "cnb_dcnv2_forward: null pointer");
-  DcnShape s;
-  int rc = check_shape("cnb_dcnv2_forward", b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h,
-                       dil_w, deformable_groups, &s);
+  DcnPlan p;
+  int rc = dcn_plan("cnb_dcnv2_forward", b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w,
+                    deformable_groups, false, false, false, &p);
   if (rc != CNB_OK) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (workspace && stride_h == stride_w && pad_h == pad_w && dil_h == dil_w &&
-      workspace_bytes >= dcn_tc_workspace_bytes(b, cin, h, w, cout, kh, kw, stride_h, pad_h, dil_h, deformable_groups) &&
-      (reinterpret_cast<uintptr_t>(workspace) & 15u) == 0)
-    return dcn_forward_tc(input, offset, mask, weight, bias, output, b, cin, h, w, cout, kh, kw, stride_h, stride_w,
-                          pad_h, pad_w, dil_h, dil_w, deformable_groups, workspace, stream);
-  const long long HWo = (long long)s.Ho * s.Wo;
-  const int tiles = (int)((HWo + DCN_TP - 1) / DCN_TP);
+  if (p.fwd_tc && workspace && workspace_bytes >= p.fwd.bytes && (reinterpret_cast<uintptr_t>(workspace) & 15u) == 0) {
+    // the weight tiles at the head of the workspace, the prepared forward's workspace behind them
+    float *wt = reinterpret_cast<float *>(workspace);
+    rc = dcn_prepare_weights_tc(weight, cin, cout, kh, kw, deformable_groups, wt, stream);
+    if (rc != CNB_OK) return rc;
+    return dcn_forward_tc_prepared(p, input, offset, mask, wt, bias, output,
+                                   reinterpret_cast<char *>(workspace) + p.fwd.wtiles_bytes, stream, 0, nullptr,
+                                   nullptr, 0);
+  }
+  const DcnShape s = fp32_shape(p.s);
+  const int tiles = (int)(((long long)s.Ho * s.Wo + DCN_TP - 1) / DCN_TP);
   const int nsets = cout > 64 ? 2 : 1;
   const int co_t = 64 * nsets;
   const size_t smem = sizeof(TapMeta) * DCN_KT_MAX * DCN_TP + sizeof(float) * DCN_CK * DCN_KT_MAX * DCN_TP +
@@ -699,93 +722,49 @@ static int dcnv2_backward_impl(const float *input, const float *offset, const fl
                                float *grad_weight, float *grad_bias, int b, int cin, int h, int w, int cout, int kh,
                                int kw, int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w,
                                int deformable_groups, void *workspace, size_t workspace_bytes, void *stream_,
-                               int layout) {
+                               bool input_cl, bool grad_input_cl) {
   CNB_REQUIRE(input && offset && mask && weight && grad_output, CNB_EINVAL, "cnb_dcnv2_backward: null pointer");
-  DcnShape s;
-  int rc = check_shape("cnb_dcnv2_backward", b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h,
-                       dil_w, deformable_groups, &s);
+  DcnPlan p;
+  int rc = dcn_plan("cnb_dcnv2_backward", b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w,
+                    deformable_groups, cnb_dcnv2_get_deterministic() != 0, input_cl, grad_input_cl && grad_input, &p);
   if (rc != CNB_OK) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
-  const long long HWo = (long long)s.Ho * s.Wo;
-  const int tiles = (int)((HWo + DCN_TP - 1) / DCN_TP);
-  constexpr int KC = DCN_CK * DCN_KT_MAX;
-  int launches = 0;
-  // tensor-core path (dcnv2_bwd_tc.cu) when the caller provides the workspace; else the fp32 CUDA-core kernels below
-  const bool det = cnb_dcnv2_get_deterministic() != 0;
-  const bool iso = stride_h == stride_w && pad_h == pad_w && dil_h == dil_w;
-  const size_t need = (iso && kh * kw <= DCN_KT_MAX)
-                          ? dcn_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride_h, pad_h, dil_h, deformable_groups, det)
-                          : 0;
-  const bool tc = workspace && need > 0 && workspace_bytes >= need && (reinterpret_cast<uintptr_t>(workspace) & 15u) == 0;
+  const bool data = grad_input || grad_offset || grad_mask;
+  // tensor-core path (dcnv2_bwd_tc.cu) when the caller provides the workspace; else the fp32 CUDA-core kernels
+  const bool tc = p.bwd_tc && workspace && workspace_bytes >= p.bwd.bytes &&
+                  (reinterpret_cast<uintptr_t>(workspace) & 15u) == 0;
   // deterministic mode is implemented by the tensor-core backward only (the fp32 kernels scatter with atomics)
-  CNB_REQUIRE(!det || tc || !(grad_input || grad_offset || grad_mask || grad_weight), CNB_EUNSUPPORTED,
+  CNB_REQUIRE(!p.det || tc || !(data || grad_weight), CNB_EUNSUPPORTED,
               "cnb_dcnv2_backward: deterministic mode (cnb_dcnv2_set_deterministic) needs the tensor-core backward: a "
               "workspace of cnb_dcnv2_backward_workspace_bytes queried in deterministic mode, at most 9 taps, isotropic "
               "stride/pad/dilation and images within its 32-bit indexing");
-  if (layout) {   // channels-last input / grad_input: tensor-core path only, whole 32-channel blocks, scatter form of dX
-    CNB_REQUIRE(tc && cout <= 256, CNB_EUNSUPPORTED, "cnb_dcnv2_backward_ex: channels-last tensors need the tensor-core path "
+  if (input_cl || grad_input_cl) {   // channels-last input / grad_input: tensor-core path only, whole 32-channel blocks, scatter form of dX
+    CNB_REQUIRE(tc && p.dw_tc, CNB_EUNSUPPORTED, "cnb_dcnv2_backward_ex: channels-last tensors need the tensor-core path "
                 "(workspace of cnb_dcnv2_backward_workspace_bytes, at most 9 taps, isotropic stride/pad/dilation, cout <= 256)");
     CNB_REQUIRE((cin / deformable_groups) % 32 == 0, CNB_EUNSUPPORTED,
                 "cnb_dcnv2_backward_ex: channels-last tensors need cin / deformable_groups to be a multiple of 32");
-    if (!grad_input) layout &= ~2;
   }
-  if (tc && (grad_input || grad_offset || grad_mask)) {
-    rc = dcn_backward_data_tc(input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask, b, cin, h, w,
-                              cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, deformable_groups, workspace,
-                              stream, 0, layout, det ? 1 : 0);
+  const DcnShape s = fp32_shape(p.s);
+  if (data) {
+    rc = tc ? dcn_backward_data_tc(p, input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask,
+                                   workspace, stream)
+            : fp32_backward_data(s, input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask, stream);
     if (rc != CNB_OK) return rc;
-  } else if (grad_input || grad_offset || grad_mask) {
-    const size_t smem = sizeof(BwdMeta) * DCN_KT_MAX * DCN_TP + sizeof(float) * KC * DCN_TP +
-                        sizeof(float) * 64 * DCN_TP + sizeof(float) * 64 * (KC + 1) +
-                        3 * sizeof(float) * DCN_KT_MAX * DCN_TP;
-    CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_data, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // small maps: fewer pixel tiles than SMs -> also split the channel chunks over blockIdx.y
-    const int chunks_pg = (cin / deformable_groups + DCN_CK - 1) / DCN_CK;
-    int csplit = (int)((2ll * num_sms() + (long long)b * tiles - 1) / ((long long)b * tiles));
-    if (csplit > chunks_pg) csplit = chunks_pg;
-    if (csplit < 1 || (long long)b * tiles >= num_sms()) csplit = 1;
-    dim3 dgrid((unsigned)(b * tiles), (unsigned)csplit);
-    k_dcn_bwd_data<<<dgrid, DCN_THREADS, smem, stream>>>(input, offset, mask, weight, grad_output, grad_input,
-                                                         grad_offset, grad_mask, s, csplit);
-    CNB_CHECK_LAUNCH("cnb_dcnv2_backward data");
-    ++launches;
   }
-  if (tc && grad_weight && cout <= 256) {
-    rc = dcn_backward_weight_tc(input, offset, mask, grad_output, grad_weight, grad_bias, b, cin, h, w, cout, kh, kw, stride_h,
-                                stride_w, pad_h, pad_w, dil_h, dil_w, deformable_groups, workspace, stream,
-                                (grad_input || grad_offset || grad_mask) ? 1 : 0, layout);
-    if (rc != CNB_OK) return rc;
+  if (grad_weight && tc && p.dw_tc) {
+    p.xt_ready = data;
+    rc = dcn_backward_weight_tc(p, input, offset, mask, grad_output, grad_weight, grad_bias, workspace, stream);
     grad_bias = nullptr;   // done by the weight pass
   } else if (grad_weight) {
-    const int cpg = cin / deformable_groups;
-    const int chunks = deformable_groups * ((cpg + DCN_CK - 1) / DCN_CK);
-    const int cot = (cout + 63) / 64;
-    const int splits = fp32_weight_splits(b, cin, cout, deformable_groups, tiles);
-    const size_t smem = sizeof(TapMeta) * DCN_KT_MAX * DCN_TP + sizeof(float) * KC * DCN_TP +
-                        sizeof(float) * DCN_TP * 65;
-    // deterministic mode (tc here): per-split partials in the region behind the tensor-core workspace
-    float *wpart = det ? reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) +
-                                                   dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, stride_h, pad_h,
-                                                                              dil_h, deformable_groups))
-                       : nullptr;
-    CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid((unsigned)chunks, (unsigned)cot, (unsigned)splits);
-    k_dcn_bwd_weight<<<grid, DCN_THREADS, smem, stream>>>(input, offset, mask, grad_output, grad_weight, wpart, s, splits);
-    CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight");
-    ++launches;
-    if (wpart) {
-      const long long n = (long long)cout * cin * kh * kw;
-      k_dcn_bwd_wsum<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(wpart, grad_weight, n, splits);
-      CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight partials");
-      ++launches;
-    }
+    float *wpart = p.det ? reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bwd.wpart32) : nullptr;
+    rc = fp32_backward_weight(s, p.fp32_dw_splits, input, offset, mask, grad_output, grad_weight, wpart, stream);
   }
+  if (rc != CNB_OK) return rc;
   if (grad_bias) {
-    k_dcn_bwd_bias<<<cout, 256, 0, stream>>>(grad_output, grad_bias, b, cout, HWo);
+    k_dcn_bwd_bias<<<cout, 256, 0, stream>>>(grad_output, grad_bias, b, cout, (long long)s.Ho * s.Wo);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward bias");
-    ++launches;
+    count_launch();
   }
-  count_launch(launches);
   return CNB_OK;
 }
 
@@ -796,7 +775,7 @@ int cnb_dcnv2_backward(const float *input, const float *offset, const float *mas
                        void *workspace, size_t workspace_bytes, void *stream_) {
   return dcnv2_backward_impl(input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask, grad_weight,
                              grad_bias, b, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w,
-                             deformable_groups, workspace, workspace_bytes, stream_, 0);
+                             deformable_groups, workspace, workspace_bytes, stream_, false, false);
 }
 
 int cnb_dcnv2_backward_ex(const float *input, int input_channels_last, const float *offset, const float *mask,
@@ -806,8 +785,8 @@ int cnb_dcnv2_backward_ex(const float *input, int input_channels_last, const flo
                           int dil, int deformable_groups, void *workspace, size_t workspace_bytes, void *stream_) {
   return dcnv2_backward_impl(input, offset, mask, weight, grad_output, grad_input, grad_offset, grad_mask, grad_weight,
                              grad_bias, b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, deformable_groups,
-                             workspace, workspace_bytes, stream_,
-                             (input_channels_last ? 1 : 0) | (grad_input_channels_last ? 2 : 0));
+                             workspace, workspace_bytes, stream_, input_channels_last != 0,
+                             grad_input_channels_last != 0);
 }
 
 }  // extern "C"

@@ -23,7 +23,10 @@
 // (never in HBM), keeps a [128 rows = 4 chunks x 32 ch] x (64|128 output channels) accumulator in the registers of two
 // warpgroups over its whole pixel range and
 // writes one partial per CTA; k_dcn_bwd_wreduce adds the partials in a fixed order (deterministic).
+// plan_backward_tc lays out every region of the workspace these passes use (DcnPlan::bwd in dcnv2_tc.cuh); the
+// hosts below only read their pointers from the plan.
 #include <stdlib.h>
+#include <algorithm>
 #include "dcnv2_tc.cuh"
 
 namespace cnb {
@@ -819,93 +822,81 @@ __global__ void __launch_bounds__(256) k_dcn_bwd_wreduce(const float *__restrict
 }
 
 // ------------------------------------------------------------------ host
-std::atomic<int> g_dcn_deterministic{0};
-static size_t bw_xt_bytes(const DcnShapeTc &s) { return align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * 4, 256); }
-static size_t bw_wtt_bytes(const BwdGeom &g) { return align_up((size_t)g.RG * g.KS * BW_TILE_FLOATS * 4, 256); }
-static size_t bw_gyt_bytes_per_image(const BwdGeom &g) { return (size_t)g.tiles * g.KS * BW_TILE_FLOATS * 4; }
-static size_t bw_dcol_bytes_per_image(const DcnShapeTc &s, const BwdGeom &g) {
-  return align_up((size_t)s.Ho * s.Wo * g.Qp * TC_CB * 4, 256);
-}
-// images per pass: the column gradient of a pass is held to ~1.5 GiB (B=16 of the largest dla_34 layer is 0.67 GB)
-static int bw_batch_chunk(const DcnShapeTc &s, const BwdGeom &g) {
-  const size_t per = bw_dcol_bytes_per_image(s, g) + bw_gyt_bytes_per_image(g);
-  long long bc = (long long)((1536ull << 20) / per);
-  if (bc < 1) bc = 1;
-  if (bc > s.B) bc = s.B;
-  return (int)bc;
-}
-
-static size_t bw_gyk_bytes(const WgGeom &wg) { return align_up((size_t)wg.n_slices * 2 * wg.co_r * TC_K * 4, 256); }
-static size_t bw_wpart_bytes(const BwdGeom &g, const WgGeom &wg) {
-  return align_up((size_t)wg.splits * g.RG * 128 * wg.co_r * 4, 256);
-}
-static size_t bw_bpart_bytes(const WgGeom &wg) { return align_up((size_t)wg.n_slices * wg.co_r * 4, 256); }
-
-// [xt][dxt][wtt][ max( gyt + dcol of one batch chunk , gyk + wpart ) ]: the data and the weight passes run one after
-// the other on the stream and share the tail
-size_t dcn_tc_bwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg) {
-  DcnShapeTc s;
-  fill_shape(&s, b, cin, h, w, cout, kh, kw, sh, sh, ph, ph, dh, dh, dg);
+void plan_backward_tc(DcnPlan *p) {
+  const DcnShapeTc &s = p->s;
   const BwdGeom g = bwd_geom(s);
   // the kernels index within one image with 32 bits (and pack hl*W+wl into 24): larger images use the fp32 path
-  const unsigned long long lim = 1ull << 31;
-  if ((unsigned long long)(h + 2) * (w + 2) >= (1ull << 24) || (unsigned long long)(h + 2) * (w + 2) * s.nb * TC_CB >= lim ||
-      (unsigned long long)s.Ho * s.Wo * g.Qp * TC_CB >= lim || (unsigned long long)s.Ho * s.Wo * dg * 2 * kh * kw >= lim)
-    return 0;
+  const unsigned long long lim = 1ull << 31, hw2 = (unsigned long long)(s.H + 2) * (s.W + 2);
+  p->bwd_tc = p->fwd_tc && hw2 < (1ull << 24) && hw2 * s.nb * TC_CB < lim &&
+              (unsigned long long)s.Ho * s.Wo * g.Qp * TC_CB < lim &&
+              (unsigned long long)s.Ho * s.Wo * s.dg * 2 * s.kh * s.kw < lim;
+  p->dw_tc = p->bwd_tc && s.Cout <= 256;
+  p->bwd = {};
+  if (!p->bwd_tc) return;
   const WgGeom wg = wg_geom(s, g);
-  const int bc = bw_batch_chunk(s, g);
-  const size_t data = align_up((size_t)bc * bw_gyt_bytes_per_image(g), 256) + (size_t)bc * bw_dcol_bytes_per_image(s, g);
-  const size_t wgt = bw_gyk_bytes(wg) + bw_wpart_bytes(g, wg) + bw_bpart_bytes(wg);
-  return 2 * bw_xt_bytes(s) + bw_wtt_bytes(g) + (data > wgt ? data : wgt);
+  const size_t gyt_img = (size_t)g.tiles * g.KS * BW_TILE_FLOATS * 4;
+  const size_t dcol_img = align_up((size_t)s.Ho * s.Wo * g.Qp * TC_CB * 4, 256);
+  // images per pass: the column gradient of a pass is held to ~1.5 GiB (B=16 of the largest dla_34 layer is 0.67 GB)
+  long long bc = (long long)((1536ull << 20) / (dcol_img + gyt_img));
+  if (bc < 1) bc = 1;
+  if (bc > s.B) bc = s.B;
+  auto &l = p->bwd;
+  l.chunk = (int)bc;
+  l.xt = 0;
+  l.dxt = l.xt + p->xt_bytes;
+  l.wtt = l.dxt + p->xt_bytes;
+  l.gyt = l.wtt + align_up((size_t)g.RG * g.KS * BW_TILE_FLOATS * 4, 256);
+  l.dcol = l.gyt + align_up((size_t)bc * gyt_img, 256);
+  const size_t data_end = l.dcol + (size_t)bc * dcol_img;
+  l.gyk = l.gyt;
+  l.wpart = l.gyk + align_up((size_t)wg.n_slices * 2 * wg.co_r * TC_K * 4, 256);
+  l.bpart = l.wpart + align_up((size_t)wg.splits * g.RG * 128 * wg.co_r * 4, 256);
+  const size_t weight_end = l.bpart + align_up((size_t)wg.n_slices * wg.co_r * 4, 256);
+  const size_t end = std::max(data_end, weight_end);
+  // deterministic mode: [bounds: KS + 2B uint32][fixed-point dX of one batch chunk: bc x HW x Cp int64], or the
+  // per-split dW partials of the fp32 kernel (cout > 256) in the same place, whichever is larger
+  l.bnd = end;
+  l.dxi = l.bnd + align_up((size_t)(g.KS + 2 * s.B) * 4, 256);
+  const size_t dxi_end = l.dxi + align_up((size_t)bc * s.H * s.W * s.nb * TC_CB * 8, 256);
+  l.wpart32 = end;
+  const size_t wpart32_end =
+      s.Cout > 256 ? l.wpart32 + align_up((size_t)p->fp32_dw_splits * s.Cout * s.Cin * s.kh * s.kw * 4, 256) : 0;
+  l.bytes = p->det ? std::max(dxi_end, wpart32_end) : end;
 }
 
-// Deterministic mode appends [bounds: KS + 2B uint32][fixed-point dX of one batch chunk: bc x HW x Cp int64] to the
-// layout above (whose size and use do not change).
-size_t dcn_tc_bwd_det_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg) {
-  DcnShapeTc s;
-  fill_shape(&s, b, cin, h, w, cout, kh, kw, sh, sh, ph, ph, dh, dh, dg);
+// dX, dOffset, dMask (each nullable; accumulated into, as cnb_dcnv2_backward documents).  p.det: dX in fixed point
+// (order-independent) in the regions bnd and dxi.
+int dcn_backward_data_tc(const DcnPlan &p, const float *input, const float *offset, const float *mask,
+                         const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                         float *grad_mask, void *workspace, cudaStream_t stream) {
+  // p.x_cl / p.gx_cl: `input` / grad_input already are channels-last [b][h*w][cin]: the layout passes and the
+  // channels-last scratch copies are skipped
+  const DcnShapeTc &s = p.s;
   const BwdGeom g = bwd_geom(s);
-  const int bc = bw_batch_chunk(s, g);
-  return align_up((size_t)(g.KS + 2 * b) * 4, 256) + align_up((size_t)bc * h * w * s.nb * TC_CB * 8, 256);
-}
-
-// dX, dOffset, dMask (each nullable; accumulated into, as cnb_dcnv2_backward documents).  det != 0: dX in fixed point
-// (order-independent), which needs the workspace of dcn_tc_bwd_det_bytes behind the default one.
-int dcn_backward_data_tc(const float *input, const float *offset, const float *mask, const float *weight,
-                         const float *grad_output, float *grad_input, float *grad_offset, float *grad_mask, int b,
-                         int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
-                         int dg, void *workspace, cudaStream_t stream, int xt_ready, int layout, int det_mode) {
-  // layout bit 0: `input` already is channels-last [b][h*w][cin]; bit 1: so is grad_input (both need cin/dg % 32 == 0,
-  // checked by the caller): the layout passes and the channels-last scratch copies are skipped
-  DcnShapeTc s;
-  fill_shape(&s, b, cin, h, w, cout, kh, kw, sh, sw, ph, pw, dh, dw, dg);
-  const BwdGeom g = bwd_geom(s);
-  const int bc = bw_batch_chunk(s, g);
-  char *wp = reinterpret_cast<char *>(workspace);
-  float *xt = reinterpret_cast<float *>(wp);  wp += bw_xt_bytes(s);
-  float *dxt = reinterpret_cast<float *>(wp); wp += bw_xt_bytes(s);
-  const float *xsrc = (layout & 1) ? input : xt;
-  if (layout & 2) dxt = grad_input;
-  float *wtt = reinterpret_cast<float *>(wp); wp += bw_wtt_bytes(g);
-  float *gyt = reinterpret_cast<float *>(wp); wp += align_up((size_t)bc * bw_gyt_bytes_per_image(g), 256);
-  float *dcol = reinterpret_cast<float *>(wp);
-  const long long HW = (long long)h * w, HWo = (long long)s.Ho * s.Wo;
+  const int b = s.B, cin = s.Cin, cout = s.Cout, bc = p.bwd.chunk;
+  char *ws = reinterpret_cast<char *>(workspace);
+  float *xt = reinterpret_cast<float *>(ws + p.bwd.xt);
+  float *dxt = p.gx_cl ? grad_input : reinterpret_cast<float *>(ws + p.bwd.dxt);
+  const float *xsrc = p.x_cl ? input : xt;
+  float *wtt = reinterpret_cast<float *>(ws + p.bwd.wtt);
+  float *gyt = reinterpret_cast<float *>(ws + p.bwd.gyt);
+  float *dcol = reinterpret_cast<float *>(ws + p.bwd.dcol);
+  const long long HW = (long long)s.H * s.W, HWo = (long long)s.Ho * s.Wo;
   // default: every sample is scattered into a channels-last dX (16-byte vector reductions) and added to grad_input at
   // the end; deterministic mode: into the fixed-point dX of the batch chunk, converted into grad_input per chunk
-  const bool det = grad_input && det_mode;
+  const bool det = grad_input && p.det;
   unsigned *bnd = nullptr;
   long long *dxi = nullptr;
   if (det) {
-    char *dp = reinterpret_cast<char *>(workspace) + dcn_tc_bwd_workspace_bytes(b, cin, h, w, cout, kh, kw, sh, ph, dh, dg);
-    bnd = reinterpret_cast<unsigned *>(dp);
-    dxi = reinterpret_cast<long long *>(dp + align_up((size_t)(g.KS + 2 * b) * 4, 256));
+    bnd = reinterpret_cast<unsigned *>(ws + p.bwd.bnd);
+    dxi = reinterpret_cast<long long *>(ws + p.bwd.dxi);
     CNB_CUDA(cudaMemsetAsync(bnd, 0, (size_t)(g.KS + 2 * b) * 4, stream));
   }
 
   int rc = CNB_OK;
-  if (!xt_ready && !(layout & 1)) rc = dcn_to_channels_last(input, xt, s, stream);
+  if (!p.x_cl) rc = dcn_to_channels_last(input, xt, s, stream);
   if (rc != CNB_OK) return rc;
-  if (grad_input && !det && !(layout & 2)) CNB_CUDA(cudaMemsetAsync(dxt, 0, (size_t)b * HW * s.nb * TC_CB * 4, stream));
+  if (grad_input && !det && !p.gx_cl) CNB_CUDA(cudaMemsetAsync(dxt, 0, (size_t)b * HW * s.nb * TC_CB * 4, stream));
   if (det) k_bwd_prep_w<true><<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtt, bnd);
   else k_bwd_prep_w<false><<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtt, nullptr);
   CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight tiles");
@@ -938,7 +929,7 @@ int dcn_backward_data_tc(const float *input, const float *offset, const float *m
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward offset/mask gradient");
     count_launch(3);
     if (det) {
-      if (layout & 2) {
+      if (p.gx_cl) {
         k_dcn_bwd_dx_fixed<true><<<dim3((unsigned)((HW + 31) / 32), 1u, (unsigned)nbimg), 256, 0, stream>>>(
             dxi, bnd, grad_input, s, g, b0);
       } else {
@@ -949,7 +940,7 @@ int dcn_backward_data_tc(const float *input, const float *offset, const float *m
       count_launch();
     }
   }
-  if (grad_input && !det && !(layout & 2)) {
+  if (grad_input && !det && !p.gx_cl) {
     dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((cin + 63) / 64), (unsigned)b);
     k_dcn_bwd_dx_nchw<<<tgrid, 256, 0, stream>>>(dxt, grad_input, s);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward input gradient");
@@ -958,27 +949,25 @@ int dcn_backward_data_tc(const float *input, const float *offset, const float *m
   return CNB_OK;
 }
 
-// dW and dBias (accumulated into grad_weight / grad_bias; grad_bias nullable).  xt_ready != 0: the channels-last input copy at the head of the workspace was
-// already written by dcn_backward_data_tc on this stream.
-int dcn_backward_weight_tc(const float *input, const float *offset, const float *mask, const float *grad_output,
-                           float *grad_weight, float *grad_bias, int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int sw,
-                           int ph, int pw, int dh, int dw, int dg, void *workspace, cudaStream_t stream, int xt_ready,
-                           int layout) {
-  DcnShapeTc s;
-  fill_shape(&s, b, cin, h, w, cout, kh, kw, sh, sw, ph, pw, dh, dw, dg);
+// dW and dBias (accumulated into grad_weight / grad_bias; grad_bias nullable).  p.xt_ready: the channels-last input
+// copy was already written by dcn_backward_data_tc on this stream.
+int dcn_backward_weight_tc(const DcnPlan &p, const float *input, const float *offset, const float *mask,
+                           const float *grad_output, float *grad_weight, float *grad_bias, void *workspace,
+                           cudaStream_t stream) {
+  const DcnShapeTc &s = p.s;
   const BwdGeom g = bwd_geom(s);
   const WgGeom wg = wg_geom(s, g);
-  char *wp = reinterpret_cast<char *>(workspace);
-  float *xt = reinterpret_cast<float *>(wp);  wp += 2 * bw_xt_bytes(s) + bw_wtt_bytes(g);
-  float *gyk = reinterpret_cast<float *>(wp); wp += bw_gyk_bytes(wg);
-  float *wpart = reinterpret_cast<float *>(wp); wp += bw_wpart_bytes(g, wg);
-  float *bpart = reinterpret_cast<float *>(wp);
-  const float *xsrc = (layout & 1) ? input : xt;
-  if (!xt_ready && !(layout & 1)) {
+  char *ws = reinterpret_cast<char *>(workspace);
+  float *xt = reinterpret_cast<float *>(ws + p.bwd.xt);
+  float *gyk = reinterpret_cast<float *>(ws + p.bwd.gyk);
+  float *wpart = reinterpret_cast<float *>(ws + p.bwd.wpart);
+  float *bpart = reinterpret_cast<float *>(ws + p.bwd.bpart);
+  const float *xsrc = p.x_cl ? input : xt;
+  if (!p.xt_ready && !p.x_cl) {
     const int rc = dcn_to_channels_last(input, xt, s, stream);
     if (rc != CNB_OK) return rc;
   }
-  dim3 pgrid((unsigned)wg.spi, (unsigned)b);
+  dim3 pgrid((unsigned)wg.spi, (unsigned)s.B);
   k_bwd_prep_gyk<<<pgrid, 256, 0, stream>>>(grad_output, s, wg, gyk, grad_bias ? bpart : nullptr);
   CNB_CHECK_LAUNCH("cnb_dcnv2_backward grad_output tiles (weight pass)");
   const size_t smem = (size_t)wg.stages * wg.stage_bytes;
@@ -1001,7 +990,7 @@ int dcn_backward_weight_tc(const float *input, const float *offset, const float 
   CNB_CHECK_LAUNCH("cnb_dcnv2_backward weight gradient reduce");
   count_launch(3);
   if (grad_bias) {
-    k_dcn_bwd_bias_reduce<<<cout, 256, 0, stream>>>(bpart, grad_bias, wg);
+    k_dcn_bwd_bias_reduce<<<s.Cout, 256, 0, stream>>>(bpart, grad_bias, wg);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward bias gradient reduce");
     count_launch();
   }

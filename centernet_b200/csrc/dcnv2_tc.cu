@@ -324,25 +324,17 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
   }
 }
 
-size_t dcn_tc_wtiles_bytes(int cin, int cout, int dg) {
-  DcnShapeTc s;
-  fill_shape(&s, 1, cin, 8, 8, cout, 3, 3, 1, 1, 1, 1, 1, 1, dg);
-  return align_up((size_t)s.n_cot * s.nb * TC_NT * 2 * s.co_t * TC_K * 4, 256);
-}
-static size_t tc_xt_bytes(const DcnShapeTc &s) { return align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * 4, 256); }
-static size_t tc_part_bytes(const DcnShapeTc &s) {
-  return s.splits > 1 ? align_up((size_t)s.splits * s.B * s.Cout * s.Ho * s.Wo * 4, 256) : 0;
-}
-
-// workspace of the prepared forward: channels-last copy of the input (+ split-K partial sums)
-size_t dcn_tc_fwd_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg) {
-  DcnShapeTc s;
-  fill_shape(&s, b, cin, h, w, cout, kh, kw, sh, sh, ph, ph, dh, dh, dg);
-  return tc_xt_bytes(s) + tc_part_bytes(s);
-}
-// workspace of the plain forward: weight tiles + the above
-size_t dcn_tc_workspace_bytes(int b, int cin, int h, int w, int cout, int kh, int kw, int sh, int ph, int dh, int dg) {
-  return dcn_tc_wtiles_bytes(cin, cout, dg) + dcn_tc_fwd_workspace_bytes(b, cin, h, w, cout, kh, kw, sh, ph, dh, dg);
+// Workspace of the prepared forward: channels-last copy of the input (+ split-K partial sums); the plain forward puts
+// the weight tiles in front of it
+void plan_forward_tc(DcnPlan *p) {
+  const DcnShapeTc &s = p->s;
+  p->xt_bytes = align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * 4, 256);
+  p->fwd.xt = 0;
+  p->fwd.part = p->fwd.xt + p->xt_bytes;
+  p->fwd.prepared_bytes = p->fwd.part;
+  if (s.splits > 1) p->fwd.prepared_bytes += align_up((size_t)s.splits * s.B * s.Cout * s.Ho * s.Wo * 4, 256);
+  p->fwd.wtiles_bytes = align_up((size_t)s.n_cot * s.nb * TC_NT * 2 * s.co_t * TC_K * 4, 256);
+  p->fwd.bytes = p->fwd.wtiles_bytes + p->fwd.prepared_bytes;
 }
 
 int dcn_prepare_weights_tc(const float *weight, int cin, int cout, int kh, int kw, int dg, float *wtiles,
@@ -384,28 +376,24 @@ static int launch_fwd(const float *xt, const float *offset, const float *mask, c
   return CNB_OK;
 }
 
-// Tensor-core forward from pre-tiled weights.  input_nhwc != 0: `input` already is [B][H*W][Cin] (torch
-// channels_last) and Cin/dg is a multiple of 32 -- no re-layout pass.  Requires kh*kw <= 9 (checked by the caller).
-int dcn_forward_tc_prepared(const float *input, int input_nhwc, const float *offset, const float *mask,
-                            const float *wtiles, const float *bias, float *output, int b, int cin, int h, int w,
-                            int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int dg,
-                            void *workspace, cudaStream_t stream, int fused_offset_mask, const float *epi_scale,
-                            const float *epi_shift, int relu) {
-  DcnShapeTc s;
-  fill_shape(&s, b, cin, h, w, cout, kh, kw, sh, sw, ph, pw, dh, dw, dg);
+// Tensor-core forward from pre-tiled weights.  p.x_cl: `input` already is [B][H*W][Cin] (torch channels_last) with
+// Cin/dg a multiple of 32 -- no re-layout pass.
+int dcn_forward_tc_prepared(const DcnPlan &p, const float *input, const float *offset, const float *mask,
+                            const float *wtiles, const float *bias, float *output, void *workspace, cudaStream_t stream,
+                            int fused_offset_mask, const float *epi_scale, const float *epi_shift, int relu) {
+  DcnShapeTc s = p.s;
   if (fused_offset_mask) {   // `offset` is the raw [b, 3*kt*dg, ho, wo] output of conv_offset_mask; mask = its last third
-    s.off_bs = s.mask_bs = (long long)dg * 3 * kh * kw * s.Ho * s.Wo;
+    s.off_bs = s.mask_bs = (long long)s.dg * 3 * s.kh * s.kw * s.Ho * s.Wo;
     s.mask_logit = 1;
-    mask = offset + (long long)dg * 2 * kh * kw * s.Ho * s.Wo;
+    mask = offset + (long long)s.dg * 2 * s.kh * s.kw * s.Ho * s.Wo;
   }
   s.epi_scale = epi_scale;
   s.epi_shift = epi_scale ? epi_shift : nullptr;
   s.relu = relu;
-  float *xt = reinterpret_cast<float *>(workspace);
-  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + tc_xt_bytes(s));
-  const long long HW = (long long)h * w;
+  float *xt = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.fwd.xt);
+  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.fwd.part);
   const float *xsrc = xt;
-  if (input_nhwc && (cin / dg) % TC_CB == 0) {
+  if (p.x_cl) {
     xsrc = input;
   } else {
     const int rc_t = dcn_to_channels_last(input, xt, s, stream);
@@ -416,26 +404,14 @@ int dcn_forward_tc_prepared(const float *input, int input_nhwc, const float *off
   else rc = launch_fwd<128, 2>(xsrc, offset, mask, wtiles, bias, output, part, s, stream);
   if (rc != CNB_OK) return rc;
   if (s.splits > 1) {
-    const long long total = (long long)b * cout * s.Ho * s.Wo;
+    const long long total = (long long)s.B * s.Cout * s.Ho * s.Wo;
     const int grid = (int)((total + 255) / 256 < 1184 ? (total + 255) / 256 : 1184);
-    k_dcn_reduce<<<grid, 256, 0, stream>>>(part, bias, output, s.splits, cout, (long long)s.Ho * s.Wo, total, s.epi_scale,
-                                           s.epi_shift, s.relu);
+    k_dcn_reduce<<<grid, 256, 0, stream>>>(part, bias, output, s.splits, s.Cout, (long long)s.Ho * s.Wo, total,
+                                           s.epi_scale, s.epi_shift, s.relu);
     CNB_CHECK_LAUNCH("cnb_dcnv2_forward split-K reduce");
     count_launch();
   }
   return CNB_OK;
-}
-
-// Plain forward: tiles the weights into the head of the workspace, then the prepared forward.
-int dcn_forward_tc(const float *input, const float *offset, const float *mask, const float *weight,
-                   const float *bias, float *output, int b, int cin, int h, int w, int cout, int kh, int kw, int sh,
-                   int sw, int ph, int pw, int dh, int dw, int dg, void *workspace, cudaStream_t stream) {
-  float *wt = reinterpret_cast<float *>(workspace);
-  int rc = dcn_prepare_weights_tc(weight, cin, cout, kh, kw, dg, wt, stream);
-  if (rc != CNB_OK) return rc;
-  return dcn_forward_tc_prepared(input, 0, offset, mask, wt, bias, output, b, cin, h, w, cout, kh, kw, sh, sw, ph, pw,
-                                 dh, dw, dg, reinterpret_cast<char *>(workspace) + dcn_tc_wtiles_bytes(cin, cout, dg),
-                                 stream, 0, nullptr, nullptr, 0);
 }
 
 }  // namespace cnb

@@ -152,7 +152,48 @@ inline void fill_shape(DcnShapeTc *s, int b, int cin, int h, int w, int cout, in
   s->epi_scale = s->epi_shift = nullptr;
 }
 
+// Host-side plan of one fp32 DCNv2 call or workspace query (dcn_plan in dcnv2.cu, after the one validation): the
+// shape, the path decisions and the byte offset of every workspace region.  Each size and offset is worked out once,
+// by plan_forward_tc and plan_backward_tc; the hosts of the kernels read their pointers from here.
+struct DcnPlan {
+  DcnShapeTc s;        // the validated shape and the tensor-core decomposition (fill_shape)
+  bool det;            // deterministic mode (cnb_dcnv2_set_deterministic), read once per call
+  bool fwd_tc;         // the tensor-core forward covers the shape: isotropic stride/pad/dilation
+  bool bwd_tc;         // so does the tensor-core backward: isotropic and within its 32-bit in-image indexing
+  bool dw_tc;          // and its weight pass: cout <= 256 (above, dW runs on the fp32 kernel)
+  bool x_cl, gx_cl;    // input / grad_input are channels-last [b][h*w][cin] (whole 32-channel blocks) and used as such
+  bool xt_ready;       // weight pass: the data pass already wrote the channels-last input copy on this stream
+  int fp32_dw_splits;  // pixel-range splits of the fp32 dW kernel
+  size_t xt_bytes;     // channels-last copy of the input [B][HW][nb][32], in both workspaces
+  struct {             // the prepared forward's workspace is [xt][part]; the plain forward's is [wtiles][that], so the
+                       // prepared one starts at wtiles_bytes there
+    size_t xt, part, prepared_bytes, wtiles_bytes, bytes;
+  } fwd;
+  struct {             // [xt][dxt][wtt][max(gyt + dcol of one batch chunk, gyk + wpart + bpart)]: the data and the
+                       // weight passes run one after the other on the stream and share the tail.  Deterministic mode
+                       // appends [bnd][dxi] or, at the same offset and for cout > 256, the fp32 dW partials wpart32
+    size_t xt, dxt, wtt, gyt, dcol, gyk, wpart, bpart, bnd, dxi, wpart32, bytes;
+    int chunk;         // images per pass of the data pass
+  } bwd;
+};
+void plan_forward_tc(DcnPlan *p);    // dcnv2_tc.cu: xt_bytes and fwd
+void plan_backward_tc(DcnPlan *p);   // dcnv2_bwd_tc.cu: bwd_tc, dw_tc and bwd (after plan_forward_tc)
+
 // x [B][Cin][HW] -> channels-last copy xt [B][HW][nb][32] (dcnv2_tc.cu)
 int dcn_to_channels_last(const float *x, float *xt, const DcnShapeTc &s, cudaStream_t stream);
+int dcn_prepare_weights_tc(const float *weight, int cin, int cout, int kh, int kw, int dg, float *wtiles,
+                           cudaStream_t stream);
+// Tensor-core forward from pre-tiled weights into the prepared forward's workspace (p.fwd).  fused_offset_mask:
+// `offset` is the raw conv_offset_mask output; epi_scale / epi_shift / relu: the folded BatchNorm + ReLU epilogue
+int dcn_forward_tc_prepared(const DcnPlan &p, const float *input, const float *offset, const float *mask,
+                            const float *wtiles, const float *bias, float *output, void *workspace, cudaStream_t stream,
+                            int fused_offset_mask, const float *epi_scale, const float *epi_shift, int relu);
+// Tensor-core backward (dcnv2_bwd_tc.cu) into the workspace of p.bwd: dX, dOffset, dMask; then dW and dBias
+int dcn_backward_data_tc(const DcnPlan &p, const float *input, const float *offset, const float *mask,
+                         const float *weight, const float *grad_output, float *grad_input, float *grad_offset,
+                         float *grad_mask, void *workspace, cudaStream_t stream);
+int dcn_backward_weight_tc(const DcnPlan &p, const float *input, const float *offset, const float *mask,
+                           const float *grad_output, float *grad_weight, float *grad_bias, void *workspace,
+                           cudaStream_t stream);
 
 }  // namespace cnb

@@ -178,14 +178,15 @@ class _DCNv2(Function):
         n, cin, h, wd = [int(v) for v in x.shape]
         cout, _, kh, kw = [int(v) for v in w.shape]
         # order-independent (fixed-point) grad_input when the user asked torch for deterministic algorithms (or
-        # CNB_DCN_DETERMINISTIC=1); the workspace query below then includes what that mode needs
+        # CNB_DCN_DETERMINISTIC=1); the workspace query, made after setting the mode, includes what that mode needs
         det = _deterministic()
-        if det and (_FORCE_FP32 or C.dcnv2_backward_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding,
-                                                                     dilation, dg) == 0):
+        C.dcnv2_set_deterministic(int(det))
+        wsb = 0 if _FORCE_FP32 else C.dcnv2_backward_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding,
+                                                                     dilation, dg)
+        if det and wsb == 0:
+            C.dcnv2_set_deterministic(0)    # the fp32 kernels run under warn_only; otherwise the alert raises
             _alert_not_deterministic("DCNv2 backward on the fp32 path (CNB_DCN_FP32=1, more than 9 taps or an image "
                                      "beyond the tensor-core kernels' 32-bit indexing)")
-            det = False                 # warn_only: run the fp32 kernels
-        C.dcnv2_set_deterministic(int(det))
         x_cl = ctx.x_cl and not _FORCE_FP32
         if ctx.x_cl and not x_cl:
             x = x.contiguous()          # the fp32 kernels work on NCHW
@@ -195,11 +196,7 @@ class _DCNv2(Function):
         gmsk = torch.zeros_like(msk)
         gw = torch.zeros_like(w)
         gb = torch.zeros_like(b) if b is not None else None
-        wsbuf, wsb = None, 0
-        if not _FORCE_FP32:
-            wsb = C.dcnv2_backward_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding, dilation, dg)
-            if wsb:
-                wsbuf = workspace(wsb, x.device)
+        wsbuf = workspace(wsb, x.device) if wsb else None
         if x_cl:
             C.dcnv2_backward_ex(ptr(x), 1, ptr(off), ptr(msk), ptr(w), ptr(go), ptr(gx), 1, ptr(goff), ptr(gmsk), ptr(gw),
                                 ptr(gb), n, cin, h, wd, cout, kh, kw, stride, padding, dilation, dg, ptr(wsbuf), wsb,

@@ -95,6 +95,12 @@ def test_dcnv2_backward_workspace_query_and_switches():
     assert q(2, 64, 64, 32, 32, 3, 3, 1, 1, 1, 3) == 0                  # cin not divisible by the groups
     assert q(1, 32, 32, 8192, 8192, 3, 3, 1, 1, 1, 1) == 0              # image too large for 32-bit in-image offsets
     assert q(2, 12, 5, 9, 11, 3, 3, 2, 1, 1, 2) > 0                     # ragged, strided, grouped: covered
+    # an empty output grid (2x2 image, 3x3 kernel, no padding) is rejected by every call, so every fp32 query returns 0
+    for det in (0, 1):
+        _C.dcnv2_set_deterministic(det)
+        for query in (q, _C.dcnv2_workspace_bytes, _C.dcnv2_prepared_workspace_bytes):
+            assert query(2, 64, 64, 2, 2, 3, 3, 1, 0, 1, 1) == 0
+    _C.dcnv2_set_deterministic(0)
     assert _C.dcnv2_get_deterministic() == 0
     _C.dcnv2_set_deterministic(1)
     assert _C.dcnv2_get_deterministic() == 1

@@ -39,6 +39,18 @@ def test_zero_offset_identity_kat():
     assert (out - x).abs().max().item() < 1e-6
 
 
+def test_empty_output_grid_raises():
+    """A 2x2 image under a 3x3 kernel without padding has no output pixel: the workspace queries return 0 for it and
+    the call is refused, so DCNv2Function raises RuntimeError."""
+    from centernet_b200.dcn_v2_func import DCNv2Function
+    x = torch.randn(2, 64, 2, 2, device="cuda")
+    off = torch.zeros(2, 18, 0, 0, device="cuda")
+    m = torch.zeros(2, 9, 0, 0, device="cuda")
+    w = torch.randn(64, 64, 3, 3, device="cuda")
+    with pytest.raises(RuntimeError):
+        DCNv2Function(1, 0, 1, 1)(x, off, m, w, torch.zeros(64, device="cuda"))
+
+
 SHAPES = [
     # B, Cin, H, W, Cout, dg, stride
     (2, 64, 32, 32, 64, 1, 1),     # dla_34 style 64->64
