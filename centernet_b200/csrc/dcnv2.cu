@@ -679,6 +679,83 @@ int cnb_dcnv2_forward_fused(const float *input, int input_channels_last, const f
                                  workspace, (cudaStream_t)stream_, 1, bn_scale, bn_shift, relu);
 }
 
+// ------------------------------------------------------------------ bf16 forward (opt-in; dcnv2_tc.cu)
+size_t cnb_dcnv2_wtiles_bf16_bytes(int cin, int cout, int kh, int kw, int dg) {
+  DcnPlan p;   // as cnb_dcnv2_wtiles_bytes: any image the kernel fits in will do
+  if (dcn_plan("cnb_dcnv2_wtiles_bf16_bytes", 1, cin, 8, 8, cout, kh, kw, 1, 1, 1, 1, 1, 1, dg, false, false, false,
+               &p) != CNB_OK)
+    return 0;
+  return p.bf16.wtiles_bytes;
+}
+
+int cnb_dcnv2_prepare_weights_bf16(const float *weight, int cin, int cout, int kh, int kw, int deformable_groups,
+                                   void *wtiles, size_t wtiles_bytes, void *stream) {
+  CNB_REQUIRE(weight && wtiles, CNB_EINVAL, "cnb_dcnv2_prepare_weights_bf16: null pointer");
+  CNB_REQUIRE(cin > 0 && cout > 0 && kh > 0 && kw > 0 && deformable_groups > 0 && cin % deformable_groups == 0,
+              CNB_EINVAL, "cnb_dcnv2_prepare_weights_bf16: bad shape");
+  CNB_REQUIRE(kh * kw <= DCN_KT_MAX, CNB_EUNSUPPORTED, "cnb_dcnv2_prepare_weights_bf16: more than %d taps", DCN_KT_MAX);
+  const size_t need = cnb_dcnv2_wtiles_bf16_bytes(cin, cout, kh, kw, deformable_groups);
+  CNB_REQUIRE(wtiles_bytes >= need, CNB_EWORKSPACE, "cnb_dcnv2_prepare_weights_bf16: buffer %zu < %zu", wtiles_bytes,
+              need);
+  CNB_REQUIRE((reinterpret_cast<uintptr_t>(wtiles) & 15u) == 0, CNB_EINVAL,
+              "cnb_dcnv2_prepare_weights_bf16: buffer must be 16-byte aligned");
+  return dcn_prepare_weights_bf16(weight, cin, cout, kh, kw, deformable_groups, wtiles, (cudaStream_t)stream);
+}
+
+size_t cnb_dcnv2_bf16_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw, int stride, int pad,
+                                      int dil, int dg) {
+  DcnPlan p;
+  if (dcn_plan("cnb_dcnv2_bf16_workspace_bytes", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg,
+               false, false, false, &p) != CNB_OK)
+    return 0;
+  return p.bf16.bytes;
+}
+
+// The checks of both bf16 entry points, in order: pointers, dtype codes, shape (dcn_plan), workspace, alignment.
+static int dcn_bf16_call(const char *fn, const void *input, int input_dtype, int input_channels_last,
+                         const float *offset, const float *mask, const void *wtiles, const float *bias,
+                         const float *bn_scale, const float *bn_shift, int relu, void *output, int output_dtype, int b,
+                         int cin, int h, int w, int cout, int kh, int kw, int stride, int pad, int dil, int dg,
+                         void *workspace, size_t workspace_bytes, void *stream, int fused) {
+  CNB_REQUIRE(input && offset && (mask || fused) && wtiles && output && workspace, CNB_EINVAL, "%s: null pointer", fn);
+  CNB_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), CNB_EINVAL, "%s: bn_scale and bn_shift go together", fn);
+  CNB_REQUIRE((input_dtype == CNB_DTYPE_F32 || input_dtype == CNB_DTYPE_BF16) &&
+                  (output_dtype == CNB_DTYPE_F32 || output_dtype == CNB_DTYPE_BF16),
+              CNB_EINVAL, "%s: unknown dtype code (input %d, output %d)", fn, input_dtype, output_dtype);
+  DcnPlan p;
+  int rc = dcn_plan(fn, b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg, false,
+                    input_channels_last != 0, false, &p);
+  if (rc != CNB_OK) return rc;
+  CNB_REQUIRE(workspace_bytes >= p.bf16.bytes, CNB_EWORKSPACE, "%s: workspace too small (%zu < %zu)", fn,
+              workspace_bytes, p.bf16.bytes);
+  CNB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15u) == 0 && (reinterpret_cast<uintptr_t>(wtiles) & 15u) == 0 &&
+                  (reinterpret_cast<uintptr_t>(input) & 15u) == 0,
+              CNB_EINVAL, "%s: buffers must be 16-byte aligned", fn);
+  return dcn_forward_bf16(p, input, input_dtype == CNB_DTYPE_BF16, offset, mask, wtiles, bias, output,
+                          output_dtype == CNB_DTYPE_BF16, workspace, (cudaStream_t)stream, fused, bn_scale, bn_shift,
+                          relu);
+}
+
+int cnb_dcnv2_forward_bf16(const void *input, int input_dtype, int input_channels_last, const float *offset,
+                           const float *mask, const void *wtiles, const float *bias, void *output, int output_dtype,
+                           int b, int cin, int h, int w, int cout, int kh, int kw, int stride, int pad, int dil,
+                           int deformable_groups, void *workspace, size_t workspace_bytes, void *stream) {
+  return dcn_bf16_call("cnb_dcnv2_forward_bf16", input, input_dtype, input_channels_last, offset, mask, wtiles, bias,
+                       nullptr, nullptr, 0, output, output_dtype, b, cin, h, w, cout, kh, kw, stride, pad, dil,
+                       deformable_groups, workspace, workspace_bytes, stream, 0);
+}
+
+int cnb_dcnv2_forward_fused_bf16(const void *input, int input_dtype, int input_channels_last,
+                                 const float *offset_mask, const void *wtiles, const float *bias,
+                                 const float *bn_scale, const float *bn_shift, int relu, void *output,
+                                 int output_dtype, int b, int cin, int h, int w, int cout, int kh, int kw, int stride,
+                                 int pad, int dil, int deformable_groups, void *workspace, size_t workspace_bytes,
+                                 void *stream) {
+  return dcn_bf16_call("cnb_dcnv2_forward_fused_bf16", input, input_dtype, input_channels_last, offset_mask, nullptr,
+                       wtiles, bias, bn_scale, bn_shift, relu, output, output_dtype, b, cin, h, w, cout, kh, kw,
+                       stride, pad, dil, deformable_groups, workspace, workspace_bytes, stream, 1);
+}
+
 int cnb_dcnv2_forward(const float *input, const float *offset, const float *mask, const float *weight,
                       const float *bias, float *output, int b, int cin, int h, int w, int cout, int kh, int kw,
                       int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int deformable_groups,

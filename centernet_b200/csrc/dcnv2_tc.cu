@@ -31,6 +31,10 @@
 // The weight tiles are pre-split / pre-tiled by k_dcn_prep_weights: once per call through the plain
 // cnb_dcnv2_forward, or once per weight version through cnb_dcnv2_prepare_weights +
 // cnb_dcnv2_forward_prepared (what the Python module does).
+//
+// k_dcn_forward_bf16 (further down) is the opt-in bf16 form of the forward: bf16 tiles, wgmma k16 bf16 -> fp32.
+#include <cuda_bf16.h>
+
 #include "dcnv2_tc.cuh"
 
 namespace cnb {
@@ -129,6 +133,42 @@ __device__ __forceinline__ ItemTc tc_item(const DcnShapeTc &s, int item) {
   return it;
 }
 
+// Bilinear geometry of every (tap, pixel) of item `it` in deformable group g, the mask folded into the corner weights
+// (dcn_v2_im2col_cuda.cu:18-47, :165); st = this thread's index among the sampler threads.  Shared by the fp32 and the
+// bf16 forward, so both sample at bit-identical fp32 weights.
+__device__ __forceinline__ void tc_build_meta(const DcnShapeTc &s, const float *__restrict__ offset,
+                                              const float *__restrict__ mask, const ItemTc &it, int g, int st,
+                                              int KT, long long HWo, TapMetaTc *meta) {
+  for (int idx = st; idx < TC_NT * TC_TP; idx += TC_SAMPLERS * 32) {
+    const int t = idx / TC_TP, pp = idx - t * TC_TP;
+    const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
+    TapMetaTc mt;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { mt.o[q] = 0; mt.w[q] = 0.f; }
+    if (ho < s.Ho && wo < s.Wo && t < KT) {
+      const long long p = (long long)ho * s.Wo + wo;
+      const int i = t / s.kw, j = t - i * s.kw;
+      const float *op = offset + (long long)it.b * s.off_bs + (long long)g * 2 * KT * HWo;
+      const float dy = __ldg(op + (2 * t) * HWo + p), dx = __ldg(op + (2 * t + 1) * HWo + p);
+      float m = __ldg(mask + (long long)it.b * s.mask_bs + ((long long)g * KT + t) * HWo + p);
+      if (s.mask_logit) m = 1.0f / (1.0f + expf(-m));        // torch.sigmoid(mask), dcn_v2.py:68
+      const float h_im = (float)(ho * s.sh - s.ph + i * s.dh) + dy;
+      const float w_im = (float)(wo * s.sw - s.pw + j * s.dw) + dx;
+      if (h_im > -1.f && w_im > -1.f && h_im < (float)s.H && w_im < (float)s.W) {   // dcn_v2_im2col_cuda.cu:165
+        const float hf = floorf(h_im), wf = floorf(w_im);
+        const int hl = (int)hf, wl = (int)wf;
+        const float lh = h_im - hf, lw = w_im - wf, hh = 1.f - lh, hw = 1.f - lw;
+        const int base = hl * s.W + wl;
+        if (hl >= 0 && wl >= 0) { mt.o[0] = base; mt.w[0] = hh * hw * m; }                       // :31-41
+        if (hl >= 0 && wl + 1 <= s.W - 1) { mt.o[1] = base + 1; mt.w[1] = hh * lw * m; }
+        if (hl + 1 <= s.H - 1 && wl >= 0) { mt.o[2] = base + s.W; mt.w[2] = lh * hw * m; }
+        if (hl + 1 <= s.H - 1 && wl + 1 <= s.W - 1) { mt.o[3] = base + s.W + 1; mt.w[3] = lh * lw * m; }
+      }
+    }
+    meta[idx] = mt;
+  }
+}
+
 template <int CO_T, int STAGES>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset, const float *__restrict__ mask,
@@ -170,34 +210,7 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
           // ---- bilinear geometry of every (tap, pixel) of this deformable group (mask folded into the weights)
           cur_g = g;
           named_bar_sync(1, TC_SAMPLERS * 32);   // everybody is done reading the previous geometry
-          for (int idx = st; idx < TC_NT * TC_TP; idx += TC_SAMPLERS * 32) {
-            const int t = idx / TC_TP, pp = idx - t * TC_TP;
-            const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
-            TapMetaTc mt;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) { mt.o[q] = 0; mt.w[q] = 0.f; }
-            if (ho < s.Ho && wo < s.Wo && t < KT) {
-              const long long p = (long long)ho * s.Wo + wo;
-              const int i = t / s.kw, j = t - i * s.kw;
-              const float *op = offset + (long long)it.b * s.off_bs + (long long)g * 2 * KT * HWo;
-              const float dy = __ldg(op + (2 * t) * HWo + p), dx = __ldg(op + (2 * t + 1) * HWo + p);
-              float m = __ldg(mask + (long long)it.b * s.mask_bs + ((long long)g * KT + t) * HWo + p);
-              if (s.mask_logit) m = 1.0f / (1.0f + expf(-m));        // torch.sigmoid(mask), dcn_v2.py:68
-              const float h_im = (float)(ho * s.sh - s.ph + i * s.dh) + dy;
-              const float w_im = (float)(wo * s.sw - s.pw + j * s.dw) + dx;
-              if (h_im > -1.f && w_im > -1.f && h_im < (float)s.H && w_im < (float)s.W) {   // dcn_v2_im2col_cuda.cu:165
-                const float hf = floorf(h_im), wf = floorf(w_im);
-                const int hl = (int)hf, wl = (int)wf;
-                const float lh = h_im - hf, lw = w_im - wf, hh = 1.f - lh, hw = 1.f - lw;
-                const int base = hl * s.W + wl;
-                if (hl >= 0 && wl >= 0) { mt.o[0] = base; mt.w[0] = hh * hw * m; }                       // :31-41
-                if (hl >= 0 && wl + 1 <= s.W - 1) { mt.o[1] = base + 1; mt.w[1] = hh * lw * m; }
-                if (hl + 1 <= s.H - 1 && wl >= 0) { mt.o[2] = base + s.W; mt.w[2] = lh * hw * m; }
-                if (hl + 1 <= s.H - 1 && wl + 1 <= s.W - 1) { mt.o[3] = base + s.W + 1; mt.w[3] = lh * lw * m; }
-              }
-            }
-            meta[idx] = mt;
-          }
+          tc_build_meta(s, offset, mask, it, g, st, KT, HWo, meta);
           named_bar_sync(1, TC_SAMPLERS * 32);
         }
         const float *xb = xbat + (long long)bi * TC_CB;
@@ -324,17 +337,382 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
   }
 }
 
+// =====================================================================================================================
+// bf16 forward: the same pipeline with one bf16 A tile and one bf16 B tile a chunk and wgmma k16 bf16 -> fp32.
+// Numeric contract (include/centernet_b200.h): the geometry and the 4-corner interpolation are the fp32 kernel's
+// (tc_build_meta, the same fmaf chain), the masked column value is rounded once to bf16 (RN); the weights were
+// rounded once (RN) by k_dcn_prep_weights_bf16; the contraction accumulates in fp32, split-K partials are added in
+// split order, bias / BN / ReLU are applied in fp32 and the result is stored as fp32 or rounded (RN) to bf16.
+
+__device__ __forceinline__ uint32_t bf_tile_off(int row, int k) {   // byte offset of (row, k) in a dense bf16 tile
+  return (uint32_t)(row >> 3) * BF_B_SBO + (uint32_t)(k >> 3) * BF_B_LBO + (uint32_t)(row & 7) * 16u +
+         (uint32_t)(k & 7) * 2u;
+}
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {   // lo -> lower address (smaller k)
+  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t *>(&v);
+}
+__device__ __forceinline__ void store_out(float *p, float v) { *p = v; }
+__device__ __forceinline__ void store_out(__nv_bfloat16 *p, float v) { *p = __float2bfloat16_rn(v); }
+__device__ __forceinline__ float load_in(const float *p) { return __ldg(p); }
+__device__ __forceinline__ float load_in(const __nv_bfloat16 *p) { return __bfloat162float(p[0]); }
+
+// W[Cout][Cin][KT] (fp32) -> per (cout tile, channel block, tap) one bf16 tile [co_t][32] (k = channel within the
+// block), the layout of bf_tile_off; tile index = (cot * nb + bi) * 9 + tap, as k_dcn_prep_weights
+__global__ void __launch_bounds__(256) k_dcn_prep_weights_bf16(const float *__restrict__ w, const DcnShapeTc s,
+                                                               unsigned char *__restrict__ ws) {
+  const int KT = s.kh * s.kw;
+  const int cpg = s.Cin / s.dg;
+  const int tile = blockIdx.x;
+  const int tap = tile % TC_NT, r = tile / TC_NT;
+  const int bi = r % s.nb, cot = r / s.nb;
+  const int g = bi / s.cbs_pg, cbi = bi - g * s.cbs_pg;
+  unsigned char *dst = ws + (size_t)tile * s.co_t * TC_K * 2;
+  for (int i = threadIdx.x; i < s.co_t * TC_K; i += blockDim.x) {
+    const int o = i / TC_K, k = i - o * TC_K;
+    const int cw = cbi * TC_CB + k;
+    const int oc = cot * s.co_t + o;
+    float v = 0.f;
+    if (oc < s.Cout && cw < cpg && tap < KT) v = w[((size_t)oc * s.Cin + g * cpg + cw) * KT + tap];
+    *reinterpret_cast<__nv_bfloat16 *>(dst + bf_tile_off(o, k)) = __float2bfloat16_rn(v);
+  }
+}
+
+// x [B][Cin][HW] (fp32 or bf16) -> bf16 xt [B][HW][nb][32], the slot mapping of k_dcn_nhwc
+template <typename T>
+__global__ void __launch_bounds__(256) k_dcn_nhwc_bf16(const T *__restrict__ x, __nv_bfloat16 *__restrict__ xt,
+                                                       const DcnShapeTc s) {
+  __shared__ float tile[64][33];
+  const long long HW = (long long)s.H * s.W;
+  const long long p0 = (long long)blockIdx.x * 32;
+  const int c0 = blockIdx.y * 64, b = blockIdx.z;
+  const int Cp = s.nb * TC_CB;
+  const int cpg = s.Cin / s.dg;
+  {
+    const int px = threadIdx.x & 31, cr = threadIdx.x >> 5;
+    for (int c = cr; c < 64; c += 8) {
+      float v = 0.f;
+      if (c0 + c < s.Cin && p0 + px < HW) v = load_in(x + ((long long)b * s.Cin + c0 + c) * HW + p0 + px);
+      tile[c][px] = v;
+    }
+  }
+  __syncthreads();
+  {
+    const int c = threadIdx.x & 63, pr = threadIdx.x >> 6;
+    const int ch = c0 + c;
+    if (ch < s.Cin) {
+      const int g = ch / cpg, within = ch - g * cpg;
+      const int slot = (g * s.cbs_pg + within / TC_CB) * TC_CB + within % TC_CB;
+      for (int px = pr; px < 32; px += 4)
+        if (p0 + px < HW) xt[((long long)b * HW + p0 + px) * Cp + slot] = __float2bfloat16_rn(tile[c][px]);
+    }
+  }
+}
+
+// fp32 channels-last [B][HW][Cin] with whole 32-channel blocks (so slot == channel) -> bf16 xt, 8 values a thread
+__global__ void __launch_bounds__(256) k_dcn_cl_to_bf16(const float4 *__restrict__ x, uint4 *__restrict__ xt,
+                                                        long long n8) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const float4 a = __ldg(x + 2 * i), b = __ldg(x + 2 * i + 1);
+    xt[i] = make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(b.x, b.y), pack_bf16x2(b.z, b.w));
+  }
+}
+
+// y[b][o][p] = epilogue(bias[o] + sum_s part[s][b][o][p]), s ascending, stored as bf16 (k_dcn_reduce writes fp32)
+__global__ void __launch_bounds__(256) k_dcn_reduce_bf16(const float *__restrict__ part, const float *__restrict__ bias,
+                                                         __nv_bfloat16 *__restrict__ y, int splits, int cout,
+                                                         long long hwo, long long total,
+                                                         const float *__restrict__ epi_scale,
+                                                         const float *__restrict__ epi_shift, int relu) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int o = (int)((i / hwo) % cout);
+    float v = 0.f;
+    for (int s = 0; s < splits; ++s) v += __ldg(part + (long long)s * total + i);
+    if (bias) v += __ldg(bias + o);
+    if (epi_scale) v = fmaf(v, __ldg(epi_scale + o), __ldg(epi_shift + o));
+    if (relu) v = fmaxf(v, 0.f);
+    y[i] = __float2bfloat16_rn(v);
+  }
+}
+
+// Warp roles, items and mbarrier hand-over as k_dcn_forward_tc.  Sampler warp item = one 8-row group of the A tile
+// (8 pixels): lane = pixel * 4 + k-chunk, every lane gathers the 4 corners of its pixel as 16-byte pieces (8 bf16
+// channels), interpolates in fp32 and stores one rounded 16-byte k-chunk; each warp fills two row groups a chunk, both
+// gathered before either is reduced.
+template <int CO_T, int STAGES, typename TOut>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict__ offset,
+                   const float *__restrict__ mask, const __nv_bfloat16 *__restrict__ wtiles,
+                   const float *__restrict__ bias, TOut *__restrict__ y, float *__restrict__ part, const DcnShapeTc s) {
+  extern __shared__ __align__(128) unsigned char tc_smem[];
+  constexpr int B_BYTES = CO_T * TC_K * 2;
+  constexpr int STAGE_BYTES = BF_A_BYTES + B_BYTES;
+  constexpr int ROWGROUPS = TC_TP / 8 / TC_SAMPLERS;   // 2 row groups a sampler warp
+  static_assert(ROWGROUPS == 2, "k_dcn_forward_bf16: two row groups a sampler warp");
+  TapMetaTc *meta = reinterpret_cast<TapMetaTc *>(tc_smem + (size_t)STAGES * STAGE_BYTES);     // [9][128]
+  __shared__ __align__(8) uint64_t a_full[STAGES], b_full[STAGES], empty[STAGES];
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int KT = s.kh * s.kw;
+  const long long HWo = (long long)s.Ho * s.Wo, HW = (long long)s.H * s.W;
+  const int Cp = s.nb * TC_CB;
+
+  if (tid == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&a_full[i], TC_SAMPLERS);
+      mbar_init(&b_full[i], 1);
+      mbar_init(&empty[i], TC_MMA_WGS);
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= TC_WARP_S0) {
+    // =========================================================== samplers: A operand of every chunk
+    const int sw = warp - TC_WARP_S0, st = tid - TC_WARP_S0 * 32;
+    const int sp = lane >> 2, sq = lane & 3;
+    const int rg0 = sw * ROWGROUPS, rg1 = rg0 + 1;
+    int stage = 0, ph = 0;
+    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
+      const ItemTc it = tc_item(s, item);
+      const __nv_bfloat16 *xbat = xt + (long long)it.b * HW * Cp + sq * 8;
+      int cur_g = -1;
+      for (int bi = it.b0; bi < it.b1; ++bi) {
+        const int g = bi / s.cbs_pg;
+        if (g != cur_g) {
+          cur_g = g;
+          named_bar_sync(1, TC_SAMPLERS * 32);   // everybody is done reading the previous geometry
+          tc_build_meta(s, offset, mask, it, g, st, KT, HWo, meta);
+          named_bar_sync(1, TC_SAMPLERS * 32);
+        }
+        const __nv_bfloat16 *xb = xbat + (long long)bi * TC_CB;
+        for (int tap = 0; tap < TC_NT; ++tap) {
+          const TapMetaTc m0 = meta[tap * TC_TP + rg0 * 8 + sp], m1 = meta[tap * TC_TP + rg1 * 8 + sp];
+          uint4 u0[4], u1[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) u0[q] = __ldg(reinterpret_cast<const uint4 *>(xb + (long long)m0.o[q] * Cp));
+#pragma unroll
+          for (int q = 0; q < 4; ++q) u1[q] = __ldg(reinterpret_cast<const uint4 *>(xb + (long long)m1.o[q] * Cp));
+          // fp32 value of channel 2e (lower half) / 2e + 1 (upper half) of a 4 x 32-bit piece: exact widening
+          auto reduce = [&](const TapMetaTc &mt, const uint4 (&u)[4]) {
+            uint32_t r[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              float v[2];
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float c[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                  const uint32_t word = e == 0 ? u[q].x : e == 1 ? u[q].y : e == 2 ? u[q].z : u[q].w;
+                  c[q] = __uint_as_float(h == 0 ? word << 16 : word & 0xffff0000u);
+                }
+                v[h] = fmaf(mt.w[3], c[3], fmaf(mt.w[2], c[2], fmaf(mt.w[1], c[1], mt.w[0] * c[0])));
+              }
+              r[e] = pack_bf16x2(v[0], v[1]);
+            }
+            return make_uint4(r[0], r[1], r[2], r[3]);
+          };
+          const uint4 v0 = reduce(m0, u0), v1 = reduce(m1, u1);
+          mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));   // drained by the MMAs that last read it
+          unsigned char *a = tc_smem + (size_t)stage * STAGE_BYTES;
+          const uint32_t off = (uint32_t)sq * BF_LBO + (uint32_t)sp * 16u;
+          *reinterpret_cast<uint4 *>(a + (uint32_t)rg0 * BF_SBO + off) = v0;
+          *reinterpret_cast<uint4 *>(a + (uint32_t)rg1 * BF_SBO + off) = v1;
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> async proxy (wgmma reads)
+          __syncwarp();
+          if (lane == 0) mbar_arrive_tc(&a_full[stage]);
+          if (++stage == STAGES) { stage = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else if (warp == TC_WARP_TMA) {
+    // =========================================================== B operand: one bf16 weight tile by TMA bulk copy
+    if (lane == 0) {
+      int stage = 0, ph = 0;
+      for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
+        const ItemTc it = tc_item(s, item);
+        for (int bi = it.b0; bi < it.b1; ++bi) {
+          for (int tap = 0; tap < TC_NT; ++tap) {
+            mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
+            unsigned char *b = tc_smem + (size_t)stage * STAGE_BYTES + BF_A_BYTES;
+            const __nv_bfloat16 *src = wtiles + (((size_t)it.cot * s.nb + bi) * TC_NT + tap) * (size_t)CO_T * TC_K;
+            mbar_expect_tx(&b_full[stage], (uint32_t)B_BYTES);
+            bulk_g2s(b, src, (uint32_t)B_BYTES, &b_full[stage]);
+            if (++stage == STAGES) { stage = 0; ph ^= 1; }
+          }
+        }
+      }
+    }
+  } else {
+    // =========================================================== consumers: wgmma over the ring, epilogue from registers
+    const int wgi = warp >> 2, wq = warp & 3;
+    int stage = 0, ph = 0;
+    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
+      const ItemTc it = tc_item(s, item);
+      float d[CO_T / 2];
+#pragma unroll
+      for (int i = 0; i < CO_T / 2; ++i) d[i] = 0.f;
+      const int n_ch = (it.b1 - it.b0) * TC_NT;
+      for (int ch = 0; ch < n_ch; ++ch) {
+        mbar_wait(&a_full[stage], (uint32_t)ph);
+        mbar_wait(&b_full[stage], (uint32_t)ph);
+        const uint32_t base = smem_u32(tc_smem + (size_t)stage * STAGE_BYTES);
+        const uint32_t a = base + (uint32_t)wgi * 8u * BF_SBO;   // this warpgroup's 64 rows
+        const uint32_t b = base + (uint32_t)BF_A_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < TC_K / 16; ++ks)   // one k16 step = two 16-byte k-chunks
+          wgmma_bf16<CO_T>(d, wg_desc(a + (uint32_t)ks * 2u * BF_LBO, BF_LBO, BF_SBO),
+                           wg_desc(b + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO, BF_B_SBO), (ch > 0 || ks > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        if ((tid & 127) == 0) mbar_arrive_tc(&empty[stage]);
+        if (++stage == STAGES) { stage = 0; ph ^= 1; }
+      }
+      // epilogue: the accumulator fragment of k_dcn_forward_tc; split-K partials stay fp32
+      const long long img = (long long)it.b * s.Cout * HWo;
+      float *pdst = s.splits > 1 ? part + (long long)it.split * s.B * s.Cout * HWo + img : nullptr;
+      TOut *ydst = y + img;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int pp = wgi * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
+        if (ho >= s.Ho || wo >= s.Wo) continue;
+        const long long p = (long long)ho * s.Wo + wo;
+#pragma unroll
+        for (int j = 0; j < CO_T / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int o = it.cot * CO_T + 8 * j + 2 * (lane & 3) + e;
+            if (o < s.Cout) {
+              float r = d[4 * j + 2 * h + e];
+              if (pdst) {
+                pdst[(long long)o * HWo + p] = r;
+              } else {
+                if (bias) r += __ldg(bias + o);
+                if (s.epi_scale) r = fmaf(r, __ldg(s.epi_scale + o), __ldg(s.epi_shift + o));
+                if (s.relu) r = fmaxf(r, 0.f);
+                store_out(ydst + (long long)o * HWo + p, r);
+              }
+            }
+          }
+        }
+      }
+    }
+  }
+}
+
+int dcn_prepare_weights_bf16(const float *weight, int cin, int cout, int kh, int kw, int dg, void *wtiles,
+                             cudaStream_t stream) {
+  DcnShapeTc s;
+  fill_shape(&s, 1, cin, 8, 8, cout, kh, kw, 1, 1, 1, 1, 1, 1, dg);
+  k_dcn_prep_weights_bf16<<<s.n_cot * s.nb * TC_NT, 256, 0, stream>>>(weight, s,
+                                                                       reinterpret_cast<unsigned char *>(wtiles));
+  CNB_CHECK_LAUNCH("cnb_dcnv2 bf16 weight tiles");
+  count_launch();
+  return CNB_OK;
+}
+
+template <int CO_T, typename TOut>
+static int launch_fwd_bf16(const __nv_bfloat16 *xt, const float *offset, const float *mask, const void *wtiles,
+                           const float *bias, void *output, float *part, const DcnShapeTc &s, cudaStream_t stream) {
+  constexpr int STAGES = BF_STAGES;
+  const size_t smem = (size_t)STAGES * (BF_A_BYTES + CO_T * TC_K * 2) + sizeof(TapMetaTc) * TC_NT * TC_TP;
+  static thread_local int dev_done = -1;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev_done != dev) {
+    CNB_CUDA(cudaFuncSetAttribute(k_dcn_forward_bf16<CO_T, STAGES, TOut>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
+    dev_done = dev;
+  }
+  const int grid = s.n_items < num_sms() ? s.n_items : num_sms();
+  k_dcn_forward_bf16<CO_T, STAGES, TOut><<<grid, TC_THREADS, smem, stream>>>(
+      xt, offset, mask, reinterpret_cast<const __nv_bfloat16 *>(wtiles), bias, reinterpret_cast<TOut *>(output), part,
+      s);
+  CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 (wgmma)");
+  count_launch();
+  return CNB_OK;
+}
+
+int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
+                     const void *wtiles, const float *bias, void *output, bool out_bf16, void *workspace,
+                     cudaStream_t stream, int fused_offset_mask, const float *epi_scale, const float *epi_shift,
+                     int relu) {
+  DcnShapeTc s = p.s;
+  if (fused_offset_mask) {   // `offset` is the raw [b, 3*kt*dg, ho, wo] output of conv_offset_mask; mask = its last third
+    s.off_bs = s.mask_bs = (long long)s.dg * 3 * s.kh * s.kw * s.Ho * s.Wo;
+    s.mask_logit = 1;
+    mask = offset + (long long)s.dg * 2 * s.kh * s.kw * s.Ho * s.Wo;
+  }
+  s.epi_scale = epi_scale;
+  s.epi_shift = epi_scale ? epi_shift : nullptr;
+  s.relu = relu;
+  __nv_bfloat16 *xt = reinterpret_cast<__nv_bfloat16 *>(reinterpret_cast<char *>(workspace) + p.bf16.xt);
+  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
+  const long long HW = (long long)s.H * s.W;
+  const __nv_bfloat16 *xsrc = xt;
+  if (p.x_cl && in_bf16) {
+    xsrc = reinterpret_cast<const __nv_bfloat16 *>(input);   // sampled in place
+  } else if (p.x_cl) {
+    const long long n8 = (long long)s.B * HW * s.Cin / 8;
+    const int grid = (int)((n8 + 255) / 256 < 4096 ? (n8 + 255) / 256 : 4096);
+    k_dcn_cl_to_bf16<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4 *>(input), reinterpret_cast<uint4 *>(xt), n8);
+    CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 bf16 copy");
+    count_launch();
+  } else {
+    if ((s.Cin / s.dg) % TC_CB != 0)   // pad slots of the last channel block of every group must read as zero
+      CNB_CUDA(cudaMemsetAsync(xt, 0, (size_t)s.B * HW * s.nb * TC_CB * 2, stream));
+    dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((s.Cin + 63) / 64), (unsigned)s.B);
+    if (in_bf16)
+      k_dcn_nhwc_bf16<__nv_bfloat16><<<tgrid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16 *>(input), xt, s);
+    else
+      k_dcn_nhwc_bf16<float><<<tgrid, 256, 0, stream>>>(reinterpret_cast<const float *>(input), xt, s);
+    CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 channels-last copy");
+    count_launch();
+  }
+  int rc;
+  if (s.co_t == 64)
+    rc = out_bf16 ? launch_fwd_bf16<64, __nv_bfloat16>(xsrc, offset, mask, wtiles, bias, output, part, s, stream)
+                  : launch_fwd_bf16<64, float>(xsrc, offset, mask, wtiles, bias, output, part, s, stream);
+  else
+    rc = out_bf16 ? launch_fwd_bf16<128, __nv_bfloat16>(xsrc, offset, mask, wtiles, bias, output, part, s, stream)
+                  : launch_fwd_bf16<128, float>(xsrc, offset, mask, wtiles, bias, output, part, s, stream);
+  if (rc != CNB_OK) return rc;
+  if (s.splits > 1) {
+    const long long total = (long long)s.B * s.Cout * s.Ho * s.Wo;
+    const int grid = (int)((total + 255) / 256 < 1184 ? (total + 255) / 256 : 1184);
+    if (out_bf16)
+      k_dcn_reduce_bf16<<<grid, 256, 0, stream>>>(part, bias, reinterpret_cast<__nv_bfloat16 *>(output), s.splits,
+                                                  s.Cout, (long long)s.Ho * s.Wo, total, s.epi_scale, s.epi_shift,
+                                                  s.relu);
+    else
+      k_dcn_reduce<<<grid, 256, 0, stream>>>(part, bias, reinterpret_cast<float *>(output), s.splits, s.Cout,
+                                             (long long)s.Ho * s.Wo, total, s.epi_scale, s.epi_shift, s.relu);
+    CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 split-K reduce");
+    count_launch();
+  }
+  return CNB_OK;
+}
+
 // Workspace of the prepared forward: channels-last copy of the input (+ split-K partial sums); the plain forward puts
-// the weight tiles in front of it
+// the weight tiles in front of it.  The bf16 forward's workspace has the same regions with a bf16 copy.
 void plan_forward_tc(DcnPlan *p) {
   const DcnShapeTc &s = p->s;
+  const size_t part_bytes = s.splits > 1 ? align_up((size_t)s.splits * s.B * s.Cout * s.Ho * s.Wo * 4, 256) : 0;
   p->xt_bytes = align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * 4, 256);
   p->fwd.xt = 0;
   p->fwd.part = p->fwd.xt + p->xt_bytes;
-  p->fwd.prepared_bytes = p->fwd.part;
-  if (s.splits > 1) p->fwd.prepared_bytes += align_up((size_t)s.splits * s.B * s.Cout * s.Ho * s.Wo * 4, 256);
+  p->fwd.prepared_bytes = p->fwd.part + part_bytes;
   p->fwd.wtiles_bytes = align_up((size_t)s.n_cot * s.nb * TC_NT * 2 * s.co_t * TC_K * 4, 256);
   p->fwd.bytes = p->fwd.wtiles_bytes + p->fwd.prepared_bytes;
+  p->bf16.xt = 0;
+  p->bf16.xt_bytes = align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * 2, 256);
+  p->bf16.part = p->bf16.xt + p->bf16.xt_bytes;
+  p->bf16.bytes = p->bf16.part + part_bytes;
+  p->bf16.wtiles_bytes = align_up((size_t)s.n_cot * s.nb * TC_NT * s.co_t * TC_K * 2, 256);
 }
 
 int dcn_prepare_weights_tc(const float *weight, int cin, int cout, int kh, int kw, int dg, float *wtiles,

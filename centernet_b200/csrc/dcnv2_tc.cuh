@@ -25,6 +25,16 @@ constexpr uint32_t FW_LBO = 144;                    // bytes between consecutive
 constexpr uint32_t FW_SBO = TC_KC * FW_LBO;         // bytes between 8-row groups (1152)
 constexpr int FW_A_BYTES = (TC_TP / 8) * FW_SBO;    // 18432 per hi / lo tile
 
+// bf16 forward (k_dcn_forward_bf16): a 32-channel block is a 64-byte line of the bf16 channels-last copy and one row
+// of a tile is four 16-byte k-chunks (8 channels each).  A tile: k-chunks pitched 160 bytes, so the eight 16-byte
+// stores of a quarter-warp (2 rows x 4 k-chunks) land in eight different bank groups (DESIGN 4.4).  B tile: dense.
+constexpr uint32_t BF_LBO = 160;                    // A: bytes between consecutive k-chunks (8 rows x 16 B + 32 B)
+constexpr uint32_t BF_SBO = 4 * BF_LBO;             // A: bytes between 8-row groups (640)
+constexpr int BF_A_BYTES = (TC_TP / 8) * BF_SBO;    // 10240
+constexpr uint32_t BF_B_LBO = 128;                  // B: bytes between consecutive k-chunks
+constexpr uint32_t BF_B_SBO = 4 * BF_B_LBO;         // B: bytes between 8-row groups (512)
+constexpr int BF_STAGES = 4;                        // ring depth: (10240 + 64 * co_t) bytes a stage
+
 struct DcnShapeTc {
   int B, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, Ho, Wo;
   int co_t;       // output channels per item (64 or 128)
@@ -111,6 +121,45 @@ __device__ __forceinline__ void wgmma_3xtf32(float (&d)[N / 2], uint64_t dah, ui
   wgmma_tf32<N>(d, dah, dbl, 1u);
   wgmma_tf32<N>(d, dah, dbh, 1u);
 }
+// bf16 operands, fp32 accumulate: D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, both K-major (imm-trans-a/b = 0); the
+// accumulator fragment is the one of the TF32 form above
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
+      "%26,%27,%28,%29,%30,%31}"
+      ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
+      "%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,"
+      "%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+      ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  static_assert(N == 64 || N == 128, "wgmma_bf16: N is 64 or 128");
+  if constexpr (N == 64) wgmma_bf16_n64(d, da, db, scale_d);
+  else wgmma_bf16_n128(d, da, db, scale_d);
+}
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 __device__ __forceinline__ void mbar_arrive_tc(uint64_t *bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -169,6 +218,10 @@ struct DcnPlan {
                        // prepared one starts at wtiles_bytes there
     size_t xt, part, prepared_bytes, wtiles_bytes, bytes;
   } fwd;
+  struct {             // the bf16 forward's workspace is [xt: bf16 channels-last copy][part: fp32 split-K partials];
+                       // its weight tiles (one bf16 tile a chunk) live in a buffer of their own
+    size_t xt, xt_bytes, part, bytes, wtiles_bytes;
+  } bf16;
   struct {             // [xt][dxt][wtt][max(gyt + dcol of one batch chunk, gyk + wpart + bpart)]: the data and the
                        // weight passes run one after the other on the stream and share the tail.  Deterministic mode
                        // appends [bnd][dxi] or, at the same offset and for cout > 256, the fp32 dW partials wpart32
@@ -176,7 +229,7 @@ struct DcnPlan {
     int chunk;         // images per pass of the data pass
   } bwd;
 };
-void plan_forward_tc(DcnPlan *p);    // dcnv2_tc.cu: xt_bytes and fwd
+void plan_forward_tc(DcnPlan *p);    // dcnv2_tc.cu: xt_bytes, fwd and bf16
 void plan_backward_tc(DcnPlan *p);   // dcnv2_bwd_tc.cu: bwd_tc, dw_tc and bwd (after plan_forward_tc)
 
 // x [B][Cin][HW] -> channels-last copy xt [B][HW][nb][32] (dcnv2_tc.cu)
@@ -188,6 +241,15 @@ int dcn_prepare_weights_tc(const float *weight, int cin, int cout, int kh, int k
 int dcn_forward_tc_prepared(const DcnPlan &p, const float *input, const float *offset, const float *mask,
                             const float *wtiles, const float *bias, float *output, void *workspace, cudaStream_t stream,
                             int fused_offset_mask, const float *epi_scale, const float *epi_shift, int relu);
+// bf16 forward (dcnv2_tc.cu): bf16 weight tiles of one chunk each, [co_t][32] K-major, from an fp32 weight (RN)
+int dcn_prepare_weights_bf16(const float *weight, int cin, int cout, int kh, int kw, int dg, void *wtiles,
+                             cudaStream_t stream);
+// bf16 forward into the workspace of p.bf16.  in_bf16 / out_bf16: input / output are bf16 (else fp32); p.x_cl: the
+// input is channels-last and read in place when it is bf16 (an fp32 one is rounded into p.bf16.xt by a flat pass)
+int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
+                     const void *wtiles, const float *bias, void *output, bool out_bf16, void *workspace,
+                     cudaStream_t stream, int fused_offset_mask, const float *epi_scale, const float *epi_shift,
+                     int relu);
 // Tensor-core backward (dcnv2_bwd_tc.cu) into the workspace of p.bwd: dX, dOffset, dMask; then dW and dBias
 int dcn_backward_data_tc(const DcnPlan &p, const float *input, const float *offset, const float *mask,
                          const float *weight, const float *grad_output, float *grad_input, float *grad_offset,

@@ -267,6 +267,34 @@ PYBIND11_MODULE(_C, m) {
                                   wsb, ptr<void>(stream)),
           "cnb_dcnv2_forward_fused");
   });
+  m.attr("DTYPE_F32") = CNB_DTYPE_F32;
+  m.attr("DTYPE_BF16") = CNB_DTYPE_BF16;
+  m.def("dcnv2_wtiles_bf16_bytes", &cnb_dcnv2_wtiles_bf16_bytes);
+  m.def("dcnv2_prepare_weights_bf16", [](P weight, int cin, int cout, int kh, int kw, int dg, P wt, size_t wtb,
+                                         P stream) {
+    check(cnb_dcnv2_prepare_weights_bf16(ptr<const float>(weight), cin, cout, kh, kw, dg, ptr<void>(wt), wtb,
+                                         ptr<void>(stream)),
+          "cnb_dcnv2_prepare_weights_bf16");
+  });
+  m.def("dcnv2_bf16_workspace_bytes", &cnb_dcnv2_bf16_workspace_bytes);
+  m.def("dcnv2_forward_bf16", [](P input, int in_dt, int nhwc, P offset, P mask, P wt, P bias, P output, int out_dt,
+                                 int b, int cin, int h, int w, int cout, int kh, int kw, int stride, int pad, int dil,
+                                 int dg, P ws, size_t wsb, P stream) {
+    check(cnb_dcnv2_forward_bf16(ptr<const void>(input), in_dt, nhwc, ptr<const float>(offset),
+                                 ptr<const float>(mask), ptr<const void>(wt), ptr<const float>(bias), ptr<void>(output),
+                                 out_dt, b, cin, h, w, cout, kh, kw, stride, pad, dil, dg, ptr<void>(ws), wsb,
+                                 ptr<void>(stream)),
+          "cnb_dcnv2_forward_bf16");
+  });
+  m.def("dcnv2_forward_fused_bf16", [](P input, int in_dt, int nhwc, P om, P wt, P bias, P sc, P sh_, int relu,
+                                       P output, int out_dt, int b, int cin, int h, int w, int cout, int kh, int kw,
+                                       int stride, int pad, int dil, int dg, P ws, size_t wsb, P stream) {
+    check(cnb_dcnv2_forward_fused_bf16(ptr<const void>(input), in_dt, nhwc, ptr<const float>(om), ptr<const void>(wt),
+                                       ptr<const float>(bias), ptr<const float>(sc), ptr<const float>(sh_), relu,
+                                       ptr<void>(output), out_dt, b, cin, h, w, cout, kh, kw, stride, pad, dil, dg,
+                                       ptr<void>(ws), wsb, ptr<void>(stream)),
+          "cnb_dcnv2_forward_fused_bf16");
+  });
   m.def("dcnv2_backward", [](P input, P offset, P mask, P weight, P gout, P gin, P goff, P gmask, P gw, P gb, int b,
                              int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh,
                              int dw, int dg, P ws, size_t wsb, P stream) {

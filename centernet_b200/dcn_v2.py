@@ -7,14 +7,16 @@ import torch
 from torch import nn
 from torch.nn.modules.utils import _pair
 
-from .dcn_v2_func import DCNv2Function, DCNv2PoolingFunction, dcn_fused_inference
+from .dcn_v2_func import DCNv2Function, DCNv2PoolingFunction, _check_compute_dtype, dcn_fused_inference
 
 
 class DCNv2(nn.Module):
-    """dcn_v2.py:14-41."""
+    """dcn_v2.py:14-41.  compute_dtype=torch.bfloat16 opts this module into the bf16 forward (DCNv2Function)."""
 
-    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1):
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1,
+                 compute_dtype=None):
         super().__init__()
+        self.compute_dtype = _check_compute_dtype(compute_dtype)
         self.in_channels = in_channels
         self.out_channels = out_channels
         self.kernel_size = _pair(kernel_size)
@@ -35,15 +37,18 @@ class DCNv2(nn.Module):
         self.bias.data.zero_()
 
     def forward(self, input, offset, mask):
-        func = DCNv2Function(self.stride, self.padding, self.dilation, self.deformable_groups)
+        func = DCNv2Function(self.stride, self.padding, self.dilation, self.deformable_groups,
+                             getattr(self, "compute_dtype", None))
         return func(input, offset, mask, self.weight, self.bias)
 
 
 class DCN(DCNv2):
     """dcn_v2.py:44-70: DCNv2 + the zero-initialised offset/mask conv."""
 
-    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1):
-        super().__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, deformable_groups)
+    def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1,
+                 compute_dtype=None):
+        super().__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, deformable_groups,
+                         compute_dtype)
         self.conv_offset_mask = nn.Conv2d(self.in_channels,
                                           self.deformable_groups * 3 * self.kernel_size[0] * self.kernel_size[1],
                                           kernel_size=self.kernel_size, stride=(self.stride, self.stride),
@@ -61,11 +66,13 @@ class DCN(DCNv2):
                 input.dtype != torch.float64:
             # inference: chunk / cat / sigmoid (the three lines below) run inside the DCN kernel's sampler
             return dcn_fused_inference(input, out, self.weight, self.bias, self.stride, self.padding, self.dilation,
-                                       self.deformable_groups)
+                                       self.deformable_groups,
+                                       compute_dtype=getattr(self, "compute_dtype", None))
         o1, o2, mask = torch.chunk(out, 3, dim=1)
         offset = torch.cat((o1, o2), dim=1)
         mask = torch.sigmoid(mask)
-        func = DCNv2Function(self.stride, self.padding, self.dilation, self.deformable_groups)
+        func = DCNv2Function(self.stride, self.padding, self.dilation, self.deformable_groups,
+                             getattr(self, "compute_dtype", None))
         return func(input, offset, mask, self.weight, self.bias)
 
 
@@ -153,8 +160,23 @@ def fuse_dcn_bn_relu(model):
             scale, shift = fold_bn(bn)
             om = c.conv_offset_mask(x)
             return dcn_fused_inference(x, om, c.weight, c.bias, c.stride, c.padding, c.dilation, c.deformable_groups,
-                                       bn_scale=scale, bn_shift=shift, relu=True)
+                                       bn_scale=scale, bn_shift=shift, relu=True,
+                                       compute_dtype=getattr(c, "compute_dtype", None))
 
         m.forward = fused
         n += 1
+    return n
+
+
+def set_compute_dtype(model, dtype):
+    """Sets `compute_dtype` on every DCNv2 / DCN module of `model` (None: the default fp32-accurate forward;
+    torch.bfloat16: the bf16 forward) and returns how many it set.  The reference network code builds DCN(...)
+    without keywords; this turns the bf16 path on for such a model without touching its code.  Composes with
+    fuse_dcn_bn_relu in either order (the fused forward reads the attribute at call time)."""
+    _check_compute_dtype(dtype)
+    n = 0
+    for m in model.modules():
+        if isinstance(m, DCNv2):
+            m.compute_dtype = dtype
+            n += 1
     return n

@@ -56,25 +56,30 @@ def _out_hw(h, w, kh, kw, stride, padding, dilation):
     return ho, wo
 
 
-_WT_CACHE = {}      # id(weight) -> (weakref to it, its version when tiled, tiles); evicted when the tensor dies
+_WT_CACHE = {}      # (id(weight), bf16) -> (weakref to it, its version when tiled, tiles); evicted when the tensor dies
 
 
-def _weight_tiles(weight, dg):
-    """TF32 hi/lo weight tiles in the wgmma K-major layout (cnb_dcnv2_prepare_weights), rebuilt only when the parameter
-    changes: torch bumps `_version` on every in-place update (optimizer step, load_state_dict), and the entry
-    is tied to the tensor OBJECT by a weak reference, so a new tensor that happens to reuse the address never
-    sees stale tiles."""
+def _weight_tiles(weight, dg, bf16=False):
+    """TF32 hi/lo weight tiles in the wgmma K-major layout (cnb_dcnv2_prepare_weights), or with bf16=True the bf16
+    tiles of the bf16 forward (cnb_dcnv2_prepare_weights_bf16), rebuilt only when the parameter changes: torch bumps
+    `_version` on every in-place update (optimizer step, load_state_dict), and the entry is tied to the tensor OBJECT
+    by a weak reference, so a new tensor that happens to reuse the address never sees stale tiles.  The two kinds of
+    tiles of one parameter are cached side by side.  bf16 tiles are cached for a weight of any dtype (a bf16 model's
+    parameters are bf16; the tiles are built from its fp32 upcast, which is exact)."""
     w = f32c(weight)
     cout, cin, kh, kw = [int(v) for v in w.shape]
-    own = w is weight or w.data_ptr() == weight.data_ptr()
-    key = id(weight)
+    own = bf16 or w is weight or w.data_ptr() == weight.data_ptr()
+    key = (id(weight), bool(bf16))
     ver = weight._version
     hit = _WT_CACHE.get(key) if own else None
     if hit is not None and hit[0]() is weight and hit[1] == ver and hit[2].device == w.device:
         return hit[2]
-    nbytes = C.dcnv2_wtiles_bytes(cin, cout, kh, kw, dg)
-    wt = workspace(nbytes, w.device)
-    C.dcnv2_prepare_weights(ptr(w), cin, cout, kh, kw, dg, ptr(wt), wt.numel(), stream_ptr(w))
+    if bf16:
+        wt = workspace(C.dcnv2_wtiles_bf16_bytes(cin, cout, kh, kw, dg), w.device)
+        C.dcnv2_prepare_weights_bf16(ptr(w), cin, cout, kh, kw, dg, ptr(wt), wt.numel(), stream_ptr(w))
+    else:
+        wt = workspace(C.dcnv2_wtiles_bytes(cin, cout, kh, kw, dg), w.device)
+        C.dcnv2_prepare_weights(ptr(w), cin, cout, kh, kw, dg, ptr(wt), wt.numel(), stream_ptr(w))
     if own:
         try:
             _WT_CACHE[key] = (weakref.ref(weight, lambda _r, k=key: _WT_CACHE.pop(k, None)), ver, wt)
@@ -173,47 +178,138 @@ class _DCNv2(Function):
         if ctx.f64:
             return _dcn_backward_f64(ctx, grad_output)
         x, off, msk, w, b = ctx.saved_tensors
-        stride, padding, dilation, dg = ctx.cfg
-        go = f32c(grad_output)
-        n, cin, h, wd = [int(v) for v in x.shape]
-        cout, _, kh, kw = [int(v) for v in w.shape]
-        # order-independent (fixed-point) grad_input when the user asked torch for deterministic algorithms (or
-        # CNB_DCN_DETERMINISTIC=1); the workspace query, made after setting the mode, includes what that mode needs
-        det = _deterministic()
-        C.dcnv2_set_deterministic(int(det))
-        wsb = 0 if _FORCE_FP32 else C.dcnv2_backward_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding,
-                                                                     dilation, dg)
-        if det and wsb == 0:
-            C.dcnv2_set_deterministic(0)    # the fp32 kernels run under warn_only; otherwise the alert raises
-            _alert_not_deterministic("DCNv2 backward on the fp32 path (CNB_DCN_FP32=1, more than 9 taps or an image "
-                                     "beyond the tensor-core kernels' 32-bit indexing)")
-        x_cl = ctx.x_cl and not _FORCE_FP32
-        if ctx.x_cl and not x_cl:
-            x = x.contiguous()          # the fp32 kernels work on NCHW
-        # zero-filled, accumulated into -- dcn_v2_func.py:44-48 (zeros_like keeps a channels_last input's layout)
-        gx = torch.zeros_like(x)
-        goff = torch.zeros_like(off)
-        gmsk = torch.zeros_like(msk)
-        gw = torch.zeros_like(w)
-        gb = torch.zeros_like(b) if b is not None else None
-        wsbuf = workspace(wsb, x.device) if wsb else None
-        if x_cl:
-            C.dcnv2_backward_ex(ptr(x), 1, ptr(off), ptr(msk), ptr(w), ptr(go), ptr(gx), 1, ptr(goff), ptr(gmsk), ptr(gw),
-                                ptr(gb), n, cin, h, wd, cout, kh, kw, stride, padding, dilation, dg, ptr(wsbuf), wsb,
-                                stream_ptr(x))
-        else:
-            C.dcnv2_backward(ptr(x), ptr(off), ptr(msk), ptr(w), ptr(go), ptr(gx), ptr(goff), ptr(gmsk), ptr(gw), ptr(gb),
-                             n, cin, h, wd, cout, kh, kw, stride, stride, padding, padding, dilation, dilation, dg,
-                             ptr(wsbuf) if wsbuf is not None else 0, wsb, stream_ptr(x))
-        return gx, goff, gmsk, gw, gb, None, None, None, None
+        return _dcn_backward_f32(x, off, msk, w, b, f32c(grad_output), ctx.cfg, ctx.x_cl) + (None,) * 4
+
+
+def _dcn_backward_f32(x, off, msk, w, b, go, cfg, x_cl):
+    """The fp32 backward (tensor cores when the workspace query allows, else the fp32 kernels): gradients of input,
+    offset, mask, weight and bias, all fp32.  x_cl: x is a channels_last input the tensor-core backward reads as is."""
+    stride, padding, dilation, dg = cfg
+    n, cin, h, wd = [int(v) for v in x.shape]
+    cout, _, kh, kw = [int(v) for v in w.shape]
+    # order-independent (fixed-point) grad_input when the user asked torch for deterministic algorithms (or
+    # CNB_DCN_DETERMINISTIC=1); the workspace query, made after setting the mode, includes what that mode needs
+    det = _deterministic()
+    C.dcnv2_set_deterministic(int(det))
+    wsb = 0 if _FORCE_FP32 else C.dcnv2_backward_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding,
+                                                                 dilation, dg)
+    if det and wsb == 0:
+        C.dcnv2_set_deterministic(0)    # the fp32 kernels run under warn_only; otherwise the alert raises
+        _alert_not_deterministic("DCNv2 backward on the fp32 path (CNB_DCN_FP32=1, more than 9 taps or an image "
+                                 "beyond the tensor-core kernels' 32-bit indexing)")
+    use_cl = x_cl and not _FORCE_FP32
+    if x_cl and not use_cl:
+        x = x.contiguous()          # the fp32 kernels work on NCHW
+    # zero-filled, accumulated into -- dcn_v2_func.py:44-48 (zeros_like keeps a channels_last input's layout)
+    gx = torch.zeros_like(x)
+    goff = torch.zeros_like(off)
+    gmsk = torch.zeros_like(msk)
+    gw = torch.zeros_like(w)
+    gb = torch.zeros_like(b) if b is not None else None
+    wsbuf = workspace(wsb, x.device) if wsb else None
+    if use_cl:
+        C.dcnv2_backward_ex(ptr(x), 1, ptr(off), ptr(msk), ptr(w), ptr(go), ptr(gx), 1, ptr(goff), ptr(gmsk), ptr(gw),
+                            ptr(gb), n, cin, h, wd, cout, kh, kw, stride, padding, dilation, dg, ptr(wsbuf), wsb,
+                            stream_ptr(x))
+    else:
+        C.dcnv2_backward(ptr(x), ptr(off), ptr(msk), ptr(w), ptr(go), ptr(gx), ptr(goff), ptr(gmsk), ptr(gw), ptr(gb),
+                         n, cin, h, wd, cout, kh, kw, stride, stride, padding, padding, dilation, dilation, dg,
+                         ptr(wsbuf) if wsbuf is not None else 0, wsb, stream_ptr(x))
+    return gx, goff, gmsk, gw, gb
+
+
+# ------------------------------------------------------------------ bf16 forward (opt-in: compute_dtype=torch.bfloat16)
+def _check_compute_dtype(compute_dtype):
+    if compute_dtype is not None and compute_dtype != torch.bfloat16:
+        raise ValueError("compute_dtype must be None (fp32-accurate contraction) or torch.bfloat16, got %r"
+                         % (compute_dtype,))
+    return compute_dtype
+
+
+def _bf16_forward(what, input, offset, mask, offset_mask, weight, bias, stride, padding, dilation, dg,
+                  bn_scale=None, bn_shift=None, relu=False):
+    """One call of cnb_dcnv2_forward_bf16 (or, with offset_mask, cnb_dcnv2_forward_fused_bf16).  The output has the
+    input's dtype.  A channels_last input with whole 32-channel blocks is read as it is (a bf16 one in place)."""
+    if not input.is_cuda:
+        raise NotImplementedError
+    if input.dtype not in (torch.float32, torch.bfloat16):
+        raise RuntimeError("%s: compute_dtype=torch.bfloat16 takes a float32 or bfloat16 input, got %s"
+                           % (what, input.dtype))
+    n, cin, h, wd = [int(v) for v in input.shape]
+    cout, cin_w, kh, kw = [int(v) for v in weight.shape]
+    if cin_w != cin:
+        raise RuntimeError("Input shape and kernel channels wont match: (%d vs %d)." % (cin, cin_w))
+    if kh * kw > 9:
+        raise NotImplementedError("%s: compute_dtype=torch.bfloat16 runs at most 9 taps" % what)
+    ho, wo = _out_hw(h, wd, kh, kw, stride, padding, dilation)
+    kt = kh * kw
+    if offset_mask is not None:
+        om = f32c(offset_mask)
+        if tuple(om.shape) != (n, 3 * kt * dg, ho, wo):
+            raise RuntimeError("%s: offset_mask must be [%d, %d, %d, %d]" % (what, n, 3 * kt * dg, ho, wo))
+    else:
+        off, msk = f32c(offset), f32c(mask)
+        if tuple(off.shape) != (n, 2 * kt * dg, ho, wo) or tuple(msk.shape) != (n, kt * dg, ho, wo):
+            raise RuntimeError("DCNv2: offset/mask shape does not match the output grid")
+    cl = (cin // dg) % 32 == 0 and input.is_contiguous(memory_format=torch.channels_last) and \
+        not input.is_contiguous()
+    x = input if cl else input.contiguous()
+    if x.data_ptr() % 16:
+        x = x.clone()               # the kernels read 16-byte pieces (clone keeps the memory format)
+    dt = C.DTYPE_BF16 if x.dtype == torch.bfloat16 else C.DTYPE_F32
+    wt = _weight_tiles(weight, dg, bf16=True)
+    out = torch.empty((n, cout, ho, wo), dtype=input.dtype, device=input.device)
+    ws = workspace(C.dcnv2_bf16_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding, dilation, dg),
+                   input.device)
+    b = f32c(bias)
+    if offset_mask is not None:
+        sc, sh = f32c(bn_scale), f32c(bn_shift)
+        C.dcnv2_forward_fused_bf16(ptr(x), dt, int(cl), ptr(om), ptr(wt), ptr(b), ptr(sc), ptr(sh), int(bool(relu)),
+                                   ptr(out), dt, n, cin, h, wd, cout, kh, kw, stride, padding, dilation, dg, ptr(ws),
+                                   ws.numel(), stream_ptr(om))
+        return out, None, None
+    C.dcnv2_forward_bf16(ptr(x), dt, int(cl), ptr(off), ptr(msk), ptr(wt), ptr(b), ptr(out), dt, n, cin, h, wd, cout,
+                         kh, kw, stride, padding, dilation, dg, ptr(ws), ws.numel(), stream_ptr(off))
+    return out, off, msk
+
+
+class _DCNv2BF16(Function):
+    """bf16 forward; the backward is the fp32 one evaluated at the operands the forward used (the bf16 activation and
+    weight, upcast exactly), each gradient returned in its input's dtype.  The activation is saved as bf16."""
+
+    @staticmethod
+    def forward(ctx, input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups):
+        out, off, msk = _bf16_forward("DCNv2", input, offset, mask, None, weight, bias, stride, padding, dilation,
+                                      deformable_groups)
+        if any(ctx.needs_input_grad[:5]):
+            xb = input if input.dtype == torch.bfloat16 else input.bfloat16()
+            ctx.save_for_backward(xb, off, msk, weight, bias)
+        ctx.dtypes = tuple(None if t is None else t.dtype for t in (input, offset, mask, weight, bias))
+        ctx.cfg = (stride, padding, dilation, deformable_groups)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        if not grad_output.is_cuda:
+            raise NotImplementedError
+        xb, off, msk, weight, bias = ctx.saved_tensors
+        x = xb.float().contiguous()
+        w = weight.bfloat16().float().contiguous()
+        grads = _dcn_backward_f32(x, off, msk, w, f32c(bias), f32c(grad_output), ctx.cfg, False)
+        grads = tuple(None if g is None else g.to(dt) for g, dt in zip(grads, ctx.dtypes))
+        return grads + (None,) * 4
 
 
 def dcn_fused_inference(input, offset_mask, weight, bias, stride, padding, dilation, deformable_groups,
-                        bn_scale=None, bn_shift=None, relu=False):
+                        bn_scale=None, bn_shift=None, relu=False, compute_dtype=None):
     """Inference form of the whole DCN module around ONE kernel (cnb_dcnv2_forward_fused): `offset_mask` is the raw
     conv_offset_mask output (chunk / cat / sigmoid of dcn_v2.py:64-70 happen inside the sampler), bn_scale /
     bn_shift / relu the folded BatchNorm + ReLU that follow the DCN in DeformConv (pose_dla_dcn.py:345-357).
+    compute_dtype=torch.bfloat16: the bf16 forward (cnb_dcnv2_forward_fused_bf16), output in the input's dtype.
     No autograd (use DCNv2Function for training)."""
+    if _check_compute_dtype(compute_dtype) is not None:
+        return _bf16_forward("dcn_fused_inference", input, None, None, offset_mask, weight, bias, stride, padding,
+                             dilation, deformable_groups, bn_scale, bn_shift, relu)[0]
     if not input.is_cuda:
         raise NotImplementedError
     if input.dtype == torch.float64:
@@ -244,17 +340,20 @@ def dcn_fused_inference(input, offset_mask, weight, bias, stride, padding, dilat
 
 
 class DCNv2Function(object):
-    """Callable instance, same constructor as the reference's old-style Function."""
+    """Callable instance, same constructor as the reference's old-style Function.  compute_dtype=torch.bfloat16
+    selects the bf16 forward (float32 or bfloat16 input, output in the input's dtype); None keeps the default."""
 
-    def __init__(self, stride, padding, dilation=1, deformable_groups=1):
+    def __init__(self, stride, padding, dilation=1, deformable_groups=1, compute_dtype=None):
         self.stride = stride
         self.padding = padding
         self.dilation = dilation
         self.deformable_groups = deformable_groups
+        self.compute_dtype = _check_compute_dtype(compute_dtype)
 
     def __call__(self, input, offset, mask, weight, bias):
-        return _DCNv2.apply(input, offset, mask, weight, bias, self.stride, self.padding, self.dilation,
-                            self.deformable_groups)
+        fn = _DCNv2BF16 if self.compute_dtype is not None else _DCNv2
+        return fn.apply(input, offset, mask, weight, bias, self.stride, self.padding, self.dilation,
+                        self.deformable_groups)
 
     forward = __call__
 

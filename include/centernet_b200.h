@@ -41,6 +41,10 @@ extern "C" {
 #define CNB_ECUDA 3        /* CUDA runtime / launch error                        */
 #define CNB_EWORKSPACE 4   /* workspace_bytes smaller than cnb_*_workspace_bytes */
 
+/* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16). */
+#define CNB_DTYPE_F32 0
+#define CNB_DTYPE_BF16 1
+
 /* Library version (major*10000 + minor*100 + patch). */
 int cnb_version(void);
 /* Thread-local text of the last error returned on this thread ("" if none). */
@@ -252,6 +256,45 @@ int cnb_dcnv2_forward_fused(const float *input, int input_channels_last, const f
                             int b, int cin, int h, int w, int cout, int kh, int kw,
                             int stride, int pad, int dil, int deformable_groups,
                             void *workspace, size_t workspace_bytes, void *stream);
+/* bf16 forward (opt-in): bf16 operands on the bf16 tensor cores (wgmma k16), fp32 accumulate.
+ * Numeric contract:
+ *   - activations: a bf16 input is used as it is; an fp32 input is rounded to bf16 (RN) first, so it gives the
+ *     result of the same values in bf16;
+ *   - geometry: offsets, mask, bilinear weights and the 4-corner interpolation in fp32 with the expressions of the
+ *     fp32 kernels (the (-1,H)x(-1,W) test, per-corner zeroing); the interpolated, masked column value is rounded
+ *     once to bf16 (RN);
+ *   - weights: rounded once to bf16 (RN) by cnb_dcnv2_prepare_weights_bf16 (fp32 weight in), into a buffer of
+ *     cnb_dcnv2_wtiles_bf16_bytes (16-byte aligned) that is reused while the weight does not change;
+ *   - contraction in fp32 (wgmma ... .f32.bf16.bf16); split-K partials (small maps) are added in a fixed order;
+ *     bias, bn_scale / bn_shift and relu in fp32; the output is stored as output_dtype (bf16: RN);
+ *   - bit-identical run to run (no atomics).
+ * input: [b,cin,h,w] of input_dtype (CNB_DTYPE_F32 or CNB_DTYPE_BF16); input_channels_last != 0 says it is
+ * [b][h*w][cin] (torch channels_last): a bf16 one is sampled in place, an fp32 one rounded by one flat pass; needs
+ * cin/dg % 32 == 0, else the flag is ignored and input must be NCHW (one re-layout pass).  offset / mask (or the
+ * fused form's offset_mask) and bias / bn_scale / bn_shift are fp32; output [b,cout,ho,wo] NCHW of output_dtype.
+ * At most 9 taps, one stride / pad / dilation for both axes.  workspace: cnb_dcnv2_bf16_workspace_bytes (16-byte
+ * aligned; a bf16 channels-last copy of the input and, on small maps, the fp32 split-K partials); it returns 0 for
+ * every shape the calls reject.  Errors, checked before any CUDA call: CNB_EINVAL for a null pointer, an unknown
+ * dtype code, a bad shape or a buffer that is not 16-byte aligned; CNB_EWORKSPACE for too small a workspace;
+ * CNB_EUNSUPPORTED for more than 9 taps.  cnb_dcnv2_forward_fused_bf16 is cnb_dcnv2_forward_fused in this mode. */
+size_t cnb_dcnv2_wtiles_bf16_bytes(int cin, int cout, int kh, int kw, int dg);
+int cnb_dcnv2_prepare_weights_bf16(const float *weight, int cin, int cout, int kh, int kw,
+                                   int deformable_groups, void *wtiles, size_t wtiles_bytes, void *stream);
+size_t cnb_dcnv2_bf16_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw,
+                                      int stride, int pad, int dil, int dg);
+int cnb_dcnv2_forward_bf16(const void *input, int input_dtype, int input_channels_last,
+                           const float *offset, const float *mask, const void *wtiles, const float *bias,
+                           void *output, int output_dtype,
+                           int b, int cin, int h, int w, int cout, int kh, int kw,
+                           int stride, int pad, int dil, int deformable_groups,
+                           void *workspace, size_t workspace_bytes, void *stream);
+int cnb_dcnv2_forward_fused_bf16(const void *input, int input_dtype, int input_channels_last,
+                                 const float *offset_mask, const void *wtiles, const float *bias,
+                                 const float *bn_scale, const float *bn_shift, int relu,
+                                 void *output, int output_dtype,
+                                 int b, int cin, int h, int w, int cout, int kh, int kw,
+                                 int stride, int pad, int dil, int deformable_groups,
+                                 void *workspace, size_t workspace_bytes, void *stream);
 size_t cnb_dcnv2_backward_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw,
                                           int stride, int pad, int dil, int dg);
 /* The backward for a channels-last pipeline (torch channels_last): input_channels_last / grad_input_channels_last
