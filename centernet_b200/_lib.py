@@ -89,6 +89,24 @@ def f32c(t):
     return t.contiguous()
 
 
+# Element types the decode kernels read in place (CNB_DTYPE_* of include/centernet_b200.h).
+_DTYPE_CODES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+
+
+def floatc(t):
+    """Contiguous view of t, kept in its dtype when that is fp32, fp16 or bf16, else its fp32 upcast."""
+    if t is None:
+        return None
+    if t.dtype not in _DTYPE_CODES:
+        t = t.float()
+    return t.contiguous()
+
+
+def dtype_code(t):
+    """CNB_DTYPE_* code of a tensor made by floatc (None counts as fp32)."""
+    return 0 if t is None else _DTYPE_CODES[t.dtype]
+
+
 def ptr(t):
     return 0 if t is None else t.data_ptr()
 

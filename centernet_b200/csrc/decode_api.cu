@@ -155,12 +155,42 @@ static RawTopk carve_raw(char *p, long long n) {
 
 using namespace cnb;
 
-// out = 1 / (1 + exp(-x)), the expression of torch's CUDA sigmoid (4 elements per thread)
-__global__ void __launch_bounds__(256) k_sigmoid(const float *__restrict__ x, float *__restrict__ out, long long n) {
+// out = 1 / (1 + exp(-x)), the expression of torch's CUDA sigmoid (4 elements per thread); a 16-bit x is widened
+// to fp32 first, exactly
+template <typename T>
+__global__ void __launch_bounds__(256) k_sigmoid(const T *__restrict__ x, float *__restrict__ out, long long n) {
   const long long i0 = ((long long)blockIdx.x * 256 + threadIdx.x) * 4;
 #pragma unroll
   for (int j = 0; j < 4; ++j)
-    if (i0 + j < n) out[i0 + j] = 1.0f / (1.0f + expf(-x[i0 + j]));
+    if (i0 + j < n) out[i0 + j] = 1.0f / (1.0f + expf(-to_f32(x[i0 + j])));
+}
+
+// out = x widened to fp32 (what torch's .float() gives), 4 elements per thread
+template <typename T>
+__global__ void __launch_bounds__(256) k_widen(const T *__restrict__ x, float *__restrict__ out, long long n) {
+  const long long i0 = ((long long)blockIdx.x * 256 + threadIdx.x) * 4;
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    if (i0 + j < n) out[i0 + j] = to_f32(x[i0 + j]);
+}
+
+static bool dtype_known(int dt) { return dt == CNB_DTYPE_F32 || dt == CNB_DTYPE_F16 || dt == CNB_DTYPE_BF16; }
+static int dtype_bytes(int dt) { return dt == CNB_DTYPE_F32 ? 4 : 2; }
+
+// fp32 heat map (sigmoid of the logits, or the widened map) of a 16-bit or fp32 src, n elements
+static int launch_to_f32(const void *src, int dt, bool sigmoid, float *out, long long n, cudaStream_t stream) {
+  const unsigned grid = (unsigned)((n + 1023) / 1024);
+  if (sigmoid) {
+    if (dt == CNB_DTYPE_BF16) k_sigmoid<<<grid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16 *>(src), out, n);
+    else if (dt == CNB_DTYPE_F16) k_sigmoid<<<grid, 256, 0, stream>>>(reinterpret_cast<const __half *>(src), out, n);
+    else k_sigmoid<<<grid, 256, 0, stream>>>(reinterpret_cast<const float *>(src), out, n);
+  } else {
+    if (dt == CNB_DTYPE_BF16) k_widen<<<grid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16 *>(src), out, n);
+    else k_widen<<<grid, 256, 0, stream>>>(reinterpret_cast<const __half *>(src), out, n);
+  }
+  CNB_CHECK_LAUNCH(sigmoid ? "cnb_ctdet_decode_ex sigmoid" : "cnb_ctdet_decode_ex widen");
+  count_launch();
+  return CNB_OK;
 }
 
 // Flip-test merge (detectors/ctdet.py:34-37, detectors/multi_pose.py:43-51): src [2n, c, h, w] holds the heads
@@ -169,7 +199,8 @@ __global__ void __launch_bounds__(256) k_sigmoid(const float *__restrict__ x, fl
 // perm / sign (nullable) express flip_lr (joint swap, models/utils.py:33-39) and flip_lr_off (joint swap + negated
 // x offsets, :41-50); null = flip_tensor (:28-29).  One pass instead of the reference's sigmoid_, slices, host
 // round trip through numpy, add and divide.
-__global__ void __launch_bounds__(256) k_flip_merge(const float *__restrict__ src, float *__restrict__ dst, int n, int c,
+template <typename T>
+__global__ void __launch_bounds__(256) k_flip_merge(const T *__restrict__ src, float *__restrict__ dst, int n, int c,
                                                     int h, int w, int mode, const int *__restrict__ perm,
                                                     const float *__restrict__ sign) {
   const long long total = (long long)n * c * h * w;
@@ -181,8 +212,8 @@ __global__ void __launch_bounds__(256) k_flip_merge(const float *__restrict__ sr
     r /= h;
     const int ch = (int)(r % c), img = (int)(r / c);
     const int pc = perm ? perm[ch] : ch;
-    float a = src[i];
-    float b = src[(((long long)(n + img) * c + pc) * h + y) * w + (w - 1 - x)];
+    float a = to_f32(src[i]);
+    float b = to_f32(src[(((long long)(n + img) * c + pc) * h + y) * w + (w - 1 - x)]);
     if (mode == 1) {
       a = 1.0f / (1.0f + expf(-a));
       b = 1.0f / (1.0f + expf(-b));
@@ -202,6 +233,27 @@ int cnb_flip_merge(const float *src, float *dst, int n, int c, int h, int w, int
   const int grid = (int)((total + 255) / 256 < 4736 ? (total + 255) / 256 : 4736);
   k_flip_merge<<<grid, 256, 0, (cudaStream_t)stream>>>(src, dst, n, c, h, w, apply_sigmoid ? 1 : 0, perm, sign);
   CNB_CHECK_LAUNCH("cnb_flip_merge");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_flip_merge_ex(const void *src, int src_dtype, float *dst, int n, int c, int h, int w, int apply_sigmoid,
+                      const int32_t *perm, const float *sign, void *stream) {
+  CNB_REQUIRE(dtype_known(src_dtype), CNB_EINVAL, "cnb_flip_merge_ex: unknown dtype code %d", src_dtype);
+  if (src_dtype == CNB_DTYPE_F32)
+    return cnb_flip_merge(reinterpret_cast<const float *>(src), dst, n, c, h, w, apply_sigmoid, perm, sign, stream);
+  CNB_REQUIRE(src && dst, CNB_EINVAL, "cnb_flip_merge_ex: null pointer");
+  CNB_REQUIRE(n > 0 && c > 0 && h > 0 && w > 0, CNB_EINVAL, "cnb_flip_merge_ex: non-positive dimension");
+  const long long total = (long long)n * c * h * w;
+  const int grid = (int)((total + 255) / 256 < 4736 ? (total + 255) / 256 : 4736);
+  const int mode = apply_sigmoid ? 1 : 0;
+  if (src_dtype == CNB_DTYPE_BF16)
+    k_flip_merge<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16 *>(src), dst, n, c, h,
+                                                         w, mode, perm, sign);
+  else
+    k_flip_merge<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half *>(src), dst, n, c, h, w, mode,
+                                                         perm, sign);
+  CNB_CHECK_LAUNCH("cnb_flip_merge_ex");
   count_launch();
   return CNB_OK;
 }
@@ -325,6 +377,52 @@ int cnb_ctdet_decode_logits(const float *hm_logits, const float *wh, const float
   rc = make_select_plan(heat, b, c, h, w, k, 1, &pl);
   if (rc != CNB_OK) return rc;
   return run_select(heat, pl, out, workspace, (cudaStream_t)stream);
+}
+
+/* fp32, fp16 or bf16 heads (see the header): the hot geometry reads a 16-bit map in the selection kernel itself;
+ * other geometries widen it (or take its sigmoid) into the workspace, after the selection scratch, and run the fp32
+ * path.  Layout: [selection scratch | fp32 heat map], the map at the fp32 query's size (logits == 0) or at the
+ * aligned selection scratch of the plan (logits != 0, as cnb_ctdet_decode_logits). */
+size_t cnb_ctdet_decode_ex_workspace_bytes(const void *heat, int heat_dtype, int logits, int b, int c, int h, int w,
+                                           int k) {
+  if (!dtype_known(heat_dtype)) return 0;
+  SelectPlan pl;
+  if (make_select_plan(heat, b, c, h, w, k, 1, &pl, dtype_bytes(heat_dtype)) != CNB_OK) return 0;
+  const size_t map = align_up((size_t)b * c * h * w * 4, 256);
+  if (logits) return pl.hot ? select_workspace_bytes(pl) : align_up(select_workspace_bytes(pl), 256) + map;
+  const size_t base = cnb_topk_workspace_bytes(b, c, h, w, k);
+  return (heat_dtype == CNB_DTYPE_F32 || pl.hot) ? base : base + map;
+}
+
+int cnb_ctdet_decode_ex(const void *heat, int heat_dtype, int logits, const void *wh, int wh_dtype, const void *reg,
+                        int reg_dtype, int cat_spec_wh, int b, int c, int h, int w, int k, float *dets,
+                        void *workspace, size_t workspace_bytes, void *stream) {
+  CNB_REQUIRE(dtype_known(heat_dtype) && dtype_known(wh_dtype) && dtype_known(reg_dtype), CNB_EINVAL,
+              "cnb_ctdet_decode_ex: unknown dtype code (heat %d, wh %d, reg %d)", heat_dtype, wh_dtype, reg_dtype);
+  CNB_REQUIRE(heat && wh && dets && workspace, CNB_EINVAL, "cnb_ctdet_decode_ex: null pointer");
+  SelectPlan pl;
+  int rc = make_select_plan(heat, b, c, h, w, k, 1, &pl, dtype_bytes(heat_dtype));
+  if (rc != CNB_OK) return rc;
+  const size_t need = cnb_ctdet_decode_ex_workspace_bytes(heat, heat_dtype, logits, b, c, h, w, k);
+  CNB_REQUIRE(workspace_bytes >= need, CNB_EWORKSPACE, "cnb_ctdet_decode_ex: workspace %zu < %zu", workspace_bytes,
+              need);
+  FinalizeOut out = {nullptr, nullptr, nullptr, nullptr, nullptr, wh, reg, cat_spec_wh, dets, wh_dtype, reg_dtype};
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (pl.hot) {
+    pl.logits = logits ? 1 : 0;
+    return run_select(heat, pl, out, workspace, st, heat_dtype);
+  }
+  if (!logits && heat_dtype == CNB_DTYPE_F32) return run_select(heat, pl, out, workspace, st);
+  const size_t off = logits ? align_up(select_workspace_bytes(pl), 256) : cnb_topk_workspace_bytes(b, c, h, w, k);
+  float *heat32 = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + off);
+  SelectPlan pf;
+  rc = make_select_plan(heat32, b, c, h, w, k, 1, &pf);
+  if (rc != CNB_OK) return rc;
+  CNB_REQUIRE(select_workspace_bytes(pf) <= off, CNB_EWORKSPACE, "cnb_ctdet_decode_ex: selection scratch %zu > %zu",
+              select_workspace_bytes(pf), off);
+  rc = launch_to_f32(heat, heat_dtype, logits != 0, heat32, (long long)b * c * h * w, st);
+  if (rc != CNB_OK) return rc;
+  return run_select(heat32, pf, out, workspace, st);
 }
 
 int cnb_sigmoid(const float *x, float *out, long long n, void *stream) {

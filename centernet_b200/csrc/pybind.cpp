@@ -76,6 +76,20 @@ PYBIND11_MODULE(_C, m) {
                                   k, ptr<float>(dets), ptr<void>(ws), wsb, ptr<void>(stream)),
           "cnb_ctdet_decode_logits");
   });
+  m.def("ctdet_decode_ex_workspace_bytes", [](P heat, int dt, int logits, int b, int c, int h, int w, int k) {
+    return cnb_ctdet_decode_ex_workspace_bytes(ptr<const void>(heat), dt, logits, b, c, h, w, k);
+  });
+  m.def("ctdet_decode_ex", [](P heat, int heat_dt, int logits, P wh, int wh_dt, P reg, int reg_dt, int cat, int b,
+                              int c, int h, int w, int k, P dets, P ws, size_t wsb, P stream) {
+    check(cnb_ctdet_decode_ex(ptr<const void>(heat), heat_dt, logits, ptr<const void>(wh), wh_dt, ptr<const void>(reg),
+                              reg_dt, cat, b, c, h, w, k, ptr<float>(dets), ptr<void>(ws), wsb, ptr<void>(stream)),
+          "cnb_ctdet_decode_ex");
+  });
+  m.def("flip_merge_ex", [](P src, int dt, P dst, int n, int c, int h, int w, int sig, P perm, P sign, P stream) {
+    check(cnb_flip_merge_ex(ptr<const void>(src), dt, ptr<float>(dst), n, c, h, w, sig, ptr<const int32_t>(perm),
+                            ptr<const float>(sign), ptr<void>(stream)),
+          "cnb_flip_merge_ex");
+  });
   m.def("sigmoid", [](P x, P out, long long n, P stream) {
     check(cnb_sigmoid(ptr<const float>(x), ptr<float>(out), n, ptr<void>(stream)), "cnb_sigmoid");
   });
@@ -269,6 +283,7 @@ PYBIND11_MODULE(_C, m) {
   });
   m.attr("DTYPE_F32") = CNB_DTYPE_F32;
   m.attr("DTYPE_BF16") = CNB_DTYPE_BF16;
+  m.attr("DTYPE_F16") = CNB_DTYPE_F16;
   m.def("dcnv2_wtiles_bf16_bytes", &cnb_dcnv2_wtiles_bf16_bytes);
   m.def("dcnv2_prepare_weights_bf16", [](P weight, int cin, int cout, int kh, int kw, int dg, P wt, size_t wtb,
                                          P stream) {

@@ -25,6 +25,10 @@
 //
 // Non-positive scores (zero fillers, negative peaks) only matter when an image has < K
 // positive peaks; finalize handles that exactly with an ordered rescan (rare slow path).
+//
+// The hot kernel also reads fp16 / bf16 maps (k_select_hot<__half | __nv_bfloat16, LOGITS>): 32 KiB planes in the
+// same 3-deep ring, each element widened exactly to fp32 in registers, so the result is bit for bit that of the
+// .float() upcast (DESIGN 4.1).  Other stage-1 kernels read fp32 only.
 #include "select.cuh"
 #include <stdlib.h>
 
@@ -236,16 +240,16 @@ __device__ __forceinline__ float collide_margin(float M) {
 }
 
 // ------------------------------------------------------------------ finalize (shared by both paths)
-// v'(i): the reference's heat*keep value of flat pixel i (keep only in NMS mode).
-template <bool NMS>
-__device__ __forceinline__ float nms_value(const float *__restrict__ img, int C, int H, int W, long long i,
+// v'(i): the reference's heat*keep value of flat pixel i (keep only in NMS mode); T = map element type.
+template <bool NMS, typename T>
+__device__ __forceinline__ float nms_value(const T *__restrict__ img, int C, int H, int W, long long i,
                                            bool logits = false) {
-  const float v = img[i];
+  const float v = to_f32(img[i]);
   if (!NMS) return logits ? sigmoid_ref(v) : v;
   const long long HW = (long long)H * W;
   const long long c = i / HW, sp = i - c * HW;
   const int y = (int)(sp / W), x = (int)(sp - (long long)y * W);
-  const float *pl = img + c * HW;
+  const T *pl = img + c * HW;
   float m = v;
   for (int dy = -1; dy <= 1; ++dy) {
     const int yy = y + dy;
@@ -253,7 +257,7 @@ __device__ __forceinline__ float nms_value(const float *__restrict__ img, int C,
     for (int dx = -1; dx <= 1; ++dx) {
       const int xx = x + dx;
       if (xx < 0 || xx >= W) continue;
-      m = fmaxf(m, pl[(long long)yy * W + xx]);
+      m = fmaxf(m, to_f32(pl[(long long)yy * W + xx]));
     }
   }
   if (logits) {  // monotone sigmoid: max of the heat neighbourhood == sigmoid(max of the logits)
@@ -263,8 +267,8 @@ __device__ __forceinline__ float nms_value(const float *__restrict__ img, int C,
   return (m == v) ? v : 0.0f;
 }
 
-template <bool NMS, typename G>
-__device__ void finalize_fill(const float *__restrict__ img, const SelectPlan &pl, u64 *sbuf, int have, int K,
+template <bool NMS, typename G, typename T>
+__device__ void finalize_fill(const T *__restrict__ img, const SelectPlan &pl, u64 *sbuf, int have, int K,
                               int *s_tmp, u64 *s_red) {
   // Need K-have more entries ranked (value desc, index asc) among NON-positive v'.
   const int tid = G::tid(), lane = tid & 31, warp = tid >> 5, nw = G::n() >> 5;
@@ -325,6 +329,12 @@ __device__ void finalize_fill(const float *__restrict__ img, const SelectPlan &p
 // Row k of image b from its key (raw top-K outputs and/or the fused ctdet epilogue, models/decode.py:472-493).
 // The four gathered values (reg x, reg y, wh w, wh h) may come pre-loaded (gath != nullptr).
 struct RowGather { float rx, ry, ww, wh_; };
+// Element i of a head of dtype code dt, widened (K rows per image: a runtime switch, no template instances).
+__device__ __forceinline__ float ld_head(const void *p, int dt, size_t i) {
+  if (dt == CNB_DTYPE_BF16) return __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16 *>(p) + i));
+  if (dt == CNB_DTYPE_F16) return __half2float(__ldg(reinterpret_cast<const __half *>(p) + i));
+  return __ldg(reinterpret_cast<const float *>(p) + i);
+}
 __device__ __forceinline__ RowGather gather_row(const SelectPlan &pl, int b, u64 key, const FinalizeOut &out) {
   RowGather g = {0.5f, 0.5f, 0.f, 0.f};
   if (!out.dets) return g;
@@ -333,14 +343,14 @@ __device__ __forceinline__ RowGather gather_row(const SelectPlan &pl, int b, u64
   const int cls = (int)(flat / (uint32_t)HW);
   const int sp = (int)(flat - (uint32_t)cls * (uint32_t)HW);
   if (out.reg) {  // decode.py:472-476
-    const float *r = out.reg + (size_t)b * 2 * HW;
-    g.rx = __ldg(r + sp);
-    g.ry = __ldg(r + HW + sp);
+    const size_t r = (size_t)b * 2 * HW + sp;
+    g.rx = ld_head(out.reg, out.reg_dtype, r);
+    g.ry = ld_head(out.reg, out.reg_dtype, r + HW);
   }
   const int whc = out.cat_spec_wh ? 2 * pl.C : 2;  // :480-486
-  const float *wp = out.wh + ((size_t)b * whc + (out.cat_spec_wh ? 2 * cls : 0)) * HW;
-  g.ww = __ldg(wp + sp);
-  g.wh_ = __ldg(wp + HW + sp);
+  const size_t wp = ((size_t)b * whc + (out.cat_spec_wh ? 2 * cls : 0)) * HW + sp;
+  g.ww = ld_head(out.wh, out.wh_dtype, wp);
+  g.wh_ = ld_head(out.wh, out.wh_dtype, wp + HW);
   return g;
 }
 __device__ __forceinline__ void emit_one(const SelectPlan &pl, int b, int k, u64 key, const FinalizeOut &out,
@@ -832,7 +842,8 @@ enum { SW_BOTH = 0, SW_HIST = 1, SW_KEYS = 2 };  // what a qualifying pixel upda
 // Finalize image b inside the hot kernel (all SEL_THREADS threads).  `local`: the keys are already in
 // sbuf[0..n_local) (image owned by this CTA alone); otherwise they are merged from the `nslots` segments.
 // sbuf holds SEL_CAP keys; s_fcnt holds >= nslots ints.
-__device__ void finalize_hot(const float *__restrict__ src, const SelectPlan &pl, int b, int nslots, bool local,
+template <typename MapT>
+__device__ void finalize_hot(const MapT *__restrict__ src, const SelectPlan &pl, int b, int nslots, bool local,
                              int n_local, const u64 *__restrict__ cand, const int *__restrict__ cand_cnt,
                              const uint32_t *__restrict__ cand_thr, const FinalizeOut &out, u64 *sbuf, int *s_fcnt,
                              int *s_tmp, u64 *s_red, int *fine, int *coarse) {
@@ -1039,13 +1050,22 @@ __device__ void finalize_hot(const float *__restrict__ src, const SelectPlan &pl
 #endif
 }
 
-template <bool LOGITS>
+// Stage ring of the hot kernel for map element type T: SEL_STAGES stages of one whole 128x128 plane each (64 KiB
+// for fp32, 32 KiB for fp16 / bf16; DESIGN 4.1 has the measurement behind 3 half-size stages rather than 6).
+template <typename T>
+constexpr size_t hot_smem_bytes() {
+  return (size_t)SEL_STAGES * (128 * 128 * sizeof(T)) + (size_t)SEL_CAP * 8 +
+         (size_t)(SEL_HIST_FINE + SEL_HIST_COARSE) * 4 + (size_t)SEL_MASK_WORDS * 4 + SEL_STAGES * 8 + 32;
+}
+
+template <typename T, bool LOGITS>
 __global__ void __launch_bounds__(SEL_THREADS, 1)
-k_select_hot(const float *__restrict__ src, const SelectPlan pl, u64 *__restrict__ cand, int *__restrict__ cand_cnt,
+k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ cand, int *__restrict__ cand_cnt,
              int *__restrict__ img_done, uint32_t *__restrict__ cand_thr, const FinalizeOut fout) {
+  constexpr uint32_t PLANE_BYTES = 128 * 128 * sizeof(T);
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  float *stages = reinterpret_cast<float *>(smem_raw);
-  u64 *buf = reinterpret_cast<u64 *>(smem_raw + (size_t)SEL_STAGES * SEL_STAGE_BYTES);
+  T *stages = reinterpret_cast<T *>(smem_raw);
+  u64 *buf = reinterpret_cast<u64 *>(smem_raw + (size_t)SEL_STAGES * PLANE_BYTES);
   int *fine = reinterpret_cast<int *>(buf + SEL_CAP);
   int *coarse = fine + SEL_HIST_FINE;
   int *s_fcnt = reinterpret_cast<int *>(coarse + SEL_HIST_COARSE);   // SEL_MASK_WORDS (512) ints >= SEL_MAX_CTA
@@ -1073,10 +1093,10 @@ k_select_hot(const float *__restrict__ src, const SelectPlan pl, u64 *__restrict
   auto issue = [&](int u) {  // one lane
     const int s = u % SEL_STAGES;
     const char *gsrc = reinterpret_cast<const char *>(src + (p_begin + u) * (long long)HW);
-    char *dst = reinterpret_cast<char *>(stages) + (size_t)s * SEL_STAGE_BYTES;
-    mbar_expect_tx(&full[s], (uint32_t)SEL_STAGE_BYTES);
+    char *dst = reinterpret_cast<char *>(stages) + (size_t)s * PLANE_BYTES;
+    mbar_expect_tx(&full[s], PLANE_BYTES);
 #pragma unroll
-    for (uint32_t off = 0; off < (uint32_t)SEL_STAGE_BYTES; off += 16384u)
+    for (uint32_t off = 0; off < PLANE_BYTES; off += 16384u)
       bulk_g2s(dst + off, gsrc + off, 16384u, &full[s]);
   };
   auto clear_hist = [&]() {
@@ -1205,7 +1225,7 @@ k_select_hot(const float *__restrict__ src, const SelectPlan pl, u64 *__restrict
       __syncthreads();
       u64 thr64 = 0ull;
       const long long lo = max(p_begin, (long long)img * C), hi = min(p_end, (long long)(img + 1) * C);
-      const float *ibase = src + (long long)img * C * HW;
+      const T *ibase = src + (long long)img * C * HW;
       for (long long p = lo; p < hi; ++p) {
         const int c = (int)(p - (long long)img * C);
         for (int base = 0; base < HW; base += SEL_THREADS) {
@@ -1279,23 +1299,24 @@ k_select_hot(const float *__restrict__ src, const SelectPlan pl, u64 *__restrict
   // Per row: 4 vertical FMNMX3, 2 SHFL, 2 FADD (lane-edge -inf, keeps the ALU pipe free), the
   // horizontal max with the running threshold folded in, 4 compares and one (rarely taken) branch.
   const float edge_l = (lane == 0) ? NI : 0.0f, edge_r = (lane == 31) ? NI : 0.0f;
-  auto sweep = [&](const float *st, int c, int mode) {
+  // T = fp16 / bf16: a lane loads 4 elements (8 bytes) per row and widens them; everything after the load is the
+  // fp32 sweep.
+  auto sweep = [&](const T *st, int c, int mode) {
     const bool use_thr = (mode != SW_HIST);
     const int y0 = warp * 4;
-    const float *p = st + (size_t)y0 * 128 + lane * 4;
-    const float4 ninf = make_float4(NI, NI, NI, NI);
-    float4 r_[6];
-    r_[0] = (y0 > 0) ? *reinterpret_cast<const float4 *>(p - 128) : ninf;
+    const T *p = st + (size_t)y0 * 128 + lane * 4;
+    typename Raw4<T>::type r_[6];
+    r_[0] = (y0 > 0) ? ld_raw4(p - 128) : raw4_ninf<T>();
 #pragma unroll
-    for (int i = 0; i < 4; ++i) r_[i + 1] = *reinterpret_cast<const float4 *>(p + i * 128);
-    r_[5] = (y0 + 4 < 128) ? *reinterpret_cast<const float4 *>(p + 4 * 128) : ninf;
+    for (int i = 0; i < 4; ++i) r_[i + 1] = ld_raw4(p + i * 128);
+    r_[5] = (y0 + 4 < 128) ? ld_raw4(p + 4 * 128) : raw4_ninf<T>();
     const uint32_t fbase = (uint32_t)c * (uint32_t)HW + (uint32_t)(y0 * 128 + lane * 4);
     float lane_best = LOGITS ? NI : 0.0f;   // SW_HIST: best peak among this lane's 16 pixels
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       // threshold >= smallest positive float, so `b == max(.., thr)` also rejects b <= 0; it is
       // re-read per row (one broadcast LDS): fresher threshold = fewer pushes
-      const float4 a = r_[i], b = r_[i + 1], cc = r_[i + 2];
+      const float4 a = widen4<T>(r_[i]), b = widen4<T>(r_[i + 1]), cc = widen4<T>(r_[i + 2]);
       const float v0 = fmax3(a.x, b.x, cc.x), v1 = fmax3(a.y, b.y, cc.y);
       const float v2 = fmax3(a.z, b.z, cc.z), v3 = fmax3(a.w, b.w, cc.w);
       const float l = __shfl_up_sync(0xffffffffu, v3, 1) + edge_l;
@@ -1355,7 +1376,7 @@ k_select_hot(const float *__restrict__ src, const SelectPlan pl, u64 *__restrict
   CNB_STAT(long long st_t0 = clock64(); long long st_wait = 0; long long st_boot = 0; long long st_flush = 0;
            int st_nboot = 0; int st_nflush = 0; long long st_q;)
   for (int u = 0; u < total_units; ++u) {
-    const float *st = stages + (size_t)stage * (SEL_STAGE_BYTES / 4);
+    const T *st = stages + (size_t)stage * (128 * 128);
     CNB_STAT(st_q = clock64();)
     mbar_wait(&full[stage], (uint32_t)par);
     CNB_STAT(st_wait += clock64() - st_q; st_q = clock64();)
@@ -1440,7 +1461,7 @@ static size_t stage1_smem_bytes() {
 }
 
 
-int make_select_plan(const float *src, int n_img, int C, int H, int W, int K, int nms, SelectPlan *pl) {
+int make_select_plan(const void *src, int n_img, int C, int H, int W, int K, int nms, SelectPlan *pl, int elem_size) {
   CNB_REQUIRE(n_img > 0 && C > 0 && H > 0 && W > 0 && K > 0, CNB_EINVAL,
               "top-k: non-positive dimension (n_img=%d c=%d h=%d w=%d k=%d)", n_img, C, H, W, K);
   CNB_REQUIRE((long long)K <= (long long)H * W, CNB_EINVAL,
@@ -1453,7 +1474,8 @@ int make_select_plan(const float *src, int n_img, int C, int H, int W, int K, in
   pl->Wp = (W + 3) / 4 * 4;
   pl->ncb = (W + 127) / 128;
   pl->P = (long long)n_img * C;
-  pl->use_tma = (W % 4 == 0) && ((reinterpret_cast<uintptr_t>(src) & 15u) == 0);
+  // rows of whole 16-byte chunks from a 16-byte aligned base
+  pl->use_tma = ((long long)W * elem_size % 16 == 0) && ((reinterpret_cast<uintptr_t>(src) & 15u) == 0);
   const int max_rows = SEL_STAGE_BYTES / (pl->Wp * 4);
   CNB_REQUIRE(max_rows >= 3 && pl->ncb <= 32, CNB_EUNSUPPORTED, "top-k: w=%d too wide for a 64 KiB stage", W);
   int rb_cap = SEL_MASK_WORDS / (4 * pl->ncb);
@@ -1551,26 +1573,36 @@ static int launch_stage1(const float *src, const SelectPlan &pl, const FinalizeO
   return CNB_OK;
 }
 
+template <typename T>
+static int launch_hot(const void *src, const SelectPlan &pl, const FinalizeOut &out, u64 *cand, int *cnt, int *done,
+                      uint32_t *thr, cudaStream_t stream) {
+  constexpr size_t smem1 = hot_smem_bytes<T>();
+  static thread_local int hot_dev = -1;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (hot_dev != dev) {
+    CNB_CUDA(cudaFuncSetAttribute(k_select_hot<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+    CNB_CUDA(cudaFuncSetAttribute(k_select_hot<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+    hot_dev = dev;
+  }
+  const T *s = reinterpret_cast<const T *>(src);
+  if (pl.logits) k_select_hot<T, true><<<pl.n_cta, SEL_THREADS, smem1, stream>>>(s, pl, cand, cnt, done, thr, out);
+  else k_select_hot<T, false><<<pl.n_cta, SEL_THREADS, smem1, stream>>>(s, pl, cand, cnt, done, thr, out);
+  CNB_CHECK_LAUNCH("select stage 1 (hot)");
+  count_launch();
+  return CNB_OK;
+}
+
 template <bool NMS>
-static int launch_select(const float *src, const SelectPlan &pl, const FinalizeOut &out, u64 *cand, int *cnt,
-                         int *done, uint32_t *thr, cudaStream_t stream) {
+static int launch_select(const void *src_v, int src_dtype, const SelectPlan &pl, const FinalizeOut &out, u64 *cand,
+                         int *cnt, int *done, uint32_t *thr, cudaStream_t stream) {
+  const float *src = reinterpret_cast<const float *>(src_v);   // every path but the hot one reads fp32
   if (pl.fused_finalize) CNB_CUDA(cudaMemsetAsync(done, 0, (size_t)pl.n_img * 4, stream));
   int rc;
   if (NMS && pl.hot) {
-    const size_t smem1 = stage1_smem_bytes();
-    static thread_local int hot_dev = -1;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (hot_dev != dev) {
-      CNB_CUDA(cudaFuncSetAttribute(k_select_hot<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-      CNB_CUDA(cudaFuncSetAttribute(k_select_hot<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-      hot_dev = dev;
-    }
-    if (pl.logits) k_select_hot<true><<<pl.n_cta, SEL_THREADS, smem1, stream>>>(src, pl, cand, cnt, done, thr, out);
-    else k_select_hot<false><<<pl.n_cta, SEL_THREADS, smem1, stream>>>(src, pl, cand, cnt, done, thr, out);
-    CNB_CHECK_LAUNCH("select stage 1 (hot)");
-    count_launch();
-    rc = CNB_OK;
+    if (src_dtype == CNB_DTYPE_BF16) rc = launch_hot<__nv_bfloat16>(src_v, pl, out, cand, cnt, done, thr, stream);
+    else if (src_dtype == CNB_DTYPE_F16) rc = launch_hot<__half>(src_v, pl, out, cand, cnt, done, thr, stream);
+    else rc = launch_hot<float>(src_v, pl, out, cand, cnt, done, thr, stream);
   } else if (NMS && pl.use_tma && pl.W == 128 && pl.H == 128 && pl.rb == 128)
     rc = launch_stage1<NMS, true, 2>(src, pl, out, cand, cnt, done, stream);
   else if (pl.use_tma && pl.ncb == 1)
@@ -1590,7 +1622,10 @@ static int launch_select(const float *src, const SelectPlan &pl, const FinalizeO
   return CNB_OK;
 }
 
-int run_select(const float *src, const SelectPlan &pl, const FinalizeOut &out, void *ws, cudaStream_t stream) {
+int run_select(const void *src, const SelectPlan &pl, const FinalizeOut &out, void *ws, cudaStream_t stream,
+               int src_dtype) {
+  CNB_REQUIRE(src_dtype == CNB_DTYPE_F32 || (pl.hot && pl.nms), CNB_EINVAL,
+              "select: a 16-bit map needs the hot geometry (128x128 planes, k <= 256, 16-byte aligned)");
   char *p = reinterpret_cast<char *>(ws);
   u64 *cand = reinterpret_cast<u64 *>(p);
   p += align_up((size_t)pl.n_img * pl.max_slots * (pl.seg_cap > 256 ? pl.seg_cap : 256) * 8, 256);
@@ -1599,8 +1634,8 @@ int run_select(const float *src, const SelectPlan &pl, const FinalizeOut &out, v
   int *done = reinterpret_cast<int *>(p);
   p += align_up((size_t)pl.n_img * 4, 256);
   uint32_t *thr = reinterpret_cast<uint32_t *>(p);
-  return pl.nms ? launch_select<true>(src, pl, out, cand, cnt, done, thr, stream)
-                : launch_select<false>(src, pl, out, cand, cnt, done, thr, stream);
+  return pl.nms ? launch_select<true>(src, src_dtype, pl, out, cand, cnt, done, thr, stream)
+                : launch_select<false>(src, src_dtype, pl, out, cand, cnt, done, thr, stream);
 }
 
 #ifdef CNB_SELECT_STATS

@@ -1,13 +1,17 @@
 // Fused 3x3 peak-NMS + exact top-K selection over [n_img, C, H, W] score maps.
 // Replaces models/decode.py:9-15 (_nms) + :92-119 (_topk / _topk_channel).
+// The score map is fp32, or fp16 / bf16 in the hot geometry (k_select_hot widens each element to fp32 in
+// registers, exactly, so a half map selects what its .float() upcast selects).
 #pragma once
+#include <cuda_fp16.h>
+#include <cuda_bf16.h>
 #include "common.cuh"
 
 namespace cnb {
 
 constexpr int SEL_THREADS = 1024;
 constexpr int SEL_WARPS = SEL_THREADS / 32;
-constexpr int SEL_STAGES = 3;
+constexpr int SEL_STAGES = 3;           // stage ring depth (the hot kernel's too, for fp16 / bf16 maps as well)
 constexpr int SEL_STAGE_BYTES = 65536;  // one 128x128 fp32 plane
 constexpr int SEL_CAP = 2048;           // per-CTA candidate buffer (64-bit keys)
 constexpr int SEL_HIST_FINE = 2048;     // running-threshold histogram: 128 bins per octave over [2^-16, 1)
@@ -46,16 +50,57 @@ struct FinalizeOut {
   float *ys;
   float *xs;
   // ctdet epilogue (models/decode.py:472-493); dets == null -> raw only
-  const float *wh;
-  const float *reg;
+  const void *wh;   // element type: wh_dtype / reg_dtype (CNB_DTYPE_*; zero-initialised = fp32)
+  const void *reg;
   int cat_spec_wh;
   float *dets;
+  int wh_dtype, reg_dtype;
 };
 
-// Returns CNB_OK or an error; fills `pl`.
-int make_select_plan(const float *src, int n_img, int C, int H, int W, int K, int nms, SelectPlan *pl);
+// Returns CNB_OK or an error; fills `pl`.  elem_size (4, or 2 for fp16 / bf16) and the alignment of src decide
+// whether the map can be loaded with TMA bulk copies.
+int make_select_plan(const void *src, int n_img, int C, int H, int W, int K, int nms, SelectPlan *pl,
+                     int elem_size = 4);
 size_t select_workspace_bytes(const SelectPlan &pl);
-// Enqueue stage 1 + finalize.  `ws` must hold select_workspace_bytes(pl).
-int run_select(const float *src, const SelectPlan &pl, const FinalizeOut &out, void *ws, cudaStream_t stream);
+// Enqueue stage 1 + finalize.  `ws` must hold select_workspace_bytes(pl).  src_dtype other than CNB_DTYPE_F32 is
+// only accepted for a hot plan (pl.hot) made with elem_size 2.
+int run_select(const void *src, const SelectPlan &pl, const FinalizeOut &out, void *ws, cudaStream_t stream,
+               int src_dtype = CNB_DTYPE_F32);
+
+#ifdef __CUDACC__
+// Exact widening of one map / head element to fp32 (every fp16 and bf16 value, subnormals and infinities included,
+// is a float: the result equals torch's .float()).
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+// Four consecutive map elements as loaded from shared memory (16 bytes of fp32, 8 of fp16 / bf16: the 16-bit sweep
+// keeps its row window in half the registers) and their exact widening to fp32.
+template <typename T> struct Raw4;
+template <> struct Raw4<float> { typedef float4 type; };
+template <> struct Raw4<__half> { typedef uint2 type; };
+template <> struct Raw4<__nv_bfloat16> { typedef uint2 type; };
+template <typename T>
+__device__ __forceinline__ typename Raw4<T>::type ld_raw4(const T *p) {
+  return *reinterpret_cast<const typename Raw4<T>::type *>(p);
+}
+template <typename T> __device__ __forceinline__ typename Raw4<T>::type raw4_ninf();   // four -inf
+template <> __device__ __forceinline__ float4 raw4_ninf<float>() {
+  return make_float4(CNB_NEG_INF, CNB_NEG_INF, CNB_NEG_INF, CNB_NEG_INF);
+}
+template <> __device__ __forceinline__ uint2 raw4_ninf<__half>() { return make_uint2(0xfc00fc00u, 0xfc00fc00u); }
+template <> __device__ __forceinline__ uint2 raw4_ninf<__nv_bfloat16>() { return make_uint2(0xff80ff80u, 0xff80ff80u); }
+template <typename T> __device__ __forceinline__ float4 widen4(typename Raw4<T>::type r);
+template <> __device__ __forceinline__ float4 widen4<float>(float4 r) { return r; }
+template <> __device__ __forceinline__ float4 widen4<__half>(uint2 u) {
+  return make_float4(__half2float(__ushort_as_half((unsigned short)(u.x & 0xffffu))),
+                     __half2float(__ushort_as_half((unsigned short)(u.x >> 16))),
+                     __half2float(__ushort_as_half((unsigned short)(u.y & 0xffffu))),
+                     __half2float(__ushort_as_half((unsigned short)(u.y >> 16))));
+}
+template <> __device__ __forceinline__ float4 widen4<__nv_bfloat16>(uint2 u) {
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xffff0000u));
+}
+#endif
 
 }  // namespace cnb

@@ -2,7 +2,10 @@
 
 Every function takes fp32 CUDA tensors (NCHW; heat maps already sigmoided by the
 caller, as in detectors/ctdet.py:31,40), does not mutate its inputs, and returns a new
-fp32 tensor on the same device, enqueued on the current stream.  The work is done by
+fp32 tensor on the same device, enqueued on the current stream.  Other dtypes are upcast
+to fp32 first, except in ctdet_decode, ctdet_decode_from_logits, flip_merge (and so the
+*_flip_from_logits wrappers) and ctdet_decode_from_host: they read bf16 and fp16 heads in
+place, and return, bit for bit, what they return for the .float() upcast.  The work is done by
 the hand-written sm_90a kernels behind ``include/centernet_b200.h``; there is no
 CPU path (non-CUDA inputs raise NotImplementedError).
 
@@ -11,7 +14,7 @@ Tie order, which the reference leaves to torch.topk, is defined here as
 """
 import torch
 
-from ._lib import C, f32c, ptr, require_cuda, stream_ptr, workspace
+from ._lib import C, dtype_code, f32c, floatc, ptr, require_cuda, stream_ptr, workspace
 from .utils import _gather_feat, _transpose_and_gather_feat  # noqa: F401  (re-exported like the reference)
 
 
@@ -118,9 +121,24 @@ def _topk(scores, K=40):
 
 
 # ------------------------------------------------------------------ decode.py:464-495
+def _all_f32(*tensors):
+    return all(t is None or t.dtype == torch.float32 for t in tensors)
+
+
+def _decode_ex(heat, wh, reg, cat_spec_wh, K, logits, dets):
+    """cnb_ctdet_decode_ex: heat / wh / reg each fp32, fp16 or bf16."""
+    b, c, h, w = _dims(heat)
+    ws = workspace(C.ctdet_decode_ex_workspace_bytes(ptr(heat), dtype_code(heat), logits, b, c, h, w, K), heat.device)
+    C.ctdet_decode_ex(ptr(heat), dtype_code(heat), logits, ptr(wh), dtype_code(wh), ptr(reg), dtype_code(reg),
+                      int(bool(cat_spec_wh)), b, c, h, w, K, ptr(dets), ptr(ws), ws.numel(), stream_ptr(heat))
+    return dets
+
+
 def ctdet_decode(heat, wh, reg=None, cat_spec_wh=False, K=100):
+    """bf16 / fp16 heat, wh and reg (each its own dtype) are read in place: the dets equal, bit for bit, those of
+    the .float() upcast."""
     require_cuda(heat, wh, reg, what="ctdet_decode")
-    heat, wh, reg = f32c(heat), f32c(wh), f32c(reg)
+    heat, wh, reg = floatc(heat), floatc(wh), floatc(reg)
     b, c, h, w = _dims(heat)
     want = 2 * c if cat_spec_wh else 2
     if wh.shape[0] != b or wh.shape[1] != want or tuple(wh.shape[2:]) != (h, w):
@@ -128,6 +146,8 @@ def ctdet_decode(heat, wh, reg=None, cat_spec_wh=False, K=100):
     if reg is not None and tuple(reg.shape) != (b, 2, h, w):
         raise RuntimeError("ctdet_decode: reg must be [%d, 2, %d, %d], got %s" % (b, h, w, tuple(reg.shape)))
     dets = torch.empty((b, K, 6), dtype=torch.float32, device=heat.device)
+    if not _all_f32(heat, wh, reg):
+        return _decode_ex(heat, wh, reg, cat_spec_wh, K, 0, dets)
     ws = workspace(C.topk_workspace_bytes(b, c, h, w, K), heat.device)
     C.ctdet_decode(ptr(heat), ptr(wh), ptr(reg), int(bool(cat_spec_wh)), b, c, h, w, K, ptr(dets), ptr(ws),
                    ws.numel(), stream_ptr(heat))
@@ -138,9 +158,12 @@ def ctdet_decode_from_logits(hm, wh, reg=None, cat_spec_wh=False, K=100):
     """`ctdet_decode(hm.sigmoid_(), wh, reg, ...)` (detectors/ctdet.py:30-45) in one launch, reading the
     head's raw logits: the selection runs in logit space (the sigmoid is monotone) and only the
     candidates are pushed through 1/(1+exp(-x)).  Scores are bit-identical to torch's CUDA sigmoid,
-    indices / classes / boxes identical to ctdet_decode on that heat map; `hm` is not modified."""
+    indices / classes / boxes identical to ctdet_decode on that heat map; `hm` is not modified.
+    bf16 / fp16 logits (and wh / reg) are read in place and scored with the fp32 sigmoid of the widened logit, so
+    the dets equal those of the .float() upcast (the reference's `hm.sigmoid_()` on a half tensor would round the
+    scores to half precision first)."""
     require_cuda(hm, wh, reg, what="ctdet_decode_from_logits")
-    hm, wh, reg = f32c(hm), f32c(wh), f32c(reg)
+    hm, wh, reg = floatc(hm), floatc(wh), floatc(reg)
     b, c, h, w = _dims(hm)
     want = 2 * c if cat_spec_wh else 2
     if wh.shape[0] != b or wh.shape[1] != want or tuple(wh.shape[2:]) != (h, w):
@@ -148,6 +171,8 @@ def ctdet_decode_from_logits(hm, wh, reg=None, cat_spec_wh=False, K=100):
     if reg is not None and tuple(reg.shape) != (b, 2, h, w):
         raise RuntimeError("ctdet_decode_from_logits: reg must be [%d, 2, %d, %d], got %s" % (b, h, w, tuple(reg.shape)))
     dets = torch.empty((b, K, 6), dtype=torch.float32, device=hm.device)
+    if not _all_f32(hm, wh, reg):
+        return _decode_ex(hm, wh, reg, cat_spec_wh, K, 1, dets)
     ws = workspace(C.ctdet_logits_workspace_bytes(ptr(hm), b, c, h, w, K), hm.device)
     C.ctdet_decode_logits(ptr(hm), ptr(wh), ptr(reg), int(bool(cat_spec_wh)), b, c, h, w, K, ptr(dets), ptr(ws),
                           ws.numel(), stream_ptr(hm))
@@ -168,9 +193,10 @@ def flip_merge(x, sigmoid=False, flip_idx=None, offsets=False):
     """(f(x[:n]) + flip(f(x[n:]))) / 2 for a batch x [2n, C, H, W] = n images followed by their mirrored copies
     (base_detector.py:63-64).  flip: flip_tensor; with `flip_idx` the joint channels are swapped as in flip_lr
     (models/utils.py:33-39), with `offsets` as in flip_lr_off (:41-50: C = 2 x joints, x offsets negated).
-    One kernel, no host round trip (the reference's flip_lr / flip_lr_off go through numpy)."""
+    One kernel, no host round trip (the reference's flip_lr / flip_lr_off go through numpy).  A bf16 / fp16 x is
+    read in place (widened exactly); the result is fp32 either way."""
     require_cuda(x, what="flip_merge")
-    x = f32c(x)
+    x = floatc(x)
     b2, c, h, w = _dims(x)
     if b2 % 2:
         raise RuntimeError("flip_merge: batch must hold image / mirrored-image pairs")
@@ -190,7 +216,11 @@ def flip_merge(x, sigmoid=False, flip_idx=None, offsets=False):
                 p[a], p[b_] = p[b_], p[a]
             perm = torch.tensor(p, dtype=torch.int32, device=x.device)
     out = torch.empty((n, c, h, w), dtype=torch.float32, device=x.device)
-    C.flip_merge(ptr(x), ptr(out), n, c, h, w, int(bool(sigmoid)), ptr(perm), ptr(sign), stream_ptr(x))
+    if x.dtype == torch.float32:
+        C.flip_merge(ptr(x), ptr(out), n, c, h, w, int(bool(sigmoid)), ptr(perm), ptr(sign), stream_ptr(x))
+    else:
+        C.flip_merge_ex(ptr(x), dtype_code(x), ptr(out), n, c, h, w, int(bool(sigmoid)), ptr(perm), ptr(sign),
+                        stream_ptr(x))
     return out
 
 
@@ -294,14 +324,18 @@ def ctdet_decode_from_host(heat, wh, reg=None, cat_spec_wh=False, K=100, chunk=8
     decode kernels of the previous piece; the [B, K, 6] detections come back in pinned host
     memory.  This is the call a detector makes when the heat maps are produced off-device
     (and what bench.py times as `e2e`).  Same semantics as ctdet_decode: the result is a FRESH host
-    tensor the caller owns (the pinned staging buffer is copied out, 2.4 KB per image)."""
+    tensor the caller owns (the pinned staging buffer is copied out, 2.4 KB per image).  bf16 / fp16 host
+    tensors are staged in their own dtype (no CPU-side conversion, half the bytes over PCIe) and decoded in
+    place."""
     if heat.is_cuda:
         return ctdet_decode(heat, wh, reg=reg, cat_spec_wh=cat_spec_wh, K=K).cpu()
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-    heat, wh, reg = f32c(heat), f32c(wh), f32c(reg)
+    heat, wh, reg = floatc(heat), floatc(wh), floatc(reg)
     b, c, h, w = _dims(heat)
     chunk = max(1, min(chunk, b))
-    key = (dev.index, c, h, w, int(wh.shape[1]), reg is not None, chunk, b, K)
+    native = _all_f32(heat, wh, reg)
+    key = (dev.index, c, h, w, int(wh.shape[1]), reg is not None, chunk, b, K, heat.dtype, wh.dtype,
+           None if reg is None else reg.dtype)
     cache = getattr(_HOST_TLS, "ctx", None)
     if cache is None:
         cache = _HOST_TLS.ctx = {}
@@ -309,16 +343,21 @@ def ctdet_decode_from_host(heat, wh, reg=None, cat_spec_wh=False, K=100, chunk=8
     if ctx is None:
         ctx = {
             "copy": torch.cuda.Stream(device=dev),
-            "heat": [torch.empty((chunk, c, h, w), dtype=torch.float32, device=dev) for _ in range(2)],
-            "wh": [torch.empty((chunk, int(wh.shape[1]), h, w), dtype=torch.float32, device=dev) for _ in range(2)],
-            "reg": [torch.empty((chunk, 2, h, w), dtype=torch.float32, device=dev) for _ in range(2)]
+            "heat": [torch.empty((chunk, c, h, w), dtype=heat.dtype, device=dev) for _ in range(2)],
+            "wh": [torch.empty((chunk, int(wh.shape[1]), h, w), dtype=wh.dtype, device=dev) for _ in range(2)],
+            "reg": [torch.empty((chunk, 2, h, w), dtype=reg.dtype, device=dev) for _ in range(2)]
                    if reg is not None else [None, None],
             "dets": torch.empty((b, K, 6), dtype=torch.float32, device=dev),
             "out": torch.empty((b, K, 6), dtype=torch.float32).pin_memory(),
-            "ws": workspace(C.topk_workspace_bytes(chunk, c, h, w, K), dev),
             "free": [torch.cuda.Event(), torch.cuda.Event()],
             "ready": [torch.cuda.Event(), torch.cuda.Event()],
         }
+        if native:
+            ctx["ws"] = workspace(C.topk_workspace_bytes(chunk, c, h, w, K), dev)
+        else:  # the staging buffers are fresh allocations: both slots share one alignment and so one path
+            hp = ptr(ctx["heat"][0])
+            ctx["ws"] = workspace(max(C.ctdet_decode_ex_workspace_bytes(hp, dtype_code(heat), 0, n, c, h, w, K)
+                                      for n in {chunk, b % chunk or chunk}), dev)
         cache.clear()  # keep one geometry resident per thread
         cache[key] = ctx
     main = torch.cuda.current_stream(dev)
@@ -337,9 +376,14 @@ def ctdet_decode_from_host(heat, wh, reg=None, cat_spec_wh=False, K=100, chunk=8
             ctx["ready"][slot].record(copy)
         main.wait_event(ctx["ready"][slot])
         dets = ctx["dets"][s:s + n]
-        C.ctdet_decode(ptr(ctx["heat"][slot]), ptr(ctx["wh"][slot]), ptr(ctx["reg"][slot]),
-                       int(bool(cat_spec_wh)), n, c, h, w, K, ptr(dets), ptr(ctx["ws"]), ctx["ws"].numel(),
-                       main.cuda_stream)
+        if native:
+            C.ctdet_decode(ptr(ctx["heat"][slot]), ptr(ctx["wh"][slot]), ptr(ctx["reg"][slot]),
+                           int(bool(cat_spec_wh)), n, c, h, w, K, ptr(dets), ptr(ctx["ws"]), ctx["ws"].numel(),
+                           main.cuda_stream)
+        else:
+            C.ctdet_decode_ex(ptr(ctx["heat"][slot]), dtype_code(heat), 0, ptr(ctx["wh"][slot]), dtype_code(wh),
+                              ptr(ctx["reg"][slot]), dtype_code(reg), int(bool(cat_spec_wh)), n, c, h, w, K,
+                              ptr(dets), ptr(ctx["ws"]), ctx["ws"].numel(), main.cuda_stream)
         ctx["free"][slot].record(main)
     ctx["out"].copy_(ctx["dets"], non_blocking=True)
     main.synchronize()

@@ -13,7 +13,8 @@
  *       (dcn_v2_cuda_forward / dcn_v2_cuda_backward / dcn_v2_psroi_pooling_*).
  *
  * Conventions
- *   - every tensor is fp32 (double in the *_f64 entry points), NCHW, contiguous, resident on the current device;
+ *   - every tensor is fp32 (double in the *_f64 entry points; fp32, fp16 or bf16 where a dtype code is passed), NCHW,
+ *     contiguous, resident on the current device;
  *     index outputs use the reference's dtypes (int64 indices, int32 classes);
  *   - the caller owns every buffer, including the scratch `workspace`
  *     (size from the matching cnb_*_workspace_bytes); the library never calls
@@ -41,9 +42,11 @@ extern "C" {
 #define CNB_ECUDA 3        /* CUDA runtime / launch error                        */
 #define CNB_EWORKSPACE 4   /* workspace_bytes smaller than cnb_*_workspace_bytes */
 
-/* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16). */
+/* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16, cnb_ctdet_decode_ex,
+ * cnb_flip_merge_ex). */
 #define CNB_DTYPE_F32 0
 #define CNB_DTYPE_BF16 1
+#define CNB_DTYPE_F16 2
 
 /* Library version (major*10000 + minor*100 + patch). */
 int cnb_version(void);
@@ -111,6 +114,23 @@ int cnb_ctdet_decode_logits(const float *hm_logits, const float *wh, const float
                             int b, int c, int h, int w, int k, float *dets,
                             void *workspace, size_t workspace_bytes, void *stream);
 
+/* ----------------------------------- N1: ctdet_decode of fp32, fp16 or bf16 heads
+ * cnb_ctdet_decode (logits == 0) or cnb_ctdet_decode_logits (logits != 0) for heads of any of the three float
+ * types, each of heat, wh and reg with its own dtype code (CNB_DTYPE_F32 / _F16 / _BF16).  Contract: for fp16 or
+ * bf16 tensors the dets, bit for bit, are those the fp32 calls return for the .float() upcast of the same
+ * tensors (both widen exactly to fp32; the logits path scores with the fp32 sigmoid of the widened logit).
+ * dets stay fp32.  In the hot geometry (h = w = 128, k <= 256, heat 16-byte aligned) the selection kernel reads
+ * the 16-bit map itself; any other geometry widens the map once into the workspace (logits: the sigmoid pass reads
+ * the 16-bit logits) and runs the fp32 path.  The query takes the heat pointer because its alignment decides the
+ * path; with CNB_DTYPE_F32 it equals cnb_topk_workspace_bytes (logits == 0) or cnb_ctdet_logits_workspace_bytes,
+ * and it returns 0 for every shape the call rejects.  Errors, checked before any CUDA call: CNB_EINVAL for an
+ * unknown dtype code, a null pointer or a bad shape; CNB_EWORKSPACE for too small a workspace. */
+size_t cnb_ctdet_decode_ex_workspace_bytes(const void *heat, int heat_dtype, int logits,
+                                           int b, int c, int h, int w, int k);
+int cnb_ctdet_decode_ex(const void *heat, int heat_dtype, int logits, const void *wh, int wh_dtype,
+                        const void *reg, int reg_dtype, int cat_spec_wh, int b, int c, int h, int w, int k,
+                        float *dets, void *workspace, size_t workspace_bytes, void *stream);
+
 /* out[i] = 1 / (1 + exp(-x[i])): the bare `sigmoid_()` of detectors/ctdet.py:31, the very expression the
  * fused path applies to its candidates (exposed so tests can pin it against torch and prove it monotone). */
 int cnb_sigmoid(const float *x, float *out, long long n, void *stream);
@@ -123,6 +143,11 @@ int cnb_sigmoid(const float *x, float *out, long long n, void *stream);
  * joint swap for flip_lr (:33-39); perm + sign for flip_lr_off (:41-50). */
 int cnb_flip_merge(const float *src, float *dst, int n, int c, int h, int w, int apply_sigmoid,
                    const int32_t *perm, const float *sign, void *stream);
+/* The same merge for a src of src_dtype (CNB_DTYPE_F32 / _F16 / _BF16): elements are widened exactly to fp32
+ * first, so the fp32 dst equals cnb_flip_merge of the .float() upcast.  CNB_EINVAL for an unknown dtype code, a
+ * null pointer or a non-positive dimension, before any CUDA call. */
+int cnb_flip_merge_ex(const void *src, int src_dtype, float *dst, int n, int c, int h, int w, int apply_sigmoid,
+                      const int32_t *perm, const float *sign, void *stream);
 
 /* ------------------------------------------------------------ A9: ddd_decode
  * models/decode.py:426-462.  rot [b,8,h,w], depth [b,1,h,w], dim [b,3,h,w],
