@@ -520,6 +520,7 @@ static int dcn_plan(const char *fn, int b, int cin, int h, int w, int cout, int 
   p->fp32_dw_splits = fp32_weight_splits(b, cin, cout, dg, ((long long)ho * wo + DCN_TP - 1) / DCN_TP);
   plan_forward_tc(p);
   plan_backward_tc(p);
+  plan_backward_bf16(p);
   return CNB_OK;
 }
 
@@ -606,6 +607,47 @@ size_t cnb_dcnv2_backward_workspace_bytes(int b, int cin, int cout, int h, int w
                cnb_dcnv2_get_deterministic() != 0, false, false, &p) != CNB_OK || !p.bwd_tc)
     return 0;
   return p.bwd.bytes;
+}
+
+size_t cnb_dcnv2_backward_bf16_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw, int stride,
+                                               int pad, int dil, int dg) {
+  DcnPlan p;
+  if (dcn_plan("cnb_dcnv2_backward_bf16_workspace_bytes", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil,
+               dg, cnb_dcnv2_get_deterministic() != 0, false, false, &p) != CNB_OK)
+    return 0;
+  return p.bwd16.bytes;   // 0 where the bf16 backward does not run
+}
+
+// Checks in order: pointers, dtype codes, shape (dcn_plan), coverage, layout, workspace, alignment.
+int cnb_dcnv2_backward_bf16(const void *input, int input_dtype, int input_channels_last, const float *offset,
+                            const float *mask, const float *weight, const void *grad_output, int grad_output_dtype,
+                            float *grad_input, int grad_input_channels_last, float *grad_offset, float *grad_mask,
+                            float *grad_weight, float *grad_bias, int b, int cin, int h, int w, int cout, int kh,
+                            int kw, int stride, int pad, int dil, int deformable_groups, void *workspace,
+                            size_t workspace_bytes, void *stream) {
+  const char *fn = "cnb_dcnv2_backward_bf16";
+  CNB_REQUIRE(input && offset && mask && weight && grad_output && workspace, CNB_EINVAL, "%s: null pointer", fn);
+  CNB_REQUIRE((input_dtype == CNB_DTYPE_F32 || input_dtype == CNB_DTYPE_BF16) &&
+                  (grad_output_dtype == CNB_DTYPE_F32 || grad_output_dtype == CNB_DTYPE_BF16),
+              CNB_EINVAL, "%s: unknown dtype code (input %d, grad_output %d)", fn, input_dtype, grad_output_dtype);
+  const bool gx_cl = grad_input_channels_last && grad_input;
+  DcnPlan p;
+  int rc = dcn_plan(fn, b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, deformable_groups,
+                    cnb_dcnv2_get_deterministic() != 0, input_channels_last != 0, gx_cl, &p);
+  if (rc != CNB_OK) return rc;
+  CNB_REQUIRE(p.bwd16.bytes > 0, CNB_EUNSUPPORTED,
+              "%s: the bf16 backward needs both tensor-core passes (cout <= 256, images within their 32-bit indexing)",
+              fn);
+  CNB_REQUIRE(!(input_channels_last || gx_cl) || (cin / deformable_groups) % 32 == 0, CNB_EUNSUPPORTED,
+              "%s: channels-last tensors need cin / deformable_groups to be a multiple of 32", fn);
+  CNB_REQUIRE(workspace_bytes >= p.bwd16.bytes, CNB_EWORKSPACE, "%s: workspace too small (%zu < %zu)", fn,
+              workspace_bytes, p.bwd16.bytes);
+  CNB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15u) == 0 && (reinterpret_cast<uintptr_t>(input) & 15u) == 0 &&
+                  (!gx_cl || (reinterpret_cast<uintptr_t>(grad_input) & 15u) == 0),
+              CNB_EINVAL, "%s: buffers must be 16-byte aligned", fn);
+  return dcn_backward_bf16(p, input, input_dtype == CNB_DTYPE_BF16, offset, mask, weight, grad_output,
+                           grad_output_dtype == CNB_DTYPE_BF16, grad_input, grad_offset, grad_mask, grad_weight,
+                           grad_bias, workspace, (cudaStream_t)stream);
 }
 
 size_t cnb_dcnv2_wtiles_bytes(int cin, int cout, int kh, int kw, int dg) {

@@ -821,6 +821,404 @@ __global__ void __launch_bounds__(256) k_dcn_bwd_wreduce(const float *__restrict
   }
 }
 
+// =====================================================================================================================
+// bf16 backward (opt-in, cnb_dcnv2_backward_bf16): both contractions on wgmma m64nNk16 .f32.bf16.bf16, one bf16 tile
+// per operand where the passes above use a TF32 hi/lo pair.  With W_b = bf16(W) and dY_b = bf16(dY) (RN; exact for a
+// bf16 grad_output):
+//   dcol = sum_o W_b dY_b  (exact products, fp32 sums), stored fp32 in the layout above, so that k_dcn_bwd_offmask, the
+//          dX scatter (atomics or fixed point), k_dcn_bwd_dx_nchw and k_dcn_bwd_dx_fixed run unchanged;
+//   dW   = sum_p bf16(col) dY_b, col the masked bilinear value of the forward sampler (same fmaf chain) rounded RN as
+//          k_dcn_forward_bf16 rounds it; per-CTA partials added by k_dcn_bwd_wreduce in split order;
+//   dBias  sums grad_output as given, in the order of k_bwd_prep_gyk and k_dcn_bwd_bias_reduce.
+constexpr int BB_TILE_BYTES = TC_TP * TC_K * 2;    // one bf16 tile [128 rows][32 k], dense K-major (bf_tile_off): 8 KB
+constexpr int BB_STAGES = 4;
+constexpr int BB_STAGE_BYTES = 2 * BB_TILE_BYTES;  // column-gradient stage: dY tile + W tile, 16 KB
+constexpr uint32_t WB_SBO = 528;                   // weight pass A tile: 8-row groups 512 + 16 bytes apart (DESIGN 4.4.3)
+constexpr int WB_A_BYTES = (TC_TP / 8) * WB_SBO;   // 8448
+constexpr int WB_STAGES = 4;
+
+__device__ __forceinline__ float ld_f32(const float *p) { return __ldg(p); }
+__device__ __forceinline__ float ld_f32(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
+
+// W -> per (row group rg, slice ks) one bf16 tile [128 rows = (chunk ql, ch)][32 k = output channel], the rows and
+// zero fill of k_bwd_prep_w.  DET: bnd[ks] from |W_b|.
+template <bool DET>
+__global__ void __launch_bounds__(256) k_bwd_prep_w_bf16(const float *__restrict__ w, const DcnShapeTc s,
+                                                         const BwdGeom g, unsigned char *__restrict__ wtb,
+                                                         unsigned *__restrict__ bnd) {
+  const int KT = s.kh * s.kw, cpg = s.Cin / s.dg;
+  const int rg = blockIdx.x / g.KS, ks = blockIdx.x - rg * g.KS;
+  unsigned char *tile = wtb + (size_t)blockIdx.x * BB_TILE_BYTES;
+  unsigned rmax = 0;
+  for (int i = threadIdx.x; i < TC_TP * TC_K; i += blockDim.x) {
+    const int k = i & (TC_K - 1), row = i >> 5;
+    const int q = rg * 4 + (row >> 5), ch = row & 31;
+    const int bi = q / TC_NT, tap = q - bi * TC_NT;
+    const int gi = bi / s.cbs_pg, cw = (bi - gi * s.cbs_pg) * TC_CB + ch;
+    const int o = ks * TC_K + k;
+    float v = 0.f;
+    if (q < g.Q && o < s.Cout && cw < cpg && tap < KT) v = __ldg(w + ((size_t)o * s.Cin + gi * cpg + cw) * KT + tap);
+    const __nv_bfloat16 vb = __float2bfloat16_rn(v);
+    *reinterpret_cast<__nv_bfloat16 *>(tile + bf_tile_off(row, k)) = vb;
+    if (DET) {
+      float sum = fabsf(__bfloat162float(vb));
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
+      rmax = max(rmax, abs_bits(sum));
+    }
+  }
+  if (DET && (threadIdx.x & 31) == 0) atomicMax(bnd + ks, rmax);
+}
+
+// dY [B][Cout][HWo] (fp32 or bf16) -> per (image, pixel tile, slice ks) one bf16 tile [128 px][32 k = output channel].
+// grid (tiles, KS, B); a thread rounds 16 output channels of one pixel into two 16-byte k-chunks.  DET: the bounds of
+// k_bwd_prep_gy, max |dY_b| and max |mask|.
+template <typename T, bool DET>
+__global__ void __launch_bounds__(256) k_bwd_prep_gy_bf16(const T *__restrict__ gy, const DcnShapeTc s, const BwdGeom g,
+                                                          unsigned char *__restrict__ gyt, const float *__restrict__ mask,
+                                                          unsigned *__restrict__ bnd_img) {
+  const int t = blockIdx.x, ks = blockIdx.y, b = blockIdx.z;
+  const int pp = threadIdx.x & (TC_TP - 1), half = threadIdx.x >> 7;
+  const int ho = (t / s.tiles_x) * s.th + pp / s.tw, wo = (t % s.tiles_x) * s.tw + pp % s.tw;
+  const bool ok = ho < s.Ho && wo < s.Wo;
+  const long long HWo = (long long)s.Ho * s.Wo, p = (long long)ho * s.Wo + wo;
+  unsigned char *tile = gyt + ((size_t)((size_t)b * g.tiles + t) * g.KS + ks) * BB_TILE_BYTES;
+  unsigned ymax = 0;
+#pragma unroll
+  for (int kc = 0; kc < 2; ++kc) {
+    const int k0 = half * 16 + kc * 8;
+    uint32_t r[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int o = ks * TC_K + k0 + 2 * j;
+      const float v0 = (ok && o < s.Cout) ? ld_f32(gy + ((long long)b * s.Cout + o) * HWo + p) : 0.f;
+      const float v1 = (ok && o + 1 < s.Cout) ? ld_f32(gy + ((long long)b * s.Cout + o + 1) * HWo + p) : 0.f;
+      const __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1);   // v0 at the lower address
+      r[j] = *reinterpret_cast<const uint32_t *>(&h);
+      if (DET) ymax = max(ymax, max(abs_bits(__low2float(h)), abs_bits(__high2float(h))));
+    }
+    *reinterpret_cast<uint4 *>(tile + bf_tile_off(pp, k0)) = make_uint4(r[0], r[1], r[2], r[3]);
+  }
+  if (DET) {
+    unsigned mmax = 0;
+    if (ks == 0 && ok) {
+      const float *mp = mask + (long long)b * s.mask_bs + p;
+      for (int c = half; c < s.dg * s.kh * s.kw; c += 2) mmax = max(mmax, abs_bits(__ldg(mp + (long long)c * HWo)));
+    }
+    ymax = warp_max_u32(ymax);
+    mmax = warp_max_u32(mmax);
+    if ((threadIdx.x & 31) == 0) {
+      atomicMax(bnd_img + 2 * b, ymax);
+      if (mmax) atomicMax(bnd_img + 2 * b + 1, mmax);
+    }
+  }
+}
+
+// dcol = dY_b^T . W_b: k_dcn_bwd_dcol_tc with a 16 KB stage (one bf16 tile each of dY and W) and two k16 steps a slice
+__global__ void __launch_bounds__(BW_THREADS, 1)
+k_dcn_bwd_dcol_bf16(const unsigned char *__restrict__ gyt, const unsigned char *__restrict__ wtb,
+                    float *__restrict__ dcol, const DcnShapeTc s, const BwdGeom g, const int n_items) {
+  extern __shared__ __align__(128) unsigned char tc_smem[];
+  __shared__ __align__(8) uint64_t full[BB_STAGES], empty[BB_STAGES];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    for (int i = 0; i < BB_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TC_MMA_WGS); }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp == TC_WARP_TMA) {
+    if (lane == 0) {
+      int stage = 0, ph = 0;
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const int rg = item % g.RG, bt = item / g.RG;          // bt = image * tiles + tile
+        for (int ks = 0; ks < g.KS; ++ks) {
+          mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
+          unsigned char *dst = tc_smem + (size_t)stage * BB_STAGE_BYTES;
+          mbar_expect_tx(&full[stage], (uint32_t)BB_STAGE_BYTES);
+          bulk_g2s(dst, gyt + ((size_t)bt * g.KS + ks) * BB_TILE_BYTES, (uint32_t)BB_TILE_BYTES, &full[stage]);
+          bulk_g2s(dst + BB_TILE_BYTES, wtb + ((size_t)rg * g.KS + ks) * BB_TILE_BYTES, (uint32_t)BB_TILE_BYTES,
+                   &full[stage]);
+          if (++stage == BB_STAGES) { stage = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else if (warp < TC_WARP_TMA) {
+    // consumers and epilogue as k_dcn_bwd_dcol_tc: warpgroup wgi owns pixels 64 wgi .. 64 wgi + 63 of the tile
+    const int wgi = warp >> 2, wq = warp & 3;
+    const long long HWo = (long long)s.Ho * s.Wo;
+    int stage = 0, ph = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int rg = item % g.RG, bt = item / g.RG;
+      const int t = bt % g.tiles, b = bt / g.tiles;
+      const int ty0 = (t / s.tiles_x) * s.th, tx0 = (t % s.tiles_x) * s.tw;
+      float d[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) d[i] = 0.f;
+      for (int ks = 0; ks < g.KS; ++ks) {
+        mbar_wait(&full[stage], (uint32_t)ph);
+        const uint32_t base = smem_u32(tc_smem + (size_t)stage * BB_STAGE_BYTES);
+        const uint32_t a = base + (uint32_t)wgi * 8u * BF_B_SBO, bw = base + (uint32_t)BB_TILE_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < TC_K / 16; ++kk) {   // one k16 step = two 16-byte k-chunks
+          const uint32_t koff = (uint32_t)kk * 2u * BF_B_LBO;
+          wgmma_bf16<128>(d, wg_desc(a + koff, BF_B_LBO, BF_B_SBO), wg_desc(bw + koff, BF_B_LBO, BF_B_SBO),
+                          (ks > 0 || kk > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        if ((tid & 127) == 0) mbar_arrive_tc(&empty[stage]);
+        if (++stage == BB_STAGES) { stage = 0; ph ^= 1; }
+      }
+      float *dimg = dcol + (long long)b * HWo * g.Qp * TC_CB + (long long)rg * 4 * TC_CB + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int pp = wgi * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        const int ho = ty0 + pp / s.tw, wo = tx0 + pp % s.tw;
+        if (ho >= s.Ho || wo >= s.Wo) continue;
+        float *dp = dimg + ((long long)ho * s.Wo + wo) * g.Qp * TC_CB;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) *reinterpret_cast<float2 *>(dp + 8 * j) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+      }
+    }
+  }
+}
+
+// dY (fp32 or bf16) -> per (image, 32-pixel slice) one bf16 tile [co_r rows = output channel][32 k = pixel]; the bias
+// partials bpart exactly as k_bwd_prep_gyk makes them (the same values, lanes and shuffle order).  grid (spi, B)
+template <typename T>
+__global__ void __launch_bounds__(256) k_bwd_prep_gyk_bf16(const T *__restrict__ gy, const DcnShapeTc s,
+                                                           const WgGeom wg, unsigned char *__restrict__ gyk,
+                                                           float *__restrict__ bpart) {
+  const int sl = blockIdx.x, b = blockIdx.y;
+  const long long HWo = (long long)s.Ho * s.Wo, p0 = (long long)sl * TC_K;
+  unsigned char *tile = gyk + ((size_t)b * wg.spi + sl) * wg.co_r * TC_K * 2;
+  for (int i = threadIdx.x; i < wg.co_r * TC_K; i += blockDim.x) {
+    const int k = i & (TC_K - 1), o = i >> 5;
+    const float v = (o < s.Cout && p0 + k < HWo) ? ld_f32(gy + ((long long)b * s.Cout + o) * HWo + p0 + k) : 0.f;
+    *reinterpret_cast<__nv_bfloat16 *>(tile + bf_tile_off(o, k)) = __float2bfloat16_rn(v);
+    if (bpart) {
+      float sum = v;
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
+      if (k == 0) bpart[((size_t)b * wg.spi + sl) * wg.co_r + o] = sum;
+    }
+  }
+}
+
+// The geometry warps of the bf16 weight pass: the producer loop of k_dcn_bwd_weight_tc (which keeps it inline -- called
+// through this function, that kernel's registers are allocated differently), 4 taps x 32 pixels of a slice, one entry
+// per thread, WG_MR slices ahead of the samplers
+__device__ __forceinline__ void wg_geometry(const DcnShapeTc &s, const BwdGeom &g, const WgGeom &wg, int rg, int sl0,
+                                            int sl1, const float *__restrict__ offset, const float *__restrict__ mask,
+                                            int st, BwdMetaTc (*wmeta)[128], uint64_t *m_full, uint64_t *m_empty) {
+  const int KT = s.kh * s.kw, lane = st & 31;
+  const long long HWo = (long long)s.Ho * s.Wo;
+  const int m_q = rg * 4 + (st >> 5);
+  const int m_bi = m_q / TC_NT, m_tap = m_q < g.Q ? m_q - m_bi * TC_NT : TC_NT;     // TC_NT = "no such tap"
+  const int m_gi = m_bi / s.cbs_pg;
+  const bool m_ok = m_tap < KT;
+  const int ki = m_ok ? m_tap / s.kw : 0, kj = m_tap - ki * s.kw;
+  const int hb = ki * s.dh - s.ph, wb = kj * s.dw - s.pw;
+  const long long o_dy = ((long long)m_gi * 2 * KT + 2 * (m_ok ? m_tap : 0)) * HWo;
+  const long long o_m = ((long long)m_gi * KT + (m_ok ? m_tap : 0)) * HWo;
+  const int HWo_i = (int)HWo;
+  int b = sl0 / wg.spi, sll = sl0 - b * wg.spi;
+  float dy = 0.f, dx = 0.f, mk = 0.f;
+  auto fetch = [&](int bb, int sl_local) {
+    const int p = sl_local * TC_K + lane;
+    dy = dx = mk = 0.f;
+    if (m_ok && p < HWo_i) {
+      const float *op = offset + (long long)bb * s.off_bs + o_dy + p;
+      dy = __ldg(op);
+      dx = __ldg(op + HWo);
+      mk = __ldg(mask + (long long)bb * s.mask_bs + o_m + p);
+    }
+  };
+  if (sl0 < sl1) fetch(b, sll);
+  int ms = 0, mph = 0;
+  for (int sl = sl0; sl < sl1; ++sl) {
+    const float cdy = dy, cdx = dx, cm = mk;
+    const int p = sll * TC_K + lane;
+    int nb_ = b, nsl = sll + 1;
+    if (nsl == wg.spi) { nsl = 0; ++nb_; }
+    if (sl + 1 < sl1) fetch(nb_, nsl);
+    BwdMetaTc mt;
+    mt.lh = mt.lw = mt.m = 0.f;
+    mt.packed = 0;
+    if (m_ok && p < HWo_i) {
+      const int ho = wg.wo_magic ? (int)__umulhi((unsigned)p, wg.wo_magic) : p / s.Wo;
+      const int wo = p - ho * s.Wo;
+      const float h_im = (float)(ho * s.sh + hb) + cdy, w_im = (float)(wo * s.sw + wb) + cdx;
+      if (h_im > -1.f && w_im > -1.f && h_im < (float)s.H && w_im < (float)s.W) {
+        const float hf = floorf(h_im), wf = floorf(w_im);
+        const int hl = (int)hf, wl = (int)wf;
+        int flags = 16;
+        if (hl >= 0 && wl >= 0) flags |= 1;
+        if (hl >= 0 && wl + 1 <= s.W - 1) flags |= 2;
+        if (hl + 1 <= s.H - 1 && wl >= 0) flags |= 4;
+        if (hl + 1 <= s.H - 1 && wl + 1 <= s.W - 1) flags |= 8;
+        mt.lh = h_im - hf;
+        mt.lw = w_im - wf;
+        mt.m = cm;
+        mt.packed = ((hl * s.W + wl + s.W + 1) << 7) | flags;
+      }
+    }
+    mbar_wait(&m_empty[ms], (uint32_t)(mph ^ 1));
+    wmeta[ms][st] = mt;
+    __syncwarp();
+    if (lane == 0) mbar_arrive_tc(&m_full[ms]);
+    if (++ms == WG_MR) { ms = 0; mph ^= 1; }
+    b = nb_;
+    sll = nsl;
+  }
+}
+
+// dW = dY_b . bf16(col)^T: the warp roles, work split and epilogue of k_dcn_bwd_weight_tc.  The samplers round each
+// interpolated value once to bf16 and store it as a 2-byte scalar into the K-major A tile [128 rows = channels][32 k =
+// pixels]; its 8-row groups are pitched WB_SBO = 528 bytes so that the 32 lanes of a store (4 pixels x 8 channel
+// quads) hit 16 different 4-byte words, two lanes each (DESIGN 4.4.3).  The B tile (NT rows of the slice's dY tile) is
+// dense and arrives by TMA.
+template <int NT>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+k_dcn_bwd_weight_bf16(const float *__restrict__ xt, const float *__restrict__ offset, const float *__restrict__ mask,
+                      const unsigned char *__restrict__ gyk, float *__restrict__ wpart, const DcnShapeTc s,
+                      const BwdGeom g, const WgGeom wg) {
+  constexpr int B_BYTES = NT * TC_K * 2;
+  constexpr int STAGE_BYTES = WB_A_BYTES + B_BYTES;
+  extern __shared__ __align__(128) unsigned char tc_smem[];
+  __shared__ __align__(8) uint64_t a_full[WB_STAGES], b_full[WB_STAGES], empty[WB_STAGES], m_full[WG_MR], m_empty[WG_MR];
+  __shared__ BwdMetaTc wmeta[WG_MR][128];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int rg = blockIdx.x % g.RG, nti = (blockIdx.x / g.RG) % wg.n_nt, split = blockIdx.x / g.RG / wg.n_nt;
+  const int sl0 = (int)((long long)split * wg.n_slices / wg.splits), sl1 = (int)((long long)(split + 1) * wg.n_slices / wg.splits);
+  const long long HW = (long long)s.H * s.W;
+  const int Cp = s.nb * TC_CB;
+
+  if (tid == 0) {
+    for (int i = 0; i < WB_STAGES; ++i) {
+      mbar_init(&a_full[i], WG_SAMPLERS);
+      mbar_init(&b_full[i], 1);
+      mbar_init(&empty[i], TC_MMA_WGS);
+    }
+    for (int i = 0; i < WG_MR; ++i) { mbar_init(&m_full[i], WG_GEOM); mbar_init(&m_empty[i], WG_SAMPLERS); }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= WG_WARP_S0) {
+    // =========================================================== samplers: task = (chunk ql, 4 pixels), lane = (pixel j,
+    // channel quad c4), as in k_dcn_bwd_weight_tc
+    const int sw = warp - WG_WARP_S0;
+    const int j = lane >> 3, c4 = lane & 7;
+    int t_meta[WG_TASKS], t_xc[WG_TASKS];
+    uint32_t t_dst[WG_TASKS];
+#pragma unroll
+    for (int it = 0; it < WG_TASKS; ++it) {
+      const int task = sw + it * WG_SAMPLERS;
+      const int ql = task >> 3, pg = task & 7;
+      const int q = rg * 4 + ql;
+      const int bi = q < g.Q ? q / TC_NT : 0;
+      t_meta[it] = ql * 32 + pg * 4 + j;
+      t_xc[it] = bi * TC_CB + c4 * 4;
+      const int row = ql * 32 + c4 * 4, k = pg * 4 + j;     // + i for channel i < 4: the next 16 bytes, same row group
+      t_dst[it] = (uint32_t)(row >> 3) * WB_SBO + (uint32_t)(k >> 3) * BF_B_LBO + (uint32_t)(row & 7) * 16u +
+                  (uint32_t)(k & 7) * 2u;
+    }
+    const int xs1 = Cp, xs2 = s.W * Cp, xs3 = (s.W + 1) * Cp;
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    int stage = 0, ph = 0, ms = 0, mph = 0;
+    int b = sl0 / wg.spi, sll = sl0 - b * wg.spi;
+    const size_t tile_bytes = (size_t)wg.co_r * TC_K * 2;          // one dY tile, all output channels
+    for (int sl = sl0; sl < sl1; ++sl) {
+      mbar_wait(&m_full[ms], (uint32_t)mph);
+      BwdMetaTc mt[WG_TASKS];
+#pragma unroll
+      for (int it = 0; it < WG_TASKS; ++it) mt[it] = wmeta[ms][t_meta[it]];
+      __syncwarp();
+      if (lane == 0) mbar_arrive_tc(&m_empty[ms]);
+      if (++ms == WG_MR) { ms = 0; mph ^= 1; }
+      const float *x_img = xt + (long long)b * HW * Cp;
+      unsigned char *a = tc_smem + (size_t)stage * STAGE_BYTES;
+#pragma unroll
+      for (int r = 0; r < WG_TASKS; r += 2) {
+        float4 xc[2][4];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int flags = mt[r + u].packed;
+          const int xo = ((flags >> 7) - (s.W + 1)) * Cp + t_xc[r + u];
+          xc[u][0] = (flags & 1) ? __ldg(reinterpret_cast<const float4 *>(x_img + xo)) : z4;
+          xc[u][1] = (flags & 2) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs1))) : z4;
+          xc[u][2] = (flags & 4) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs2))) : z4;
+          xc[u][3] = (flags & 8) ? __ldg(reinterpret_cast<const float4 *>(x_img + (xo + xs3))) : z4;
+        }
+        if (r == 0) {
+          mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
+          if (sw == 0 && lane == 0) {
+            // B operand: rows nti*NT .. nti*NT + NT - 1 of the slice's dY tile (contiguous 8-row groups)
+            mbar_expect_tx(&b_full[stage], (uint32_t)B_BYTES);
+            bulk_g2s(a + WB_A_BYTES, gyk + (size_t)sl * tile_bytes + (size_t)nti * B_BYTES, (uint32_t)B_BYTES,
+                     &b_full[stage]);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const BwdMetaTc &m = mt[r + u];
+          const float lh = m.lh, lw = m.lw, mm = m.m, hh = 1.f - lh, hw = 1.f - lw;
+          const float w1 = hh * hw * mm, w2 = hh * lw * mm, w3 = lh * hw * mm, w4 = lh * lw * mm;   // as the forward sampler
+          const float4 x1 = xc[u][0], x2 = xc[u][1], x3 = xc[u][2], x4 = xc[u][3];
+          __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(a + t_dst[r + u]);
+          dst[0] = __float2bfloat16_rn(fmaf(w4, x4.x, fmaf(w3, x3.x, fmaf(w2, x2.x, w1 * x1.x))));
+          dst[8] = __float2bfloat16_rn(fmaf(w4, x4.y, fmaf(w3, x3.y, fmaf(w2, x2.y, w1 * x1.y))));    // rows c4*4 + 0..3:
+          dst[16] = __float2bfloat16_rn(fmaf(w4, x4.z, fmaf(w3, x3.z, fmaf(w2, x2.z, w1 * x1.z))));   // 16 bytes apart
+          dst[24] = __float2bfloat16_rn(fmaf(w4, x4.w, fmaf(w3, x3.w, fmaf(w2, x2.w, w1 * x1.w))));
+        }
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      __syncwarp();
+      if (lane == 0) mbar_arrive_tc(&a_full[stage]);
+      if (++stage == WB_STAGES) { stage = 0; ph ^= 1; }
+      if (++sll == wg.spi) { sll = 0; ++b; }
+    }
+  } else if (warp >= WG_WARP_C0) {
+    // =========================================================== consumers: warpgroup cw accumulates rows 64 cw .. 64 cw + 63
+    const int cw = (warp - WG_WARP_C0) >> 2, wq = warp & 3;
+    float d[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) d[i] = 0.f;
+    int stage = 0, ph = 0;
+    for (int sl = sl0; sl < sl1; ++sl) {
+      mbar_wait(&a_full[stage], (uint32_t)ph);
+      mbar_wait(&b_full[stage], (uint32_t)ph);
+      const uint32_t base = smem_u32(tc_smem + (size_t)stage * STAGE_BYTES);
+      const uint32_t a = base + (uint32_t)cw * 8u * WB_SBO, bw = base + (uint32_t)WB_A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < TC_K / 16; ++kk) {
+        const uint32_t koff = (uint32_t)kk * 2u * BF_B_LBO;
+        wgmma_bf16<NT>(d, wg_desc(a + koff, BF_B_LBO, WB_SBO), wg_desc(bw + koff, BF_B_LBO, BF_B_SBO),
+                       (sl > sl0 || kk > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+      if (((tid - WG_WARP_C0 * 32) & 127) == 0) mbar_arrive_tc(&empty[stage]);
+      if (++stage == WB_STAGES) { stage = 0; ph ^= 1; }
+    }
+    // epilogue: wpart[split][rg][row][co_r], columns nti*NT .. nti*NT + NT - 1 (zeros for a CTA without slices)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      float *dst = wpart + (((size_t)split * g.RG + rg) * 128 + row) * wg.co_r + nti * NT + 2 * (lane & 3);
+#pragma unroll
+      for (int jj = 0; jj < NT / 8; ++jj)
+        *reinterpret_cast<float2 *>(dst + 8 * jj) = make_float2(d[4 * jj + 2 * h], d[4 * jj + 2 * h + 1]);
+    }
+  } else {
+    wg_geometry(s, g, wg, rg, sl0, sl1, offset, mask, tid, wmeta, m_full, m_empty);
+  }
+}
+
 // ------------------------------------------------------------------ host
 void plan_backward_tc(DcnPlan *p) {
   const DcnShapeTc &s = p->s;
@@ -993,6 +1391,172 @@ int dcn_backward_weight_tc(const DcnPlan &p, const float *input, const float *of
     k_dcn_bwd_bias_reduce<<<s.Cout, 256, 0, stream>>>(bpart, grad_bias, wg);
     CNB_CHECK_LAUNCH("cnb_dcnv2_backward bias gradient reduce");
     count_launch();
+  }
+  return CNB_OK;
+}
+
+// The bf16 backward's workspace: plan_backward_tc's regions with bf16 tiles.  It needs both tensor-core passes (the
+// weight pass covers cout <= 256): elsewhere bytes stays 0 and cnb_dcnv2_backward_bf16 returns CNB_EUNSUPPORTED.
+void plan_backward_bf16(DcnPlan *p) {
+  const DcnShapeTc &s = p->s;
+  p->bwd16 = {};
+  if (!p->bwd_tc || !p->dw_tc) return;
+  const BwdGeom g = bwd_geom(s);
+  const WgGeom wg = wg_geom(s, g);
+  const size_t gyt_img = (size_t)g.tiles * g.KS * BB_TILE_BYTES;
+  const size_t dcol_img = align_up((size_t)s.Ho * s.Wo * g.Qp * TC_CB * 4, 256);
+  long long bc = (long long)((1536ull << 20) / (dcol_img + gyt_img));   // as plan_backward_tc: ~1.5 GiB a pass
+  if (bc < 1) bc = 1;
+  if (bc > s.B) bc = s.B;
+  auto &l = p->bwd16;
+  l.chunk = (int)bc;
+  l.xt = 0;
+  l.dxt = l.xt + p->xt_bytes;
+  l.wtb = l.dxt + p->xt_bytes;
+  l.gyt = l.wtb + align_up((size_t)g.RG * g.KS * BB_TILE_BYTES, 256);
+  l.dcol = l.gyt + align_up((size_t)bc * gyt_img, 256);
+  const size_t data_end = l.dcol + (size_t)bc * dcol_img;
+  l.gyk = l.gyt;
+  l.wpart = l.gyk + align_up((size_t)wg.n_slices * wg.co_r * TC_K * 2, 256);
+  l.bpart = l.wpart + align_up((size_t)wg.splits * g.RG * 128 * wg.co_r * 4, 256);
+  const size_t weight_end = l.bpart + align_up((size_t)wg.n_slices * wg.co_r * 4, 256);
+  const size_t end = std::max(data_end, weight_end);
+  l.bnd = end;
+  l.dxi = l.bnd + align_up((size_t)(g.KS + 2 * s.B) * 4, 256);
+  l.bytes = p->det ? l.dxi + align_up((size_t)bc * s.H * s.W * s.nb * TC_CB * 8, 256) : end;
+}
+
+int dcn_backward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
+                      const float *weight, const void *grad_output, bool gy_bf16, float *grad_input, float *grad_offset,
+                      float *grad_mask, float *grad_weight, float *grad_bias, void *workspace, cudaStream_t stream) {
+  const DcnShapeTc &s = p.s;
+  const BwdGeom g = bwd_geom(s);
+  const WgGeom wg = wg_geom(s, g);
+  const auto &l = p.bwd16;
+  const int b = s.B, cin = s.Cin, bc = l.chunk;
+  const long long HW = (long long)s.H * s.W, HWo = (long long)s.Ho * s.Wo;
+  char *ws = reinterpret_cast<char *>(workspace);
+  float *xt = reinterpret_cast<float *>(ws + l.xt);
+  const float *gy32 = reinterpret_cast<const float *>(grad_output);
+  const __nv_bfloat16 *gy16 = reinterpret_cast<const __nv_bfloat16 *>(grad_output);
+  const bool data = grad_input || grad_offset || grad_mask;
+  int rc = CNB_OK;
+  // the samplers read an fp32 channels-last input: an fp32 channels-last one in place, else the copy xt
+  const float *xsrc = xt;
+  if (data || grad_weight) {
+    if (in_bf16) rc = dcn_to_channels_last(reinterpret_cast<const __nv_bfloat16 *>(input), p.x_cl, xt, s, stream);
+    else if (p.x_cl) xsrc = reinterpret_cast<const float *>(input);
+    else rc = dcn_to_channels_last(reinterpret_cast<const float *>(input), xt, s, stream);
+    if (rc != CNB_OK) return rc;
+  }
+
+  if (data) {
+    // the data pass of dcn_backward_data_tc with bf16 operand tiles and k_dcn_bwd_dcol_bf16
+    float *dxt = p.gx_cl ? grad_input : reinterpret_cast<float *>(ws + l.dxt);
+    unsigned char *wtb = reinterpret_cast<unsigned char *>(ws + l.wtb);
+    unsigned char *gyt = reinterpret_cast<unsigned char *>(ws + l.gyt);
+    float *dcol = reinterpret_cast<float *>(ws + l.dcol);
+    const bool det = grad_input && p.det;
+    unsigned *bnd = nullptr;
+    long long *dxi = nullptr;
+    if (det) {
+      bnd = reinterpret_cast<unsigned *>(ws + l.bnd);
+      dxi = reinterpret_cast<long long *>(ws + l.dxi);
+      CNB_CUDA(cudaMemsetAsync(bnd, 0, (size_t)(g.KS + 2 * b) * 4, stream));
+    }
+    if (grad_input && !det && !p.gx_cl) CNB_CUDA(cudaMemsetAsync(dxt, 0, (size_t)b * HW * s.nb * TC_CB * 4, stream));
+    if (det) k_bwd_prep_w_bf16<true><<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtb, bnd);
+    else k_bwd_prep_w_bf16<false><<<g.RG * g.KS, 256, 0, stream>>>(weight, s, g, wtb, nullptr);
+    CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 weight tiles");
+    count_launch();
+    const size_t smem = (size_t)BB_STAGES * BB_STAGE_BYTES;
+    static thread_local int dev_done = -1;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev_done != dev) {
+      CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_dcol_bf16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      dev_done = dev;
+    }
+    for (int b0 = 0; b0 < b; b0 += bc) {
+      const int nbimg = (b - b0 < bc) ? b - b0 : bc;
+      const dim3 pgrid((unsigned)g.tiles, (unsigned)g.KS, (unsigned)nbimg);
+      const long long go = (long long)b0 * s.Cout * HWo;
+      if (det) {
+        CNB_CUDA(cudaMemsetAsync(dxi, 0, (size_t)nbimg * HW * s.nb * TC_CB * 8, stream));
+        const float *mk = mask + (long long)b0 * s.mask_bs;
+        if (gy_bf16) k_bwd_prep_gy_bf16<__nv_bfloat16, true><<<pgrid, 256, 0, stream>>>(gy16 + go, s, g, gyt, mk, bnd + g.KS + 2 * b0);
+        else k_bwd_prep_gy_bf16<float, true><<<pgrid, 256, 0, stream>>>(gy32 + go, s, g, gyt, mk, bnd + g.KS + 2 * b0);
+      } else {
+        if (gy_bf16) k_bwd_prep_gy_bf16<__nv_bfloat16, false><<<pgrid, 256, 0, stream>>>(gy16 + go, s, g, gyt, nullptr, nullptr);
+        else k_bwd_prep_gy_bf16<float, false><<<pgrid, 256, 0, stream>>>(gy32 + go, s, g, gyt, nullptr, nullptr);
+      }
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 grad_output tiles");
+      const int n_items = nbimg * g.tiles * g.RG;
+      const int grid = n_items < num_sms() ? n_items : num_sms();
+      k_dcn_bwd_dcol_bf16<<<grid, BW_THREADS, smem, stream>>>(gyt, wtb, dcol, s, g, n_items);
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 column gradient (wgmma bf16)");
+      k_dcn_bwd_offmask<3><<<nbimg * g.tiles, 256, 0, stream>>>(xsrc, offset, mask, dcol, (grad_input && !det) ? dxt : nullptr,
+                                                                grad_offset, grad_mask, dxi, bnd, s, g, b0);
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 offset/mask gradient");
+      count_launch(3);
+      if (det) {
+        if (p.gx_cl) {
+          k_dcn_bwd_dx_fixed<true><<<dim3((unsigned)((HW + 31) / 32), 1u, (unsigned)nbimg), 256, 0, stream>>>(
+              dxi, bnd, grad_input, s, g, b0);
+        } else {
+          dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((cin + 63) / 64), (unsigned)nbimg);
+          k_dcn_bwd_dx_fixed<false><<<tgrid, 256, 0, stream>>>(dxi, bnd, grad_input, s, g, b0);
+        }
+        CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 input gradient (fixed point)");
+        count_launch();
+      }
+    }
+    if (grad_input && !det && !p.gx_cl) {
+      dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((cin + 63) / 64), (unsigned)b);
+      k_dcn_bwd_dx_nchw<<<tgrid, 256, 0, stream>>>(dxt, grad_input, s);
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 input gradient");
+      count_launch();
+    }
+  }
+
+  if (grad_weight || grad_bias) {
+    // the weight pass of dcn_backward_weight_tc; the bias partials come from the same grad_output pass either way
+    unsigned char *gyk = reinterpret_cast<unsigned char *>(ws + l.gyk);
+    float *wpart = reinterpret_cast<float *>(ws + l.wpart);
+    float *bpart = grad_bias ? reinterpret_cast<float *>(ws + l.bpart) : nullptr;
+    const dim3 pgrid((unsigned)wg.spi, (unsigned)b);
+    if (gy_bf16) k_bwd_prep_gyk_bf16<__nv_bfloat16><<<pgrid, 256, 0, stream>>>(gy16, s, wg, gyk, bpart);
+    else k_bwd_prep_gyk_bf16<float><<<pgrid, 256, 0, stream>>>(gy32, s, wg, gyk, bpart);
+    CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 grad_output tiles (weight pass)");
+    count_launch();
+    if (grad_weight) {
+      const size_t smem = (size_t)WB_STAGES * (WB_A_BYTES + wg.nt * TC_K * 2);
+      static thread_local int dev_done = -1;
+      int dev = 0;
+      cudaGetDevice(&dev);
+      if (dev_done != dev) {
+        CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight_bf16<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      WB_STAGES * (WB_A_BYTES + 64 * TC_K * 2)));
+        CNB_CUDA(cudaFuncSetAttribute(k_dcn_bwd_weight_bf16<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      WB_STAGES * (WB_A_BYTES + 128 * TC_K * 2)));
+        dev_done = dev;
+      }
+      const unsigned wgrid = (unsigned)(g.RG * wg.n_nt * wg.splits);
+      if (wg.nt == 64)
+        k_dcn_bwd_weight_bf16<64><<<wgrid, WG_THREADS, smem, stream>>>(xsrc, offset, mask, gyk, wpart, s, g, wg);
+      else
+        k_dcn_bwd_weight_bf16<128><<<wgrid, WG_THREADS, smem, stream>>>(xsrc, offset, mask, gyk, wpart, s, g, wg);
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 weight gradient (wgmma bf16)");
+      const long long total = (long long)g.RG * 128 * wg.co_r;
+      k_dcn_bwd_wreduce<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(wpart, grad_weight, s, g, wg);
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 weight gradient reduce");
+      count_launch(2);
+    }
+    if (grad_bias) {
+      k_dcn_bwd_bias_reduce<<<s.Cout, 256, 0, stream>>>(bpart, grad_bias, wg);
+      CNB_CHECK_LAUNCH("cnb_dcnv2_backward_bf16 bias gradient reduce");
+      count_launch();
+    }
   }
   return CNB_OK;
 }

@@ -344,10 +344,6 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
 // rounded once (RN) by k_dcn_prep_weights_bf16; the contraction accumulates in fp32, split-K partials are added in
 // split order, bias / BN / ReLU are applied in fp32 and the result is stored as fp32 or rounded (RN) to bf16.
 
-__device__ __forceinline__ uint32_t bf_tile_off(int row, int k) {   // byte offset of (row, k) in a dense bf16 tile
-  return (uint32_t)(row >> 3) * BF_B_SBO + (uint32_t)(k >> 3) * BF_B_LBO + (uint32_t)(row & 7) * 16u +
-         (uint32_t)(k & 7) * 2u;
-}
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {   // lo -> lower address (smaller k)
   const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<const uint32_t *>(&v);
@@ -415,6 +411,47 @@ __global__ void __launch_bounds__(256) k_dcn_cl_to_bf16(const float4 *__restrict
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
     const float4 a = __ldg(x + 2 * i), b = __ldg(x + 2 * i + 1);
     xt[i] = make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(b.x, b.y), pack_bf16x2(b.z, b.w));
+  }
+}
+
+// bf16 x [B][Cin][HW] -> fp32 xt [B][HW][nb][32] (exact widening): k_dcn_nhwc reading bf16, for the bf16 backward
+__global__ void __launch_bounds__(256) k_dcn_nhwc_widen(const __nv_bfloat16 *__restrict__ x, float *__restrict__ xt,
+                                                        const DcnShapeTc s) {
+  __shared__ float tile[64][33];
+  const long long HW = (long long)s.H * s.W;
+  const long long p0 = (long long)blockIdx.x * 32;
+  const int c0 = blockIdx.y * 64, b = blockIdx.z;
+  const int Cp = s.nb * TC_CB;
+  const int cpg = s.Cin / s.dg;
+  {
+    const int px = threadIdx.x & 31, cr = threadIdx.x >> 5;
+    for (int c = cr; c < 64; c += 8) {
+      float v = 0.f;
+      if (c0 + c < s.Cin && p0 + px < HW) v = load_in(x + ((long long)b * s.Cin + c0 + c) * HW + p0 + px);
+      tile[c][px] = v;
+    }
+  }
+  __syncthreads();
+  {
+    const int c = threadIdx.x & 63, pr = threadIdx.x >> 6;
+    const int ch = c0 + c;
+    if (ch < s.Cin) {
+      const int g = ch / cpg, within = ch - g * cpg;
+      const int slot = (g * s.cbs_pg + within / TC_CB) * TC_CB + within % TC_CB;
+      for (int px = pr; px < 32; px += 4)
+        if (p0 + px < HW) xt[((long long)b * HW + p0 + px) * Cp + slot] = tile[c][px];
+    }
+  }
+}
+
+// bf16 channels-last [B][HW][Cin] with whole 32-channel blocks (slot == channel) -> fp32 xt, 8 values a thread
+__global__ void __launch_bounds__(256) k_dcn_cl_widen(const uint4 *__restrict__ x, float4 *__restrict__ xt, long long n8) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 u = __ldg(x + i);
+    xt[2 * i] = make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                            __uint_as_float(u.y & 0xffff0000u));
+    xt[2 * i + 1] = make_float4(__uint_as_float(u.z << 16), __uint_as_float(u.z & 0xffff0000u),
+                                __uint_as_float(u.w << 16), __uint_as_float(u.w & 0xffff0000u));
   }
 }
 
@@ -732,6 +769,25 @@ int dcn_to_channels_last(const float *x, float *xt, const DcnShapeTc &s, cudaStr
   dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((s.Cin + 63) / 64), (unsigned)s.B);
   k_dcn_nhwc<<<tgrid, 256, 0, stream>>>(x, xt, s);
   CNB_CHECK_LAUNCH("cnb_dcnv2 channels-last copy");
+  count_launch();
+  return CNB_OK;
+}
+
+int dcn_to_channels_last(const __nv_bfloat16 *x, bool x_cl, float *xt, const DcnShapeTc &s, cudaStream_t stream) {
+  const long long HW = (long long)s.H * s.W;
+  if (x_cl) {
+    const long long n8 = (long long)s.B * HW * s.Cin / 8;
+    const int grid = (int)((n8 + 255) / 256 < 4096 ? (n8 + 255) / 256 : 4096);
+    k_dcn_cl_widen<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint4 *>(x), reinterpret_cast<float4 *>(xt), n8);
+    CNB_CHECK_LAUNCH("cnb_dcnv2 channels-last fp32 copy of a bf16 input");
+    count_launch();
+    return CNB_OK;
+  }
+  if ((s.Cin / s.dg) % TC_CB != 0)
+    CNB_CUDA(cudaMemsetAsync(xt, 0, (size_t)s.B * HW * s.nb * TC_CB * 4, stream));
+  dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((s.Cin + 63) / 64), (unsigned)s.B);
+  k_dcn_nhwc_widen<<<tgrid, 256, 0, stream>>>(x, xt, s);
+  CNB_CHECK_LAUNCH("cnb_dcnv2 channels-last fp32 copy of a bf16 input");
   count_launch();
   return CNB_OK;
 }

@@ -1,6 +1,7 @@
 // Shared by the wgmma DCNv2 kernels (dcnv2_tc.cu: forward, dcnv2_bwd_tc.cu: backward): the shared-memory tile
 // layout (K-major, no swizzle), the wgmma descriptor and instruction wrappers and the shape / work decomposition.
 #pragma once
+#include <cuda_bf16.h>
 #include "common.cuh"
 
 namespace cnb {
@@ -59,6 +60,10 @@ struct __align__(16) TapMetaTc {
 
 __device__ __forceinline__ uint32_t tc_tile_off(int row, int k) {  // byte offset of element (row, k) in a K-major tile
   return (uint32_t)(row >> 3) * TC_SBO + (uint32_t)(k >> 2) * TC_LBO + (uint32_t)(row & 7) * 16u + (uint32_t)(k & 3) * 4u;
+}
+__device__ __forceinline__ uint32_t bf_tile_off(int row, int k) {   // byte offset of (row, k) in a dense bf16 tile
+  return (uint32_t)(row >> 3) * BF_B_SBO + (uint32_t)(k >> 3) * BF_B_LBO + (uint32_t)(row & 7) * 16u +
+         (uint32_t)(k & 7) * 2u;
 }
 // sm_90 shared-memory matrix descriptor: start address, leading (k-chunk) and stride (8-row group) byte offsets,
 // base offset 0, layout type 0 = no swizzle
@@ -228,12 +233,20 @@ struct DcnPlan {
     size_t xt, dxt, wtt, gyt, dcol, gyk, wpart, bpart, bnd, dxi, wpart32, bytes;
     int chunk;         // images per pass of the data pass
   } bwd;
+  struct {             // the bf16 backward's: the regions of bwd with one bf16 tile in place of each TF32 hi/lo pair
+                       // (wtb, gyt, gyk) and no wpart32; bytes == 0 where it does not run (!bwd_tc || !dw_tc)
+    size_t xt, dxt, wtb, gyt, dcol, gyk, wpart, bpart, bnd, dxi, bytes;
+    int chunk;
+  } bwd16;
 };
-void plan_forward_tc(DcnPlan *p);    // dcnv2_tc.cu: xt_bytes, fwd and bf16
-void plan_backward_tc(DcnPlan *p);   // dcnv2_bwd_tc.cu: bwd_tc, dw_tc and bwd (after plan_forward_tc)
+void plan_forward_tc(DcnPlan *p);     // dcnv2_tc.cu: xt_bytes, fwd and bf16
+void plan_backward_tc(DcnPlan *p);    // dcnv2_bwd_tc.cu: bwd_tc, dw_tc and bwd (after plan_forward_tc)
+void plan_backward_bf16(DcnPlan *p);  // dcnv2_bwd_tc.cu: bwd16 (after plan_backward_tc)
 
 // x [B][Cin][HW] -> channels-last copy xt [B][HW][nb][32] (dcnv2_tc.cu)
 int dcn_to_channels_last(const float *x, float *xt, const DcnShapeTc &s, cudaStream_t stream);
+// the same fp32 copy from a bf16 x (exact widening): NCHW, or x_cl: [B][HW][Cin] with whole 32-channel blocks
+int dcn_to_channels_last(const __nv_bfloat16 *x, bool x_cl, float *xt, const DcnShapeTc &s, cudaStream_t stream);
 int dcn_prepare_weights_tc(const float *weight, int cin, int cout, int kh, int kw, int dg, float *wtiles,
                            cudaStream_t stream);
 // Tensor-core forward from pre-tiled weights into the prepared forward's workspace (p.fwd).  fused_offset_mask:
@@ -257,5 +270,10 @@ int dcn_backward_data_tc(const DcnPlan &p, const float *input, const float *offs
 int dcn_backward_weight_tc(const DcnPlan &p, const float *input, const float *offset, const float *mask,
                            const float *grad_output, float *grad_weight, float *grad_bias, void *workspace,
                            cudaStream_t stream);
+// bf16 backward (dcnv2_bwd_tc.cu) into the workspace of p.bwd16: all five gradients (each nullable, fp32, accumulated
+// into).  in_bf16 / gy_bf16: input / grad_output are bf16 (else fp32); offset, mask and weight are fp32
+int dcn_backward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
+                      const float *weight, const void *grad_output, bool gy_bf16, float *grad_input, float *grad_offset,
+                      float *grad_mask, float *grad_weight, float *grad_bias, void *workspace, cudaStream_t stream);
 
 }  // namespace cnb

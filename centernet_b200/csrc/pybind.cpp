@@ -247,6 +247,17 @@ PYBIND11_MODULE(_C, m) {
                                 kh, kw, stride, pad, dil, dg, ptr<void>(ws), wsb, ptr<void>(stream)),
           "cnb_dcnv2_backward_ex");
   });
+  m.def("dcnv2_backward_bf16_workspace_bytes", &cnb_dcnv2_backward_bf16_workspace_bytes);
+  m.def("dcnv2_backward_bf16", [](P input, int in_dt, int in_cl, P offset, P mask, P weight, P gout, int gout_dt, P gin,
+                                  int gin_cl, P goff, P gmask, P gw, P gb, int b, int cin, int h, int w, int cout, int kh,
+                                  int kw, int stride, int pad, int dil, int dg, P ws, size_t wsb, P stream) {
+    check(cnb_dcnv2_backward_bf16(ptr<const void>(input), in_dt, in_cl, ptr<const float>(offset),
+                                  ptr<const float>(mask), ptr<const float>(weight), ptr<const void>(gout), gout_dt,
+                                  ptr<float>(gin), gin_cl, ptr<float>(goff), ptr<float>(gmask), ptr<float>(gw),
+                                  ptr<float>(gb), b, cin, h, w, cout, kh, kw, stride, pad, dil, dg, ptr<void>(ws), wsb,
+                                  ptr<void>(stream)),
+          "cnb_dcnv2_backward_bf16");
+  });
   m.def("dcnv2_set_deterministic", &cnb_dcnv2_set_deterministic);
   m.def("dcnv2_get_deterministic", &cnb_dcnv2_get_deterministic);
   m.def("dcnv2_forward", [](P input, P offset, P mask, P weight, P bias, P output, int b, int cin, int h, int w,

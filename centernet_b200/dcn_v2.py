@@ -7,16 +7,19 @@ import torch
 from torch import nn
 from torch.nn.modules.utils import _pair
 
-from .dcn_v2_func import DCNv2Function, DCNv2PoolingFunction, _check_compute_dtype, dcn_fused_inference
+from .dcn_v2_func import (DCNv2Function, DCNv2PoolingFunction, _check_backward_dtype, _check_compute_dtype,
+                          dcn_fused_inference)
 
 
 class DCNv2(nn.Module):
-    """dcn_v2.py:14-41.  compute_dtype=torch.bfloat16 opts this module into the bf16 forward (DCNv2Function)."""
+    """dcn_v2.py:14-41.  compute_dtype=torch.bfloat16 opts this module into the bf16 forward, and with it
+    backward_dtype=torch.bfloat16 into the bf16 backward (DCNv2Function)."""
 
     def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1,
-                 compute_dtype=None):
+                 compute_dtype=None, backward_dtype=None):
         super().__init__()
         self.compute_dtype = _check_compute_dtype(compute_dtype)
+        self.backward_dtype = _check_backward_dtype(compute_dtype, backward_dtype)
         self.in_channels = in_channels
         self.out_channels = out_channels
         self.kernel_size = _pair(kernel_size)
@@ -38,7 +41,7 @@ class DCNv2(nn.Module):
 
     def forward(self, input, offset, mask):
         func = DCNv2Function(self.stride, self.padding, self.dilation, self.deformable_groups,
-                             getattr(self, "compute_dtype", None))
+                             getattr(self, "compute_dtype", None), getattr(self, "backward_dtype", None))
         return func(input, offset, mask, self.weight, self.bias)
 
 
@@ -46,9 +49,9 @@ class DCN(DCNv2):
     """dcn_v2.py:44-70: DCNv2 + the zero-initialised offset/mask conv."""
 
     def __init__(self, in_channels, out_channels, kernel_size, stride, padding, dilation=1, deformable_groups=1,
-                 compute_dtype=None):
+                 compute_dtype=None, backward_dtype=None):
         super().__init__(in_channels, out_channels, kernel_size, stride, padding, dilation, deformable_groups,
-                         compute_dtype)
+                         compute_dtype, backward_dtype)
         self.conv_offset_mask = nn.Conv2d(self.in_channels,
                                           self.deformable_groups * 3 * self.kernel_size[0] * self.kernel_size[1],
                                           kernel_size=self.kernel_size, stride=(self.stride, self.stride),
@@ -72,7 +75,7 @@ class DCN(DCNv2):
         offset = torch.cat((o1, o2), dim=1)
         mask = torch.sigmoid(mask)
         func = DCNv2Function(self.stride, self.padding, self.dilation, self.deformable_groups,
-                             getattr(self, "compute_dtype", None))
+                             getattr(self, "compute_dtype", None), getattr(self, "backward_dtype", None))
         return func(input, offset, mask, self.weight, self.bias)
 
 
@@ -168,15 +171,18 @@ def fuse_dcn_bn_relu(model):
     return n
 
 
-def set_compute_dtype(model, dtype):
-    """Sets `compute_dtype` on every DCNv2 / DCN module of `model` (None: the default fp32-accurate forward;
-    torch.bfloat16: the bf16 forward) and returns how many it set.  The reference network code builds DCN(...)
-    without keywords; this turns the bf16 path on for such a model without touching its code.  Composes with
-    fuse_dcn_bn_relu in either order (the fused forward reads the attribute at call time)."""
+def set_compute_dtype(model, dtype, backward_dtype=None):
+    """Sets `compute_dtype` and `backward_dtype` on every DCNv2 / DCN module of `model` (None: the default
+    fp32-accurate forward; torch.bfloat16: the bf16 forward, and with backward_dtype=torch.bfloat16 the bf16 backward)
+    and returns how many it set.  The reference network code builds DCN(...) without keywords; this turns the bf16
+    path on for such a model without touching its code.  Composes with fuse_dcn_bn_relu in either order (the fused
+    forward reads the attribute at call time)."""
     _check_compute_dtype(dtype)
+    _check_backward_dtype(dtype, backward_dtype)
     n = 0
     for m in model.modules():
         if isinstance(m, DCNv2):
             m.compute_dtype = dtype
+            m.backward_dtype = backward_dtype
             n += 1
     return n

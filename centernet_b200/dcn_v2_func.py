@@ -226,6 +226,17 @@ def _check_compute_dtype(compute_dtype):
     return compute_dtype
 
 
+def _check_backward_dtype(compute_dtype, backward_dtype):
+    """backward_dtype=torch.bfloat16 (the bf16 backward) goes with compute_dtype=torch.bfloat16 only."""
+    if backward_dtype is None:
+        return None
+    if backward_dtype != torch.bfloat16 or compute_dtype != torch.bfloat16:
+        raise ValueError("backward_dtype must be None (the fp32 backward) or torch.bfloat16 together with "
+                         "compute_dtype=torch.bfloat16, got backward_dtype=%r with compute_dtype=%r"
+                         % (backward_dtype, compute_dtype))
+    return backward_dtype
+
+
 def _bf16_forward(what, input, offset, mask, offset_mask, weight, bias, stride, padding, dilation, dg,
                   bn_scale=None, bn_shift=None, relu=False):
     """One call of cnb_dcnv2_forward_bf16 (or, with offset_mask, cnb_dcnv2_forward_fused_bf16).  The output has the
@@ -274,11 +285,14 @@ def _bf16_forward(what, input, offset, mask, offset_mask, weight, bias, stride, 
 
 
 class _DCNv2BF16(Function):
-    """bf16 forward; the backward is the fp32 one evaluated at the operands the forward used (the bf16 activation and
-    weight, upcast exactly), each gradient returned in its input's dtype.  The activation is saved as bf16."""
+    """bf16 forward.  bf16_backward=False: the backward is the fp32 one evaluated at the operands the forward used (the
+    bf16 activation and weight, upcast exactly); True: the bf16 backward (cnb_dcnv2_backward_bf16) where it runs, that
+    fp32 one elsewhere (cout > 256).  Each gradient is returned in its input's dtype; the activation is saved as
+    bf16."""
 
     @staticmethod
-    def forward(ctx, input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups):
+    def forward(ctx, input, offset, mask, weight, bias, stride, padding, dilation, deformable_groups,
+                bf16_backward=False):
         out, off, msk = _bf16_forward("DCNv2", input, offset, mask, None, weight, bias, stride, padding, dilation,
                                       deformable_groups)
         if any(ctx.needs_input_grad[:5]):
@@ -286,6 +300,7 @@ class _DCNv2BF16(Function):
             ctx.save_for_backward(xb, off, msk, weight, bias)
         ctx.dtypes = tuple(None if t is None else t.dtype for t in (input, offset, mask, weight, bias))
         ctx.cfg = (stride, padding, dilation, deformable_groups)
+        ctx.bf16_backward = bool(bf16_backward)
         return out
 
     @staticmethod
@@ -293,11 +308,43 @@ class _DCNv2BF16(Function):
         if not grad_output.is_cuda:
             raise NotImplementedError
         xb, off, msk, weight, bias = ctx.saved_tensors
-        x = xb.float().contiguous()
-        w = weight.bfloat16().float().contiguous()
-        grads = _dcn_backward_f32(x, off, msk, w, f32c(bias), f32c(grad_output), ctx.cfg, False)
+        grads = _dcn_backward_bf16(xb, off, msk, weight, bias, grad_output, ctx.cfg) if ctx.bf16_backward else None
+        if grads is None:
+            x = xb.float().contiguous()
+            w = weight.bfloat16().float().contiguous()
+            grads = _dcn_backward_f32(x, off, msk, w, f32c(bias), f32c(grad_output), ctx.cfg, False)
         grads = tuple(None if g is None else g.to(dt) for g, dt in zip(grads, ctx.dtypes))
-        return grads + (None,) * 4
+        return grads + (None,) * 5
+
+
+def _dcn_backward_bf16(xb, off, msk, weight, bias, grad_output, cfg):
+    """One call of cnb_dcnv2_backward_bf16 on the saved bf16 activation: the five gradients in fp32, or None where
+    that backward does not run (the workspace query returns 0: cout > 256 or an image beyond its 32-bit indexing).
+    A channels_last activation with whole 32-channel blocks is read as it is and gets a channels_last grad_input."""
+    stride, padding, dilation, dg = cfg
+    n, cin, h, wd = [int(v) for v in xb.shape]
+    cout, _, kh, kw = [int(v) for v in weight.shape]
+    det = _deterministic()
+    C.dcnv2_set_deterministic(int(det))
+    wsb = C.dcnv2_backward_bf16_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding, dilation, dg)
+    if wsb == 0:
+        return None
+    cl = (cin // dg) % 32 == 0 and xb.is_contiguous(memory_format=torch.channels_last) and not xb.is_contiguous()
+    x = xb if cl else xb.contiguous()
+    if x.data_ptr() % 16:
+        x = x.clone()               # the kernels read 16-byte pieces (clone keeps the memory format)
+    go = grad_output if grad_output.dtype == torch.bfloat16 else grad_output.float()
+    go = go.contiguous()
+    w = f32c(weight)
+    gx = torch.zeros_like(x, dtype=torch.float32)     # keeps x's layout: channels_last when cl
+    goff, gmsk, gw = torch.zeros_like(off), torch.zeros_like(msk), torch.zeros_like(w)
+    gb = torch.zeros(cout, dtype=torch.float32, device=x.device) if bias is not None else None
+    ws = workspace(wsb, x.device)
+    C.dcnv2_backward_bf16(ptr(x), C.DTYPE_BF16, int(cl), ptr(off), ptr(msk), ptr(w), ptr(go),
+                          C.DTYPE_BF16 if go.dtype == torch.bfloat16 else C.DTYPE_F32, ptr(gx), int(cl), ptr(goff),
+                          ptr(gmsk), ptr(gw), ptr(gb), n, cin, h, wd, cout, kh, kw, stride, padding, dilation, dg,
+                          ptr(ws), ws.numel(), stream_ptr(x))
+    return gx, goff, gmsk, gw, gb
 
 
 def dcn_fused_inference(input, offset_mask, weight, bias, stride, padding, dilation, deformable_groups,
@@ -341,19 +388,24 @@ def dcn_fused_inference(input, offset_mask, weight, bias, stride, padding, dilat
 
 class DCNv2Function(object):
     """Callable instance, same constructor as the reference's old-style Function.  compute_dtype=torch.bfloat16
-    selects the bf16 forward (float32 or bfloat16 input, output in the input's dtype); None keeps the default."""
+    selects the bf16 forward (float32 or bfloat16 input, output in the input's dtype); None keeps the default.
+    backward_dtype=torch.bfloat16 (with compute_dtype=torch.bfloat16 only) selects the bf16 backward; None keeps the
+    fp32 backward at the operands the bf16 forward used."""
 
-    def __init__(self, stride, padding, dilation=1, deformable_groups=1, compute_dtype=None):
+    def __init__(self, stride, padding, dilation=1, deformable_groups=1, compute_dtype=None, backward_dtype=None):
         self.stride = stride
         self.padding = padding
         self.dilation = dilation
         self.deformable_groups = deformable_groups
         self.compute_dtype = _check_compute_dtype(compute_dtype)
+        self.backward_dtype = _check_backward_dtype(self.compute_dtype, backward_dtype)
 
     def __call__(self, input, offset, mask, weight, bias):
-        fn = _DCNv2BF16 if self.compute_dtype is not None else _DCNv2
-        return fn.apply(input, offset, mask, weight, bias, self.stride, self.padding, self.dilation,
-                        self.deformable_groups)
+        if self.compute_dtype is not None:
+            return _DCNv2BF16.apply(input, offset, mask, weight, bias, self.stride, self.padding, self.dilation,
+                                    self.deformable_groups, self.backward_dtype is not None)
+        return _DCNv2.apply(input, offset, mask, weight, bias, self.stride, self.padding, self.dilation,
+                            self.deformable_groups)
 
     forward = __call__
 

@@ -356,6 +356,38 @@ int cnb_dcnv2_backward(const float *input, const float *offset, const float *mas
                        int stride_h, int stride_w, int pad_h, int pad_w,
                        int dil_h, int dil_w, int deformable_groups,
                        void *workspace, size_t workspace_bytes, void *stream);
+/* bf16 backward (opt-in, the training counterpart of cnb_dcnv2_forward_bf16): both contractions on bf16 wgmma.
+ * With W_b = bf16(weight) and dY_b = bf16(grad_output) (RN; exact when grad_output is bf16):
+ *   - column gradient dcol = sum_o W_b * dY_b: exact products, fp32 sums, kept in fp32; grad_offset, grad_mask and
+ *     grad_input follow from it with the fp32 backward's kernels (atomics, or the fixed point of deterministic mode);
+ *   - grad_weight = sum_p bf16(col) * dY_b, where col is the masked bilinear value exactly as the bf16 forward
+ *     computes it and rounds it once (RN): the gradient of the forward as computed, straight through its roundings,
+ *     with exact products and fp32 sums;
+ *   - grad_bias sums grad_output as given (no rounding) in the fixed order of cnb_dcnv2_backward's tensor-core path;
+ *   - grad_offset, grad_mask, grad_weight and grad_bias are bit-identical run to run; grad_input is too while
+ *     cnb_dcnv2_set_deterministic is on (the bound behind its scale comes from W_b and dY_b).
+ * input: [b,cin,h,w] of input_dtype (CNB_DTYPE_F32 or CNB_DTYPE_BF16), channels-last ([b][h*w][cin]) when
+ * input_channels_last != 0; grad_output: [b,cout,ho,wo] NCHW of grad_output_dtype (F32 or BF16); offset, mask and
+ * weight are fp32.  The five gradients are fp32, accumulated into (zero-fill them first) and each may be NULL;
+ * grad_input is channels-last when grad_input_channels_last != 0.  Channels-last tensors need
+ * cin / deformable_groups % 32 == 0.  workspace: cnb_dcnv2_backward_bf16_workspace_bytes (16-byte aligned), which
+ * returns 0 for every shape the call rejects and, like cnb_dcnv2_backward_workspace_bytes, more while deterministic
+ * mode is on.  The call runs where both tensor-core passes of cnb_dcnv2_backward do: at most 9 taps, one stride /
+ * pad / dilation for both axes, cout <= 256 and images within their 32-bit indexing; elsewhere it returns
+ * CNB_EUNSUPPORTED (and the query 0) and the caller runs cnb_dcnv2_backward on the upcast operands.  Errors, checked
+ * before any CUDA call: CNB_EINVAL for a null input, offset, mask, weight, grad_output or workspace, an unknown dtype
+ * code, a bad shape or a buffer (input, workspace, channels-last grad_input) that is not 16-byte aligned;
+ * CNB_EUNSUPPORTED as above; CNB_EWORKSPACE for too small a workspace. */
+size_t cnb_dcnv2_backward_bf16_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw,
+                                               int stride, int pad, int dil, int dg);
+int cnb_dcnv2_backward_bf16(const void *input, int input_dtype, int input_channels_last,
+                            const float *offset, const float *mask, const float *weight,
+                            const void *grad_output, int grad_output_dtype,
+                            float *grad_input, int grad_input_channels_last,
+                            float *grad_offset, float *grad_mask, float *grad_weight, float *grad_bias,
+                            int b, int cin, int h, int w, int cout, int kh, int kw,
+                            int stride, int pad, int dil, int deformable_groups,
+                            void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------- A10/A11: DCNv2, float64
  * The reference's second build, _ext.dcn_v2_double (dcn_v2_cuda_double.c, dcn_v2_im2col_cuda_double.cu): the
