@@ -248,7 +248,7 @@ k_dcn_bwd_data(const float *__restrict__ x, const float *__restrict__ offset, co
                const float *__restrict__ weight, const float *__restrict__ gy, float *__restrict__ gx,
                float *__restrict__ goff, float *__restrict__ gmask, const DcnShape s, const int csplit) {
   // csplit > 1 (small maps: too few pixel tiles to fill the GPU): blockIdx.y takes every csplit-th channel
-  // chunk and dOffset / dMask are accumulated with atomics into the zero-filled outputs
+  // chunk and dOffset / dMask are accumulated into the outputs with atomics
   extern __shared__ __align__(16) unsigned char dcn_smem[];
   const int KT = s.kh * s.kw;
   constexpr int KC = DCN_CK * DCN_KT_MAX;
@@ -358,9 +358,9 @@ k_dcn_bwd_data(const float *__restrict__ x, const float *__restrict__ offset, co
       if (csplit > 1) {
         if (mp) atomicAdd(mp, accm[idx]);
         if (op) { atomicAdd(op + (2 * t) * HWo, acch[idx]); atomicAdd(op + (2 * t + 1) * HWo, accw[idx]); }
-      } else {
-        if (mp) *mp = accm[idx];
-        if (op) { op[(2 * t) * HWo] = acch[idx]; op[(2 * t + 1) * HWo] = accw[idx]; }
+      } else {               // the only writer of this (tap, pixel): accumulate without atomics
+        if (mp) *mp += accm[idx];
+        if (op) { op[(2 * t) * HWo] += acch[idx]; op[(2 * t + 1) * HWo] += accw[idx]; }
       }
     }
   }

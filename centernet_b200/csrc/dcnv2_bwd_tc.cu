@@ -420,14 +420,14 @@ k_dcn_bwd_offmask(const float *__restrict__ xt, const float *__restrict__ offset
         ah += __shfl_xor_sync(0xffffffffu, ah, sh);
         aw += __shfl_xor_sync(0xffffffffu, aw, sh);
       }
-      // the gradients arrive zero-filled (dcn_v2_func.py:44-48) and every (tap, pixel) has exactly one writer:
-      // a plain store is the accumulation
+      // every (tap, pixel) has exactly one writer: a plain read-modify-write accumulates into the caller's
+      // gradients, as cnb_dcnv2_backward documents, without atomics
       if ((flags & 32) && c4 == 0) {
         const int go = (gi * KT + tap) * (int)HWo + cur.p;
-        if (gmask_img) gmask_img[go] = am;
+        if (gmask_img) gmask_img[go] += am;
         if (goff_img) {
-          goff_img[2 * go - cur.p] = ah;                 // channel 2 * (gi*KT + tap)
-          goff_img[2 * go - cur.p + (int)HWo] = aw;
+          goff_img[2 * go - cur.p] += ah;                // channel 2 * (gi*KT + tap)
+          goff_img[2 * go - cur.p + (int)HWo] += aw;
         }
       }
       cur = nxt;

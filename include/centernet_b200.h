@@ -232,8 +232,8 @@ int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, cons
  * (channel 2t = dy, 2t+1 = dx of tap t), mask [b,kh*kw*dg,ho,wo],
  * weight [cout,cin,kh,kw], bias [cout] -> output [b,cout,ho,wo].
  * Backward ACCUMULATES into grad_weight/grad_bias and into
- * grad_input/grad_offset/grad_mask, all of which must arrive zero-filled as in
- * dcn_v2_func.py:44-48.
+ * grad_input/grad_offset/grad_mask on every path (the Python wrapper
+ * zero-fills them first, as dcn_v2_func.py:44-48).
  * Forward workspace (cnb_dcnv2_workspace_bytes, 16-byte aligned): the weights
  * re-tiled for the tensor-core path, a channels-last copy of the input and, for
  * maps too small to fill the GPU, split-K partial sums; the query returns 0 for

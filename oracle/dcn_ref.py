@@ -12,17 +12,23 @@ and a cross-check against torchvision.ops.deform_conv2d (third party, same offse
 import torch
 
 
+def _pair(v):
+    return (int(v[0]), int(v[1])) if isinstance(v, (tuple, list)) else (int(v), int(v))
+
+
 def dcn_v2_forward(x, offset, mask, weight, bias, stride=1, padding=1, dilation=1, deformable_groups=1):
+    """stride, padding and dilation are ints or (h, w) pairs (the C ABI's anisotropic form)."""
     x = x.double(); offset = offset.double(); mask = mask.double(); weight = weight.double()
     B, Cin, H, W = x.shape
     Cout, _, kh, kw = weight.shape
-    Ho = (H + 2 * padding - (dilation * (kh - 1) + 1)) // stride + 1      # dcn_v2_cuda.c:40-41
-    Wo = (W + 2 * padding - (dilation * (kw - 1) + 1)) // stride + 1
+    (sh, sw), (ph, pw), (dh, dw) = _pair(stride), _pair(padding), _pair(dilation)
+    Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) // sh + 1      # dcn_v2_cuda.c:40-41
+    Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) // sw + 1
     KT = kh * kw
     dg = deformable_groups
     cpg = Cin // dg
-    hs = (torch.arange(Ho, dtype=torch.float64) * stride - padding).view(1, Ho, 1)
-    ws = (torch.arange(Wo, dtype=torch.float64) * stride - padding).view(1, 1, Wo)
+    hs = (torch.arange(Ho, dtype=torch.float64) * sh - ph).view(1, Ho, 1)
+    ws = (torch.arange(Wo, dtype=torch.float64) * sw - pw).view(1, 1, Wo)
     cols = []
     xf = x.reshape(B, Cin, H * W)
     for g in range(dg):
@@ -32,8 +38,8 @@ def dcn_v2_forward(x, offset, mask, weight, bias, stride=1, padding=1, dilation=
             dy = offset[:, g * 2 * KT + 2 * t]            # :155-159 (2t = h, 2t+1 = w)
             dx = offset[:, g * 2 * KT + 2 * t + 1]
             m = mask[:, g * KT + t]
-            h_im = hs + i * dilation + dy                 # B,Ho,Wo
-            w_im = ws + j * dilation + dx
+            h_im = hs + i * dh + dy                       # B,Ho,Wo
+            w_im = ws + j * dw + dx
             inside = (h_im > -1) & (w_im > -1) & (h_im < H) & (w_im < W)     # :165
             h_low = torch.floor(h_im); w_low = torch.floor(w_im)
             lh = h_im - h_low; lw = w_im - w_low

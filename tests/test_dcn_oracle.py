@@ -1,6 +1,9 @@
 """CPU: pins the DCNv2 oracle (oracle/dcn_ref.py) with the reference's own known-answer test
 (DCNv2/test.py:32-65: zero offsets + identity centre tap + mask 0.5 => 2*DCN(x) == x) and a
-cross-check against torchvision.ops.deform_conv2d (third party, same offset layout / bilinear rule)."""
+cross-check against torchvision.ops.deform_conv2d (third party, same offset layout / bilinear rule), and at the
+sampling boundaries with known answers worked out by hand from the reference's rule."""
+import math
+
 import pytest
 import torch
 
@@ -35,3 +38,92 @@ def test_against_torchvision(stride, dg):
     t = deform_conv2d(x.double(), off.double(), w.double(), b.double(), stride=stride, padding=1, dilation=1,
                       mask=m.double())
     assert (a - t).abs().max().item() < 1e-10
+
+
+# ---------------------------------------------------------------- sampling boundaries: known answers
+# One channel, one 1x1 tap of weight 1, mask 1 and a stride larger than the map: a single output pixel whose sampling
+# position is exactly (dy, dx).  The reference samples only when -1 < h < H and -1 < w < W (dcn_v2_im2col_cuda.cu:165),
+# and then reads each of the four corners only when it lies in the map (:18-47).  Its dOffset is the coordinate weight
+# of :75-116: zero outside the same open box, else the difference of the corner values across the cell, each corner
+# counted only when it lies in the map.
+BH, BW = 4, 5
+XB = (torch.arange(BH * BW, dtype=torch.float64) + 1).view(BH, BW)     # x[h, w] = 1 + h * W + w: never 0
+
+
+def _sample(h, w):
+    """(value, d value / d dy, d value / d dx, d value / d x) of the oracle at position (h, w)."""
+    x = XB.view(1, 1, BH, BW).clone().requires_grad_(True)
+    off = torch.tensor([h, w], dtype=torch.float64).view(1, 2, 1, 1).requires_grad_(True)
+    y = dcn_v2_forward(x, off, torch.ones(1, 1, 1, 1), torch.ones(1, 1, 1, 1), None, stride=BH + BW, padding=0)
+    assert y.shape == (1, 1, 1, 1)
+    y.sum().backward()
+    return y.item(), off.grad[0, 0, 0, 0].item(), off.grad[0, 1, 0, 0].item(), x.grad[0, 0]
+
+
+def _x(h, w):
+    return XB[h, w].item() if 0 <= h < BH and 0 <= w < BW else 0.0
+
+
+def _reference_rule(h, w):
+    """dmcn_im2col_bilinear (:18-47) behind the check of :165, and dmcn_get_coordinate_weight (:75-116), written out
+    scalar by scalar: (value, dy weight, dx weight)."""
+    if not (-1 < h < BH and -1 < w < BW):
+        return 0.0, 0.0, 0.0
+    hl, wl = math.floor(h), math.floor(w)
+    lh, lw = h - hl, w - wl
+    v1, v2, v3, v4 = _x(hl, wl), _x(hl, wl + 1), _x(hl + 1, wl), _x(hl + 1, wl + 1)   # 0 when out of range
+    val = (1 - lh) * (1 - lw) * v1 + (1 - lh) * lw * v2 + lh * (1 - lw) * v3 + lh * lw * v4
+    dh = -(1 - lw) * v1 - lw * v2 + (1 - lw) * v3 + lw * v4
+    dw = -(1 - lh) * v1 + (1 - lh) * v2 - lh * v3 + lh * v4
+    return val, dh, dw
+
+
+BOUNDARY_H = (-40.0, -1.5, -1.0, -0.75, -0.5, 0.0, 1.0, 1.5, BH - 1.0, BH - 0.5, BH - 0.25, float(BH), BH + 0.5, 40.0)
+BOUNDARY_W = (-40.0, -1.5, -1.0, -0.5, 0.0, 2.0, 2.5, BW - 1.0, BW - 0.5, float(BW), BW + 0.5, 40.0)
+
+
+def test_boundary_known_answers():
+    w = 2.0                                   # an interior integer column: only the row is at the boundary
+    for h in (-1.0, float(BH), -40.0, -1.5, BH + 0.5):
+        assert _sample(h, w)[:3] == (0.0, 0.0, 0.0), h           # outside the open box: no value, no gradient
+    assert _sample(-0.5, w)[0] == 0.5 * XB[0, 2].item()          # the row above the map counts 0
+    assert _sample(BH - 0.5, w)[0] == 0.5 * XB[BH - 1, 2].item()  # the row below the map counts 0
+    assert _sample(-0.75, w)[0] == 0.25 * XB[0, 2].item()
+    # at an exact integer row, dOffset is the one-sided (floor) difference x[h + 1] - x[h]
+    assert _sample(0.0, w)[1] == XB[1, 2].item() - XB[0, 2].item()
+    assert _sample(1.0, w)[1] == XB[2, 2].item() - XB[1, 2].item()
+    assert _sample(BH - 1.0, w)[1] == -XB[BH - 1, 2].item()      # x[H] is out of range: counted as 0
+    assert _sample(-0.5, w)[1] == XB[0, 2].item()                 # x[-1] is out of range: counted as 0
+    assert _sample(BH - 0.5, w)[1] == -XB[BH - 1, 2].item()
+    # and the same along w, at an interior integer row
+    assert _sample(1.0, -1.0)[:3] == (0.0, 0.0, 0.0) and _sample(1.0, float(BW))[:3] == (0.0, 0.0, 0.0)
+    assert _sample(1.0, -0.5)[0] == 0.5 * XB[1, 0].item() and _sample(1.0, -0.5)[2] == XB[1, 0].item()
+    assert _sample(1.0, BW - 1.0)[2] == -XB[1, BW - 1].item()
+    assert _sample(1.0, 0.0)[2] == XB[1, 1].item() - XB[1, 0].item()
+    # a corner of the map: one valid corner of the four
+    val, dh, dw, gx = _sample(-0.5, -0.5)
+    assert (val, dh, dw) == (0.25 * XB[0, 0].item(), 0.5 * XB[0, 0].item(), 0.5 * XB[0, 0].item())
+    assert gx[0, 0].item() == 0.25 and gx.abs().sum().item() == 0.25     # dX: the corner weight, on that corner only
+
+
+def test_boundary_grid_matches_reference_rule():
+    """Every combination of the boundary rows and columns against the reference's rule written out scalar by scalar."""
+    for h in BOUNDARY_H:
+        for w in BOUNDARY_W:
+            val, dh, dw, gx = _sample(h, w)
+            assert (val, dh, dw) == _reference_rule(h, w), (h, w)
+            if not (-1 < h < BH and -1 < w < BW):
+                assert gx.abs().sum().item() == 0.0, (h, w)
+
+
+def test_anisotropic_geometry():
+    """(h, w) pairs of stride, padding and dilation: at zero offsets with mask 1 the oracle is a plain convolution."""
+    g = torch.Generator().manual_seed(2)
+    x = torch.randn(2, 3, 11, 13, generator=g, dtype=torch.float64)
+    w = torch.randn(4, 3, 3, 2, generator=g, dtype=torch.float64)
+    b = torch.randn(4, generator=g, dtype=torch.float64)
+    for stride, pad, dil in (((1, 2), (2, 0), (2, 1)), ((3, 1), (0, 1), (1, 3)), (2, 1, 2)):
+        want = torch.nn.functional.conv2d(x, w, b, stride, pad, dil)
+        _, _, Ho, Wo = want.shape
+        got = dcn_v2_forward(x, torch.zeros(2, 12, Ho, Wo), torch.ones(2, 6, Ho, Wo), w, b, stride, pad, dil)
+        assert got.shape == want.shape and (got - want).abs().max().item() < 1e-12
