@@ -130,6 +130,80 @@ __global__ void __launch_bounds__(128) k_ddd_epilogue(const float *__restrict__ 
   d[o] = (float)clses[i];
 }
 
+// k_ddd_epilogue for cnb_ddd_decode_ex: each head of its own dtype code in h, widened exactly; with h.logits the
+// depth head holds the raw `dep` output and goes through ddd_depth at the K gathered positions only.
+struct DddHeads {
+  int rot, depth, dim, wh, reg;  // CNB_DTYPE_* codes
+  int logits;
+};
+
+// `1. / (dep.sigmoid() + 1e-6) - 1.` (detectors/ddd.py:62) in torch's op order on fp32 CUDA tensors: sigmoid,
+// add(1e-6), reciprocal and mul(1.0) (Tensor.__rtruediv__ is `reciprocal() * other`), sub(1.0), every step rounded to
+// fp32.  The _rn intrinsics keep nvcc from contracting or reordering them.
+__device__ __forceinline__ float ddd_depth(float x) {
+  const float s = 1.0f / (1.0f + expf(-x));  // torch's CUDA sigmoid (k_sigmoid)
+  return __fsub_rn(__fmul_rn(__frcp_rn(__fadd_rn(s, 1e-6f)), 1.0f), 1.0f);
+}
+
+// v[r] = head[i + r * HW], r < N.  One dtype switch per head, so that its N loads are in flight together.
+template <int N>
+__device__ __forceinline__ void ld_rows(float (&v)[N], const void *__restrict__ p, int dt, long long i, long long HW) {
+  if (dt == CNB_DTYPE_F32) {
+#pragma unroll
+    for (int r = 0; r < N; ++r) v[r] = __ldg(reinterpret_cast<const float *>(p) + i + r * HW);
+  } else if (dt == CNB_DTYPE_BF16) {
+#pragma unroll
+    for (int r = 0; r < N; ++r)
+      v[r] = __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16 *>(p) + i + r * HW));
+  } else {
+#pragma unroll
+    for (int r = 0; r < N; ++r) v[r] = __half2float(__ldg(reinterpret_cast<const __half *>(p) + i + r * HW));
+  }
+}
+
+__global__ void __launch_bounds__(128) k_ddd_epilogue_ex(const float *__restrict__ scores,
+                                                         const int64_t *__restrict__ inds,
+                                                         const int32_t *__restrict__ clses,
+                                                         const float *__restrict__ ys, const float *__restrict__ xs,
+                                                         const void *__restrict__ rot, const void *__restrict__ depth,
+                                                         const void *__restrict__ dim, const void *__restrict__ wh,
+                                                         const void *__restrict__ reg, DddHeads h, int B, int K,
+                                                         long long HW, float *__restrict__ dets) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * K) return;
+  const int b = i / K;
+  const long long sp = inds[i];
+  const int D = wh ? 18 : 16;
+  float *d = dets + (size_t)i * D;
+  float x = xs[i], y = ys[i];
+  if (reg) {
+    float rg[2];
+    ld_rows(rg, reg, h.reg, ((long long)b * 2) * HW + sp, HW);
+    x += rg[0];
+    y += rg[1];
+  } else {
+    x += 0.5f;
+    y += 0.5f;
+  }
+  d[0] = x; d[1] = y; d[2] = scores[i];
+  float rt[8], dp[1], dm[3];
+  ld_rows(rt, rot, h.rot, ((long long)b * 8) * HW + sp, HW);
+  ld_rows(dp, depth, h.depth, (long long)b * HW + sp, HW);
+  ld_rows(dm, dim, h.dim, ((long long)b * 3) * HW + sp, HW);
+  for (int r = 0; r < 8; ++r) d[3 + r] = rt[r];
+  d[11] = h.logits ? ddd_depth(dp[0]) : dp[0];
+  for (int r = 0; r < 3; ++r) d[12 + r] = dm[r];
+  int o = 15;
+  if (wh) {
+    float wv[2];
+    ld_rows(wv, wh, h.wh, ((long long)b * 2) * HW + sp, HW);
+    d[15] = wv[0];
+    d[16] = wv[1];
+    o = 17;
+  }
+  d[o] = (float)clses[i];
+}
+
 struct RawTopk {
   float *scores;
   int64_t *inds;
@@ -174,11 +248,8 @@ __global__ void __launch_bounds__(256) k_widen(const T *__restrict__ x, float *_
     if (i0 + j < n) out[i0 + j] = to_f32(x[i0 + j]);
 }
 
-static bool dtype_known(int dt) { return dt == CNB_DTYPE_F32 || dt == CNB_DTYPE_F16 || dt == CNB_DTYPE_BF16; }
-static int dtype_bytes(int dt) { return dt == CNB_DTYPE_F32 ? 4 : 2; }
-
 // fp32 heat map (sigmoid of the logits, or the widened map) of a 16-bit or fp32 src, n elements
-static int launch_to_f32(const void *src, int dt, bool sigmoid, float *out, long long n, cudaStream_t stream) {
+int cnb::launch_to_f32(const void *src, int dt, bool sigmoid, float *out, long long n, cudaStream_t stream) {
   const unsigned grid = (unsigned)((n + 1023) / 1024);
   if (sigmoid) {
     if (dt == CNB_DTYPE_BF16) k_sigmoid<<<grid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16 *>(src), out, n);
@@ -188,9 +259,33 @@ static int launch_to_f32(const void *src, int dt, bool sigmoid, float *out, long
     if (dt == CNB_DTYPE_BF16) k_widen<<<grid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16 *>(src), out, n);
     else k_widen<<<grid, 256, 0, stream>>>(reinterpret_cast<const __half *>(src), out, n);
   }
-  CNB_CHECK_LAUNCH(sigmoid ? "cnb_ctdet_decode_ex sigmoid" : "cnb_ctdet_decode_ex widen");
+  CNB_CHECK_LAUNCH(sigmoid ? "decode sigmoid pass" : "decode widening pass");
   count_launch();
   return CNB_OK;
+}
+
+int cnb::plan_map_select(const void *src, int dt, int logits, int n_img, int C, int H, int W, int K,
+                         const float *copy, MapSelect *m) {
+  int rc = make_select_plan(src, n_img, C, H, W, K, 1, &m->pl, dtype_bytes(dt));
+  if (rc != CNB_OK) return rc;
+  m->widen = !m->pl.hot && (dt != CNB_DTYPE_F32 || logits);
+  m->map_bytes = 0;
+  if (m->widen) {
+    rc = make_select_plan(copy, n_img, C, H, W, K, 1, &m->pl);
+    if (rc != CNB_OK) return rc;
+    m->map_bytes = align_up((size_t)n_img * C * H * W * 4, 256);
+  }
+  m->pl.logits = (logits && !m->widen) ? 1 : 0;  // a widened map holds the sigmoid already
+  m->sel_bytes = select_workspace_bytes(m->pl);
+  return CNB_OK;
+}
+
+int cnb::run_map_select(const void *src, int dt, int logits, const MapSelect &m, float *copy, const FinalizeOut &out,
+                        void *ws, cudaStream_t stream) {
+  if (!m.widen) return run_select(src, m.pl, out, ws, stream, dt);
+  const int rc = launch_to_f32(src, dt, logits != 0, copy, (long long)m.pl.n_img * m.pl.C * m.pl.H * m.pl.W, stream);
+  if (rc != CNB_OK) return rc;
+  return run_select(copy, m.pl, out, ws, stream);
 }
 
 // Flip-test merge (detectors/ctdet.py:34-37, detectors/multi_pose.py:43-51): src [2n, c, h, w] holds the heads
@@ -452,6 +547,52 @@ int cnb_ddd_decode(const float *heat, const float *rot, const float *depth, cons
                                                                          depth, dim, wh, reg, b, k,
                                                                          (long long)h * w, dets);
   CNB_CHECK_LAUNCH("cnb_ddd_decode epilogue");
+  count_launch();
+  return CNB_OK;
+}
+
+/* cnb_ddd_decode of fp32, fp16 or bf16 heads, the heat map or its logits (see the header).  Layout:
+ * [selection scratch | raw top-K | fp32 copy of the heat map (only when it is widened)]. */
+size_t cnb_ddd_decode_ex_workspace_bytes(const void *heat, int heat_dtype, int logits, int b, int c, int h, int w,
+                                         int k) {
+  if (!dtype_known(heat_dtype)) return 0;
+  MapSelect m;
+  if (plan_map_select(heat, heat_dtype, logits, b, c, h, w, k, nullptr, &m) != CNB_OK) return 0;
+  return m.sel_bytes + raw_bytes((long long)b * k) + m.map_bytes;
+}
+
+int cnb_ddd_decode_ex(const void *heat, int heat_dtype, int logits, const void *rot, int rot_dtype, const void *depth,
+                      int depth_dtype, const void *dim, int dim_dtype, const void *wh, int wh_dtype, const void *reg,
+                      int reg_dtype, int b, int c, int h, int w, int k, float *dets, void *workspace,
+                      size_t workspace_bytes, void *stream) {
+  CNB_REQUIRE(dtype_known(heat_dtype) && dtype_known(rot_dtype) && dtype_known(depth_dtype) && dtype_known(dim_dtype) &&
+                  dtype_known(wh_dtype) && dtype_known(reg_dtype),
+              CNB_EINVAL, "cnb_ddd_decode_ex: unknown dtype code (heat %d, rot %d, depth %d, dim %d, wh %d, reg %d)",
+              heat_dtype, rot_dtype, depth_dtype, dim_dtype, wh_dtype, reg_dtype);
+  CNB_REQUIRE(heat && rot && depth && dim && dets && workspace, CNB_EINVAL, "cnb_ddd_decode_ex: null pointer");
+  MapSelect m;
+  int rc = plan_map_select(heat, heat_dtype, logits, b, c, h, w, k, nullptr, &m);
+  if (rc != CNB_OK) return rc;
+  const size_t sel = m.sel_bytes, raw = raw_bytes((long long)b * k);
+  CNB_REQUIRE(workspace_bytes >= sel + raw + m.map_bytes, CNB_EWORKSPACE, "cnb_ddd_decode_ex: workspace %zu < %zu",
+              workspace_bytes, sel + raw + m.map_bytes);
+  char *p = reinterpret_cast<char *>(workspace);
+  RawTopk r = carve_raw(p + sel, (long long)b * k);
+  float *copy = reinterpret_cast<float *>(p + sel + raw);
+  if (m.widen) {  // the plan of the copy where it really lies (a workspace that is not 16-byte aligned loses TMA)
+    rc = plan_map_select(heat, heat_dtype, logits, b, c, h, w, k, copy, &m);
+    if (rc != CNB_OK) return rc;
+    CNB_REQUIRE(m.sel_bytes <= sel, CNB_EWORKSPACE, "cnb_ddd_decode_ex: selection scratch %zu > %zu", m.sel_bytes,
+                sel);
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  FinalizeOut out = {r.scores, r.inds, r.clses, r.ys, r.xs, nullptr, nullptr, 0, nullptr};
+  rc = run_map_select(heat, heat_dtype, logits, m, copy, out, workspace, st);
+  if (rc != CNB_OK) return rc;
+  const DddHeads hd = {rot_dtype, depth_dtype, dim_dtype, wh_dtype, reg_dtype, logits ? 1 : 0};
+  k_ddd_epilogue_ex<<<(b * k + 127) / 128, 128, 0, st>>>(r.scores, r.inds, r.clses, r.ys, r.xs, rot, depth, dim, wh,
+                                                         reg, hd, b, k, (long long)h * w, dets);
+  CNB_CHECK_LAUNCH("cnb_ddd_decode_ex epilogue");
   count_launch();
   return CNB_OK;
 }

@@ -158,7 +158,33 @@ PYBIND11_MODULE(_C, m) {
                          ptr<float>(dets), ptr<void>(ws), wsb, ptr<void>(stream)),
           "cnb_ddd_decode");
   });
+  m.def("ddd_decode_ex_workspace_bytes", [](P heat, int dt, int logits, int b, int c, int h, int w, int k) {
+    return cnb_ddd_decode_ex_workspace_bytes(ptr<const void>(heat), dt, logits, b, c, h, w, k);
+  });
+  m.def("ddd_decode_ex", [](P heat, int heat_dt, int logits, P rot, int rot_dt, P depth, int depth_dt, P dim,
+                            int dim_dt, P wh, int wh_dt, P reg, int reg_dt, int b, int c, int h, int w, int k, P dets,
+                            P ws, size_t wsb, P stream) {
+    check(cnb_ddd_decode_ex(ptr<const void>(heat), heat_dt, logits, ptr<const void>(rot), rot_dt,
+                            ptr<const void>(depth), depth_dt, ptr<const void>(dim), dim_dt, ptr<const void>(wh), wh_dt,
+                            ptr<const void>(reg), reg_dt, b, c, h, w, k, ptr<float>(dets), ptr<void>(ws), wsb,
+                            ptr<void>(stream)),
+          "cnb_ddd_decode_ex");
+  });
   m.def("multi_pose_workspace_bytes", &cnb_multi_pose_workspace_bytes);
+  m.def("multi_pose_decode_ex_workspace_bytes", [](P heat, int heat_dt, P hm_hp, int hm_hp_dt, int logits, int b,
+                                                   int c, int j, int h, int w, int k) {
+    return cnb_multi_pose_decode_ex_workspace_bytes(ptr<const void>(heat), heat_dt, ptr<const void>(hm_hp), hm_hp_dt,
+                                                    logits, b, c, j, h, w, k);
+  });
+  m.def("multi_pose_decode_ex", [](P heat, int heat_dt, int logits, P wh, int wh_dt, P kps, int kps_dt, P reg,
+                                   int reg_dt, P hm_hp, int hm_hp_dt, P hp_off, int hp_off_dt, int b, int c, int j,
+                                   int h, int w, int k, P dets, P ws, size_t wsb, P stream) {
+    check(cnb_multi_pose_decode_ex(ptr<const void>(heat), heat_dt, logits, ptr<const void>(wh), wh_dt,
+                                   ptr<const void>(kps), kps_dt, ptr<const void>(reg), reg_dt, ptr<const void>(hm_hp),
+                                   hm_hp_dt, ptr<const void>(hp_off), hp_off_dt, b, c, j, h, w, k, ptr<float>(dets),
+                                   ptr<void>(ws), wsb, ptr<void>(stream)),
+          "cnb_multi_pose_decode_ex");
+  });
   m.def("multi_pose_decode", [](P heat, P wh, P kps, P reg, P hm_hp, P hp_off, int b, int c, int j, int h, int w,
                                 int k, P dets, P ws, size_t wsb, P stream) {
     check(cnb_multi_pose_decode(ptr<const float>(heat), ptr<const float>(wh), ptr<const float>(kps),

@@ -329,12 +329,6 @@ __device__ void finalize_fill(const T *__restrict__ img, const SelectPlan &pl, u
 // Row k of image b from its key (raw top-K outputs and/or the fused ctdet epilogue, models/decode.py:472-493).
 // The four gathered values (reg x, reg y, wh w, wh h) may come pre-loaded (gath != nullptr).
 struct RowGather { float rx, ry, ww, wh_; };
-// Element i of a head of dtype code dt, widened (K rows per image: a runtime switch, no template instances).
-__device__ __forceinline__ float ld_head(const void *p, int dt, size_t i) {
-  if (dt == CNB_DTYPE_BF16) return __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16 *>(p) + i));
-  if (dt == CNB_DTYPE_F16) return __half2float(__ldg(reinterpret_cast<const __half *>(p) + i));
-  return __ldg(reinterpret_cast<const float *>(p) + i);
-}
 __device__ __forceinline__ RowGather gather_row(const SelectPlan &pl, int b, u64 key, const FinalizeOut &out) {
   RowGather g = {0.5f, 0.5f, 0.f, 0.f};
   if (!out.dets) return g;

@@ -67,12 +67,41 @@ size_t select_workspace_bytes(const SelectPlan &pl);
 int run_select(const void *src, const SelectPlan &pl, const FinalizeOut &out, void *ws, cudaStream_t stream,
                int src_dtype = CNB_DTYPE_F32);
 
+inline bool dtype_known(int dt) { return dt == CNB_DTYPE_F32 || dt == CNB_DTYPE_F16 || dt == CNB_DTYPE_BF16; }
+inline int dtype_bytes(int dt) { return dt == CNB_DTYPE_F32 ? 4 : 2; }
+// out = n elements of src (dtype code dt) widened to fp32, or (sigmoid) torch's CUDA sigmoid of them.  A plain
+// widening needs a 16-bit src.
+int launch_to_f32(const void *src, int dt, bool sigmoid, float *out, long long n, cudaStream_t stream);
+
+// The selection over one score map of dtype code dt as the multi-head decodes run it (logits: the map holds the
+// pre-sigmoid logits).  The hot kernel reads the map in place, and so does every fp32 selection of an fp32 heat map;
+// otherwise one launch_to_f32 pass writes an fp32 copy (map_bytes, in the caller's workspace) that the fp32 selection
+// then reads.  `copy` is where that copy goes (null in the workspace queries: a 16-byte aligned place).
+struct MapSelect {
+  SelectPlan pl;     // plan of what the selection reads: the map itself, or its fp32 copy
+  int widen;         // 1: the fp32 copy is made first
+  size_t sel_bytes;  // selection scratch of pl
+  size_t map_bytes;  // the fp32 copy (0 when !widen)
+};
+int plan_map_select(const void *src, int dt, int logits, int n_img, int C, int H, int W, int K, const float *copy,
+                    MapSelect *m);
+// Enqueue the selection planned by m; `ws` holds at least m.sel_bytes of scratch.
+int run_map_select(const void *src, int dt, int logits, const MapSelect &m, float *copy, const FinalizeOut &out,
+                   void *ws, cudaStream_t stream);
+
 #ifdef __CUDACC__
 // Exact widening of one map / head element to fp32 (every fp16 and bf16 value, subnormals and infinities included,
 // is a float: the result equals torch's .float()).
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
 __device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+// Element i of a head of dtype code dt, widened (the decode epilogues gather K rows per image: a runtime switch, no
+// template instances).
+__device__ __forceinline__ float ld_head(const void *p, int dt, size_t i) {
+  if (dt == CNB_DTYPE_BF16) return __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16 *>(p) + i));
+  if (dt == CNB_DTYPE_F16) return __half2float(__ldg(reinterpret_cast<const __half *>(p) + i));
+  return __ldg(reinterpret_cast<const float *>(p) + i);
+}
 // Four consecutive map elements as loaded from shared memory (16 bytes of fp32, 8 of fp16 / bf16: the 16-bit sweep
 // keeps its row window in half the registers) and their exact widening to fp32.
 template <typename T> struct Raw4;

@@ -3,9 +3,10 @@
 Every function takes fp32 CUDA tensors (NCHW; heat maps already sigmoided by the
 caller, as in detectors/ctdet.py:31,40), does not mutate its inputs, and returns a new
 fp32 tensor on the same device, enqueued on the current stream.  Other dtypes are upcast
-to fp32 first, except in ctdet_decode, ctdet_decode_from_logits, flip_merge (and so the
-*_flip_from_logits wrappers) and ctdet_decode_from_host: they read bf16 and fp16 heads in
-place, and return, bit for bit, what they return for the .float() upcast.  The work is done by
+to fp32 first, except in ctdet_decode, multi_pose_decode, ddd_decode, their *_from_logits
+forms, flip_merge (and so the *_flip_from_logits wrappers) and ctdet_decode_from_host: they
+read bf16 and fp16 heads in place, and return, bit for bit, what they return for the .float()
+upcast.  The work is done by
 the hand-written sm_90a kernels behind ``include/centernet_b200.h``; there is no
 CPU path (non-CUDA inputs raise NotImplementedError).
 
@@ -244,13 +245,34 @@ def multi_pose_decode_flip_from_logits(hm, wh, hps, reg=None, hm_hp=None, hp_off
 
 
 # ------------------------------------------------------------------ decode.py:426-462
-def ddd_decode(heat, rot, depth, dim, wh=None, reg=None, K=40):
-    require_cuda(heat, rot, depth, dim, wh, reg, what="ddd_decode")
-    heat, rot, depth, dim, wh, reg = [f32c(t) for t in (heat, rot, depth, dim, wh, reg)]
-    b, c, h, w = _dims(heat)
-    for name, t, ch in (("rot", rot, 8), ("depth", depth, 1), ("dim", dim, 3), ("wh", wh, 2), ("reg", reg, 2)):
+def _ddd_heads(what, heat, rot, depth, dim, wh, reg):
+    require_cuda(heat, rot, depth, dim, wh, reg, what=what)
+    heads = [floatc(t) for t in (heat, rot, depth, dim, wh, reg)]
+    b, c, h, w = _dims(heads[0])
+    for name, t, ch in zip(("rot", "depth", "dim", "wh", "reg"), heads[1:], (8, 1, 3, 2, 2)):
         if t is not None and tuple(t.shape) != (b, ch, h, w):
-            raise RuntimeError("ddd_decode: %s must be [%d, %d, %d, %d], got %s" % (name, b, ch, h, w, tuple(t.shape)))
+            raise RuntimeError("%s: %s must be [%d, %d, %d, %d], got %s" % (what, name, b, ch, h, w, tuple(t.shape)))
+    return heads
+
+
+def _ddd_ex(heat, rot, depth, dim, wh, reg, K, logits):
+    """cnb_ddd_decode_ex: every head fp32, fp16 or bf16."""
+    b, c, h, w = _dims(heat)
+    dets = torch.empty((b, K, 18 if wh is not None else 16), dtype=torch.float32, device=heat.device)
+    ws = workspace(C.ddd_decode_ex_workspace_bytes(ptr(heat), dtype_code(heat), logits, b, c, h, w, K), heat.device)
+    C.ddd_decode_ex(ptr(heat), dtype_code(heat), logits, ptr(rot), dtype_code(rot), ptr(depth), dtype_code(depth),
+                    ptr(dim), dtype_code(dim), ptr(wh), dtype_code(wh), ptr(reg), dtype_code(reg), b, c, h, w, K,
+                    ptr(dets), ptr(ws), ws.numel(), stream_ptr(heat))
+    return dets
+
+
+def ddd_decode(heat, rot, depth, dim, wh=None, reg=None, K=40):
+    """bf16 / fp16 heads (each its own dtype) are read in place: the dets equal, bit for bit, those of the .float()
+    upcast."""
+    heat, rot, depth, dim, wh, reg = _ddd_heads("ddd_decode", heat, rot, depth, dim, wh, reg)
+    if not _all_f32(heat, rot, depth, dim, wh, reg):
+        return _ddd_ex(heat, rot, depth, dim, wh, reg, K, 0)
+    b, c, h, w = _dims(heat)
     dets = torch.empty((b, K, 18 if wh is not None else 16), dtype=torch.float32, device=heat.device)
     ws = workspace(C.topk_workspace_bytes(b, c, h, w, K), heat.device)
     C.ddd_decode(ptr(heat), ptr(rot), ptr(depth), ptr(dim), ptr(wh), ptr(reg), b, c, h, w, K, ptr(dets), ptr(ws),
@@ -258,22 +280,66 @@ def ddd_decode(heat, rot, depth, dim, wh=None, reg=None, K=40):
     return dets
 
 
+def ddd_decode_from_logits(hm, rot, dep, dim, wh=None, reg=None, K=40):
+    """`ddd_decode(hm.sigmoid_(), rot, 1. / (dep.sigmoid() + 1e-6) - 1., dim, wh, reg, K)` (detectors/ddd.py:61-68)
+    on the heads' raw outputs: hm is selected through its sigmoid, and the depth transform runs, in torch's op order,
+    at the K selected positions only.  The dets equal, bit for bit, those of ddd_decode on torch's CUDA sigmoid of hm
+    and torch's transform of dep; no input is modified.  bf16 / fp16 heads are read in place, widened exactly and
+    processed as fp32 (the reference's ops on a half tensor would round every step to half precision)."""
+    hm, rot, dep, dim, wh, reg = _ddd_heads("ddd_decode_from_logits", hm, rot, dep, dim, wh, reg)
+    return _ddd_ex(hm, rot, dep, dim, wh, reg, K, 1)
+
+
 # ------------------------------------------------------------------ decode.py:497-571
-def multi_pose_decode(heat, wh, kps, reg=None, hm_hp=None, hp_offset=None, K=100):
-    require_cuda(heat, wh, kps, reg, hm_hp, hp_offset, what="multi_pose_decode")
-    heat, wh, kps, reg, hm_hp, hp_offset = [f32c(t) for t in (heat, wh, kps, reg, hm_hp, hp_offset)]
+def _pose_heads(what, heat, wh, kps, reg, hm_hp, hp_offset):
+    require_cuda(heat, wh, kps, reg, hm_hp, hp_offset, what=what)
+    heads = [floatc(t) for t in (heat, wh, kps, reg, hm_hp, hp_offset)]
+    b, c, h, w = _dims(heads[0])
+    j = int(heads[2].shape[1]) // 2
+    for name, t, ch in zip(("wh", "kps", "reg", "hm_hp", "hp_offset"), heads[1:], (2, 2 * j, 2, j, 2)):
+        if t is not None and tuple(t.shape) != (b, ch, h, w):
+            raise RuntimeError("%s: %s must be [%d, %d, %d, %d], got %s" % (what, name, b, ch, h, w, tuple(t.shape)))
+    return heads
+
+
+def _multi_pose_ex(heat, wh, kps, reg, hm_hp, hp_offset, K, logits):
+    """cnb_multi_pose_decode_ex: every head fp32, fp16 or bf16."""
     b, c, h, w = _dims(heat)
     j = int(kps.shape[1]) // 2
-    for name, t, ch in (("wh", wh, 2), ("kps", kps, 2 * j), ("reg", reg, 2), ("hm_hp", hm_hp, j),
-                        ("hp_offset", hp_offset, 2)):
-        if t is not None and tuple(t.shape) != (b, ch, h, w):
-            raise RuntimeError("multi_pose_decode: %s must be [%d, %d, %d, %d], got %s"
-                               % (name, b, ch, h, w, tuple(t.shape)))
+    dets = torch.empty((b, K, 4 + 1 + 2 * j + 1), dtype=torch.float32, device=heat.device)
+    nb = C.multi_pose_decode_ex_workspace_bytes(ptr(heat), dtype_code(heat), ptr(hm_hp), dtype_code(hm_hp), logits,
+                                                b, c, j, h, w, K)
+    ws = workspace(nb, heat.device)
+    C.multi_pose_decode_ex(ptr(heat), dtype_code(heat), logits, ptr(wh), dtype_code(wh), ptr(kps), dtype_code(kps),
+                           ptr(reg), dtype_code(reg), ptr(hm_hp), dtype_code(hm_hp), ptr(hp_offset),
+                           dtype_code(hp_offset), b, c, j, h, w, K, ptr(dets), ptr(ws), ws.numel(), stream_ptr(heat))
+    return dets
+
+
+def multi_pose_decode(heat, wh, kps, reg=None, hm_hp=None, hp_offset=None, K=100):
+    """bf16 / fp16 heads (each its own dtype) are read in place: the dets equal, bit for bit, those of the .float()
+    upcast."""
+    heat, wh, kps, reg, hm_hp, hp_offset = _pose_heads("multi_pose_decode", heat, wh, kps, reg, hm_hp, hp_offset)
+    if not _all_f32(heat, wh, kps, reg, hm_hp, hp_offset):
+        return _multi_pose_ex(heat, wh, kps, reg, hm_hp, hp_offset, K, 0)
+    b, c, h, w = _dims(heat)
+    j = int(kps.shape[1]) // 2
     dets = torch.empty((b, K, 4 + 1 + 2 * j + 1), dtype=torch.float32, device=heat.device)
     ws = workspace(C.multi_pose_workspace_bytes(b, c, j, h, w, K), heat.device)
     C.multi_pose_decode(ptr(heat), ptr(wh), ptr(kps), ptr(reg), ptr(hm_hp), ptr(hp_offset), b, c, j, h, w, K,
                         ptr(dets), ptr(ws), ws.numel(), stream_ptr(heat))
     return dets
+
+
+def multi_pose_decode_from_logits(hm, wh, hps, reg=None, hm_hp=None, hp_offset=None, K=100):
+    """`multi_pose_decode(hm.sigmoid_(), wh, hps, reg, hm_hp.sigmoid_(), hp_offset, K)` (detectors/multi_pose.py:
+    33-35,53) on the raw logits of hm and hm_hp, without the two full-map sigmoid passes: in the hot geometry both
+    selections run in logit space and only the candidates go through the sigmoid.  The dets equal, bit for bit, those
+    of multi_pose_decode on torch's CUDA sigmoid of hm and hm_hp; no input is modified.  bf16 / fp16 heads are read in
+    place, widened exactly and processed as fp32 (the reference's `sigmoid_()` on a half tensor would round the scores
+    to half precision first)."""
+    heads = _pose_heads("multi_pose_decode_from_logits", hm, wh, hps, reg, hm_hp, hp_offset)
+    return _multi_pose_ex(*heads, K, 1)
 
 
 # ------------------------------------------------------------------ decode.py:122-424

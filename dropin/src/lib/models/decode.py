@@ -8,4 +8,5 @@ from centernet_b200.decode import (  # noqa: F401
     _nms, _topk, _topk_channel, _left_aggregate, _right_aggregate, _top_aggregate, _bottom_aggregate,
     _h_aggregate, _v_aggregate, agnex_ct_decode, exct_decode, ddd_decode, ctdet_decode, multi_pose_decode,
     _gather_feat, _transpose_and_gather_feat,
-    ctdet_decode_from_logits)   # extra: fused-sigmoid variant (INTEGRATION.md section 1)
+    # extras: fused-sigmoid variants (INTEGRATION.md section 1)
+    ctdet_decode_from_logits, multi_pose_decode_from_logits, ddd_decode_from_logits)

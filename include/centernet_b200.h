@@ -43,7 +43,7 @@ extern "C" {
 #define CNB_EWORKSPACE 4   /* workspace_bytes smaller than cnb_*_workspace_bytes */
 
 /* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16, cnb_ctdet_decode_ex,
- * cnb_flip_merge_ex). */
+ * cnb_flip_merge_ex, cnb_ddd_decode_ex, cnb_multi_pose_decode_ex). */
 #define CNB_DTYPE_F32 0
 #define CNB_DTYPE_BF16 1
 #define CNB_DTYPE_F16 2
@@ -156,6 +156,27 @@ int cnb_ddd_decode(const float *heat, const float *rot, const float *depth, cons
                    const float *wh, const float *reg, int b, int c, int h, int w, int k,
                    float *dets, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ------------------------- N1: ddd_decode of fp32, fp16 or bf16 heads, from the logits
+ * cnb_ddd_decode for heads of any of the three float types, each of heat, rot, depth, dim, wh and reg with its own
+ * dtype code.  logits != 0 replaces `hm.sigmoid_()` and `dep = 1. / (dep.sigmoid() + 1e-6) - 1.`
+ * (detectors/ddd.py:61-62): heat holds the hm logits and depth the raw dep output, and the depth transform is
+ * evaluated at the k gathered positions only, in torch's op order (sigmoid, add, reciprocal, mul, sub, each rounded
+ * to fp32).  Contract: the dets, bit for bit, are those of cnb_ddd_decode on the .float() upcast of the heads (after
+ * torch's CUDA sigmoid of heat and the depth transform, with logits).  Half inputs are widened exactly and then
+ * processed as fp32; a half-precision `sigmoid_()` would round every intermediate to half instead.  The selection
+ * reads the heat map in place in the hot geometry (h = w = 128, k <= 256, 16-byte aligned) and when it is an fp32
+ * heat map; otherwise one pass writes its fp32 copy (or sigmoid) into the workspace.  The query takes the heat
+ * pointer because its alignment decides the path and returns 0 for every shape or dtype code the call rejects.
+ * Errors, checked before any CUDA call: CNB_EINVAL for an unknown dtype code, a null pointer or a bad shape,
+ * CNB_EUNSUPPORTED for k > 1024, CNB_EWORKSPACE for too small a workspace. */
+size_t cnb_ddd_decode_ex_workspace_bytes(const void *heat, int heat_dtype, int logits,
+                                         int b, int c, int h, int w, int k);
+int cnb_ddd_decode_ex(const void *heat, int heat_dtype, int logits, const void *rot, int rot_dtype,
+                      const void *depth, int depth_dtype, const void *dim, int dim_dtype,
+                      const void *wh, int wh_dtype, const void *reg, int reg_dtype,
+                      int b, int c, int h, int w, int k, float *dets,
+                      void *workspace, size_t workspace_bytes, void *stream);
+
 /* ----------------------------------------------------- A6: multi_pose_decode
  * models/decode.py:497-571.  heat [b,1,h,w]; wh, reg(NULL ok) [b,2,h,w];
  * kps [b,2j,h,w]; hm_hp [b,j,h,w] or NULL; hp_offset [b,2,h,w] or NULL
@@ -165,6 +186,27 @@ int cnb_multi_pose_decode(const float *heat, const float *wh, const float *kps, 
                           const float *hm_hp, const float *hp_offset,
                           int b, int c, int j, int h, int w, int k, float *dets,
                           void *workspace, size_t workspace_bytes, void *stream);
+
+/* --------------------- N1: multi_pose_decode of fp32, fp16 or bf16 heads, from the logits
+ * cnb_multi_pose_decode for heads of any of the three float types, each of heat, wh, kps, reg, hm_hp and hp_offset
+ * with its own dtype code (a null head's code must still be a known one).  logits != 0 replaces `hm.sigmoid_()` and
+ * `hm_hp.sigmoid_()` (detectors/multi_pose.py:33-35): heat and hm_hp hold logits.  Contract: the dets, bit for bit,
+ * are those of cnb_multi_pose_decode on the .float() upcast of the heads (after torch's CUDA sigmoid of heat and hm_hp,
+ * with logits).  Half inputs are widened exactly and then processed as fp32.  Each selection (heat as b images,
+ * hm_hp as b*j one-plane images) reads its map in place in the hot geometry (h = w = 128, k <= 256, 16-byte aligned)
+ * and when it is an fp32 heat map; otherwise one pass writes its fp32 copy (or sigmoid) into the workspace.  The query
+ * takes the heat and hm_hp pointers (hm_hp NULL: no joint selection) because their alignment decides the path, and
+ * returns 0 for every shape or dtype code the call rejects.  Errors, checked before any CUDA call: CNB_EINVAL for an
+ * unknown dtype code, a null pointer, hp_offset without hm_hp or a bad shape, CNB_EUNSUPPORTED for k > 1024,
+ * CNB_EWORKSPACE for too small a workspace. */
+size_t cnb_multi_pose_decode_ex_workspace_bytes(const void *heat, int heat_dtype, const void *hm_hp,
+                                                int hm_hp_dtype, int logits, int b, int c, int j, int h, int w,
+                                                int k);
+int cnb_multi_pose_decode_ex(const void *heat, int heat_dtype, int logits, const void *wh, int wh_dtype,
+                             const void *kps, int kps_dtype, const void *reg, int reg_dtype,
+                             const void *hm_hp, int hm_hp_dtype, const void *hp_offset, int hp_offset_dtype,
+                             int b, int c, int j, int h, int w, int k, float *dets,
+                             void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------ A7: edge aggregation
  * models/decode.py:17-77.  out = heat + weight*(dirA + dirB) with

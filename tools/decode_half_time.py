@@ -12,7 +12,22 @@ alternated; each is timed over windows of at least --window seconds, --repeats t
 images/s, algorithmic bytes per image (80*128*128*s + 100*4*s + 100*24, s the element size of the heads) and the
 share of the HBM peak (MEASURED_PEAKS.json, else 3.35 TB/s), asserts that the half and upcast arms' timed outputs
 are bit-identical, and records the card and its power limit.  If native half is less than 1.5x faster than fp32
-device-resident, a torch.profiler kernel table is added.  Writes DIR/decode_half_time.json.  GPU only."""
+device-resident, a torch.profiler kernel table is added.  Writes DIR/decode_half_time.json.  GPU only.
+
+--task multi_pose (128 x 128, 17 joints, K = 100) and --task ddd (96 x 320, C = 3, K = 100) time, at B = 1, 8 and 64
+(3 rotating batches of synthetic heads, seed 317):
+
+  detector_f32         today's detector path on fp32 logits: torch's sigmoid of hm (and hm_hp; for ddd also the
+                       depth transform 1. / (dep.sigmoid() + 1e-6) - 1.), then the fp32 decode
+  logits_f32           *_decode_from_logits on the fp32 logits
+  upcast_<dt>          a dt model today: the .float() casts of every head, then the detector path (casts timed)
+  native_<dt>_logits   *_decode_from_logits on the dt heads, read in place
+  heat_f32             the fp32 decode on fp32 heat maps (sigmoid / depth transform already applied)
+  native_<dt>_heat     the decode on those heat maps rounded to dt, read in place
+
+asserts that detector_f32 == logits_f32, upcast_<dt> == native_<dt>_logits and native_<dt>_heat == the decode of
+its .float() upcast bit for bit in every timed call, and adds a torch.profiler kernel table at B = 64 and at every
+batch size where a new arm is slower than the arm it replaces.  Writes DIR/decode_half_time_<task>.json."""
 import argparse
 import json
 import os
@@ -170,13 +185,137 @@ def profile(fn):
     return sorted(rows, key=lambda r: -r["us_per_call"])
 
 
+POSE_J, DDD_C, HEAD_K = 17, 3, 100
+
+
+def task_heads(task, B, seed, device="cuda"):
+    """Synthetic raw head outputs: logits randn - 2.19 for the heat maps (as bench.py), uniform regressions."""
+    g = torch.Generator(device=device).manual_seed(seed)
+
+    def r(c, h, w, scale=1.0, shift=0.0):
+        return torch.rand(B, c, h, w, device=device, generator=g) * scale + shift
+    if task == "multi_pose":
+        H, W, J = H_, W_, POSE_J
+        hm = torch.randn(B, 1, H, W, device=device, generator=g) - 2.19
+        wh, hps, reg = r(2, H, W, 40), r(2 * J, H, W, 24, -12), r(2, H, W)
+        hm_hp = torch.randn(B, J, H, W, device=device, generator=g) - 2.19
+        return [hm, wh, hps, reg, hm_hp, r(2, H, W)]
+    H, W = 96, 320
+    hm = torch.randn(B, DDD_C, H, W, device=device, generator=g) - 2.19
+    rot = torch.randn(B, 8, H, W, device=device, generator=g)
+    dep = torch.randn(B, 1, H, W, device=device, generator=g) * 2
+    return [hm, rot, dep, r(3, H, W, 4), r(2, H, W, 60), r(2, H, W)]
+
+
+def task_alg_bytes(task, s):
+    """Bytes per image the decode must move at least: the score maps, the K gathered rows (multi_pose: wh, reg, kps and
+    hp_offset at every (joint, candidate)), the dets.  multi_pose at s = 4 is DESIGN 4.2's 1,224,448 B."""
+    if task == "multi_pose":
+        return (1 + POSE_J) * H_ * W_ * s + HEAD_K * (72 * s + 4 * (6 + 2 * POSE_J))
+    return DDD_C * 96 * 320 * s + HEAD_K * (16 * s + 4 * 18)
+
+
+def task_fns(task):
+    """(decode on heat maps, decode from logits, the detector's glue from logits to heat maps)."""
+    if task == "multi_pose":
+        def dec(hm, wh, hps, reg, hm_hp, off):
+            return D.multi_pose_decode(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=off, K=HEAD_K)
+
+        def dec_logits(hm, wh, hps, reg, hm_hp, off):
+            return D.multi_pose_decode_from_logits(hm, wh, hps, reg=reg, hm_hp=hm_hp, hp_offset=off, K=HEAD_K)
+
+        def glue(hm, wh, hps, reg, hm_hp, off):   # detectors/multi_pose.py:33-35 (out of place: inputs are reused)
+            return [hm.sigmoid(), wh, hps, reg, hm_hp.sigmoid(), off]
+        return dec, dec_logits, glue
+
+    def dec(hm, rot, dep, dim, wh, reg):
+        return D.ddd_decode(hm, rot, dep, dim, wh=wh, reg=reg, K=HEAD_K)
+
+    def dec_logits(hm, rot, dep, dim, wh, reg):
+        return D.ddd_decode_from_logits(hm, rot, dep, dim, wh=wh, reg=reg, K=HEAD_K)
+
+    def glue(hm, rot, dep, dim, wh, reg):         # detectors/ddd.py:61-62
+        return [hm.sigmoid(), rot, 1. / (dep.sigmoid() + 1e-6) - 1., dim, wh, reg]
+    return dec, dec_logits, glue
+
+
+def run_task(task, args):
+    name, power = card()
+    peak, peak_src = hbm_peak_gbs()
+    geom = ("%d joints, %dx%d" % (POSE_J, H_, W_)) if task == "multi_pose" else "C=%d, 96x320" % DDD_C
+    result = {"card": name, "power_limit": power, "hbm_peak_gbs": peak, "hbm_peak_source": peak_src,
+              "workload": "%s, seed 317, %s, K=%d, 3 rotating batches" % (task, geom, HEAD_K), "groups": {}}
+    dec, dec_logits, glue = task_fns(task)
+    for B in (1, 8, 64):
+        raw = [task_heads(task, B, 317 + i) for i in range(3)]
+        heat = [glue(*b) for b in raw]
+        sets = {"detector_f32": raw, "logits_f32": raw, "heat_f32": heat}
+        fns = {"detector_f32": lambda *t: dec(*glue(*t)), "logits_f32": dec_logits, "heat_f32": dec}
+        elem = {"detector_f32": 4, "logits_f32": 4, "heat_f32": 4}
+        for dt, tdt in HALF.items():
+            half = [[t.to(tdt) for t in b] for b in raw]
+            sets["upcast_" + dt] = half
+            fns["upcast_" + dt] = lambda *t: dec(*glue(*[x.float() for x in t]))
+            sets["native_%s_logits" % dt] = half
+            fns["native_%s_logits" % dt] = dec_logits
+            sets["native_%s_heat" % dt] = [[t.to(tdt) for t in b] for b in heat]
+            fns["native_%s_heat" % dt] = dec
+            elem.update({"upcast_" + dt: 2, "native_%s_logits" % dt: 2, "native_%s_heat" % dt: 2})
+        outs = {n: [None] * 3 for n in sets}
+        arms = {n: rotating(fns[n], sets[n], outs[n]) for n in sets}
+        runs = time_group(arms, args.warmup, args.repeats, args.window)
+        torch.cuda.synchronize()
+        same = {"logits_f32 == detector_f32": all(map(torch.equal, outs["logits_f32"], outs["detector_f32"]))}
+        for dt in HALF:
+            same["native_%s_logits == upcast_%s" % (dt, dt)] = all(
+                map(torch.equal, outs["native_%s_logits" % dt], outs["upcast_" + dt]))
+            same["native_%s_heat == decode of its upcast" % dt] = all(
+                torch.equal(o, dec(*[t.float() for t in b])) for o, b in zip(outs["native_%s_heat" % dt],
+                                                                            sets["native_%s_heat" % dt]))
+        assert all(same.values()), "%s B=%d: timed outputs differ: %s" % (task, B, same)
+        a = {}
+        for n, ms in runs.items():
+            best = min(ms)
+            ips = B / (best * 1e-3)
+            a[n] = {"ms_runs": [round(m, 5) for m in ms], "ms": round(best, 5),
+                    "spread": round((max(ms) - min(ms)) / best, 4), "images_per_s": round(ips, 1),
+                    "alg_bytes_per_image": task_alg_bytes(task, elem[n]),
+                    "hbm_share": round(ips * task_alg_bytes(task, elem[n]) / (peak * 1e9), 4)}
+        # each new arm against the arm it replaces
+        vs = {"logits_f32": "detector_f32", "heat_f32": None}
+        for dt in HALF:
+            vs.update({"native_%s_logits" % dt: "detector_f32", "upcast_" + dt: None,
+                       "native_%s_heat" % dt: "heat_f32"})
+        speed = {"%s vs %s" % (n, o): round(a[o]["ms"] / a[n]["ms"], 3) for n, o in vs.items() if o}
+        speed.update({"native_%s_logits vs upcast_%s" % (dt, dt): round(a["upcast_" + dt]["ms"]
+                                                                          / a["native_%s_logits" % dt]["ms"], 3)
+                      for dt in HALF})
+        g = {"B": B, "arms": a, "bitwise_identical": same, "speedups": speed}
+        slower = [k.split(" vs ")[0] for k, v in speed.items() if v < 1.0]
+        if B == 64 or slower:
+            prof = set(slower) | {"detector_f32", "logits_f32", "native_bf16_logits", "upcast_bf16"}
+            g["profile"] = {n: profile(arms[n]) for n in sorted(prof)}
+        result["groups"]["B%d" % B] = g
+        print("%-10s B=%-3d " % (task, B) + "  ".join("%s %.4f ms" % (n, v["ms"]) for n, v in a.items()), flush=True)
+        print("           speedups: %s" % speed, flush=True)
+        del raw, heat, sets, outs, arms
+    os.makedirs(args.out, exist_ok=True)
+    path = os.path.join(args.out, "decode_half_time_%s.json" % task)
+    with open(path, "w") as f:
+        json.dump(result, f, indent=1)
+    print("card: %s, power limit %s; wrote %s" % (name, power, path))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="directory for decode_half_time.json (created if missing)")
+    ap.add_argument("--task", choices=("ctdet", "multi_pose", "ddd"), default="ctdet")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--window", type=float, default=1.0, help="seconds per timed window")
     args = ap.parse_args()
+    if args.task != "ctdet":
+        return run_task(args.task, args)
     name, power = card()
     peak, peak_src = hbm_peak_gbs()
     result = {"card": name, "power_limit": power, "hbm_peak_gbs": peak, "hbm_peak_source": peak_src,
