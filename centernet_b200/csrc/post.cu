@@ -91,7 +91,16 @@ __global__ void __launch_bounds__(256) k_group_by_class(const float *__restrict_
   }
 }
 
-constexpr int NMS_CAP = 1536;   // rows of one list held in shared memory (5 floats + new score + flags + perm)
+// Rows of one list held in shared memory: 5 floats + new score + perm + flags = 27 B per row.  The launch sizes its
+// shared memory from n_cap (the longest list possible), so 4096 rows take 110.6 KB of the 227 KB opt-in and a
+// typical merge (n = 200-500) a few KB.
+constexpr int NMS_MAX_ROWS = 4096;
+constexpr size_t NMS_ROW_BYTES = 5 * 4 + 4 + 2 + 1;
+
+// nms.pyx:18-22: `a if a <= b else b` / `a if a >= b else b` -- a NaN second operand is returned, a NaN first
+// operand is not (fminf / fmaxf would return the non-NaN operand in both cases)
+__device__ __forceinline__ float pyx_min(float a, float b) { return a <= b ? a : b; }
+__device__ __forceinline__ float pyx_max(float a, float b) { return a >= b ? a : b; }
 
 // One warp per list.  List l = (image l / lists_per_img, class l % lists_per_img) covers rows
 // image * n_cap + [offsets[image][class], offsets[image][class + 1]) of `in` ([*, d] floats; columns 0-4 =
@@ -102,10 +111,10 @@ __global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, f
                                                  int d, float sigma, float Nt, float threshold, int method,
                                                  int *__restrict__ final_n) {
   extern __shared__ __align__(16) unsigned char nsm[];
-  float *bx = reinterpret_cast<float *>(nsm);                 // [CAP][5]
-  float *ns = bx + NMS_CAP * 5;                               // new score of the current iteration
-  unsigned short *perm = reinterpret_cast<unsigned short *>(ns + NMS_CAP);   // original row of the extra columns
-  unsigned char *flag = reinterpret_cast<unsigned char *>(perm + NMS_CAP);   // bit0: overlapped, bit1: below threshold
+  float *bx = reinterpret_cast<float *>(nsm);                 // [n_cap][5]
+  float *ns = bx + (size_t)n_cap * 5;                         // new score of the current iteration
+  unsigned short *perm = reinterpret_cast<unsigned short *>(ns + n_cap);   // original row of the extra columns
+  unsigned char *flag = reinterpret_cast<unsigned char *>(perm + n_cap);   // bit0: overlapped, bit1: below threshold
   const int lane = threadIdx.x;
   const int l = blockIdx.x;
   const int img = l / lists_per_img, cls = l - img * lists_per_img;
@@ -116,7 +125,7 @@ __global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, f
     if (final_n && lane == 0) final_n[l] = 0;
     return;
   }
-  if (N > NMS_CAP) {   // not supported in shared memory: leave the list untouched and flag it
+  if (N > n_cap) {   // offsets inconsistent with n_cap (never from k_group_by_class): leave the list untouched, flag it
     for (int i = lane; i < N * d; i += 32) out[(size_t)r0 * d + i] = in[(size_t)r0 * d + i];
     if (final_n && lane == 0) final_n[l] = -N;
     return;
@@ -155,11 +164,11 @@ __global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, f
     for (int p = i + 1 + lane; p < N; p += 32) {
       const float x1 = bx[p * 5 + 0], y1 = bx[p * 5 + 1], x2 = bx[p * 5 + 2], y2 = bx[p * 5 + 3], s = bx[p * 5 + 4];
       const float area = (float)__dmul_rn(__dadd_rn((double)(x2 - x1), 1.0), __dadd_rn((double)(y2 - y1), 1.0));
-      const float iw = (float)__dadd_rn((double)(fminf(tx2, x2) - fmaxf(tx1, x1)), 1.0);
+      const float iw = (float)__dadd_rn((double)(pyx_min(tx2, x2) - pyx_max(tx1, x1)), 1.0);
       float nsv = s;
       unsigned char f = 0;
       if (iw > 0.f) {
-        const float ih = (float)__dadd_rn((double)(fminf(ty2, y2) - fmaxf(ty1, y1)), 1.0);
+        const float ih = (float)__dadd_rn((double)(pyx_min(ty2, y2) - pyx_max(ty1, y1)), 1.0);
         if (ih > 0.f) {
           const float inter = __fmul_rn(iw, ih);
           const double u = __dadd_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)(tx2 - tx1), 1.0), __dadd_rn((double)(ty2 - ty1), 1.0)),
@@ -215,6 +224,7 @@ __global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, f
 
 // One CTA per image: threshold = max_per_image-th largest score of the image's n rows (np.partition(scores,
 // kth)[kth], detectors/ctdet.py:85-88), keep[i] = score >= threshold.  n <= 4096.  No cut when n <= max_per_image.
+// NaN of either sign orders above +inf, as np.partition sorts it.
 __global__ void __launch_bounds__(1024) k_topk_keep(const float *__restrict__ rows, int d, const int *__restrict__ offsets,
                                                     int num_classes, int n_cap, int max_per_image,
                                                     unsigned char *__restrict__ keep, float *__restrict__ thresh_out) {
@@ -234,9 +244,9 @@ __global__ void __launch_bounds__(1024) k_topk_keep(const float *__restrict__ ro
   for (int i = tid; i < m; i += blockDim.x) {
     uint32_t k = 0u;   // pads sort below every real score
     if (i < n) {
-      const uint32_t u = __float_as_uint(r[(size_t)i * d + 4]);
-      k = (u & 0x80000000u) ? ~u : (u | 0x80000000u);   // order-preserving float -> uint
-      if (k == 0u) k = 1u;
+      uint32_t u = __float_as_uint(r[(size_t)i * d + 4]);
+      if ((u & 0x7fffffffu) > 0x7f800000u) u &= 0x7fffffffu;   // NaN: sign bit cleared, above +inf
+      k = (u & 0x80000000u) ? ~u : (u | 0x80000000u);   // order-preserving float -> uint, >= ~(-inf) > 0
     }
     key[i] = k;
   }
@@ -294,12 +304,14 @@ int cnb_soft_nms(const float *rows, float *out, const int32_t *offsets, int n_im
               "cnb_soft_nms: bad arguments");
   const int n_lists = n_img * lists_per_img;
   CNB_REQUIRE(d == 5 || rows != out, CNB_EINVAL, "cnb_soft_nms: in-place only for 5-column rows");
-  const size_t smem = (size_t)NMS_CAP * (5 * 4 + 4 + 2 + 1) + 16;
+  CNB_REQUIRE(n_cap <= NMS_MAX_ROWS, CNB_EINVAL, "cnb_soft_nms: at most 4096 rows per image");
+  const size_t smem = (size_t)n_cap * NMS_ROW_BYTES + 16;
   static thread_local int dev_done = -1;
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev_done != dev) {
-    CNB_CUDA(cudaFuncSetAttribute(k_soft_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (dev_done != dev) {   // opt in once to the largest launch; each launch asks only for what its n_cap needs
+    CNB_CUDA(cudaFuncSetAttribute(k_soft_nms, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)(NMS_MAX_ROWS * NMS_ROW_BYTES + 16)));
     dev_done = dev;
   }
   k_soft_nms<<<n_lists, 32, smem, (cudaStream_t)stream>>>(rows, out, offsets, lists_per_img, n_cap, d, sigma, nt, threshold,

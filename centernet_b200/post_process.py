@@ -14,6 +14,10 @@ import torch
 
 from ._lib import C, ptr, stream_ptr
 
+# Longest soft-NMS list and most detections per image of a merge (k_soft_nms holds a list in shared memory,
+# k_topk_keep sorts an image's scores there; csrc/post.cu).
+MAX_ROWS = 4096
+
 
 # ------------------------------------------------------------------ utils/image.py:27-60 (host, float64, B matrices)
 def _inv_affine(center, scale, output_size):
@@ -95,6 +99,8 @@ def _soft_nms(boxes, sigma, Nt, threshold, method, d):
     n = int(boxes.shape[0])
     if n == 0:
         return []
+    if n > MAX_ROWS:
+        raise NotImplementedError("soft_nms: lists longer than %d boxes are not implemented" % MAX_ROWS)
     dev = torch.device("cuda", torch.cuda.current_device())
     src = torch.from_numpy(np.ascontiguousarray(boxes[:, :d])).to(dev)
     dst = torch.empty_like(src)
@@ -104,7 +110,7 @@ def _soft_nms(boxes, sigma, Nt, threshold, method, d):
                ptr(fin), stream_ptr(src))
     keep = int(fin.item())
     if keep < 0:
-        raise NotImplementedError("soft_nms: lists longer than 1536 boxes are not implemented")
+        raise RuntimeError("soft_nms: the list of %d boxes was not processed" % n)
     boxes[:, :d] = dst.cpu().numpy()
     return list(range(keep))
 
@@ -142,19 +148,26 @@ def ctdet_merge_device(dets_per_scale, metas, num_classes, max_per_image=100, nm
         parts.append(t)
     allp = torch.cat(parts, dim=1).contiguous()          # scale-major, like np.concatenate over `detections`
     b, n, _ = [int(v) for v in allp.shape]
-    if n > 4096:
-        raise NotImplementedError("ctdet_merge_device: at most 4096 detections per image")
+    if n > MAX_ROWS:
+        raise NotImplementedError("ctdet_merge_device: at most %d detections per image" % MAX_ROWS)
     rows = torch.empty((b, n, 5), dtype=torch.float32, device=allp.device)
     offs = torch.empty((b, num_classes + 1), dtype=torch.int32, device=allp.device)
     C.group_by_class(ptr(allp), b, n, num_classes, ptr(rows), ptr(offs), stream_ptr(allp))
+    fin = None
     if S > 1 or nms:
-        C.soft_nms(ptr(rows), ptr(rows), ptr(offs), b, num_classes, n, 5, 0.5, 0.5, 0.001, 2, 0, stream_ptr(rows))
+        fin = torch.empty((b, num_classes), dtype=torch.int32, device=allp.device)
+        C.soft_nms(ptr(rows), ptr(rows), ptr(offs), b, num_classes, n, 5, 0.5, 0.5, 0.001, 2, ptr(fin), stream_ptr(rows))
     keep = torch.empty((b, n), dtype=torch.uint8, device=allp.device)
     C.topk_keep(ptr(rows), b, n, 5, ptr(offs), num_classes, int(max_per_image), ptr(keep), 0, stream_ptr(rows))
-    packed = torch.cat([rows.view(b, -1), keep.float(), offs.float()], dim=1).cpu().numpy()   # one D2H
+    cols = [rows.view(b, -1), keep.float(), offs.float()]
+    if fin is not None:
+        cols.append(fin.float())        # list lengths after soft-NMS (<= 4096: exact in float32)
+    packed = torch.cat(cols, dim=1).cpu().numpy()   # one D2H
     rows_h = packed[:, :n * 5].reshape(b, n, 5)
     keep_h = packed[:, n * 5:n * 6] > 0
-    offs_h = packed[:, n * 6:].astype(np.int64)
+    offs_h = packed[:, n * 6:n * 6 + num_classes + 1].astype(np.int64)
+    if fin is not None and (packed[:, n * 6 + num_classes + 1:] < 0).any():
+        raise RuntimeError("ctdet_merge_device: soft-NMS left a class list unprocessed")
     ret = []
     for i in range(b):
         res = {}

@@ -525,10 +525,12 @@ int cnb_psroi_pooling_backward_f64(const double *grad_out, const double *data, c
  *   extra columns follow soft_nms_39's swap rule).  The array, rows beyond the
  *   final length included, ends exactly as the reference's in-place routine
  *   leaves it; final_n (nullable, [n_img*lists_per_img]) receives len(keep)
- *   (negative: list longer than 1536 rows, left untouched).  out may alias rows
+ *   (negative: list longer than n_cap rows, left untouched).  n_cap <= 4096;
+ *   shared memory is sized from n_cap (27 B per row).  out may alias rows
  *   only when d == 5.  method 0 hard, 1 linear, 2 gaussian.
  * cnb_topk_keep: keep[b,n_cap] = score >= (max_per_image-th largest score of
- *   the image's offsets[b][classes] rows); thresh (nullable) [b]. */
+ *   the image's offsets[b][classes] rows, NaN of either sign ordered above
+ *   +inf as np.partition orders it); thresh (nullable) [b]. */
 int cnb_post_transform(const float *rows, float *out, const double *trans, int b, int n, int d,
                        int a0, int na, int b0, int nb, void *stream);
 int cnb_group_by_class(const float *dets, int b, int n, int num_classes, float *rows,

@@ -68,6 +68,26 @@ def multi_pose_post_process(dets, c, s, h, w):
     return ret
 
 
+def _min(a, b):
+    """nms.pyx:21-22 (`a if a <= b else b`): a NaN `b` is returned, a NaN `a` is not -- unlike Python's min."""
+    return a if a <= b else b
+
+
+def _max(a, b):
+    """nms.pyx:18-19 (`a if a >= b else b`)."""
+    return a if a >= b else b
+
+
+def _pivot(scores, i):
+    """nms.pyx:87-102: `maxscore = boxes[i, 4]`, then `if maxscore < boxes[pos, 4]` over the later rows.  A NaN at
+    row i is never replaced; otherwise the first maximum wins and NaN rows are never picked (np.argmax would take
+    the first NaN)."""
+    s = scores[i:]
+    if np.isnan(s[0]):
+        return i
+    return i + int(np.argmax(np.where(np.isnan(s), -np.inf, s)))
+
+
 def soft_nms(boxes, sigma=0.5, Nt=0.3, threshold=0.001, method=0, ncols_swap=0):
     """external/nms.pyx:77-169 (ncols_swap = 0) and :171-275 (soft_nms_39: ncols_swap = 34 extra columns that are
     SWAPPED where the five box columns are COPIED).  In place on the float32 array; returns the final N.
@@ -77,7 +97,7 @@ def soft_nms(boxes, sigma=0.5, Nt=0.3, threshold=0.001, method=0, ncols_swap=0):
     one = F32(1)
     i = 0
     while i < N:
-        maxpos = i + int(np.argmax(boxes[i:N, 4])) if N > i else i      # first maximum (strict '<' scan)
+        maxpos = _pivot(boxes[:N, 4], i)
         t = boxes[i, :5].copy()
         boxes[i, :5] = boxes[maxpos, :5]
         boxes[maxpos, :5] = t
@@ -93,9 +113,9 @@ def soft_nms(boxes, sigma=0.5, Nt=0.3, threshold=0.001, method=0, ncols_swap=0):
             # rounding on assignment to the `cdef float` (see the generated C of nms.pyx:133-139)
             D = np.float64
             area = F32((D(F32(x2 - x1)) + 1.0) * (D(F32(y2 - y1)) + 1.0))
-            iw = F32(D(F32(min(tx2, x2) - max(tx1, x1))) + 1.0)
+            iw = F32(D(F32(_min(tx2, x2) - _max(tx1, x1))) + 1.0)
             if iw > 0:
-                ih = F32(D(F32(min(ty2, y2) - max(ty1, y1))) + 1.0)
+                ih = F32(D(F32(_min(ty2, y2) - _max(ty1, y1))) + 1.0)
                 if ih > 0:
                     ua = F32(((D(F32(tx2 - tx1)) + 1.0) * (D(F32(ty2 - ty1)) + 1.0) + D(area)) - D(F32(iw * ih)))
                     ov = F32(F32(iw * ih) / ua)

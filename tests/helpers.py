@@ -38,3 +38,40 @@ def assert_dets_equal(ref, got, score_col=4, atol=0.0, positive_only=False, what
             else:
                 np.testing.assert_allclose(a, c, rtol=0, atol=atol, err_msg="%s: rows %d..%d image %d" % (what, k, e, b))
             k = e + 1
+
+
+def assert_same_bits(got, want, what=""):
+    """float32 arrays equal bit for bit (the sign of zero included); NaN matches NaN of any sign or payload (the
+    device's canonical NaN and x86's default NaN differ in their bits, not in what they mean)."""
+    got = np.asarray(got, np.float32); want = np.asarray(want, np.float32)
+    assert got.shape == want.shape, (what, got.shape, want.shape)
+    gn, wn = np.isnan(got), np.isnan(want)
+    bad = (gn != wn) | (~gn & ~wn & (got.view(np.uint32) != want.view(np.uint32)))
+    if bad.any():
+        idx = np.argwhere(bad)
+        i = tuple(idx[0])
+        raise AssertionError("%s: %d of %d elements differ, first at %s: got %r, want %r"
+                             % (what, len(idx), bad.size, i, got[i], want[i]))
+
+
+def flat_results(res, num_classes):
+    """Per-image {class id: [n, 5]} results -> [R, 7] rows (image, class id, x1, y1, x2, y2, score)."""
+    rows = []
+    for i, r in enumerate(res):
+        for j in range(1, num_classes + 1):
+            a = np.asarray(r[j], np.float32).reshape(-1, 5)
+            rows.append(np.concatenate([np.full((len(a), 1), i, np.float32), np.full((len(a), 1), j, np.float32), a], 1))
+    return np.concatenate(rows, 0)
+
+
+def edge_merge_case(g, name):
+    """Inputs of the merge `name` of tests/golden/post_edges.npz: per-scale [B, K, 6] detections, the per-scale
+    metas of ctdet_merge_device (per-image centre and scalar or vector scale), num_classes, max_per_image, nms."""
+    dets, c, s, scalar = g[name + "_dets"], g[name + "_c"], g[name + "_s"], g[name + "_s_scalar"]
+    scales, hw = g[name + "_scales"], g[name + "_hw"]
+    nc, mpi, run_nms = (int(v) for v in g[name + "_cfg"])
+    S, B = dets.shape[0], dets.shape[1]
+    metas = [{"c": [c[k, i] for i in range(B)],
+              "s": [np.float32(s[k, i, 0]) if scalar[i] else s[k, i] for i in range(B)],
+              "out_height": int(hw[k, 0]), "out_width": int(hw[k, 1]), "scale": float(scales[k])} for k in range(S)]
+    return [dets[k] for k in range(S)], metas, nc, mpi, bool(run_nms)
