@@ -11,13 +11,19 @@
 //   4. k_exct_merge: merges the per-group segments of an image, adds the regression offsets
 //      (or 0.5) and writes the 14-column rows (:366-421).
 // Tie order: score desc, tuple index ((i*K+j)*K+k)*K+m asc (torch.topk leaves it open).
+//
+// cnb_exct_decode_ex reads the nine inputs as fp32, fp16 or bf16, the five maps optionally as logits, and returns
+// what the fp32 call returns for the .float() upcast (after torch's CUDA sigmoid, with logits).  Only the steps that
+// read an input change: the selections (plan_map_select: in place in the hot geometry, else one widening / sigmoid
+// pass), the edge aggregation (score_f32 on load), the centre map (k_ct_agnostic / k_ct_scores write its fp32
+// scores) and the regression gathers of k_exct_merge<true>.  k_exct_tuples and the fp32 instances are unchanged.
 #include "select.cuh"
 
 namespace cnb {
 
 typedef unsigned long long u64;
-int launch_edge_aggregate(const float *heat, float *out, int n, int c, int h, int w, float weight, int horizontal,
-                          cudaStream_t stream);
+int launch_edge_aggregate_ex(const void *heat, int dt, bool sigmoid, float *out, int n, int c, int h, int w,
+                             float weight, int horizontal, cudaStream_t stream);
 
 constexpr int EX_THREADS = 512;
 constexpr int EX_CAP = 4096;       // candidate keys per CTA
@@ -65,17 +71,19 @@ __device__ __forceinline__ void sort_desc(u64 *buf, int n) {
 }
 __device__ __forceinline__ int np2(int v) { int n = 2; while (n < v) n <<= 1; return n; }
 
-// max / argmax over classes of the centre map (decode.py:159)
-__global__ void __launch_bounds__(256) k_ct_agnostic(const float *__restrict__ ct, int B, int CC, long long HW,
+// max / argmax over classes of the centre map (decode.py:159), compared as fp32 scores: with SIG the sigmoids,
+// not the logits, so classes whose sigmoids tie (e.g. both saturate to 1) yield the first one, as torch.max does
+template <typename T, bool SIG>
+__global__ void __launch_bounds__(256) k_ct_agnostic(const T *__restrict__ ct, int B, int CC, long long HW,
                                                      float *__restrict__ agn, int32_t *__restrict__ cls) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= (long long)B * HW) return;
   const long long b = i / HW, sp = i - b * HW;
-  const float *p = ct + b * CC * HW + sp;
-  float best = p[0];
+  const T *p = ct + b * CC * HW + sp;
+  float best = score_f32<SIG>(p[0]);
   int arg = 0;
   for (int c = 1; c < CC; ++c) {
-    const float v = p[(long long)c * HW];
+    const float v = score_f32<SIG>(p[(long long)c * HW]);
     if (v > best) { best = v; arg = c; }
   }
   agn[i] = best;
@@ -89,6 +97,28 @@ __global__ void __launch_bounds__(256) k_ct_max(const float *__restrict__ ct, lo
   uint32_t best = 0u;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < per_image; i += (long long)gridDim.x * blockDim.x)
     best = max(best, mono_bits(__ldg(p + i)));
+  for (int k = 16; k > 0; k >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, k));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = best;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < 8; ++i) best = max(best, red[i]);
+    atomicMax(out + blockIdx.y, best);
+  }
+}
+
+// k_ct_max for a centre map that is not an fp32 heat map: also writes its fp32 scores (widened, or the sigmoid of
+// the widened logit) to sc, the map k_exct_tuples then reads
+template <typename T, bool SIG>
+__global__ void __launch_bounds__(256) k_ct_scores(const T *__restrict__ ct, long long per_image, float *__restrict__ sc,
+                                                   uint32_t *__restrict__ out) {
+  __shared__ uint32_t red[8];
+  const long long base = (long long)blockIdx.y * per_image;
+  uint32_t best = 0u;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < per_image; i += (long long)gridDim.x * blockDim.x) {
+    const float v = score_f32<SIG>(__ldg(ct + base + i));
+    sc[base + i] = v;
+    best = max(best, mono_bits(v));
+  }
   for (int k = 16; k > 0; k >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, k));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = best;
   __syncthreads();
@@ -220,7 +250,10 @@ __global__ void __launch_bounds__(EX_THREADS, 1) k_exct_tuples(const ExctArgs a)
   if (tid == 0) a.seg_cnt[(size_t)b * a.groups + grp] = n_out;
 }
 
-__global__ void __launch_bounds__(1024, 1) k_exct_merge(const ExctArgs a) {
+// EX: the regression maps are read by their CNB_DTYPE_* codes rdt (t, l, b, r in x, y, z, w), widened exactly; the
+// regression pointers of `a` are then untyped
+template <bool EX>
+__global__ void __launch_bounds__(1024, 1) k_exct_merge(const ExctArgs a, const int4 rdt) {
   extern __shared__ __align__(16) unsigned char ex_smem[];
   u64 *sbuf = reinterpret_cast<u64 *>(ex_smem);
   const int b = blockIdx.x, tid = threadIdx.x, K = a.K, nd = a.num_dets;
@@ -252,7 +285,14 @@ __global__ void __launch_bounds__(1024, 1) k_exct_merge(const ExctArgs a) {
     } else {
       cls = (float)a.t.clses[oi];
     }
-    if (has_reg) {  // :366-384
+    if (EX && has_reg) {
+      const long long st = a.t.inds[oi], sl = a.l.inds[oj], sb = a.b.inds[ok], sr = a.r.inds[om];
+      const long long x0 = (long long)b * 2 * HW, y0 = ((long long)b * 2 + 1) * HW;
+      tx += ld_head(a.t_regr, rdt.x, x0 + st); ty += ld_head(a.t_regr, rdt.x, y0 + st);
+      lx += ld_head(a.l_regr, rdt.y, x0 + sl); ly += ld_head(a.l_regr, rdt.y, y0 + sl);
+      bx += ld_head(a.b_regr, rdt.z, x0 + sb); by += ld_head(a.b_regr, rdt.z, y0 + sb);
+      rx += ld_head(a.r_regr, rdt.w, x0 + sr); ry += ld_head(a.r_regr, rdt.w, y0 + sr);
+    } else if (has_reg) {  // :366-384
       const long long st = a.t.inds[oi], sl = a.l.inds[oj], sb = a.b.inds[ok], sr = a.r.inds[om];
       tx += a.t_regr[((long long)b * 2) * HW + st]; ty += a.t_regr[((long long)b * 2 + 1) * HW + st];
       lx += a.l_regr[((long long)b * 2) * HW + sl]; ly += a.l_regr[((long long)b * 2 + 1) * HW + sl];
@@ -284,49 +324,111 @@ static int exct_groups(int b, int k) {
   return g < 1 ? 1 : g;
 }
 
-}  // namespace cnb
+// The nine inputs of an exct decode with their CNB_DTYPE_* codes.  `logits`: the five maps hold pre-sigmoid logits.
+struct ExctIn {
+  const void *map[4];   // t, l, b, r
+  const void *ct;
+  const void *regr[4];  // all four or none
+  int map_dt[4], ct_dt, regr_dt[4];
+  int logits;
+};
 
-using namespace cnb;
+// every map and regression head fp32, no logits: the fp32 call, its plan, workspace and launches
+static bool exct_plain(const ExctIn &x) {
+  bool f32 = x.ct_dt == CNB_DTYPE_F32 && !x.logits;
+  for (int q = 0; q < 4; ++q) f32 = f32 && x.map_dt[q] == CNB_DTYPE_F32 && x.regr_dt[q] == CNB_DTYPE_F32;
+  return f32;
+}
 
-extern "C" {
-
-size_t cnb_exct_workspace_bytes(int b, int c, int cc, int h, int w, int k, int num_dets) {
-  SelectPlan pl;
-  if (make_select_plan(nullptr, b, c, h, w, k, 1, &pl) != CNB_OK) return 0;
+// everything after the selection scratch: raw lists, aggregated maps, agnostic centre map, segments, bounds
+static size_t exct_tail_bytes(int b, int c, int h, int w, int k, int num_dets) {
   const int g = exct_groups(b, k);
   const size_t maps = 4 * align_up((size_t)b * c * h * w * 4, 256);       // aggregated maps (aggr_weight > 0)
   const size_t agn = 2 * align_up((size_t)b * h * w * 4, 256);            // class-agnostic centre map
-  (void)cc;
-  return select_workspace_bytes(pl) + 4 * raw_sz((long long)b * k) + maps + agn +
-         align_up((size_t)b * g * num_dets * 8, 256) + align_up((size_t)b * g * 4, 256) + align_up((size_t)b * 4, 256) +
-         align_up((size_t)b * 8, 256);
+  return 4 * raw_sz((long long)b * k) + maps + agn + align_up((size_t)b * g * num_dets * 8, 256) +
+         align_up((size_t)b * g * 4, 256) + align_up((size_t)b * 4, 256) + align_up((size_t)b * 8, 256);
 }
 
-int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_heat, const float *r_heat,
-                    const float *ct_heat, const float *t_regr, const float *l_regr, const float *b_regr,
-                    const float *r_regr, int b, int c, int cc, int h, int w, int k, float scores_thresh,
-                    float center_thresh, float aggr_weight, int num_dets, int agnostic, float *dets, void *workspace,
-                    size_t workspace_bytes, void *stream_) {
-  CNB_REQUIRE(t_heat && l_heat && b_heat && r_heat && ct_heat && dets && workspace, CNB_EINVAL,
-              "cnb_exct_decode: null pointer");
+// Argument checks shared by the calls and the dtype-generic query (no CUDA call)
+static int exct_check(const char *fn, const ExctIn &x, int b, int c, int cc, int h, int w, int k, int num_dets,
+                      int agnostic) {
+  bool known = dtype_known(x.ct_dt);
+  for (int q = 0; q < 4; ++q) known = known && dtype_known(x.map_dt[q]) && dtype_known(x.regr_dt[q]);
+  CNB_REQUIRE(known, CNB_EINVAL, "%s: unknown dtype code (t %d, l %d, b %d, r %d, ct %d, regr %d %d %d %d)", fn,
+              x.map_dt[0], x.map_dt[1], x.map_dt[2], x.map_dt[3], x.ct_dt, x.regr_dt[0], x.regr_dt[1], x.regr_dt[2],
+              x.regr_dt[3]);
+  CNB_REQUIRE(x.map[0] && x.map[1] && x.map[2] && x.map[3] && x.ct, CNB_EINVAL, "%s: null pointer", fn);
   CNB_REQUIRE(b > 0 && c > 0 && cc > 0 && h > 0 && w > 0 && k > 0 && num_dets > 0, CNB_EINVAL,
-              "cnb_exct_decode: non-positive dimension");
-  CNB_REQUIRE(agnostic || cc == c, CNB_EINVAL, "cnb_exct_decode: centre map has %d classes, extreme maps %d", cc, c);
-  CNB_REQUIRE(k <= 255, CNB_EUNSUPPORTED, "cnb_exct_decode: k=%d (k^4 must fit 32 bits)", k);
+              "%s: non-positive dimension", fn);
+  CNB_REQUIRE(agnostic || cc == c, CNB_EINVAL, "%s: centre map has %d classes, extreme maps %d", fn, cc, c);
+  CNB_REQUIRE(k <= 255, CNB_EUNSUPPORTED, "%s: k=%d (k^4 must fit 32 bits)", fn, k);
   const long long k4 = (long long)k * k * k * k;
-  CNB_REQUIRE(num_dets <= k4, CNB_EINVAL, "cnb_exct_decode: num_dets=%d exceeds k^4=%lld (torch.topk would raise)",
-              num_dets, k4);
-  CNB_REQUIRE(num_dets <= EX_MAX_DETS, CNB_EUNSUPPORTED, "cnb_exct_decode: num_dets=%d > %d", num_dets, EX_MAX_DETS);
-  CNB_REQUIRE(workspace_bytes >= cnb_exct_workspace_bytes(b, c, cc, h, w, k, num_dets), CNB_EWORKSPACE,
-              "cnb_exct_decode: workspace %zu < %zu", workspace_bytes,
-              cnb_exct_workspace_bytes(b, c, cc, h, w, k, num_dets));
-  cudaStream_t stream = (cudaStream_t)stream_;
-  SelectPlan pl;
-  int rc = make_select_plan(t_heat, b, c, h, w, k, 1, &pl);
+  CNB_REQUIRE(num_dets <= k4, CNB_EINVAL, "%s: num_dets=%d exceeds k^4=%lld (torch.topk would raise)", fn, num_dets,
+              k4);
+  CNB_REQUIRE(num_dets <= EX_MAX_DETS, CNB_EUNSUPPORTED, "%s: num_dets=%d > %d", fn, num_dets, EX_MAX_DETS);
+  return CNB_OK;
+}
+
+// Plans of the four selections of a non-plain decode and the largest scratch they need.  Each selection reads its
+// map (in place, or through the fp32 copy at `copy`), or with aggregation the fp32 aggregated map agg[q].  The query
+// passes null agg / copy: 16-byte aligned places.
+static int exct_plans(const ExctIn &x, bool aggr, float *const agg[4], const float *copy, int b, int c, int h, int w,
+                      int k, MapSelect m[4], size_t *sel) {
+  *sel = 0;
+  for (int q = 0; q < 4; ++q) {
+    const int rc = aggr ? plan_map_select(agg[q], CNB_DTYPE_F32, 0, b, c, h, w, k, copy, &m[q])
+                        : plan_map_select(x.map[q], x.map_dt[q], x.logits, b, c, h, w, k, copy, &m[q]);
+    if (rc != CNB_OK) return rc;
+    m[q].pl.clamp_one = 1;   // decode.py:299-302: values above 1 are clamped before _topk
+    if (m[q].sel_bytes > *sel) *sel = m[q].sel_bytes;
+  }
+  return CNB_OK;
+}
+
+template <typename T>
+static void launch_ct_agnostic(const void *ct, bool sig, int b, int cc, long long hw, float *agn, int32_t *cls,
+                               cudaStream_t stream) {
+  const long long n = (long long)b * hw;
+  const T *p = reinterpret_cast<const T *>(ct);
+  if (sig) k_ct_agnostic<T, true><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p, b, cc, hw, agn, cls);
+  else k_ct_agnostic<T, false><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p, b, cc, hw, agn, cls);
+}
+
+template <typename T>
+static void launch_ct_scores(const void *ct, bool sig, dim3 grid, long long per, float *sc, uint32_t *mx,
+                             cudaStream_t stream) {
+  const T *p = reinterpret_cast<const T *>(ct);
+  if (sig) k_ct_scores<T, true><<<grid, 256, 0, stream>>>(p, per, sc, mx);
+  else k_ct_scores<T, false><<<grid, 256, 0, stream>>>(p, per, sc, mx);
+}
+
+// The host body of cnb_exct_decode (exct_plain(x): its fp32 plan, workspace and launches) and cnb_exct_decode_ex
+static int exct_decode(const char *fn, const ExctIn &x, int b, int c, int cc, int h, int w, int k, float scores_thresh,
+                       float center_thresh, float aggr_weight, int num_dets, int agnostic, float *dets, void *workspace,
+                       size_t workspace_bytes, cudaStream_t stream) {
+  int rc = exct_check(fn, x, b, c, cc, h, w, k, num_dets, agnostic);
   if (rc != CNB_OK) return rc;
-  pl.clamp_one = 1;   // decode.py:299-302: values above 1 are clamped before _topk
+  CNB_REQUIRE(dets && workspace, CNB_EINVAL, "%s: null pointer", fn);
+  const bool plain = exct_plain(x), aggr = aggr_weight > 0.0f;
+  SelectPlan pl;
+  MapSelect ms[4];
+  size_t sel = 0;
+  if (plain) {
+    CNB_REQUIRE(workspace_bytes >= cnb_exct_workspace_bytes(b, c, cc, h, w, k, num_dets), CNB_EWORKSPACE,
+                "%s: workspace %zu < %zu", fn, workspace_bytes, cnb_exct_workspace_bytes(b, c, cc, h, w, k, num_dets));
+    rc = make_select_plan(x.map[0], b, c, h, w, k, 1, &pl);
+    if (rc != CNB_OK) return rc;
+    pl.clamp_one = 1;   // decode.py:299-302: values above 1 are clamped before _topk
+    sel = select_workspace_bytes(pl);
+  } else {
+    float *const none[4] = {nullptr, nullptr, nullptr, nullptr};
+    rc = exct_plans(x, aggr, none, nullptr, b, c, h, w, k, ms, &sel);
+    if (rc != CNB_OK) return rc;
+    const size_t need = sel + exct_tail_bytes(b, c, h, w, k, num_dets);
+    CNB_REQUIRE(workspace_bytes >= need, CNB_EWORKSPACE, "%s: workspace %zu < %zu", fn, workspace_bytes, need);
+  }
   char *p = reinterpret_cast<char *>(workspace);
-  void *sel_ws = p; p += select_workspace_bytes(pl);
+  void *sel_ws = p; p += sel;
   ExctArgs a;
   a.t = carve(p, (long long)b * k); a.l = carve(p, (long long)b * k);
   a.b = carve(p, (long long)b * k); a.r = carve(p, (long long)b * k);
@@ -341,31 +443,46 @@ int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_hea
   uint32_t *ct_max = reinterpret_cast<uint32_t *>(p); p += align_up((size_t)b * 4, 256);
   a.ct_max = ct_max;
   a.gthr = reinterpret_cast<u64 *>(p);
+  if (!plain) {   // the plans where the aggregated maps and the fp32 copy (agg[0], free without aggregation) really lie
+    size_t sel2 = 0;
+    rc = exct_plans(x, aggr, agg, agg[0], b, c, h, w, k, ms, &sel2);
+    if (rc != CNB_OK) return rc;
+    CNB_REQUIRE(sel2 <= sel, CNB_EWORKSPACE, "%s: selection scratch %zu > %zu", fn, sel2, sel);
+  }
   CNB_CUDA(cudaMemsetAsync(a.gthr, 0, (size_t)b * 8, stream));
 
-  const float *maps[4] = {t_heat, l_heat, b_heat, r_heat};
-  if (aggr_weight > 0.0f) {   // :287-291: t,b horizontal; l,r vertical
+  const void *maps[4] = {x.map[0], x.map[1], x.map[2], x.map[3]};
+  if (aggr) {   // :287-291: t,b horizontal; l,r vertical
     const int horiz[4] = {1, 0, 1, 0};
     for (int q = 0; q < 4; ++q) {
-      rc = launch_edge_aggregate(maps[q], agg[q], b, c, h, w, aggr_weight, horiz[q], stream);
+      rc = launch_edge_aggregate_ex(maps[q], x.map_dt[q], x.logits != 0, agg[q], b, c, h, w, aggr_weight, horiz[q],
+                                    stream);
       if (rc != CNB_OK) return rc;
       maps[q] = agg[q];
     }
   }
   RawList *lists[4] = {&a.t, &a.l, &a.b, &a.r};
   for (int q = 0; q < 4; ++q) {
-    SelectPlan pq = pl;
-    pq.use_tma = pq.use_tma && ((reinterpret_cast<uintptr_t>(maps[q]) & 15u) == 0);
-    if (!pq.use_tma) { pq.hot = 0; pq.seg_cap = pq.K; }
     FinalizeOut o = {lists[q]->scores, lists[q]->inds, lists[q]->clses, lists[q]->ys, lists[q]->xs,
                      nullptr, nullptr, 0, nullptr};
-    rc = run_select(maps[q], pq, o, sel_ws, stream);
+    if (plain) {
+      SelectPlan pq = pl;
+      pq.use_tma = pq.use_tma && ((reinterpret_cast<uintptr_t>(maps[q]) & 15u) == 0);
+      if (!pq.use_tma) { pq.hot = 0; pq.seg_cap = pq.K; }
+      rc = run_select(maps[q], pq, o, sel_ws, stream);
+    } else {   // stream order: each selection is done with the scratch and the copy before the next one starts
+      rc = aggr ? run_map_select(maps[q], CNB_DTYPE_F32, 0, ms[q], agg[0], o, sel_ws, stream)
+                : run_map_select(maps[q], x.map_dt[q], x.logits, ms[q], agg[0], o, sel_ws, stream);
+    }
     if (rc != CNB_OK) return rc;
   }
-  a.ct_heat = ct_heat; a.ct_agn = nullptr; a.ct_cls = nullptr;
+  // centre map; the selections are done with agg[0], which may now hold its fp32 scores
+  const bool sig = x.logits != 0;
+  a.ct_heat = reinterpret_cast<const float *>(x.ct); a.ct_agn = nullptr; a.ct_cls = nullptr;
   if (agnostic) {
-    const long long n = (long long)b * h * w;
-    k_ct_agnostic<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(ct_heat, b, cc, (long long)h * w, agn, agn_cls);
+    if (x.ct_dt == CNB_DTYPE_BF16) launch_ct_agnostic<__nv_bfloat16>(x.ct, sig, b, cc, (long long)h * w, agn, agn_cls, stream);
+    else if (x.ct_dt == CNB_DTYPE_F16) launch_ct_agnostic<__half>(x.ct, sig, b, cc, (long long)h * w, agn, agn_cls, stream);
+    else launch_ct_agnostic<float>(x.ct, sig, b, cc, (long long)h * w, agn, agn_cls, stream);
     CNB_CHECK_LAUNCH("cnb_exct_decode agnostic centre");
     count_launch();
     a.ct_agn = agn; a.ct_cls = agn_cls;
@@ -376,11 +493,21 @@ int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_hea
     int blocks = (int)((per + 256 * 8 - 1) / (256 * 8));
     if (blocks > 64) blocks = 64;
     if (blocks < 1) blocks = 1;
-    k_ct_max<<<dim3((unsigned)blocks, (unsigned)b), 256, 0, stream>>>(agnostic ? agn : ct_heat, per, ct_max);
+    const dim3 grid((unsigned)blocks, (unsigned)b);
+    if (agnostic || (x.ct_dt == CNB_DTYPE_F32 && !sig)) {
+      k_ct_max<<<grid, 256, 0, stream>>>(agnostic ? agn : a.ct_heat, per, ct_max);
+    } else {   // one pass: the fp32 scores of the centre map (into agg[0]) and their maximum
+      if (x.ct_dt == CNB_DTYPE_BF16) launch_ct_scores<__nv_bfloat16>(x.ct, sig, grid, per, agg[0], ct_max, stream);
+      else if (x.ct_dt == CNB_DTYPE_F16) launch_ct_scores<__half>(x.ct, sig, grid, per, agg[0], ct_max, stream);
+      else launch_ct_scores<float>(x.ct, sig, grid, per, agg[0], ct_max, stream);
+      a.ct_heat = agg[0];
+    }
     CNB_CHECK_LAUNCH("cnb_exct_decode centre maximum");
     count_launch();
   }
-  a.t_regr = t_regr; a.l_regr = l_regr; a.b_regr = b_regr; a.r_regr = r_regr;
+  const bool has_reg = x.regr[0] && x.regr[1] && x.regr[2] && x.regr[3];
+  a.t_regr = reinterpret_cast<const float *>(x.regr[0]); a.l_regr = reinterpret_cast<const float *>(x.regr[1]);
+  a.b_regr = reinterpret_cast<const float *>(x.regr[2]); a.r_regr = reinterpret_cast<const float *>(x.regr[3]);
   a.B = b; a.CC = cc; a.H = h; a.W = w; a.K = k; a.num_dets = num_dets; a.groups = groups; a.agnostic = agnostic;
   a.scores_thresh = scores_thresh; a.center_thresh = center_thresh; a.dets = dets;
   const size_t smem1 = (size_t)EX_CAP * 8 + (size_t)16 * k * 4;
@@ -390,11 +517,76 @@ int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_hea
   int n2 = 2;
   while (n2 < groups * num_dets) n2 <<= 1;
   const size_t smem2 = (size_t)n2 * 8;
-  CNB_CUDA(cudaFuncSetAttribute(k_exct_merge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-  k_exct_merge<<<b, 1024, smem2, stream>>>(a);
+  // fp32 regression maps (or none) take the fp32 merge
+  const bool typed = has_reg && !(x.regr_dt[0] == CNB_DTYPE_F32 && x.regr_dt[1] == CNB_DTYPE_F32 &&
+                                  x.regr_dt[2] == CNB_DTYPE_F32 && x.regr_dt[3] == CNB_DTYPE_F32);
+  if (typed) {
+    CNB_CUDA(cudaFuncSetAttribute(k_exct_merge<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    k_exct_merge<true><<<b, 1024, smem2, stream>>>(a, make_int4(x.regr_dt[0], x.regr_dt[1], x.regr_dt[2], x.regr_dt[3]));
+  } else {
+    CNB_CUDA(cudaFuncSetAttribute(k_exct_merge<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    k_exct_merge<false><<<b, 1024, smem2, stream>>>(a, make_int4(0, 0, 0, 0));
+  }
   CNB_CHECK_LAUNCH("cnb_exct_decode merge");
   count_launch(2);
   return CNB_OK;
+}
+
+}  // namespace cnb
+
+using namespace cnb;
+
+extern "C" {
+
+size_t cnb_exct_workspace_bytes(int b, int c, int cc, int h, int w, int k, int num_dets) {
+  SelectPlan pl;
+  if (make_select_plan(nullptr, b, c, h, w, k, 1, &pl) != CNB_OK) return 0;
+  (void)cc;
+  return select_workspace_bytes(pl) + exct_tail_bytes(b, c, h, w, k, num_dets);
+}
+
+int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_heat, const float *r_heat,
+                    const float *ct_heat, const float *t_regr, const float *l_regr, const float *b_regr,
+                    const float *r_regr, int b, int c, int cc, int h, int w, int k, float scores_thresh,
+                    float center_thresh, float aggr_weight, int num_dets, int agnostic, float *dets, void *workspace,
+                    size_t workspace_bytes, void *stream) {
+  const int f = CNB_DTYPE_F32;
+  const ExctIn x = {{t_heat, l_heat, b_heat, r_heat}, ct_heat, {t_regr, l_regr, b_regr, r_regr}, {f, f, f, f}, f,
+                    {f, f, f, f}, 0};
+  return exct_decode("cnb_exct_decode", x, b, c, cc, h, w, k, scores_thresh, center_thresh, aggr_weight, num_dets,
+                     agnostic, dets, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t cnb_exct_decode_ex_workspace_bytes(const void *t_heat, const void *l_heat, const void *b_heat,
+                                          const void *r_heat, int t_dtype, int l_dtype, int b_dtype, int r_dtype,
+                                          int ct_dtype, int t_regr_dtype, int l_regr_dtype, int b_regr_dtype,
+                                          int r_regr_dtype, int logits, int b, int c, int cc, int h, int w, int k,
+                                          float aggr_weight, int num_dets, int agnostic) {
+  const int one = 1;   // the centre map's pointer does not enter the workspace: any non-null value
+  const ExctIn x = {{t_heat, l_heat, b_heat, r_heat}, &one, {nullptr, nullptr, nullptr, nullptr},
+                    {t_dtype, l_dtype, b_dtype, r_dtype}, ct_dtype,
+                    {t_regr_dtype, l_regr_dtype, b_regr_dtype, r_regr_dtype}, logits ? 1 : 0};
+  if (exct_check("cnb_exct_decode_ex", x, b, c, cc, h, w, k, num_dets, agnostic) != CNB_OK) return 0;
+  if (exct_plain(x)) return cnb_exct_workspace_bytes(b, c, cc, h, w, k, num_dets);
+  MapSelect m[4];
+  size_t sel = 0;
+  float *const none[4] = {nullptr, nullptr, nullptr, nullptr};
+  if (exct_plans(x, aggr_weight > 0.0f, none, nullptr, b, c, h, w, k, m, &sel) != CNB_OK) return 0;
+  return sel + exct_tail_bytes(b, c, h, w, k, num_dets);
+}
+
+int cnb_exct_decode_ex(const void *t_heat, int t_dtype, const void *l_heat, int l_dtype, const void *b_heat,
+                       int b_dtype, const void *r_heat, int r_dtype, const void *ct_heat, int ct_dtype,
+                       const void *t_regr, int t_regr_dtype, const void *l_regr, int l_regr_dtype, const void *b_regr,
+                       int b_regr_dtype, const void *r_regr, int r_regr_dtype, int logits, int b, int c, int cc,
+                       int h, int w, int k, float scores_thresh, float center_thresh, float aggr_weight,
+                       int num_dets, int agnostic, float *dets, void *workspace, size_t workspace_bytes,
+                       void *stream) {
+  const ExctIn x = {{t_heat, l_heat, b_heat, r_heat}, ct_heat, {t_regr, l_regr, b_regr, r_regr},
+                    {t_dtype, l_dtype, b_dtype, r_dtype}, ct_dtype,
+                    {t_regr_dtype, l_regr_dtype, b_regr_dtype, r_regr_dtype}, logits ? 1 : 0};
+  return exct_decode("cnb_exct_decode_ex", x, b, c, cc, h, w, k, scores_thresh, center_thresh, aggr_weight, num_dets,
+                     agnostic, dets, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -196,7 +196,31 @@ PYBIND11_MODULE(_C, m) {
     check(cnb_edge_aggregate(ptr<const float>(heat), ptr<float>(out), n, c, h, w, wt, horizontal, ptr<void>(stream)),
           "cnb_edge_aggregate");
   });
+  m.def("edge_aggregate_ex", [](P heat, int dt, int sig, P out, int n, int c, int h, int w, float wt, int horizontal,
+                                P stream) {
+    check(cnb_edge_aggregate_ex(ptr<const void>(heat), dt, sig, ptr<float>(out), n, c, h, w, wt, horizontal,
+                                ptr<void>(stream)),
+          "cnb_edge_aggregate_ex");
+  });
   m.def("exct_workspace_bytes", &cnb_exct_workspace_bytes);
+  m.def("exct_decode_ex_workspace_bytes", [](P t, P l, P b_, P r, int t_dt, int l_dt, int b_dt, int r_dt, int ct_dt,
+                                             int tr_dt, int lr_dt, int br_dt, int rr_dt, int logits, int b, int c,
+                                             int cc, int h, int w, int k, float aw, int nd, int agn) {
+    return cnb_exct_decode_ex_workspace_bytes(ptr<const void>(t), ptr<const void>(l), ptr<const void>(b_),
+                                              ptr<const void>(r), t_dt, l_dt, b_dt, r_dt, ct_dt, tr_dt, lr_dt, br_dt,
+                                              rr_dt, logits, b, c, cc, h, w, k, aw, nd, agn);
+  });
+  m.def("exct_decode_ex", [](P t, int t_dt, P l, int l_dt, P b_, int b_dt, P r, int r_dt, P ct, int ct_dt, P tr,
+                             int tr_dt, P lr, int lr_dt, P br, int br_dt, P rr, int rr_dt, int logits, int b, int c,
+                             int cc, int h, int w, int k, float st, float cth, float aw, int nd, int agn, P dets, P ws,
+                             size_t wsb, P stream) {
+    check(cnb_exct_decode_ex(ptr<const void>(t), t_dt, ptr<const void>(l), l_dt, ptr<const void>(b_), b_dt,
+                             ptr<const void>(r), r_dt, ptr<const void>(ct), ct_dt, ptr<const void>(tr), tr_dt,
+                             ptr<const void>(lr), lr_dt, ptr<const void>(br), br_dt, ptr<const void>(rr), rr_dt,
+                             logits, b, c, cc, h, w, k, st, cth, aw, nd, agn, ptr<float>(dets), ptr<void>(ws), wsb,
+                             ptr<void>(stream)),
+          "cnb_exct_decode_ex");
+  });
   m.def("exct_decode", [](P t, P l, P b_, P r, P ct, P tr, P lr, P br, P rr, int b, int c, int cc, int h, int w,
                           int k, float st, float cth, float aw, int nd, int agn, P dets, P ws, size_t wsb, P stream) {
     check(cnb_exct_decode(ptr<const float>(t), ptr<const float>(l), ptr<const float>(b_), ptr<const float>(r),

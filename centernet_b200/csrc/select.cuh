@@ -95,6 +95,13 @@ int run_map_select(const void *src, int dt, int logits, const MapSelect &m, floa
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
 __device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+// A score-map element as fp32: the exact widening, or (SIG: the element is a logit) torch's CUDA sigmoid of it,
+// 1 / (1 + exp(-x)) on the widened value (the expression of k_sigmoid).
+template <bool SIG, typename T>
+__device__ __forceinline__ float score_f32(T v) {
+  const float x = to_f32(v);
+  return SIG ? 1.0f / (1.0f + expf(-x)) : x;
+}
 // Element i of a head of dtype code dt, widened (the decode epilogues gather K rows per image: a runtime switch, no
 // template instances).
 __device__ __forceinline__ float ld_head(const void *p, int dt, size_t i) {

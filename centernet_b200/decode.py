@@ -3,10 +3,11 @@
 Every function takes fp32 CUDA tensors (NCHW; heat maps already sigmoided by the
 caller, as in detectors/ctdet.py:31,40), does not mutate its inputs, and returns a new
 fp32 tensor on the same device, enqueued on the current stream.  Other dtypes are upcast
-to fp32 first, except in ctdet_decode, multi_pose_decode, ddd_decode, their *_from_logits
-forms, flip_merge (and so the *_flip_from_logits wrappers) and ctdet_decode_from_host: they
-read bf16 and fp16 heads in place, and return, bit for bit, what they return for the .float()
-upcast.  The work is done by
+to fp32 first, except in ctdet_decode, multi_pose_decode, ddd_decode, exct_decode,
+agnex_ct_decode, their *_from_logits forms, the edge aggregation helpers (_h_aggregate,
+_v_aggregate, _left/_right/_top/_bottom_aggregate), flip_merge (and so the *_flip_from_logits
+wrappers) and ctdet_decode_from_host: they read bf16 and fp16 heads in place, and return, bit
+for bit, what they return for the .float() upcast.  The work is done by
 the hand-written sm_90a kernels behind ``include/centernet_b200.h``; there is no
 CPU path (non-CUDA inputs raise NotImplementedError).
 
@@ -40,10 +41,14 @@ def _nms(heat, kernel=3):
 # ------------------------------------------------------------------ decode.py:17-77
 def _aggregate(heat, aggr_weight, horizontal):
     require_cuda(heat, what="_aggregate")
-    heat = f32c(heat)
+    heat = floatc(heat)
     b, c, h, w = _dims(heat)
-    out = torch.empty_like(heat)
-    C.edge_aggregate(ptr(heat), ptr(out), b, c, h, w, float(aggr_weight), int(horizontal), stream_ptr(heat))
+    out = torch.empty(heat.shape, dtype=torch.float32, device=heat.device)
+    if heat.dtype == torch.float32:
+        C.edge_aggregate(ptr(heat), ptr(out), b, c, h, w, float(aggr_weight), int(horizontal), stream_ptr(heat))
+    else:  # a bf16 / fp16 map is read in place; the fp32 result equals that of its .float() upcast
+        C.edge_aggregate_ex(ptr(heat), dtype_code(heat), 0, ptr(out), b, c, h, w, float(aggr_weight), int(horizontal),
+                            stream_ptr(heat))
     return out
 
 
@@ -79,12 +84,7 @@ def _bottom_aggregate(heat):
 
 def _directional(heat, direction):
     # weight=1 with the opposite direction disabled is encoded as horizontal = 2 + direction
-    require_cuda(heat, what="_aggregate")
-    heat = f32c(heat)
-    b, c, h, w = _dims(heat)
-    out = torch.empty_like(heat)
-    C.edge_aggregate(ptr(heat), ptr(out), b, c, h, w, 1.0, 2 + direction, stream_ptr(heat))
-    return out
+    return _aggregate(heat, 1.0, 2 + direction)
 
 
 # ------------------------------------------------------------------ decode.py:92-119
@@ -344,19 +344,30 @@ def multi_pose_decode_from_logits(hm, wh, hps, reg=None, hm_hp=None, hp_offset=N
 
 # ------------------------------------------------------------------ decode.py:122-424
 def _exct(t_heat, l_heat, b_heat, r_heat, ct_heat, regs, K, scores_thresh, center_thresh, aggr_weight, num_dets,
-          agnostic, name):
+          agnostic, name, logits=0):
     require_cuda(t_heat, l_heat, b_heat, r_heat, ct_heat, *regs, what=name)
-    t_heat, l_heat, b_heat, r_heat, ct_heat = [f32c(t) for t in (t_heat, l_heat, b_heat, r_heat, ct_heat)]
+    t_heat, l_heat, b_heat, r_heat, ct_heat = [floatc(t) for t in (t_heat, l_heat, b_heat, r_heat, ct_heat)]
     b, c, h, w = _dims(t_heat)
     cc = int(ct_heat.shape[1])
     for t in (l_heat, b_heat, r_heat):
         if tuple(t.shape) != (b, c, h, w):
             raise RuntimeError("%s: extreme-point heat maps must share one shape" % name)
     if all(r is not None for r in regs):  # decode.py:366-367: all four or none
-        regs = [f32c(r) for r in regs]
+        regs = [floatc(r) for r in regs]
     else:
         regs = [None] * 4
     dets = torch.empty((b, num_dets, 14), dtype=torch.float32, device=t_heat.device)
+    maps = (t_heat, l_heat, b_heat, r_heat)
+    if logits or not _all_f32(*maps, ct_heat, *regs):  # cnb_exct_decode_ex: each input its own dtype
+        inputs = maps + (ct_heat,) + tuple(regs)
+        codes = [dtype_code(t) for t in inputs]
+        nb = C.exct_decode_ex_workspace_bytes(*[ptr(t) for t in maps], *codes, int(logits), b, c, cc, h, w, K,
+                                              float(aggr_weight), int(num_dets), int(agnostic))
+        ws = workspace(nb, t_heat.device)
+        C.exct_decode_ex(*[a for t, dt in zip(inputs, codes) for a in (ptr(t), dt)], int(logits), b, c, cc, h, w, K,
+                         float(scores_thresh), float(center_thresh), float(aggr_weight), int(num_dets), int(agnostic),
+                         ptr(dets), ptr(ws), ws.numel(), stream_ptr(t_heat))
+        return dets
     ws = workspace(C.exct_workspace_bytes(b, c, cc, h, w, K, num_dets), t_heat.device)
     C.exct_decode(ptr(t_heat), ptr(l_heat), ptr(b_heat), ptr(r_heat), ptr(ct_heat), ptr(regs[0]), ptr(regs[1]),
                   ptr(regs[2]), ptr(regs[3]), b, c, cc, h, w, K, float(scores_thresh), float(center_thresh),
@@ -367,14 +378,37 @@ def _exct(t_heat, l_heat, b_heat, r_heat, ct_heat, regs, K, scores_thresh, cente
 
 def agnex_ct_decode(t_heat, l_heat, b_heat, r_heat, ct_heat, t_regr=None, l_regr=None, b_regr=None, r_regr=None,
                     K=40, scores_thresh=0.1, center_thresh=0.1, aggr_weight=0.0, num_dets=1000):
+    """bf16 / fp16 maps and regression heads (each its own dtype) are read in place: the dets equal, bit for bit,
+    those of the .float() upcast."""
     return _exct(t_heat, l_heat, b_heat, r_heat, ct_heat, (t_regr, l_regr, b_regr, r_regr), K, scores_thresh,
                  center_thresh, aggr_weight, num_dets, True, "agnex_ct_decode")
 
 
 def exct_decode(t_heat, l_heat, b_heat, r_heat, ct_heat, t_regr=None, l_regr=None, b_regr=None, r_regr=None,
                 K=40, scores_thresh=0.1, center_thresh=0.1, aggr_weight=0.0, num_dets=1000):
+    """bf16 / fp16 maps and regression heads (each its own dtype) are read in place: the dets equal, bit for bit,
+    those of the .float() upcast."""
     return _exct(t_heat, l_heat, b_heat, r_heat, ct_heat, (t_regr, l_regr, b_regr, r_regr), K, scores_thresh,
                  center_thresh, aggr_weight, num_dets, False, "exct_decode")
+
+
+def agnex_ct_decode_from_logits(t, l, b, r, ct, t_regr=None, l_regr=None, b_regr=None, r_regr=None, K=40,
+                                scores_thresh=0.1, center_thresh=0.1, aggr_weight=0.0, num_dets=1000):
+    """`agnex_ct_decode` on torch's sigmoid of the five maps, read as raw logits; see exct_decode_from_logits."""
+    return _exct(t, l, b, r, ct, (t_regr, l_regr, b_regr, r_regr), K, scores_thresh, center_thresh, aggr_weight,
+                 num_dets, True, "agnex_ct_decode_from_logits", logits=1)
+
+
+def exct_decode_from_logits(t, l, b, r, ct, t_regr=None, l_regr=None, b_regr=None, r_regr=None, K=40,
+                            scores_thresh=0.1, center_thresh=0.1, aggr_weight=0.0, num_dets=1000):
+    """`exct_decode(t.sigmoid_(), l.sigmoid_(), b.sigmoid_(), r.sigmoid_(), ct.sigmoid_(), ...)` (detectors/exdet.py:
+    32-36) on the raw logits of the five maps, without the five full-map sigmoid passes: in the hot geometry the four
+    selections run in logit space, and the edge aggregation and the centre map apply the sigmoid as they load.  The
+    dets equal, bit for bit and filler rows included, those of exct_decode on torch's CUDA sigmoid of the five maps;
+    no input is modified.  bf16 / fp16 inputs are read in place, widened exactly and processed as fp32 (the
+    reference's `sigmoid_()` on a half tensor would round the scores to half precision first)."""
+    return _exct(t, l, b, r, ct, (t_regr, l_regr, b_regr, r_regr), K, scores_thresh, center_thresh, aggr_weight,
+                 num_dets, False, "exct_decode_from_logits", logits=1)
 
 
 # ------------------------------------------------------------------ host-buffer entry (end-to-end path)

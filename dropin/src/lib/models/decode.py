@@ -9,4 +9,5 @@ from centernet_b200.decode import (  # noqa: F401
     _h_aggregate, _v_aggregate, agnex_ct_decode, exct_decode, ddd_decode, ctdet_decode, multi_pose_decode,
     _gather_feat, _transpose_and_gather_feat,
     # extras: fused-sigmoid variants (INTEGRATION.md section 1)
-    ctdet_decode_from_logits, multi_pose_decode_from_logits, ddd_decode_from_logits)
+    ctdet_decode_from_logits, multi_pose_decode_from_logits, ddd_decode_from_logits, exct_decode_from_logits,
+    agnex_ct_decode_from_logits)

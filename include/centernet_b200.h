@@ -43,7 +43,7 @@ extern "C" {
 #define CNB_EWORKSPACE 4   /* workspace_bytes smaller than cnb_*_workspace_bytes */
 
 /* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16, cnb_ctdet_decode_ex,
- * cnb_flip_merge_ex, cnb_ddd_decode_ex, cnb_multi_pose_decode_ex). */
+ * cnb_flip_merge_ex, cnb_ddd_decode_ex, cnb_multi_pose_decode_ex, cnb_edge_aggregate_ex, cnb_exct_decode_ex). */
 #define CNB_DTYPE_F32 0
 #define CNB_DTYPE_BF16 1
 #define CNB_DTYPE_F16 2
@@ -214,6 +214,13 @@ int cnb_multi_pose_decode_ex(const void *heat, int heat_dtype, int logits, const
  * Strictly sequential fp32 running sums, as the reference. */
 int cnb_edge_aggregate(const float *heat, float *out, int n, int c, int h, int w,
                        float aggr_weight, int horizontal, void *stream);
+/* The same for a heat map of dtype code dtype (CNB_DTYPE_F32 / _F16 / _BF16), or for its logits (apply_sigmoid):
+ * every element is widened exactly to fp32, then (apply_sigmoid) put through torch's CUDA sigmoid, and the fp32 out
+ * equals, bit for bit, cnb_edge_aggregate of the .float() upcast (of torch.sigmoid of it).  horizontal also takes
+ * the direction codes 2..5 (left, right, top, bottom: raw ret - heat).  CNB_EINVAL for an unknown dtype code, a
+ * null pointer, in-place use, a non-positive dimension or a bad direction code, before any CUDA call. */
+int cnb_edge_aggregate_ex(const void *heat, int dtype, int apply_sigmoid, float *out, int n, int c, int h, int w,
+                          float aggr_weight, int horizontal, void *stream);
 
 /* ------------------------------------------- A8: exct_decode / agnex_ct_decode
  * models/decode.py:273-424 and :122-271.  t,l,b,r heat [b,c,h,w] (c==1 for
@@ -227,6 +234,34 @@ int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_hea
                     float scores_thresh, float center_thresh, float aggr_weight,
                     int num_dets, int agnostic, float *dets,
                     void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------ N1: exct_decode / agnex_ct_decode of fp32, fp16 or bf16 inputs, from the logits
+ * cnb_exct_decode for inputs of any of the three float types, each of the four extreme maps, the centre map and the
+ * four regression maps with its own dtype code (a null regression map's code must still be a known one).  logits != 0
+ * replaces the `sigmoid_()` of the five maps (detectors/exdet.py:32-36): they hold logits.  Contract: the dets, bit
+ * for bit and filler rows included, are those of cnb_exct_decode on the .float() upcast of the inputs (after
+ * torch's CUDA sigmoid of the five maps, with logits).  Half inputs are widened exactly and then processed as fp32.
+ * Each selection reads its map in place in the hot geometry (h = w = 128, k <= 256, 16-byte aligned) and when it is
+ * an fp32 heat map; otherwise one pass writes its fp32 copy (or sigmoid) into the workspace, one copy shared by the
+ * four selections.  With aggr_weight > 0 the aggregation reads the maps in their dtype and the selections read the
+ * fp32 aggregated maps.  A centre map that is not an fp32 heat map is read in its dtype by the agnostic max /
+ * argmax, or written once as fp32 scores into the workspace.  The query takes the four extreme-map pointers because
+ * their alignment decides the path; with every code CNB_DTYPE_F32 and logits == 0 it equals
+ * cnb_exct_workspace_bytes, and it returns 0 for every argument the call rejects.  Errors, checked before any CUDA
+ * call: CNB_EINVAL for an unknown dtype code, a null pointer or a bad shape, CNB_EUNSUPPORTED for k > 255 or
+ * num_dets > 2048, CNB_EWORKSPACE for too small a workspace. */
+size_t cnb_exct_decode_ex_workspace_bytes(const void *t_heat, const void *l_heat, const void *b_heat,
+                                          const void *r_heat, int t_dtype, int l_dtype, int b_dtype, int r_dtype,
+                                          int ct_dtype, int t_regr_dtype, int l_regr_dtype, int b_regr_dtype,
+                                          int r_regr_dtype, int logits, int b, int c, int cc, int h, int w, int k,
+                                          float aggr_weight, int num_dets, int agnostic);
+int cnb_exct_decode_ex(const void *t_heat, int t_dtype, const void *l_heat, int l_dtype, const void *b_heat,
+                       int b_dtype, const void *r_heat, int r_dtype, const void *ct_heat, int ct_dtype,
+                       const void *t_regr, int t_regr_dtype, const void *l_regr, int l_regr_dtype,
+                       const void *b_regr, int b_regr_dtype, const void *r_regr, int r_regr_dtype, int logits,
+                       int b, int c, int cc, int h, int w, int k, float scores_thresh, float center_thresh,
+                       float aggr_weight, int num_dets, int agnostic, float *dets, void *workspace,
+                       size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------- A13/A14/A15: focal + splat
  * _sigmoid (models/utils.py:8-10), _neg_loss (models/losses.py:42-67) and the

@@ -27,7 +27,15 @@ device-resident, a torch.profiler kernel table is added.  Writes DIR/decode_half
 
 asserts that detector_f32 == logits_f32, upcast_<dt> == native_<dt>_logits and native_<dt>_heat == the decode of
 its .float() upcast bit for bit in every timed call, and adds a torch.profiler kernel table at B = 64 and at every
-batch size where a new arm is slower than the arm it replaces.  Writes DIR/decode_half_time_<task>.json."""
+batch size where a new arm is slower than the arm it replaces.  Writes DIR/decode_half_time_<task>.json.
+
+--task exdet times exct_decode and agnex_ct_decode on five 80 x 128 x 128 maps and four regression maps (3 rotating
+batches, seed 317, logits randn - 2.19) at K = 40 (B = 1 and 8) and K = 100 (B = 2), aggr_weight 0 and 0.1, with the
+same six arms (detector_f32: torch's sigmoid of the five maps, detectors/exdet.py:32-36, then the fp32 decode; the
+*_logits arms call *_decode_from_logits; the upcast arms cast all nine tensors), the same bit-identity asserts, the
+algorithmic bytes per image (the five maps at s bytes each, plus, with aggregation, the four fp32 aggregated maps
+written and read once) and their share of the HBM peak at K = 40, and a torch.profiler kernel table wherever a new arm
+is slower than the arm it replaces.  Writes DIR/decode_half_time_exdet.json."""
 import argparse
 import json
 import os
@@ -306,14 +314,114 @@ def run_task(task, args):
     print("card: %s, power limit %s; wrote %s" % (name, power, path))
 
 
+EX_C = 80
+
+
+def exdet_inputs(B, seed, device="cuda"):
+    """Logits of the t, l, b, r and centre maps (randn - 2.19, as bench.py's heat) and four uniform regressions."""
+    g = torch.Generator(device=device).manual_seed(seed)
+    maps = [torch.randn(B, EX_C, H_, W_, device=device, generator=g) - 2.19 for _ in range(5)]
+    regs = [torch.rand(B, 2, H_, W_, device=device, generator=g) for _ in range(4)]
+    return maps + regs
+
+
+def exdet_alg_bytes(s, aggr):
+    maps = EX_C * H_ * W_
+    return 5 * maps * s + (4 * maps * 8 if aggr else 0) + 1000 * 14 * 4
+
+
+def run_exdet(args):
+    name, power = card()
+    peak, peak_src = hbm_peak_gbs()
+    result = {"card": name, "power_limit": power, "hbm_peak_gbs": peak, "hbm_peak_source": peak_src,
+              "workload": "exdet, seed 317, 5 x %dx%dx%d maps + 4 regressions, num_dets=1000, 3 rotating batches"
+                          % (EX_C, H_, W_), "groups": {}}
+    for K, B in ((40, 1), (40, 8), (100, 2)):
+        raw = [exdet_inputs(B, 317 + i) for i in range(3)]
+        heat = [[torch.sigmoid(t) for t in b[:5]] + b[5:] for b in raw]
+        for agnostic in (False, True):
+            dec0 = D.agnex_ct_decode if agnostic else D.exct_decode
+            dec0_logits = D.agnex_ct_decode_from_logits if agnostic else D.exct_decode_from_logits
+            for aggr in (0.0, 0.1):
+                kw = dict(K=K, aggr_weight=aggr)
+
+                def dec(*t, _f=dec0, _kw=kw):
+                    return _f(*t, **_kw)
+
+                def dec_logits(*t, _f=dec0_logits, _kw=kw):
+                    return _f(*t, **_kw)
+
+                def detector(*t, _dec=dec):   # detectors/exdet.py:32-36 (out of place: the inputs are reused)
+                    return _dec(*[torch.sigmoid(x) for x in t[:5]], *t[5:])
+                sets = {"detector_f32": raw, "logits_f32": raw, "heat_f32": heat}
+                fns = {"detector_f32": detector, "logits_f32": dec_logits, "heat_f32": dec}
+                elem = {"detector_f32": 4, "logits_f32": 4, "heat_f32": 4}
+                for dt, tdt in HALF.items():
+                    half = [[t.to(tdt) for t in b] for b in raw]
+                    sets["upcast_" + dt] = half
+                    fns["upcast_" + dt] = lambda *t, _d=detector: _d(*[x.float() for x in t])
+                    sets["native_%s_logits" % dt] = half
+                    fns["native_%s_logits" % dt] = dec_logits
+                    sets["native_%s_heat" % dt] = [[t.to(tdt) for t in b] for b in heat]
+                    fns["native_%s_heat" % dt] = dec
+                    elem.update({"upcast_" + dt: 2, "native_%s_logits" % dt: 2, "native_%s_heat" % dt: 2})
+                outs = {n: [None] * 3 for n in sets}
+                arms = {n: rotating(fns[n], sets[n], outs[n]) for n in sets}
+                runs = time_group(arms, args.warmup, args.repeats, args.window)
+                torch.cuda.synchronize()
+                same = {"logits_f32 == detector_f32": all(map(torch.equal, outs["logits_f32"], outs["detector_f32"]))}
+                for dt in HALF:
+                    same["native_%s_logits == upcast_%s" % (dt, dt)] = all(
+                        map(torch.equal, outs["native_%s_logits" % dt], outs["upcast_" + dt]))
+                    same["native_%s_heat == decode of its upcast" % dt] = all(
+                        torch.equal(o, dec(*[t.float() for t in b])) for o, b in zip(outs["native_%s_heat" % dt],
+                                                                                    sets["native_%s_heat" % dt]))
+                gname = "%s_K%d_B%d_aggr%g" % ("agnex" if agnostic else "exct", K, B, aggr)
+                assert all(same.values()), "%s: timed outputs differ: %s" % (gname, same)
+                a = {}
+                for n, ms in runs.items():
+                    best = min(ms)
+                    ips = B / (best * 1e-3)
+                    a[n] = {"ms_runs": [round(m, 5) for m in ms], "ms": round(best, 5),
+                            "spread": round((max(ms) - min(ms)) / best, 4), "images_per_s": round(ips, 1),
+                            "alg_bytes_per_image": exdet_alg_bytes(elem[n], aggr)}
+                    if K == 40:   # memory-bound; at K = 100 the K^4 tuple stage dominates
+                        a[n]["hbm_share"] = round(ips * exdet_alg_bytes(elem[n], aggr) / (peak * 1e9), 4)
+                vs = {"logits_f32": "detector_f32"}
+                for dt in HALF:
+                    vs.update({"native_%s_logits" % dt: "detector_f32", "native_%s_heat" % dt: "heat_f32"})
+                speed = {"%s vs %s" % (n, o): round(a[o]["ms"] / a[n]["ms"], 3) for n, o in vs.items()}
+                speed.update({"native_%s_logits vs upcast_%s" % (dt, dt): round(
+                    a["upcast_" + dt]["ms"] / a["native_%s_logits" % dt]["ms"], 3) for dt in HALF})
+                g = {"K": K, "B": B, "aggr_weight": aggr, "agnostic": agnostic, "arms": a,
+                     "bitwise_identical": same, "speedups": speed}
+                slower = sorted({k.split(" vs ")[0] for k, v in speed.items() if v < 1.0})
+                if slower:   # each slower arm and the arms it replaces
+                    prof = set(slower) | {vs[n] for n in slower if n in vs}
+                    prof |= {"upcast_" + n.split("_")[1] for n in slower if n.endswith("_logits")}
+                    g["profile"] = {n: profile(arms[n]) for n in sorted(prof)}
+                result["groups"][gname] = g
+                print("%-24s " % gname + "  ".join("%s %.4f ms" % (n, v["ms"]) for n, v in a.items()), flush=True)
+                print("           speedups: %s" % speed, flush=True)
+                del sets, outs, arms
+        del raw, heat
+    os.makedirs(args.out, exist_ok=True)
+    path = os.path.join(args.out, "decode_half_time_exdet.json")
+    with open(path, "w") as f:
+        json.dump(result, f, indent=1)
+    print("card: %s, power limit %s; wrote %s" % (name, power, path))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="directory for decode_half_time.json (created if missing)")
-    ap.add_argument("--task", choices=("ctdet", "multi_pose", "ddd"), default="ctdet")
+    ap.add_argument("--task", choices=("ctdet", "multi_pose", "ddd", "exdet"), default="ctdet")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--window", type=float, default=1.0, help="seconds per timed window")
     args = ap.parse_args()
+    if args.task == "exdet":
+        return run_exdet(args)
     if args.task != "ctdet":
         return run_task(args.task, args)
     name, power = card()
