@@ -11,7 +11,7 @@
 // The fused kernel streams pred once and writes the gradient once (10.49 MB/image): the
 // dense target map of the reference (built on the CPU, copied H2D, read by ~12 ATen kernels)
 // is never materialised.  num_pos -- needed to normalise the gradient in the same pass -- is
-// known up front from the object lists (one positive per distinct valid centre).
+// known up front from the object lists (one positive per distinct valid centre inside the map).
 #include <stdlib.h>
 #include "common.cuh"
 
@@ -37,8 +37,9 @@ struct Obj { int x, y, r; };
 
 __device__ __forceinline__ float gauss_value(int dx, int dy, int r) {
   // gaussian2D (utils/image.py:118-124) in float64, cast to fp32 like np.maximum(..., out=fp32 map)
+  // d2 in float64 (exact, as in numpy): with the centre outside the map |dx| may exceed the map size
   const double sigma = (double)(2 * r + 1) / 6.0;
-  return (float)exp(-(double)(dx * dx + dy * dy) / (2.0 * sigma * sigma));
+  return (float)exp(-((double)dx * dx + (double)dy * dy) / (2.0 * sigma * sigma));
 }
 
 // Gaussian tables (shared memory).  exp(-(dx^2+dy^2)/(2 sigma^2)) depends on d2 = dx^2 + dy^2 only, so every
@@ -111,10 +112,11 @@ __device__ __forceinline__ int gather_objects(const int32_t *cls, const int32_t 
   for (int m = threadIdx.x; m < M; m += blockDim.x) {
     const size_t o = (size_t)b * M + m;
     if (valid[o] && cls[o] == c) {
-      const int x = cx[o], y = cy[o];
-      if (x >= 0 && x < W && y >= 0 && y < H && rad[o] >= 0 && y + rad[o] >= y0 && y - rad[o] < y1) {   // rows [y0, y1) of this CTA
+      // draw_umich_gaussian clips the window to the map: a centre outside it still paints the overlap
+      const long long x = cx[o], y = cy[o], r = rad[o];
+      if (r >= 0 && x + r >= 0 && x - r < W && y + r >= 0 && y - r < H && y + r >= y0 && y - r < y1) {   // rows [y0, y1) of this CTA
         const int slot = atomicAdd(s_n, 1);
-        if (slot < MAX_OBJ_PER_PLANE) s_obj[slot] = Obj{x, y, rad[o]};
+        if (slot < MAX_OBJ_PER_PLANE) s_obj[slot] = Obj{(int)x, (int)y, (int)r};
       }
     }
   }
@@ -124,15 +126,44 @@ __device__ __forceinline__ int gather_objects(const int32_t *cls, const int32_t 
 
 struct Elem { float loss_pos, loss_neg, grad, is_pos; };
 
-// One element of _neg_loss (+ its gradient w.r.t. pred or, when LOGITS, w.r.t. the logit).
+// One element of _neg_loss outside the fast path's assumptions (p or gt NaN, p outside (0, 1), gt outside [0, 1]):
+// the reference's masked products as IEEE fp32 evaluates them, pos_loss = log(p) (1-p)^2 [gt == 1] and
+// neg_loss = log(1-p) p^2 (1-gt)^4 [gt < 1], with the gradient autograd takes through them factor by factor.  A mask
+// of 0 times an infinite or NaN factor is NaN, so the loss and the gradient are NaN or inf exactly where the
+// reference's are (a NaN target: (1-gt)^4 = NaN times 0; p = 1 at a positive: log(0) times 0).
 template <bool LOGITS>
-__device__ __forceinline__ Elem focal_elem(float v, float gt, float inv_norm) {
-  float p = v, chain = 1.0f;
+__device__ __forceinline__ Elem focal_elem_ieee(float p, float s, bool in_clamp, float gt, float inv_norm,
+                                                bool pos_live) {
+  const float pos = (gt == 1.0f) ? 1.0f : 0.0f, neg = (gt < 1.0f) ? 1.0f : 0.0f;
+  const float omp = 1.0f - p, w1 = 1.0f - gt, w = (w1 * w1) * (w1 * w1);
+  const float lp = logf(p), lq = logf(omp);
+  Elem e;
+  e.loss_pos = lp * (omp * omp) * pos;
+  e.loss_neg = lq * (p * p) * w * neg;
+  e.is_pos = pos;
+  // with num_pos == 0 the reference returns -neg_loss: the positive terms are not in its graph
+  const float dpos = pos_live ? (pos * (omp * omp)) / p - (pos * lp) * (2.0f * omp) : 0.0f;
+  const float dneg = (neg * w * lq) * (2.0f * p) - (neg * w * (p * p)) / omp;
+  const float g = -(dpos + dneg) * inv_norm;
+  // clamp's backward selects (0 outside [min, max], whatever flows in); sigmoid's then multiplies by s (1 - s)
+  e.grad = LOGITS ? (in_clamp ? g * (s * (1.0f - s)) : 0.0f * s) : g;
+  return e;
+}
+
+// One element of _neg_loss (+ its gradient w.r.t. pred or, when LOGITS, w.r.t. the logit).  pos_live: num_pos > 0.
+template <bool LOGITS>
+__device__ __forceinline__ Elem focal_elem(float v, float gt, float inv_norm, bool pos_live) {
+  float p = v, s = v, chain = 1.0f;
+  bool in_clamp = true;
   if (LOGITS) {  // _sigmoid: in-place sigmoid, clamp; clamp passes gradient only inside [min, max]
-    const float s = 1.0f / (1.0f + expf(-v));
-    p = fminf(fmaxf(s, 1e-4f), 1.0f - 1e-4f);
-    chain = (s >= 1e-4f && s <= 1.0f - 1e-4f) ? s * (1.0f - s) : 0.0f;
+    s = 1.0f / (1.0f + expf(-v));
+    p = s < 1e-4f ? 1e-4f : (s > 1.0f - 1e-4f ? 1.0f - 1e-4f : s);   // NaN stays NaN, as in torch.clamp
+    in_clamp = (s >= 1e-4f && s <= 1.0f - 1e-4f);
+    chain = in_clamp ? s * (1.0f - s) : 0.0f;
   }
+  // p in (0, 1) and gt in [+0, 1] as two unsigned compares of the bit patterns (NaN and negatives fail both)
+  const bool fast = (__float_as_uint(p) - 1u < 0x3f7fffffu) & (__float_as_uint(gt) <= 0x3f800000u);
+  if (!fast) return focal_elem_ieee<LOGITS>(p, s, in_clamp, gt, inv_norm, pos_live);
   Elem e;
   const float omp = 1.0f - p;
   if (gt == 1.0f) {
@@ -141,15 +172,13 @@ __device__ __forceinline__ Elem focal_elem(float v, float gt, float inv_norm) {
     e.loss_neg = 0.0f;
     e.is_pos = 1.0f;
     e.grad = -((omp * omp) / p - 2.0f * omp * lg) * inv_norm * chain;
-  } else if (gt < 1.0f) {
+  } else {
     const float lg = logf(omp);
     const float w1 = 1.0f - gt, w2 = w1 * w1, w4 = w2 * w2;
     e.loss_pos = 0.0f;
     e.loss_neg = lg * (p * p) * w4;
     e.is_pos = 0.0f;
     e.grad = -(w4 * (2.0f * p * lg - (p * p) / omp)) * inv_norm * chain;
-  } else {  // gt > 1 or NaN: neither mask fires in the reference
-    e.loss_pos = e.loss_neg = e.is_pos = e.grad = 0.0f;
   }
   return e;
 }
@@ -247,6 +276,7 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense(const float *__re
                                                                FocalAcc *acc, float *out2) {
   const double np_ = acc->num_pos;  // written by pass 0 (previous kernel on the stream)
   const float inv_norm = grad_scale / (np_ > 0.0 ? (float)np_ : 1.0f);
+  const bool pos_live = np_ > 0.0;
   double pos = 0, neg = 0;
   const long long n4 = n >> 2;
   const bool vec = ((((uintptr_t)pred | (uintptr_t)gt | (uintptr_t)grad) & 15u) == 0);
@@ -255,8 +285,8 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense(const float *__re
          i += (long long)gridDim.x * blockDim.x) {
       const float4 p = __ldg(reinterpret_cast<const float4 *>(pred) + i);
       const float4 g = __ldg(reinterpret_cast<const float4 *>(gt) + i);
-      const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm);
-      const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm);
+      const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
+      const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
       pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
       neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
       if (grad) reinterpret_cast<float4 *>(grad)[i] = make_float4(e0.grad, e1.grad, e2.grad, e3.grad);
@@ -264,7 +294,7 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense(const float *__re
   }
   for (long long i = (vec ? (n4 << 2) : 0) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
-    const Elem e = focal_elem<LOGITS>(pred[i], gt[i], inv_norm);
+    const Elem e = focal_elem<LOGITS>(pred[i], gt[i], inv_norm, pos_live);
     pos += e.loss_pos; neg += e.loss_neg;
     if (grad) grad[i] = e.grad;
   }
@@ -287,9 +317,11 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
   __shared__ float s_gauss[GAUSS_TAB_FLOATS];
   __shared__ int s_n, s_total;
   float inv_norm = 0.0f;
+  bool pos_live = false;
   if (!WRITE_HM) {
     const double np_ = acc->num_pos;
     inv_norm = grad_scale / (np_ > 0.0 ? (float)np_ : 1.0f);
+    pos_live = np_ > 0.0;
   }
   double pos = 0, neg = 0;
   const int n_items = B * C * parts;
@@ -315,8 +347,8 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
         reinterpret_cast<float4 *>(hm + base)[i] = g;
       } else {
         const float4 p = __ldg(reinterpret_cast<const float4 *>(pred + base) + i);
-        const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm);
-        const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm);
+        const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
+        const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
         pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
         neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
         if (grad) reinterpret_cast<float4 *>(grad + base)[i] = make_float4(e0.grad, e1.grad, e2.grad, e3.grad);
@@ -329,7 +361,7 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
       if (WRITE_HM) {
         hm[base + i] = g;
       } else {
-        const Elem e = focal_elem<LOGITS>(pred[base + i], g, inv_norm);
+        const Elem e = focal_elem<LOGITS>(pred[base + i], g, inv_norm, pos_live);
         pos += e.loss_pos; neg += e.loss_neg;
         if (grad) grad[base + i] = e.grad;
       }
@@ -343,15 +375,13 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
 }
 
 // ---- Reg*Loss: B*M*D is tiny (e.g. 64*128*2); one CTA does sums, loss and the scatter of the gradient.
-__global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ output, const void *mask_,
+__global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ output, const float *mask_f,
                                                    const int64_t *__restrict__ ind, const float *__restrict__ target,
                                                    int B, int D, long long HW, int M, int mode, float grad_scale,
                                                    float *out1, float *grad_output) {
   __shared__ double red[2][32];
   __shared__ double s_tot[2];
   const long long n = (long long)B * M * D;
-  const uint8_t *mask_u8 = reinterpret_cast<const uint8_t *>(mask_);
-  const float *mask_f = reinterpret_cast<const float *>(mask_);
   double loss = 0, msum = 0;
   // pass 0: the sums (strided per thread, fixed tree); pass 1: the gradient, one thread per (image, channel) plane
   // walking m in ascending order, so repeated indices add up in a fixed order without atomics
@@ -367,7 +397,7 @@ __global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ out
         const int b = (int)(bm / M);
         const long long sp = ind[bm];
         if (sp < 0 || sp >= HW) continue;   // torch's gather raises on such an index; never read or write outside the map
-        const float m = (mode == 3) ? mask_f[i] : (float)mask_u8[bm];
+        const float m = mask_f[(mode == 3) ? i : bm];   // mask.float(): fractional weights stay fractional
         float pred = output[((long long)b * D + d) * HW + sp];
         float tgt = target[i];
         float scale = 1.0f;
@@ -504,7 +534,7 @@ int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, cons
   CNB_REQUIRE(output && mask && ind && target && out1, CNB_EINVAL, "cnb_reg_loss: null pointer");
   CNB_REQUIRE(b > 0 && d > 0 && hw > 0 && m > 0, CNB_EINVAL, "cnb_reg_loss: non-positive dimension");
   CNB_REQUIRE(mode >= 0 && mode <= 3, CNB_EINVAL, "cnb_reg_loss: mode %d", mode);
-  k_reg_loss<<<1, 1024, 0, (cudaStream_t)stream_>>>(output, mask, ind, target, b, d, hw, m, mode, grad_scale, out1,
+  k_reg_loss<<<1, 1024, 0, (cudaStream_t)stream_>>>(output, static_cast<const float *>(mask), ind, target, b, d, hw, m, mode, grad_scale, out1,
                                                     grad_output);
   CNB_CHECK_LAUNCH("cnb_reg_loss");
   count_launch();

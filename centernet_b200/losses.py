@@ -85,7 +85,16 @@ class FocalSplatLoss(nn.Module):
 
     forward(out [B,C,H,W], obj_cls, obj_cx, obj_cy, obj_radius, obj_valid  (all [B,M])):
     obj_cx/obj_cy are the integer centres ``ct_int`` and obj_radius the
-    ``max(0, int(gaussian_radius(...)))`` of datasets/sample/ctdet.py:111-117."""
+    ``max(0, int(gaussian_radius(...)))`` of datasets/sample/ctdet.py:111-117.
+    A centre outside the map paints the part of its window that overlaps the map, as
+    draw_umich_gaussian does; objects with obj_valid = 0, a negative radius or a class
+    outside [0, C) are skipped.
+
+    num_pos is counted from the lists: one positive per distinct valid centre inside the
+    map.  That is the reference's count of target pixels equal to 1 up to a radius of about
+    12,000: beyond it the fp32 target next to the centre rounds to 1 as well, and the
+    reference counts those pixels too.  gaussian_radius of any box on a 512x512 input
+    stays far below that."""
 
     def __init__(self, from_logits=False):
         super().__init__()
@@ -96,7 +105,8 @@ class FocalSplatLoss(nn.Module):
 
 
 def splat_gaussian(obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, num_classes, height, width):
-    """Dense [B,C,H,W] target built on the device (draw_umich_gaussian, utils/image.py:126-141)."""
+    """Dense [B,C,H,W] target built on the device (draw_umich_gaussian, utils/image.py:126-141), bit for
+    bit; centres outside the map paint the overlap of their window, as there."""
     require_cuda(obj_cls, what="splat_gaussian")
     i32 = lambda t: t.to(torch.int32).contiguous()
     cls, cx, cy, rad = i32(obj_cls), i32(obj_cx), i32(obj_cy), i32(obj_radius)
@@ -116,7 +126,7 @@ class _RegFn(torch.autograd.Function):
         b, d = int(o.shape[0]), int(o.shape[1])
         hw = int(o.shape[2]) * int(o.shape[3])
         m = int(ind.shape[1])
-        msk = f32c(mask) if mode == 3 else mask.to(torch.uint8).contiguous()
+        msk = f32c(mask)   # mask.float() as in the reference: bool, uint8 and fractional float weights alike
         ind = ind.long().contiguous()
         out = torch.empty(1, dtype=torch.float32, device=o.device)
         grad = torch.zeros_like(o) if output.requires_grad else None

@@ -275,7 +275,9 @@ int cnb_exct_decode_ex(const void *t_heat, int t_dtype, const void *l_heat, int 
  *   it is rebuilt on the fly from per-image object lists
  *   obj_cls[b,m] i32, obj_cx/obj_cy[b,m] i32 (ct_int), obj_radius[b,m] i32,
  *   obj_valid[b,m] u8 -- exactly the draw_umich_gaussian calls of
- *   datasets/sample/ctdet.py:111-117.  m <= 128 (the reference's max_objs,
+ *   datasets/sample/ctdet.py:111-117, so a centre outside the map paints the part
+ *   of its window that overlaps it (and is no positive).  Objects with valid = 0,
+ *   a negative radius or a class outside [0, c) are skipped.  m <= 128 (the reference's max_objs,
  *   datasets/dataset/coco.py:38); larger lists return CNB_EUNSUPPORTED.
  * Both losses are bit-identical run to run: the workspace (cnb_focal_workspace_bytes) holds one partial sum
  * per CTA, added in CTA order by the last CTA. */
@@ -294,8 +296,9 @@ int cnb_focal_splat_loss(const float *pred, const int32_t *obj_cls, const int32_
 
 /* ------------------------------------------------------------ A16: RegL1Loss
  * models/losses.py:139-149 (mode 0), RegLoss smooth-L1 :123-137 (mode 1),
- * NormRegL1Loss :151-163 (mode 2), RegWeightedL1Loss :165-175 (mode 3; mask is
- * then float [b,m,d]).  output [b,d,h*w], ind [b,m] i64, target [b,m,d].
+ * NormRegL1Loss :151-163 (mode 2), RegWeightedL1Loss :165-175 (mode 3).  mask is
+ * float [b,m] in modes 0-2 (the reference's mask.float(): fractional weights are kept)
+ * and float [b,m,d] in mode 3.  output [b,d,h*w], ind [b,m] i64, target [b,m,d].
  * out[0] = loss; grad_output (nullable, [b,d,hw], must be zero-filled) gets
  * d loss/d output * grad_scale; repeated ind entries add up in ascending m (bit-identical run to run). */
 int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, const float *target,
