@@ -39,24 +39,60 @@ __global__ void __launch_bounds__(256) k_post_transform(const float *__restrict_
   }
 }
 
-// One CTA per image.  dets [n][6] = x1,y1,x2,y2,score,class (float) -> rows [n][5] grouped by class in
-// class order, input order kept inside a class (boolean-mask indexing of post_process.py:93-97), and
-// offsets [num_classes + 1].  Rows whose class id is outside [0, num_classes) are dropped (as the mask does).
-__global__ void __launch_bounds__(256) k_group_by_class(const float *__restrict__ dets, int n, int num_classes,
-                                                        float *__restrict__ rows, int *__restrict__ offsets) {
+// exdet post_process (detectors/exdet.py:85-95) of one scale: rows [b][n][d], image i = rows [i*n, (i+1)*n) split in
+// two equal halves as reshape(2, -1, 14) splits them.  In the second half x1 <- out_w - x2 and x2 <- out_w - x1
+// (float32), then the point pairs (0,1) and (2,3) are mapped through the image's matrix as k_post_transform maps
+// them; every other column is copied.
+__global__ void __launch_bounds__(256) k_exdet_transform(const float *__restrict__ in, float *__restrict__ out,
+                                                         const double *__restrict__ trans, int b, int n, int d,
+                                                         float out_w) {
+  const long long total = (long long)b * n * d;
+  const int half = n >> 1;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int col = (int)(i % d);
+    const long long row = i / d;
+    const int img = (int)(row / n);
+    float v = in[i];
+    if (col < 4) {
+      const float *p = in + row * d;
+      const bool mirrored = (int)(row - (long long)img * n) >= half;
+      const int isy = col & 1;
+      float x = p[col - isy];
+      if (mirrored) x = __fsub_rn(out_w, p[2 - (col - isy)]);
+      const float y = p[col - isy + 1];
+      const double *t = trans + (size_t)img * 6 + isy * 3;
+      v = (float)__dadd_rn(__dadd_rn(__dmul_rn(t[0], (double)x), __dmul_rn(t[1], (double)y)), t[2]);
+    }
+    out[i] = v;
+  }
+}
+
+// One CTA per image.  dets [n][d] with x1,y1,x2,y2,score in columns 0-4 and a float class id in column cls_col ->
+// rows [n][5] grouped by class in class order, input order kept inside a class (boolean-mask indexing of
+// post_process.py:93-97), and offsets [num_classes + 1].  Rows whose class id is outside [0, num_classes) are
+// dropped (as the mask does), and with kPositive so are rows whose score is not > 0 (NaN included).
+template <bool kPositive>
+__device__ __forceinline__ void group_rows(const float *__restrict__ dets, int n, int dw, int cls_col, int num_classes,
+                                           float *__restrict__ rows, int *__restrict__ offsets) {
   extern __shared__ int gsm[];
   int *cnt = gsm;                    // [num_classes + 1] counts -> running offsets
   int *cls_chunk = gsm + num_classes + 1;   // [256]
   const int img = blockIdx.x, tid = threadIdx.x;
-  const float *d = dets + (size_t)img * n * 6;
+  const float *d = dets + (size_t)img * n * dw;
   float *r = rows + (size_t)img * n * 5;
   int *off = offsets + (size_t)img * (num_classes + 1);
+  auto in_class = [&](int i, int &c) {   // c = the row's class id; false when the row is dropped
+    const float cf = d[(size_t)i * dw + cls_col];
+    c = (int)cf;
+    if (kPositive && !(d[(size_t)i * dw + 4] > 0.f)) return false;
+    return (float)c == cf && c >= 0 && c < num_classes;
+  };
   for (int c = tid; c <= num_classes; c += blockDim.x) cnt[c] = 0;
   __syncthreads();
   for (int i = tid; i < n; i += blockDim.x) {
-    const float cf = d[(size_t)i * 6 + 5];
-    const int c = (int)cf;
-    if ((float)c == cf && c >= 0 && c < num_classes) atomicAdd(&cnt[c + 1], 1);
+    int c;
+    if (in_class(i, c)) atomicAdd(&cnt[c + 1], 1);
   }
   __syncthreads();
   if (tid == 0) {
@@ -70,9 +106,8 @@ __global__ void __launch_bounds__(256) k_group_by_class(const float *__restrict_
     const int i = base + tid;
     int c = -1;
     if (i < n) {
-      const float cf = d[(size_t)i * 6 + 5];
-      const int ci = (int)cf;
-      if ((float)ci == cf && ci >= 0 && ci < num_classes) c = ci;
+      int ci;
+      if (in_class(i, ci)) c = ci;
     }
     cls_chunk[tid] = c;
     __syncthreads();
@@ -85,10 +120,23 @@ __global__ void __launch_bounds__(256) k_group_by_class(const float *__restrict_
     if (c >= 0) {
       atomicAdd(&cnt[c], 1);          // running offset for the next chunk (all adds of a chunk land before the next read)
 #pragma unroll
-      for (int k = 0; k < 5; ++k) r[(size_t)dst * 5 + k] = d[(size_t)i * 6 + k];
+      for (int k = 0; k < 5; ++k) r[(size_t)dst * 5 + k] = d[(size_t)i * dw + k];
     }
     __syncthreads();
   }
+}
+
+// ctdet rows: [n][6] = x1,y1,x2,y2,score,class.
+__global__ void __launch_bounds__(256) k_group_by_class(const float *__restrict__ dets, int n, int num_classes,
+                                                        float *__restrict__ rows, int *__restrict__ offsets) {
+  group_rows<false>(dets, n, 6, 5, num_classes, rows, offsets);
+}
+
+// Rows of any width, class in column cls_col, only rows with score > 0 (exdet merge_outputs, detectors/exdet.py:99-108).
+__global__ void __launch_bounds__(256) k_group_positive_by_class(const float *__restrict__ dets, int n, int d,
+                                                                 int cls_col, int num_classes, float *__restrict__ rows,
+                                                                 int *__restrict__ offsets) {
+  group_rows<true>(dets, n, d, cls_col, num_classes, rows, offsets);
 }
 
 // Rows of one list held in shared memory: 5 floats + new score + perm + flags = 27 B per row.  The launch sizes its
@@ -103,13 +151,14 @@ __device__ __forceinline__ float pyx_min(float a, float b) { return a <= b ? a :
 __device__ __forceinline__ float pyx_max(float a, float b) { return a >= b ? a : b; }
 
 // One warp per list.  List l = (image l / lists_per_img, class l % lists_per_img) covers rows
-// image * n_cap + [offsets[image][class], offsets[image][class + 1]) of `in` ([*, d] floats; columns 0-4 =
+// image * img_stride + [offsets[image][class], offsets[image][class + 1]) of `in` ([*, d] floats; columns 0-4 =
 // x1,y1,x2,y2,score; d = 5 or 39).  Result written to `out` (may alias `in` when d == 5).  The whole array --
-// rows beyond the final N included -- ends up exactly as the reference's in-place routine leaves it.
-__global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, float *__restrict__ out,
-                                                 const int *__restrict__ offsets, int lists_per_img, int n_cap,
-                                                 int d, float sigma, float Nt, float threshold, int method,
-                                                 int *__restrict__ final_n) {
+// rows beyond the final N included -- ends up exactly as the reference's in-place routine leaves it.  Shared
+// memory holds list_cap rows; a longer list is left untouched and flagged.
+__device__ __forceinline__ void soft_nms_list(const float *__restrict__ in, float *__restrict__ out,
+                                              const int *__restrict__ offsets, int lists_per_img, int img_stride,
+                                              int n_cap, int d, float sigma, float Nt, float threshold, int method,
+                                              int *__restrict__ final_n) {
   extern __shared__ __align__(16) unsigned char nsm[];
   float *bx = reinterpret_cast<float *>(nsm);                 // [n_cap][5]
   float *ns = bx + (size_t)n_cap * 5;                         // new score of the current iteration
@@ -119,13 +168,13 @@ __global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, f
   const int l = blockIdx.x;
   const int img = l / lists_per_img, cls = l - img * lists_per_img;
   const int *off = offsets + (size_t)img * (lists_per_img + 1) + cls;
-  const int r0 = img * n_cap + off[0];
+  const int r0 = img * img_stride + off[0];
   int N = off[1] - off[0];
   if (N <= 0) {
     if (final_n && lane == 0) final_n[l] = 0;
     return;
   }
-  if (N > n_cap) {   // offsets inconsistent with n_cap (never from k_group_by_class): leave the list untouched, flag it
+  if (N > n_cap) {   // a list longer than the shared-memory capacity: leave it untouched, flag it
     for (int i = lane; i < N * d; i += 32) out[(size_t)r0 * d + i] = in[(size_t)r0 * d + i];
     if (final_n && lane == 0) final_n[l] = -N;
     return;
@@ -222,6 +271,22 @@ __global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, f
   if (final_n && lane == 0) final_n[l] = N;
 }
 
+// Images of n_cap rows, lists of at most n_cap rows (offsets from k_group_by_class are never longer).
+__global__ void __launch_bounds__(32) k_soft_nms(const float *__restrict__ in, float *__restrict__ out,
+                                                 const int *__restrict__ offsets, int lists_per_img, int n_cap,
+                                                 int d, float sigma, float Nt, float threshold, int method,
+                                                 int *__restrict__ final_n) {
+  soft_nms_list(in, out, offsets, lists_per_img, n_cap, n_cap, d, sigma, Nt, threshold, method, final_n);
+}
+
+// Images of img_stride rows (up to TOPK_WIDE_MAX_ROWS), lists of at most list_cap <= NMS_MAX_ROWS rows.
+__global__ void __launch_bounds__(32) k_soft_nms_strided(const float *__restrict__ in, float *__restrict__ out,
+                                                         const int *__restrict__ offsets, int lists_per_img,
+                                                         int img_stride, int list_cap, int d, float sigma, float Nt,
+                                                         float threshold, int method, int *__restrict__ final_n) {
+  soft_nms_list(in, out, offsets, lists_per_img, img_stride, list_cap, d, sigma, Nt, threshold, method, final_n);
+}
+
 // One CTA per image: threshold = max_per_image-th largest score of the image's n rows (np.partition(scores,
 // kth)[kth], detectors/ctdet.py:85-88), keep[i] = score >= threshold.  n <= 4096.  No cut when n <= max_per_image.
 // NaN of either sign orders above +inf, as np.partition sorts it.
@@ -263,6 +328,74 @@ __global__ void __launch_bounds__(1024) k_topk_keep(const float *__restrict__ ro
     }
   }
   const uint32_t tk = key[max_per_image - 1];
+  const float thr = __uint_as_float((tk & 0x80000000u) ? (tk & 0x7fffffffu) : ~tk);
+  for (int i = tid; i < n; i += blockDim.x) kp[i] = (r[(size_t)i * d + 4] >= thr) ? 1 : 0;
+  if (tid == 0 && thresh_out) thresh_out[img] = thr;
+}
+
+// k_topk_keep's cut for images of up to TOPK_WIDE_MAX_ROWS rows: the same sortable keys, held in shared memory
+// (4 B per row), and the max_per_image-th largest found by a most-significant-digit-first radix select (four 8-bit
+// digits) instead of a full sort.
+constexpr int TOPK_WIDE_MAX_ROWS = 32768;
+
+__global__ void __launch_bounds__(1024) k_topk_keep_wide(const float *__restrict__ rows, int d,
+                                                         const int *__restrict__ offsets, int num_classes, int n_cap,
+                                                         int max_per_image, unsigned char *__restrict__ keep,
+                                                         float *__restrict__ thresh_out) {
+  extern __shared__ uint32_t wsm[];
+  uint32_t *hist = wsm;              // [256]
+  uint32_t *sel = wsm + 256;         // [0] prefix of the selected key, [1] rank still to find inside that prefix
+  uint32_t *key = wsm + 260;         // [n]
+  const int img = blockIdx.x, tid = threadIdx.x;
+  const int n = offsets[(size_t)img * (num_classes + 1) + num_classes];
+  const float *r = rows + (size_t)img * n_cap * d;
+  unsigned char *kp = keep + (size_t)img * n_cap;
+  if (n <= max_per_image) {
+    for (int i = tid; i < n; i += blockDim.x) kp[i] = 1;
+    if (tid == 0 && thresh_out) thresh_out[img] = -__int_as_float(0x7f800000);
+    return;
+  }
+  for (int i = tid; i < n; i += blockDim.x) {
+    uint32_t u = __float_as_uint(r[(size_t)i * d + 4]);
+    if ((u & 0x7fffffffu) > 0x7f800000u) u &= 0x7fffffffu;   // NaN: sign bit cleared, above +inf
+    key[i] = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  }
+  if (tid == 0) { sel[0] = 0u; sel[1] = (uint32_t)max_per_image; }
+  uint32_t mask = 0u;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int b = tid; b < 256; b += blockDim.x) hist[b] = 0u;
+    __syncthreads();
+    const uint32_t prefix = sel[0];
+    for (int i = tid; i < n; i += blockDim.x) {
+      const uint32_t k = key[i];
+      if ((k & mask) == prefix) atomicAdd(&hist[(k >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (tid < 32) {   // lane l holds digits 255 - 8l down to 248 - 8l: the lanes cover the digits from the top
+      uint32_t c[8], sum = 0;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) { c[q] = hist[255 - 8 * tid - q]; sum += c[q]; }
+      uint32_t incl = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (tid >= o) incl += v;
+      }
+      uint32_t rank = sel[1];
+      const uint32_t before = incl - sum;
+      __syncwarp();
+      if (before < rank && rank <= incl) {   // exactly one lane: the digit holding the rank-th largest key
+        rank -= before;
+        int q = 0;
+        while (rank > c[q]) { rank -= c[q]; ++q; }
+        sel[0] = prefix | ((uint32_t)(255 - 8 * tid - q) << shift);
+        sel[1] = rank;
+      }
+    }
+    mask |= 255u << shift;
+    __syncthreads();
+  }
+  const uint32_t tk = sel[0];
   const float thr = __uint_as_float((tk & 0x80000000u) ? (tk & 0x7fffffffu) : ~tk);
   for (int i = tid; i < n; i += blockDim.x) kp[i] = (r[(size_t)i * d + 4] >= thr) ? 1 : 0;
   if (tid == 0 && thresh_out) thresh_out[img] = thr;
@@ -329,6 +462,80 @@ int cnb_topk_keep(const float *rows, int b, int n_cap, int d, const int32_t *off
   k_topk_keep<<<b, 1024, 4096 * 4, (cudaStream_t)stream>>>(rows, d, offsets, num_classes, n_cap, max_per_image, keep,
                                                             thresh);
   CNB_CHECK_LAUNCH("cnb_topk_keep");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_exdet_transform(const float *rows, float *out, const double *trans, int b, int n, int d, float out_width,
+                        void *stream) {
+  CNB_REQUIRE(rows && out && trans, CNB_EINVAL, "cnb_exdet_transform: null pointer");
+  CNB_REQUIRE(rows != out, CNB_EINVAL, "cnb_exdet_transform: out must not alias rows");
+  CNB_REQUIRE(b > 0 && n > 0 && d >= 4, CNB_EINVAL, "cnb_exdet_transform: bad shape");
+  CNB_REQUIRE(n % 2 == 0, CNB_EINVAL, "cnb_exdet_transform: an image's rows split into two equal halves (n even)");
+  const long long total = (long long)b * n * d;
+  const int grid = (int)((total + 255) / 256 < 2368 ? (total + 255) / 256 : 2368);
+  k_exdet_transform<<<grid, 256, 0, (cudaStream_t)stream>>>(rows, out, trans, b, n, d, out_width);
+  CNB_CHECK_LAUNCH("cnb_exdet_transform");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_group_positive_by_class(const float *dets, int b, int n, int d, int cls_col, int num_classes, float *rows,
+                                int32_t *offsets, void *stream) {
+  CNB_REQUIRE(dets && rows && offsets, CNB_EINVAL, "cnb_group_positive_by_class: null pointer");
+  CNB_REQUIRE(b > 0 && n > 0 && d >= 5 && cls_col >= 0 && cls_col < d && num_classes > 0 && num_classes <= 8192,
+              CNB_EINVAL, "cnb_group_positive_by_class: bad shape");
+  const size_t smem = (size_t)(num_classes + 1 + 256) * 4;
+  k_group_positive_by_class<<<b, 256, smem, (cudaStream_t)stream>>>(dets, n, d, cls_col, num_classes, rows, offsets);
+  CNB_CHECK_LAUNCH("cnb_group_positive_by_class");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_soft_nms_strided(const float *rows, float *out, const int32_t *offsets, int n_img, int lists_per_img,
+                         int img_stride, int list_cap, int d, float sigma, float nt, float threshold, int method,
+                         int32_t *final_n, void *stream) {
+  CNB_REQUIRE(rows && out && offsets, CNB_EINVAL, "cnb_soft_nms_strided: null pointer");
+  CNB_REQUIRE(n_img > 0 && lists_per_img > 0 && img_stride > 0 && list_cap > 0 && d >= 5 && method >= 0 &&
+                  method <= 2 && (long long)n_img * lists_per_img <= 0x7fffffffll,
+              CNB_EINVAL, "cnb_soft_nms_strided: bad arguments");
+  CNB_REQUIRE(d == 5 || rows != out, CNB_EINVAL, "cnb_soft_nms_strided: in-place only for 5-column rows");
+  CNB_REQUIRE(img_stride <= TOPK_WIDE_MAX_ROWS, CNB_EUNSUPPORTED, "cnb_soft_nms_strided: at most 32768 rows per image");
+  CNB_REQUIRE(list_cap <= NMS_MAX_ROWS, CNB_EUNSUPPORTED, "cnb_soft_nms_strided: at most 4096 rows per list");
+  const size_t smem = (size_t)list_cap * NMS_ROW_BYTES + 16;
+  static thread_local int dev_done = -1;
+  int dev = 0;
+  CNB_CUDA(cudaGetDevice(&dev));
+  if (dev_done != dev) {
+    CNB_CUDA(cudaFuncSetAttribute(k_soft_nms_strided, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)(NMS_MAX_ROWS * NMS_ROW_BYTES + 16)));
+    dev_done = dev;
+  }
+  k_soft_nms_strided<<<n_img * lists_per_img, 32, smem, (cudaStream_t)stream>>>(
+      rows, out, offsets, lists_per_img, img_stride, list_cap, d, sigma, nt, threshold, method, final_n);
+  CNB_CHECK_LAUNCH("cnb_soft_nms_strided");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_topk_keep_wide(const float *rows, int b, int n_cap, int d, const int32_t *offsets, int num_classes,
+                       int max_per_image, uint8_t *keep, float *thresh, void *stream) {
+  CNB_REQUIRE(rows && offsets && keep, CNB_EINVAL, "cnb_topk_keep_wide: null pointer");
+  CNB_REQUIRE(b > 0 && n_cap > 0 && d >= 5 && num_classes > 0 && max_per_image > 0, CNB_EINVAL,
+              "cnb_topk_keep_wide: bad shape");
+  CNB_REQUIRE(n_cap <= TOPK_WIDE_MAX_ROWS, CNB_EUNSUPPORTED, "cnb_topk_keep_wide: at most 32768 rows per image");
+  const size_t smem = (size_t)(260 + n_cap) * 4;
+  static thread_local int dev_done = -1;
+  int dev = 0;
+  CNB_CUDA(cudaGetDevice(&dev));
+  if (dev_done != dev) {
+    CNB_CUDA(cudaFuncSetAttribute(k_topk_keep_wide, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)((260 + TOPK_WIDE_MAX_ROWS) * 4)));
+    dev_done = dev;
+  }
+  k_topk_keep_wide<<<b, 1024, smem, (cudaStream_t)stream>>>(rows, d, offsets, num_classes, n_cap, max_per_image, keep,
+                                                            thresh);
+  CNB_CHECK_LAUNCH("cnb_topk_keep_wide");
   count_launch();
   return CNB_OK;
 }

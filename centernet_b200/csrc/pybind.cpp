@@ -277,6 +277,28 @@ PYBIND11_MODULE(_C, m) {
                         ptr<float>(thresh), ptr<void>(stream)),
           "cnb_topk_keep");
   });
+  m.def("exdet_transform", [](P rows, P out, P trans, int b, int n, int d, float out_w, P stream) {
+    check(cnb_exdet_transform(ptr<const float>(rows), ptr<float>(out), ptr<const double>(trans), b, n, d, out_w,
+                              ptr<void>(stream)),
+          "cnb_exdet_transform");
+  });
+  m.def("group_positive_by_class", [](P dets, int b, int n, int d, int cls_col, int nc, P rows, P offsets, P stream) {
+    check(cnb_group_positive_by_class(ptr<const float>(dets), b, n, d, cls_col, nc, ptr<float>(rows),
+                                      ptr<int32_t>(offsets), ptr<void>(stream)),
+          "cnb_group_positive_by_class");
+  });
+  m.def("soft_nms_strided", [](P rows, P out, P offsets, int n_img, int lists, int img_stride, int list_cap, int d,
+                               float sigma, float nt, float thr, int method, P final_n, P stream) {
+    check(cnb_soft_nms_strided(ptr<const float>(rows), ptr<float>(out), ptr<const int32_t>(offsets), n_img, lists,
+                               img_stride, list_cap, d, sigma, nt, thr, method, ptr<int32_t>(final_n),
+                               ptr<void>(stream)),
+          "cnb_soft_nms_strided");
+  });
+  m.def("topk_keep_wide", [](P rows, int b, int n_cap, int d, P offsets, int nc, int mpi, P keep, P thresh, P stream) {
+    check(cnb_topk_keep_wide(ptr<const float>(rows), b, n_cap, d, ptr<const int32_t>(offsets), nc, mpi,
+                             ptr<uint8_t>(keep), ptr<float>(thresh), ptr<void>(stream)),
+          "cnb_topk_keep_wide");
+  });
   m.def("resize_image", [](P img, int h, int w, P out, int oh, int ow, P stream) {
     check(cnb_resize_image(ptr<const uint8_t>(img), h, w, ptr<uint8_t>(out), oh, ow, ptr<void>(stream)),
           "cnb_resize_image");

@@ -7,12 +7,13 @@ Two ways in:
     in-place arrays out) so `detectors/*.py` work unchanged -- but they also accept the CUDA tensor that
     `ctdet_decode` returned, which removes the `dets.detach().cpu().numpy()` of detectors/ctdet.py:48;
   * `ctdet_merge_device` is the whole tail of a detector run (back-projection of every scale, per-class
-    concat, soft-NMS, top max_per_image) in four launches with ONE device->host copy at the end.
+    concat, soft-NMS, top max_per_image) in four launches with ONE device->host copy at the end;
+    `multi_pose_merge_device` and `exdet_merge_device` are the same for MultiPoseDetector and ExdetDetector.
 """
 import numpy as np
 import torch
 
-from ._lib import C, ptr, stream_ptr
+from ._lib import C, ptr, same_device, stream_ptr
 
 # Longest soft-NMS list and most detections per image of a merge (k_soft_nms holds a list in shared memory,
 # k_topk_keep sorts an image's scores there; csrc/post.cu).
@@ -168,6 +169,151 @@ def ctdet_merge_device(dets_per_scale, metas, num_classes, max_per_image=100, nm
     offs_h = packed[:, n * 6:n * 6 + num_classes + 1].astype(np.int64)
     if fin is not None and (packed[:, n * 6 + num_classes + 1:] < 0).any():
         raise RuntimeError("ctdet_merge_device: soft-NMS left a class list unprocessed")
+    ret = []
+    for i in range(b):
+        res = {}
+        for j in range(num_classes):
+            a, e = offs_h[i, j], offs_h[i, j + 1]
+            res[j + 1] = rows_h[i, a:e][keep_h[i, a:e]].astype(np.float32)
+        ret.append(res)
+    return ret
+
+
+# ------------------------------------------------------------------ detectors/multi_pose.py and exdet.py tails
+# Most rows per image of the exdet merge (k_soft_nms_strided and k_topk_keep_wide, csrc/post.cu).
+MAX_IMAGE_ROWS = 32768
+
+
+def _check_tail_inputs(what, dets_per_scale, metas, width):
+    """Shapes, devices and metas of a device tail, checked before anything is launched.  Returns B (rows of the
+    first dimension) and the device."""
+    if len(dets_per_scale) == 0 or len(metas) != len(dets_per_scale):
+        raise ValueError("%s: one meta per scale and at least one scale (got %d detections, %d metas)"
+                         % (what, len(dets_per_scale), len(metas)))
+    for d in dets_per_scale:
+        if not isinstance(d, torch.Tensor) or not d.is_cuda:
+            raise NotImplementedError("%s: CUDA tensors only (no CPU path)" % what)
+    dev = same_device(*dets_per_scale)
+    b = int(dets_per_scale[0].shape[0]) if dets_per_scale[0].dim() == 3 else -1
+    for d in dets_per_scale:
+        if d.dim() != 3 or int(d.shape[2]) != width or int(d.shape[0]) != b or int(d.shape[1]) < 1 or b < 1:
+            raise ValueError("%s: every scale must be [B, N, %d] with one B, got %s"
+                             % (what, width, [tuple(t.shape) for t in dets_per_scale]))
+    return b, dev
+
+
+def _tail_transforms(what, metas, n_img, device):
+    """[S, n_img, 6] float64 inverse affines of every scale and image, in ONE copy from pinned memory (no host
+    synchronisation)."""
+    mats = []
+    for m in metas:
+        if len(m["c"]) != n_img or len(m["s"]) != n_img:
+            raise ValueError("%s: metas need one 'c' and one 's' per image (%d)" % (what, n_img))
+        mats.append([_inv_affine(m["c"][i], m["s"][i], (m["out_width"], m["out_height"])).reshape(6)
+                     for i in range(n_img)])
+    host = torch.from_numpy(np.ascontiguousarray(np.array(mats, np.float64))).pin_memory()
+    return host.to(device, non_blocking=True)
+
+
+def _divide_by_scale(t, cols, scale):
+    """`dets[..., cols] /= scale` in float32, as numpy divides a float32 array by a Python float (a tensor
+    divisor: torch turns division by a Python scalar into a multiplication by 1/scale)."""
+    if scale != 1.0:
+        div = torch.full((), scale, dtype=torch.float32, device=t.device)
+        for a, e in cols:
+            t[:, :, a:e] /= div
+
+
+def multi_pose_merge_device(dets_per_scale, metas, nms=False):
+    """The tail of MultiPoseDetector.run for one image batch: for every test scale `post_process`
+    (detectors/multi_pose.py:62-73: multi_pose_post_process, then the box and the keypoints divided by the scale),
+    then `merge_outputs` (:75-81): concatenation over the scales and, when `nms` is set or there are several
+    scales, soft_nms_39 (Nt 0.5, Gaussian) on the whole list.  Every row is kept, as the reference keeps it.
+      dets_per_scale: list of [B, K, 40] CUDA tensors (multi_pose_decode outputs), one per test scale;
+      metas: one dict per scale, the keys of ctdet_merge_device ('c', 's' per image, 'out_height', 'out_width',
+             'scale').
+    Returns a list (per image) of {1: list of 39-float rows} -- one device->host copy in total.  The inputs are
+    left unmodified."""
+    what = "multi_pose_merge_device"
+    b, dev = _check_tail_inputs(what, dets_per_scale, metas, 40)
+    n = sum(int(d.shape[1]) for d in dets_per_scale)
+    run_nms = bool(nms) or len(dets_per_scale) > 1
+    if run_nms and n > MAX_ROWS:
+        raise NotImplementedError("%s: soft-NMS takes at most %d rows per image (got %d)" % (what, MAX_ROWS, n))
+    trans = _tail_transforms(what, metas, b, dev)
+    parts = []
+    for k, (d, m) in enumerate(zip(dets_per_scale, metas)):
+        d = d.detach().float().contiguous()
+        t = torch.empty_like(d)
+        C.post_transform(ptr(d), ptr(t), ptr(trans[k]), b, int(d.shape[1]), 40, 0, 2, 5, 17, stream_ptr(d))
+        t = t[:, :, :39]
+        _divide_by_scale(t, ((0, 4), (5, 39)), float(m.get("scale", 1.0)))
+        parts.append(t)
+    allp = torch.cat(parts, dim=1).contiguous()          # scale-major, like np.concatenate over `detections`
+    if run_nms:
+        offs = torch.zeros((b, 2), dtype=torch.int32, device=dev)
+        offs[:, 1] = n
+        out = torch.empty_like(allp)
+        C.soft_nms(ptr(allp), ptr(out), ptr(offs), b, 1, n, 39, 0.5, 0.5, 0.001, 2, 0, stream_ptr(allp))
+        allp = out
+    host = allp.cpu().numpy()                             # one D2H
+    return [{1: host[i].tolist()} for i in range(b)]
+
+
+def exdet_merge_device(dets_per_scale, metas, num_classes, max_per_image=100, flip=False):
+    """The tail of ExdetDetector.run for one image batch: for every test scale `post_process`
+    (detectors/exdet.py:85-95), then `merge_outputs` (:97-122) with the reference's compiled soft_nms.
+      dets_per_scale: list of [P*B, N, 14] CUDA tensors (exct_decode / agnex_ct_decode outputs), one per test
+             scale.  With `flip` P = 2 and image i is the pair of rows (2i, 2i+1) that base_detector.pre_process
+             builds: the image, then its mirror;
+      metas: one dict per scale, the keys of ctdet_merge_device.
+    Per scale an image's P*N rows are split into two equal halves (as `reshape(2, -1, 14)` splits them), the
+    second half is un-mirrored, both corners are back-projected and divided by the scale.  The merge keeps the
+    rows with score > 0, groups them by the class in column 13, runs Gaussian soft-NMS (Nt 0.5) on every class
+    list and cuts to the max_per_image best scores.  Like the reference, an image without `flip` has its N rows
+    split in two and the second half mirrored, so N must be even.
+    Returns a list (per image) of {class id: float32 [n, 5] array}, every row soft-NMS leaves included -- one
+    device->host copy in total.  The inputs are left unmodified."""
+    what = "exdet_merge_device"
+    pb, dev = _check_tail_inputs(what, dets_per_scale, metas, 14)
+    p = 2 if flip else 1
+    if pb % p:
+        raise ValueError("%s: with flip the batch holds image / mirror pairs (got %d rows)" % (what, pb))
+    b = pb // p
+    per_img = [p * int(d.shape[1]) for d in dets_per_scale]
+    if any(r % 2 for r in per_img):
+        raise ValueError("%s: an image's rows are split into two equal halves (detectors/exdet.py:87), so N must "
+                         "be even without flip (got %s)" % (what, [int(d.shape[1]) for d in dets_per_scale]))
+    n = sum(per_img)
+    if n > MAX_IMAGE_ROWS:
+        raise NotImplementedError("%s: at most %d rows per image (got %d)" % (what, MAX_IMAGE_ROWS, n))
+    if not 0 < int(num_classes) <= 8192 or int(max_per_image) < 1:
+        raise ValueError("%s: num_classes must be in [1, 8192] and max_per_image >= 1" % what)
+    num_classes, max_per_image = int(num_classes), int(max_per_image)
+    trans = _tail_transforms(what, metas, b, dev)
+    parts = []
+    for k, (d, m) in enumerate(zip(dets_per_scale, metas)):
+        d = d.detach().float().contiguous()
+        t = torch.empty((b, per_img[k], 14), dtype=torch.float32, device=dev)
+        C.exdet_transform(ptr(d), ptr(t), ptr(trans[k]), b, per_img[k], 14, float(m["out_width"]), stream_ptr(d))
+        _divide_by_scale(t, ((0, 4),), float(m.get("scale", 1.0)))
+        parts.append(t)
+    allp = torch.cat(parts, dim=1).contiguous() if len(parts) > 1 else parts[0]
+    rows = torch.empty((b, n, 5), dtype=torch.float32, device=dev)
+    offs = torch.empty((b, num_classes + 1), dtype=torch.int32, device=dev)
+    C.group_positive_by_class(ptr(allp), b, n, 14, 13, num_classes, ptr(rows), ptr(offs), stream_ptr(allp))
+    fin = torch.empty((b, num_classes), dtype=torch.int32, device=dev)
+    C.soft_nms_strided(ptr(rows), ptr(rows), ptr(offs), b, num_classes, n, min(n, MAX_ROWS), 5, 0.5, 0.5, 0.001, 2,
+                       ptr(fin), stream_ptr(rows))
+    keep = torch.empty((b, n), dtype=torch.uint8, device=dev)
+    C.topk_keep_wide(ptr(rows), b, n, 5, ptr(offs), num_classes, max_per_image, ptr(keep), 0, stream_ptr(rows))
+    packed = torch.cat([rows.view(b, -1), keep.float(), offs.float(), fin.float()], dim=1).cpu().numpy()   # one D2H
+    rows_h = packed[:, :n * 5].reshape(b, n, 5)
+    keep_h = packed[:, n * 5:n * 6] > 0
+    offs_h = packed[:, n * 6:n * 6 + num_classes + 1].astype(np.int64)      # <= 32768: exact in float32
+    fin_h = packed[:, n * 6 + num_classes + 1:]
+    if (fin_h < 0).any():
+        raise RuntimeError("%s: a class list of more than %d rows was not processed by soft-NMS" % (what, MAX_ROWS))
     ret = []
     for i in range(b):
         res = {}

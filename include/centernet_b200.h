@@ -579,6 +579,30 @@ int cnb_soft_nms(const float *rows, float *out, const int32_t *offsets, int n_im
 int cnb_topk_keep(const float *rows, int b, int n_cap, int d, const int32_t *offsets, int num_classes,
                   int max_per_image, uint8_t *keep, float *thresh, void *stream);
 
+/* The exdet tail (detectors/exdet.py:85-122) and images of more than 4096 rows.
+ * cnb_exdet_transform: rows [b,n,d] (d >= 4, n even) -> out [b,n,d]; image i's
+ *   rows split in two equal halves, in the second x1 <- out_width - x2 and
+ *   x2 <- out_width - x1 (float32), then the pairs (0,1) and (2,3) mapped as
+ *   cnb_post_transform maps them; other columns copied.  out must not alias rows.
+ * cnb_group_positive_by_class: dets [b,n,d] (x1,y1,x2,y2,score in columns 0-4,
+ *   float class id in column cls_col) -> rows [b,n,5] and offsets [b,classes+1]
+ *   as cnb_group_by_class, keeping only rows whose score is > 0.
+ * cnb_soft_nms_strided: cnb_soft_nms with images of img_stride rows
+ *   (<= 32768) and lists of at most list_cap rows (<= 4096; shared memory is
+ *   sized from list_cap).  A longer list is left untouched, final_n < 0.
+ * cnb_topk_keep_wide: cnb_topk_keep for n_cap <= 32768 rows per image (radix
+ *   select instead of a sort; the same threshold).
+ * Capacities above those bounds return CNB_EUNSUPPORTED. */
+int cnb_exdet_transform(const float *rows, float *out, const double *trans, int b, int n, int d,
+                        float out_width, void *stream);
+int cnb_group_positive_by_class(const float *dets, int b, int n, int d, int cls_col, int num_classes,
+                                float *rows, int32_t *offsets, void *stream);
+int cnb_soft_nms_strided(const float *rows, float *out, const int32_t *offsets, int n_img,
+                         int lists_per_img, int img_stride, int list_cap, int d, float sigma, float nt,
+                         float threshold, int method, int32_t *final_n, void *stream);
+int cnb_topk_keep_wide(const float *rows, int b, int n_cap, int d, const int32_t *offsets, int num_classes,
+                       int max_per_image, uint8_t *keep, float *thresh, void *stream);
+
 /* ------------------------------------------- N4: detector input pre-processing
  * detectors/base_detector.py:37-65 for one image: cv2.warpAffine(INTER_LINEAR,
  * border 0) + (x/255 - mean)/std + HWC->CHW (+ mirrored copy when flip_test).
