@@ -12,6 +12,12 @@
 
 namespace cnb {
 
+// One row of np.dot(t, [x, y, 1.]) (utils/image.py:63-66): the float64 2x3 matrix row t times a float32 point,
+// (t0 * x + t1 * y) + t2 with no fused multiply-add, stored to float32 as the reference's float32 arrays store it.
+__device__ __forceinline__ float affine_row(const double *__restrict__ t, float x, float y) {
+  return (float)__dadd_rn(__dadd_rn(__dmul_rn(t[0], (double)x), __dmul_rn(t[1], (double)y)), t[2]);
+}
+
 // rows [b][n][d] -> out (same shape): columns copied, the point pairs (x, y) at columns
 // [a0, a0 + 2 na) and [b0, b0 + 2 nb) mapped through the image's 2x3 float64 matrix.
 __global__ void __launch_bounds__(256) k_post_transform(const float *__restrict__ in, float *__restrict__ out,
@@ -30,10 +36,7 @@ __global__ void __launch_bounds__(256) k_post_transform(const float *__restrict_
     if (rel >= 0) {
       const int isy = rel & 1;
       const float x = in[i - isy], y = in[i - isy + 1];
-      const double *t = trans + (size_t)img * 6 + isy * 3;
-      // np.dot(t, [x, y, 1.]): (t0 * x + t1 * y) + t2, no fused multiply-add
-      const double r = __dadd_rn(__dadd_rn(__dmul_rn(t[0], (double)x), __dmul_rn(t[1], (double)y)), t[2]);
-      v = (float)r;
+      v = affine_row(trans + (size_t)img * 6 + isy * 3, x, y);
     }
     out[i] = v;
   }
@@ -61,31 +64,30 @@ __global__ void __launch_bounds__(256) k_exdet_transform(const float *__restrict
       float x = p[col - isy];
       if (mirrored) x = __fsub_rn(out_w, p[2 - (col - isy)]);
       const float y = p[col - isy + 1];
-      const double *t = trans + (size_t)img * 6 + isy * 3;
-      v = (float)__dadd_rn(__dadd_rn(__dmul_rn(t[0], (double)x), __dmul_rn(t[1], (double)y)), t[2]);
+      v = affine_row(trans + (size_t)img * 6 + isy * 3, x, y);
     }
     out[i] = v;
   }
 }
 
-// One CTA per image.  dets [n][d] with x1,y1,x2,y2,score in columns 0-4 and a float class id in column cls_col ->
-// rows [n][5] grouped by class in class order, input order kept inside a class (boolean-mask indexing of
-// post_process.py:93-97), and offsets [num_classes + 1].  Rows whose class id is outside [0, num_classes) are
-// dropped (as the mask does), and with kPositive so are rows whose score is not > 0 (NaN included).
-template <bool kPositive>
+// One CTA per image.  dets [n][dw] with a float class id in column cls_col -> rows [n][Rows::kWidth] grouped by class
+// in class order, input order kept inside a class (boolean-mask indexing of post_process.py:93-97), and offsets
+// [num_classes + 1].  Rows whose class id is outside [0, num_classes) are dropped (as the mask does), and so are
+// rows the policy's keep() refuses; emit() writes a kept row's output columns.
+template <class Rows>
 __device__ __forceinline__ void group_rows(const float *__restrict__ dets, int n, int dw, int cls_col, int num_classes,
-                                           float *__restrict__ rows, int *__restrict__ offsets) {
+                                           float *__restrict__ rows, int *__restrict__ offsets, const Rows &rw) {
   extern __shared__ int gsm[];
   int *cnt = gsm;                    // [num_classes + 1] counts -> running offsets
   int *cls_chunk = gsm + num_classes + 1;   // [256]
   const int img = blockIdx.x, tid = threadIdx.x;
   const float *d = dets + (size_t)img * n * dw;
-  float *r = rows + (size_t)img * n * 5;
+  float *r = rows + (size_t)img * n * Rows::kWidth;
   int *off = offsets + (size_t)img * (num_classes + 1);
   auto in_class = [&](int i, int &c) {   // c = the row's class id; false when the row is dropped
     const float cf = d[(size_t)i * dw + cls_col];
     c = (int)cf;
-    if (kPositive && !(d[(size_t)i * dw + 4] > 0.f)) return false;
+    if (!rw.keep(d + (size_t)i * dw)) return false;
     return (float)c == cf && c >= 0 && c < num_classes;
   };
   for (int c = tid; c <= num_classes; c += blockDim.x) cnt[c] = 0;
@@ -119,24 +121,101 @@ __device__ __forceinline__ void group_rows(const float *__restrict__ dets, int n
     __syncthreads();
     if (c >= 0) {
       atomicAdd(&cnt[c], 1);          // running offset for the next chunk (all adds of a chunk land before the next read)
-#pragma unroll
-      for (int k = 0; k < 5; ++k) r[(size_t)dst * 5 + k] = d[(size_t)i * dw + k];
+      rw.emit(d + (size_t)i * dw, r + (size_t)dst * Rows::kWidth);
     }
     __syncthreads();
   }
 }
 
+// x1,y1,x2,y2,score of columns 0-4; with kPositive only rows whose score is > 0 (NaN dropped).
+template <bool kPositive>
+struct BoxRows {
+  static constexpr int kWidth = 5;
+  __device__ __forceinline__ bool keep(const float *__restrict__ row) const { return !kPositive || row[4] > 0.f; }
+  __device__ __forceinline__ void emit(const float *__restrict__ row, float *__restrict__ out) const {
+#pragma unroll
+    for (int k = 0; k < 5; ++k) out[k] = row[k];
+  }
+};
+
 // ctdet rows: [n][6] = x1,y1,x2,y2,score,class.
 __global__ void __launch_bounds__(256) k_group_by_class(const float *__restrict__ dets, int n, int num_classes,
                                                         float *__restrict__ rows, int *__restrict__ offsets) {
-  group_rows<false>(dets, n, 6, 5, num_classes, rows, offsets);
+  group_rows(dets, n, 6, 5, num_classes, rows, offsets, BoxRows<false>());
 }
 
 // Rows of any width, class in column cls_col, only rows with score > 0 (exdet merge_outputs, detectors/exdet.py:99-108).
 __global__ void __launch_bounds__(256) k_group_positive_by_class(const float *__restrict__ dets, int n, int d,
                                                                  int cls_col, int num_classes, float *__restrict__ rows,
                                                                  int *__restrict__ offsets) {
-  group_rows<true>(dets, n, d, cls_col, num_classes, rows, offsets);
+  group_rows(dets, n, d, cls_col, num_classes, rows, offsets, BoxRows<true>());
+}
+
+// The ddd tail of one row: ddd_post_process (utils/post_process.py:13-80 with ddd2locrot, utils/ddd_utils.py:66-111)
+// of a ddd_decode row [18] = x, y, score, rot[8], depth, dim[3], w, h, class -> [13] = alpha, x1, y1, x2, y2,
+// dim[3], X, Y, Z, rot_y, score.  Every step is the reference's float32 (or, for the affine, float64) operation,
+// rounded where numpy rounds it; nothing is contracted into a fused multiply-add.
+//   * (x, y) and (w, h) both go through the full inverse affine, translation included (the reference transforms
+//     wh with transform_preds), and the box is centre -+ transformed wh / 2;
+//   * get_alpha: bin 1 when rot[1] > rot[5] (NaN and ties: bin 2), atan2(sin, cos) -+ float32(pi / 2) in float32;
+//     alpha1 * idx + alpha2 * (1 - idx) is float64, so a NaN in either bin makes alpha NaN;
+//   * unproject_2d_to_3d, left to right in float32, then Y += dim0 / 2;
+//   * alpha2rot_y: alpha + atan2(u - P[0,2], P[0,0]), wrapped once each way against float32(pi) (numpy 2 compares a
+//     float32 scalar with a Python float in float32).
+// atan2 is evaluated in float64 and rounded, the closest float32 to the angle; numpy's float32 arctan2 is within
+// a few ulp of it.
+struct DddRows {
+  static constexpr int kWidth = 13;
+  const double *t;   // the image's 2x3 inverse affine
+  const float *P;    // the image's 3x4 calibration, row major
+  bool cut;          // merge_outputs: keep score > thresh (NaN dropped); post_process: keep every row
+  float thresh;
+  __device__ __forceinline__ bool keep(const float *__restrict__ row) const { return !cut || row[2] > thresh; }
+  __device__ __forceinline__ void emit(const float *__restrict__ r, float *__restrict__ o) const {
+    const float kHalfPi = 1.57079632679489661923f, kPi = 3.14159265358979323846f, kTwoPi = 6.28318530717958647692f;
+    const float cx = affine_row(t, r[0], r[1]), cy = affine_row(t + 3, r[0], r[1]);
+    const float tw = affine_row(t, r[15], r[16]), th = affine_row(t + 3, r[15], r[16]);
+    const float a1 = __fadd_rn((float)atan2((double)r[5], (double)r[6]), -kHalfPi);
+    const float a2 = __fadd_rn((float)atan2((double)r[9], (double)r[10]), kHalfPi);
+    float alpha = (r[4] > r[8]) ? a1 : a2;
+    if (a1 != a1 || a2 != a2) alpha = __int_as_float(0x7fffffff);
+    const float depth = r[11], dim0 = r[12];
+    const float z = __fsub_rn(depth, P[11]);
+    const float X = __fdiv_rn(__fsub_rn(__fsub_rn(__fmul_rn(cx, depth), P[3]), __fmul_rn(P[2], z)), P[0]);
+    const float Y = __fdiv_rn(__fsub_rn(__fsub_rn(__fmul_rn(cy, depth), P[7]), __fmul_rn(P[6], z)), P[5]);
+    float ry = __fadd_rn(alpha, (float)atan2((double)__fsub_rn(cx, P[2]), (double)P[0]));
+    if (ry > kPi) ry = __fsub_rn(ry, kTwoPi);
+    if (ry < -kPi) ry = __fadd_rn(ry, kTwoPi);
+    const float hw = __fdiv_rn(tw, 2.f), hh = __fdiv_rn(th, 2.f);
+    o[0] = alpha;
+    o[1] = __fsub_rn(cx, hw); o[2] = __fsub_rn(cy, hh); o[3] = __fadd_rn(cx, hw); o[4] = __fadd_rn(cy, hh);
+    o[5] = dim0; o[6] = r[13]; o[7] = r[14];
+    o[8] = X; o[9] = __fadd_rn(Y, __fdiv_rn(dim0, 2.f)); o[10] = z;
+    o[11] = ry;
+    o[12] = r[2];
+  }
+};
+
+// ddd rows [n][18] (class in column 17) -> rows [n][13] grouped by class and offsets, the score cut applied when
+// `cut` is set.  seen (nullable) [num_classes]: 1 where the class has a row before the cut, else 0 -- what tells
+// merge_outputs' untouched empty list (shape (0,)) from a list the cut emptied (shape (0, 13)).
+__global__ void __launch_bounds__(256) k_ddd_tail(const float *__restrict__ dets, int n, const double *__restrict__ trans,
+                                                  const float *__restrict__ calib, int num_classes, int cut, float thresh,
+                                                  float *__restrict__ rows, int *__restrict__ offsets,
+                                                  unsigned char *__restrict__ seen) {
+  const int img = blockIdx.x;
+  if (seen) {
+    unsigned char *sn = seen + (size_t)img * num_classes;
+    for (int c = threadIdx.x; c < num_classes; c += blockDim.x) sn[c] = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const float cf = dets[((size_t)img * n + i) * 18 + 17];
+      const int c = (int)cf;
+      if ((float)c == cf && c >= 0 && c < num_classes) sn[c] = 1;
+    }
+  }
+  group_rows(dets, n, 18, 17, num_classes, rows, offsets,
+             DddRows{trans + (size_t)img * 6, calib + (size_t)img * 12, cut != 0, thresh});
 }
 
 // Rows of one list held in shared memory: 5 floats + new score + perm + flags = 27 B per row.  The launch sizes its
@@ -540,6 +619,33 @@ int cnb_topk_keep_wide(const float *rows, int b, int n_cap, int d, const int32_t
   return CNB_OK;
 }
 
+int cnb_ddd_tail(const float *dets, int b, int n, int d, const double *trans, const float *calib, int num_classes,
+                 int cut, float thresh, float *rows, int32_t *offsets, uint8_t *seen, void *stream) {
+  CNB_REQUIRE(dets && trans && calib && rows && offsets, CNB_EINVAL, "cnb_ddd_tail: null pointer");
+  CNB_REQUIRE(d == 18, CNB_EINVAL,
+              "cnb_ddd_tail: rows must have the 18 columns of ddd_decode with wh (x, y, score, rot[8], depth, dim[3], "
+              "w, h, class)");
+  CNB_REQUIRE(b > 0 && n > 0 && num_classes > 0 && num_classes <= 8192, CNB_EINVAL, "cnb_ddd_tail: bad shape");
+  // every output range disjoint from every other buffer
+  const char *in_p[3] = {(const char *)dets, (const char *)trans, (const char *)calib};
+  const size_t in_n[3] = {(size_t)b * n * 18 * 4, (size_t)b * 6 * 8, (size_t)b * 12 * 4};
+  const char *out_p[3] = {(const char *)rows, (const char *)offsets, (const char *)seen};
+  const size_t out_n[3] = {(size_t)b * n * 13 * 4, (size_t)b * (num_classes + 1) * 4, (size_t)b * num_classes};
+  auto overlap = [](const char *p, size_t pn, const char *q, size_t qn) { return p && q && p < q + qn && q < p + pn; };
+  for (int o = 0; o < 3; ++o) {
+    for (int i = 0; i < 3; ++i)
+      CNB_REQUIRE(!overlap(out_p[o], out_n[o], in_p[i], in_n[i]), CNB_EINVAL, "cnb_ddd_tail: an output aliases an input");
+    for (int k = o + 1; k < 3; ++k)
+      CNB_REQUIRE(!overlap(out_p[o], out_n[o], out_p[k], out_n[k]), CNB_EINVAL, "cnb_ddd_tail: outputs alias each other");
+  }
+  const size_t smem = (size_t)(num_classes + 1 + 256) * 4;
+  k_ddd_tail<<<b, 256, smem, (cudaStream_t)stream>>>(dets, n, trans, calib, num_classes, cut ? 1 : 0, thresh, rows,
+                                                     offsets, seen);
+  CNB_CHECK_LAUNCH("cnb_ddd_tail");
+  count_launch();
+  return CNB_OK;
+}
+
 }  // extern "C"
 
 // ------------------------------------------------------------------ N4: detector input pre-processing
@@ -549,11 +655,14 @@ int cnb_topk_keep_wide(const float *rows, int b, int n_cap, int d, const int32_t
 // (imgwarp.cpp): coordinates on a 1/1024 grid from the INVERTED matrix `minv` (cvRound = round half to even),
 // +16, >> 5 -> integer pixel + 5-bit phase; weights 32 * (32 - fy | fy) * (32 - fx | fx) (sum 32768);
 // value = (sum w * p + 2^14) >> 15 with out-of-image taps reading the border value 0.
+// kF32: DddDetector.pre_process's normalisation (detectors/ddd.py:50-51), x.astype(float32) / 255. then
+// (x - mean) / std all in float32, instead of base_detector's float64 -- the warp is the same.
 namespace cnb {
-__global__ void __launch_bounds__(256) k_preprocess(const unsigned char *__restrict__ img, int H, int W,
-                                                    const double *__restrict__ minv, const float *__restrict__ mean,
-                                                    const float *__restrict__ stdv, float *__restrict__ out, int oh,
-                                                    int ow, int flip) {
+template <bool kF32>
+__device__ __forceinline__ void preprocess_px(const unsigned char *__restrict__ img, int H, int W,
+                                              const double *__restrict__ minv, const float *__restrict__ mean,
+                                              const float *__restrict__ stdv, float *__restrict__ out, int oh, int ow,
+                                              int flip) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= ow) return;
   const double m0 = minv[0], m1 = minv[1], m2 = minv[2], m3 = minv[3], m4 = minv[4], m5 = minv[5];
@@ -580,11 +689,30 @@ __global__ void __launch_bounds__(256) k_preprocess(const unsigned char *__restr
     const int p11 = (y1ok && x1ok) ? img[((size_t)(sy + 1) * W + sx + 1) * 3 + c] : 0;
     int v = (p00 * w0 + p01 * w1 + p10 * w2 + p11 * w3 + (1 << 14)) >> 15;
     v = min(max(v, 0), 255);
-    const double r = __ddiv_rn(__dadd_rn(__ddiv_rn((double)v, 255.0), -(double)mean[c]), (double)stdv[c]);
-    const float f = (float)r;
+    float f;
+    if (kF32) {
+      f = __fdiv_rn(__fsub_rn(__fdiv_rn((float)v, 255.f), mean[c]), stdv[c]);
+    } else {
+      const double r = __ddiv_rn(__dadd_rn(__ddiv_rn((double)v, 255.0), -(double)mean[c]), (double)stdv[c]);
+      f = (float)r;
+    }
     out[c * plane + (size_t)y * ow + x] = f;
     if (flip) out[(3 + c) * plane + (size_t)y * ow + (ow - 1 - x)] = f;
   }
+}
+
+__global__ void __launch_bounds__(256) k_preprocess(const unsigned char *__restrict__ img, int H, int W,
+                                                    const double *__restrict__ minv, const float *__restrict__ mean,
+                                                    const float *__restrict__ stdv, float *__restrict__ out, int oh,
+                                                    int ow, int flip) {
+  preprocess_px<false>(img, H, W, minv, mean, stdv, out, oh, ow, flip);
+}
+
+__global__ void __launch_bounds__(256) k_preprocess_f32(const unsigned char *__restrict__ img, int H, int W,
+                                                        const double *__restrict__ minv, const float *__restrict__ mean,
+                                                        const float *__restrict__ stdv, float *__restrict__ out, int oh,
+                                                        int ow, int flip) {
+  preprocess_px<true>(img, H, W, minv, mean, stdv, out, oh, ow, flip);
 }
 }  // namespace cnb
 
@@ -640,6 +768,20 @@ extern "C" int cnb_preprocess_image(const uint8_t *image_hwc, int h, int w, cons
   cnb::k_preprocess<<<grid, 256, 0, (cudaStream_t)stream>>>(image_hwc, h, w, minv6, mean3, std3, out, out_h, out_w,
                                                             flip_test ? 1 : 0);
   CNB_CHECK_LAUNCH("cnb_preprocess_image");
+  cnb::count_launch();
+  return CNB_OK;
+}
+
+extern "C" int cnb_preprocess_image_f32(const uint8_t *image_hwc, int h, int w, const double *minv6, const float *mean3,
+                                        const float *std3, float *out, int out_h, int out_w, int flip_test,
+                                        void *stream) {
+  CNB_REQUIRE(image_hwc && minv6 && mean3 && std3 && out, CNB_EINVAL, "cnb_preprocess_image_f32: null pointer");
+  CNB_REQUIRE(h > 0 && w > 0 && out_h > 0 && out_w > 0 && h < 32768 && w < 32768, CNB_EINVAL,
+              "cnb_preprocess_image_f32: bad shape");
+  dim3 grid((unsigned)((out_w + 255) / 256), (unsigned)out_h);
+  cnb::k_preprocess_f32<<<grid, 256, 0, (cudaStream_t)stream>>>(image_hwc, h, w, minv6, mean3, std3, out, out_h, out_w,
+                                                                flip_test ? 1 : 0);
+  CNB_CHECK_LAUNCH("cnb_preprocess_image_f32");
   cnb::count_launch();
   return CNB_OK;
 }

@@ -299,6 +299,12 @@ PYBIND11_MODULE(_C, m) {
                              ptr<uint8_t>(keep), ptr<float>(thresh), ptr<void>(stream)),
           "cnb_topk_keep_wide");
   });
+  m.def("ddd_tail", [](P dets, int b, int n, int d, P trans, P calib, int nc, int cut, float thresh, P rows, P offsets,
+                       P seen, P stream) {
+    check(cnb_ddd_tail(ptr<const float>(dets), b, n, d, ptr<const double>(trans), ptr<const float>(calib), nc, cut,
+                       thresh, ptr<float>(rows), ptr<int32_t>(offsets), ptr<uint8_t>(seen), ptr<void>(stream)),
+          "cnb_ddd_tail");
+  });
   m.def("resize_image", [](P img, int h, int w, P out, int oh, int ow, P stream) {
     check(cnb_resize_image(ptr<const uint8_t>(img), h, w, ptr<uint8_t>(out), oh, ow, ptr<void>(stream)),
           "cnb_resize_image");
@@ -307,6 +313,12 @@ PYBIND11_MODULE(_C, m) {
     check(cnb_preprocess_image(ptr<const uint8_t>(img), h, w, ptr<const double>(minv), ptr<const float>(mean),
                                ptr<const float>(stdv), ptr<float>(out), oh, ow, flip, ptr<void>(stream)),
           "cnb_preprocess_image");
+  });
+  m.def("preprocess_image_f32", [](P img, int h, int w, P minv, P mean, P stdv, P out, int oh, int ow, int flip,
+                                   P stream) {
+    check(cnb_preprocess_image_f32(ptr<const uint8_t>(img), h, w, ptr<const double>(minv), ptr<const float>(mean),
+                                   ptr<const float>(stdv), ptr<float>(out), oh, ow, flip, ptr<void>(stream)),
+          "cnb_preprocess_image_f32");
   });
   m.def("dcnv2_workspace_bytes", &cnb_dcnv2_workspace_bytes);
   m.def("dcnv2_backward_workspace_bytes", &cnb_dcnv2_backward_workspace_bytes);

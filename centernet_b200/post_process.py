@@ -21,10 +21,9 @@ MAX_ROWS = 4096
 
 
 # ------------------------------------------------------------------ utils/image.py:27-60 (host, float64, B matrices)
-def _inv_affine(center, scale, output_size):
-    """2x3 float64 matrix of get_affine_transform(center, scale, 0, output_size, inv=1): output-grid -> image.
-    rot = 0, so the three point pairs of the reference define a uniform scale + translation; it is solved
-    from the same float32 points in float64 (cv2.getAffineTransform there)."""
+def _affine_points(center, scale, output_size):
+    """The three float32 point pairs (src in the image, dst on the output grid) of get_affine_transform(center,
+    scale, 0, output_size)."""
     f32 = np.float32
     if not isinstance(scale, (np.ndarray, list, tuple)):
         scale = np.array([scale, scale], dtype=f32)
@@ -40,8 +39,60 @@ def _inv_affine(center, scale, output_size):
     for p in (src, dst):
         d = p[0] - p[1]
         p[2] = p[1] + np.array([-d[1], d[0]], f32)
+    return src, dst
+
+
+def _inv_affine(center, scale, output_size):
+    """2x3 float64 matrix of get_affine_transform(center, scale, 0, output_size, inv=1): output-grid -> image.
+    rot = 0, so the three point pairs of the reference define a uniform scale + translation; it is solved
+    from the same float32 points in float64 (cv2.getAffineTransform there)."""
+    src, dst = _affine_points(center, scale, output_size)
     a = np.concatenate([dst.astype(np.float64), np.ones((3, 1))], axis=1)
     return np.linalg.solve(a, src.astype(np.float64)).T
+
+
+def cv_affine_transform(src, dst):
+    """cv2.getAffineTransform(src, dst) to the bit, without OpenCV: the 6x6 system of imgwarp.cpp (rows
+    [x, y, 1, 0, 0, 0] / [0, 0, 0, x, y, 1] per point, right-hand side the dst coordinates) solved as cv::solve's
+    DECOMP_LU solves it (hal LUImpl: partial pivoting on the largest |a|, elimination by multiples of -1 / pivot,
+    back substitution dividing by the pivot), every step a rounded float64 operation.  Returns 2x3 float64."""
+    src = np.asarray(src, np.float32).reshape(3, 2).astype(np.float64).tolist()
+    dst = np.asarray(dst, np.float32).reshape(3, 2).astype(np.float64).tolist()
+    a, b = [], []
+    for (x, y), (u, v) in zip(src, dst):
+        a += [[x, y, 1.0, 0.0, 0.0, 0.0], [0.0, 0.0, 0.0, x, y, 1.0]]
+        b += [u, v]
+    m = 6
+    for i in range(m):
+        k = i
+        for j in range(i + 1, m):
+            if abs(a[j][i]) > abs(a[k][i]):
+                k = j
+        if a[k][i] == 0.0:
+            raise ValueError("cv_affine_transform: the three points are collinear")
+        if k != i:
+            a[i], a[k] = a[k], a[i]
+            b[i], b[k] = b[k], b[i]
+        d = -1.0 / a[i][i]
+        for j in range(i + 1, m):
+            alpha = a[j][i] * d
+            for c in range(i + 1, m):
+                a[j][c] += alpha * a[i][c]
+            b[j] += alpha * b[i]
+    for i in range(m - 1, -1, -1):
+        s = b[i]
+        for c in range(i + 1, m):
+            s -= a[i][c] * b[c]
+        b[i] = s / a[i][i]
+    return np.array(b, np.float64).reshape(2, 3)
+
+
+def cv_inv_affine(center, scale, output_size):
+    """get_affine_transform(center, scale, 0, output_size, inv=1) as the reference computes it (cv2 included), for
+    the ddd tail: at the KITTI metas (int32 image-size scales) the float64 solve of _inv_affine misses cv2 by one
+    ulp in some entries, which moves a back-projected coordinate by one float32 ulp now and then."""
+    src, dst = _affine_points(center, scale, output_size)
+    return cv_affine_transform(dst, src)
 
 
 def _trans_tensor(c, s, w, h, device):
@@ -322,3 +373,86 @@ def exdet_merge_device(dets_per_scale, metas, num_classes, max_per_image=100, fl
             res[j + 1] = rows_h[i, a:e][keep_h[i, a:e]].astype(np.float32)
         ret.append(res)
     return ret
+
+
+# ------------------------------------------------------------------ utils/post_process.py:13-80, detectors/ddd.py:75-88
+DDD_COLS = 13        # alpha, x1, y1, x2, y2, dim[3], X, Y, Z, rot_y, score
+
+
+def _ddd_tail(what, dets, c, s, calibs, out_w, out_h, num_classes, thresh):
+    """cnb_ddd_tail on dets [B, N, 18] (numpy or CUDA), one inverse affine and one calibration per image, and ONE
+    device->host copy.  thresh None: every row (ddd_post_process); else merge_outputs' score > float32(thresh).
+    Returns a list (per image) of {class id: float32 [n, 13]}, a class without rows being np.array([], float32) as
+    the reference builds it, and with a cut a class the cut emptied [0, 13]."""
+    if isinstance(dets, torch.Tensor) and not dets.is_cuda:
+        raise NotImplementedError("%s: CUDA tensors or numpy arrays only (no CPU path)" % what)
+    shape = tuple(dets.shape)
+    if len(shape) == 3 and shape[2] == 16:
+        raise ValueError("%s: dets has 16 columns (ddd_decode without wh, --not_reg_bbox); the reference's "
+                         "ddd_post_process_3d reads the box size from columns 8:10 of every row and raises IndexError "
+                         "without it" % what)
+    if len(shape) != 3 or shape[2] != 18 or shape[0] < 1 or shape[1] < 1:
+        raise ValueError("%s: dets must be [B, N, 18] (ddd_decode with wh), got %s" % (what, shape))
+    num_classes = int(num_classes)
+    if not 0 < num_classes <= 8192:
+        raise ValueError("%s: num_classes must be in [1, 8192]" % what)
+    b, n = shape[0], shape[1]
+    if n >= 1 << 24:
+        raise NotImplementedError("%s: at most %d rows per image" % (what, (1 << 24) - 1))
+    if len(c) != b or len(s) != b or len(calibs) != b:
+        raise ValueError("%s: one 'c', 's' and calib per image (%d)" % (what, b))
+    d = _as_cuda(dets)
+    dev = d.device
+    mats = np.stack([cv_inv_affine(c[i], s[i], (out_w, out_h)).reshape(6) for i in range(b)], 0)
+    cal = np.stack([np.asarray(k, np.float32).reshape(12) for k in calibs], 0)
+    # the matrices and the calibrations in ONE copy from pinned memory (no host synchronisation)
+    host = np.concatenate([mats.astype(np.float64).view(np.uint8).reshape(-1), cal.view(np.uint8).reshape(-1)])
+    params = torch.from_numpy(host).pin_memory().to(dev, non_blocking=True)
+    trans, calib = params[:b * 48].view(torch.float64), params[b * 48:].view(torch.float32)
+    rows = torch.empty((b, n * DDD_COLS), dtype=torch.float32, device=dev)
+    offs = torch.empty((b, num_classes + 1), dtype=torch.int32, device=dev)
+    seen = torch.empty((b, num_classes), dtype=torch.uint8, device=dev)
+    C.ddd_tail(ptr(d), b, n, 18, ptr(trans), ptr(calib), num_classes, int(thresh is not None),
+               float(np.float32(0.0 if thresh is None else thresh)), ptr(rows), ptr(offs), ptr(seen), stream_ptr(d))
+    packed = torch.cat([rows, offs.float(), seen.float()], dim=1).cpu().numpy()   # one D2H
+    rows_h = packed[:, :n * DDD_COLS].reshape(b, n, DDD_COLS)
+    offs_h = packed[:, n * DDD_COLS:n * DDD_COLS + num_classes + 1].astype(np.int64)     # < 2^24: exact in float32
+    seen_h = packed[:, n * DDD_COLS + num_classes + 1:] > 0
+    ret = []
+    for i in range(b):
+        res = {}
+        for j in range(num_classes):
+            a, e = offs_h[i, j], offs_h[i, j + 1]
+            res[j + 1] = rows_h[i, a:e].copy() if seen_h[i, j] else np.array([], np.float32)
+        ret.append(res)
+    return ret
+
+
+def ddd_post_process(dets, c, s, calibs, opt):
+    """Drop-in for utils/post_process.py:75-80 (ddd_post_process_2d then _3d) on the device.
+      dets: [B, K, 18] ddd_decode output, numpy array or CUDA tensor (left unmodified; the reference writes the
+            back-projected centres into it);
+      c, s: per-image centres and scales; calibs: per-image 3x4 calibrations, of which -- as the reference does --
+            calibs[0] is used for EVERY image (taken as float32, the dtype DddDetector and the dataset give it);
+      opt: reads output_w, output_h and num_classes.
+    Returns a list (per image) of {class id: float32 [n, 13] array of alpha, x1, y1, x2, y2, dim[3], X, Y, Z, rot_y,
+    score}, a class without rows being np.array([], float32) of shape (0,).  Every value that does not go through an
+    arctan2 equals the reference's bit for bit; alpha and rot_y are the float32 closest to the angle, numpy's float32
+    arctan2 is within a few ulp of it.  16-column dets (no wh) raise ValueError: the reference cannot process them."""
+    b = int(dets.shape[0])
+    return _ddd_tail("ddd_post_process", dets, c, s, [calibs[0]] * b, int(opt.output_w), int(opt.output_h),
+                     int(opt.num_classes), None)
+
+
+def ddd_merge_device(dets, meta, num_classes, peak_thresh=0.2):
+    """The tail of DddDetector.run for one image batch: `post_process` (detectors/ddd.py:75-80) of every image with
+    its OWN calibration, then `merge_outputs` (:82-88), the cut to score > float32(peak_thresh) (NaN dropped, +inf
+    kept).  Equals running the reference detector once per image.
+      dets: [B, K, 18] CUDA tensor (or numpy array) from ddd_decode / ddd_decode_from_logits; one tensor, not a
+            list of scales: DddDetector.pre_process ignores the test scale and merge_outputs reads detections[0] only;
+      meta: 'c', 's' and 'calib' ([3, 4] float32) as per-image sequences, 'out_height', 'out_width' (ddd_pre_process
+            returns them for one image).
+    Returns a list (per image) of {class id: float32 [n, 13]}: a class without rows is np.array([], float32) of shape
+    (0,), a class the cut emptied has shape (0, 13), as merge_outputs leaves them -- one device->host copy."""
+    return _ddd_tail("ddd_merge_device", dets, meta["c"], meta["s"], meta["calib"], int(meta["out_width"]),
+                     int(meta["out_height"]), num_classes, float(peak_thresh))

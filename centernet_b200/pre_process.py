@@ -7,6 +7,7 @@ import numpy as np
 import torch
 
 from ._lib import C, ptr, stream_ptr
+from .post_process import _affine_points, cv_affine_transform
 
 
 def _forward_affine(center, scale, output_size):
@@ -80,4 +81,44 @@ def pre_process(image, scale, mean, std, fix_res=True, input_h=512, input_w=512,
     C.preprocess_image(ptr(img), new_height, new_width, ptr(minv), ptr(mean_t), ptr(std_t), ptr(out), inp_height, inp_width,
                        int(bool(flip_test)), stream_ptr(out))
     meta = {'c': c, 's': s, 'out_height': inp_height // down_ratio, 'out_width': inp_width // down_ratio}
+    return out, meta
+
+
+# DddDetector.__init__'s calibration (detectors/ddd.py:25-27), the default of ddd_pre_process.
+KITTI_CALIB = np.array([[707.0493, 0, 604.0814, 45.75831],
+                        [0, 707.0493, 180.5066, -0.3454157],
+                        [0, 0, 1., 0.004981016]], dtype=np.float32)
+
+
+def ddd_pre_process(image, input_h, input_w, mean, std, keep_res=False, calib=None, down_ratio=4, device=None):
+    """DddDetector.pre_process (detectors/ddd.py:30-55) on the device, bit-identical to the reference: no resize (the
+    detector ignores the test scale), c = (w / 2, h / 2), s = int32 [input_w, input_h] with keep_res else int32
+    [w, h], the same warp as pre_process, and the detector's float32 normalisation (x / 255 then (x - mean) / std in
+    float32, where BaseDetector normalises in float64).
+      image: uint8 [H, W, 3] numpy array (BGR) or CUDA uint8 tensor; mean, std: 3 values each;
+      calib: the image's 3x4 projection matrix (float32), default the detector's KITTI matrix.
+    Returns (images [1, 3, input_h, input_w] fp32 CUDA tensor, meta {'c', 's', 'out_height', 'out_width', 'calib'});
+    the uint8 image and the warp parameters are the only host->device copies."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if isinstance(image, torch.Tensor):
+        if not image.is_cuda or image.dtype != torch.uint8:
+            raise NotImplementedError("ddd_pre_process: uint8 CUDA tensor or numpy array")
+        img = image.contiguous()
+        dev = img.device
+    else:
+        img = torch.from_numpy(np.ascontiguousarray(image, dtype=np.uint8)).to(dev, non_blocking=True)
+    if img.dim() != 3 or int(img.shape[2]) != 3:
+        raise ValueError("ddd_pre_process: image must be [H, W, 3], got %s" % (tuple(img.shape),))
+    height, width = int(img.shape[0]), int(img.shape[1])
+    c = np.array([width / 2, height / 2], dtype=np.float32)
+    s = np.array([input_w, input_h] if keep_res else [width, height], dtype=np.int32)
+    # cv2.getAffineTransform's own matrix, OpenCV or not (the float64 solve misses it by one ulp at KITTI sizes)
+    minv = np.array(_invert(cv_affine_transform(*_affine_points(c, s, [input_w, input_h]))), np.float64)
+    norm = np.concatenate([np.asarray(mean, np.float32).reshape(3), np.asarray(std, np.float32).reshape(3)])
+    params = torch.from_numpy(np.concatenate([minv.view(np.uint8), norm.view(np.uint8)])).to(dev, non_blocking=True)
+    out = torch.empty((1, 3, input_h, input_w), dtype=torch.float32, device=dev)
+    C.preprocess_image_f32(ptr(img), height, width, ptr(params[:48]), ptr(params[48:60]), ptr(params[60:72]),
+                           ptr(out), input_h, input_w, 0, stream_ptr(out))
+    calib = np.array(calib, dtype=np.float32) if calib is not None else KITTI_CALIB.copy()
+    meta = {'c': c, 's': s, 'out_height': input_h // down_ratio, 'out_width': input_w // down_ratio, 'calib': calib}
     return out, meta

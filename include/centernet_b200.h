@@ -603,6 +603,19 @@ int cnb_soft_nms_strided(const float *rows, float *out, const int32_t *offsets, 
 int cnb_topk_keep_wide(const float *rows, int b, int n_cap, int d, const int32_t *offsets, int num_classes,
                        int max_per_image, uint8_t *keep, float *thresh, void *stream);
 
+/* The ddd tail (utils/post_process.py:13-80 with utils/ddd_utils.py:66-111, and
+ * DddDetector.merge_outputs, detectors/ddd.py:82-88).
+ * cnb_ddd_tail: dets [b,n,18] (ddd_decode with wh: x, y, score, rot[8], depth,
+ *   dim[3], w, h, class) -> rows [b,n,13] = alpha, x1, y1, x2, y2, dim[3], X, Y, Z,
+ *   rot_y, score, grouped by class as cnb_group_by_class groups them, and offsets
+ *   [b,classes+1].  trans [b][6]: each image's inverse affine (cnb_post_transform);
+ *   calib [b][12]: each image's 3x4 float32 projection matrix.  With cut != 0 only
+ *   rows with score > thresh are kept (NaN dropped).  seen (nullable) [b,classes]:
+ *   1 where the class has a row before the cut.  d must be 18; outputs must not
+ *   overlap any other buffer. */
+int cnb_ddd_tail(const float *dets, int b, int n, int d, const double *trans, const float *calib, int num_classes,
+                 int cut, float thresh, float *rows, int32_t *offsets, uint8_t *seen, void *stream);
+
 /* ------------------------------------------- N4: detector input pre-processing
  * detectors/base_detector.py:37-65 for one image: cv2.warpAffine(INTER_LINEAR,
  * border 0) + (x/255 - mean)/std + HWC->CHW (+ mirrored copy when flip_test).
@@ -617,6 +630,11 @@ int cnb_resize_image(const uint8_t *image_hwc, int h, int w, uint8_t *out_hwc, i
 int cnb_preprocess_image(const uint8_t *image_hwc, int h, int w, const double *minv6,
                          const float *mean3, const float *std3, float *out,
                          int out_h, int out_w, int flip_test, void *stream);
+/* cnb_preprocess_image with DddDetector.pre_process's normalisation (detectors/ddd.py:50-51):
+ * x / 255 then (x - mean) / std in float32 rather than float64; the same warp. */
+int cnb_preprocess_image_f32(const uint8_t *image_hwc, int h, int w, const double *minv6,
+                             const float *mean3, const float *std3, float *out,
+                             int out_h, int out_w, int flip_test, void *stream);
 
 #ifdef __cplusplus
 }

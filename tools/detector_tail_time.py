@@ -10,7 +10,13 @@ Workloads (seed 317): exdet at B = 1 and B = 32, flip test, 1 and 5 test scales 
 without --nms.  Both tails start from the same decode outputs on the device; every timed pair of results is checked
 to be equal bit for bit.  Also times the two top-K cuts (k_topk_keep's sort, k_topk_keep_wide's radix select) at
 <= 4096 rows per image.  Prints per-image ms (median of --repeats calls after --warmup), the card name and its
-power limit, and with --out DIR writes DIR/detector_tail_time.json.  GPU only."""
+power limit, and with --out DIR writes DIR/detector_tail_time.json.  GPU only.
+
+--task ddd times the ddd tail instead: ddd_merge_device against what detectors/ddd.py:75-88 does per image (the D2H
+copy of the decode output, ddd_post_process and merge_outputs), restated row by row by tests/ddd_tail_np.py, from the
+same ddd_decode_from_logits outputs (seed 317, 3-class 96 x 320 heads, K = 100) at B = 1 and B = 32, KITTI metas
+and one calibration per image; every timed pair of results is checked (bit for bit but alpha and rot_y, which must
+agree within 2.5e-6 rad)."""
 import argparse
 import json
 import os
@@ -29,6 +35,8 @@ from centernet_b200 import decode as D  # noqa: E402
 from centernet_b200 import post_process as P  # noqa: E402
 from centernet_b200._lib import C, ptr, stream_ptr  # noqa: E402
 from oracle import build_ref  # noqa: E402
+import ddd_tail_cases as DC  # noqa: E402
+import ddd_tail_np as DO  # noqa: E402
 import detector_tails_np as O  # noqa: E402
 
 F32 = np.float32
@@ -145,12 +153,58 @@ def cut_times(warmup, repeats):
     return res
 
 
+def ddd_times(warmup, repeats):
+    """ddd_merge_device against the per-image host tail, from the same decode outputs."""
+    res = []
+    for B in (1, 32):
+        g = torch.Generator().manual_seed(317)
+        H, W = DC.INPUT_HW[0] // 4, DC.INPUT_HW[1] // 4
+        heads = [torch.randn(B, ch, H, W, generator=g).cuda() for ch in (DC.NUM_CLASSES, 8, 1, 3, 2, 2)]
+        heads[3] = heads[3] * 0.3 + 1.5                                  # dims
+        heads[4] = heads[4].abs() * 20                                   # wh
+        dets = D.ddd_decode_from_logits(*heads, K=100)
+        base = np.array([[707.0493, 0, 604.0814, 45.75831], [0, 707.0493, 180.5066, -0.3454157],
+                         [0, 0, 1., 0.004981016]], F32)
+        meta = {"c": [np.array([621.0, 187.5], F32)] * B, "s": [np.array([1242, 375], np.int32)] * B,
+                "calib": [base + F32(i) * F32(0.25) for i in range(B)], "out_height": H, "out_width": W}
+
+        def host():
+            out = []
+            for i in range(B):
+                h = dets[i:i + 1].cpu().numpy()                  # the per-image copy of detectors/ddd.py:76
+                r = DO.ddd_post_process(h, [meta["c"][i]], [meta["s"][i]], [meta["calib"][i]], W, H, DC.NUM_CLASSES)
+                out.append(DO.merge_outputs(r[0], DC.NUM_CLASSES, DC.PEAK_THRESH))
+            return out
+
+        td, rd = timed(lambda: P.ddd_merge_device(dets, meta, DC.NUM_CLASSES, DC.PEAK_THRESH), warmup, repeats)
+        th, rh = timed(host, min(warmup, 1), max(1, repeats // 2))
+        DC.assert_ddd_equal(DC.flatten(rd), DC.flatten(rh), "ddd B=%d" % B)
+        n = int(sum(len(r[j]) for r in rd for j in r))
+        row = {"B": B, "K": 100, "rows_kept": n, "device_ms_per_image": td / B, "host_ms_per_image": th / B,
+               "equal": True}
+        res.append(row)
+        print("ddd B=%d K=100: device %.3f ms/image, host %.3f ms/image, %d rows kept, equal True"
+              % (B, td / B, th / B, n))
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="directory for detector_tail_time.json (default: print only)")
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--repeats", type=int, default=5)
+    ap.add_argument("--task", choices=("exdet_multi_pose", "ddd"), default="exdet_multi_pose")
     a = ap.parse_args()
+    if a.task == "ddd":
+        torch.cuda.set_device(0)
+        name, limit = card()
+        print("card: %s, power limit %s" % (name, limit))
+        results = {"card": name, "power_limit": limit, "ddd": ddd_times(a.warmup, a.repeats)}
+        if a.out:
+            os.makedirs(a.out, exist_ok=True)
+            with open(os.path.join(a.out, "detector_tail_time_ddd.json"), "w") as f:
+                json.dump(results, f, indent=1)
+        return
     nms = build_ref.load_nms()
     if nms is None:
         sys.exit("oracle/_ref has no compiled reference soft_nms: run python -m oracle.build_ref where the reference "
