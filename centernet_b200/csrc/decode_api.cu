@@ -93,6 +93,50 @@ __global__ void __launch_bounds__(256) k_gather_feat_bwd(const float *__restrict
   }
 }
 
+// The gather of a bf16 / fp16 feat read in place: each value widens exactly, so out is the gather of the upcast.
+template <typename T>
+__global__ void __launch_bounds__(256) k_gather_feat_half(const T *__restrict__ feat, const int64_t *__restrict__ ind,
+                                                          float *__restrict__ out, int B, int C, long long HW, int M) {
+  const long long total = (long long)B * M * C;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int ch = (int)(i % C);
+    const long long bm = i / C;
+    const int b = (int)(bm / M);
+    const long long sp = ind[bm];
+    float v = 0.0f;
+    if (sp >= 0 && sp < HW) v = (float)__ldg(feat + ((long long)b * C + ch) * HW + sp);
+    out[i] = v;
+  }
+}
+
+// Its adjoint into a zero-filled bf16 / fp16 grad_feat.  One thread per (image, m, channel); the thread of the first
+// m that holds a map index is that element's only writer: it adds the rows of every m with the same index in fp32 in
+// ascending m, starting from the map's 0 as k_gather_feat_bwd does, and rounds the sum once.
+template <typename T>
+__global__ void __launch_bounds__(256) k_gather_feat_bwd_half(const float *__restrict__ grad_out,
+                                                              const int64_t *__restrict__ ind,
+                                                              T *__restrict__ grad_feat, int B, int C, long long HW,
+                                                              int M) {
+  const long long total = (long long)B * M * C;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int ch = (int)(i % C);
+    const long long bm = i / C;
+    const int b = (int)(bm / M), m0 = (int)(bm % M);
+    const int64_t *row = ind + (long long)b * M;
+    const long long sp = __ldg(row + m0);
+    if (sp < 0 || sp >= HW) continue;
+    bool first = true;
+    for (int q = 0; first && q < m0; ++q) first = (__ldg(row + q) != sp);
+    if (!first) continue;
+    float sum = 0.0f;
+    for (int q = m0; q < M; ++q)
+      if (__ldg(row + q) == sp) sum += __ldg(grad_out + ((long long)b * M + q) * C + ch);
+    grad_feat[((long long)b * C + ch) * HW + sp] = T(sum);
+  }
+}
+
 // ------------------------------------------------------------------ A9: ddd epilogue
 // models/decode.py:432-460: [xs, ys, score, rot(8), depth, dim(3), (wh(2)), cls]
 __global__ void __launch_bounds__(128) k_ddd_epilogue(const float *__restrict__ scores,
@@ -388,6 +432,48 @@ int cnb_gather_feat(const float *feat, const int64_t *ind, float *out, int b, in
   const int grid = (int)((total + 255) / 256 < 65535 ? (total + 255) / 256 : 65535);
   k_gather_feat<<<grid, 256, 0, (cudaStream_t)stream>>>(feat, ind, out, b, c, hw, m);
   CNB_CHECK_LAUNCH("cnb_gather_feat");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_gather_feat_ex(const void *feat, int feat_dtype, const int64_t *ind, float *out, int b, int c, int hw, int m,
+                       void *stream) {
+  CNB_REQUIRE(dtype_known(feat_dtype), CNB_EINVAL, "cnb_gather_feat_ex: unknown dtype code %d", feat_dtype);
+  if (feat_dtype == CNB_DTYPE_F32) return cnb_gather_feat(reinterpret_cast<const float *>(feat), ind, out, b, c, hw, m, stream);
+  CNB_REQUIRE(feat && ind && out, CNB_EINVAL, "cnb_gather_feat_ex: null pointer");
+  CNB_REQUIRE(b > 0 && c > 0 && hw > 0 && m > 0, CNB_EINVAL, "cnb_gather_feat_ex: non-positive dimension");
+  const long long total = (long long)b * m * c;
+  const int grid = (int)((total + 255) / 256 < 65535 ? (total + 255) / 256 : 65535);
+  if (feat_dtype == CNB_DTYPE_BF16)
+    k_gather_feat_half<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16 *>(feat), ind, out,
+                                                               b, c, hw, m);
+  else
+    k_gather_feat_half<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half *>(feat), ind, out, b, c,
+                                                               hw, m);
+  CNB_CHECK_LAUNCH("cnb_gather_feat_ex");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_gather_feat_backward_ex(const float *grad_out, const int64_t *ind, void *grad_feat, int feat_dtype, int b,
+                                int c, int hw, int m, void *stream) {
+  CNB_REQUIRE(dtype_known(feat_dtype), CNB_EINVAL, "cnb_gather_feat_backward_ex: unknown dtype code %d", feat_dtype);
+  CNB_REQUIRE(grad_out && ind && grad_feat, CNB_EINVAL, "cnb_gather_feat_backward_ex: null pointer");
+  CNB_REQUIRE(b > 0 && c > 0 && hw > 0 && m > 0, CNB_EINVAL, "cnb_gather_feat_backward_ex: non-positive dimension");
+  const size_t elem = feat_dtype == CNB_DTYPE_F32 ? 4 : 2;
+  CNB_CUDA(cudaMemsetAsync(grad_feat, 0, (size_t)b * c * hw * elem, (cudaStream_t)stream));
+  if (feat_dtype == CNB_DTYPE_F32)
+    return cnb_gather_feat_backward(grad_out, ind, reinterpret_cast<float *>(grad_feat), b, c, hw, m, stream);
+  const long long total = (long long)b * m * c;
+  const int grid = (int)((total + 255) / 256 < 65535 ? (total + 255) / 256 : 65535);
+  if (feat_dtype == CNB_DTYPE_BF16)
+    k_gather_feat_bwd_half<<<grid, 256, 0, (cudaStream_t)stream>>>(grad_out, ind,
+                                                                   reinterpret_cast<__nv_bfloat16 *>(grad_feat), b, c,
+                                                                   hw, m);
+  else
+    k_gather_feat_bwd_half<<<grid, 256, 0, (cudaStream_t)stream>>>(grad_out, ind, reinterpret_cast<__half *>(grad_feat),
+                                                                   b, c, hw, m);
+  CNB_CHECK_LAUNCH("cnb_gather_feat_backward_ex");
   count_launch();
   return CNB_OK;
 }

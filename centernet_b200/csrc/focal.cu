@@ -13,6 +13,8 @@
 // is never materialised.  num_pos -- needed to normalise the gradient in the same pass -- is
 // known up front from the object lists (one positive per distinct valid centre inside the map).
 #include <stdlib.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include "common.cuh"
 
 namespace cnb {
@@ -437,6 +439,281 @@ __global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ out
   }
 }
 
+// ------------------------------------------------------------------ bf16 / fp16 pred, read in place
+// Both formats widen to fp32 exactly and everything after the load is the fp32 arithmetic above, so the loss is
+// bit for bit the loss of the fp32 kernels on the .float() upcast: same grid, same elements per thread, same
+// (e0 + e1) + (e2 + e3) groups, same partials.  The gradient cannot be finished in the forward pass as the fp32
+// kernels do: it has to be rounded to T once, AFTER the scale by the loss's incoming gradient, which only backward
+// knows.  For the dense loss the same kernel body runs twice: BWD = false adds the loss, BWD = true evaluates
+// focal_elem again and stores T(grad * *grad_out).  __fmul_rn keeps that product out of any contraction with
+// focal_elem's last multiply.
+template <typename T> __device__ __forceinline__ float widen(T v);
+template <> __device__ __forceinline__ float widen<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <> __device__ __forceinline__ float widen<__half>(__half v) { return __half2float(v); }
+template <typename T> __device__ __forceinline__ T narrow(float v);   // round to nearest even; fp16 overflows to inf
+template <> __device__ __forceinline__ __nv_bfloat16 narrow<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ __half narrow<__half>(float v) { return __float2half_rn(v); }
+
+template <typename T> union Pack4 { uint2 u; T t[4]; };
+// 4 consecutive elements: one 8-byte access when p is 8-byte aligned (al8), else four 2-byte ones
+template <typename T>
+__device__ __forceinline__ float4 load4(const T *p, bool al8) {
+  Pack4<T> r;
+  if (al8) {
+    r.u = __ldg(reinterpret_cast<const uint2 *>(p));
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) r.t[j] = __ldg(p + j);
+  }
+  return make_float4(widen<T>(r.t[0]), widen<T>(r.t[1]), widen<T>(r.t[2]), widen<T>(r.t[3]));
+}
+template <typename T>
+__device__ __forceinline__ void store4(T *p, bool al8, float a, float b, float c, float d) {
+  Pack4<T> r;
+  r.t[0] = narrow<T>(a); r.t[1] = narrow<T>(b); r.t[2] = narrow<T>(c); r.t[3] = narrow<T>(d);
+  if (al8) {
+    *reinterpret_cast<uint2 *>(p) = r.u;
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) p[j] = r.t[j];
+  }
+}
+__device__ __forceinline__ float incoming_grad(const float *grad_out) { return grad_out ? __ldg(grad_out) : 1.0f; }
+
+// Dense target.  The fp32 kernel takes its float4 path when pred, gt and grad are 16-byte aligned; a .float() upcast
+// and its gradient are fresh allocations, so on the upcast that is decided by gt alone, and so is the grouping here.
+// BWD = false: acc holds num_pos (pass 0), the loss goes to out2.  BWD = true: out2 is the forward's result.
+template <typename T, bool LOGITS, bool BWD>
+__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense_half(const T *__restrict__ pred,
+                                                                    const float *__restrict__ gt, long long n,
+                                                                    FocalAcc *acc, float *out2,
+                                                                    const float *__restrict__ grad_out,
+                                                                    T *__restrict__ grad) {
+  const float np_ = BWD ? out2[1] : (float)acc->num_pos;
+  const float inv_norm = 1.0f / (np_ > 0.0f ? np_ : 1.0f);
+  const bool pos_live = np_ > 0.0f;
+  const float go = BWD ? incoming_grad(grad_out) : 0.0f;
+  double pos = 0, neg = 0;
+  const long long n4 = n >> 2;
+  const bool group4 = (((uintptr_t)gt & 15u) == 0);
+  const bool al8 = ((((uintptr_t)pred | (uintptr_t)grad) & 7u) == 0);
+  if (group4) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4;
+         i += (long long)gridDim.x * blockDim.x) {
+      const float4 p = load4<T>(pred + 4 * i, al8);
+      const float4 g = __ldg(reinterpret_cast<const float4 *>(gt) + i);
+      const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
+      const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
+      if (BWD) {
+        store4<T>(grad + 4 * i, al8, __fmul_rn(e0.grad, go), __fmul_rn(e1.grad, go), __fmul_rn(e2.grad, go),
+                  __fmul_rn(e3.grad, go));
+      } else {
+        pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
+        neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
+      }
+    }
+  }
+  for (long long i = (group4 ? (n4 << 2) : 0) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x) {
+    const Elem e = focal_elem<LOGITS>(widen<T>(pred[i]), gt[i], inv_norm, pos_live);
+    if (BWD) grad[i] = narrow<T>(__fmul_rn(e.grad, go));
+    else { pos += e.loss_pos; neg += e.loss_neg; }
+  }
+  if (!BWD) {
+    block_accumulate(pos, neg, acc);
+    finish_loss(acc, gridDim.x, out2);
+  }
+}
+
+// Target rebuilt from the object lists: k_focal_splat with half loads (its items, bands and tables).  This kernel is
+// issue-bound, and evaluating the tables and focal_elem a second time in backward measured slower than storing the
+// gradient (DESIGN 4.3.1): so, unlike the dense loss, the forward stores the fp32 gradient (grad32, nullable) and
+// backward is k_scale_round.  On the upcast the fp32 kernel groups by four whenever W % 4 == 0 (its pred and grad
+// are aligned); the plane bases are then 8-byte multiples.
+template <typename T, bool LOGITS>
+__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat_half(const T *__restrict__ pred, const int32_t *cls,
+                                                                    const int32_t *cx, const int32_t *cy,
+                                                                    const int32_t *rad, const uint8_t *valid, int M,
+                                                                    int C, int H, int W, float *__restrict__ grad32,
+                                                                    FocalAcc *acc, float *out2, int parts, int B) {
+  __shared__ Obj s_obj[MAX_OBJ_PER_PLANE];
+  __shared__ ObjTab s_tab[MAX_OBJ_PER_PLANE];
+  __shared__ float s_gauss[GAUSS_TAB_FLOATS];
+  __shared__ int s_n, s_total;
+  const float np_ = (float)acc->num_pos;
+  const float inv_norm = 1.0f / (np_ > 0.0f ? np_ : 1.0f);
+  const bool pos_live = np_ > 0.0f;
+  double pos = 0, neg = 0;
+  const int n_items = B * C * parts;
+  const bool group4 = (W % 4 == 0);
+  const bool al8 = (((uintptr_t)pred & 7u) == 0), g_al16 = (((uintptr_t)grad32 & 15u) == 0);
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    __syncthreads();   // the previous item's objects and tables are no longer read
+    const int plane = item / parts, part = item - plane * parts;
+    const int b = plane / C, c = plane - b * C;
+    const int y_lo = (int)((long long)H * part / parts), y_hi = (int)((long long)H * (part + 1) / parts);
+    const int nobj = gather_objects(cls, cx, cy, rad, valid, b, M, c, H, W, s_obj, &s_n, y_lo, y_hi);
+    if (nobj) build_tables(s_obj, nobj, s_tab, s_gauss, &s_total);
+    const long long base = (long long)plane * H * W;
+    if (group4) {
+      const int w4 = W / 4;
+      int y = y_lo + (int)threadIdx.x / w4, x = ((int)threadIdx.x - ((int)threadIdx.x / w4) * w4) * 4;
+      const int dyq = (int)blockDim.x / w4, dxq = ((int)blockDim.x - dyq * w4) * 4;
+      for (int i = y_lo * w4 + threadIdx.x; i < y_hi * w4; i += blockDim.x, y += dyq, x += dxq) {
+        if (x >= W) { x -= W; ++y; }
+        float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (nobj) g = target_at4(s_obj, s_tab, s_gauss, nobj, x, y);
+        const float4 p = load4<T>(pred + base + 4ll * i, al8);
+        const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
+        const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
+        pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
+        neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
+        if (grad32 && g_al16) {
+          reinterpret_cast<float4 *>(grad32 + base)[i] = make_float4(e0.grad, e1.grad, e2.grad, e3.grad);
+        } else if (grad32) {
+          float *gp = grad32 + base + 4ll * i;
+          gp[0] = e0.grad; gp[1] = e1.grad; gp[2] = e2.grad; gp[3] = e3.grad;
+        }
+      }
+    } else {
+      for (int i = y_lo * W + threadIdx.x; i < y_hi * W; i += blockDim.x) {
+        const int y = i / W, x = i - y * W;
+        const float g = nobj ? target_at(s_obj, s_tab, s_gauss, nobj, x, y) : 0.0f;
+        const Elem e = focal_elem<LOGITS>(widen<T>(pred[base + i]), g, inv_norm, pos_live);
+        pos += e.loss_pos; neg += e.loss_neg;
+        if (grad32) grad32[base + i] = e.grad;
+      }
+    }
+  }
+  block_accumulate(pos, neg, acc);
+  finish_loss(acc, gridDim.x, out2);
+}
+
+// out = T(g32 * *grad_out): the scale by the loss's incoming gradient, then the one rounding
+template <typename T>
+__global__ void __launch_bounds__(256) k_scale_round(const float *__restrict__ g32, long long n,
+                                                     const float *__restrict__ grad_out, T *__restrict__ out) {
+  const float go = incoming_grad(grad_out);
+  const bool vec = ((((uintptr_t)g32 & 15u) | ((uintptr_t)out & 7u)) == 0);
+  const long long n4 = vec ? (n >> 2) : 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const float4 g = __ldg(reinterpret_cast<const float4 *>(g32) + i);
+    store4<T>(out + 4 * i, true, __fmul_rn(g.x, go), __fmul_rn(g.y, go), __fmul_rn(g.z, go), __fmul_rn(g.w, go));
+  }
+  for (long long i = (n4 << 2) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x)
+    out[i] = narrow<T>(__fmul_rn(g32[i], go));
+}
+
+// ---- Reg*Loss on a bf16 / fp16 map: the map is read at the gathered positions only.
+// One (image, object, channel) element i of k_reg_loss: false when its index is outside the map.
+template <typename T>
+__device__ __forceinline__ bool reg_elem(const T *__restrict__ output, const float *mask_f,
+                                         const int64_t *__restrict__ ind, const float *__restrict__ target, int D,
+                                         long long HW, int M, int mode, long long i, float *diff, float *m,
+                                         float *scale) {
+  const int d = (int)(i % D);
+  const long long bm = i / D;
+  const int b = (int)(bm / M);
+  const long long sp = ind[bm];
+  if (sp < 0 || sp >= HW) return false;
+  *m = mask_f[(mode == 3) ? i : bm];
+  float pred = widen<T>(output[((long long)b * D + d) * HW + sp]);
+  float tgt = target[i];
+  *scale = 1.0f;
+  if (mode == 2) {
+    *scale = 1.0f / (tgt + 1e-4f);
+    pred = pred / (tgt + 1e-4f);
+    tgt = tgt * 0.0f + 1.0f;
+  }
+  *diff = pred * *m - tgt * *m;
+  return true;
+}
+
+// k_reg_loss's pass 0 (same single CTA, same strides and tree).  out2 = (loss, (float)(mask sum + 1e-4)): the second
+// is the denominator k_reg_loss divides its gradient by, kept for k_reg_grad_half.
+template <typename T>
+__global__ void __launch_bounds__(1024) k_reg_loss_half(const T *__restrict__ output, const float *mask_f,
+                                                        const int64_t *__restrict__ ind,
+                                                        const float *__restrict__ target, int B, int D, long long HW,
+                                                        int M, int mode, float *out2) {
+  __shared__ double red[2][32];
+  const long long n = (long long)B * M * D;
+  double loss = 0, msum = 0;
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+    float diff, m, scale;
+    if (!reg_elem<T>(output, mask_f, ind, target, D, HW, M, mode, i, &diff, &m, &scale)) continue;
+    const float ad = fabsf(diff);
+    loss += (mode == 1) ? (ad < 1.0f ? 0.5 * (double)ad * ad : (double)ad - 0.5) : (double)ad;
+    msum += (mode == 1) ? ((i % D == 0) ? (double)m : 0.0) : (double)m;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    loss += __shfl_xor_sync(0xffffffffu, loss, o);
+    msum += __shfl_xor_sync(0xffffffffu, msum, o);
+  }
+  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = loss; red[1][threadIdx.x >> 5] = msum; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double a = 0, c = 0;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { a += red[0][i]; c += red[1][i]; }
+    out2[0] = (float)(a / (c + 1e-4));
+    out2[1] = (float)(c + 1e-4);
+  }
+}
+
+// Every element of the fp32 gradient map that no index selects is +0, and autograd's scale makes it 0 * grad_out
+// (-0 for a negative grad_out): the fill of the half map.
+template <typename T>
+__global__ void __launch_bounds__(256) k_fill_scaled_zero(T *__restrict__ p, long long n,
+                                                          const float *__restrict__ grad_out) {
+  const T z = narrow<T>(__fmul_rn(0.0f, incoming_grad(grad_out)));
+  const bool al8 = (((uintptr_t)p & 7u) == 0);
+  Pack4<T> r;
+  r.t[0] = r.t[1] = r.t[2] = r.t[3] = z;
+  const long long n4 = al8 ? (n >> 2) : 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x)
+    reinterpret_cast<uint2 *>(p)[i] = r.u;
+  for (long long i = (n4 << 2) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x)
+    p[i] = z;
+}
+
+// The gradient k_reg_loss's pass 1 leaves in an fp32 map, scaled and rounded once.  One thread per (image, object,
+// channel); the thread of the first m that holds a map index is that element's only writer: it adds the
+// contributions of every m with the same index in fp32 in ascending m, as pass 1 does in the map, multiplies the sum
+// by *grad_out and rounds it to T.  Nothing is accumulated in the half map and there are no atomics.
+template <typename T>
+__global__ void __launch_bounds__(256) k_reg_grad_half(const T *__restrict__ output, const float *mask_f,
+                                                       const int64_t *__restrict__ ind,
+                                                       const float *__restrict__ target, int B, int D, long long HW,
+                                                       int M, int mode, const float *__restrict__ loss_den,
+                                                       const float *__restrict__ grad_out, T *__restrict__ grad) {
+  const long long n = (long long)B * M * D;
+  const float den = loss_den[1], go = incoming_grad(grad_out);
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int d = (int)(i % D);
+    const long long bm = i / D;
+    const int b = (int)(bm / M), m0 = (int)(bm % M);
+    const int64_t *row = ind + (long long)b * M;
+    const long long sp = row[m0];
+    if (sp < 0 || sp >= HW) continue;
+    bool first = true;
+    for (int q = 0; first && q < m0; ++q) first = (row[q] != sp);
+    if (!first) continue;
+    float sum = 0.0f;
+    for (int q = m0; q < M; ++q) {
+      if (row[q] != sp) continue;
+      float diff, m, scale;
+      reg_elem<T>(output, mask_f, ind, target, D, HW, M, mode, ((long long)b * M + q) * D + d, &diff, &m, &scale);
+      float g = (diff > 0.0f) ? 1.0f : (diff < 0.0f ? -1.0f : 0.0f);
+      if (mode == 1 && fabsf(diff) < 1.0f) g = diff;
+      g = g * m * scale / den;
+      if (g != 0.0f) sum += g;
+    }
+    grad[((long long)b * D + d) * HW + sp] = narrow<T>(__fmul_rn(sum, go));
+  }
+}
+
 static int focal_grid(long long n4) {
   long long g = (n4 + FOCAL_THREADS - 1) / FOCAL_THREADS;
   long long cap = (long long)num_sms() * 8;
@@ -538,6 +815,189 @@ int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, cons
                                                     grad_output);
   CNB_CHECK_LAUNCH("cnb_reg_loss");
   count_launch();
+  return CNB_OK;
+}
+
+}  // extern "C"
+
+// ---- bf16 / fp16 pred: forward (loss) and backward (gradient in pred's dtype) as two calls
+static bool half_code(int dt) { return dt == CNB_DTYPE_BF16 || dt == CNB_DTYPE_F16; }
+static bool dtype_code_known(int dt) { return dt == CNB_DTYPE_F32 || half_code(dt); }
+
+template <typename T, bool BWD>
+static void launch_focal_dense_half(int logits, int grid, cudaStream_t stream, const void *pred, const float *gt,
+                                    long long n, FocalAcc *acc, float *out2, const float *grad_out, void *grad) {
+  if (logits)
+    k_focal_dense_half<T, true, BWD><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), gt, n, acc, out2,
+                                                                         grad_out, static_cast<T *>(grad));
+  else
+    k_focal_dense_half<T, false, BWD><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), gt, n, acc, out2,
+                                                                          grad_out, static_cast<T *>(grad));
+}
+
+template <typename T>
+static void launch_focal_splat_half(int logits, cudaStream_t stream, const void *pred, const int32_t *cls,
+                                    const int32_t *cx, const int32_t *cy, const int32_t *rad, const uint8_t *valid,
+                                    int b, int m, int c, int h, int w, float *grad32, FocalAcc *acc, float *out2) {
+  const int parts = focal_parts(h), grid = splat_grid((long long)b * c * parts);
+  if (logits)
+    k_focal_splat_half<T, true><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), cls, cx, cy, rad, valid, m, c, h, w,
+                                                                    grad32, acc, out2, parts, b);
+  else
+    k_focal_splat_half<T, false><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), cls, cx, cy, rad, valid, m, c, h, w,
+                                                                     grad32, acc, out2, parts, b);
+}
+
+template <typename T>
+static void launch_reg_grad_half(cudaStream_t stream, const void *output, const float *mask_f, const int64_t *ind,
+                                 const float *target, int b, int d, long long hw, int m, int mode,
+                                 const float *loss_den, const float *grad_out, void *grad) {
+  const long long total = (long long)b * d * hw, work = (long long)b * m * d;
+  const long long fill_ctas = (total / 4 + 255) / 256 + 1, cap = (long long)num_sms() * 16;
+  k_fill_scaled_zero<<<(int)(fill_ctas < cap ? fill_ctas : cap), 256, 0, stream>>>(static_cast<T *>(grad), total,
+                                                                                    grad_out);
+  k_reg_grad_half<<<(int)((work + 255) / 256 < cap ? (work + 255) / 256 : cap), 256, 0, stream>>>(
+      static_cast<const T *>(output), mask_f, ind, target, b, d, hw, m, mode, loss_den, grad_out,
+      static_cast<T *>(grad));
+}
+
+extern "C" {
+
+int cnb_focal_loss_ex(const void *pred, int pred_dtype, const float *gt, long long n, int logits, float *out2,
+                      void *workspace, size_t workspace_bytes, void *stream_) {
+  CNB_REQUIRE(dtype_code_known(pred_dtype), CNB_EINVAL, "cnb_focal_loss_ex: unknown dtype code %d", pred_dtype);
+  if (pred_dtype == CNB_DTYPE_F32)
+    return cnb_focal_loss(static_cast<const float *>(pred), gt, n, logits, 1.0f, out2, nullptr, workspace,
+                          workspace_bytes, stream_);
+  CNB_REQUIRE(pred && gt && out2 && workspace, CNB_EINVAL, "cnb_focal_loss_ex: null pointer");
+  CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_loss_ex: n=%lld", n);
+  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes(n), CNB_EWORKSPACE, "cnb_focal_loss_ex: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
+  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
+  const int grid = focal_grid(n / 4 + 1);
+  k_count_pos_dense<<<grid, FOCAL_THREADS, 0, stream>>>(gt, n, acc);
+  CNB_CHECK_LAUNCH("cnb_focal_loss_ex count");
+  if (pred_dtype == CNB_DTYPE_BF16)
+    launch_focal_dense_half<__nv_bfloat16, false>(logits, grid, stream, pred, gt, n, acc, out2, nullptr, nullptr);
+  else
+    launch_focal_dense_half<__half, false>(logits, grid, stream, pred, gt, n, acc, out2, nullptr, nullptr);
+  CNB_CHECK_LAUNCH("cnb_focal_loss_ex");
+  count_launch(2);
+  return CNB_OK;
+}
+
+int cnb_focal_grad_ex(const void *pred, int pred_dtype, const float *gt, long long n, int logits,
+                      const float *loss_num_pos, const float *grad_out, void *grad, void *stream_) {
+  CNB_REQUIRE(dtype_code_known(pred_dtype), CNB_EINVAL, "cnb_focal_grad_ex: unknown dtype code %d", pred_dtype);
+  CNB_REQUIRE(half_code(pred_dtype), CNB_EUNSUPPORTED,
+              "cnb_focal_grad_ex: bf16 / fp16 only (cnb_focal_loss writes the fp32 gradient in its one pass)");
+  CNB_REQUIRE(pred && gt && loss_num_pos && grad, CNB_EINVAL, "cnb_focal_grad_ex: null pointer");
+  CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_grad_ex: n=%lld", n);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int grid = focal_grid(n / 4 + 1);
+  float *out2 = const_cast<float *>(loss_num_pos);   // read only when BWD
+  if (pred_dtype == CNB_DTYPE_BF16)
+    launch_focal_dense_half<__nv_bfloat16, true>(logits, grid, stream, pred, gt, n, nullptr, out2, grad_out, grad);
+  else
+    launch_focal_dense_half<__half, true>(logits, grid, stream, pred, gt, n, nullptr, out2, grad_out, grad);
+  CNB_CHECK_LAUNCH("cnb_focal_grad_ex");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_focal_splat_loss_ex(const void *pred, int pred_dtype, const int32_t *obj_cls, const int32_t *obj_cx,
+                            const int32_t *obj_cy, const int32_t *obj_radius, const uint8_t *obj_valid, int b, int m,
+                            int c, int h, int w, int logits, float *out2, float *grad32, void *workspace,
+                            size_t workspace_bytes, void *stream_) {
+  CNB_REQUIRE(dtype_code_known(pred_dtype), CNB_EINVAL, "cnb_focal_splat_loss_ex: unknown dtype code %d", pred_dtype);
+  if (pred_dtype == CNB_DTYPE_F32)
+    return cnb_focal_splat_loss(static_cast<const float *>(pred), obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, b, m,
+                                c, h, w, logits, 1.0f, out2, grad32, workspace, workspace_bytes, stream_);
+  CNB_REQUIRE(pred && obj_cls && obj_cx && obj_cy && obj_radius && obj_valid && out2 && workspace, CNB_EINVAL,
+              "cnb_focal_splat_loss_ex: null pointer");
+  CNB_REQUIRE(b > 0 && m > 0 && c > 0 && h > 0 && w > 0, CNB_EINVAL, "cnb_focal_splat_loss_ex: non-positive dimension");
+  CNB_REQUIRE(m <= MAX_OBJ_PER_PLANE, CNB_EUNSUPPORTED,
+              "cnb_focal_splat_loss_ex: at most %d objects per image (got %d)", MAX_OBJ_PER_PLANE, m);
+  CNB_REQUIRE((long long)c * h * w < (1ll << 31), CNB_EUNSUPPORTED, "cnb_focal_splat_loss_ex: c*h*w must be < 2^31");
+  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes((long long)b * c * h * w), CNB_EWORKSPACE,
+              "cnb_focal_splat_loss_ex: workspace too small");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
+  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
+  k_count_pos_objects<<<b, 128, (size_t)m * sizeof(int), stream>>>(obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, m, c, h,
+                                                                    w, acc);
+  CNB_CHECK_LAUNCH("cnb_focal_splat_loss_ex count");
+  if (pred_dtype == CNB_DTYPE_BF16)
+    launch_focal_splat_half<__nv_bfloat16>(logits, stream, pred, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, b, m,
+                                           c, h, w, grad32, acc, out2);
+  else
+    launch_focal_splat_half<__half>(logits, stream, pred, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, b, m, c, h,
+                                    w, grad32, acc, out2);
+  CNB_CHECK_LAUNCH("cnb_focal_splat_loss_ex");
+  count_launch(2);
+  return CNB_OK;
+}
+
+int cnb_focal_splat_grad_ex(const float *grad32, long long n, const float *grad_out, void *grad, int grad_dtype,
+                            void *stream_) {
+  CNB_REQUIRE(dtype_code_known(grad_dtype), CNB_EINVAL, "cnb_focal_splat_grad_ex: unknown dtype code %d", grad_dtype);
+  CNB_REQUIRE(half_code(grad_dtype), CNB_EUNSUPPORTED,
+              "cnb_focal_splat_grad_ex: bf16 / fp16 only (an fp32 gradient is grad32 times grad_out)");
+  CNB_REQUIRE(grad32 && grad, CNB_EINVAL, "cnb_focal_splat_grad_ex: null pointer");
+  CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_splat_grad_ex: n=%lld", n);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const long long ctas = (n / 4 + 255) / 256 + 1, cap = (long long)num_sms() * 16;
+  const int grid = (int)(ctas < cap ? ctas : cap);
+  if (grad_dtype == CNB_DTYPE_BF16)
+    k_scale_round<<<grid, 256, 0, stream>>>(grad32, n, grad_out, static_cast<__nv_bfloat16 *>(grad));
+  else
+    k_scale_round<<<grid, 256, 0, stream>>>(grad32, n, grad_out, static_cast<__half *>(grad));
+  CNB_CHECK_LAUNCH("cnb_focal_splat_grad_ex");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_reg_loss_ex(const void *output, int output_dtype, const void *mask, const int64_t *ind, const float *target,
+                    int b, int d, int hw, int m, int mode, float *out2, void *stream_) {
+  CNB_REQUIRE(dtype_code_known(output_dtype), CNB_EINVAL, "cnb_reg_loss_ex: unknown dtype code %d", output_dtype);
+  CNB_REQUIRE(half_code(output_dtype), CNB_EUNSUPPORTED, "cnb_reg_loss_ex: bf16 / fp16 only (fp32: cnb_reg_loss)");
+  CNB_REQUIRE(output && mask && ind && target && out2, CNB_EINVAL, "cnb_reg_loss_ex: null pointer");
+  CNB_REQUIRE(b > 0 && d > 0 && hw > 0 && m > 0, CNB_EINVAL, "cnb_reg_loss_ex: non-positive dimension");
+  CNB_REQUIRE(mode >= 0 && mode <= 3, CNB_EINVAL, "cnb_reg_loss_ex: mode %d", mode);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const float *mask_f = static_cast<const float *>(mask);
+  if (output_dtype == CNB_DTYPE_BF16)
+    k_reg_loss_half<<<1, 1024, 0, stream>>>(static_cast<const __nv_bfloat16 *>(output), mask_f, ind, target, b, d,
+                                            (long long)hw, m, mode, out2);
+  else
+    k_reg_loss_half<<<1, 1024, 0, stream>>>(static_cast<const __half *>(output), mask_f, ind, target, b, d,
+                                            (long long)hw, m, mode, out2);
+  CNB_CHECK_LAUNCH("cnb_reg_loss_ex");
+  count_launch();
+  return CNB_OK;
+}
+
+int cnb_reg_loss_grad_ex(const void *output, int output_dtype, const void *mask, const int64_t *ind,
+                         const float *target, int b, int d, int hw, int m, int mode, const float *loss_den,
+                         const float *grad_out, void *grad_output, void *stream_) {
+  CNB_REQUIRE(dtype_code_known(output_dtype), CNB_EINVAL, "cnb_reg_loss_grad_ex: unknown dtype code %d", output_dtype);
+  CNB_REQUIRE(half_code(output_dtype), CNB_EUNSUPPORTED,
+              "cnb_reg_loss_grad_ex: bf16 / fp16 only (cnb_reg_loss writes the fp32 gradient in its one pass)");
+  CNB_REQUIRE(output && mask && ind && target && loss_den && grad_output, CNB_EINVAL,
+              "cnb_reg_loss_grad_ex: null pointer");
+  CNB_REQUIRE(b > 0 && d > 0 && hw > 0 && m > 0, CNB_EINVAL, "cnb_reg_loss_grad_ex: non-positive dimension");
+  CNB_REQUIRE(mode >= 0 && mode <= 3, CNB_EINVAL, "cnb_reg_loss_grad_ex: mode %d", mode);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const float *mask_f = static_cast<const float *>(mask);
+  if (output_dtype == CNB_DTYPE_BF16)
+    launch_reg_grad_half<__nv_bfloat16>(stream, output, mask_f, ind, target, b, d, hw, m, mode, loss_den, grad_out,
+                                        grad_output);
+  else
+    launch_reg_grad_half<__half>(stream, output, mask_f, ind, target, b, d, hw, m, mode, loss_den, grad_out,
+                                 grad_output);
+  CNB_CHECK_LAUNCH("cnb_reg_loss_grad_ex");
+  count_launch(2);
   return CNB_OK;
 }
 

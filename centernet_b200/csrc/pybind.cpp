@@ -256,6 +256,52 @@ PYBIND11_MODULE(_C, m) {
                        ptr<void>(stream)),
           "cnb_reg_loss");
   });
+  m.def("focal_loss_ex", [](P pred, int dt, P gt, long long n, int logits, P out2, P ws, size_t wsb, P stream) {
+    check(cnb_focal_loss_ex(ptr<const void>(pred), dt, ptr<const float>(gt), n, logits, ptr<float>(out2),
+                            ptr<void>(ws), wsb, ptr<void>(stream)),
+          "cnb_focal_loss_ex");
+  });
+  m.def("focal_grad_ex", [](P pred, int dt, P gt, long long n, int logits, P out2, P gout, P grad, P stream) {
+    check(cnb_focal_grad_ex(ptr<const void>(pred), dt, ptr<const float>(gt), n, logits, ptr<const float>(out2),
+                            ptr<const float>(gout), ptr<void>(grad), ptr<void>(stream)),
+          "cnb_focal_grad_ex");
+  });
+  m.def("focal_splat_loss_ex", [](P pred, int dt, P cls, P cx, P cy, P rad, P valid, int b, int mm, int c, int h,
+                                  int w, int logits, P out2, P grad32, P ws, size_t wsb, P stream) {
+    check(cnb_focal_splat_loss_ex(ptr<const void>(pred), dt, ptr<const int32_t>(cls), ptr<const int32_t>(cx),
+                                  ptr<const int32_t>(cy), ptr<const int32_t>(rad), ptr<const uint8_t>(valid), b, mm,
+                                  c, h, w, logits, ptr<float>(out2), ptr<float>(grad32), ptr<void>(ws), wsb,
+                                  ptr<void>(stream)),
+          "cnb_focal_splat_loss_ex");
+  });
+  m.def("focal_splat_grad_ex", [](P grad32, long long n, P gout, P grad, int dt, P stream) {
+    check(cnb_focal_splat_grad_ex(ptr<const float>(grad32), n, ptr<const float>(gout), ptr<void>(grad), dt,
+                                  ptr<void>(stream)),
+          "cnb_focal_splat_grad_ex");
+  });
+  m.def("reg_loss_ex", [](P output, int dt, P mask, P ind, P target, int b, int d, int hw, int mm, int mode, P out2,
+                          P stream) {
+    check(cnb_reg_loss_ex(ptr<const void>(output), dt, ptr<const void>(mask), ptr<const int64_t>(ind),
+                          ptr<const float>(target), b, d, hw, mm, mode, ptr<float>(out2), ptr<void>(stream)),
+          "cnb_reg_loss_ex");
+  });
+  m.def("reg_loss_grad_ex", [](P output, int dt, P mask, P ind, P target, int b, int d, int hw, int mm, int mode,
+                               P out2, P gout, P grad, P stream) {
+    check(cnb_reg_loss_grad_ex(ptr<const void>(output), dt, ptr<const void>(mask), ptr<const int64_t>(ind),
+                               ptr<const float>(target), b, d, hw, mm, mode, ptr<const float>(out2),
+                               ptr<const float>(gout), ptr<void>(grad), ptr<void>(stream)),
+          "cnb_reg_loss_grad_ex");
+  });
+  m.def("gather_feat_ex", [](P feat, int dt, P ind, P out, int b, int c, int hw, int mm, P stream) {
+    check(cnb_gather_feat_ex(ptr<const void>(feat), dt, ptr<const int64_t>(ind), ptr<float>(out), b, c, hw, mm,
+                             ptr<void>(stream)),
+          "cnb_gather_feat_ex");
+  });
+  m.def("gather_feat_backward_ex", [](P gout, P ind, P gfeat, int dt, int b, int c, int hw, int mm, P stream) {
+    check(cnb_gather_feat_backward_ex(ptr<const float>(gout), ptr<const int64_t>(ind), ptr<void>(gfeat), dt, b, c, hw,
+                                      mm, ptr<void>(stream)),
+          "cnb_gather_feat_backward_ex");
+  });
   m.def("post_transform", [](P rows, P out, P trans, int b, int n, int d, int a0, int na, int b0, int nb, P stream) {
     check(cnb_post_transform(ptr<const float>(rows), ptr<float>(out), ptr<const double>(trans), b, n, d, a0, na, b0, nb,
                              ptr<void>(stream)),

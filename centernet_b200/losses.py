@@ -7,17 +7,36 @@ dense target map is never built on the CPU nor copied to the device.
 
 Each loss is a torch.autograd.Function whose forward runs ONE fused CUDA pass that also
 produces the gradient (saved for backward), i.e. forward+backward read the prediction once.
+
+A bf16 / fp16 prediction (the head of a bf16 backbone, or of one under autocast) is read in place: forward runs
+the loss pass on the half tensor and saves it, backward runs the gradient pass, which reads the incoming gradient
+on the device and writes the gradient in the input's dtype (FocalSplatLoss keeps its unscaled fp32 gradient
+instead and backward scales and rounds it).  Loss and gradient are bit for bit those of the fp32 path on the
+.float() upcast (the gradient rounded once, after the scale); no fp32 copy of the input is made.
 """
 import torch
 from torch import nn
 
-from ._lib import C, f32c, ptr, require_cuda, stream_ptr, workspace
+from ._lib import C, dtype_code, f32c, floatc, ptr, require_cuda, stream_ptr, workspace
+
+_HALF = (torch.bfloat16, torch.float16)
 
 
 class _FocalFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, gt, logits):
         require_cuda(pred, gt, what="FocalLoss")
+        ctx.half = pred.dtype in _HALF
+        if ctx.half:
+            p, g = floatc(pred), f32c(gt)
+            out = torch.empty(2, dtype=torch.float32, device=p.device)
+            ws = workspace(C.focal_workspace_bytes(p.numel()), p.device)
+            C.focal_loss_ex(ptr(p), dtype_code(p), ptr(g), p.numel(), int(logits), ptr(out), ptr(ws), ws.numel(),
+                            stream_ptr(p))
+            if pred.requires_grad:
+                ctx.save_for_backward(p, g, out)
+                ctx.logits = int(logits)
+            return out[0]
         p, g = f32c(pred), f32c(gt)
         out = torch.empty(2, dtype=torch.float32, device=p.device)
         need_grad = pred.requires_grad
@@ -30,6 +49,14 @@ class _FocalFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
+        if ctx.half:
+            if not ctx.needs_input_grad[0]:
+                return None, None, None
+            p, g, out = ctx.saved_tensors
+            grad, go = torch.empty_like(p), f32c(grad_out)
+            C.focal_grad_ex(ptr(p), dtype_code(p), ptr(g), p.numel(), ctx.logits, ptr(out), ptr(go),
+                            ptr(grad), stream_ptr(p))
+            return grad, None, None
         (grad,) = ctx.saved_tensors
         return (grad * grad_out if grad is not None else None), None, None
 
@@ -60,15 +87,23 @@ class _FocalSplatFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, logits):
         require_cuda(pred, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, what="FocalSplatLoss")
-        p = f32c(pred)
+        ctx.half = pred.dtype in _HALF
+        p = floatc(pred) if ctx.half else f32c(pred)
         b, c, h, w = [int(v) for v in p.shape]
         m = int(obj_cls.shape[1])
         i32 = lambda t: t.to(torch.int32).contiguous()
         cls, cx, cy, rad = i32(obj_cls), i32(obj_cx), i32(obj_cy), i32(obj_radius)
         val = obj_valid.to(torch.uint8).contiguous()
         out = torch.empty(2, dtype=torch.float32, device=p.device)
-        grad = torch.empty_like(p) if pred.requires_grad else None
         ws = workspace(C.focal_workspace_bytes(p.numel()), p.device)
+        if ctx.half:   # the unscaled fp32 gradient is kept: rebuilding the target in backward costs more (DESIGN 4.3.1)
+            g32 = torch.empty(p.shape, dtype=torch.float32, device=p.device) if pred.requires_grad else None
+            C.focal_splat_loss_ex(ptr(p), dtype_code(p), ptr(cls), ptr(cx), ptr(cy), ptr(rad), ptr(val), b, m, c, h, w,
+                                  int(logits), ptr(out), ptr(g32), ptr(ws), ws.numel(), stream_ptr(p))
+            ctx.save_for_backward(g32)
+            ctx.dtype = p.dtype
+            return out[0]
+        grad = torch.empty_like(p) if pred.requires_grad else None
         C.focal_splat_loss(ptr(p), ptr(cls), ptr(cx), ptr(cy), ptr(rad), ptr(val), b, m, c, h, w, int(logits), 1.0,
                            ptr(out), ptr(grad), ptr(ws), ws.numel(), stream_ptr(p))
         ctx.save_for_backward(grad)
@@ -76,6 +111,13 @@ class _FocalSplatFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
+        if ctx.half:
+            (g32,) = ctx.saved_tensors
+            if g32 is None or not ctx.needs_input_grad[0]:
+                return (None,) * 7
+            grad, go = torch.empty(g32.shape, dtype=ctx.dtype, device=g32.device), f32c(grad_out)
+            C.focal_splat_grad_ex(ptr(g32), g32.numel(), ptr(go), ptr(grad), dtype_code(grad), stream_ptr(g32))
+            return (grad,) + (None,) * 6
         (grad,) = ctx.saved_tensors
         return (grad * grad_out if grad is not None else None), None, None, None, None, None, None
 
@@ -122,12 +164,20 @@ class _RegFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, output, mask, ind, target, mode):
         require_cuda(output, mask, ind, target, what="RegLoss")
-        o, t = f32c(output), f32c(target)
+        ctx.half = output.dtype in _HALF
+        o, t = (floatc(output) if ctx.half else f32c(output)), f32c(target)
         b, d = int(o.shape[0]), int(o.shape[1])
         hw = int(o.shape[2]) * int(o.shape[3])
         m = int(ind.shape[1])
         msk = f32c(mask)   # mask.float() as in the reference: bool, uint8 and fractional float weights alike
         ind = ind.long().contiguous()
+        if ctx.half:
+            out = torch.empty(2, dtype=torch.float32, device=o.device)   # loss, the gradient's denominator
+            C.reg_loss_ex(ptr(o), dtype_code(o), ptr(msk), ptr(ind), ptr(t), b, d, hw, m, mode, ptr(out), stream_ptr(o))
+            if output.requires_grad:
+                ctx.save_for_backward(o, msk, ind, t, out)
+                ctx.mode = mode
+            return out[0]
         out = torch.empty(1, dtype=torch.float32, device=o.device)
         grad = torch.zeros_like(o) if output.requires_grad else None
         C.reg_loss(ptr(o), ptr(msk), ptr(ind), ptr(t), b, d, hw, m, mode, 1.0, ptr(out), ptr(grad), stream_ptr(o))
@@ -136,6 +186,15 @@ class _RegFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
+        if ctx.half:
+            if not ctx.needs_input_grad[0]:
+                return (None,) * 5
+            o, msk, ind, t, out = ctx.saved_tensors
+            grad, go = torch.empty_like(o), f32c(grad_out)   # the call fills all of grad
+            C.reg_loss_grad_ex(ptr(o), dtype_code(o), ptr(msk), ptr(ind), ptr(t), int(o.shape[0]), int(o.shape[1]),
+                               int(o.shape[2]) * int(o.shape[3]), int(ind.shape[1]), ctx.mode, ptr(out),
+                               ptr(go), ptr(grad), stream_ptr(o))
+            return (grad,) + (None,) * 4
         (grad,) = ctx.saved_tensors
         return (grad * grad_out if grad is not None else None), None, None, None, None
 

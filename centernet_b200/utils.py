@@ -1,7 +1,7 @@
 """Mirror of src/lib/models/utils.py (reference lines cited per function)."""
 import torch
 
-from ._lib import C, f32c, ptr, require_cuda, stream_ptr
+from ._lib import C, dtype_code, f32c, floatc, ptr, require_cuda, stream_ptr
 
 
 def _sigmoid(x):
@@ -24,16 +24,21 @@ def _gather_feat(feat, ind, mask=None):
 class _TransposeGather(torch.autograd.Function):
     """Differentiable like the reference's permute + gather: the losses of models/losses.py
     (RegL1Loss, RegLoss, NormRegL1Loss, RegWeightedL1Loss, L1Loss, BinRotLoss) back-propagate
-    through `pred = _transpose_and_gather_feat(output, ind)`."""
+    through `pred = _transpose_and_gather_feat(output, ind)`.  A bf16 / fp16 feat is read in place (the rows
+    come out in fp32, as for any dtype) and its gradient is written in its dtype: the fp32 scatter of the upcast
+    rounded once, with no fp32 map in between."""
 
     @staticmethod
     def forward(ctx, feat, ind):
-        f = f32c(feat)
+        half = feat.dtype in (torch.bfloat16, torch.float16)
+        f = floatc(feat) if half else f32c(feat)
         ind = ind.contiguous().long()
         B, Cc, H, W = f.shape
         M = ind.shape[1]
         out = torch.empty((B, M, Cc), dtype=torch.float32, device=f.device)
-        if B * M * Cc:
+        if B * M * Cc and half:
+            C.gather_feat_ex(ptr(f), dtype_code(f), ptr(ind), ptr(out), B, Cc, H * W, M, stream_ptr(f))
+        elif B * M * Cc:
             C.gather_feat(ptr(f), ptr(ind), ptr(out), B, Cc, H * W, M, stream_ptr(f))
         ctx.save_for_backward(ind)
         ctx.shape = (B, Cc, H, W)
@@ -45,8 +50,15 @@ class _TransposeGather(torch.autograd.Function):
         (ind,) = ctx.saved_tensors
         B, Cc, H, W = ctx.shape
         g = f32c(grad_out)
-        grad_feat = torch.zeros((B, Cc, H, W), dtype=torch.float32, device=g.device)
         M = ind.shape[1]
+        if ctx.in_dtype in (torch.bfloat16, torch.float16):
+            if B * M * Cc == 0:
+                return torch.zeros((B, Cc, H, W), dtype=ctx.in_dtype, device=g.device), None
+            grad_feat = torch.empty((B, Cc, H, W), dtype=ctx.in_dtype, device=g.device)   # the call zero-fills it
+            C.gather_feat_backward_ex(ptr(g), ptr(ind), ptr(grad_feat), dtype_code(grad_feat), B, Cc, H * W, M,
+                                      stream_ptr(g))
+            return grad_feat, None
+        grad_feat = torch.zeros((B, Cc, H, W), dtype=torch.float32, device=g.device)
         if B * M * Cc:
             C.gather_feat_backward(ptr(g), ptr(ind), ptr(grad_feat), B, Cc, H * W, M, stream_ptr(g))
         return grad_feat.to(ctx.in_dtype), None

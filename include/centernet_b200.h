@@ -43,7 +43,8 @@ extern "C" {
 #define CNB_EWORKSPACE 4   /* workspace_bytes smaller than cnb_*_workspace_bytes */
 
 /* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16, cnb_ctdet_decode_ex,
- * cnb_flip_merge_ex, cnb_ddd_decode_ex, cnb_multi_pose_decode_ex, cnb_edge_aggregate_ex, cnb_exct_decode_ex). */
+ * cnb_flip_merge_ex, cnb_ddd_decode_ex, cnb_multi_pose_decode_ex, cnb_edge_aggregate_ex, cnb_exct_decode_ex,
+ * cnb_gather_feat_ex and the loss calls cnb_focal_*_ex / cnb_reg_loss_*ex). */
 #define CNB_DTYPE_F32 0
 #define CNB_DTYPE_BF16 1
 #define CNB_DTYPE_F16 2
@@ -94,6 +95,17 @@ int cnb_gather_feat(const float *feat, const int64_t *ind, float *out,
  * zero-filled; repeated indices accumulate. */
 int cnb_gather_feat_backward(const float *grad_out, const int64_t *ind, float *grad_feat,
                              int b, int c, int hw, int m, void *stream);
+/* The same pair for a feat of feat_dtype (CNB_DTYPE_F32 / _BF16 / _F16), read and written in place: no fp32 copy
+ * of the map is made.  out stays fp32 [b, m, c] and equals cnb_gather_feat of the .float() upcast (both formats
+ * widen exactly).  cnb_gather_feat_backward_ex zero-fills grad_feat ([b, c, hw] of feat_dtype) itself and leaves
+ * in it, bit for bit, cnb_gather_feat_backward's fp32 map rounded once to feat_dtype: the rows of a repeated
+ * index are added in fp32 in ascending m and only the sum is rounded; nothing is accumulated in the half map and
+ * there are no atomics, so it is bit-identical run to run.  Indices outside [0, hw) are skipped.  Errors, checked
+ * before any CUDA call: CNB_EINVAL for an unknown dtype code, a null pointer or a bad shape. */
+int cnb_gather_feat_ex(const void *feat, int feat_dtype, const int64_t *ind, float *out,
+                       int b, int c, int hw, int m, void *stream);
+int cnb_gather_feat_backward_ex(const float *grad_out, const int64_t *ind, void *grad_feat, int feat_dtype,
+                                int b, int c, int hw, int m, void *stream);
 
 /* ---------------------------------------------------------- A5: ctdet_decode
  * models/decode.py:464-495.  heat [b,c,h,w] (post-sigmoid), wh [b,2,h,w] (or
@@ -304,6 +316,51 @@ int cnb_focal_splat_loss(const float *pred, const int32_t *obj_cls, const int32_
 int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, const float *target,
                  int b, int d, int hw, int m, int mode, float grad_scale,
                  float *out1, float *grad_output, void *stream);
+
+/* ------------------------------------- the losses on bf16 / fp16 heads, read in place
+ * For a pred / output of dtype code CNB_DTYPE_BF16 or CNB_DTYPE_F16 (gt, mask, target, ind and the object lists
+ * as in the fp32 calls above).  No fp32 copy of the map is made.  Contract, with the fp32 call on the .float()
+ * upcast as the oracle (the reference evaluated ON half tensors -- log, pow and the sums in bf16 -- is not the
+ * target):
+ *   1. the loss (and num_pos) are bit for bit what the fp32 call returns for the upcast: both formats widen to
+ *      fp32 exactly, and the grid, the elements of each thread, the partials and their order are the fp32 call's;
+ *   2. the gradient is bit for bit (g32 * *grad_out) rounded once (to nearest even) to the input's dtype, g32
+ *      being the fp32 call's gradient for the upcast with grad_scale = 1: what autograd hands back today for a
+ *      half input, for any grad_out (loss weights, AMP scales, 0, negative).  An fp16 overflow becomes inf;
+ *   3. the contributions of a repeated ind entry are added in fp32 in ascending m, then scaled, then rounded:
+ *      never accumulated in the half map;
+ *   4. no atomics on floats: bit-identical run to run.
+ * grad_out is only known in backward and must be read on the device, so each loss is two calls:
+ *   cnb_*_loss_ex  forward: out2[0] = loss; out2[1] = num_pos (focal) or the fp32 denominator mask sum + 1e-4
+ *                  (Reg*Loss).  Same workspace as the fp32 call (cnb_focal_workspace_bytes).
+ *   cnb_*_grad_ex  backward: multiplies the gradient by *grad_out (device pointer to one fp32 value; NULL means
+ *                  1.0) and writes it in the input's dtype.  cnb_focal_grad_ex and cnb_reg_loss_grad_ex read the
+ *                  input again and out2 as the forward left it (device pointer) and evaluate the gradient with
+ *                  the forward's arithmetic: no temporary.  cnb_reg_loss_grad_ex fills the whole grad_output map
+ *                  itself (elements no index selects get 0 * *grad_out, as in the fp32 path).  The fused splat is
+ *                  bound by instruction issue, not by bytes, and evaluating it twice is the slower choice there:
+ *                  cnb_focal_splat_loss_ex also stores the unscaled fp32 gradient in grad32 ([b,c,h,w]; NULL when
+ *                  no gradient is wanted) and cnb_focal_splat_grad_ex is the scale-and-round pass over those n
+ *                  values.
+ * CNB_DTYPE_F32: cnb_focal_loss_ex is cnb_focal_loss without a gradient and cnb_focal_splat_loss_ex is
+ * cnb_focal_splat_loss with grad_scale = 1; the other four return CNB_EUNSUPPORTED.  Errors, checked before any
+ * CUDA call: CNB_EINVAL for an unknown dtype code, a null pointer or a bad shape, CNB_EUNSUPPORTED for m > 128
+ * object lists, CNB_EWORKSPACE for too small a workspace. */
+int cnb_focal_loss_ex(const void *pred, int pred_dtype, const float *gt, long long n, int logits, float *out2,
+                      void *workspace, size_t workspace_bytes, void *stream);
+int cnb_focal_grad_ex(const void *pred, int pred_dtype, const float *gt, long long n, int logits,
+                      const float *loss_num_pos, const float *grad_out, void *grad, void *stream);
+int cnb_focal_splat_loss_ex(const void *pred, int pred_dtype, const int32_t *obj_cls, const int32_t *obj_cx,
+                            const int32_t *obj_cy, const int32_t *obj_radius, const uint8_t *obj_valid,
+                            int b, int m, int c, int h, int w, int logits, float *out2, float *grad32,
+                            void *workspace, size_t workspace_bytes, void *stream);
+int cnb_focal_splat_grad_ex(const float *grad32, long long n, const float *grad_out, void *grad, int grad_dtype,
+                            void *stream);
+int cnb_reg_loss_ex(const void *output, int output_dtype, const void *mask, const int64_t *ind,
+                    const float *target, int b, int d, int hw, int m, int mode, float *out2, void *stream);
+int cnb_reg_loss_grad_ex(const void *output, int output_dtype, const void *mask, const int64_t *ind,
+                         const float *target, int b, int d, int hw, int m, int mode, const float *loss_den,
+                         const float *grad_out, void *grad_output, void *stream);
 
 /* ---------------------------------------------------------- A10/A11: DCNv2
  * Replaces dcn_v2_cuda_forward / dcn_v2_cuda_backward
