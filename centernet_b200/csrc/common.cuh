@@ -1,6 +1,8 @@
 // Shared device/host helpers for the centernet_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <stddef.h>
 #include <stdio.h>
@@ -52,6 +54,7 @@ inline int num_sms() {
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
   return n > 0 ? n : 132;
 }
+inline bool dtype_known(int dt) { return dt == CNB_DTYPE_F32 || dt == CNB_DTYPE_F16 || dt == CNB_DTYPE_BF16; }
 
 // ---------------------------------------------------------------- device side
 #ifdef __CUDACC__
@@ -99,6 +102,11 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
       : "memory");
 }
 __device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
+// Exact widening of one map / head element to fp32 (every fp16 and bf16 value, subnormals and infinities included,
+// is a float: the result equals torch's .float()).
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
 
 #define CNB_NEG_INF (__int_as_float(0xff800000))
 

@@ -57,8 +57,10 @@ __global__ void __launch_bounds__(256) k_nms(const float *__restrict__ heat, flo
 }
 
 // ------------------------------------------------------------------ A4: gather
-// out[b, m, ch] = feat[b, ch, ind[b, m]]   (models/utils.py:12-26 without the transpose copy)
-__global__ void __launch_bounds__(256) k_gather_feat(const float *__restrict__ feat,
+// out[b, m, ch] = feat[b, ch, ind[b, m]]   (models/utils.py:12-26 without the transpose copy).  A bf16 / fp16 feat is
+// read in place: each value widens exactly, so out is the gather of the upcast.
+template <typename T>
+__global__ void __launch_bounds__(256) k_gather_feat(const T *__restrict__ feat,
                                                      const int64_t *__restrict__ ind, float *__restrict__ out,
                                                      int B, int C, long long HW, int M) {
   const long long total = (long long)B * M * C;
@@ -69,7 +71,7 @@ __global__ void __launch_bounds__(256) k_gather_feat(const float *__restrict__ f
     const int b = (int)(bm / M);
     const long long sp = ind[bm];
     float v = 0.0f;
-    if (sp >= 0 && sp < HW) v = __ldg(feat + ((long long)b * C + ch) * HW + sp);
+    if (sp >= 0 && sp < HW) v = to_f32(__ldg(feat + ((long long)b * C + ch) * HW + sp));
     out[i] = v;
   }
 }
@@ -93,24 +95,7 @@ __global__ void __launch_bounds__(256) k_gather_feat_bwd(const float *__restrict
   }
 }
 
-// The gather of a bf16 / fp16 feat read in place: each value widens exactly, so out is the gather of the upcast.
-template <typename T>
-__global__ void __launch_bounds__(256) k_gather_feat_half(const T *__restrict__ feat, const int64_t *__restrict__ ind,
-                                                          float *__restrict__ out, int B, int C, long long HW, int M) {
-  const long long total = (long long)B * M * C;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int ch = (int)(i % C);
-    const long long bm = i / C;
-    const int b = (int)(bm / M);
-    const long long sp = ind[bm];
-    float v = 0.0f;
-    if (sp >= 0 && sp < HW) v = (float)__ldg(feat + ((long long)b * C + ch) * HW + sp);
-    out[i] = v;
-  }
-}
-
-// Its adjoint into a zero-filled bf16 / fp16 grad_feat.  One thread per (image, m, channel); the thread of the first
+// The adjoint of the gather into a zero-filled bf16 / fp16 grad_feat.  One thread per (image, m, channel); the thread of the first
 // m that holds a map index is that element's only writer: it adds the rows of every m with the same index in fp32 in
 // ascending m, starting from the map's 0 as k_gather_feat_bwd does, and rounds the sum once.
 template <typename T>
@@ -445,11 +430,11 @@ int cnb_gather_feat_ex(const void *feat, int feat_dtype, const int64_t *ind, flo
   const long long total = (long long)b * m * c;
   const int grid = (int)((total + 255) / 256 < 65535 ? (total + 255) / 256 : 65535);
   if (feat_dtype == CNB_DTYPE_BF16)
-    k_gather_feat_half<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16 *>(feat), ind, out,
-                                                               b, c, hw, m);
+    k_gather_feat<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16 *>(feat), ind, out, b, c,
+                                                          hw, m);
   else
-    k_gather_feat_half<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half *>(feat), ind, out, b, c,
-                                                               hw, m);
+    k_gather_feat<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half *>(feat), ind, out, b, c, hw,
+                                                          m);
   CNB_CHECK_LAUNCH("cnb_gather_feat_ex");
   count_launch();
   return CNB_OK;

@@ -12,9 +12,13 @@
 // dense target map of the reference (built on the CPU, copied H2D, read by ~12 ATen kernels)
 // is never materialised.  num_pos -- needed to normalise the gradient in the same pass -- is
 // known up front from the object lists (one positive per distinct valid centre inside the map).
+//
+// pred may be fp32, bf16 or fp16; each loss has one kernel body, templated on pred's type T.  Both half formats widen
+// to fp32 exactly (to_f32) and everything after the load is the fp32 arithmetic, with the same grid, elements per
+// thread, (e0 + e1) + (e2 + e3) groups and partials, so a half pred gives bit for bit the loss of the T = float
+// instance on its .float() upcast.
 #include <stdlib.h>
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
+#include <type_traits>
 #include "common.cuh"
 
 namespace cnb {
@@ -270,43 +274,107 @@ __global__ void __launch_bounds__(128) k_count_pos_objects(const int32_t *cls, c
   if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&acc->num_pos, (double)cnt);
 }
 
-// ---- main pass, dense target
-template <bool LOGITS>
-__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense(const float *__restrict__ pred,
+template <typename T> __device__ __forceinline__ T narrow(float v);   // round to nearest even; fp16 overflows to inf
+template <> __device__ __forceinline__ float narrow<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 narrow<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ __half narrow<__half>(float v) { return __float2half_rn(v); }
+
+template <typename T> union Pack4 { uint2 u; T t[4]; };
+// Elements 4i .. 4i+3 of p.  bf16 / fp16: one 8-byte access when p is 8-byte aligned (al8), else four 2-byte ones.
+// fp32: one 16-byte access, al8 unused (the fp32 kernels group by four only when p is 16-byte aligned).
+template <typename T>
+__device__ __forceinline__ float4 load4(const T *p, long long i, bool al8) {
+  Pack4<T> r;
+  p += 4 * i;
+  if (al8) {
+    r.u = __ldg(reinterpret_cast<const uint2 *>(p));
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) r.t[j] = __ldg(p + j);
+  }
+  return make_float4(to_f32(r.t[0]), to_f32(r.t[1]), to_f32(r.t[2]), to_f32(r.t[3]));
+}
+template <> __device__ __forceinline__ float4 load4<float>(const float *p, long long i, bool) {
+  return __ldg(reinterpret_cast<const float4 *>(p) + i);
+}
+template <typename T>
+__device__ __forceinline__ void store4(T *p, long long i, bool al8, float a, float b, float c, float d) {
+  Pack4<T> r;
+  r.t[0] = narrow<T>(a); r.t[1] = narrow<T>(b); r.t[2] = narrow<T>(c); r.t[3] = narrow<T>(d);
+  p += 4 * i;
+  if (al8) {
+    *reinterpret_cast<uint2 *>(p) = r.u;
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) p[j] = r.t[j];
+  }
+}
+template <> __device__ __forceinline__ void store4<float>(float *p, long long i, bool, float a, float b, float c,
+                                                          float d) {
+  reinterpret_cast<float4 *>(p)[i] = make_float4(a, b, c, d);
+}
+__device__ __forceinline__ float incoming_grad(const float *grad_out) { return grad_out ? __ldg(grad_out) : 1.0f; }
+
+// ---- main pass, dense target.  One body, three uses:
+//   fp32 forward  (T = float, BWD = false): the loss, and the gradient, scaled by grad_scale, into grad (nullable);
+//   half forward  (BWD = false, grad_scale = 1, grad null): the loss only;
+//   half backward (BWD = true, acc null): out2 holds the forward's (loss, num_pos); stores T(grad * *grad_out).
+// A half gradient cannot be finished in the forward pass as the fp32 one is: it has to be rounded to T once, AFTER
+// the scale by the loss's incoming gradient, which only backward knows.  So backward evaluates focal_elem again, and
+// __fmul_rn keeps that product out of any contraction with focal_elem's last multiply.
+template <typename T, bool LOGITS, bool BWD>
+__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense(const T *__restrict__ pred,
                                                                const float *__restrict__ gt, long long n,
-                                                               float grad_scale, float *__restrict__ grad,
-                                                               FocalAcc *acc, float *out2) {
-  const double np_ = acc->num_pos;  // written by pass 0 (previous kernel on the stream)
+                                                               float grad_scale, T *__restrict__ grad,
+                                                               FocalAcc *acc, float *out2,
+                                                               const float *__restrict__ grad_out) {
+  // num_pos: written by pass 0 (previous kernel on the stream), or in backward by the forward
+  const double np_ = BWD ? (double)out2[1] : acc->num_pos;
   const float inv_norm = grad_scale / (np_ > 0.0 ? (float)np_ : 1.0f);
   const bool pos_live = np_ > 0.0;
+  constexpr bool F32 = std::is_same<T, float>::value;
+  constexpr bool STORE = F32 || BWD;   // a half forward computes no gradient
+  const float go = BWD ? incoming_grad(grad_out) : 1.0f;
+  auto scaled = [go](float g) { return BWD ? __fmul_rn(g, go) : g; };
   double pos = 0, neg = 0;
   const long long n4 = n >> 2;
-  const bool vec = ((((uintptr_t)pred | (uintptr_t)gt | (uintptr_t)grad) & 15u) == 0);
-  if (vec) {
+  // fp32 groups by four when pred, gt and grad are 16-byte aligned.  A half pred groups as the fp32 kernel does on
+  // its .float() upcast and that gradient, fresh allocations: by gt's alignment alone.
+  const bool group4 = F32 ? ((((uintptr_t)pred | (uintptr_t)gt | (uintptr_t)grad) & 15u) == 0)
+                          : (((uintptr_t)gt & 15u) == 0);
+  const bool al8 = ((((uintptr_t)pred | (uintptr_t)grad) & 7u) == 0);
+  if (group4) {
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4;
          i += (long long)gridDim.x * blockDim.x) {
-      const float4 p = __ldg(reinterpret_cast<const float4 *>(pred) + i);
+      const float4 p = load4<T>(pred, i, al8);
       const float4 g = __ldg(reinterpret_cast<const float4 *>(gt) + i);
       const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
       const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
-      pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
-      neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
-      if (grad) reinterpret_cast<float4 *>(grad)[i] = make_float4(e0.grad, e1.grad, e2.grad, e3.grad);
+      if (!BWD) {
+        pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
+        neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
+      }
+      if (STORE && grad) store4<T>(grad, i, al8, scaled(e0.grad), scaled(e1.grad), scaled(e2.grad), scaled(e3.grad));
     }
   }
-  for (long long i = (vec ? (n4 << 2) : 0) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+  for (long long i = (group4 ? (n4 << 2) : 0) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
-    const Elem e = focal_elem<LOGITS>(pred[i], gt[i], inv_norm, pos_live);
-    pos += e.loss_pos; neg += e.loss_neg;
-    if (grad) grad[i] = e.grad;
+    const Elem e = focal_elem<LOGITS>(to_f32(pred[i]), gt[i], inv_norm, pos_live);
+    if (!BWD) { pos += e.loss_pos; neg += e.loss_neg; }
+    if (STORE && grad) grad[i] = narrow<T>(scaled(e.grad));
   }
-  block_accumulate(pos, neg, acc);
-  finish_loss(acc, gridDim.x, out2);
+  if (!BWD) {
+    block_accumulate(pos, neg, acc);
+    finish_loss(acc, gridDim.x, out2);
+  }
 }
 
-// ---- main pass, target rebuilt from object lists: one CTA per (image, class) plane
-template <bool LOGITS, bool WRITE_HM>
-__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__restrict__ pred, const int32_t *cls,
+// ---- main pass, target rebuilt from object lists: one CTA per (image, class) plane.  The gradient is stored in fp32,
+// scaled by grad_scale, into grad (nullable).  With a half pred (grad_scale = 1) that is the unscaled fp32 gradient
+// k_scale_round turns into T: this kernel is issue-bound, and evaluating the tables and focal_elem a second time in
+// backward measured slower than storing the gradient (DESIGN 4.3.1).  WRITE_HM (T = float): only the target, to hm.
+template <typename T, bool LOGITS, bool WRITE_HM>
+__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const T *__restrict__ pred, const int32_t *cls,
                                                                const int32_t *cx, const int32_t *cy,
                                                                const int32_t *rad, const uint8_t *valid, int M, int C,
                                                                int H, int W, float grad_scale,
@@ -327,6 +395,11 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
   }
   double pos = 0, neg = 0;
   const int n_items = B * C * parts;
+  // Groups of four need W % 4 == 0; fp32 also needs pred, grad and hm 16-byte aligned.  A half pred groups as the
+  // fp32 kernel does on its .float() upcast and that gradient, fresh allocations: whenever W % 4 == 0 (its plane bases
+  // are then 8-byte multiples).  A half pred's fp32 gradient group is one 16-byte store when grad is so aligned.
+  constexpr bool F32 = std::is_same<T, float>::value;
+  const bool al8 = (((uintptr_t)pred & 7u) == 0), g_al16 = F32 || (((uintptr_t)grad & 15u) == 0);
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
   __syncthreads();   // the previous item's objects and tables are no longer read
   const int plane = item / parts, part = item - plane * parts;
@@ -335,7 +408,7 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
   const int nobj = gather_objects(cls, cx, cy, rad, valid, b, M, c, H, W, s_obj, &s_n, y_lo, y_hi);
   if (nobj) build_tables(s_obj, nobj, s_tab, s_gauss, &s_total);
   const long long base = (long long)plane * H * W;
-  const bool vec = (W % 4 == 0) && ((((uintptr_t)pred | (uintptr_t)grad | (uintptr_t)hm) & 15u) == 0);
+  const bool vec = (W % 4 == 0) && (!F32 || ((((uintptr_t)pred | (uintptr_t)grad | (uintptr_t)hm) & 15u) == 0));
   if (vec) {
     // (x, y) of the thread's float4 advance incrementally: no division in the loop (the kernel is issue-bound)
     const int w4 = W / 4;
@@ -348,12 +421,17 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
       if (WRITE_HM) {
         reinterpret_cast<float4 *>(hm + base)[i] = g;
       } else {
-        const float4 p = __ldg(reinterpret_cast<const float4 *>(pred + base) + i);
+        const float4 p = load4<T>(pred + base, i, al8);
         const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
         const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
         pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
         neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
-        if (grad) reinterpret_cast<float4 *>(grad + base)[i] = make_float4(e0.grad, e1.grad, e2.grad, e3.grad);
+        if (grad && g_al16) {
+          reinterpret_cast<float4 *>(grad + base)[i] = make_float4(e0.grad, e1.grad, e2.grad, e3.grad);
+        } else if (grad) {
+          float *gp = grad + base + 4ll * i;
+          gp[0] = e0.grad; gp[1] = e1.grad; gp[2] = e2.grad; gp[3] = e3.grad;
+        }
       }
     }
   } else {
@@ -363,7 +441,7 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
       if (WRITE_HM) {
         hm[base + i] = g;
       } else {
-        const Elem e = focal_elem<LOGITS>(pred[base + i], g, inv_norm, pos_live);
+        const Elem e = focal_elem<LOGITS>(to_f32(pred[base + i]), g, inv_norm, pos_live);
         pos += e.loss_pos; neg += e.loss_neg;
         if (grad) grad[base + i] = e.grad;
       }
@@ -377,47 +455,66 @@ __global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat(const float *__re
 }
 
 // ---- Reg*Loss: B*M*D is tiny (e.g. 64*128*2); one CTA does sums, loss and the scatter of the gradient.
-__global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ output, const float *mask_f,
+// One (image, object, channel) element i and its offset `at` in the output map: false when its index is outside the
+// map (torch's gather raises on such an index; never read or write outside the map).
+template <typename T>
+__device__ __forceinline__ bool reg_elem(const T *__restrict__ output, const float *mask_f,
+                                         const int64_t *__restrict__ ind, const float *__restrict__ target, int D,
+                                         long long HW, int M, int mode, long long i, float *diff, float *m,
+                                         float *scale, long long *at) {
+  const int d = (int)(i % D);
+  const long long bm = i / D;
+  const int b = (int)(bm / M);
+  const long long sp = ind[bm];
+  if (sp < 0 || sp >= HW) return false;
+  *m = mask_f[(mode == 3) ? i : bm];   // mask.float(): fractional weights stay fractional
+  *at = ((long long)b * D + d) * HW + sp;
+  float pred = to_f32(output[*at]);
+  float tgt = target[i];
+  *scale = 1.0f;
+  if (mode == 2) {  // NormRegL1Loss: pred / (target + 1e-4) against 1
+    *scale = 1.0f / (tgt + 1e-4f);
+    pred = pred / (tgt + 1e-4f);
+    tgt = tgt * 0.0f + 1.0f;
+  }
+  *diff = pred * *m - tgt * *m;
+  return true;
+}
+
+// out[0] = the loss.  A half output (read at the gathered positions only) also gets out[1] = (float)(mask sum + 1e-4),
+// the denominator k_reg_grad_half divides its gradient by; an fp32 output gets its gradient here instead (grad_output,
+// nullable), which half leaves null.
+template <typename T>
+__global__ void __launch_bounds__(1024) k_reg_loss(const T *__restrict__ output, const float *mask_f,
                                                    const int64_t *__restrict__ ind, const float *__restrict__ target,
                                                    int B, int D, long long HW, int M, int mode, float grad_scale,
-                                                   float *out1, float *grad_output) {
+                                                   float *out, float *grad_output) {
+  constexpr bool F32 = std::is_same<T, float>::value;
   __shared__ double red[2][32];
   __shared__ double s_tot[2];
   const long long n = (long long)B * M * D;
   double loss = 0, msum = 0;
   // pass 0: the sums (strided per thread, fixed tree); pass 1: the gradient, one thread per (image, channel) plane
   // walking m in ascending order, so repeated indices add up in a fixed order without atomics
-  for (int pass = 0; pass < 2; ++pass) {
+  for (int pass = 0; pass < (F32 ? 2 : 1); ++pass) {
     const double denom = pass ? (s_tot[1] + 1e-4) : 1.0;
     const long long n_it = pass ? (long long)B * D : n;
     for (long long it = threadIdx.x; it < n_it; it += blockDim.x) {
       if (pass && !grad_output) break;
       for (int mm = 0; mm < (pass ? M : 1); ++mm) {
         const long long i = pass ? ((it / D) * M + mm) * D + it % D : it;
-        const int d = (int)(i % D);
-        const long long bm = i / D;
-        const int b = (int)(bm / M);
-        const long long sp = ind[bm];
-        if (sp < 0 || sp >= HW) continue;   // torch's gather raises on such an index; never read or write outside the map
-        const float m = mask_f[(mode == 3) ? i : bm];   // mask.float(): fractional weights stay fractional
-        float pred = output[((long long)b * D + d) * HW + sp];
-        float tgt = target[i];
-        float scale = 1.0f;
-        if (mode == 2) {  // NormRegL1Loss: pred / (target + 1e-4) against 1
-          scale = 1.0f / (tgt + 1e-4f);
-          pred = pred / (tgt + 1e-4f);
-          tgt = tgt * 0.0f + 1.0f;
-        }
-        const float diff = pred * m - tgt * m;
+        float diff, m, scale;
+        long long at;
+        if (!reg_elem<T>(output, mask_f, ind, target, D, HW, M, mode, i, &diff, &m, &scale, &at)) continue;
         if (pass == 0) {
           const float ad = fabsf(diff);
           loss += (mode == 1) ? (ad < 1.0f ? 0.5 * (double)ad * ad : (double)ad - 0.5) : (double)ad;
-          msum += (mode == 1) ? ((d == 0) ? (double)m : 0.0) : (double)m;  // RegLoss divides by mask.sum() un-expanded
+          msum += (mode == 1) ? (((int)(i % D) == 0) ? (double)m : 0.0) : (double)m;  // RegLoss divides by mask.sum() un-expanded
         } else {
           float g = (diff > 0.0f) ? 1.0f : (diff < 0.0f ? -1.0f : 0.0f);
           if (mode == 1 && fabsf(diff) < 1.0f) g = diff;
           g = g * m * scale * grad_scale / (float)denom;
-          if (g != 0.0f) grad_output[((long long)b * D + d) * HW + sp] += g;
+          if (g != 0.0f) grad_output[at] += g;
         }
       }
     }
@@ -432,163 +529,15 @@ __global__ void __launch_bounds__(1024) k_reg_loss(const float *__restrict__ out
         double a = 0, c = 0;
         for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { a += red[0][i]; c += red[1][i]; }
         s_tot[0] = a; s_tot[1] = c;
-        out1[0] = (float)(a / (c + 1e-4));
+        out[0] = (float)(a / (c + 1e-4));
+        if (!F32) out[1] = (float)(c + 1e-4);
       }
       __syncthreads();
     }
   }
 }
 
-// ------------------------------------------------------------------ bf16 / fp16 pred, read in place
-// Both formats widen to fp32 exactly and everything after the load is the fp32 arithmetic above, so the loss is
-// bit for bit the loss of the fp32 kernels on the .float() upcast: same grid, same elements per thread, same
-// (e0 + e1) + (e2 + e3) groups, same partials.  The gradient cannot be finished in the forward pass as the fp32
-// kernels do: it has to be rounded to T once, AFTER the scale by the loss's incoming gradient, which only backward
-// knows.  For the dense loss the same kernel body runs twice: BWD = false adds the loss, BWD = true evaluates
-// focal_elem again and stores T(grad * *grad_out).  __fmul_rn keeps that product out of any contraction with
-// focal_elem's last multiply.
-template <typename T> __device__ __forceinline__ float widen(T v);
-template <> __device__ __forceinline__ float widen<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-template <> __device__ __forceinline__ float widen<__half>(__half v) { return __half2float(v); }
-template <typename T> __device__ __forceinline__ T narrow(float v);   // round to nearest even; fp16 overflows to inf
-template <> __device__ __forceinline__ __nv_bfloat16 narrow<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-template <> __device__ __forceinline__ __half narrow<__half>(float v) { return __float2half_rn(v); }
-
-template <typename T> union Pack4 { uint2 u; T t[4]; };
-// 4 consecutive elements: one 8-byte access when p is 8-byte aligned (al8), else four 2-byte ones
-template <typename T>
-__device__ __forceinline__ float4 load4(const T *p, bool al8) {
-  Pack4<T> r;
-  if (al8) {
-    r.u = __ldg(reinterpret_cast<const uint2 *>(p));
-  } else {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) r.t[j] = __ldg(p + j);
-  }
-  return make_float4(widen<T>(r.t[0]), widen<T>(r.t[1]), widen<T>(r.t[2]), widen<T>(r.t[3]));
-}
-template <typename T>
-__device__ __forceinline__ void store4(T *p, bool al8, float a, float b, float c, float d) {
-  Pack4<T> r;
-  r.t[0] = narrow<T>(a); r.t[1] = narrow<T>(b); r.t[2] = narrow<T>(c); r.t[3] = narrow<T>(d);
-  if (al8) {
-    *reinterpret_cast<uint2 *>(p) = r.u;
-  } else {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) p[j] = r.t[j];
-  }
-}
-__device__ __forceinline__ float incoming_grad(const float *grad_out) { return grad_out ? __ldg(grad_out) : 1.0f; }
-
-// Dense target.  The fp32 kernel takes its float4 path when pred, gt and grad are 16-byte aligned; a .float() upcast
-// and its gradient are fresh allocations, so on the upcast that is decided by gt alone, and so is the grouping here.
-// BWD = false: acc holds num_pos (pass 0), the loss goes to out2.  BWD = true: out2 is the forward's result.
-template <typename T, bool LOGITS, bool BWD>
-__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_dense_half(const T *__restrict__ pred,
-                                                                    const float *__restrict__ gt, long long n,
-                                                                    FocalAcc *acc, float *out2,
-                                                                    const float *__restrict__ grad_out,
-                                                                    T *__restrict__ grad) {
-  const float np_ = BWD ? out2[1] : (float)acc->num_pos;
-  const float inv_norm = 1.0f / (np_ > 0.0f ? np_ : 1.0f);
-  const bool pos_live = np_ > 0.0f;
-  const float go = BWD ? incoming_grad(grad_out) : 0.0f;
-  double pos = 0, neg = 0;
-  const long long n4 = n >> 2;
-  const bool group4 = (((uintptr_t)gt & 15u) == 0);
-  const bool al8 = ((((uintptr_t)pred | (uintptr_t)grad) & 7u) == 0);
-  if (group4) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4;
-         i += (long long)gridDim.x * blockDim.x) {
-      const float4 p = load4<T>(pred + 4 * i, al8);
-      const float4 g = __ldg(reinterpret_cast<const float4 *>(gt) + i);
-      const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
-      const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
-      if (BWD) {
-        store4<T>(grad + 4 * i, al8, __fmul_rn(e0.grad, go), __fmul_rn(e1.grad, go), __fmul_rn(e2.grad, go),
-                  __fmul_rn(e3.grad, go));
-      } else {
-        pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
-        neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
-      }
-    }
-  }
-  for (long long i = (group4 ? (n4 << 2) : 0) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
-       i += (long long)gridDim.x * blockDim.x) {
-    const Elem e = focal_elem<LOGITS>(widen<T>(pred[i]), gt[i], inv_norm, pos_live);
-    if (BWD) grad[i] = narrow<T>(__fmul_rn(e.grad, go));
-    else { pos += e.loss_pos; neg += e.loss_neg; }
-  }
-  if (!BWD) {
-    block_accumulate(pos, neg, acc);
-    finish_loss(acc, gridDim.x, out2);
-  }
-}
-
-// Target rebuilt from the object lists: k_focal_splat with half loads (its items, bands and tables).  This kernel is
-// issue-bound, and evaluating the tables and focal_elem a second time in backward measured slower than storing the
-// gradient (DESIGN 4.3.1): so, unlike the dense loss, the forward stores the fp32 gradient (grad32, nullable) and
-// backward is k_scale_round.  On the upcast the fp32 kernel groups by four whenever W % 4 == 0 (its pred and grad
-// are aligned); the plane bases are then 8-byte multiples.
-template <typename T, bool LOGITS>
-__global__ void __launch_bounds__(FOCAL_THREADS) k_focal_splat_half(const T *__restrict__ pred, const int32_t *cls,
-                                                                    const int32_t *cx, const int32_t *cy,
-                                                                    const int32_t *rad, const uint8_t *valid, int M,
-                                                                    int C, int H, int W, float *__restrict__ grad32,
-                                                                    FocalAcc *acc, float *out2, int parts, int B) {
-  __shared__ Obj s_obj[MAX_OBJ_PER_PLANE];
-  __shared__ ObjTab s_tab[MAX_OBJ_PER_PLANE];
-  __shared__ float s_gauss[GAUSS_TAB_FLOATS];
-  __shared__ int s_n, s_total;
-  const float np_ = (float)acc->num_pos;
-  const float inv_norm = 1.0f / (np_ > 0.0f ? np_ : 1.0f);
-  const bool pos_live = np_ > 0.0f;
-  double pos = 0, neg = 0;
-  const int n_items = B * C * parts;
-  const bool group4 = (W % 4 == 0);
-  const bool al8 = (((uintptr_t)pred & 7u) == 0), g_al16 = (((uintptr_t)grad32 & 15u) == 0);
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-    __syncthreads();   // the previous item's objects and tables are no longer read
-    const int plane = item / parts, part = item - plane * parts;
-    const int b = plane / C, c = plane - b * C;
-    const int y_lo = (int)((long long)H * part / parts), y_hi = (int)((long long)H * (part + 1) / parts);
-    const int nobj = gather_objects(cls, cx, cy, rad, valid, b, M, c, H, W, s_obj, &s_n, y_lo, y_hi);
-    if (nobj) build_tables(s_obj, nobj, s_tab, s_gauss, &s_total);
-    const long long base = (long long)plane * H * W;
-    if (group4) {
-      const int w4 = W / 4;
-      int y = y_lo + (int)threadIdx.x / w4, x = ((int)threadIdx.x - ((int)threadIdx.x / w4) * w4) * 4;
-      const int dyq = (int)blockDim.x / w4, dxq = ((int)blockDim.x - dyq * w4) * 4;
-      for (int i = y_lo * w4 + threadIdx.x; i < y_hi * w4; i += blockDim.x, y += dyq, x += dxq) {
-        if (x >= W) { x -= W; ++y; }
-        float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (nobj) g = target_at4(s_obj, s_tab, s_gauss, nobj, x, y);
-        const float4 p = load4<T>(pred + base + 4ll * i, al8);
-        const Elem e0 = focal_elem<LOGITS>(p.x, g.x, inv_norm, pos_live), e1 = focal_elem<LOGITS>(p.y, g.y, inv_norm, pos_live);
-        const Elem e2 = focal_elem<LOGITS>(p.z, g.z, inv_norm, pos_live), e3 = focal_elem<LOGITS>(p.w, g.w, inv_norm, pos_live);
-        pos += (double)((e0.loss_pos + e1.loss_pos) + (e2.loss_pos + e3.loss_pos));
-        neg += (double)((e0.loss_neg + e1.loss_neg) + (e2.loss_neg + e3.loss_neg));
-        if (grad32 && g_al16) {
-          reinterpret_cast<float4 *>(grad32 + base)[i] = make_float4(e0.grad, e1.grad, e2.grad, e3.grad);
-        } else if (grad32) {
-          float *gp = grad32 + base + 4ll * i;
-          gp[0] = e0.grad; gp[1] = e1.grad; gp[2] = e2.grad; gp[3] = e3.grad;
-        }
-      }
-    } else {
-      for (int i = y_lo * W + threadIdx.x; i < y_hi * W; i += blockDim.x) {
-        const int y = i / W, x = i - y * W;
-        const float g = nobj ? target_at(s_obj, s_tab, s_gauss, nobj, x, y) : 0.0f;
-        const Elem e = focal_elem<LOGITS>(widen<T>(pred[base + i]), g, inv_norm, pos_live);
-        pos += e.loss_pos; neg += e.loss_neg;
-        if (grad32) grad32[base + i] = e.grad;
-      }
-    }
-  }
-  block_accumulate(pos, neg, acc);
-  finish_loss(acc, gridDim.x, out2);
-}
-
+// ------------------------------------------------------------------ bf16 / fp16 gradients, no fp32 counterpart
 // out = T(g32 * *grad_out): the scale by the loss's incoming gradient, then the one rounding
 template <typename T>
 __global__ void __launch_bounds__(256) k_scale_round(const float *__restrict__ g32, long long n,
@@ -598,67 +547,11 @@ __global__ void __launch_bounds__(256) k_scale_round(const float *__restrict__ g
   const long long n4 = vec ? (n >> 2) : 0;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     const float4 g = __ldg(reinterpret_cast<const float4 *>(g32) + i);
-    store4<T>(out + 4 * i, true, __fmul_rn(g.x, go), __fmul_rn(g.y, go), __fmul_rn(g.z, go), __fmul_rn(g.w, go));
+    store4<T>(out, i, true, __fmul_rn(g.x, go), __fmul_rn(g.y, go), __fmul_rn(g.z, go), __fmul_rn(g.w, go));
   }
   for (long long i = (n4 << 2) + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x)
     out[i] = narrow<T>(__fmul_rn(g32[i], go));
-}
-
-// ---- Reg*Loss on a bf16 / fp16 map: the map is read at the gathered positions only.
-// One (image, object, channel) element i of k_reg_loss: false when its index is outside the map.
-template <typename T>
-__device__ __forceinline__ bool reg_elem(const T *__restrict__ output, const float *mask_f,
-                                         const int64_t *__restrict__ ind, const float *__restrict__ target, int D,
-                                         long long HW, int M, int mode, long long i, float *diff, float *m,
-                                         float *scale) {
-  const int d = (int)(i % D);
-  const long long bm = i / D;
-  const int b = (int)(bm / M);
-  const long long sp = ind[bm];
-  if (sp < 0 || sp >= HW) return false;
-  *m = mask_f[(mode == 3) ? i : bm];
-  float pred = widen<T>(output[((long long)b * D + d) * HW + sp]);
-  float tgt = target[i];
-  *scale = 1.0f;
-  if (mode == 2) {
-    *scale = 1.0f / (tgt + 1e-4f);
-    pred = pred / (tgt + 1e-4f);
-    tgt = tgt * 0.0f + 1.0f;
-  }
-  *diff = pred * *m - tgt * *m;
-  return true;
-}
-
-// k_reg_loss's pass 0 (same single CTA, same strides and tree).  out2 = (loss, (float)(mask sum + 1e-4)): the second
-// is the denominator k_reg_loss divides its gradient by, kept for k_reg_grad_half.
-template <typename T>
-__global__ void __launch_bounds__(1024) k_reg_loss_half(const T *__restrict__ output, const float *mask_f,
-                                                        const int64_t *__restrict__ ind,
-                                                        const float *__restrict__ target, int B, int D, long long HW,
-                                                        int M, int mode, float *out2) {
-  __shared__ double red[2][32];
-  const long long n = (long long)B * M * D;
-  double loss = 0, msum = 0;
-  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-    float diff, m, scale;
-    if (!reg_elem<T>(output, mask_f, ind, target, D, HW, M, mode, i, &diff, &m, &scale)) continue;
-    const float ad = fabsf(diff);
-    loss += (mode == 1) ? (ad < 1.0f ? 0.5 * (double)ad * ad : (double)ad - 0.5) : (double)ad;
-    msum += (mode == 1) ? ((i % D == 0) ? (double)m : 0.0) : (double)m;
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    loss += __shfl_xor_sync(0xffffffffu, loss, o);
-    msum += __shfl_xor_sync(0xffffffffu, msum, o);
-  }
-  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = loss; red[1][threadIdx.x >> 5] = msum; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double a = 0, c = 0;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { a += red[0][i]; c += red[1][i]; }
-    out2[0] = (float)(a / (c + 1e-4));
-    out2[1] = (float)(c + 1e-4);
-  }
 }
 
 // Every element of the fp32 gradient map that no index selects is +0, and autograd's scale makes it 0 * grad_out
@@ -704,7 +597,9 @@ __global__ void __launch_bounds__(256) k_reg_grad_half(const T *__restrict__ out
     for (int q = m0; q < M; ++q) {
       if (row[q] != sp) continue;
       float diff, m, scale;
-      reg_elem<T>(output, mask_f, ind, target, D, HW, M, mode, ((long long)b * M + q) * D + d, &diff, &m, &scale);
+      long long at;
+      reg_elem<T>(output, mask_f, ind, target, D, HW, M, mode, ((long long)b * M + q) * D + d, &diff, &m, &scale,
+                  &at);
       float g = (diff > 0.0f) ? 1.0f : (diff < 0.0f ? -1.0f : 0.0f);
       if (mode == 1 && fabsf(diff) < 1.0f) g = diff;
       g = g * m * scale / den;
@@ -734,28 +629,72 @@ static int focal_parts(int h) {
   return p < 1 ? 1 : p;
 }
 
+// The dense focal loss of cnb_focal_loss (T = float) and cnb_focal_loss_ex (bf16 / fp16: grad_scale = 1, grad null).
+// Errors name `who`, the entry point the caller used.
+template <typename T>
+static int focal_loss(const char *who, const T *pred, const float *gt, long long n, int logits, float grad_scale,
+                      float *out2, T *grad, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
+  CNB_REQUIRE(pred && gt && out2 && workspace, CNB_EINVAL, "%s: null pointer", who);
+  CNB_REQUIRE(n > 0, CNB_EINVAL, "%s: n=%lld", who, n);
+  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes(n), CNB_EWORKSPACE, "%s: workspace too small", who);
+  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
+  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
+  const int grid = focal_grid(n / 4 + 1);
+  k_count_pos_dense<<<grid, FOCAL_THREADS, 0, stream>>>(gt, n, acc);
+  const cudaError_t e = cudaGetLastError();
+  CNB_REQUIRE(e == cudaSuccess, CNB_ECUDA, "%s count: CUDA error: %s", who, cudaGetErrorString(e));
+  if (logits)
+    k_focal_dense<T, true, false><<<grid, FOCAL_THREADS, 0, stream>>>(pred, gt, n, grad_scale, grad, acc, out2, nullptr);
+  else
+    k_focal_dense<T, false, false><<<grid, FOCAL_THREADS, 0, stream>>>(pred, gt, n, grad_scale, grad, acc, out2, nullptr);
+  CNB_CHECK_LAUNCH(who);
+  count_launch(2);
+  return CNB_OK;
+}
+
+// The fused splat loss of cnb_focal_splat_loss (T = float) and cnb_focal_splat_loss_ex (bf16 / fp16: grad_scale = 1,
+// grad the unscaled fp32 gradient).  Errors name `who`, the entry point the caller used.
+template <typename T>
+static int focal_splat_loss(const char *who, const T *pred, const int32_t *obj_cls, const int32_t *obj_cx,
+                            const int32_t *obj_cy, const int32_t *obj_radius, const uint8_t *obj_valid, int b, int m,
+                            int c, int h, int w, int logits, float grad_scale, float *out2, float *grad,
+                            void *workspace, size_t workspace_bytes, cudaStream_t stream) {
+  CNB_REQUIRE(pred && obj_cls && obj_cx && obj_cy && obj_radius && obj_valid && out2 && workspace, CNB_EINVAL,
+              "%s: null pointer", who);
+  CNB_REQUIRE(b > 0 && m > 0 && c > 0 && h > 0 && w > 0, CNB_EINVAL, "%s: non-positive dimension", who);
+  CNB_REQUIRE(m <= MAX_OBJ_PER_PLANE, CNB_EUNSUPPORTED, "%s: at most %d objects per image (got %d)", who,
+              MAX_OBJ_PER_PLANE, m);
+  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes((long long)b * c * h * w), CNB_EWORKSPACE,
+              "%s: workspace too small", who);
+  CNB_REQUIRE((long long)c * h * w < (1ll << 31), CNB_EUNSUPPORTED, "%s: c*h*w must be < 2^31", who);
+  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
+  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
+  k_count_pos_objects<<<b, 128, (size_t)m * sizeof(int), stream>>>(obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, m, c, h,
+                                                                    w, acc);
+  const cudaError_t e = cudaGetLastError();
+  CNB_REQUIRE(e == cudaSuccess, CNB_ECUDA, "%s count: CUDA error: %s", who, cudaGetErrorString(e));
+  const int parts = focal_parts(h), grid = splat_grid((long long)b * c * parts);
+  if (logits)
+    k_focal_splat<T, true, false><<<grid, FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
+                                                                      obj_valid, m, c, h, w, grad_scale, grad,
+                                                                      nullptr, acc, out2, parts, b);
+  else
+    k_focal_splat<T, false, false><<<grid, FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
+                                                                       obj_valid, m, c, h, w, grad_scale, grad,
+                                                                       nullptr, acc, out2, parts, b);
+  CNB_CHECK_LAUNCH(who);
+  count_launch(2);
+  return CNB_OK;
+}
+
 extern "C" {
 
 size_t cnb_focal_workspace_bytes(long long) { return FOCAL_PART_OFF + (size_t)FOCAL_MAX_CTAS * sizeof(double2); }
 
 int cnb_focal_loss(const float *pred, const float *gt, long long n, int logits, float grad_scale, float *out2,
                    float *grad, void *workspace, size_t workspace_bytes, void *stream_) {
-  CNB_REQUIRE(pred && gt && out2 && workspace, CNB_EINVAL, "cnb_focal_loss: null pointer");
-  CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_loss: n=%lld", n);
-  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes(n), CNB_EWORKSPACE, "cnb_focal_loss: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
-  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
-  const int grid = focal_grid(n / 4 + 1);
-  k_count_pos_dense<<<grid, FOCAL_THREADS, 0, stream>>>(gt, n, acc);
-  CNB_CHECK_LAUNCH("cnb_focal_loss count");
-  if (logits)
-    k_focal_dense<true><<<grid, FOCAL_THREADS, 0, stream>>>(pred, gt, n, grad_scale, grad, acc, out2);
-  else
-    k_focal_dense<false><<<grid, FOCAL_THREADS, 0, stream>>>(pred, gt, n, grad_scale, grad, acc, out2);
-  CNB_CHECK_LAUNCH("cnb_focal_loss");
-  count_launch(2);
-  return CNB_OK;
+  return focal_loss("cnb_focal_loss", pred, gt, n, logits, grad_scale, out2, grad, workspace, workspace_bytes,
+                    (cudaStream_t)stream_);
 }
 
 int cnb_splat_gaussian(const int32_t *obj_cls, const int32_t *obj_cx, const int32_t *obj_cy,
@@ -767,7 +706,7 @@ int cnb_splat_gaussian(const int32_t *obj_cls, const int32_t *obj_cx, const int3
   CNB_REQUIRE(m <= MAX_OBJ_PER_PLANE, CNB_EUNSUPPORTED, "cnb_splat_gaussian: at most %d objects per image (got %d)",
               MAX_OBJ_PER_PLANE, m);
   const int parts = focal_parts(h);
-  k_focal_splat<false, true><<<splat_grid((long long)b * c * parts), FOCAL_THREADS, 0, (cudaStream_t)stream_>>>(
+  k_focal_splat<float, false, true><<<splat_grid((long long)b * c * parts), FOCAL_THREADS, 0, (cudaStream_t)stream_>>>(
       nullptr, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, m, c, h, w, 0.0f, nullptr, hm, nullptr, nullptr, parts, b);
   CNB_CHECK_LAUNCH("cnb_splat_gaussian");
   count_launch();
@@ -778,32 +717,8 @@ int cnb_focal_splat_loss(const float *pred, const int32_t *obj_cls, const int32_
                          const int32_t *obj_radius, const uint8_t *obj_valid, int b, int m, int c, int h, int w,
                          int logits, float grad_scale, float *out2, float *grad, void *workspace,
                          size_t workspace_bytes, void *stream_) {
-  CNB_REQUIRE(pred && obj_cls && obj_cx && obj_cy && obj_radius && obj_valid && out2 && workspace, CNB_EINVAL,
-              "cnb_focal_splat_loss: null pointer");
-  CNB_REQUIRE(b > 0 && m > 0 && c > 0 && h > 0 && w > 0, CNB_EINVAL, "cnb_focal_splat_loss: non-positive dimension");
-  CNB_REQUIRE(m <= MAX_OBJ_PER_PLANE, CNB_EUNSUPPORTED, "cnb_focal_splat_loss: at most %d objects per image (got %d)",
-              MAX_OBJ_PER_PLANE, m);
-  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes((long long)b * c * h * w), CNB_EWORKSPACE,
-              "cnb_focal_splat_loss: workspace too small");
-  cudaStream_t stream = (cudaStream_t)stream_;
-  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
-  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
-  CNB_REQUIRE((long long)c * h * w < (1ll << 31), CNB_EUNSUPPORTED, "cnb_focal_splat_loss: c*h*w must be < 2^31");
-  k_count_pos_objects<<<b, 128, (size_t)m * sizeof(int), stream>>>(obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, m, c, h,
-                                                                    w, acc);
-  CNB_CHECK_LAUNCH("cnb_focal_splat_loss count");
-  const int parts = focal_parts(h);
-  if (logits)
-    k_focal_splat<true, false><<<splat_grid((long long)b * c * parts), FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
-                                                                             obj_valid, m, c, h, w, grad_scale, grad,
-                                                                             nullptr, acc, out2, parts, b);
-  else
-    k_focal_splat<false, false><<<splat_grid((long long)b * c * parts), FOCAL_THREADS, 0, stream>>>(pred, obj_cls, obj_cx, obj_cy, obj_radius,
-                                                                              obj_valid, m, c, h, w, grad_scale, grad,
-                                                                              nullptr, acc, out2, parts, b);
-  CNB_CHECK_LAUNCH("cnb_focal_splat_loss");
-  count_launch(2);
-  return CNB_OK;
+  return focal_splat_loss("cnb_focal_splat_loss", pred, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, b, m, c, h, w,
+                          logits, grad_scale, out2, grad, workspace, workspace_bytes, (cudaStream_t)stream_);
 }
 
 int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, const float *target, int b, int d, int hw,
@@ -818,89 +733,45 @@ int cnb_reg_loss(const float *output, const void *mask, const int64_t *ind, cons
   return CNB_OK;
 }
 
-}  // extern "C"
-
-// ---- bf16 / fp16 pred: forward (loss) and backward (gradient in pred's dtype) as two calls
-static bool half_code(int dt) { return dt == CNB_DTYPE_BF16 || dt == CNB_DTYPE_F16; }
-static bool dtype_code_known(int dt) { return dt == CNB_DTYPE_F32 || half_code(dt); }
-
-template <typename T, bool BWD>
-static void launch_focal_dense_half(int logits, int grid, cudaStream_t stream, const void *pred, const float *gt,
-                                    long long n, FocalAcc *acc, float *out2, const float *grad_out, void *grad) {
-  if (logits)
-    k_focal_dense_half<T, true, BWD><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), gt, n, acc, out2,
-                                                                         grad_out, static_cast<T *>(grad));
-  else
-    k_focal_dense_half<T, false, BWD><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), gt, n, acc, out2,
-                                                                          grad_out, static_cast<T *>(grad));
-}
-
-template <typename T>
-static void launch_focal_splat_half(int logits, cudaStream_t stream, const void *pred, const int32_t *cls,
-                                    const int32_t *cx, const int32_t *cy, const int32_t *rad, const uint8_t *valid,
-                                    int b, int m, int c, int h, int w, float *grad32, FocalAcc *acc, float *out2) {
-  const int parts = focal_parts(h), grid = splat_grid((long long)b * c * parts);
-  if (logits)
-    k_focal_splat_half<T, true><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), cls, cx, cy, rad, valid, m, c, h, w,
-                                                                    grad32, acc, out2, parts, b);
-  else
-    k_focal_splat_half<T, false><<<grid, FOCAL_THREADS, 0, stream>>>(static_cast<const T *>(pred), cls, cx, cy, rad, valid, m, c, h, w,
-                                                                     grad32, acc, out2, parts, b);
-}
-
-template <typename T>
-static void launch_reg_grad_half(cudaStream_t stream, const void *output, const float *mask_f, const int64_t *ind,
-                                 const float *target, int b, int d, long long hw, int m, int mode,
-                                 const float *loss_den, const float *grad_out, void *grad) {
-  const long long total = (long long)b * d * hw, work = (long long)b * m * d;
-  const long long fill_ctas = (total / 4 + 255) / 256 + 1, cap = (long long)num_sms() * 16;
-  k_fill_scaled_zero<<<(int)(fill_ctas < cap ? fill_ctas : cap), 256, 0, stream>>>(static_cast<T *>(grad), total,
-                                                                                    grad_out);
-  k_reg_grad_half<<<(int)((work + 255) / 256 < cap ? (work + 255) / 256 : cap), 256, 0, stream>>>(
-      static_cast<const T *>(output), mask_f, ind, target, b, d, hw, m, mode, loss_den, grad_out,
-      static_cast<T *>(grad));
-}
-
-extern "C" {
+// ---- bf16 / fp16 pred: forward (loss) and backward (gradient in pred's dtype) as two calls.  An fp32 code given to a
+// call that has an fp32 form is that call.
 
 int cnb_focal_loss_ex(const void *pred, int pred_dtype, const float *gt, long long n, int logits, float *out2,
                       void *workspace, size_t workspace_bytes, void *stream_) {
-  CNB_REQUIRE(dtype_code_known(pred_dtype), CNB_EINVAL, "cnb_focal_loss_ex: unknown dtype code %d", pred_dtype);
+  CNB_REQUIRE(dtype_known(pred_dtype), CNB_EINVAL, "cnb_focal_loss_ex: unknown dtype code %d", pred_dtype);
   if (pred_dtype == CNB_DTYPE_F32)
     return cnb_focal_loss(static_cast<const float *>(pred), gt, n, logits, 1.0f, out2, nullptr, workspace,
                           workspace_bytes, stream_);
-  CNB_REQUIRE(pred && gt && out2 && workspace, CNB_EINVAL, "cnb_focal_loss_ex: null pointer");
-  CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_loss_ex: n=%lld", n);
-  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes(n), CNB_EWORKSPACE, "cnb_focal_loss_ex: workspace too small");
   cudaStream_t stream = (cudaStream_t)stream_;
-  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
-  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
-  const int grid = focal_grid(n / 4 + 1);
-  k_count_pos_dense<<<grid, FOCAL_THREADS, 0, stream>>>(gt, n, acc);
-  CNB_CHECK_LAUNCH("cnb_focal_loss_ex count");
   if (pred_dtype == CNB_DTYPE_BF16)
-    launch_focal_dense_half<__nv_bfloat16, false>(logits, grid, stream, pred, gt, n, acc, out2, nullptr, nullptr);
-  else
-    launch_focal_dense_half<__half, false>(logits, grid, stream, pred, gt, n, acc, out2, nullptr, nullptr);
-  CNB_CHECK_LAUNCH("cnb_focal_loss_ex");
-  count_launch(2);
-  return CNB_OK;
+    return focal_loss<__nv_bfloat16>("cnb_focal_loss_ex", static_cast<const __nv_bfloat16 *>(pred), gt, n, logits,
+                                     1.0f, out2, nullptr, workspace, workspace_bytes, stream);
+  return focal_loss<__half>("cnb_focal_loss_ex", static_cast<const __half *>(pred), gt, n, logits, 1.0f, out2, nullptr,
+                            workspace, workspace_bytes, stream);
 }
 
 int cnb_focal_grad_ex(const void *pred, int pred_dtype, const float *gt, long long n, int logits,
                       const float *loss_num_pos, const float *grad_out, void *grad, void *stream_) {
-  CNB_REQUIRE(dtype_code_known(pred_dtype), CNB_EINVAL, "cnb_focal_grad_ex: unknown dtype code %d", pred_dtype);
-  CNB_REQUIRE(half_code(pred_dtype), CNB_EUNSUPPORTED,
+  CNB_REQUIRE(dtype_known(pred_dtype), CNB_EINVAL, "cnb_focal_grad_ex: unknown dtype code %d", pred_dtype);
+  CNB_REQUIRE(pred_dtype != CNB_DTYPE_F32, CNB_EUNSUPPORTED,
               "cnb_focal_grad_ex: bf16 / fp16 only (cnb_focal_loss writes the fp32 gradient in its one pass)");
   CNB_REQUIRE(pred && gt && loss_num_pos && grad, CNB_EINVAL, "cnb_focal_grad_ex: null pointer");
   CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_grad_ex: n=%lld", n);
   cudaStream_t stream = (cudaStream_t)stream_;
   const int grid = focal_grid(n / 4 + 1);
   float *out2 = const_cast<float *>(loss_num_pos);   // read only when BWD
-  if (pred_dtype == CNB_DTYPE_BF16)
-    launch_focal_dense_half<__nv_bfloat16, true>(logits, grid, stream, pred, gt, n, nullptr, out2, grad_out, grad);
+  const auto *pb = static_cast<const __nv_bfloat16 *>(pred);
+  const auto *ph = static_cast<const __half *>(pred);
+  auto *gb = static_cast<__nv_bfloat16 *>(grad);
+  auto *gh = static_cast<__half *>(grad);
+  if (pred_dtype == CNB_DTYPE_BF16 && logits)
+    k_focal_dense<__nv_bfloat16, true, true><<<grid, FOCAL_THREADS, 0, stream>>>(pb, gt, n, 1.0f, gb, nullptr, out2, grad_out);
+  else if (pred_dtype == CNB_DTYPE_BF16)
+    k_focal_dense<__nv_bfloat16, false, true><<<grid, FOCAL_THREADS, 0, stream>>>(pb, gt, n, 1.0f, gb, nullptr, out2, grad_out);
+  else if (logits)
+    k_focal_dense<__half, true, true><<<grid, FOCAL_THREADS, 0, stream>>>(ph, gt, n, 1.0f, gh, nullptr, out2, grad_out);
   else
-    launch_focal_dense_half<__half, true>(logits, grid, stream, pred, gt, n, nullptr, out2, grad_out, grad);
+    k_focal_dense<__half, false, true><<<grid, FOCAL_THREADS, 0, stream>>>(ph, gt, n, 1.0f, gh, nullptr, out2, grad_out);
   CNB_CHECK_LAUNCH("cnb_focal_grad_ex");
   count_launch();
   return CNB_OK;
@@ -910,39 +781,24 @@ int cnb_focal_splat_loss_ex(const void *pred, int pred_dtype, const int32_t *obj
                             const int32_t *obj_cy, const int32_t *obj_radius, const uint8_t *obj_valid, int b, int m,
                             int c, int h, int w, int logits, float *out2, float *grad32, void *workspace,
                             size_t workspace_bytes, void *stream_) {
-  CNB_REQUIRE(dtype_code_known(pred_dtype), CNB_EINVAL, "cnb_focal_splat_loss_ex: unknown dtype code %d", pred_dtype);
+  CNB_REQUIRE(dtype_known(pred_dtype), CNB_EINVAL, "cnb_focal_splat_loss_ex: unknown dtype code %d", pred_dtype);
   if (pred_dtype == CNB_DTYPE_F32)
     return cnb_focal_splat_loss(static_cast<const float *>(pred), obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, b, m,
                                 c, h, w, logits, 1.0f, out2, grad32, workspace, workspace_bytes, stream_);
-  CNB_REQUIRE(pred && obj_cls && obj_cx && obj_cy && obj_radius && obj_valid && out2 && workspace, CNB_EINVAL,
-              "cnb_focal_splat_loss_ex: null pointer");
-  CNB_REQUIRE(b > 0 && m > 0 && c > 0 && h > 0 && w > 0, CNB_EINVAL, "cnb_focal_splat_loss_ex: non-positive dimension");
-  CNB_REQUIRE(m <= MAX_OBJ_PER_PLANE, CNB_EUNSUPPORTED,
-              "cnb_focal_splat_loss_ex: at most %d objects per image (got %d)", MAX_OBJ_PER_PLANE, m);
-  CNB_REQUIRE((long long)c * h * w < (1ll << 31), CNB_EUNSUPPORTED, "cnb_focal_splat_loss_ex: c*h*w must be < 2^31");
-  CNB_REQUIRE(workspace_bytes >= cnb_focal_workspace_bytes((long long)b * c * h * w), CNB_EWORKSPACE,
-              "cnb_focal_splat_loss_ex: workspace too small");
   cudaStream_t stream = (cudaStream_t)stream_;
-  FocalAcc *acc = reinterpret_cast<FocalAcc *>(workspace);
-  CNB_CUDA(cudaMemsetAsync(acc, 0, sizeof(FocalAcc), stream));
-  k_count_pos_objects<<<b, 128, (size_t)m * sizeof(int), stream>>>(obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, m, c, h,
-                                                                    w, acc);
-  CNB_CHECK_LAUNCH("cnb_focal_splat_loss_ex count");
   if (pred_dtype == CNB_DTYPE_BF16)
-    launch_focal_splat_half<__nv_bfloat16>(logits, stream, pred, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, b, m,
-                                           c, h, w, grad32, acc, out2);
-  else
-    launch_focal_splat_half<__half>(logits, stream, pred, obj_cls, obj_cx, obj_cy, obj_radius, obj_valid, b, m, c, h,
-                                    w, grad32, acc, out2);
-  CNB_CHECK_LAUNCH("cnb_focal_splat_loss_ex");
-  count_launch(2);
-  return CNB_OK;
+    return focal_splat_loss("cnb_focal_splat_loss_ex", static_cast<const __nv_bfloat16 *>(pred), obj_cls, obj_cx,
+                            obj_cy, obj_radius, obj_valid, b, m, c, h, w, logits, 1.0f, out2, grad32, workspace,
+                            workspace_bytes, stream);
+  return focal_splat_loss("cnb_focal_splat_loss_ex", static_cast<const __half *>(pred), obj_cls, obj_cx, obj_cy,
+                          obj_radius, obj_valid, b, m, c, h, w, logits, 1.0f, out2, grad32, workspace, workspace_bytes,
+                          stream);
 }
 
 int cnb_focal_splat_grad_ex(const float *grad32, long long n, const float *grad_out, void *grad, int grad_dtype,
                             void *stream_) {
-  CNB_REQUIRE(dtype_code_known(grad_dtype), CNB_EINVAL, "cnb_focal_splat_grad_ex: unknown dtype code %d", grad_dtype);
-  CNB_REQUIRE(half_code(grad_dtype), CNB_EUNSUPPORTED,
+  CNB_REQUIRE(dtype_known(grad_dtype), CNB_EINVAL, "cnb_focal_splat_grad_ex: unknown dtype code %d", grad_dtype);
+  CNB_REQUIRE(grad_dtype != CNB_DTYPE_F32, CNB_EUNSUPPORTED,
               "cnb_focal_splat_grad_ex: bf16 / fp16 only (an fp32 gradient is grad32 times grad_out)");
   CNB_REQUIRE(grad32 && grad, CNB_EINVAL, "cnb_focal_splat_grad_ex: null pointer");
   CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_focal_splat_grad_ex: n=%lld", n);
@@ -960,19 +816,19 @@ int cnb_focal_splat_grad_ex(const float *grad32, long long n, const float *grad_
 
 int cnb_reg_loss_ex(const void *output, int output_dtype, const void *mask, const int64_t *ind, const float *target,
                     int b, int d, int hw, int m, int mode, float *out2, void *stream_) {
-  CNB_REQUIRE(dtype_code_known(output_dtype), CNB_EINVAL, "cnb_reg_loss_ex: unknown dtype code %d", output_dtype);
-  CNB_REQUIRE(half_code(output_dtype), CNB_EUNSUPPORTED, "cnb_reg_loss_ex: bf16 / fp16 only (fp32: cnb_reg_loss)");
+  CNB_REQUIRE(dtype_known(output_dtype), CNB_EINVAL, "cnb_reg_loss_ex: unknown dtype code %d", output_dtype);
+  CNB_REQUIRE(output_dtype != CNB_DTYPE_F32, CNB_EUNSUPPORTED, "cnb_reg_loss_ex: bf16 / fp16 only (fp32: cnb_reg_loss)");
   CNB_REQUIRE(output && mask && ind && target && out2, CNB_EINVAL, "cnb_reg_loss_ex: null pointer");
   CNB_REQUIRE(b > 0 && d > 0 && hw > 0 && m > 0, CNB_EINVAL, "cnb_reg_loss_ex: non-positive dimension");
   CNB_REQUIRE(mode >= 0 && mode <= 3, CNB_EINVAL, "cnb_reg_loss_ex: mode %d", mode);
   cudaStream_t stream = (cudaStream_t)stream_;
   const float *mask_f = static_cast<const float *>(mask);
   if (output_dtype == CNB_DTYPE_BF16)
-    k_reg_loss_half<<<1, 1024, 0, stream>>>(static_cast<const __nv_bfloat16 *>(output), mask_f, ind, target, b, d,
-                                            (long long)hw, m, mode, out2);
+    k_reg_loss<<<1, 1024, 0, stream>>>(static_cast<const __nv_bfloat16 *>(output), mask_f, ind, target, b, d,
+                                       (long long)hw, m, mode, 1.0f, out2, nullptr);
   else
-    k_reg_loss_half<<<1, 1024, 0, stream>>>(static_cast<const __half *>(output), mask_f, ind, target, b, d,
-                                            (long long)hw, m, mode, out2);
+    k_reg_loss<<<1, 1024, 0, stream>>>(static_cast<const __half *>(output), mask_f, ind, target, b, d, (long long)hw,
+                                       m, mode, 1.0f, out2, nullptr);
   CNB_CHECK_LAUNCH("cnb_reg_loss_ex");
   count_launch();
   return CNB_OK;
@@ -981,8 +837,8 @@ int cnb_reg_loss_ex(const void *output, int output_dtype, const void *mask, cons
 int cnb_reg_loss_grad_ex(const void *output, int output_dtype, const void *mask, const int64_t *ind,
                          const float *target, int b, int d, int hw, int m, int mode, const float *loss_den,
                          const float *grad_out, void *grad_output, void *stream_) {
-  CNB_REQUIRE(dtype_code_known(output_dtype), CNB_EINVAL, "cnb_reg_loss_grad_ex: unknown dtype code %d", output_dtype);
-  CNB_REQUIRE(half_code(output_dtype), CNB_EUNSUPPORTED,
+  CNB_REQUIRE(dtype_known(output_dtype), CNB_EINVAL, "cnb_reg_loss_grad_ex: unknown dtype code %d", output_dtype);
+  CNB_REQUIRE(output_dtype != CNB_DTYPE_F32, CNB_EUNSUPPORTED,
               "cnb_reg_loss_grad_ex: bf16 / fp16 only (cnb_reg_loss writes the fp32 gradient in its one pass)");
   CNB_REQUIRE(output && mask && ind && target && loss_den && grad_output, CNB_EINVAL,
               "cnb_reg_loss_grad_ex: null pointer");
@@ -990,12 +846,21 @@ int cnb_reg_loss_grad_ex(const void *output, int output_dtype, const void *mask,
   CNB_REQUIRE(mode >= 0 && mode <= 3, CNB_EINVAL, "cnb_reg_loss_grad_ex: mode %d", mode);
   cudaStream_t stream = (cudaStream_t)stream_;
   const float *mask_f = static_cast<const float *>(mask);
-  if (output_dtype == CNB_DTYPE_BF16)
-    launch_reg_grad_half<__nv_bfloat16>(stream, output, mask_f, ind, target, b, d, hw, m, mode, loss_den, grad_out,
-                                        grad_output);
-  else
-    launch_reg_grad_half<__half>(stream, output, mask_f, ind, target, b, d, hw, m, mode, loss_den, grad_out,
-                                 grad_output);
+  const long long total = (long long)b * d * hw, work = (long long)b * m * d;
+  const long long fill_ctas = (total / 4 + 255) / 256 + 1, cap = (long long)num_sms() * 16;
+  const int fill_grid = (int)(fill_ctas < cap ? fill_ctas : cap);
+  const int grid = (int)((work + 255) / 256 < cap ? (work + 255) / 256 : cap);
+  if (output_dtype == CNB_DTYPE_BF16) {
+    auto *g = static_cast<__nv_bfloat16 *>(grad_output);
+    k_fill_scaled_zero<<<fill_grid, 256, 0, stream>>>(g, total, grad_out);
+    k_reg_grad_half<<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16 *>(output), mask_f, ind, target, b, d,
+                                              (long long)hw, m, mode, loss_den, grad_out, g);
+  } else {
+    auto *g = static_cast<__half *>(grad_output);
+    k_fill_scaled_zero<<<fill_grid, 256, 0, stream>>>(g, total, grad_out);
+    k_reg_grad_half<<<grid, 256, 0, stream>>>(static_cast<const __half *>(output), mask_f, ind, target, b, d,
+                                              (long long)hw, m, mode, loss_den, grad_out, g);
+  }
   CNB_CHECK_LAUNCH("cnb_reg_loss_grad_ex");
   count_launch(2);
   return CNB_OK;

@@ -67,7 +67,6 @@ size_t select_workspace_bytes(const SelectPlan &pl);
 int run_select(const void *src, const SelectPlan &pl, const FinalizeOut &out, void *ws, cudaStream_t stream,
                int src_dtype = CNB_DTYPE_F32);
 
-inline bool dtype_known(int dt) { return dt == CNB_DTYPE_F32 || dt == CNB_DTYPE_F16 || dt == CNB_DTYPE_BF16; }
 inline int dtype_bytes(int dt) { return dt == CNB_DTYPE_F32 ? 4 : 2; }
 // out = n elements of src (dtype code dt) widened to fp32, or (sigmoid) torch's CUDA sigmoid of them.  A plain
 // widening needs a 16-bit src.
@@ -90,11 +89,6 @@ int run_map_select(const void *src, int dt, int logits, const MapSelect &m, floa
                    void *ws, cudaStream_t stream);
 
 #ifdef __CUDACC__
-// Exact widening of one map / head element to fp32 (every fp16 and bf16 value, subnormals and infinities included,
-// is a float: the result equals torch's .float()).
-__device__ __forceinline__ float to_f32(float v) { return v; }
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
-__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
 // A score-map element as fp32: the exact widening, or (SIG: the element is a logit) torch's CUDA sigmoid of it,
 // 1 / (1 + exp(-x)) on the widened value (the expression of k_sigmoid).
 template <bool SIG, typename T>
