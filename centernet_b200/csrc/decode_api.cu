@@ -305,7 +305,9 @@ int cnb::plan_map_select(const void *src, int dt, int logits, int n_img, int C, 
     m->map_bytes = align_up((size_t)n_img * C * H * W * 4, 256);
   }
   m->pl.logits = (logits && !m->widen) ? 1 : 0;  // a widened map holds the sigmoid already
-  m->sel_bytes = select_workspace_bytes(m->pl);
+  // what the fp32 queries (cnb_topk_workspace_bytes, ...) reserve for this shape: enough for the plan of a map at any
+  // address and of either element size, so every query of a shape agrees whatever the map's dtype and alignment
+  m->sel_bytes = select_workspace_bytes_any_align(n_img, C, H, W, K);
   return CNB_OK;
 }
 
@@ -464,10 +466,9 @@ int cnb_gather_feat_backward_ex(const float *grad_out, const int64_t *ind, void 
 }
 
 size_t cnb_topk_workspace_bytes(int n_img, int c, int h, int w, int k) {
-  SelectPlan pl;
-  // worst case over alignment: the non-TMA plan has the same grid / slot count
-  if (make_select_plan(nullptr, n_img, c, h, w, k, 1, &pl) != CNB_OK) return 0;
-  return select_workspace_bytes(pl) + raw_bytes((long long)n_img * k);
+  const size_t sel = select_workspace_bytes_any_align(n_img, c, h, w, k);
+  if (sel == 0) return 0;
+  return sel + raw_bytes((long long)n_img * k);
 }
 
 int cnb_topk(const float *scores, int b, int c, int h, int w, int k, int fuse_nms, float *out_scores,

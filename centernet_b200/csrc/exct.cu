@@ -539,10 +539,10 @@ using namespace cnb;
 extern "C" {
 
 size_t cnb_exct_workspace_bytes(int b, int c, int cc, int h, int w, int k, int num_dets) {
-  SelectPlan pl;
-  if (make_select_plan(nullptr, b, c, h, w, k, 1, &pl) != CNB_OK) return 0;
+  const size_t sel = select_workspace_bytes_any_align(b, c, h, w, k);
+  if (sel == 0) return 0;
   (void)cc;
-  return select_workspace_bytes(pl) + exct_tail_bytes(b, c, h, w, k, num_dets);
+  return sel + exct_tail_bytes(b, c, h, w, k, num_dets);
 }
 
 int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_heat, const float *r_heat,

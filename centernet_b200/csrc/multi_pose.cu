@@ -110,12 +110,11 @@ using namespace cnb;
 extern "C" {
 
 size_t cnb_multi_pose_workspace_bytes(int b, int c, int j, int h, int w, int k) {
-  SelectPlan p1, p2;
-  if (make_select_plan(nullptr, b, c, h, w, k, 1, &p1) != CNB_OK) return 0;
-  size_t sel = select_workspace_bytes(p1);
+  size_t sel = select_workspace_bytes_any_align(b, c, h, w, k);
+  if (sel == 0) return 0;
   if (j > 0) {
-    if (make_select_plan(nullptr, b * j, 1, h, w, k, 1, &p2) != CNB_OK) return 0;
-    const size_t s2 = select_workspace_bytes(p2);
+    const size_t s2 = select_workspace_bytes_any_align(b * j, 1, h, w, k);
+    if (s2 == 0) return 0;
     sel = s2 > sel ? s2 : sel;
   }
   return sel + raw_bytes_((long long)b * k) + raw_bytes_((long long)b * j * k);

@@ -45,6 +45,16 @@ PYBIND11_MODULE(_C, m) {
                    ptr<int32_t>(oc), ptr<float>(oy), ptr<float>(ox), ptr<void>(ws), wsb, ptr<void>(stream)),
           "cnb_topk");
   });
+  m.def("select_plan_info", [](P src, int n_img, int c, int h, int w, int k, int nms, int elem_size) {
+    int v[CNB_SELECT_PLAN_FIELDS];
+    check(cnb_select_plan_info(ptr<const void>(src), n_img, c, h, w, k, nms, elem_size, v, CNB_SELECT_PLAN_FIELDS),
+          "cnb_select_plan_info");
+    static const char *names[CNB_SELECT_PLAN_FIELDS] = {"hot", "n_cta", "wb", "max_slots", "seg_cap",
+                                                         "fused_finalize", "use_tma", "rb", "local_img"};
+    py::dict d;
+    for (int i = 0; i < CNB_SELECT_PLAN_FIELDS; ++i) d[names[i]] = v[i];
+    return d;
+  });
   m.def("topk_channel", [](P scores, int b, int c, int h, int w, int k, int fuse_nms, P os, P oi, P oy, P ox, P ws,
                            size_t wsb, P stream) {
     check(cnb_topk_channel(ptr<const float>(scores), b, c, h, w, k, fuse_nms, ptr<float>(os), ptr<int64_t>(oi),

@@ -1549,6 +1549,14 @@ size_t select_workspace_bytes(const SelectPlan &pl) {
   return keys + cnts + done + cnts;  // + per-segment thresholds
 }
 
+size_t select_workspace_bytes_any_align(int n_img, int C, int H, int W, int K) {
+  SelectPlan aligned, misaligned;
+  if (make_select_plan(nullptr, n_img, C, H, W, K, 1, &aligned) != CNB_OK) return 0;
+  if (make_select_plan(reinterpret_cast<const void *>(4), n_img, C, H, W, K, 1, &misaligned) != CNB_OK) return 0;
+  const size_t a = select_workspace_bytes(aligned), m = select_workspace_bytes(misaligned);
+  return a > m ? a : m;
+}
+
 template <bool NMS, bool TMA, int MODE>
 static int launch_stage1(const float *src, const SelectPlan &pl, const FinalizeOut &out, u64 *cand, int *cnt,
                          int *done, cudaStream_t stream) {
@@ -1639,3 +1647,23 @@ extern "C" int cnb_debug_select_stats(unsigned long long *out, int n_cta) {
 #endif
 
 }  // namespace cnb
+
+extern "C" int cnb_select_plan_info(const void *src, int n_img, int C, int H, int W, int K, int nms, int elem_size,
+                                    int *out, int n_out) {
+  CNB_REQUIRE(out != nullptr && n_out >= 0, CNB_EINVAL, "cnb_select_plan_info: null pointer");
+  CNB_REQUIRE(elem_size == 4 || elem_size == 2, CNB_EINVAL, "cnb_select_plan_info: elem_size %d", elem_size);
+  cnb::SelectPlan pl;
+  const int rc = cnb::make_select_plan(src, n_img, C, H, W, K, nms, &pl, elem_size);
+  if (rc != CNB_OK) return rc;
+  // some image lies inside one CTA's range: that CTA finalizes it without a global segment
+  int local_img = 0;
+  for (int i = 0; i < pl.n_cta && !local_img; ++i) {
+    const long long lo = pl.cta_start[i], hi = pl.cta_start[i + 1];
+    const long long first = (lo + C - 1) / C * C;   // first image boundary at or after lo
+    local_img = (first + C <= hi) ? 1 : 0;
+  }
+  const int v[CNB_SELECT_PLAN_FIELDS] = {pl.hot, pl.n_cta, pl.wb, pl.max_slots, pl.seg_cap, pl.fused_finalize,
+                                         pl.use_tma, pl.rb, local_img};
+  for (int i = 0; i < n_out && i < CNB_SELECT_PLAN_FIELDS; ++i) out[i] = v[i];
+  return CNB_OK;
+}

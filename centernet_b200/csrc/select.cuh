@@ -62,6 +62,9 @@ struct FinalizeOut {
 int make_select_plan(const void *src, int n_img, int C, int H, int W, int K, int nms, SelectPlan *pl,
                      int elem_size = 4);
 size_t select_workspace_bytes(const SelectPlan &pl);
+// select_workspace_bytes for an fp32 map at any address (0 when no plan exists): an aligned 128x128 map takes the hot
+// plan, a misaligned one the generic plan, whose grid and segment count differ, so neither bounds the other.
+size_t select_workspace_bytes_any_align(int n_img, int C, int H, int W, int K);
 // Enqueue stage 1 + finalize.  `ws` must hold select_workspace_bytes(pl).  src_dtype other than CNB_DTYPE_F32 is
 // only accepted for a hot plan (pl.hot) made with elem_size 2.
 int run_select(const void *src, const SelectPlan &pl, const FinalizeOut &out, void *ws, cudaStream_t stream,

@@ -77,6 +77,18 @@ int cnb_topk(const float *scores, int b, int c, int h, int w, int k, int fuse_nm
              float *out_ys, float *out_xs,
              void *workspace, size_t workspace_bytes, void *stream);
 
+/* Read-only view of the plan every selection above (and every decode built on it) makes for an
+ * [n_img, C, H, W] map at `src` (its alignment and elem_size -- 4, or 2 for fp16 / bf16 -- decide whether
+ * TMA can load it) on the current device.  Writes min(n_out, CNB_SELECT_PLAN_FIELDS) ints to out, in this
+ * order: hot (warp-asynchronous 128x128 kernel), n_cta (stage-1 grid), wb (planes one image boundary weighs
+ * in the partition, 0 = equal split), max_slots (segments one image can receive), seg_cap (keys per
+ * segment), fused_finalize (0: the separate finalize kernel runs), use_tma, rb (rows per unit) and
+ * local_img (some image lies inside one CTA's range, so that CTA finalizes it from shared memory).
+ * Launches nothing; errors are those of the selection itself for the same arguments. */
+#define CNB_SELECT_PLAN_FIELDS 9
+int cnb_select_plan_info(const void *src, int n_img, int c, int h, int w, int k, int nms, int elem_size,
+                         int *out, int n_out);
+
 /* models/decode.py:92-101 (_topk_channel): per (b, channel) top-K.
  * Outputs are [b, c, k]. */
 int cnb_topk_channel(const float *scores, int b, int c, int h, int w, int k, int fuse_nms,

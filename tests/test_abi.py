@@ -37,6 +37,34 @@ def test_pybind_layer_and_validation():
     assert "exceeds" in _C.last_error()
 
 
+def test_select_plan_info():
+    """cnb_select_plan_info: the selection's plan without a launch (no GPU needed: without a device the plan is
+    made for 132 SMs)."""
+    from centernet_b200 import _C
+    keys = ["hot", "n_cta", "wb", "max_slots", "seg_cap", "fused_finalize", "use_tma", "rb", "local_img"]
+    p = _C.select_plan_info(256, 64, 80, 128, 128, 100, 1, 4)
+    assert sorted(p) == sorted(keys)
+    assert p["hot"] == 1 and p["use_tma"] == 1 and p["rb"] == 128 and p["fused_finalize"] == 1
+    assert p["seg_cap"] == 256 and p["wb"] == 4 and 1 <= p["n_cta"] <= 192 and p["max_slots"] >= 2
+    assert _C.select_plan_info(256, 64, 80, 128, 128, 200, 1, 4)["seg_cap"] == 200
+    assert _C.select_plan_info(256, 64, 80, 128, 128, 100, 1, 2)["hot"] == 1          # fp16 / bf16 map
+    assert _C.select_plan_info(258, 64, 80, 128, 128, 100, 1, 2)["use_tma"] == 0      # misaligned: generic path
+    assert _C.select_plan_info(256, 64, 80, 128, 128, 100, 0, 4)["hot"] == 0          # no peak test
+    big = _C.select_plan_info(256, 1, 80, 128, 128, 1000, 1, 4)
+    assert big["hot"] == 0 and big["fused_finalize"] == 0 and big["max_slots"] * 1000 <= 8192
+    one = _C.select_plan_info(256, 1, 3, 128, 128, 100, 1, 4)
+    assert one["n_cta"] == 1 and one["local_img"] == 1
+    assert _C.select_plan_info(256, 100, 1, 128, 128, 100, 1, 4)["local_img"] == 1    # C=1: one plane per image
+    strips = _C.select_plan_info(256, 2, 4, 200, 152, 64, 1, 4)
+    assert strips["hot"] == 0 and strips["rb"] < 200
+    with pytest.raises(NotImplementedError):
+        _C.select_plan_info(256, 1, 80, 128, 128, 1025, 1, 4)
+    with pytest.raises(RuntimeError, match="exceeds"):
+        _C.select_plan_info(256, 1, 1, 4, 4, 17, 1, 4)
+    with pytest.raises(RuntimeError, match="elem_size"):
+        _C.select_plan_info(256, 1, 1, 4, 4, 1, 1, 8)
+
+
 def test_no_cpu_fallback():
     import torch
     from centernet_b200 import decode
