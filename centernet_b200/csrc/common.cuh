@@ -39,11 +39,14 @@ inline void count_launch(int n = 1) { g_launches.fetch_add((unsigned long long)n
     }                                                                            \
   } while (0)
 
+// A failed runtime call also leaves its (non-sticky) error as the last error; CNB_CUDA clears it, or the next
+// CNB_CHECK_LAUNCH would report it against an unrelated launch.
 #define CNB_CUDA(call)                                                           \
   do {                                                                           \
     cudaError_t e__ = (call);                                                    \
     if (e__ != cudaSuccess) {                                                    \
       cnb::set_error("%s: CUDA error: %s", #call, cudaGetErrorString(e__));      \
+      (void)cudaGetLastError();                                                  \
       return CNB_ECUDA;                                                          \
     }                                                                            \
   } while (0)

@@ -29,7 +29,8 @@ constexpr int EX_THREADS = 512;
 constexpr int EX_CAP = 4096;       // candidate keys per CTA
 constexpr int EX_STEP = 2048;      // tuples scored between two capacity checks
 constexpr int EX_MAX_DETS = 2048;  // num_dets limit (CAP - STEP)
-constexpr int EX_MAX_GROUPS = 16;   // segments per image (the merge sorts groups * num_dets keys in shared memory: 128 KB at 16 x 1000)
+constexpr int EX_MAX_GROUPS = 16;  // segments per image
+constexpr int EX_MERGE_KEYS = 16384;  // the merge sorts np2(groups * num_dets) keys in shared memory: 128 KiB at most
 
 struct RawList {
   float *scores; int64_t *inds; int32_t *clses; float *ys; float *xs;
@@ -57,6 +58,10 @@ __device__ __forceinline__ uint32_t mono_bits(float v) {  // order-preserving ma
 __device__ __forceinline__ float mono_inv(uint32_t m) {
   return __uint_as_float((m & 0x80000000u) ? (m & 0x7fffffffu) : ~m);
 }
+// mono_bits for the centre-map bound of the pruning test: a NaN of either sign is the top value, because a tuple
+// that reads it scores the device's positive NaN, whose key lies above +inf (mono_bits puts a sign-bit NaN below
+// every number)
+__device__ __forceinline__ uint32_t bound_bits(float v) { return v != v ? 0xffffffffu : mono_bits(v); }
 
 __device__ __forceinline__ void sort_desc(u64 *buf, int n) {
   for (int k = 2; k <= n; k <<= 1)
@@ -72,7 +77,8 @@ __device__ __forceinline__ void sort_desc(u64 *buf, int n) {
 __device__ __forceinline__ int np2(int v) { int n = 2; while (n < v) n <<= 1; return n; }
 
 // max / argmax over classes of the centre map (decode.py:159), compared as fp32 scores: with SIG the sigmoids,
-// not the logits, so classes whose sigmoids tie (e.g. both saturate to 1) yield the first one, as torch.max does
+// not the logits, so classes whose sigmoids tie (e.g. both saturate to 1) yield the first one, as torch.max does.
+// As torch.max, a NaN wins over every number and the first NaN class is taken.
 template <typename T, bool SIG>
 __global__ void __launch_bounds__(256) k_ct_agnostic(const T *__restrict__ ct, int B, int CC, long long HW,
                                                      float *__restrict__ agn, int32_t *__restrict__ cls) {
@@ -81,22 +87,24 @@ __global__ void __launch_bounds__(256) k_ct_agnostic(const T *__restrict__ ct, i
   const long long b = i / HW, sp = i - b * HW;
   const T *p = ct + b * CC * HW + sp;
   float best = score_f32<SIG>(p[0]);
-  int arg = 0;
+  int arg = 0, nan_arg = best != best ? 0 : CC;
   for (int c = 1; c < CC; ++c) {
     const float v = score_f32<SIG>(p[(long long)c * HW]);
     if (v > best) { best = v; arg = c; }
+    if (v != v) nan_arg = min(nan_arg, c);   // a chain of its own: the max above does not wait for it
   }
+  if (nan_arg < CC) { arg = nan_arg; best = score_f32<SIG>(p[(long long)nan_arg * HW]); }
   agn[i] = best;
   cls[i] = arg;
 }
 
-// out[b] = max over the image's centre map, as order-preserving bits (out zero-filled: below every float)
+// out[b] = max over the image's centre map, as bound_bits (out zero-filled: below every float)
 __global__ void __launch_bounds__(256) k_ct_max(const float *__restrict__ ct, long long per_image, uint32_t *__restrict__ out) {
   __shared__ uint32_t red[8];
   const float *p = ct + (long long)blockIdx.y * per_image;
   uint32_t best = 0u;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < per_image; i += (long long)gridDim.x * blockDim.x)
-    best = max(best, mono_bits(__ldg(p + i)));
+    best = max(best, bound_bits(__ldg(p + i)));
   for (int k = 16; k > 0; k >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, k));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = best;
   __syncthreads();
@@ -117,7 +125,7 @@ __global__ void __launch_bounds__(256) k_ct_scores(const T *__restrict__ ct, lon
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < per_image; i += (long long)gridDim.x * blockDim.x) {
     const float v = score_f32<SIG>(__ldg(ct + base + i));
     sc[base + i] = v;
-    best = max(best, mono_bits(v));
+    best = max(best, bound_bits(v));
   }
   for (int k = 16; k > 0; k >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, k));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = best;
@@ -181,7 +189,14 @@ __global__ void __launch_bounds__(EX_THREADS, 1) k_exct_tuples(const ExctArgs a)
         ub = __fdiv_rn(ub, 6.0f);
         for (int q = 0; q < lb; ++q) ub = __fsub_rn(ub, 1.0f);
         ub = __fadd_rn(ub, 0.0f);      // -0 -> +0: the key order puts -0 below +0
-        if (mono_bits(ub) < (uint32_t)(thr >> 32)) continue;
+        // The list scores are never NaN and at most 1 (the clamp), so besides a NaN centre value (which bound_bits
+        // makes the bound) only 2*ct = +inf meeting a -inf sum of the four scores makes a tuple NaN, ranked first:
+        // such a block is not pruned.  The block's smallest sum takes the last (lowest) bottom and right scores of
+        // the descending lists, fp32 addition being monotone; tested only for a block about to be pruned.
+        if (mono_bits(ub) < (uint32_t)(thr >> 32)) {
+          if (__fmul_rn(2.0f, ctmax) < INFINITY) continue;
+          if (__fadd_rn(__fadd_rn(__fadd_rn(ts, lsx), S[2][K - 1]), S[3][K - 1]) != -INFINITY) continue;
+        }
       }
       for (int base = 0; base < K2; base += EX_STEP) {
         // the num_dets-th key of ANY group of the image bounds the result from below: adopt the best one published
@@ -229,7 +244,9 @@ __global__ void __launch_bounds__(EX_THREADS, 1) k_exct_tuples(const ExctArgs a)
           sc = __fsub_rn(sc, top_bad ? 1.0f : 0.0f);
           sc = __fsub_rn(sc, left_bad ? 1.0f : 0.0f);
           sc = __fsub_rn(sc, bot_bad ? 1.0f : 0.0f);
-          sc = __fsub_rn(sc, right_bad ? 1.0f : 0.0f);
+          // sc - 1 as sc + (-1), the same rounding; sc + 0 folds -0 to +0: one value, ordered by tuple index (a
+          // negative subnormal sum / 6 rounds to -0)
+          sc = __fadd_rn(sc, right_bad ? -1.0f : 0.0f);
           const uint32_t tuple = (uint32_t)((long long)i * K3 + (long long)j * K2 + e);
           const u64 key = ((u64)mono_bits(sc) << 32) | (u64)(0xffffffffu - tuple);
           if (key > thr) buf[atomicAdd(&s_cnt, 1)] = key;
@@ -317,10 +334,14 @@ static RawList carve(char *&p, long long n) {
   r.xs = reinterpret_cast<float *>(p); p += align_up((size_t)n * 4, 256);
   return r;
 }
-static int exct_groups(int b, int k) {
+// CTAs per image of k_exct_tuples: two CTAs per SM over the batch, at most 16, one per top index, and no more
+// segments than the merge can sort (at the default num_dets = 1000, 16)
+static int exct_groups(int b, int k, int num_dets) {
+  if (b < 1 || k < 1 || num_dets < 1) return 1;   // sizes a workspace query on arguments the call then rejects
   int g = (2 * num_sms() + b - 1) / b;
   if (g > EX_MAX_GROUPS) g = EX_MAX_GROUPS;
   if (g > k) g = k;
+  if (g > EX_MERGE_KEYS / num_dets) g = EX_MERGE_KEYS / num_dets;
   return g < 1 ? 1 : g;
 }
 
@@ -342,7 +363,7 @@ static bool exct_plain(const ExctIn &x) {
 
 // everything after the selection scratch: raw lists, aggregated maps, agnostic centre map, segments, bounds
 static size_t exct_tail_bytes(int b, int c, int h, int w, int k, int num_dets) {
-  const int g = exct_groups(b, k);
+  const int g = exct_groups(b, k, num_dets);
   const size_t maps = 4 * align_up((size_t)b * c * h * w * 4, 256);       // aggregated maps (aggr_weight > 0)
   const size_t agn = 2 * align_up((size_t)b * h * w * 4, 256);            // class-agnostic centre map
   return 4 * raw_sz((long long)b * k) + maps + agn + align_up((size_t)b * g * num_dets * 8, 256) +
@@ -437,7 +458,7 @@ static int exct_decode(const char *fn, const ExctIn &x, int b, int c, int cc, in
   for (int q = 0; q < 4; ++q) { agg[q] = reinterpret_cast<float *>(p); p += map_bytes; }
   float *agn = reinterpret_cast<float *>(p); p += align_up((size_t)b * h * w * 4, 256);
   int32_t *agn_cls = reinterpret_cast<int32_t *>(p); p += align_up((size_t)b * h * w * 4, 256);
-  const int groups = exct_groups(b, k);
+  const int groups = exct_groups(b, k, num_dets);
   a.seg = reinterpret_cast<u64 *>(p); p += align_up((size_t)b * groups * num_dets * 8, 256);
   a.seg_cnt = reinterpret_cast<int *>(p); p += align_up((size_t)b * groups * 4, 256);
   uint32_t *ct_max = reinterpret_cast<uint32_t *>(p); p += align_up((size_t)b * 4, 256);
@@ -543,6 +564,11 @@ size_t cnb_exct_workspace_bytes(int b, int c, int cc, int h, int w, int k, int n
   if (sel == 0) return 0;
   (void)cc;
   return sel + exct_tail_bytes(b, c, h, w, k, num_dets);
+}
+
+int cnb_exct_groups(int b, int k, int num_dets) {
+  if (b < 1 || k < 1 || num_dets < 1) return 0;
+  return exct_groups(b, k, num_dets);
 }
 
 int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_heat, const float *r_heat,

@@ -213,6 +213,7 @@ PYBIND11_MODULE(_C, m) {
           "cnb_edge_aggregate_ex");
   });
   m.def("exct_workspace_bytes", &cnb_exct_workspace_bytes);
+  m.def("exct_groups", &cnb_exct_groups);
   m.def("exct_decode_ex_workspace_bytes", [](P t, P l, P b_, P r, int t_dt, int l_dt, int b_dt, int r_dt, int ct_dt,
                                              int tr_dt, int lr_dt, int br_dt, int rr_dt, int logits, int b, int c,
                                              int cc, int h, int w, int k, float aw, int nd, int agn) {

@@ -251,6 +251,11 @@ int cnb_edge_aggregate_ex(const void *heat, int dtype, int apply_sigmoid, float 
  * agnostic), ct heat [b,cc,h,w]; regr [b,2,h,w] each or all NULL
  * -> dets [b,num_dets,14]. */
 size_t cnb_exct_workspace_bytes(int b, int c, int cc, int h, int w, int k, int num_dets);
+/* Number of CTAs (groups) per image the tuple kernel of a decode with these sizes launches on the current device:
+ * min(16, ceil(2 * SMs / b), k, 16384 / num_dets).  Each group keeps its num_dets best tuples, and the merge sorts
+ * the groups' segments of an image in shared memory, which holds at most 16384 keys.  Launches nothing; returns 0
+ * when b, k or num_dets is below 1. */
+int cnb_exct_groups(int b, int k, int num_dets);
 int cnb_exct_decode(const float *t_heat, const float *l_heat, const float *b_heat,
                     const float *r_heat, const float *ct_heat,
                     const float *t_regr, const float *l_regr, const float *b_regr,

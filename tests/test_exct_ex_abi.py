@@ -169,3 +169,16 @@ def test_python_functions_refuse_cpu_tensors(dt):
                D._bottom_aggregate):
         with pytest.raises(NotImplementedError, match="only implemented for CUDA"):
             fn(m())
+
+
+def test_shape_queries_survive_rejected_num_dets_and_batch():
+    """The fp32 workspace query and the group query take num_dets and b before any argument check: a zero must not
+    reach a division (the call itself then rejects it)."""
+    from centernet_b200 import _C
+    b, c, cc, h, w, k = HOT
+    for nd in (0, -3):
+        assert isinstance(_C.exct_workspace_bytes(b, c, cc, h, w, k, nd), int)
+        assert _C.exct_groups(1, 40, nd) == 0
+    assert isinstance(_C.exct_workspace_bytes(0, c, cc, h, w, k, ND), int)
+    assert _C.exct_groups(0, 40, ND) == 0
+    assert _C.exct_groups(1, 0, ND) == 0
