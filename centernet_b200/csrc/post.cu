@@ -9,6 +9,7 @@
 // soft-NMS overlaps use the float32 storage / float64 intermediates of the Cython-generated C (integer
 // literals become the double 1.0) and the Gaussian weight goes through a float64 exp.
 #include "common.cuh"
+#include "warp.cuh"
 
 namespace cnb {
 
@@ -651,10 +652,7 @@ int cnb_ddd_tail(const float *dets, int b, int n, int d, const double *trans, co
 // ------------------------------------------------------------------ N4: detector input pre-processing
 // detectors/base_detector.py:37-65: cv2.warpAffine(INTER_LINEAR, BORDER_CONSTANT 0) of the uint8 HWC image,
 // (x / 255 - mean) / std in float64, HWC -> CHW fp32, optional mirrored copy (flip test) -- one pass, the image
-// crosses PCIe as uint8 (3 B / pixel instead of 12-24).  The warp restates OpenCV's fixed-point algorithm
-// (imgwarp.cpp): coordinates on a 1/1024 grid from the INVERTED matrix `minv` (cvRound = round half to even),
-// +16, >> 5 -> integer pixel + 5-bit phase; weights 32 * (32 - fy | fy) * (32 - fx | fx) (sum 32768);
-// value = (sum w * p + 2^14) >> 15 with out-of-image taps reading the border value 0.
+// crosses PCIe as uint8 (3 B / pixel instead of 12-24).  The warp is OpenCV's fixed-point algorithm (warp.cuh).
 // kF32: DddDetector.pre_process's normalisation (detectors/ddd.py:50-51), x.astype(float32) / 255. then
 // (x - mean) / std all in float32, instead of base_detector's float64 -- the warp is the same.
 namespace cnb {
@@ -665,21 +663,9 @@ __device__ __forceinline__ void preprocess_px(const unsigned char *__restrict__ 
                                               int flip) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= ow) return;
-  const double m0 = minv[0], m1 = minv[1], m2 = minv[2], m3 = minv[3], m4 = minv[4], m5 = minv[5];
-  const long long adelta = (long long)__double2ll_rn(__dmul_rn(__dmul_rn(m0, (double)x), 1024.0));
-  const long long bdelta = (long long)__double2ll_rn(__dmul_rn(__dmul_rn(m3, (double)x), 1024.0));
-  const long long X0 = (long long)__double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(m1, (double)y), m2), 1024.0)) + 16;
-  const long long Y0 = (long long)__double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(m4, (double)y), m5), 1024.0)) + 16;
-  auto sat_int = [](long long v) { return v > 2147483647ll ? 2147483647ll : (v < -2147483648ll ? -2147483648ll : v); };
-  const int X = (int)((sat_int(X0 - 16) + 16 + sat_int(adelta)) >> 5);   // saturate_cast<int> of each rounded term
-  const int Y = (int)((sat_int(Y0 - 16) + 16 + sat_int(bdelta)) >> 5);
-  int sx = X >> 5, sy = Y >> 5;
-  sx = min(max(sx, -32768), 32767);
-  sy = min(max(sy, -32768), 32767);
-  const int fx = X & 31, fy = Y & 31;
-  const int w0 = (32 - fy) * (32 - fx) * 32, w1 = (32 - fy) * fx * 32, w2 = fy * (32 - fx) * 32, w3 = fy * fx * 32;
-  const bool y0ok = sy >= 0 && sy < H, y1ok = sy + 1 >= 0 && sy + 1 < H;
-  const bool x0ok = sx >= 0 && sx < W, x1ok = sx + 1 >= 0 && sx + 1 < W;
+  const WarpTaps t = warp_taps(minv, x, y, H, W);
+  const int sx = t.sx, sy = t.sy, w0 = t.w0, w1 = t.w1, w2 = t.w2, w3 = t.w3;
+  const bool y0ok = t.y0ok, y1ok = t.y1ok, x0ok = t.x0ok, x1ok = t.x1ok;
   const size_t plane = (size_t)oh * ow;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {

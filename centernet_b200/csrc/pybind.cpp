@@ -377,6 +377,27 @@ PYBIND11_MODULE(_C, m) {
                                    ptr<const float>(stdv), ptr<float>(out), oh, ow, flip, ptr<void>(stream)),
           "cnb_preprocess_image_f32");
   });
+  m.attr("TRAIN_MAX_PIXELS") = CNB_TRAIN_MAX_PIXELS;
+  m.def("train_images_workspace_bytes", &cnb_train_images_workspace_bytes);
+  m.def("train_images", [](P src, P off, P hw, P minv, P flip, P order, P blend, P light, P mean, P stdv, int b,
+                           int oh, int ow, P out, int dt, int cl, P ws, size_t wsb, P stream) {
+    check(cnb_train_images(ptr<const uint8_t>(src), ptr<const int64_t>(off), ptr<const int32_t>(hw),
+                           ptr<const double>(minv), ptr<const uint8_t>(flip), ptr<const int32_t>(order),
+                           ptr<const float>(blend), ptr<const double>(light), ptr<const float>(mean),
+                           ptr<const float>(stdv), b, oh, ow, ptr<void>(out), dt, cl, ptr<void>(ws), wsb,
+                           ptr<void>(stream)),
+          "cnb_train_images");
+  });
+  m.def("ctdet_targets", [](P boxes, P cls, P nobj, P flip, P hw, P trans, int b, int mm, int nc, int oh, int ow,
+                            P wh, P ind, P reg, P reg_mask, P csw, P csm, P ocls, P ocx, P ocy, P orad, P oval,
+                            P stream) {
+    check(cnb_ctdet_targets(ptr<const float>(boxes), ptr<const int32_t>(cls), ptr<const int32_t>(nobj),
+                            ptr<const uint8_t>(flip), ptr<const int32_t>(hw), ptr<const double>(trans), b, mm, nc, oh,
+                            ow, ptr<float>(wh), ptr<int64_t>(ind), ptr<float>(reg), ptr<uint8_t>(reg_mask),
+                            ptr<float>(csw), ptr<uint8_t>(csm), ptr<int32_t>(ocls), ptr<int32_t>(ocx),
+                            ptr<int32_t>(ocy), ptr<int32_t>(orad), ptr<uint8_t>(oval), ptr<void>(stream)),
+          "cnb_ctdet_targets");
+  });
   m.def("dcnv2_workspace_bytes", &cnb_dcnv2_workspace_bytes);
   m.def("dcnv2_backward_workspace_bytes", &cnb_dcnv2_backward_workspace_bytes);
   m.def("dcnv2_backward_ex", [](P input, int in_cl, P offset, P mask, P weight, P gout, P gin, int gin_cl, P goff, P gmask,

@@ -1,0 +1,318 @@
+"""Training input of the ctdet sampler on the device (datasets/sample/ctdet.py:29-145 and color_aug,
+utils/image.py:198-230).
+
+The reference's loader warps, colour-augments, normalises and transposes every image on the host CPU, paints an
+80 x 128 x 128 heat map in Python and copies the float batch across PCIe.  Here the host keeps what it must do --
+cv2.imread, the COCO annotations and the random draws, from the same generators in the same order -- and the
+device does the per-pixel arithmetic and the target geometry:
+
+    loader = DataLoader(CTDetTrainInput(dataset), batch_size=..., collate_fn=collate_ctdet, pin_memory=True, ...)
+    for packed in loader:
+        batch = build_ctdet_batch(packed)      # one H2D copy of the uint8 images + parameters, 2-3 launches
+
+`batch` holds what the reference's collated batch holds, on the device and bit for bit for the same RNG states
+('input', 'reg_mask', 'ind', 'wh' or 'cat_spec_wh' / 'cat_spec_mask', 'reg' with opt.reg_offset; 'hm' with
+dense_hm=True), plus the object lists FocalSplatLoss takes ('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius',
+'obj_valid').  `augment_images` is the image half alone, for explicit matrices, flips and colour parameters.
+The numeric contract is DESIGN.md section 4.9."""
+import itertools
+import os
+import random
+
+import numpy as np
+import torch
+
+from ._lib import C, _DTYPE_CODES, ptr, stream_ptr, workspace
+from .losses import splat_gaussian
+from .post_process import _affine_points, cv_affine_transform
+from .pre_process import _invert
+
+F32 = np.float32
+
+# color_aug's functions list [brightness_, contrast_, saturation_] as kinds 0, 1, 2; an order code is the index
+# of the shuffled list among the six permutations in lexicographic order (include/centernet_b200.h).
+ORDERS = tuple(itertools.permutations(range(3)))
+# Largest source side: the warp clamps source coordinates to [-32768, 32767].
+MAX_SIDE = 32767
+
+
+def _get_border(border, size):
+    """CTDetDataset._get_border (ctdet.py:22-26)."""
+    i = 1
+    while size - border // i <= border // i:
+        i *= 2
+    return border // i
+
+
+def affine_transform(center, scale, output_size):
+    """get_affine_transform(center, scale, 0, output_size) (utils/image.py:27-60) as a 2x3 float64, to the bit.
+    A scale that is not an array becomes a float32 pair as there; a float64 array scale (keep_res with a random
+    crop) keeps its float64 half-width, which the reference adds to the float32 centre in float64."""
+    if not isinstance(scale, np.ndarray):
+        scale = np.array([scale, scale], dtype=F32)
+    src, dst = _affine_points(center, scale.astype(F32), output_size)
+    src[1, 1] = F32(np.float64(F32(center[1])) + np.float64(scale[0]) * -0.5)
+    d = src[0] - src[1]
+    src[2] = src[1] + np.array([-d[1], d[0]], F32)
+    return cv_affine_transform(src, dst)
+
+
+def sample_params(height, width, opt, split, data_rng, eig_val, eig_vec):
+    """The random draws of CTDetDataset.__getitem__ (ctdet.py:41-67) and color_aug for one height x width image,
+    from np.random, random and data_rng in the reference's order, and the matrices they give.  After the call
+    the three generators are where the reference leaves them."""
+    c = np.array([width / 2., height / 2.], dtype=np.float32)
+    if opt.keep_res:
+        input_h = (height | opt.pad) + 1
+        input_w = (width | opt.pad) + 1
+        s = np.array([input_w, input_h], dtype=np.float32)
+    else:
+        s = max(height, width) * 1.0
+        input_h, input_w = opt.input_h, opt.input_w
+    flipped = False
+    if split == 'train':
+        if not opt.not_rand_crop:
+            s = s * np.random.choice(np.arange(0.6, 1.4, 0.1))
+            w_border = _get_border(128, width)
+            h_border = _get_border(128, height)
+            c[0] = np.random.randint(low=w_border, high=width - w_border)
+            c[1] = np.random.randint(low=h_border, high=height - h_border)
+        else:
+            sf, cf = opt.scale, opt.shift
+            c[0] += s * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+            c[1] += s * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+            s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
+        if np.random.random() < opt.flip:
+            flipped = True
+            c[0] = width - c[0] - 1
+    order, blend, light = -1, np.zeros(6, F32), np.zeros(3, np.float64)
+    if split == 'train' and not opt.no_color_aug:
+        kinds = [0, 1, 2]
+        random.shuffle(kinds)                  # color_aug's random.shuffle of its three functions
+        for k in kinds:                        # one uniform per blend, in the order they run
+            alpha = 1. + data_rng.uniform(low=-0.4, high=0.4)
+            blend[2 * k], blend[2 * k + 1] = F32(alpha), F32(1 - alpha)
+        light = np.dot(eig_vec, eig_val * data_rng.normal(scale=0.1, size=(3,)))
+        order = ORDERS.index(tuple(kinds))
+    output_h, output_w = input_h // opt.down_ratio, input_w // opt.down_ratio
+    return {'c': c, 's': s, 'flip': flipped, 'input_h': input_h, 'input_w': input_w,
+            'output_h': output_h, 'output_w': output_w,
+            'minv': np.array(_invert(affine_transform(c, s, [input_w, input_h])), np.float64),
+            'trans_output': affine_transform(c, s, [output_w, output_h]).reshape(6),
+            'order': order, 'blend': blend, 'light': np.asarray(light, np.float64)}
+
+
+class CTDetTrainInput(torch.utils.data.Dataset):
+    """Wraps a reference CTDetDataset instance (duck-typed on opt, coco, images, img_dir, max_objs, cat_ids,
+    num_classes, mean, std, _data_rng, _eig_val, _eig_vec and split).  __getitem__ reads the image and the
+    annotations and draws the random parameters as the reference does, and returns them with the uint8 image and
+    the float32 box corners; it does no pixel work (collate_ctdet + build_ctdet_batch do)."""
+
+    def __init__(self, dataset):
+        opt = dataset.opt
+        if opt.mse_loss:
+            raise NotImplementedError("CTDetTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not implemented")
+        if opt.dense_wh:
+            raise NotImplementedError("CTDetTrainInput: opt.dense_wh targets are not implemented")
+        self.dataset = dataset
+
+    def __len__(self):
+        return len(self.dataset)
+
+    def __getitem__(self, index):
+        import cv2
+        ds = self.dataset
+        img_id = ds.images[index]
+        file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
+        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
+        num_objs = min(len(anns), ds.max_objs)
+        img = cv2.imread(os.path.join(ds.img_dir, file_name))
+        sample = sample_params(img.shape[0], img.shape[1], ds.opt, ds.split, ds._data_rng, ds._eig_val, ds._eig_vec)
+        boxes = np.zeros((num_objs, 4), F32)
+        cls = np.zeros(num_objs, np.int32)
+        for k in range(num_objs):
+            b = anns[k]['bbox']
+            boxes[k] = np.array([b[0], b[1], b[0] + b[2], b[1] + b[3]], dtype=np.float32)
+            cls[k] = int(ds.cat_ids[anns[k]['category_id']])
+        sample.update(image=img, boxes=boxes, cls=cls, max_objs=ds.max_objs, num_classes=ds.num_classes,
+                      mean=np.asarray(ds.mean, F32).reshape(3), std=np.asarray(ds.std, F32).reshape(3),
+                      cat_spec_wh=bool(ds.opt.cat_spec_wh), reg_offset=bool(ds.opt.reg_offset))
+        return sample
+
+
+class _Packer(object):
+    """Arrays laid end to end in one byte buffer, each at a 16-byte aligned offset."""
+
+    def __init__(self):
+        self.parts, self.layout, self.size = [], {}, 0
+
+    def add(self, name, a):
+        a = np.ascontiguousarray(a)
+        self.layout[name] = (self.size, a.dtype.str, a.shape)
+        self.parts.append((self.size, a.reshape(-1).view(np.uint8)))
+        self.size += (a.nbytes + 15) // 16 * 16
+
+    def tensor(self, pin):
+        buf = torch.empty(max(self.size, 16), dtype=torch.uint8, pin_memory=pin)
+        host = buf.numpy()
+        for off, a in self.parts:
+            host[off:off + a.size] = a
+        return buf
+
+
+def _pin():
+    # pinned here when collating in the main process; a DataLoader worker leaves that to pin_memory=True
+    return torch.utils.data.get_worker_info() is None and torch.cuda.is_available()
+
+
+def _check_images(images):
+    for img in images:
+        if img.ndim != 3 or img.shape[2] != 3 or img.dtype != np.uint8:
+            raise ValueError("train_input: images must be uint8 [H, W, 3], got %s %s" % (img.dtype, img.shape))
+        if not (1 <= img.shape[0] <= MAX_SIDE and 1 <= img.shape[1] <= MAX_SIDE):
+            raise NotImplementedError("train_input: source sides up to %d (got %s)" % (MAX_SIDE, img.shape[:2]))
+
+
+def _pack_images(pk, images, minv, flip, order, blend, light, mean, std):
+    b = len(images)
+    sizes = [img.nbytes for img in images]
+    pk.add('src', np.concatenate([np.ascontiguousarray(img).reshape(-1) for img in images]))
+    pk.add('src_off', np.concatenate([[0], np.cumsum(sizes[:-1])]).astype(np.int64))
+    pk.add('src_hw', np.array([img.shape[:2] for img in images], np.int32).reshape(b, 2))
+    pk.add('minv', np.asarray(minv, np.float64).reshape(b, 6))
+    pk.add('flip', np.asarray(flip, np.uint8).reshape(b))
+    order = np.asarray(order, np.int64).reshape(b)
+    if ((order < -1) | (order > 5)).any():
+        raise ValueError("train_input: blend order codes are -1 (off) or 0..5")
+    pk.add('order', order.astype(np.int32))
+    pk.add('blend', np.asarray(blend, F32).reshape(b, 6))
+    pk.add('light', np.asarray(light, np.float64).reshape(b, 3))
+    pk.add('norm', np.concatenate([np.asarray(mean, F32).reshape(3), np.asarray(std, F32).reshape(3)]))
+
+
+def _views(buf, layout):
+    out = {}
+    for name, (off, dt, shape) in layout.items():
+        dt = np.dtype(dt)
+        n = int(np.prod(shape, dtype=np.int64)) * dt.itemsize
+        out[name] = buf[off:off + n].view(getattr(torch, dt.name)).reshape(shape)
+    return out
+
+
+def _launch_images(v, b, out_h, out_w, color, dtype, memory_format, dev):
+    if dtype not in _DTYPE_CODES:
+        raise ValueError("train_input: dtype must be float32, bfloat16 or float16, got %s" % (dtype,))
+    if memory_format not in (torch.contiguous_format, torch.channels_last):
+        raise ValueError("train_input: memory_format must be contiguous_format or channels_last")
+    if out_h * out_w > C.TRAIN_MAX_PIXELS:
+        raise NotImplementedError("train_input: at most %d output pixels per image" % C.TRAIN_MAX_PIXELS)
+    out = torch.empty((b, 3, out_h, out_w), dtype=dtype, device=dev, memory_format=memory_format)
+    wsb = C.train_images_workspace_bytes(b, out_h, out_w) if color else 0
+    ws = workspace(wsb, dev) if color else None
+    C.train_images(ptr(v['src']), ptr(v['src_off']), ptr(v['src_hw']), ptr(v['minv']), ptr(v['flip']),
+                   ptr(v['order']) if color else 0, ptr(v['blend']), ptr(v['light']), ptr(v['norm'][:3]),
+                   ptr(v['norm'][3:]), b, out_h, out_w, ptr(out), _DTYPE_CODES[dtype],
+                   int(memory_format == torch.channels_last), ptr(ws), wsb, stream_ptr(out))
+    return out
+
+
+def _device(device):
+    return torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+
+
+def augment_images(images, matrices, out_h, out_w, mean, std, flips=None, orders=None, blends=None, lights=None,
+                   device=None, dtype=torch.float32, memory_format=torch.contiguous_format):
+    """The image half of the training samplers for explicit parameters: per image cv2.warpAffine(img, M,
+    (out_w, out_h), INTER_LINEAR) of the uint8 BGR source (mirrored first, img[:, ::-1], where flips says so),
+    x / 255, color_aug when orders[b] >= 0, (x - mean) / std, as [B, 3, out_h, out_w] of dtype in memory_format.
+      images: list of uint8 [H, W, 3] numpy arrays (any sizes); matrices: the FORWARD 2x3 matrices, as passed to
+      cv2.warpAffine (rotated ones included); orders: blend order codes (ORDERS index, -1 = no colour
+      augmentation), blends [B, 6] the float32 (alpha, 1 - alpha) of brightness, contrast and saturation,
+      lights [B, 3] the float64 lighting offsets (see sample_params).
+    One host->device copy and one launch (two with colour augmentation)."""
+    dev = _device(device)
+    images = [np.asarray(img) for img in images]
+    _check_images(images)
+    b = len(images)
+    if b == 0:
+        raise ValueError("augment_images: no images")
+    minv = np.array([_invert(m) for m in np.asarray(matrices, np.float64).reshape(b, 2, 3)], np.float64)
+    flips = np.zeros(b, np.uint8) if flips is None else np.asarray(flips, np.uint8)
+    orders = np.full(b, -1) if orders is None else np.asarray(orders)
+    pk = _Packer()
+    _pack_images(pk, images, minv, flips, orders, np.zeros((b, 6), F32) if blends is None else blends,
+                 np.zeros((b, 3)) if lights is None else lights, mean, std)
+    buf = pk.tensor(_pin() and dev.type == "cuda").to(dev, non_blocking=True)
+    return _launch_images(_views(buf, pk.layout), b, int(out_h), int(out_w), bool((orders >= 0).any()), dtype,
+                          memory_format, dev)
+
+
+def collate_ctdet(samples):
+    """Packs CTDetTrainInput samples into one uint8 buffer (images, then the small per-image arrays) and the
+    scalars build_ctdet_batch needs.  Raises ValueError when the samples have different input sizes (keep_res
+    with images of different sizes), where the reference's default_collate fails too."""
+    s0 = samples[0]
+    for s in samples:
+        if (s['input_h'], s['input_w']) != (s0['input_h'], s0['input_w']):
+            raise ValueError("collate_ctdet: samples of different input sizes (%dx%d and %dx%d) cannot be batched"
+                             % (s0['input_h'], s0['input_w'], s['input_h'], s['input_w']))
+    images = [s['image'] for s in samples]
+    _check_images(images)
+    b, m = len(samples), int(s0['max_objs'])
+    boxes = np.zeros((b, m, 4), F32)
+    cls = np.zeros((b, m), np.int32)
+    nobj = np.zeros(b, np.int32)
+    for i, s in enumerate(samples):
+        n = min(len(s['boxes']), m)
+        boxes[i, :n], cls[i, :n], nobj[i] = s['boxes'][:n], s['cls'][:n], n
+        if n and (cls[i, :n].min() < 0 or cls[i, :n].max() >= s0['num_classes']):
+            raise ValueError("collate_ctdet: class id outside [0, %d)" % s0['num_classes'])
+    pk = _Packer()
+    _pack_images(pk, images, [s['minv'] for s in samples], [s['flip'] for s in samples],
+                 [s['order'] for s in samples], [s['blend'] for s in samples], [s['light'] for s in samples],
+                 s0['mean'], s0['std'])
+    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
+    pk.add('nobj', nobj)
+    pk.add('boxes', boxes)
+    pk.add('cls', cls)
+    scalars = {k: s0[k] for k in ('input_h', 'input_w', 'output_h', 'output_w', 'max_objs', 'num_classes',
+                                  'cat_spec_wh', 'reg_offset')}
+    scalars.update(batch=b, color=any(s['order'] >= 0 for s in samples))
+    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+
+
+def build_ctdet_batch(packed, device=None, dtype=torch.float32, memory_format=torch.contiguous_format,
+                      dense_hm=False):
+    """The reference's collated ctdet batch, on the device, from a collate_ctdet result: one non-blocking H2D
+    copy on the current stream, the image pass (one launch, two with colour augmentation) and the target kernel,
+    plus splat_gaussian with dense_hm.  Keys, shapes and dtypes as ctdet.py:128-140 returns them; 'hm' only with
+    dense_hm; always the FocalSplatLoss lists obj_cls, obj_cx, obj_cy, obj_radius (int32) and obj_valid (uint8).
+    The packed host buffer is not modified."""
+    dev = _device(device)
+    sc = packed['scalars']
+    b, m, nc, oh, ow = sc['batch'], sc['max_objs'], sc['num_classes'], sc['output_h'], sc['output_w']
+    buf = packed['buffer'].to(dev, non_blocking=True)
+    v = _views(buf, packed['layout'])
+    inp = _launch_images(v, b, sc['input_h'], sc['input_w'], sc['color'], dtype, memory_format, dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    u8 = dict(dtype=torch.uint8, device=dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    wh, reg = torch.empty((b, m, 2), **f32), torch.empty((b, m, 2), **f32)
+    ind, reg_mask = torch.empty((b, m), dtype=torch.int64, device=dev), torch.empty((b, m), **u8)
+    csw = torch.empty((b, m, 2 * nc), **f32) if sc['cat_spec_wh'] else None
+    csm = torch.empty((b, m, 2 * nc), **u8) if sc['cat_spec_wh'] else None
+    lists = [torch.empty((b, m), **i32) for _ in range(4)] + [torch.empty((b, m), **u8)]
+    C.ctdet_targets(ptr(v['boxes']), ptr(v['cls']), ptr(v['nobj']), ptr(v['flip']), ptr(v['src_hw']),
+                    ptr(v['trans_output']), b, m, nc, oh, ow, ptr(wh), ptr(ind), ptr(reg), ptr(reg_mask), ptr(csw),
+                    ptr(csm), *[ptr(t) for t in lists], stream_ptr(wh))
+    ret = {'input': inp, 'reg_mask': reg_mask, 'ind': ind}
+    if dense_hm:
+        ret['hm'] = splat_gaussian(*lists, nc, oh, ow)
+    if sc['cat_spec_wh']:
+        ret.update(cat_spec_wh=csw, cat_spec_mask=csm)
+    else:
+        ret['wh'] = wh
+    if sc['reg_offset']:
+        ret['reg'] = reg
+    ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
+    return ret

@@ -710,6 +710,52 @@ int cnb_preprocess_image_f32(const uint8_t *image_hwc, int h, int w, const doubl
                              const float *mean3, const float *std3, float *out,
                              int out_h, int out_w, int flip_test, void *stream);
 
+/* ------------------------------------------------ training input of the ctdet sampler
+ * CTDetDataset.__getitem__ (datasets/sample/ctdet.py:29-145) after the random draws, for a whole batch.
+ *
+ * cnb_train_images: per image b, the uint8 BGR source [h_b, w_b, 3] at src + src_off[b] (src_hw[b] = (h_b, w_b)),
+ * mirrored (img[:, ::-1]) when flip[b] != 0 -- sampled at mirrored columns, never materialised -- and warped with
+ * the INVERTED 2x3 float64 matrix minv6[b] (cv2.warpAffine INTER_LINEAR, border 0, OpenCV's fixed point as in
+ * cnb_preprocess_image); then x / 255, color_aug (utils/image.py:198-230) and (x - mean) / std, all float32.
+ *   order: NULL = no colour augmentation for any image; else order[b] = -1 (off for image b) or the blend order
+ *     0..5 = BCS, BSC, CBS, CSB, SBC, SCB (B brightness_, C contrast_, S saturation_, applied left to right);
+ *   blend[b, 6] = (a, b) of B, C, S with a = f32(alpha), b = f32(1 - alpha) (the difference in float64);
+ *   light[b, 3] = np.dot(eig_vec, eig_val * normal(0.1, 3)) in float64.
+ * Per pixel: gs = fma(r, 0.299f, fma(b, 0.114f, g * 0.587f)); gs_mean = numpy's pairwise float32 sum of gs over
+ * the out_h * out_w pixels (its exact tree) / n; B: x * a; C: x * a + f32(gs_mean * b); S: x * a + f32(gs * b);
+ * lighting f32(f64(x) + light[c]); each step a rounded float32 operation unless stated.
+ *   out: [b, 3, out_h, out_w] (channels_last == 0) or [b, out_h, out_w, 3] (channels_last == 1) of out_dtype
+ *     (CNB_DTYPE_F32 / _BF16 / _F16; half types are the fp32 value rounded once to nearest even);
+ *   mean3 / std3: fp32 on the device.  Every image has the one output size of the batch.
+ * With colour augmentation two launches (the grey sums, then the image), else one; the workspace
+ * (cnb_train_images_workspace_bytes, 0 for a bad shape) holds the grey partial sums.  No atomics: the output is
+ * identical run to run.  Errors, checked before any CUDA call: CNB_EINVAL for a null pointer, a bad shape, an
+ * unknown dtype code or a channels_last other than 0 / 1; CNB_EUNSUPPORTED for more than CNB_TRAIN_MAX_PIXELS
+ * output pixels; CNB_EWORKSPACE for too small a workspace.  The per-image records live on the device, out of
+ * the host's sight: an image whose side lies outside [1, 32767] (the warp clamps source coordinates there) or
+ * whose order code is not in -1..5 is written as quiet NaN.  centernet_b200.train_input rejects both first.
+ *
+ * cnb_ctdet_targets: ctdet.py:99-127 for m = max_objs slots per image, one thread per (image, slot): slot k <
+ * min(num_objs[b], m) holds the float32 corners boxes[b, k] = [x, y, x + w, y + h] and the class cls[b, k] in
+ * [0, num_classes); they are mirrored when flip[b] != 0 (width src_hw[b][1]), mapped by the FORWARD 2x3 float64
+ * trans6[b] (get_affine_transform(c, s, 0, [out_w, out_h]), float64 t0 x + t1 y + t2 rounded to float32),
+ * clipped, and a box with h > 0 and w > 0 gets wh [b,m,2] f32, ind [b,m] i64, reg [b,m,2] f32, reg_mask [b,m]
+ * u8 = 1, cat_spec_wh [b,m,2*num_classes] f32 / cat_spec_mask u8 (both NULL to skip) and the FocalSplatLoss
+ * lists obj_cls / obj_cx / obj_cy / obj_radius i32 and obj_valid u8 [b,m] (ct_int, max(0, int(gaussian_radius(
+ * ceil(h), ceil(w)))) in float64, reg_mask); every other slot is zero.  Errors, checked before any CUDA call:
+ * CNB_EINVAL for a null pointer, only one of the cat_spec pair or a bad shape. */
+#define CNB_TRAIN_MAX_PIXELS 4194304
+size_t cnb_train_images_workspace_bytes(int b, int out_h, int out_w);
+int cnb_train_images(const uint8_t *src, const int64_t *src_off, const int32_t *src_hw, const double *minv6,
+                     const uint8_t *flip, const int32_t *order, const float *blend, const double *light,
+                     const float *mean3, const float *std3, int b, int out_h, int out_w, void *out, int out_dtype,
+                     int channels_last, void *workspace, size_t workspace_bytes, void *stream);
+int cnb_ctdet_targets(const float *boxes, const int32_t *cls, const int32_t *num_objs, const uint8_t *flip,
+                      const int32_t *src_hw, const double *trans6, int b, int m, int num_classes, int out_h,
+                      int out_w, float *wh, int64_t *ind, float *reg, uint8_t *reg_mask, float *cat_spec_wh,
+                      uint8_t *cat_spec_mask, int32_t *obj_cls, int32_t *obj_cx, int32_t *obj_cy,
+                      int32_t *obj_radius, uint8_t *obj_valid, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,114 @@
+"""Device time per ctdet training batch (centernet_b200.train_input), the host->device bytes per image against the
+reference loader's, and the numpy oracle's CPU time per image.
+
+    python tools/train_input_time.py [--iters 50]
+
+Synthetic COCO-sized sources (ragged 640x480 / 480x640 / 500x375 / 427x640), 512x512 input, 80 classes, 128
+object slots, about 7 objects per image, colour augmentation on; B = 32, 64 and 114.  Per batch it times, with
+CUDA events over --iters batches after a warm-up, build_ctdet_batch (H2D copy of the packed pinned buffer + image
+kernels + targets) with and without the dense hm, and the same from a buffer already on the device (kernels
+only).  The reference's loader is not part of the repository, so the host-side figure is the numpy oracle
+(tests/train_np.py: warp, color_aug, normalisation, targets, hm splat) on one core: a stand-in for the per-pixel
+work this moves off the host, not a measurement of cv2.  Prints one JSON line."""
+import argparse
+import json
+import os
+import random
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+from centernet_b200 import train_input as T  # noqa: E402
+import train_cases as TC  # noqa: E402
+
+SIZES = [(480, 640), (640, 480), (375, 500), (640, 427), (427, 640), (333, 500)]
+
+
+def make_samples(b, seed):
+    opt = TC.make_opt(dict(TC.CASES["crop"]))
+    rng = np.random.default_rng(seed)
+    np.random.seed(seed); random.seed(seed)
+    data_rng = np.random.RandomState(seed)
+    out = []
+    for i in range(b):
+        h, w = SIZES[i % len(SIZES)]
+        s = T.sample_params(h, w, opt, 'train', data_rng, TC.EIG_VAL, TC.EIG_VEC)
+        n = int(rng.integers(1, 15))
+        x0, y0 = rng.uniform(0, w, n), rng.uniform(0, h, n)
+        boxes = np.stack([x0, y0, x0 + rng.uniform(4, 200, n), y0 + rng.uniform(4, 200, n)], 1).astype(np.float32)
+        s.update(image=rng.integers(0, 256, (h, w, 3), dtype=np.uint8), boxes=boxes,
+                 cls=rng.integers(0, 80, n).astype(np.int32), max_objs=128, num_classes=80, mean=TC.MEAN,
+                 std=TC.STD, cat_spec_wh=False, reg_offset=True)
+        out.append(s)
+    return out
+
+
+def time_batches(packed, iters, dense_hm):
+    for _ in range(3):
+        T.build_ctdet_batch(packed, dense_hm=dense_hm)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        T.build_ctdet_batch(packed, dense_hm=dense_hm)
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / iters
+
+
+def oracle_cpu_ms(samples, n):
+    import train_np as TN
+    from oracle import image_np
+    t0 = time.perf_counter()
+    for s in samples[:n]:
+        TN.train_image(s['image'], T.affine_transform(s['c'], s['s'], [512, 512]), s['flip'], 512, 512, TC.MEAN,
+                       TC.STD, s['order'], s['blend'], s['light'])
+        t = TN.ctdet_targets(s['boxes'], s['cls'], s['flip'], s['image'].shape[1], s['trans_output'], 128, 80, 128,
+                             128)
+        lists = [t[k][None] for k in ('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid')]
+        image_np.splat_objects(*lists, 80, 128, 128)
+    return (time.perf_counter() - t0) * 1e3 / n
+
+
+def gpu_info():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
+    except (OSError, subprocess.SubprocessError):
+        return torch.cuda.get_device_name()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--iters", type=int, default=50)
+    ap.add_argument("--oracle-images", type=int, default=4)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("train_input_time: needs a CUDA device (no CPU timing is reported)")
+    res = {"gpu": gpu_info(), "batches": {}}
+    ref_bytes = 3 * 512 * 512 * 4 + 80 * 128 * 128 * 4 + 128 * (2 * 4 + 2 * 4 + 8 + 1)
+    for b in (32, 64, 114):
+        samples = make_samples(b, b)
+        packed = T.collate_ctdet(samples)
+        on_device = dict(packed, buffer=packed['buffer'].cuda())   # the same batch without the H2D copy
+        r = {"ms_per_batch": time_batches(packed, args.iters, False),
+             "ms_per_batch_kernels_only": time_batches(on_device, args.iters, False),
+             "ms_per_batch_dense_hm": time_batches(packed, args.iters, True),
+             "h2d_bytes_per_image": packed['buffer'].numel() / b,
+             "reference_h2d_bytes_per_image": ref_bytes}
+        r["us_per_image"] = r["ms_per_batch"] * 1e3 / b
+        res["batches"][b] = r
+    res["oracle_cpu_ms_per_image_stand_in"] = oracle_cpu_ms(make_samples(args.oracle_images, 7), args.oracle_images)
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
