@@ -398,6 +398,21 @@ PYBIND11_MODULE(_C, m) {
                             ptr<int32_t>(ocy), ptr<int32_t>(orad), ptr<uint8_t>(oval), ptr<void>(stream)),
           "cnb_ctdet_targets");
   });
+  m.def("multi_pose_targets", [](P boxes, P cls, P nobj, P kps, P flip, P rotated, P hw, P trans, P trans_rot,
+                                 P perm, int b, int mm, int nj, int res, P wh, P ind, P reg, P reg_mask, P hps,
+                                 P hps_mask, P hp_offset, P hp_ind, P hp_mask, P ocls, P ocx, P ocy, P orad, P oval,
+                                 P hcx, P hcy, P hrad, P hval, P stream) {
+    check(cnb_multi_pose_targets(ptr<const float>(boxes), ptr<const int32_t>(cls), ptr<const int32_t>(nobj),
+                                 ptr<const float>(kps), ptr<const uint8_t>(flip), ptr<const uint8_t>(rotated),
+                                 ptr<const int32_t>(hw), ptr<const double>(trans), ptr<const double>(trans_rot),
+                                 ptr<const int32_t>(perm), b, mm, nj, res, ptr<float>(wh), ptr<int64_t>(ind),
+                                 ptr<float>(reg), ptr<uint8_t>(reg_mask), ptr<float>(hps), ptr<uint8_t>(hps_mask),
+                                 ptr<float>(hp_offset), ptr<int64_t>(hp_ind), ptr<int64_t>(hp_mask),
+                                 ptr<int32_t>(ocls), ptr<int32_t>(ocx), ptr<int32_t>(ocy), ptr<int32_t>(orad),
+                                 ptr<uint8_t>(oval), ptr<int32_t>(hcx), ptr<int32_t>(hcy), ptr<int32_t>(hrad),
+                                 ptr<uint8_t>(hval), ptr<void>(stream)),
+          "cnb_multi_pose_targets");
+  });
   m.def("dcnv2_workspace_bytes", &cnb_dcnv2_workspace_bytes);
   m.def("dcnv2_backward_workspace_bytes", &cnb_dcnv2_backward_workspace_bytes);
   m.def("dcnv2_backward_ex", [](P input, int in_cl, P offset, P mask, P weight, P gout, P gin, int gin_cl, P goff, P gmask,

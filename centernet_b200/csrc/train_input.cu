@@ -348,6 +348,113 @@ __global__ void __launch_bounds__(kThreads) k_ctdet_targets(
   }
 }
 
+// ---------------------------------------------------------------- multi_pose targets (multi_pose.py:104-160)
+// One thread per (image, slot), looping over the joints; the box half is k_ctdet_targets' arithmetic.  A slot gets
+// targets when (h > 0 && w > 0) || rotated; reg_mask is 1 only when it has a visible joint (num_kpts != 0: the
+// visibilities are finite and >= 0, checked on the host, so the float32 sum is 0 exactly when all are) and the
+// image is not rotated.  The centre list is "got targets": hm[cls, ct] = 0.9999 for num_kpts == 0 is overwritten
+// by the Gaussian's peak of 1 on the next line of the reference.
+__global__ void __launch_bounds__(kThreads) k_multi_pose_targets(
+    const float *__restrict__ boxes, const int *__restrict__ cls, const int *__restrict__ num_objs,
+    const float *__restrict__ kps, const unsigned char *__restrict__ flip, const unsigned char *__restrict__ rotated,
+    const int *__restrict__ src_hw, const double *__restrict__ trans, const double *__restrict__ trans_rot,
+    const int *__restrict__ perm, int nb, int m, int nj, int res, float *__restrict__ wh, long long *__restrict__ ind,
+    float *__restrict__ reg, unsigned char *__restrict__ reg_mask, float *__restrict__ hps,
+    unsigned char *__restrict__ hps_mask, float *__restrict__ hp_offset, long long *__restrict__ hp_ind,
+    long long *__restrict__ hp_mask, int *__restrict__ obj_cls, int *__restrict__ obj_cx, int *__restrict__ obj_cy,
+    int *__restrict__ obj_radius, unsigned char *__restrict__ obj_valid, int *__restrict__ hp_cx,
+    int *__restrict__ hp_cy, int *__restrict__ hp_radius, unsigned char *__restrict__ hp_valid) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)nb * m) return;
+  const int b = (int)(i / m), k = (int)(i % m);
+  const bool rot = rotated[b] != 0, fl = flip[b] != 0;
+  const float wd = (float)src_hw[2 * b + 1];
+  float w = 0.f, h = 0.f, rx = 0.f, ry = 0.f;
+  int c = 0, cx = 0, cy = 0, rad = 0;
+  bool valid = false, any_kpt = false;
+  if (k < min(num_objs[b], m)) {
+    const float *bb = boxes + i * 4;
+    float x0 = bb[0], y0 = bb[1], x1 = bb[2], y1 = bb[3];
+    if (fl) {   // bbox[[0, 2]] = width - bbox[[2, 0]] - 1 in float32
+      const float nx0 = __fsub_rn(__fsub_rn(wd, x1), 1.f), nx1 = __fsub_rn(__fsub_rn(wd, x0), 1.f);
+      x0 = nx0;
+      x1 = nx1;
+    }
+    const double *t = trans + 6 * b;
+    float p0 = affine_f32(t, x0, y0), q0 = affine_f32(t + 3, x0, y0);
+    float p1 = affine_f32(t, x1, y1), q1 = affine_f32(t + 3, x1, y1);
+    const float mx = (float)(res - 1);
+    p0 = fminf(fmaxf(p0, 0.f), mx);
+    p1 = fminf(fmaxf(p1, 0.f), mx);
+    q0 = fminf(fmaxf(q0, 0.f), mx);
+    q1 = fminf(fmaxf(q1, 0.f), mx);
+    h = __fsub_rn(q1, q0);
+    w = __fsub_rn(p1, p0);
+    if ((h > 0.f && w > 0.f) || rot) {
+      const double r = gaussian_radius_f64((long long)ceilf(h), (long long)ceilf(w));
+      rad = r > 0.0 ? (int)r : 0;   // max(0, int(radius))
+      const float ctx = __fdiv_rn(__fadd_rn(p0, p1), 2.f), cty = __fdiv_rn(__fadd_rn(q0, q1), 2.f);
+      cx = (int)ctx;
+      cy = (int)cty;
+      rx = __fsub_rn(ctx, (float)cx);
+      ry = __fsub_rn(cty, (float)cy);
+      c = cls[i];
+      valid = true;
+    } else {
+      w = h = 0.f;
+    }
+  }
+  const float *pk = kps + i * nj * 3;
+  const double *tr = trans_rot + 6 * b;
+  for (int j = 0; j < nj; ++j) {
+    const long long o = i * nj + j;                     // [b, k * nj + j] of hp_*, [b, k, j] of hps
+    const long long l = ((long long)b * nj + j) * m + k; // [b, j, k] of the joint lists
+    float hx = 0.f, hy = 0.f, ox = 0.f, oy = 0.f;
+    int jx = 0, jy = 0;
+    bool in = false;
+    if (valid) {
+      const float *q = pk + 3 * (fl ? perm[j] : j);
+      const float v = q[2];
+      any_kpt = any_kpt || v != 0.f;
+      if (v > 0.f) {
+        const float x = fl ? __fsub_rn(__fsub_rn(wd, q[0]), 1.f) : q[0];
+        const float px = affine_f32(tr, x, q[1]), py = affine_f32(tr + 3, x, q[1]);
+        if (px >= 0.f && px < (float)res && py >= 0.f && py < (float)res) {
+          in = true;
+          jx = (int)px;
+          jy = (int)py;
+          hx = __fsub_rn(px, (float)cx);
+          hy = __fsub_rn(py, (float)cy);
+          ox = __fsub_rn(px, (float)jx);
+          oy = __fsub_rn(py, (float)jy);
+        }
+      }
+    }
+    hps[2 * o] = hx;
+    hps[2 * o + 1] = hy;
+    hps_mask[2 * o] = hps_mask[2 * o + 1] = (in && !rot) ? 1 : 0;
+    hp_offset[2 * o] = ox;
+    hp_offset[2 * o + 1] = oy;
+    hp_ind[o] = in ? (long long)jy * res + jx : 0;
+    hp_mask[o] = in ? 1 : 0;
+    hp_cx[l] = jx;
+    hp_cy[l] = jy;
+    hp_radius[l] = in ? rad : 0;
+    hp_valid[l] = in ? 1 : 0;
+  }
+  wh[2 * i] = w;
+  wh[2 * i + 1] = h;
+  reg[2 * i] = rx;
+  reg[2 * i + 1] = ry;
+  ind[i] = valid ? (long long)cy * res + cx : 0;
+  reg_mask[i] = (valid && any_kpt && !rot) ? 1 : 0;
+  obj_cls[i] = c;
+  obj_cx[i] = cx;
+  obj_cy[i] = cy;
+  obj_radius[i] = rad;
+  obj_valid[i] = valid ? 1 : 0;
+}
+
 // Depth of the grey tree and the number of its levels combined per block of the grey pass.
 void grey_plan(int out_h, int out_w, int *depth, int *leaf_log) {
   *depth = pw_depth((long long)out_h * out_w);
@@ -433,6 +540,34 @@ extern "C" int cnb_ctdet_targets(const float *boxes, const int32_t *cls, const i
                                                  out_w, wh, (long long *)ind, reg, reg_mask, cat_spec_wh, cat_spec_mask,
                                                  obj_cls, obj_cx, obj_cy, obj_radius, obj_valid);
   CNB_CHECK_LAUNCH("cnb_ctdet_targets");
+  cnb::count_launch();
+  return CNB_OK;
+}
+
+extern "C" int cnb_multi_pose_targets(const float *boxes, const int32_t *cls, const int32_t *num_objs,
+                                      const float *kps, const uint8_t *flip, const uint8_t *rotated,
+                                      const int32_t *src_hw, const double *trans6, const double *trans_rot6,
+                                      const int32_t *flip_perm, int b, int m, int num_joints, int out_res, float *wh,
+                                      int64_t *ind, float *reg, uint8_t *reg_mask, float *hps, uint8_t *hps_mask,
+                                      float *hp_offset, int64_t *hp_ind, int64_t *hp_mask, int32_t *obj_cls,
+                                      int32_t *obj_cx, int32_t *obj_cy, int32_t *obj_radius, uint8_t *obj_valid,
+                                      int32_t *hp_cx, int32_t *hp_cy, int32_t *hp_radius, uint8_t *hp_valid,
+                                      void *stream) {
+  CNB_REQUIRE(boxes && cls && num_objs && kps && flip && rotated && src_hw && trans6 && trans_rot6 && flip_perm &&
+                  wh && ind && reg && reg_mask && hps && hps_mask && hp_offset && hp_ind && hp_mask && obj_cls &&
+                  obj_cx && obj_cy && obj_radius && obj_valid && hp_cx && hp_cy && hp_radius && hp_valid,
+              CNB_EINVAL, "cnb_multi_pose_targets: null pointer");
+  CNB_REQUIRE(b > 0 && m > 0 && num_joints > 0 && out_res > 0 && (long long)out_res * out_res <= INT32_MAX &&
+                  (long long)b * m * num_joints <= INT32_MAX,
+              CNB_EINVAL, "cnb_multi_pose_targets: bad shape (b = %d, m = %d, joints = %d, out_res = %d)", b, m,
+              num_joints, out_res);
+  const long long n = (long long)b * m;
+  cnb::k_multi_pose_targets<<<(unsigned)((n + cnb::kThreads - 1) / cnb::kThreads), cnb::kThreads, 0,
+                              (cudaStream_t)stream>>>(
+      boxes, cls, num_objs, kps, flip, rotated, src_hw, trans6, trans_rot6, flip_perm, b, m, num_joints, out_res, wh,
+      (long long *)ind, reg, reg_mask, hps, hps_mask, hp_offset, (long long *)hp_ind, (long long *)hp_mask, obj_cls,
+      obj_cx, obj_cy, obj_radius, obj_valid, hp_cx, hp_cy, hp_radius, hp_valid);
+  CNB_CHECK_LAUNCH("cnb_multi_pose_targets");
   cnb::count_launch();
   return CNB_OK;
 }

@@ -14,7 +14,11 @@ device does the per-pixel arithmetic and the target geometry:
 ('input', 'reg_mask', 'ind', 'wh' or 'cat_spec_wh' / 'cat_spec_mask', 'reg' with opt.reg_offset; 'hm' with
 dense_hm=True), plus the object lists FocalSplatLoss takes ('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius',
 'obj_valid').  `augment_images` is the image half alone, for explicit matrices, flips and colour parameters.
-The numeric contract is DESIGN.md section 4.9."""
+The numeric contract is DESIGN.md section 4.9.
+
+The multi_pose sampler (datasets/sample/multi_pose.py:29-183) works the same way: MultiPoseTrainInput,
+collate_multi_pose and build_multi_pose_batch, with the rotated crop, the keypoint targets, hm / hm_hp and the
+joint lists of FocalSplatLoss (DESIGN.md section 4.10)."""
 import itertools
 import os
 import random
@@ -44,17 +48,54 @@ def _get_border(border, size):
     return border // i
 
 
-def affine_transform(center, scale, output_size):
-    """get_affine_transform(center, scale, 0, output_size) (utils/image.py:27-60) as a 2x3 float64, to the bit.
+def affine_transform(center, scale, output_size, rot=0):
+    """get_affine_transform(center, scale, rot, output_size) (utils/image.py:27-60) as a 2x3 float64, to the bit.
     A scale that is not an array becomes a float32 pair as there; a float64 array scale (keep_res with a random
-    crop) keeps its float64 half-width, which the reference adds to the float32 centre in float64."""
+    crop) keeps its float64 half-width, which the reference adds to the float32 centre in float64.  get_dir turns
+    (0, -src_w / 2) by np.pi * rot / 180 in float64 (np.sin / np.cos, as there) and src[1] is the float64 sum
+    rounded to float32; rot = 0 gives the unrotated point exactly."""
     if not isinstance(scale, np.ndarray):
         scale = np.array([scale, scale], dtype=F32)
     src, dst = _affine_points(center, scale.astype(F32), output_size)
-    src[1, 1] = F32(np.float64(F32(center[1])) + np.float64(scale[0]) * -0.5)
+    rot_rad = np.pi * rot / 180
+    sn, cs = np.sin(rot_rad), np.cos(rot_rad)
+    half = np.float64(scale[0]) * -0.5                  # src_point = [0, src_w * -0.5]
+    src[1, 0] = F32(np.float64(F32(center[0])) + (0 * cs - half * sn))
+    src[1, 1] = F32(np.float64(F32(center[1])) + (0 * sn + half * cs))
     d = src[0] - src[1]
     src[2] = src[1] + np.array([-d[1], d[0]], F32)
     return cv_affine_transform(src, dst)
+
+
+def crop_draws(height, width, c, s, opt):
+    """The crop draws of the train split (ctdet.py:44-57, multi_pose.py:45-57): np.random.choice and two
+    randint, or the three randn of not_rand_crop.  Updates the float32 centre c in place; returns the scale."""
+    if not opt.not_rand_crop:
+        s = s * np.random.choice(np.arange(0.6, 1.4, 0.1))
+        w_border = _get_border(128, width)
+        h_border = _get_border(128, height)
+        c[0] = np.random.randint(low=w_border, high=width - w_border)
+        c[1] = np.random.randint(low=h_border, high=height - h_border)
+    else:
+        sf, cf = opt.scale, opt.shift
+        c[0] += s * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+        c[1] += s * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+        s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
+    return s
+
+
+def color_draws(data_rng, eig_val, eig_vec):
+    """color_aug's draws (utils/image.py:221-230): random.shuffle of its three functions, one data_rng.uniform
+    per blend in the order they run, then the lighting normal.  Returns (order code, blend [6] float32 (alpha,
+    1 - alpha) of brightness, contrast, saturation, light [3] float64)."""
+    blend = np.zeros(6, F32)
+    kinds = [0, 1, 2]
+    random.shuffle(kinds)
+    for k in kinds:
+        alpha = 1. + data_rng.uniform(low=-0.4, high=0.4)
+        blend[2 * k], blend[2 * k + 1] = F32(alpha), F32(1 - alpha)
+    light = np.dot(eig_vec, eig_val * data_rng.normal(scale=0.1, size=(3,)))
+    return ORDERS.index(tuple(kinds)), blend, np.asarray(light, np.float64)
 
 
 def sample_params(height, width, opt, split, data_rng, eig_val, eig_vec):
@@ -71,35 +112,19 @@ def sample_params(height, width, opt, split, data_rng, eig_val, eig_vec):
         input_h, input_w = opt.input_h, opt.input_w
     flipped = False
     if split == 'train':
-        if not opt.not_rand_crop:
-            s = s * np.random.choice(np.arange(0.6, 1.4, 0.1))
-            w_border = _get_border(128, width)
-            h_border = _get_border(128, height)
-            c[0] = np.random.randint(low=w_border, high=width - w_border)
-            c[1] = np.random.randint(low=h_border, high=height - h_border)
-        else:
-            sf, cf = opt.scale, opt.shift
-            c[0] += s * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
-            c[1] += s * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
-            s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
+        s = crop_draws(height, width, c, s, opt)
         if np.random.random() < opt.flip:
             flipped = True
             c[0] = width - c[0] - 1
     order, blend, light = -1, np.zeros(6, F32), np.zeros(3, np.float64)
     if split == 'train' and not opt.no_color_aug:
-        kinds = [0, 1, 2]
-        random.shuffle(kinds)                  # color_aug's random.shuffle of its three functions
-        for k in kinds:                        # one uniform per blend, in the order they run
-            alpha = 1. + data_rng.uniform(low=-0.4, high=0.4)
-            blend[2 * k], blend[2 * k + 1] = F32(alpha), F32(1 - alpha)
-        light = np.dot(eig_vec, eig_val * data_rng.normal(scale=0.1, size=(3,)))
-        order = ORDERS.index(tuple(kinds))
+        order, blend, light = color_draws(data_rng, eig_val, eig_vec)
     output_h, output_w = input_h // opt.down_ratio, input_w // opt.down_ratio
     return {'c': c, 's': s, 'flip': flipped, 'input_h': input_h, 'input_w': input_w,
             'output_h': output_h, 'output_w': output_w,
             'minv': np.array(_invert(affine_transform(c, s, [input_w, input_h])), np.float64),
             'trans_output': affine_transform(c, s, [output_w, output_h]).reshape(6),
-            'order': order, 'blend': blend, 'light': np.asarray(light, np.float64)}
+            'order': order, 'blend': blend, 'light': light}
 
 
 class CTDetTrainInput(torch.utils.data.Dataset):
@@ -315,4 +340,207 @@ def build_ctdet_batch(packed, device=None, dtype=torch.float32, memory_format=to
     if sc['reg_offset']:
         ret['reg'] = reg
     ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
+    return ret
+
+
+# ---------------------------------------------------------------- multi_pose (datasets/sample/multi_pose.py)
+def multi_pose_params(height, width, opt, split, data_rng, eig_val, eig_vec):
+    """The random draws of MultiPoseDataset.__getitem__ (multi_pose.py:39-75) for one height x width image, in the
+    reference's order -- crop draws, then ALWAYS one np.random.random() < aug_rot in the train split (a second
+    randn for the angle when it succeeds), the flip draw, color_aug -- and the three matrices they give:
+    trans_input (rotated; inverted for the warp), trans_output_rot (rotated, for the keypoints) and trans_output
+    (rot 0, for the boxes).  The input is input_res square (there is no keep_res branch)."""
+    c = np.array([width / 2., height / 2.], dtype=np.float32)
+    s = max(height, width) * 1.0
+    rot = 0
+    flipped = False
+    if split == 'train':
+        s = crop_draws(height, width, c, s, opt)
+        if np.random.random() < opt.aug_rot:
+            rf = opt.rotate
+            rot = np.clip(np.random.randn() * rf, -rf * 2, rf * 2)
+        if np.random.random() < opt.flip:
+            flipped = True
+            c[0] = width - c[0] - 1
+    order, blend, light = -1, np.zeros(6, F32), np.zeros(3, np.float64)
+    if split == 'train' and not opt.no_color_aug:
+        order, blend, light = color_draws(data_rng, eig_val, eig_vec)
+    res, out_res = int(opt.input_res), int(opt.output_res)
+    return {'c': c, 's': s, 'rot': rot, 'flip': flipped, 'input_res': res, 'output_res': out_res,
+            'minv': np.array(_invert(affine_transform(c, s, [res, res], rot)), np.float64),
+            'trans_output_rot': affine_transform(c, s, [out_res, out_res], rot).reshape(6),
+            'trans_output': affine_transform(c, s, [out_res, out_res]).reshape(6),
+            'order': order, 'blend': blend, 'light': light}
+
+
+class MultiPoseTrainInput(torch.utils.data.Dataset):
+    """Wraps a reference MultiPoseDataset instance (duck-typed on opt, coco, images, img_dir, max_objs,
+    num_classes, num_joints, flip_idx, mean, std, _data_rng, _eig_val, _eig_vec and split).  __getitem__ reads the
+    image, the annotations and their keypoints and draws the random parameters as the reference does; it does no
+    pixel work (collate_multi_pose + build_multi_pose_batch do).  The class is int(category_id) - 1, as there."""
+
+    def __init__(self, dataset):
+        opt = dataset.opt
+        if opt.mse_loss:
+            raise NotImplementedError("MultiPoseTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not "
+                                      "implemented")
+        if opt.dense_hp:
+            raise NotImplementedError("MultiPoseTrainInput: opt.dense_hp targets are not implemented")
+        self.dataset = dataset
+
+    def __len__(self):
+        return len(self.dataset)
+
+    def __getitem__(self, index):
+        import cv2
+        ds = self.dataset
+        img_id = ds.images[index]
+        file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
+        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
+        num_objs = min(len(anns), ds.max_objs)
+        img = cv2.imread(os.path.join(ds.img_dir, file_name))
+        sample = multi_pose_params(img.shape[0], img.shape[1], ds.opt, ds.split, ds._data_rng, ds._eig_val,
+                                   ds._eig_vec)
+        boxes = np.zeros((num_objs, 4), F32)
+        cls = np.zeros(num_objs, np.int64)
+        kps = []
+        for k in range(num_objs):
+            b = anns[k]['bbox']
+            boxes[k] = np.array([b[0], b[1], b[0] + b[2], b[1] + b[3]], dtype=np.float32)
+            cls[k] = int(anns[k]['category_id']) - 1
+            kps.append(np.array(anns[k]['keypoints'], np.float32).reshape(-1))
+        opt = ds.opt
+        sample.update(image=img, boxes=boxes, cls=cls, keypoints=kps, max_objs=ds.max_objs,
+                      num_classes=ds.num_classes, num_joints=ds.num_joints,
+                      flip_idx=[tuple(e) for e in ds.flip_idx], mean=np.asarray(ds.mean, F32).reshape(3),
+                      std=np.asarray(ds.std, F32).reshape(3), reg_offset=bool(opt.reg_offset),
+                      hm_hp=bool(opt.hm_hp), reg_hp_offset=bool(opt.reg_hp_offset))
+        return sample
+
+
+def flip_permutation(num_joints, flip_idx):
+    """The joint order after multi_pose.py:112-113's swaps: new joint j is old joint perm[j].  The swaps are
+    applied to arange(J) in order, so pairs that share a joint compose as they do there."""
+    perm = list(range(num_joints))
+    for a, b in flip_idx:
+        perm[a], perm[b] = perm[b], perm[a]
+    return np.array(perm, np.int32)
+
+
+def collate_multi_pose(samples):
+    """Packs MultiPoseTrainInput samples into one uint8 buffer: what collate_ctdet packs plus the keypoints
+    [B, M, J, 3] float32, both output matrices, a per-image rotated byte and the joint permutation of the flip.
+    Raises ValueError for input the target kernel cannot match or the reference cannot run: a keypoint list whose
+    length is not 3 J, a visibility that is negative or not finite, a class outside [0, num_classes), more than
+    128 slots, a rotated sample with a box of negative width or height, or samples of different settings."""
+    s0 = samples[0]
+    keys = ('input_res', 'output_res', 'max_objs', 'num_classes', 'num_joints', 'flip_idx', 'reg_offset', 'hm_hp',
+            'reg_hp_offset')
+    for s in samples:
+        if any(s[k] != s0[k] for k in keys):
+            raise ValueError("collate_multi_pose: samples with different settings cannot be batched")
+    images = [s['image'] for s in samples]
+    _check_images(images)
+    b, m, nj, nc = len(samples), int(s0['max_objs']), int(s0['num_joints']), int(s0['num_classes'])
+    if not 1 <= m <= 128:
+        raise ValueError("collate_multi_pose: 1 to 128 object slots (FocalSplatLoss / splat_gaussian), got %d" % m)
+    if nj < 1:
+        raise ValueError("collate_multi_pose: no joints")
+    perm = flip_permutation(nj, s0['flip_idx'])
+    boxes = np.zeros((b, m, 4), F32)
+    cls = np.zeros((b, m), np.int32)
+    kps = np.zeros((b, m, nj, 3), F32)
+    nobj = np.zeros(b, np.int32)
+    rotated = np.zeros(b, np.uint8)
+    for i, s in enumerate(samples):
+        n = min(len(s['boxes']), m)
+        nobj[i], rotated[i] = n, s['rot'] != 0
+        c = np.asarray(s['cls'][:n], np.int64)
+        if n and (c.min() < 0 or c.max() >= nc):
+            raise ValueError("collate_multi_pose: class id outside [0, %d)" % nc)
+        for k in range(n):
+            p = np.asarray(s['keypoints'][k], F32).reshape(-1)
+            if p.size != 3 * nj:
+                raise ValueError("collate_multi_pose: %d keypoint values, expected 3 x %d joints" % (p.size, nj))
+            kps[i, k] = p.reshape(nj, 3)
+        vis = kps[i, :n, :, 2]
+        if not (np.isfinite(vis).all() and (vis >= 0).all()):
+            raise ValueError("collate_multi_pose: keypoint visibilities must be finite and >= 0")
+        bx = np.asarray(s['boxes'][:n], F32).reshape(n, 4)
+        if rotated[i] and ((bx[:, 2] < bx[:, 0]) | (bx[:, 3] < bx[:, 1])).any():
+            raise ValueError("collate_multi_pose: a box with negative width or height in a rotated sample "
+                             "(gaussian_radius of it is NaN in the reference)")
+        boxes[i, :n], cls[i, :n] = bx, c
+    pk = _Packer()
+    _pack_images(pk, images, [s['minv'] for s in samples], [s['flip'] for s in samples],
+                 [s['order'] for s in samples], [s['blend'] for s in samples], [s['light'] for s in samples],
+                 s0['mean'], s0['std'])
+    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
+    pk.add('trans_output_rot', np.array([s['trans_output_rot'] for s in samples], np.float64).reshape(b, 6))
+    pk.add('nobj', nobj)
+    pk.add('boxes', boxes)
+    pk.add('cls', cls)
+    pk.add('kps', kps)
+    pk.add('rotated', rotated)
+    pk.add('perm', perm)
+    scalars = {k: s0[k] for k in ('input_res', 'output_res', 'max_objs', 'num_classes', 'num_joints', 'reg_offset',
+                                  'hm_hp', 'reg_hp_offset')}
+    scalars.update(batch=b, color=any(s['order'] >= 0 for s in samples), rotated=rotated.astype(bool).tolist())
+    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+
+
+def build_multi_pose_batch(packed, device=None, dtype=torch.float32, memory_format=torch.contiguous_format,
+                           dense_hm=False):
+    """The reference's collated multi_pose batch, on the device, from a collate_multi_pose result: one
+    non-blocking H2D copy on the current stream, the image pass at input_res x input_res and the target kernel,
+    plus splat_gaussian with dense_hm.  Keys, shapes and dtypes as multi_pose.py:161-177 returns them: input,
+    reg_mask u8, ind i64, wh, hps f32 [B,M,2J], hps_mask u8; reg with reg_offset; hp_offset f32 [B,M*J,2], hp_ind
+    i64, hp_mask i64 with reg_hp_offset; hm [B,C,R,R] and, with hm_hp, hm_hp [B,J,R,R] only with dense_hm.  Always
+    the FocalSplatLoss lists of the centres, obj_cls / obj_cx / obj_cy / obj_radius (int32) and obj_valid (uint8)
+    [B,M], and with hm_hp those of the joints, hp_cx / hp_cy / hp_radius (int32) and hp_valid (uint8) [B,J,M]: as
+    [B*J, M] views with class 0 they give hm_hp as [B*J, 1, R, R].  The reference fills hm of a rotated image
+    with 0.9999, which no list expresses: dense_hm=False with a rotated sample raises ValueError.  The packed host
+    buffer is not modified."""
+    sc = packed['scalars']
+    if not dense_hm and any(sc['rotated']):
+        raise ValueError("build_multi_pose_batch: a rotated sample's hm is the constant 0.9999, which the object "
+                         "lists cannot express; use dense_hm=True")
+    dev = _device(device)
+    b, m, nj, nc, r = sc['batch'], sc['max_objs'], sc['num_joints'], sc['num_classes'], sc['output_res']
+    buf = packed['buffer'].to(dev, non_blocking=True)
+    v = _views(buf, packed['layout'])
+    inp = _launch_images(v, b, sc['input_res'], sc['input_res'], sc['color'], dtype, memory_format, dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    u8 = dict(dtype=torch.uint8, device=dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    i64 = dict(dtype=torch.int64, device=dev)
+    wh, reg = torch.empty((b, m, 2), **f32), torch.empty((b, m, 2), **f32)
+    ind, reg_mask = torch.empty((b, m), **i64), torch.empty((b, m), **u8)
+    hps, hps_mask = torch.empty((b, m, 2 * nj), **f32), torch.empty((b, m, 2 * nj), **u8)
+    hp_offset, hp_ind, hp_mask = torch.empty((b, m * nj, 2), **f32), torch.empty((b, m * nj), **i64), \
+        torch.empty((b, m * nj), **i64)
+    lists = [torch.empty((b, m), **i32) for _ in range(4)] + [torch.empty((b, m), **u8)]
+    hp_lists = [torch.empty((b, nj, m), **i32) for _ in range(3)] + [torch.empty((b, nj, m), **u8)]
+    C.multi_pose_targets(ptr(v['boxes']), ptr(v['cls']), ptr(v['nobj']), ptr(v['kps']), ptr(v['flip']),
+                         ptr(v['rotated']), ptr(v['src_hw']), ptr(v['trans_output']), ptr(v['trans_output_rot']),
+                         ptr(v['perm']), b, m, nj, r, ptr(wh), ptr(ind), ptr(reg), ptr(reg_mask), ptr(hps),
+                         ptr(hps_mask), ptr(hp_offset), ptr(hp_ind), ptr(hp_mask), *[ptr(t) for t in lists],
+                         *[ptr(t) for t in hp_lists], stream_ptr(wh))
+    ret = {'input': inp}
+    if dense_hm:
+        hm = splat_gaussian(*lists, nc, r, r)
+        if any(sc['rotated']):   # hm * 0 + 0.9999 (multi_pose.py:157-158), from the device copy of the flags
+            hm.masked_fill_(v['rotated'].view(b, 1, 1, 1).bool(), F32(0.9999).item())
+        ret['hm'] = hm
+    ret.update(reg_mask=reg_mask, ind=ind, wh=wh, hps=hps, hps_mask=hps_mask)
+    if sc['reg_offset']:
+        ret['reg'] = reg
+    if dense_hm and sc['hm_hp']:
+        flat = [t.view(b * nj, m) for t in hp_lists]
+        ret['hm_hp'] = splat_gaussian(torch.zeros_like(flat[0]), *flat, 1, r, r).view(b, nj, r, r)
+    if sc['reg_hp_offset']:
+        ret.update(hp_offset=hp_offset, hp_ind=hp_ind, hp_mask=hp_mask)
+    ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
+    if sc['hm_hp']:
+        ret.update(zip(('hp_cx', 'hp_cy', 'hp_radius', 'hp_valid'), hp_lists))
     return ret

@@ -743,7 +743,25 @@ int cnb_preprocess_image_f32(const uint8_t *image_hwc, int h, int w, const doubl
  * u8 = 1, cat_spec_wh [b,m,2*num_classes] f32 / cat_spec_mask u8 (both NULL to skip) and the FocalSplatLoss
  * lists obj_cls / obj_cx / obj_cy / obj_radius i32 and obj_valid u8 [b,m] (ct_int, max(0, int(gaussian_radius(
  * ceil(h), ceil(w)))) in float64, reg_mask); every other slot is zero.  Errors, checked before any CUDA call:
- * CNB_EINVAL for a null pointer, only one of the cat_spec pair or a bad shape. */
+ * CNB_EINVAL for a null pointer, only one of the cat_spec pair or a bad shape.
+ *
+ * cnb_multi_pose_targets: multi_pose.py:104-160 for m = max_objs slots per image and J = num_joints, one thread per
+ * (image, slot) looping over the joints, R = out_res.  Slot k < min(num_objs[b], m) holds the float32 corners
+ * boxes[b, k] (as cnb_ctdet_targets), the class cls[b, k] and the keypoints kps[b, k] [J, 3] (x, y, visibility,
+ * float32; visibilities finite and >= 0).  When flip[b] != 0 the box and every joint's x are mirrored (width -
+ * x - 1 in float32, width src_hw[b][1]) and new joint j is old joint flip_perm[j].  The box goes through the
+ * FORWARD trans6[b] (rot 0) and is clipped to [0, R - 1]; the slot gets targets when (h > 0 && w > 0) or
+ * rotated[b] != 0: wh [b,m,2] f32, ind [b,m] i64 = ct_int.y R + ct_int.x, reg [b,m,2] f32 = ct - ct_int and the
+ * centre lists obj_cls / obj_cx / obj_cy / obj_radius i32 and obj_valid u8 = 1 [b,m] (radius max(0, int(
+ * gaussian_radius(ceil(h), ceil(w)))) in float64); reg_mask [b,m] u8 = 1 only when some visibility is non-zero
+ * and the image is not rotated.  Each joint with visibility > 0 is mapped by trans_rot6[b] (float64 t0 x + t1 y +
+ * t2 rounded to float32) and counts when 0 <= x < R and 0 <= y < R: hps [b,m,2J] f32 = pt - ct_int, hps_mask
+ * [b,m,2J] u8 = 1 on both entries unless rotated, hp_offset [b,m*J,2] f32 = pt - pt_int, hp_ind [b,m*J] i64 =
+ * pt_int.y R + pt_int.x, hp_mask [b,m*J] i64 = 1 (kept on rotated images, as there), and the joint lists hp_cx /
+ * hp_cy / hp_radius i32, hp_valid u8 [b,J,m] (pt_int and the slot's radius), a [b*J, m] list of class 0 that
+ * splat_gaussian / FocalSplatLoss read as hm_hp [b*J, 1, R, R].  Differences float32 - int32 are one rounding of
+ * the exact difference.  Every other entry is zero.  No atomics: the output is identical run to run.  Errors,
+ * checked before any CUDA call: CNB_EINVAL for a null pointer or a bad shape. */
 #define CNB_TRAIN_MAX_PIXELS 4194304
 size_t cnb_train_images_workspace_bytes(int b, int out_h, int out_w);
 int cnb_train_images(const uint8_t *src, const int64_t *src_off, const int32_t *src_hw, const double *minv6,
@@ -755,6 +773,13 @@ int cnb_ctdet_targets(const float *boxes, const int32_t *cls, const int32_t *num
                       int out_w, float *wh, int64_t *ind, float *reg, uint8_t *reg_mask, float *cat_spec_wh,
                       uint8_t *cat_spec_mask, int32_t *obj_cls, int32_t *obj_cx, int32_t *obj_cy,
                       int32_t *obj_radius, uint8_t *obj_valid, void *stream);
+int cnb_multi_pose_targets(const float *boxes, const int32_t *cls, const int32_t *num_objs, const float *kps,
+                           const uint8_t *flip, const uint8_t *rotated, const int32_t *src_hw, const double *trans6,
+                           const double *trans_rot6, const int32_t *flip_perm, int b, int m, int num_joints,
+                           int out_res, float *wh, int64_t *ind, float *reg, uint8_t *reg_mask, float *hps,
+                           uint8_t *hps_mask, float *hp_offset, int64_t *hp_ind, int64_t *hp_mask, int32_t *obj_cls,
+                           int32_t *obj_cx, int32_t *obj_cy, int32_t *obj_radius, uint8_t *obj_valid, int32_t *hp_cx,
+                           int32_t *hp_cy, int32_t *hp_radius, uint8_t *hp_valid, void *stream);
 
 #ifdef __cplusplus
 }

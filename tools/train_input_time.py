@@ -1,7 +1,7 @@
-"""Device time per ctdet training batch (centernet_b200.train_input), the host->device bytes per image against the
-reference loader's, and the numpy oracle's CPU time per image.
+"""Device time per ctdet or multi_pose training batch (centernet_b200.train_input), the host->device bytes per image
+against the reference loader's, and (ctdet) the numpy oracle's CPU time per image.
 
-    python tools/train_input_time.py [--iters 50]
+    python tools/train_input_time.py [--iters 50] [--sampler ctdet|multi_pose]
 
 Synthetic COCO-sized sources (ragged 640x480 / 480x640 / 500x375 / 427x640), 512x512 input, 80 classes, 128
 object slots, about 7 objects per image, colour augmentation on; B = 32, 64 and 114.  Per batch it times, with
@@ -9,7 +9,13 @@ CUDA events over --iters batches after a warm-up, build_ctdet_batch (H2D copy of
 kernels + targets) with and without the dense hm, and the same from a buffer already on the device (kernels
 only).  The reference's loader is not part of the repository, so the host-side figure is the numpy oracle
 (tests/train_np.py: warp, color_aug, normalisation, targets, hm splat) on one core: a stand-in for the per-pixel
-work this moves off the host, not a measurement of cv2.  Prints one JSON line."""
+work this moves off the host, not a measurement of cv2.
+
+--sampler multi_pose: the same sources at 512x512 input, 17 joints, 32 slots, about 7 people per image with
+random joint visibilities, colour augmentation on; B = 32 and 64, with aug_rot 0 and 1 (every image rotated, up to
++-60 degrees), each timed as build_multi_pose_batch with the H2D copy, from a buffer already on the device, and
+per image; with dense hm / hm_hp and, for aug_rot 0, without (a rotated batch needs the dense hm).  Prints one
+JSON line, with the card's name and power limit read in the same run."""
 import argparse
 import json
 import os
@@ -26,6 +32,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from centernet_b200 import train_input as T  # noqa: E402
+import multi_pose_train_cases as MC  # noqa: E402
 import train_cases as TC  # noqa: E402
 
 SIZES = [(480, 640), (640, 480), (375, 500), (640, 427), (427, 640), (333, 500)]
@@ -50,14 +57,39 @@ def make_samples(b, seed):
     return out
 
 
-def time_batches(packed, iters, dense_hm):
+def make_pose_samples(b, seed, aug_rot):
+    case = dict(MC.CASES["mp_coco"], aug_rot=aug_rot, rotate=30.0)
+    opt = MC.make_opt(case)
+    rng = np.random.default_rng(seed)
+    np.random.seed(seed); random.seed(seed)
+    data_rng = np.random.RandomState(seed)
+    out = []
+    for i in range(b):
+        h, w = SIZES[i % len(SIZES)]
+        s = T.multi_pose_params(h, w, opt, 'train', data_rng, MC.EIG_VAL, MC.EIG_VEC)
+        n = int(rng.integers(1, 15))
+        x0, y0 = rng.uniform(0, w, n), rng.uniform(0, h, n)
+        bw, bh = rng.uniform(4, 200, n), rng.uniform(4, 200, n)
+        boxes = np.stack([x0, y0, x0 + bw, y0 + bh], 1).astype(np.float32)
+        kps = [np.stack([x0[k] + rng.uniform(-0.2, 1.2, 17) * bw[k], y0[k] + rng.uniform(-0.2, 1.2, 17) * bh[k],
+                         rng.choice([0., 1., 2.], 17)], 1).astype(np.float32).reshape(-1) for k in range(n)]
+        s.update(image=rng.integers(0, 256, (h, w, 3), dtype=np.uint8), boxes=boxes, cls=np.zeros(n, np.int64),
+                 keypoints=kps, max_objs=32, num_classes=1, num_joints=17,
+                 flip_idx=[tuple(e) for e in MC.COCO_FLIP_IDX], mean=MC.MEAN, std=MC.STD, reg_offset=True,
+                 hm_hp=True, reg_hp_offset=True)
+        out.append(s)
+    return out
+
+
+def time_batches(packed, iters, dense_hm, build=None):
+    build = build or T.build_ctdet_batch
     for _ in range(3):
-        T.build_ctdet_batch(packed, dense_hm=dense_hm)
+        build(packed, dense_hm=dense_hm)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(iters):
-        T.build_ctdet_batch(packed, dense_hm=dense_hm)
+        build(packed, dense_hm=dense_hm)
     e1.record()
     torch.cuda.synchronize()
     return e0.elapsed_time(e1) / iters
@@ -86,13 +118,40 @@ def gpu_info():
         return torch.cuda.get_device_name()
 
 
+def main_multi_pose(iters):
+    # the reference's per-image transfer: input, hm, hm_hp and the targets of multi_pose.py:161-177
+    m, j, r = 32, 17, 128
+    ref_bytes = 3 * 512 * 512 * 4 + (1 + j) * r * r * 4 + m * (1 + 8 + 2 * 4 + 2 * 4 + 2 * j * 4 + 2 * j) \
+        + m * j * (2 * 4 + 8 + 8)
+    res = {"gpu": gpu_info(), "sampler": "multi_pose", "batches": {}}
+    build = T.build_multi_pose_batch
+    for b in (32, 64):
+        for aug_rot in (0.0, 1.0):
+            packed = T.collate_multi_pose(make_pose_samples(b, b, aug_rot))
+            on_device = dict(packed, buffer=packed['buffer'].cuda())
+            rr = {"rotated_images": int(sum(packed['scalars']['rotated'])),
+                  "ms_per_batch_dense": time_batches(packed, iters, True, build),
+                  "ms_per_batch_dense_kernels_only": time_batches(on_device, iters, True, build),
+                  "h2d_bytes_per_image": packed['buffer'].numel() / b, "reference_h2d_bytes_per_image": ref_bytes}
+            rr["us_per_image_dense"] = rr["ms_per_batch_dense"] * 1e3 / b
+            if aug_rot == 0:
+                rr["ms_per_batch_lists"] = time_batches(packed, iters, False, build)
+                rr["ms_per_batch_lists_kernels_only"] = time_batches(on_device, iters, False, build)
+                rr["us_per_image_lists"] = rr["ms_per_batch_lists"] * 1e3 / b
+            res["batches"]["B%d_aug_rot%g" % (b, aug_rot)] = rr
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--oracle-images", type=int, default=4)
+    ap.add_argument("--sampler", choices=("ctdet", "multi_pose"), default="ctdet")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("train_input_time: needs a CUDA device (no CPU timing is reported)")
+    if args.sampler == "multi_pose":
+        return main_multi_pose(args.iters)
     res = {"gpu": gpu_info(), "batches": {}}
     ref_bytes = 3 * 512 * 512 * 4 + 80 * 128 * 128 * 4 + 128 * (2 * 4 + 2 * 4 + 8 + 1)
     for b in (32, 64, 114):
