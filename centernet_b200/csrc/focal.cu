@@ -20,6 +20,7 @@
 #include <stdlib.h>
 #include <type_traits>
 #include "common.cuh"
+#include "gauss.cuh"
 
 namespace cnb {
 
@@ -40,13 +41,6 @@ __device__ __forceinline__ double2 *focal_partials(FocalAcc *acc) {
 }
 
 struct Obj { int x, y, r; };
-
-__device__ __forceinline__ float gauss_value(int dx, int dy, int r) {
-  // gaussian2D (utils/image.py:118-124) in float64, cast to fp32 like np.maximum(..., out=fp32 map)
-  // d2 in float64 (exact, as in numpy): with the centre outside the map |dx| may exceed the map size
-  const double sigma = (double)(2 * r + 1) / 6.0;
-  return (float)exp(-((double)dx * dx + (double)dy * dy) / (2.0 * sigma * sigma));
-}
 
 // Gaussian tables (shared memory).  exp(-(dx^2+dy^2)/(2 sigma^2)) depends on d2 = dx^2 + dy^2 only, so every
 // object gets a table over d2 in [0, 2 r^2] -- about half the size of its (2r+1)^2 window -- filled once per

@@ -413,6 +413,22 @@ PYBIND11_MODULE(_C, m) {
                                  ptr<uint8_t>(hval), ptr<void>(stream)),
           "cnb_multi_pose_targets");
   });
+  m.def("ddd_targets", [](P boxes, P cls, P nobj, P alpha, P depth, P dim, P aug, P trans, int b, int mm, int nc,
+                          int oh, int ow, int rect_mask, P hm, P dep, P dim_out, P ind, P rotbin, P rotres, P reg_mask,
+                          P rot_mask, P wh, P reg, P stream) {
+    check(cnb_ddd_targets(ptr<const float>(boxes), ptr<const int32_t>(cls), ptr<const int32_t>(nobj),
+                          ptr<const double>(alpha), ptr<const float>(depth), ptr<const float>(dim),
+                          ptr<const uint8_t>(aug), ptr<const double>(trans), b, mm, nc, oh, ow, rect_mask,
+                          ptr<float>(hm), ptr<float>(dep), ptr<float>(dim_out), ptr<int64_t>(ind),
+                          ptr<int64_t>(rotbin), ptr<float>(rotres), ptr<uint8_t>(reg_mask), ptr<uint8_t>(rot_mask),
+                          ptr<float>(wh), ptr<float>(reg), ptr<void>(stream)),
+          "cnb_ddd_targets");
+  });
+  m.def("ddd_gaussian_radius", [](P h, P w, int n, P radius, P stream) {
+    check(cnb_ddd_gaussian_radius(ptr<const float>(h), ptr<const float>(w), n, ptr<int32_t>(radius),
+                                  ptr<void>(stream)),
+          "cnb_ddd_gaussian_radius");
+  });
   m.def("dcnv2_workspace_bytes", &cnb_dcnv2_workspace_bytes);
   m.def("dcnv2_backward_workspace_bytes", &cnb_dcnv2_backward_workspace_bytes);
   m.def("dcnv2_backward_ex", [](P input, int in_cl, P offset, P mask, P weight, P gout, P gin, int gin_cl, P goff, P gmask,

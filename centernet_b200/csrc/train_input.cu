@@ -2,10 +2,12 @@
 // the random crop / flip warp, /255, color_aug, the normalisation and the layout change of a whole batch of
 // ragged uint8 sources, and the ctdet regression targets plus the object lists of FocalSplatLoss.  Every value
 // is the one the reference's loader computes for the same drawn parameters, bit for bit; no atomics, so the
-// output is also identical run to run.  The numeric contract is DESIGN.md section 4.9.
+// output is also identical run to run.  The numeric contract is DESIGN.md section 4.9.  The multi_pose and ddd
+// targets (sections 4.10 and 4.11) reuse the warp and the box arithmetic.
 #include <map>
 
 #include "common.cuh"
+#include "gauss.cuh"
 #include "warp.cuh"
 
 namespace cnb {
@@ -455,6 +457,283 @@ __global__ void __launch_bounds__(kThreads) k_multi_pose_targets(
   obj_valid[i] = valid ? 1 : 0;
 }
 
+// ---------------------------------------------------------------- ddd targets and heat map (ddd.py:86-140)
+// ddd calls gaussian_radius((h, w)) on float32 numpy scalars: every operation is float32 (NEP 50), the Python
+// constants rounded to float32 at each use, and b ** 2 is numpy's float32 scalar power, i.e. the C library's
+// powf(b, 2), which is NOT always the rounded b * b.  powf_sq restates glibc's powf (ARM optimized-routines: a
+// 16-entry log2 table and a degree-5 polynomial, then a 32-entry exp2 table and a cubic, in float64 with the fused
+// multiply-adds of its FMA build) for y = 2.
+__constant__ double kPowfInvc[16] = {
+    0x1.661ec79f8f3bep+0, 0x1.571ed4aaf883dp+0, 0x1.49539f0f010b0p+0, 0x1.3c995b0b80385p+0,
+    0x1.30d190c8864a5p+0, 0x1.25e227b0b8ea0p+0, 0x1.1bb4a4a1a343fp+0, 0x1.12358f08ae5bap+0,
+    0x1.0953f419900a7p+0, 0x1.0000000000000p+0, 0x1.e608cfd9a47acp-1, 0x1.ca4b31f026aa0p-1,
+    0x1.b2036576afce6p-1, 0x1.9c2d163a1aa2dp-1, 0x1.886e6037841edp-1, 0x1.767dcf5534862p-1};
+__constant__ double kPowfLogc[16] = {
+    -0x1.efec65b963019p-2, -0x1.b0b6832d4fca4p-2, -0x1.7418b0a1fb77bp-2, -0x1.39de91a6dcf7bp-2,
+    -0x1.01d9bf3f2b631p-2, -0x1.97c1d1b3b7af0p-3, -0x1.2f9e393af3c9fp-3, -0x1.960cbbf788d5cp-4,
+    -0x1.a6f9db6475fcep-5, 0x0.0p+0,               0x1.338ca9f24f53dp-4,  0x1.476a9543891bap-3,
+    0x1.e840b4ac4e4d2p-3,  0x1.40645f0c6651cp-2,  0x1.88e9c2c1b9ff8p-2,  0x1.ce0a44eb17bccp-2};
+__constant__ unsigned long long kExp2fTab[32] = {
+    0x3ff0000000000000ull, 0x3fefd9b0d3158574ull, 0x3fefb5586cf9890full, 0x3fef9301d0125b51ull,
+    0x3fef72b83c7d517bull, 0x3fef54873168b9aaull, 0x3fef387a6e756238ull, 0x3fef1e9df51fdee1ull,
+    0x3fef06fe0a31b715ull, 0x3feef1a7373aa9cbull, 0x3feedea64c123422ull, 0x3feece086061892dull,
+    0x3feebfdad5362a27ull, 0x3feeb42b569d4f82ull, 0x3feeab07dd485429ull, 0x3feea47eb03a5585ull,
+    0x3feea09e667f3bcdull, 0x3fee9f75e8ec5f74ull, 0x3feea11473eb0187ull, 0x3feea589994cce13ull,
+    0x3feeace5422aa0dbull, 0x3feeb737b0cdc5e5ull, 0x3feec49182a3f090ull, 0x3feed503b23e255dull,
+    0x3feee89f995ad3adull, 0x3feeff76f2fb5e47ull, 0x3fef199bdd85529cull, 0x3fef3720dcef9069ull,
+    0x3fef5818dcfba487ull, 0x3fef7c97337b9b5full, 0x3fefa4afa2a490daull, 0x3fefd0765b6e4540ull};
+
+__device__ __forceinline__ float powf_sq(float x) {
+  unsigned int ix = __float_as_uint(x) & 0x7fffffffu;   // (-x) ** 2 == x ** 2: the even-integer y path
+  if (ix == 0u) return 0.f;
+  if (ix < 0x00800000u) ix = (__float_as_uint(__fmul_rn(__uint_as_float(ix), 0x1p23f)) & 0x7fffffffu) - (23u << 23);
+  // log2(x): x = 2^k z with z in [0x3f330000, 2 * 0x3f330000), log2(z) = log2(c) + log2(z / c)
+  const unsigned int tmp = ix - 0x3f330000u;
+  const int i = (int)((tmp >> 19) & 15u);
+  const unsigned int top = tmp & 0xff800000u;
+  const int k = (int)top >> 23;
+  const double z = (double)__uint_as_float(ix - top);
+  const double r = __fma_rn(z, kPowfInvc[i], -1.0);
+  const double y0 = __dadd_rn(kPowfLogc[i], (double)k);
+  const double r2 = __dmul_rn(r, r);
+  double y = __fma_rn(0x1.27616c9496e0bp-2, r, -0x1.71969a075c67ap-2);
+  const double p = __fma_rn(0x1.ec70a6ca7baddp-2, r, -0x1.7154748bef6c8p-1);
+  const double r4 = __dmul_rn(r2, r2);
+  double q = __fma_rn(0x1.71547652ab82bp+0, r, y0);
+  q = __fma_rn(p, r2, q);
+  y = __fma_rn(y, r4, q);
+  const double xd = __dmul_rn(2.0, y);   // y * log2(x)
+  if (xd > 0x1.fffffffd1d571p+6) return __int_as_float(0x7f800000);
+  if (xd <= -150.0) return 0.f;
+  // exp2(xd) = 2^(ki / 32) 2^rr
+  double kd = __dadd_rn(xd, 0x1.8p+47);
+  const unsigned long long ki = (unsigned long long)__double_as_longlong(kd);
+  kd = __dsub_rn(kd, 0x1.8p+47);
+  const double rr = __dsub_rn(xd, kd);
+  const double s = __longlong_as_double((long long)(kExp2fTab[ki & 31] + (ki << 47)));
+  const double zz = __fma_rn(0x1.c6af84b912394p-5, rr, 0x1.ebfce50fac4f3p-3);
+  const double rr2 = __dmul_rn(rr, rr);
+  double e = __fma_rn(0x1.62e42ff0c52d6p-1, rr, 1.0);
+  e = __fma_rn(zz, rr2, e);
+  return __double2float_rn(__dmul_rn(e, s));
+}
+
+// gaussian_radius((h, w)) of utils/image.py:95-115 on float32 h, w, in numpy's left-to-right order; min(r1, r2, r3)
+// is Python's min (the first smallest).
+__device__ __forceinline__ float gaussian_radius_f32(float h, float w) {
+  const float b1 = __fadd_rn(h, w);
+  const float c1 = __fdiv_rn(__fmul_rn(__fmul_rn(w, h), 0.3f), 1.7f);
+  const float r1 = __fdiv_rn(__fadd_rn(b1, __fsqrt_rn(__fsub_rn(powf_sq(b1), __fmul_rn(4.f, c1)))), 2.f);
+  const float b2 = __fmul_rn(2.f, __fadd_rn(h, w));
+  const float c2 = __fmul_rn(__fmul_rn(0.3f, w), h);
+  const float r2 = __fdiv_rn(__fadd_rn(b2, __fsqrt_rn(__fsub_rn(powf_sq(b2), __fmul_rn(16.f, c2)))), 2.f);
+  const float b3 = __fmul_rn(-1.4f, __fadd_rn(h, w));
+  const float c3 = __fmul_rn(__fmul_rn(-0.3f, w), h);
+  const float r3 = __fdiv_rn(__fadd_rn(b3, __fsqrt_rn(__fsub_rn(powf_sq(b3), __fmul_rn(11.2f, c3)))), 2.f);
+  float m = r1;
+  if (r2 < m) m = r2;
+  if (r3 < m) m = r3;
+  return m;
+}
+
+// max(0, int(radius)); NaN (never for h, w > 0) gives 0.
+__device__ __forceinline__ int ddd_radius(float h, float w) {
+  const float r = gaussian_radius_f32(h, w);
+  return r >= 1.f ? (int)r : 0;
+}
+
+// One slot of ddd.py:86-140 for an image: what the targets and hm both read, so they cannot disagree.
+struct DddSlot {
+  int kind;                 // 0 nothing (empty, cls <= -99, h or w <= 0), 1 positive, 2 ignore
+  int cls;                  // the positive class, the ignore class, or -1 for all classes
+  bool gauss;               // draws draw_umich_gaussian(hm[cls], ct, r)
+  int cx, cy, r;            // ct_int and the radius
+  int ox0, oy0, ox1, oy1;   // then hm[cls, oy0:oy1 + 1, ox0:ox1 + 1] = 0.9999 (empty when ox0 > ox1)
+  float ctx, cty, w, h;
+};
+
+__device__ __forceinline__ DddSlot ddd_slot(const float *bb, int cls, const double *t, int num_classes, int oh, int ow,
+                                            bool rect_mask) {
+  DddSlot s;
+  s.kind = 0;
+  s.cls = 0;
+  s.gauss = false;
+  s.cx = s.cy = s.r = 0;
+  s.ox0 = 0;
+  s.ox1 = -1;
+  s.oy0 = 0;
+  s.oy1 = -1;
+  s.ctx = s.cty = s.w = s.h = 0.f;
+  const bool pos = cls >= 0 && cls < num_classes;
+  const bool ign = cls == -1 || (cls <= -2 && cls >= -num_classes - 1);
+  if (!pos && !ign) return s;
+  float p0 = affine_f32(t, bb[0], bb[1]), q0 = affine_f32(t + 3, bb[0], bb[1]);
+  float p1 = affine_f32(t, bb[2], bb[3]), q1 = affine_f32(t + 3, bb[2], bb[3]);
+  const float xm = (float)(ow - 1), ym = (float)(oh - 1);
+  p0 = fminf(fmaxf(p0, 0.f), xm);
+  p1 = fminf(fmaxf(p1, 0.f), xm);
+  q0 = fminf(fmaxf(q0, 0.f), ym);
+  q1 = fminf(fmaxf(q1, 0.f), ym);
+  const float h = __fsub_rn(q1, q0), w = __fsub_rn(p1, p0);
+  if (!(h > 0.f && w > 0.f)) return s;
+  s.h = h;
+  s.w = w;
+  s.r = ddd_radius(h, w);
+  s.ctx = __fdiv_rn(__fadd_rn(p0, p1), 2.f);
+  s.cty = __fdiv_rn(__fadd_rn(q0, q1), 2.f);
+  s.cx = (int)s.ctx;
+  s.cy = (int)s.cty;
+  if (pos) {
+    s.kind = 1;
+    s.cls = cls;
+    s.gauss = true;
+  } else {
+    s.kind = 2;
+    s.cls = cls == -1 ? -1 : -cls - 2;
+    if (rect_mask) {   // hm[ignore_id, int(y0):int(y1) + 1, int(x0):int(x1) + 1] = 0.9999
+      s.ox0 = (int)p0;
+      s.ox1 = (int)p1;
+      s.oy0 = (int)q0;
+      s.oy1 = (int)q1;
+    } else {           // the Gaussian, then hm[ignore_id, ct_int.y, ct_int.x] = 0.9999
+      s.gauss = true;
+      s.ox0 = s.ox1 = s.cx;
+      s.oy0 = s.oy1 = s.cy;
+    }
+  }
+  return s;
+}
+
+constexpr double kPi = 3.141592653589793;
+
+__global__ void __launch_bounds__(kThreads) k_ddd_targets(
+    const float *__restrict__ boxes, const int *__restrict__ cls, const int *__restrict__ num_objs,
+    const double *__restrict__ alpha, const float *__restrict__ depth, const float *__restrict__ dim,
+    const unsigned char *__restrict__ aug, const double *__restrict__ trans, int nb, int m, int num_classes, int oh,
+    int ow, int rect_mask, float *__restrict__ dep, float *__restrict__ dim_out,
+    long long *__restrict__ ind, long long *__restrict__ rotbin, float *__restrict__ rotres,
+    unsigned char *__restrict__ reg_mask, unsigned char *__restrict__ rot_mask, float *__restrict__ wh,
+    float *__restrict__ reg) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)nb * m) return;
+  const int b = (int)(i / m), k = (int)(i % m);
+  DddSlot s;
+  s.kind = 0;
+  if (k < min(num_objs[b], m))
+    s = ddd_slot(boxes + i * 4, cls[i], trans + 6 * b, num_classes, oh, ow, rect_mask != 0);
+  const bool on = s.kind == 1;
+  long long bin0 = 0, bin1 = 0;
+  float res0 = 0.f, res1 = 0.f;
+  if (on) {   // _convert_alpha(alpha) in float64; rotres f32(alpha -/+ pi / 2)
+    const double a = alpha[i];
+    if (a < kPi / 6. || a > 5 * kPi / 6.) {
+      bin0 = 1;
+      res0 = __double2float_rn(__dsub_rn(a, -0.5 * kPi));
+    }
+    if (a > -kPi / 6. || a < -5 * kPi / 6.) {
+      bin1 = 1;
+      res1 = __double2float_rn(__dsub_rn(a, 0.5 * kPi));
+    }
+  }
+  wh[2 * i] = on ? s.w : 0.f;
+  wh[2 * i + 1] = on ? s.h : 0.f;
+  reg[2 * i] = on ? __fsub_rn(s.ctx, (float)s.cx) : 0.f;
+  reg[2 * i + 1] = on ? __fsub_rn(s.cty, (float)s.cy) : 0.f;
+  ind[i] = on ? (long long)s.cy * ow + s.cx : 0;
+  dep[i] = on ? depth[i] : 0.f;
+  dim_out[3 * i] = on ? dim[3 * i] : 0.f;
+  dim_out[3 * i + 1] = on ? dim[3 * i + 1] : 0.f;
+  dim_out[3 * i + 2] = on ? dim[3 * i + 2] : 0.f;
+  rotbin[2 * i] = bin0;
+  rotbin[2 * i + 1] = bin1;
+  rotres[2 * i] = res0;
+  rotres[2 * i + 1] = res1;
+  reg_mask[i] = (on && !aug[b]) ? 1 : 0;
+  rot_mask[i] = on ? 1 : 0;
+}
+
+constexpr int kDddMaxSlots = 128;
+constexpr int kDddRows = 4;   // output rows per CTA of the heat map
+
+// The slots of one image as the heat map reads them: class (-1 all), the Gaussian's window and the overwrite
+// rectangle, both clipped to the map, and ct_int / r for the Gaussian's value.
+struct DddRec {
+  int cls, cx, cy, r;
+  int gx0, gy0, gx1, gy1;   // Gaussian window on the map (empty when gx0 > gx1)
+  int ox0, oy0, ox1, oy1;   // overwrite rectangle
+};
+
+// hm [b, C, oh, ow]: each CTA covers kDddRows rows of one image for every class.  It rebuilds the image's slot
+// records in shared memory, keeps those (in slot order) that touch its rows, and per pixel and class scans them
+// backwards: the max of the Gaussians up to the first slot whose overwrite covers the pixel, then max(that, 0.9999)
+// -- the value of the reference's in-order np.maximum / assignment sequence.
+__global__ void __launch_bounds__(kThreads) k_ddd_heatmap(const float *__restrict__ boxes,
+                                                           const int *__restrict__ cls,
+                                                           const int *__restrict__ num_objs,
+                                                           const double *__restrict__ trans, int m, int num_classes,
+                                                           int oh, int ow, int rect_mask, float *__restrict__ hm) {
+  __shared__ DddRec all[kDddMaxSlots];
+  __shared__ unsigned char keep[kDddMaxSlots];
+  __shared__ DddRec recs[kDddMaxSlots];
+  __shared__ int s_n;
+  const int b = blockIdx.y;
+  const int y0 = blockIdx.x * kDddRows, y1 = min(y0 + kDddRows, oh) - 1;
+  const int n = min(num_objs[b], m);
+  for (int k = threadIdx.x; k < n; k += blockDim.x) {
+    const long long i = (long long)b * m + k;
+    const DddSlot s = ddd_slot(boxes + i * 4, cls[i], trans + 6 * b, num_classes, oh, ow, rect_mask != 0);
+    DddRec r;
+    r.cls = s.cls;
+    r.cx = s.cx;
+    r.cy = s.cy;
+    r.r = s.r;
+    r.gx0 = s.gauss ? max(s.cx - s.r, 0) : 0;
+    r.gx1 = s.gauss ? min(s.cx + s.r, ow - 1) : -1;
+    r.gy0 = s.gauss ? max(s.cy - s.r, 0) : 0;
+    r.gy1 = s.gauss ? min(s.cy + s.r, oh - 1) : -1;
+    r.ox0 = s.ox0;
+    r.ox1 = s.ox1;
+    r.oy0 = s.oy0;
+    r.oy1 = s.oy1;
+    all[k] = r;
+    const bool g_rows = r.gx0 <= r.gx1 && r.gy0 <= y1 && r.gy1 >= y0;
+    const bool o_rows = r.ox0 <= r.ox1 && r.oy0 <= y1 && r.oy1 >= y0;
+    keep[k] = s.kind != 0 && (g_rows || o_rows);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int c = 0;
+    for (int k = 0; k < n; ++k)
+      if (keep[k]) recs[c++] = all[k];
+    s_n = c;
+  }
+  __syncthreads();
+  const int nr = s_n;
+  const size_t plane = (size_t)oh * ow;
+  const int npx = (y1 - y0 + 1) * ow;
+  for (int p = threadIdx.x; p < npx * num_classes; p += blockDim.x) {
+    const int c = p / npx, q = p % npx;
+    const int y = y0 + q / ow, x = q % ow;
+    float acc = 0.f;
+    for (int k = nr - 1; k >= 0; --k) {
+      const DddRec &r = recs[k];
+      if (r.cls != c && r.cls != -1) continue;
+      if (x >= r.ox0 && x <= r.ox1 && y >= r.oy0 && y <= r.oy1) {
+        acc = fmaxf(acc, 0.9999f);
+        break;
+      }
+      if (x >= r.gx0 && x <= r.gx1 && y >= r.gy0 && y <= r.gy1) acc = fmaxf(acc, gauss_value(x - r.cx, y - r.cy, r.r));
+    }
+    hm[((size_t)b * num_classes + c) * plane + (size_t)y * ow + x] = acc;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) k_ddd_radius(const float *__restrict__ h, const float *__restrict__ w,
+                                                          int n, int *__restrict__ radius) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) radius[i] = h[i] > 0.f && w[i] > 0.f ? ddd_radius(h[i], w[i]) : 0;
+}
+
 // Depth of the grey tree and the number of its levels combined per block of the grey pass.
 void grey_plan(int out_h, int out_w, int *depth, int *leaf_log) {
   *depth = pw_depth((long long)out_h * out_w);
@@ -568,6 +847,46 @@ extern "C" int cnb_multi_pose_targets(const float *boxes, const int32_t *cls, co
       (long long *)ind, reg, reg_mask, hps, hps_mask, hp_offset, (long long *)hp_ind, (long long *)hp_mask, obj_cls,
       obj_cx, obj_cy, obj_radius, obj_valid, hp_cx, hp_cy, hp_radius, hp_valid);
   CNB_CHECK_LAUNCH("cnb_multi_pose_targets");
+  cnb::count_launch();
+  return CNB_OK;
+}
+
+extern "C" int cnb_ddd_targets(const float *boxes, const int32_t *cls, const int32_t *num_objs, const double *alpha,
+                               const float *depth, const float *dim, const uint8_t *aug, const double *trans6, int b,
+                               int m, int num_classes, int out_h, int out_w, int rect_mask, float *hm, float *dep,
+                               float *dim_out, int64_t *ind, int64_t *rotbin, float *rotres, uint8_t *reg_mask,
+                               uint8_t *rot_mask, float *wh, float *reg, void *stream) {
+  CNB_REQUIRE(boxes && cls && num_objs && alpha && depth && dim && aug && trans6 && hm && dep && dim_out && ind &&
+                  rotbin && rotres && reg_mask && rot_mask && wh && reg,
+              CNB_EINVAL, "cnb_ddd_targets: null pointer");
+  CNB_REQUIRE(b > 0 && b <= 65535 && m > 0 && num_classes > 0 && out_h > 0 && out_w > 0 &&
+                  (long long)out_h * out_w <= INT32_MAX && (long long)num_classes * out_h * out_w <= INT32_MAX &&
+                  (rect_mask == 0 || rect_mask == 1),
+              CNB_EINVAL, "cnb_ddd_targets: bad shape (b = %d, m = %d, classes = %d, out %d x %d, rect_mask %d)", b, m,
+              num_classes, out_h, out_w, rect_mask);
+  CNB_REQUIRE(m <= cnb::kDddMaxSlots, CNB_EUNSUPPORTED, "cnb_ddd_targets: at most %d slots per image (got %d)",
+              cnb::kDddMaxSlots, m);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long n = (long long)b * m;
+  cnb::k_ddd_targets<<<(unsigned)((n + cnb::kThreads - 1) / cnb::kThreads), cnb::kThreads, 0, st>>>(
+      boxes, cls, num_objs, alpha, depth, dim, aug, trans6, b, m, num_classes, out_h, out_w, rect_mask, dep, dim_out,
+      (long long *)ind, (long long *)rotbin, rotres, reg_mask, rot_mask, wh, reg);
+  CNB_CHECK_LAUNCH("cnb_ddd_targets");
+  cnb::count_launch();
+  dim3 g((unsigned)((out_h + cnb::kDddRows - 1) / cnb::kDddRows), (unsigned)b);
+  cnb::k_ddd_heatmap<<<g, cnb::kThreads, 0, st>>>(boxes, cls, num_objs, trans6, m, num_classes, out_h, out_w,
+                                                   rect_mask, hm);
+  CNB_CHECK_LAUNCH("cnb_ddd_targets (hm)");
+  cnb::count_launch();
+  return CNB_OK;
+}
+
+extern "C" int cnb_ddd_gaussian_radius(const float *h, const float *w, int n, int32_t *radius, void *stream) {
+  CNB_REQUIRE(h && w && radius, CNB_EINVAL, "cnb_ddd_gaussian_radius: null pointer");
+  CNB_REQUIRE(n > 0, CNB_EINVAL, "cnb_ddd_gaussian_radius: bad length %d", n);
+  cnb::k_ddd_radius<<<(unsigned)((n + cnb::kThreads - 1) / cnb::kThreads), cnb::kThreads, 0, (cudaStream_t)stream>>>(
+      h, w, n, radius);
+  CNB_CHECK_LAUNCH("cnb_ddd_gaussian_radius");
   cnb::count_launch();
   return CNB_OK;
 }

@@ -18,8 +18,12 @@ The numeric contract is DESIGN.md section 4.9.
 
 The multi_pose sampler (datasets/sample/multi_pose.py:29-183) works the same way: MultiPoseTrainInput,
 collate_multi_pose and build_multi_pose_batch, with the rotated crop, the keypoint targets, hm / hm_hp and the
-joint lists of FocalSplatLoss (DESIGN.md section 4.10)."""
+joint lists of FocalSplatLoss (DESIGN.md section 4.10).
+
+The ddd sampler (datasets/sample/ddd.py:27-157) too: DddTrainInput, collate_ddd and build_ddd_batch, with the
+KITTI ignore regions painted into a dense hm on the device (DESIGN.md section 4.11)."""
 import itertools
+import math
 import os
 import random
 
@@ -50,18 +54,19 @@ def _get_border(border, size):
 
 def affine_transform(center, scale, output_size, rot=0):
     """get_affine_transform(center, scale, rot, output_size) (utils/image.py:27-60) as a 2x3 float64, to the bit.
-    A scale that is not an array becomes a float32 pair as there; a float64 array scale (keep_res with a random
-    crop) keeps its float64 half-width, which the reference adds to the float32 centre in float64.  get_dir turns
-    (0, -src_w / 2) by np.pi * rot / 180 in float64 (np.sin / np.cos, as there) and src[1] is the float64 sum
-    rounded to float32; rot = 0 gives the unrotated point exactly."""
+    A scale that is not an array becomes a float32 pair as there; an array scale (keep_res with a random crop, or
+    ddd's int32 / float64 pair) keeps its float64 half-width, which the reference adds to the centre in float64.
+    get_dir turns (0, -src_w / 2) by np.pi * rot / 180 in float64 (np.sin / np.cos, as there) and src[1] is the
+    float64 sum rounded to float32; rot = 0 gives the unrotated point exactly.  The centre enters that sum as given:
+    ctdet's and multi_pose's float32 centre exactly, ddd's float64 centre without a float32 rounding first."""
     if not isinstance(scale, np.ndarray):
         scale = np.array([scale, scale], dtype=F32)
     src, dst = _affine_points(center, scale.astype(F32), output_size)
     rot_rad = np.pi * rot / 180
     sn, cs = np.sin(rot_rad), np.cos(rot_rad)
     half = np.float64(scale[0]) * -0.5                  # src_point = [0, src_w * -0.5]
-    src[1, 0] = F32(np.float64(F32(center[0])) + (0 * cs - half * sn))
-    src[1, 1] = F32(np.float64(F32(center[1])) + (0 * sn + half * cs))
+    src[1, 0] = F32(np.float64(center[0]) + (0 * cs - half * sn))
+    src[1, 1] = F32(np.float64(center[1]) + (0 * sn + half * cs))
     d = src[0] - src[1]
     src[2] = src[1] + np.array([-d[1], d[0]], F32)
     return cv_affine_transform(src, dst)
@@ -543,4 +548,170 @@ def build_multi_pose_batch(packed, device=None, dtype=torch.float32, memory_form
     ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
     if sc['hm_hp']:
         ret.update(zip(('hp_cx', 'hp_cy', 'hp_radius', 'hp_valid'), hp_lists))
+    return ret
+
+
+# ---------------------------------------------------------------- ddd (datasets/sample/ddd.py)
+def ddd_params(height, width, opt, split):
+    """The random draws of DddDataset.__getitem__ (ddd.py:37-66) for one height x width image and the matrices they
+    give.  Only np.random draws: in the train split one np.random.random() < aug_ddd (none in val: the `and`
+    short-circuits) and, when it succeeds, three randn in the order scale, x shift, y shift, the shifts scaled by
+    the image's width and height.  There is no flip and no colour augmentation.  The centre is float64 and the scale
+    an int32 pair ([input_w, input_h] under keep_res, else [width, height]), float64 once augmented."""
+    c = np.array([width / 2., height / 2.])
+    if opt.keep_res:
+        s = np.array([opt.input_w, opt.input_h], dtype=np.int32)
+    else:
+        s = np.array([width, height], dtype=np.int32)
+    aug = False
+    if split == 'train' and np.random.random() < opt.aug_ddd:
+        aug = True
+        sf, cf = opt.scale, opt.shift
+        s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
+        c[0] += width * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+        c[1] += height * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+    input_h, input_w = int(opt.input_h), int(opt.input_w)
+    output_h, output_w = int(opt.output_h), int(opt.output_w)
+    return {'c': c, 's': s, 'aug': aug, 'input_h': input_h, 'input_w': input_w, 'output_h': output_h,
+            'output_w': output_w,
+            'minv': np.array(_invert(affine_transform(c, s, [input_w, input_h])), np.float64),
+            'trans_output': affine_transform(c, s, [output_w, output_h]).reshape(6)}
+
+
+_DDD_IGNORED = {'alpha': 0., 'depth': 0., 'dim': [0., 0., 0.]}
+
+
+class DddTrainInput(torch.utils.data.Dataset):
+    """Wraps a reference DddDataset instance (duck-typed on opt, coco, images, img_dir, max_objs, cat_ids,
+    alpha_in_degree, mean, std and split).  __getitem__ reads the image and the annotations -- box, class
+    cat_ids[category_id], _convert_alpha(alpha) as float64, depth and dim -- and draws the parameters as the
+    reference does; it does no pixel work (collate_ddd + build_ddd_batch do).  The number of classes is
+    opt.num_classes, as there."""
+
+    def __init__(self, dataset):
+        if dataset.opt.mse_loss:
+            raise NotImplementedError("DddTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not implemented")
+        self.dataset = dataset
+
+    def __len__(self):
+        return len(self.dataset)
+
+    def __getitem__(self, index):
+        import cv2
+        ds = self.dataset
+        img_id = ds.images[index]
+        file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
+        img = cv2.imread(os.path.join(ds.img_dir, file_name))
+        opt = ds.opt
+        sample = ddd_params(img.shape[0], img.shape[1], opt, ds.split)
+        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
+        num_objs = min(len(anns), ds.max_objs)
+        boxes = np.zeros((num_objs, 4), F32)
+        cls = np.zeros(num_objs, np.int64)
+        alpha = np.zeros(num_objs, np.float64)
+        depth = np.zeros(num_objs, np.float64)
+        dims = []
+        for k in range(num_objs):
+            a = anns[k]
+            b = a['bbox']
+            boxes[k] = np.array([b[0], b[1], b[0] + b[2], b[1] + b[3]], dtype=np.float32)
+            cls[k] = int(ds.cat_ids[a['category_id']])
+            # only positive classes read these in the reference; an ignore object may lack them
+            val = a if cls[k] >= 0 else dict(_DDD_IGNORED, **a)
+            alpha[k] = math.radians(val['alpha'] + 45) if ds.alpha_in_degree else val['alpha']
+            depth[k] = val['depth']
+            dims.append(np.asarray(val['dim'], np.float64).reshape(-1))
+        sample.update(image=img, boxes=boxes, cls=cls, alpha=alpha, depth=depth, dim=dims, max_objs=ds.max_objs,
+                      num_classes=int(opt.num_classes), mean=np.asarray(ds.mean, F32).reshape(3),
+                      std=np.asarray(ds.std, F32).reshape(3), rect_mask=bool(opt.rect_mask),
+                      reg_bbox=bool(opt.reg_bbox), reg_offset=bool(opt.reg_offset))
+        return sample
+
+
+def collate_ddd(samples):
+    """Packs DddTrainInput samples into one uint8 buffer: the images (no flip, no colour augmentation), the output
+    matrices, the per-image augmented byte and per slot the box, class, alpha (float64), depth and dim (float32).
+    Raises ValueError for samples of different settings, max_objs outside [1, 128], a class the reference cannot
+    index (anything but <= -99, -1, [-C - 1, -2] or [0, C)) and a dim that is not 3 values."""
+    s0 = samples[0]
+    keys = ('input_h', 'input_w', 'output_h', 'output_w', 'max_objs', 'num_classes', 'rect_mask', 'reg_bbox',
+            'reg_offset')
+    for s in samples:
+        if any(s[k] != s0[k] for k in keys):
+            raise ValueError("collate_ddd: samples with different settings cannot be batched")
+    images = [s['image'] for s in samples]
+    _check_images(images)
+    b, m, nc = len(samples), int(s0['max_objs']), int(s0['num_classes'])
+    if not 1 <= m <= 128:
+        raise ValueError("collate_ddd: 1 to 128 object slots, got %d" % m)
+    boxes = np.zeros((b, m, 4), F32)
+    cls = np.zeros((b, m), np.int32)
+    alpha = np.zeros((b, m), np.float64)
+    depth = np.zeros((b, m), F32)
+    dim = np.zeros((b, m, 3), F32)
+    nobj = np.zeros(b, np.int32)
+    for i, s in enumerate(samples):
+        n = min(len(s['boxes']), m)
+        c = np.asarray(s['cls'][:n], np.int64)
+        ok = (c <= -99) | (c == -1) | ((c >= -nc - 1) & (c <= -2)) | ((c >= 0) & (c < nc))
+        if not ok.all():
+            raise ValueError("collate_ddd: class id %d is none of <= -99, -1, [%d, -2] or [0, %d)"
+                             % (c[~ok][0], -nc - 1, nc))
+        for k in range(n):
+            d = np.asarray(s['dim'][k], np.float64).reshape(-1)
+            if d.size != 3:
+                raise ValueError("collate_ddd: dim has %d values, expected 3" % d.size)
+            dim[i, k] = d
+        nobj[i] = n
+        boxes[i, :n] = np.asarray(s['boxes'][:n], F32).reshape(n, 4)
+        cls[i, :n] = np.maximum(c, -99)
+        alpha[i, :n] = np.asarray(s['alpha'][:n], np.float64)
+        depth[i, :n] = np.asarray(s['depth'][:n], np.float64)
+    pk = _Packer()
+    _pack_images(pk, images, [s['minv'] for s in samples], np.zeros(b, np.uint8), np.full(b, -1),
+                 np.zeros((b, 6), F32), np.zeros((b, 3)), s0['mean'], s0['std'])
+    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
+    pk.add('aug', np.array([bool(s['aug']) for s in samples], np.uint8))
+    pk.add('nobj', nobj)
+    pk.add('boxes', boxes)
+    pk.add('cls', cls)
+    pk.add('alpha', alpha)
+    pk.add('depth', depth)
+    pk.add('dim', dim)
+    scalars = {k: s0[k] for k in keys}
+    scalars.update(batch=b)
+    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+
+
+def build_ddd_batch(packed, device=None, dtype=torch.float32, memory_format=torch.contiguous_format):
+    """The reference's collated ddd batch, on the device, from a collate_ddd result: one non-blocking H2D copy on
+    the current stream, the image pass at input_h x input_w and cnb_ddd_targets (targets, then hm).  Keys, shapes and
+    dtypes as ddd.py:143-149 returns them: input, hm [B,C,oh,ow] f32, dep [B,M,1] f32, dim [B,M,3] f32, ind i64,
+    rotbin [B,M,2] i64, rotres [B,M,2] f32, reg_mask u8, rot_mask u8; wh with reg_bbox, reg with reg_offset.  hm is
+    always dense: the ignore regions overwrite it in object order, which no object list expresses.  The packed host
+    buffer is not modified."""
+    dev = _device(device)
+    sc = packed['scalars']
+    b, m, nc, oh, ow = sc['batch'], sc['max_objs'], sc['num_classes'], sc['output_h'], sc['output_w']
+    buf = packed['buffer'].to(dev, non_blocking=True)
+    v = _views(buf, packed['layout'])
+    inp = _launch_images(v, b, sc['input_h'], sc['input_w'], False, dtype, memory_format, dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    u8 = dict(dtype=torch.uint8, device=dev)
+    i64 = dict(dtype=torch.int64, device=dev)
+    hm = torch.empty((b, nc, oh, ow), **f32)
+    dep, dim = torch.empty((b, m, 1), **f32), torch.empty((b, m, 3), **f32)
+    ind, rotbin, rotres = torch.empty((b, m), **i64), torch.empty((b, m, 2), **i64), torch.empty((b, m, 2), **f32)
+    reg_mask, rot_mask = torch.empty((b, m), **u8), torch.empty((b, m), **u8)
+    wh, reg = torch.empty((b, m, 2), **f32), torch.empty((b, m, 2), **f32)
+    C.ddd_targets(ptr(v['boxes']), ptr(v['cls']), ptr(v['nobj']), ptr(v['alpha']), ptr(v['depth']), ptr(v['dim']),
+                  ptr(v['aug']), ptr(v['trans_output']), b, m, nc, oh, ow, int(sc['rect_mask']), ptr(hm), ptr(dep),
+                  ptr(dim), ptr(ind), ptr(rotbin), ptr(rotres), ptr(reg_mask), ptr(rot_mask), ptr(wh), ptr(reg),
+                  stream_ptr(hm))
+    ret = {'input': inp, 'hm': hm, 'dep': dep, 'dim': dim, 'ind': ind, 'rotbin': rotbin, 'rotres': rotres,
+           'reg_mask': reg_mask, 'rot_mask': rot_mask}
+    if sc['reg_bbox']:
+        ret['wh'] = wh
+    if sc['reg_offset']:
+        ret['reg'] = reg
     return ret

@@ -761,7 +761,30 @@ int cnb_preprocess_image_f32(const uint8_t *image_hwc, int h, int w, const doubl
  * hp_cy / hp_radius i32, hp_valid u8 [b,J,m] (pt_int and the slot's radius), a [b*J, m] list of class 0 that
  * splat_gaussian / FocalSplatLoss read as hm_hp [b*J, 1, R, R].  Differences float32 - int32 are one rounding of
  * the exact difference.  Every other entry is zero.  No atomics: the output is identical run to run.  Errors,
- * checked before any CUDA call: CNB_EINVAL for a null pointer or a bad shape. */
+ * checked before any CUDA call: CNB_EINVAL for a null pointer or a bad shape.
+ *
+ * cnb_ddd_targets: ddd.py:86-140 for m = max_objs slots per image, C = num_classes, and the dense hm; two launches
+ * (targets: one thread per (image, slot); hm: one CTA per 4 rows of an image), no atomics, no workspace.  Slot k <
+ * min(num_objs[b], m) holds the float32 corners boxes[b, k], the class cls[b, k], alpha[b, k] (float64, after
+ * _convert_alpha), depth[b, k] and dim[b, k, 3] (float32).  A class <= -99, or one outside [0, C), -1 and
+ * [-C - 1, -2], is skipped.  The box goes through the FORWARD trans6[b] (get_affine_transform(c, s, 0, [out_w,
+ * out_h]), float64 t0 x + t1 y + t2 rounded to float32, no flip) and is clipped to [0, out_w - 1] x [0, out_h - 1];
+ * nothing happens unless h > 0 and w > 0.  Its radius is max(0, int(gaussian_radius((h, w)))) evaluated on float32
+ * h, w as numpy does: every operation float32, b ** 2 the C library's powf(b, 2) (glibc's algorithm, restated) --
+ * cnb_ddd_gaussian_radius returns it for n pairs, for testing.  ct = f32((x0 + x1) / 2, (y0 + y1) / 2), ct_int its
+ * truncation.
+ *   cls in [0, C): draw_umich_gaussian(hm[cls], ct, r) and the targets: wh [b,m,2] f32 = (w, h), rotbin [b,m,2] i64
+ *     / rotres [b,m,2] f32 (alpha < pi/6 or > 5pi/6: bin 0, f32(alpha + pi/2); alpha > -pi/6 or < -5pi/6: bin 1,
+ *     f32(alpha - pi/2); float64 compares), dep [b,m,1] f32 = depth, dim_out [b,m,3] f32 = dim, ind [b,m] i64 =
+ *     ct_int.y out_w + ct_int.x, reg [b,m,2] f32 = ct - ct_int, rot_mask [b,m] u8 = 1, reg_mask [b,m] u8 = 1 only
+ *     when aug[b] == 0.
+ *   cls < 0 (ignore; classes -cls - 2, or all for -1): no targets.  rect_mask == 1: hm[ignore, int(y0):int(y1) + 1,
+ *     int(x0):int(x1) + 1] = f32(0.9999); rect_mask == 0: the Gaussian on each ignore class, then hm[ignore,
+ *     ct_int.y, ct_int.x] = f32(0.9999).
+ * hm [b,C,out_h,out_w] f32 is the result of doing that in slot order on a zero map (Gaussians as np.maximum of the
+ * float64 values rounded to float32, overwrites as assignments), whatever the order.  Every other entry is zero.
+ * Errors, checked before any CUDA call: CNB_EINVAL for a null pointer, a bad shape or a rect_mask other than 0 / 1;
+ * CNB_EUNSUPPORTED for m > 128. */
 #define CNB_TRAIN_MAX_PIXELS 4194304
 size_t cnb_train_images_workspace_bytes(int b, int out_h, int out_w);
 int cnb_train_images(const uint8_t *src, const int64_t *src_off, const int32_t *src_hw, const double *minv6,
@@ -780,6 +803,12 @@ int cnb_multi_pose_targets(const float *boxes, const int32_t *cls, const int32_t
                            uint8_t *hps_mask, float *hp_offset, int64_t *hp_ind, int64_t *hp_mask, int32_t *obj_cls,
                            int32_t *obj_cx, int32_t *obj_cy, int32_t *obj_radius, uint8_t *obj_valid, int32_t *hp_cx,
                            int32_t *hp_cy, int32_t *hp_radius, uint8_t *hp_valid, void *stream);
+int cnb_ddd_targets(const float *boxes, const int32_t *cls, const int32_t *num_objs, const double *alpha,
+                    const float *depth, const float *dim, const uint8_t *aug, const double *trans6, int b, int m,
+                    int num_classes, int out_h, int out_w, int rect_mask, float *hm, float *dep, float *dim_out,
+                    int64_t *ind, int64_t *rotbin, float *rotres, uint8_t *reg_mask, uint8_t *rot_mask, float *wh,
+                    float *reg, void *stream);
+int cnb_ddd_gaussian_radius(const float *h, const float *w, int n, int32_t *radius, void *stream);
 
 #ifdef __cplusplus
 }

@@ -1,7 +1,7 @@
-"""Device time per ctdet or multi_pose training batch (centernet_b200.train_input), the host->device bytes per image
+"""Device time per ctdet, multi_pose or ddd training batch (centernet_b200.train_input), the host->device bytes per image
 against the reference loader's, and (ctdet) the numpy oracle's CPU time per image.
 
-    python tools/train_input_time.py [--iters 50] [--sampler ctdet|multi_pose]
+    python tools/train_input_time.py [--iters 50] [--sampler ctdet|multi_pose|ddd]
 
 Synthetic COCO-sized sources (ragged 640x480 / 480x640 / 500x375 / 427x640), 512x512 input, 80 classes, 128
 object slots, about 7 objects per image, colour augmentation on; B = 32, 64 and 114.  Per batch it times, with
@@ -15,7 +15,12 @@ work this moves off the host, not a measurement of cv2.
 random joint visibilities, colour augmentation on; B = 32 and 64, with aug_rot 0 and 1 (every image rotated, up to
 +-60 degrees), each timed as build_multi_pose_batch with the H2D copy, from a buffer already on the device, and
 per image; with dense hm / hm_hp and, for aug_rot 0, without (a rotated batch needs the dense hm).  Prints one
-JSON line, with the card's name and power limit read in the same run."""
+JSON line, with the card's name and power limit read in the same run.
+
+--sampler ddd: synthetic KITTI-sized sources (ragged around 1242x375), 1280x384 input, 3 classes, 50 slots, about 8
+positives, 4 ignore objects (DontCare and single-class) and a skipped one per image, aug_ddd 0.5; B = 32 and 64,
+with point ignores and with rect_mask, each timed as build_ddd_batch with the H2D copy and from a buffer already
+on the device (kernels only).  Prints one JSON line, with the card's name and power limit read in the same run."""
 import argparse
 import json
 import os
@@ -32,6 +37,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from centernet_b200 import train_input as T  # noqa: E402
+import ddd_train_cases as DC  # noqa: E402
 import multi_pose_train_cases as MC  # noqa: E402
 import train_cases as TC  # noqa: E402
 
@@ -81,15 +87,38 @@ def make_pose_samples(b, seed, aug_rot):
     return out
 
 
+def make_ddd_samples(b, seed, rect_mask):
+    case = dict(DC.CASES["kitti"], rect_mask=rect_mask)
+    opt = DC.make_opt(case)
+    rng = np.random.default_rng(seed)
+    np.random.seed(seed); random.seed(seed)
+    out = []
+    for i in range(b):
+        h, w = DC.KITTI_SIZES[i % len(DC.KITTI_SIZES)]
+        s = T.ddd_params(h, w, opt, 'train')
+        n = 13
+        x0, y0 = rng.uniform(0, 0.9 * w, n), rng.uniform(0.3 * h, 0.8 * h, n)
+        bw, bh = rng.uniform(15, 250, n), rng.uniform(15, 150, n)
+        boxes = np.stack([x0, y0, x0 + bw, y0 + bh], 1).astype(np.float32)
+        cls = np.array([0, 1, 1, 2, 1, 1, 0, 1, -1, -3, -2, -1, -99])[rng.permutation(n)]
+        s.update(image=rng.integers(0, 256, (h, w, 3), dtype=np.uint8), boxes=boxes, cls=cls,
+                 alpha=rng.uniform(-np.pi, np.pi, n), depth=rng.uniform(3, 70, n),
+                 dim=list(rng.uniform(0.5, 4, (n, 3))), max_objs=50, num_classes=3, mean=DC.MEAN, std=DC.STD,
+                 rect_mask=rect_mask, reg_bbox=True, reg_offset=True)
+        out.append(s)
+    return out
+
+
 def time_batches(packed, iters, dense_hm, build=None):
     build = build or T.build_ctdet_batch
+    kw = {} if dense_hm is None else dict(dense_hm=dense_hm)
     for _ in range(3):
-        build(packed, dense_hm=dense_hm)
+        build(packed, **kw)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(iters):
-        build(packed, dense_hm=dense_hm)
+        build(packed, **kw)
     e1.record()
     torch.cuda.synchronize()
     return e0.elapsed_time(e1) / iters
@@ -142,16 +171,36 @@ def main_multi_pose(iters):
     print(json.dumps(res))
 
 
+def main_ddd(iters):
+    # the reference's per-image transfer: input, hm and the targets of ddd.py:143-149
+    m, oh, ow = 50, 96, 320
+    ref_bytes = 3 * 384 * 1280 * 4 + 3 * oh * ow * 4 + m * (4 + 3 * 4 + 8 + 2 * 8 + 2 * 4 + 1 + 1 + 2 * 4 + 2 * 4)
+    res = {"gpu": gpu_info(), "sampler": "ddd", "batches": {}}
+    for b in (32, 64):
+        for rect in (False, True):
+            packed = T.collate_ddd(make_ddd_samples(b, b, rect))
+            on_device = dict(packed, buffer=packed['buffer'].cuda())
+            rr = {"ms_per_batch": time_batches(packed, iters, None, T.build_ddd_batch),
+                  "ms_per_batch_kernels_only": time_batches(on_device, iters, None, T.build_ddd_batch),
+                  "h2d_bytes_per_image": packed['buffer'].numel() / b, "reference_h2d_bytes_per_image": ref_bytes}
+            rr["us_per_image"] = rr["ms_per_batch"] * 1e3 / b
+            rr["us_per_image_kernels_only"] = rr["ms_per_batch_kernels_only"] * 1e3 / b
+            res["batches"]["B%d_%s" % (b, "rect_mask" if rect else "point_ignores")] = rr
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--oracle-images", type=int, default=4)
-    ap.add_argument("--sampler", choices=("ctdet", "multi_pose"), default="ctdet")
+    ap.add_argument("--sampler", choices=("ctdet", "multi_pose", "ddd"), default="ctdet")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("train_input_time: needs a CUDA device (no CPU timing is reported)")
     if args.sampler == "multi_pose":
         return main_multi_pose(args.iters)
+    if args.sampler == "ddd":
+        return main_ddd(args.iters)
     res = {"gpu": gpu_info(), "batches": {}}
     ref_bytes = 3 * 512 * 512 * 4 + 80 * 128 * 128 * 4 + 128 * (2 * 4 + 2 * 4 + 8 + 1)
     for b in (32, 64, 114):
