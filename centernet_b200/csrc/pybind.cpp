@@ -429,6 +429,17 @@ PYBIND11_MODULE(_C, m) {
                                   ptr<void>(stream)),
           "cnb_ddd_gaussian_radius");
   });
+  m.def("exdet_targets", [](P pts, P cls, P nobj, P flip, P hw, P trans, int b, int mm, int res, int agnostic, P reg,
+                            P ind, P reg_mask, P ocls, P ocx, P ocy, P orad, P oval, P ecls, P ecx, P ecy, P erad,
+                            P eval, P stream) {
+    check(cnb_exdet_targets(ptr<const float>(pts), ptr<const int32_t>(cls), ptr<const int32_t>(nobj),
+                            ptr<const uint8_t>(flip), ptr<const int32_t>(hw), ptr<const double>(trans), b, mm, res,
+                            agnostic, ptr<float>(reg), ptr<int64_t>(ind), ptr<uint8_t>(reg_mask), ptr<int32_t>(ocls),
+                            ptr<int32_t>(ocx), ptr<int32_t>(ocy), ptr<int32_t>(orad), ptr<uint8_t>(oval),
+                            ptr<int32_t>(ecls), ptr<int32_t>(ecx), ptr<int32_t>(ecy), ptr<int32_t>(erad),
+                            ptr<uint8_t>(eval), ptr<void>(stream)),
+          "cnb_exdet_targets");
+  });
   m.def("dcnv2_workspace_bytes", &cnb_dcnv2_workspace_bytes);
   m.def("dcnv2_backward_workspace_bytes", &cnb_dcnv2_backward_workspace_bytes);
   m.def("dcnv2_backward_ex", [](P input, int in_cl, P offset, P mask, P weight, P gout, P gin, int gin_cl, P goff, P gmask,

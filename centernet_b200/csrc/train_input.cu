@@ -2,8 +2,8 @@
 // the random crop / flip warp, /255, color_aug, the normalisation and the layout change of a whole batch of
 // ragged uint8 sources, and the ctdet regression targets plus the object lists of FocalSplatLoss.  Every value
 // is the one the reference's loader computes for the same drawn parameters, bit for bit; no atomics, so the
-// output is also identical run to run.  The numeric contract is DESIGN.md section 4.9.  The multi_pose and ddd
-// targets (sections 4.10 and 4.11) reuse the warp and the box arithmetic.
+// output is also identical run to run.  The numeric contract is DESIGN.md section 4.9.  The multi_pose, ddd and
+// exdet targets (sections 4.10 to 4.12) reuse the warp and the box arithmetic.
 #include <map>
 
 #include "common.cuh"
@@ -734,6 +734,79 @@ __global__ void __launch_bounds__(kThreads) k_ddd_radius(const float *__restrict
   if (i < n) radius[i] = h[i] > 0.f && w[i] > 0.f ? ddd_radius(h[i], w[i]) : 0;
 }
 
+// ---------------------------------------------------------------- exdet targets (exdet.py:95-129)
+constexpr int kExdetMaxSlots = 128;
+
+// np.clip(x, 0, hi) of a float32: a bound replaces x only when x lies strictly outside it, so -0 stays -0 as there
+// (and reaches reg as -0 - 0 = -0).
+__device__ __forceinline__ float clip_f32(float x, float hi) {
+  x = x < 0.f ? 0.f : x;
+  return x > hi ? hi : x;
+}
+
+// One thread per (image, slot).  Slot k < min(num_objs[b], m) holds the extreme points pts[b, k] [4, 2] (t, l, b, r)
+// and the class cls[b, k].  Part p's outputs live at [p, b, k]: reg [4, nb, m, 2], ind [4, nb, m] and the lists
+// ex_* [4, nb, m]; the centre lists obj_* and reg_mask are [nb, m].
+__global__ void __launch_bounds__(kThreads) k_exdet_targets(
+    const float *__restrict__ pts, const int *__restrict__ cls, const int *__restrict__ num_objs,
+    const unsigned char *__restrict__ flip, const int *__restrict__ src_hw, const double *__restrict__ trans, int nb,
+    int m, int res, int agnostic, float *__restrict__ reg, long long *__restrict__ ind,
+    unsigned char *__restrict__ reg_mask, int *__restrict__ obj_cls, int *__restrict__ obj_cx,
+    int *__restrict__ obj_cy, int *__restrict__ obj_radius, unsigned char *__restrict__ obj_valid,
+    int *__restrict__ ex_cls, int *__restrict__ ex_cx, int *__restrict__ ex_cy, int *__restrict__ ex_radius,
+    unsigned char *__restrict__ ex_valid) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)nb * m) return;
+  const int b = (int)(i / m), k = (int)(i % m);
+  float px[4] = {0.f, 0.f, 0.f, 0.f}, py[4] = {0.f, 0.f, 0.f, 0.f};
+  int c = 0, rad = 0, cx = 0, cy = 0;
+  bool valid = false;
+  if (k < min(num_objs[b], m)) {
+    const float *q = pts + i * 8;
+    const bool fl = flip[b] != 0;
+    const float wd = (float)src_hw[2 * b + 1];
+    const double *t = trans + 6 * b;
+    const float hi = (float)(res - 1);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      // pts[:, 0] = width - pts[:, 0] - 1 in float32, then pts[1] <-> pts[3]
+      const int s = fl && (j & 1) ? 4 - j : j;
+      const float x = fl ? __fsub_rn(__fsub_rn(wd, q[2 * s]), 1.f) : q[2 * s], y = q[2 * s + 1];
+      px[j] = clip_f32(affine_f32(t, x, y), hi);
+      py[j] = clip_f32(affine_f32(t + 3, x, y), hi);
+    }
+    const float h = __fsub_rn(py[2], py[0]), w = __fsub_rn(px[3], px[1]);
+    valid = h > 0.f && w > 0.f;
+    if (valid) {
+      const double r = gaussian_radius_f64((long long)ceilf(h), (long long)ceilf(w));
+      rad = r > 0.0 ? (int)r : 0;   // max(0, int(radius))
+      cx = (int)__fdiv_rn(__fadd_rn(px[3], px[1]), 2.f);
+      cy = (int)__fdiv_rn(__fadd_rn(py[0], py[2]), 2.f);
+      c = cls[i];
+    }
+  }
+  const long long plane = (long long)nb * m;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const long long o = j * plane + i;
+    const int ix = valid ? (int)px[j] : 0, iy = valid ? (int)py[j] : 0;   // the clip makes both >= 0
+    reg[2 * o] = valid ? __fsub_rn(px[j], (float)ix) : 0.f;
+    reg[2 * o + 1] = valid ? __fsub_rn(py[j], (float)iy) : 0.f;
+    ind[o] = (long long)iy * res + ix;
+    ex_cls[o] = agnostic ? 0 : c;
+    ex_cx[o] = ix;
+    ex_cy[o] = iy;
+    ex_radius[o] = rad;
+    ex_valid[o] = valid ? 1 : 0;
+  }
+  reg_mask[i] = valid ? 1 : 0;
+  obj_cls[i] = c;
+  obj_cx[i] = cx;
+  obj_cy[i] = cy;
+  obj_radius[i] = rad;
+  obj_valid[i] = valid ? 1 : 0;
+}
+
 // Depth of the grey tree and the number of its levels combined per block of the grey pass.
 void grey_plan(int out_h, int out_w, int *depth, int *leaf_log) {
   *depth = pw_depth((long long)out_h * out_w);
@@ -887,6 +960,30 @@ extern "C" int cnb_ddd_gaussian_radius(const float *h, const float *w, int n, in
   cnb::k_ddd_radius<<<(unsigned)((n + cnb::kThreads - 1) / cnb::kThreads), cnb::kThreads, 0, (cudaStream_t)stream>>>(
       h, w, n, radius);
   CNB_CHECK_LAUNCH("cnb_ddd_gaussian_radius");
+  cnb::count_launch();
+  return CNB_OK;
+}
+
+extern "C" int cnb_exdet_targets(const float *pts, const int32_t *cls, const int32_t *num_objs, const uint8_t *flip,
+                                 const int32_t *src_hw, const double *trans6, int b, int m, int out_res, int agnostic_ex,
+                                 float *reg, int64_t *ind, uint8_t *reg_mask, int32_t *obj_cls, int32_t *obj_cx,
+                                 int32_t *obj_cy, int32_t *obj_radius, uint8_t *obj_valid, int32_t *ex_cls,
+                                 int32_t *ex_cx, int32_t *ex_cy, int32_t *ex_radius, uint8_t *ex_valid, void *stream) {
+  CNB_REQUIRE(pts && cls && num_objs && flip && src_hw && trans6 && reg && ind && reg_mask && obj_cls && obj_cx &&
+                  obj_cy && obj_radius && obj_valid && ex_cls && ex_cx && ex_cy && ex_radius && ex_valid,
+              CNB_EINVAL, "cnb_exdet_targets: null pointer");
+  CNB_REQUIRE(b > 0 && m > 0 && out_res > 0 && (long long)out_res * out_res <= INT32_MAX &&
+                  (agnostic_ex == 0 || agnostic_ex == 1),
+              CNB_EINVAL, "cnb_exdet_targets: bad shape (b = %d, m = %d, out_res = %d, agnostic_ex %d)", b, m, out_res,
+              agnostic_ex);
+  CNB_REQUIRE(m <= cnb::kExdetMaxSlots, CNB_EUNSUPPORTED, "cnb_exdet_targets: at most %d slots per image (got %d)",
+              cnb::kExdetMaxSlots, m);
+  const long long n = (long long)b * m;
+  cnb::k_exdet_targets<<<(unsigned)((n + cnb::kThreads - 1) / cnb::kThreads), cnb::kThreads, 0,
+                         (cudaStream_t)stream>>>(pts, cls, num_objs, flip, src_hw, trans6, b, m, out_res, agnostic_ex,
+                                                 reg, (long long *)ind, reg_mask, obj_cls, obj_cx, obj_cy, obj_radius,
+                                                 obj_valid, ex_cls, ex_cx, ex_cy, ex_radius, ex_valid);
+  CNB_CHECK_LAUNCH("cnb_exdet_targets");
   cnb::count_launch();
   return CNB_OK;
 }

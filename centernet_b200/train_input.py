@@ -21,7 +21,11 @@ collate_multi_pose and build_multi_pose_batch, with the rotated crop, the keypoi
 joint lists of FocalSplatLoss (DESIGN.md section 4.10).
 
 The ddd sampler (datasets/sample/ddd.py:27-157) too: DddTrainInput, collate_ddd and build_ddd_batch, with the
-KITTI ignore regions painted into a dense hm on the device (DESIGN.md section 4.11)."""
+KITTI ignore regions painted into a dense hm on the device (DESIGN.md section 4.11).
+
+The exdet sampler (datasets/sample/exdet.py:30-137) too: ExdetTrainInput, collate_exdet and build_exdet_batch, with
+the extreme-point and centre targets and the object lists of the five heat maps, which FocalSplatLoss reads without
+the maps ever existing (DESIGN.md section 4.12)."""
 import itertools
 import math
 import os
@@ -74,7 +78,8 @@ def affine_transform(center, scale, output_size, rot=0):
 
 def crop_draws(height, width, c, s, opt):
     """The crop draws of the train split (ctdet.py:44-57, multi_pose.py:45-57): np.random.choice and two
-    randint, or the three randn of not_rand_crop.  Updates the float32 centre c in place; returns the scale."""
+    randint, or the three randn of not_rand_crop.  Updates the centre c in place (float32 for ctdet and multi_pose;
+    exdet's float64 one takes the random crop only); returns the scale."""
     if not opt.not_rand_crop:
         s = s * np.random.choice(np.arange(0.6, 1.4, 0.1))
         w_border = _get_border(128, width)
@@ -714,4 +719,157 @@ def build_ddd_batch(packed, device=None, dtype=torch.float32, memory_format=torc
         ret['wh'] = wh
     if sc['reg_offset']:
         ret['reg'] = reg
+    return ret
+
+
+# ---------------------------------------------------------------- exdet (datasets/sample/exdet.py)
+def exdet_params(height, width, opt, split, data_rng, eig_val, eig_vec):
+    """The random draws of EXDetDataset.__getitem__ (exdet.py:36-65) for one height x width image, in the reference's
+    order, and the matrices they give.  The centre is float64.  In the train split: the random crop's choice and two
+    randint (ctdet's crop_draws), or under not_rand_crop three randn in the order scale, x shift, y shift, the shifts
+    scaled by the image's width and height; then the flip draw.  The flip mirrors the image but leaves the centre,
+    so trans_input / trans_output are the unflipped get_affine_transform(c, s, 0, [res, res]) applied to the mirrored
+    source.  color_aug's draws follow as in ctdet.  The input is input_res square (there is no keep_res branch)."""
+    c = np.array([width / 2., height / 2.])
+    s = max(height, width) * 1.0
+    flipped = False
+    if split == 'train':
+        if not opt.not_rand_crop:
+            s = crop_draws(height, width, c, s, opt)
+        else:
+            sf, cf = opt.scale, opt.shift
+            s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
+            c[0] += width * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+            c[1] += height * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+        if np.random.random() < opt.flip:
+            flipped = True
+    order, blend, light = -1, np.zeros(6, F32), np.zeros(3, np.float64)
+    if split == 'train' and not opt.no_color_aug:
+        order, blend, light = color_draws(data_rng, eig_val, eig_vec)
+    res, out_res = int(opt.input_res), int(opt.output_res)
+    return {'c': c, 's': s, 'flip': flipped, 'input_res': res, 'output_res': out_res,
+            'minv': np.array(_invert(affine_transform(c, s, [res, res])), np.float64),
+            'trans_output': affine_transform(c, s, [out_res, out_res]).reshape(6),
+            'order': order, 'blend': blend, 'light': light}
+
+
+class ExdetTrainInput(torch.utils.data.Dataset):
+    """Wraps a reference EXDetDataset instance (duck-typed on opt, coco, images, img_dir, max_objs, cat_ids, mean,
+    std, _data_rng, _eig_val, _eig_vec and split).  __getitem__ reads the image and the annotations -- extreme_points
+    as float32 (t, l, b, r), class cat_ids[category_id] -- and draws the parameters as the reference does; it does no
+    pixel work (collate_exdet + build_exdet_batch do).  The number of classes is opt.num_classes, as there."""
+
+    def __init__(self, dataset):
+        if dataset.opt.mse_loss:
+            raise NotImplementedError("ExdetTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not implemented")
+        self.dataset = dataset
+
+    def __len__(self):
+        return len(self.dataset)
+
+    def __getitem__(self, index):
+        import cv2
+        ds = self.dataset
+        img_id = ds.images[index]
+        file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
+        img = cv2.imread(os.path.join(ds.img_dir, file_name))
+        opt = ds.opt
+        sample = exdet_params(img.shape[0], img.shape[1], opt, ds.split, ds._data_rng, ds._eig_val, ds._eig_vec)
+        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
+        num_objs = min(len(anns), ds.max_objs)
+        pts = [np.array(anns[k]['extreme_points'], dtype=np.float32).reshape(-1) for k in range(num_objs)]
+        cls = np.array([int(ds.cat_ids[anns[k]['category_id']]) for k in range(num_objs)], np.int64)
+        sample.update(image=img, points=pts, cls=cls, max_objs=ds.max_objs, num_classes=int(opt.num_classes),
+                      mean=np.asarray(ds.mean, F32).reshape(3), std=np.asarray(ds.std, F32).reshape(3),
+                      agnostic_ex=bool(opt.agnostic_ex), reg_offset=bool(opt.reg_offset))
+        return sample
+
+
+def collate_exdet(samples):
+    """Packs ExdetTrainInput samples into one uint8 buffer: what collate_ctdet packs for the images (flip bytes and
+    colour parameters included), trans_output, and per slot the extreme points [B, M, 4, 2] float32 (t, l, b, r) and
+    the class.  Raises ValueError for samples of different settings, max_objs outside [1, 128], an extreme_points
+    entry that is not 8 values, a class outside [0, num_classes) (the reference would index hm_c from the end) and a
+    coordinate that is not finite (the reference's pts.astype(np.int32) of it is undefined)."""
+    s0 = samples[0]
+    keys = ('input_res', 'output_res', 'max_objs', 'num_classes', 'agnostic_ex', 'reg_offset')
+    for s in samples:
+        if any(s[k] != s0[k] for k in keys):
+            raise ValueError("collate_exdet: samples with different settings cannot be batched")
+    images = [s['image'] for s in samples]
+    _check_images(images)
+    b, m, nc = len(samples), int(s0['max_objs']), int(s0['num_classes'])
+    if not 1 <= m <= 128:
+        raise ValueError("collate_exdet: 1 to 128 object slots (FocalSplatLoss / splat_gaussian), got %d" % m)
+    pts = np.zeros((b, m, 4, 2), F32)
+    cls = np.zeros((b, m), np.int32)
+    nobj = np.zeros(b, np.int32)
+    for i, s in enumerate(samples):
+        n = min(len(s['points']), m)
+        c = np.asarray(s['cls'][:n], np.int64)
+        if n and (c.min() < 0 or c.max() >= nc):
+            raise ValueError("collate_exdet: class id outside [0, %d)" % nc)
+        for k in range(n):
+            p = np.asarray(s['points'][k], F32).reshape(-1)
+            if p.size != 8:
+                raise ValueError("collate_exdet: extreme_points has %d values, expected 4 x 2" % p.size)
+            if not np.isfinite(p).all():
+                raise ValueError("collate_exdet: extreme_points must be finite")
+            pts[i, k] = p.reshape(4, 2)
+        nobj[i], cls[i, :n] = n, c
+    pk = _Packer()
+    _pack_images(pk, images, [s['minv'] for s in samples], [s['flip'] for s in samples],
+                 [s['order'] for s in samples], [s['blend'] for s in samples], [s['light'] for s in samples],
+                 s0['mean'], s0['std'])
+    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
+    pk.add('nobj', nobj)
+    pk.add('pts', pts)
+    pk.add('cls', cls)
+    scalars = {k: s0[k] for k in keys}
+    scalars.update(batch=b, color=any(s['order'] >= 0 for s in samples))
+    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+
+
+EXDET_PARTS = ('t', 'l', 'b', 'r')
+
+
+def build_exdet_batch(packed, device=None, dtype=torch.float32, memory_format=torch.contiguous_format,
+                      dense_hm=False):
+    """The reference's collated exdet batch, on the device, from a collate_exdet result: one non-blocking H2D copy on
+    the current stream, the image pass at input_res x input_res (the mirrored source under the unflipped matrix) and
+    cnb_exdet_targets, plus splat_gaussian with dense_hm.  Keys, shapes and dtypes as exdet.py:130-135 returns them:
+    input; with reg_offset reg_mask u8 [B,M], reg_t / reg_l / reg_b / reg_r f32 [B,M,2] and ind_t / ind_l / ind_b /
+    ind_r i64 [B,M]; with dense_hm hm_t / hm_l / hm_b / hm_r f32 [B,num_hm,R,R] (num_hm 1 under agnostic_ex, else C)
+    and hm_c f32 [B,C,R,R].  Always the FocalSplatLoss lists: the centres obj_cls / obj_cx / obj_cy / obj_radius
+    (int32) and obj_valid (uint8) [B,M], and the extreme points ex_cls / ex_cx / ex_cy / ex_radius (int32) and
+    ex_valid (uint8) [4,B,M] in the order t, l, b, r -- ex_*[p] is part p's [B,M] list set, and the [4B, M] view
+    of all four gives the four extreme maps in one splat.  The packed host buffer is not modified."""
+    dev = _device(device)
+    sc = packed['scalars']
+    b, m, nc, r = sc['batch'], sc['max_objs'], sc['num_classes'], sc['output_res']
+    num_hm = 1 if sc['agnostic_ex'] else nc
+    buf = packed['buffer'].to(dev, non_blocking=True)
+    v = _views(buf, packed['layout'])
+    inp = _launch_images(v, b, sc['input_res'], sc['input_res'], sc['color'], dtype, memory_format, dev)
+    u8 = dict(dtype=torch.uint8, device=dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    reg = torch.empty((4, b, m, 2), dtype=torch.float32, device=dev)
+    ind = torch.empty((4, b, m), dtype=torch.int64, device=dev)
+    reg_mask = torch.empty((b, m), **u8)
+    lists = [torch.empty((b, m), **i32) for _ in range(4)] + [torch.empty((b, m), **u8)]
+    ex_lists = [torch.empty((4, b, m), **i32) for _ in range(4)] + [torch.empty((4, b, m), **u8)]
+    C.exdet_targets(ptr(v['pts']), ptr(v['cls']), ptr(v['nobj']), ptr(v['flip']), ptr(v['src_hw']),
+                    ptr(v['trans_output']), b, m, r, int(sc['agnostic_ex']), ptr(reg), ptr(ind), ptr(reg_mask),
+                    *[ptr(t) for t in lists], *[ptr(t) for t in ex_lists], stream_ptr(reg))
+    ret = {'input': inp}
+    if dense_hm:
+        hm = splat_gaussian(*[t.view(4 * b, m) for t in ex_lists], num_hm, r, r).view(4, b, num_hm, r, r)
+        ret.update(('hm_' + p, hm[j]) for j, p in enumerate(EXDET_PARTS))
+        ret['hm_c'] = splat_gaussian(*lists, nc, r, r)
+    if sc['reg_offset']:
+        ret['reg_mask'] = reg_mask
+        ret.update(('reg_' + p, reg[j]) for j, p in enumerate(EXDET_PARTS))
+        ret.update(('ind_' + p, ind[j]) for j, p in enumerate(EXDET_PARTS))
+    ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
+    ret.update(zip(('ex_cls', 'ex_cx', 'ex_cy', 'ex_radius', 'ex_valid'), ex_lists))
     return ret

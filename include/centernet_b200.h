@@ -784,7 +784,21 @@ int cnb_preprocess_image_f32(const uint8_t *image_hwc, int h, int w, const doubl
  * hm [b,C,out_h,out_w] f32 is the result of doing that in slot order on a zero map (Gaussians as np.maximum of the
  * float64 values rounded to float32, overwrites as assignments), whatever the order.  Every other entry is zero.
  * Errors, checked before any CUDA call: CNB_EINVAL for a null pointer, a bad shape or a rect_mask other than 0 / 1;
- * CNB_EUNSUPPORTED for m > 128. */
+ * CNB_EUNSUPPORTED for m > 128.
+ *
+ * cnb_exdet_targets: exdet.py:95-129 for m = max_objs slots per image, R = out_res; one launch, one thread per
+ * (image, slot), no atomics, no workspace.  Slot k < min(num_objs[b], m) holds the float32 extreme points pts[b, k]
+ * [4, 2] in the order t, l, b, r (finite) and the class cls[b, k] in [0, C).  When flip[b] != 0 every x becomes
+ * width - x - 1 in float32 (width src_hw[b][1]) and points 1 and 3 (l, r) swap.  Each point goes through the
+ * FORWARD trans6[b] (get_affine_transform(c, s, 0, [R, R]), float64 t0 x + t1 y + t2 rounded to float32) and is
+ * clipped to [0, R - 1] as np.clip does (-0 stays -0).  h = b.y - t.y and w = r.x - l.x in float32; nothing is
+ * written unless h > 0 and w > 0.  Then the radius max(0, int(gaussian_radius(ceil(h), ceil(w)))) in float64, shared
+ * by all five parts; per part p, pt_int the truncation of the point: reg [4,b,m,2] f32 = pt - pt_int, ind [4,b,m] i64
+ * = pt_int.y R + pt_int.x, and the lists ex_cls (cls, or 0 when agnostic_ex == 1) / ex_cx / ex_cy / ex_radius i32
+ * and ex_valid u8 [4,b,m], each part a [b, m] list set of splat_gaussian / FocalSplatLoss; the centre ct =
+ * (int(f32(r.x + l.x) / 2), int(f32(t.y + b.y) / 2)) goes to obj_cls (cls) / obj_cx / obj_cy / obj_radius i32 and
+ * obj_valid u8 [b,m]; reg_mask [b,m] u8 = 1.  Every other entry is zero.  Errors, checked before any CUDA call:
+ * CNB_EINVAL for a null pointer, a bad shape or an agnostic_ex other than 0 / 1; CNB_EUNSUPPORTED for m > 128. */
 #define CNB_TRAIN_MAX_PIXELS 4194304
 size_t cnb_train_images_workspace_bytes(int b, int out_h, int out_w);
 int cnb_train_images(const uint8_t *src, const int64_t *src_off, const int32_t *src_hw, const double *minv6,
@@ -809,6 +823,11 @@ int cnb_ddd_targets(const float *boxes, const int32_t *cls, const int32_t *num_o
                     int64_t *ind, int64_t *rotbin, float *rotres, uint8_t *reg_mask, uint8_t *rot_mask, float *wh,
                     float *reg, void *stream);
 int cnb_ddd_gaussian_radius(const float *h, const float *w, int n, int32_t *radius, void *stream);
+int cnb_exdet_targets(const float *pts, const int32_t *cls, const int32_t *num_objs, const uint8_t *flip,
+                      const int32_t *src_hw, const double *trans6, int b, int m, int out_res, int agnostic_ex,
+                      float *reg, int64_t *ind, uint8_t *reg_mask, int32_t *obj_cls, int32_t *obj_cx, int32_t *obj_cy,
+                      int32_t *obj_radius, uint8_t *obj_valid, int32_t *ex_cls, int32_t *ex_cx, int32_t *ex_cy,
+                      int32_t *ex_radius, uint8_t *ex_valid, void *stream);
 
 #ifdef __cplusplus
 }

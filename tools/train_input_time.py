@@ -1,7 +1,7 @@
-"""Device time per ctdet, multi_pose or ddd training batch (centernet_b200.train_input), the host->device bytes per image
-against the reference loader's, and (ctdet) the numpy oracle's CPU time per image.
+"""Device time per ctdet, multi_pose, ddd or exdet training batch (centernet_b200.train_input), the host->device
+bytes per image against the reference loader's, and (ctdet) the numpy oracle's CPU time per image.
 
-    python tools/train_input_time.py [--iters 50] [--sampler ctdet|multi_pose|ddd]
+    python tools/train_input_time.py [--iters 50] [--sampler ctdet|multi_pose|ddd|exdet]
 
 Synthetic COCO-sized sources (ragged 640x480 / 480x640 / 500x375 / 427x640), 512x512 input, 80 classes, 128
 object slots, about 7 objects per image, colour augmentation on; B = 32, 64 and 114.  Per batch it times, with
@@ -20,7 +20,13 @@ JSON line, with the card's name and power limit read in the same run.
 --sampler ddd: synthetic KITTI-sized sources (ragged around 1242x375), 1280x384 input, 3 classes, 50 slots, about 8
 positives, 4 ignore objects (DontCare and single-class) and a skipped one per image, aug_ddd 0.5; B = 32 and 64,
 with point ignores and with rect_mask, each timed as build_ddd_batch with the H2D copy and from a buffer already
-on the device (kernels only).  Prints one JSON line, with the card's name and power limit read in the same run."""
+on the device (kernels only).  Prints one JSON line, with the card's name and power limit read in the same run.
+
+--sampler exdet: the COCO-sized sources at 512x512 input, 80 classes, 128 slots, about 7 objects per image with
+random extreme points on their box sides, flip 0.5 and colour augmentation on; B = 32 and 64, each timed as
+build_exdet_batch with the H2D copy and from a buffer already on the device (kernels only), with the object lists
+only and with the five dense maps.  Prints one JSON line, with the card's name, power limit and max SM clock read in
+the same run."""
 import argparse
 import json
 import os
@@ -38,6 +44,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from centernet_b200 import train_input as T  # noqa: E402
 import ddd_train_cases as DC  # noqa: E402
+import exdet_train_cases as EC  # noqa: E402
 import multi_pose_train_cases as MC  # noqa: E402
 import train_cases as TC  # noqa: E402
 
@@ -105,6 +112,29 @@ def make_ddd_samples(b, seed, rect_mask):
                  alpha=rng.uniform(-np.pi, np.pi, n), depth=rng.uniform(3, 70, n),
                  dim=list(rng.uniform(0.5, 4, (n, 3))), max_objs=50, num_classes=3, mean=DC.MEAN, std=DC.STD,
                  rect_mask=rect_mask, reg_bbox=True, reg_offset=True)
+        out.append(s)
+    return out
+
+
+def make_exdet_samples(b, seed):
+    case = dict(EC.CASES["ex_coco"])
+    opt = EC.make_opt(case)
+    rng = np.random.default_rng(seed)
+    np.random.seed(seed); random.seed(seed)
+    data_rng = np.random.RandomState(seed)
+    out = []
+    for i in range(b):
+        h, w = SIZES[i % len(SIZES)]
+        s = T.exdet_params(h, w, opt, 'train', data_rng, EC.EIG_VAL, EC.EIG_VEC)
+        n = int(rng.integers(1, 15))
+        x0, y0 = rng.uniform(0, w, n), rng.uniform(0, h, n)
+        bw, bh = rng.uniform(4, 200, n), rng.uniform(4, 200, n)
+        u = rng.random((n, 4))
+        pts = np.stack([x0 + u[:, 0] * bw, y0, x0, y0 + u[:, 1] * bh, x0 + u[:, 2] * bw, y0 + bh, x0 + bw,
+                        y0 + u[:, 3] * bh], 1).astype(np.float32)
+        s.update(image=rng.integers(0, 256, (h, w, 3), dtype=np.uint8), points=list(pts),
+                 cls=rng.integers(0, 80, n), max_objs=128, num_classes=80, mean=EC.MEAN, std=EC.STD,
+                 agnostic_ex=False, reg_offset=True)
         out.append(s)
     return out
 
@@ -189,11 +219,30 @@ def main_ddd(iters):
     print(json.dumps(res))
 
 
+def main_exdet(iters):
+    # the reference's per-image transfer: input, the five maps and the targets of exdet.py:130-135
+    m, c, r = 128, 80, 128
+    ref_bytes = 3 * 512 * 512 * 4 + 5 * c * r * r * 4 + m * (1 + 4 * (2 * 4 + 8))
+    res = {"gpu": gpu_info(), "sampler": "exdet", "batches": {}}
+    for b in (32, 64):
+        packed = T.collate_exdet(make_exdet_samples(b, b))
+        on_device = dict(packed, buffer=packed['buffer'].cuda())
+        rr = {"h2d_bytes_per_image": packed['buffer'].numel() / b, "reference_h2d_bytes_per_image": ref_bytes}
+        for dense in (False, True):
+            tag = "dense" if dense else "lists"
+            rr["ms_per_batch_" + tag] = time_batches(packed, iters, dense, T.build_exdet_batch)
+            rr["ms_per_batch_%s_kernels_only" % tag] = time_batches(on_device, iters, dense, T.build_exdet_batch)
+            rr["us_per_image_" + tag] = rr["ms_per_batch_" + tag] * 1e3 / b
+            rr["us_per_image_%s_kernels_only" % tag] = rr["ms_per_batch_%s_kernels_only" % tag] * 1e3 / b
+        res["batches"]["B%d" % b] = rr
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--oracle-images", type=int, default=4)
-    ap.add_argument("--sampler", choices=("ctdet", "multi_pose", "ddd"), default="ctdet")
+    ap.add_argument("--sampler", choices=("ctdet", "multi_pose", "ddd", "exdet"), default="ctdet")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("train_input_time: needs a CUDA device (no CPU timing is reported)")
@@ -201,6 +250,8 @@ def main():
         return main_multi_pose(args.iters)
     if args.sampler == "ddd":
         return main_ddd(args.iters)
+    if args.sampler == "exdet":
+        return main_exdet(args.iters)
     res = {"gpu": gpu_info(), "batches": {}}
     ref_bytes = 3 * 512 * 512 * 4 + 80 * 128 * 128 * 4 + 128 * (2 * 4 + 2 * 4 + 8 + 1)
     for b in (32, 64, 114):
