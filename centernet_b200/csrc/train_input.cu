@@ -276,9 +276,61 @@ __device__ __forceinline__ double gaussian_radius_f64(long long height, long lon
   return fmin(fmin(r1, r2), r3);
 }
 
+// max(0, int(gaussian_radius((ceil(h), ceil(w))))) of ctdet, multi_pose and exdet.
+__device__ __forceinline__ int radius_f64(float h, float w) {
+  const double r = gaussian_radius_f64((long long)ceilf(h), (long long)ceilf(w));
+  return r > 0.0 ? (int)r : 0;
+}
+
 // affine_transform (utils/image.py:62-65) in the plain float64 order t0 x + t1 y + t2, rounded to float32.
 __device__ __forceinline__ float affine_f32(const double *t, float x, float y) {
   return __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn(t[0], (double)x), __dmul_rn(t[1], (double)y)), t[2]));
+}
+
+// A box [x0, y0, x1, y1] on the output map, as ctdet, multi_pose and ddd place it.
+// Every field but the corners is 0 unless the box is placed (ok).
+struct MapBox {
+  bool ok;                 // h > 0 && w > 0, or forced
+  float w, h;
+  float p0, q0, p1, q1;    // the clipped corners
+  int r;                   // the sampler's radius
+  int cx, cy;              // ct_int
+  float rx, ry;            // ct - ct_int
+};
+
+// With a non-null width the box is mirrored first (bbox[[0, 2]] = width - bbox[[2, 0]] - 1 in float32).  Both
+// corners go through affine_transform and np.clip to [0, xm] x [0, ym]; h = q1 - q0 and w = p1 - p0.  A box with
+// h > 0 and w > 0, or any box under `force` (multi_pose's rotated images), is placed: Radius(h, w), then
+// ct = (p0 + p1) / 2, ct_int and the offset, all in float32.
+template <int (*Radius)(float, float)>
+__device__ __forceinline__ MapBox map_box(const float *bb, const int *width, const double *t, float xm, float ym,
+                                          bool force) {
+  float x0 = bb[0], y0 = bb[1], x1 = bb[2], y1 = bb[3];
+  if (width) {
+    const float wd = (float)*width;
+    const float nx0 = __fsub_rn(__fsub_rn(wd, x1), 1.f), nx1 = __fsub_rn(__fsub_rn(wd, x0), 1.f);
+    x0 = nx0;
+    x1 = nx1;
+  }
+  MapBox g = {};
+  g.p0 = fminf(fmaxf(affine_f32(t, x0, y0), 0.f), xm);
+  g.q0 = fminf(fmaxf(affine_f32(t + 3, x0, y0), 0.f), ym);
+  g.p1 = fminf(fmaxf(affine_f32(t, x1, y1), 0.f), xm);
+  g.q1 = fminf(fmaxf(affine_f32(t + 3, x1, y1), 0.f), ym);
+  g.h = __fsub_rn(g.q1, g.q0);
+  g.w = __fsub_rn(g.p1, g.p0);
+  g.ok = (g.h > 0.f && g.w > 0.f) || force;
+  if (g.ok) {
+    g.r = Radius(g.h, g.w);
+    const float ctx = __fdiv_rn(__fadd_rn(g.p0, g.p1), 2.f), cty = __fdiv_rn(__fadd_rn(g.q0, g.q1), 2.f);
+    g.cx = (int)ctx;
+    g.cy = (int)cty;
+    g.rx = __fsub_rn(ctx, (float)g.cx);
+    g.ry = __fsub_rn(cty, (float)g.cy);
+  } else {
+    g.w = g.h = 0.f;
+  }
+  return g;
 }
 
 __global__ void __launch_bounds__(kThreads) k_ctdet_targets(
@@ -291,67 +343,37 @@ __global__ void __launch_bounds__(kThreads) k_ctdet_targets(
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)nb * m) return;
   const int b = (int)(i / m), k = (int)(i % m);
-  float w = 0.f, h = 0.f, rx = 0.f, ry = 0.f;
-  int c = 0, cx = 0, cy = 0, rad = 0;
-  bool valid = false;
-  if (k < min(num_objs[b], m)) {
-    const float *bb = boxes + i * 4;
-    float x0 = bb[0], y0 = bb[1], x1 = bb[2], y1 = bb[3];
-    if (flip[b]) {   // bbox[[0, 2]] = width - bbox[[2, 0]] - 1 in float32
-      const float wd = (float)src_hw[2 * b + 1];
-      const float nx0 = __fsub_rn(__fsub_rn(wd, x1), 1.f), nx1 = __fsub_rn(__fsub_rn(wd, x0), 1.f);
-      x0 = nx0;
-      x1 = nx1;
-    }
-    const double *t = trans + 6 * b;
-    float p0 = affine_f32(t, x0, y0), q0 = affine_f32(t + 3, x0, y0);
-    float p1 = affine_f32(t, x1, y1), q1 = affine_f32(t + 3, x1, y1);
-    const float xm = (float)(ow - 1), ym = (float)(oh - 1);
-    p0 = fminf(fmaxf(p0, 0.f), xm);
-    p1 = fminf(fmaxf(p1, 0.f), xm);
-    q0 = fminf(fmaxf(q0, 0.f), ym);
-    q1 = fminf(fmaxf(q1, 0.f), ym);
-    h = __fsub_rn(q1, q0);
-    w = __fsub_rn(p1, p0);
-    if (h > 0.f && w > 0.f) {
-      const double r = gaussian_radius_f64((long long)ceilf(h), (long long)ceilf(w));
-      rad = r > 0.0 ? (int)r : 0;   // max(0, int(radius))
-      const float ctx = __fdiv_rn(__fadd_rn(p0, p1), 2.f), cty = __fdiv_rn(__fadd_rn(q0, q1), 2.f);
-      cx = (int)ctx;
-      cy = (int)cty;
-      rx = __fsub_rn(ctx, (float)cx);
-      ry = __fsub_rn(cty, (float)cy);
-      c = cls[i];
-      valid = true;
-    } else {
-      w = h = 0.f;
-    }
-  }
-  wh[2 * i] = w;
-  wh[2 * i + 1] = h;
-  reg[2 * i] = rx;
-  reg[2 * i + 1] = ry;
-  ind[i] = valid ? (long long)cy * ow + cx : 0;
+  MapBox g = {};
+  if (k < min(num_objs[b], m))
+    g = map_box<radius_f64>(boxes + i * 4, flip[b] ? src_hw + 2 * b + 1 : nullptr, trans + 6 * b, (float)(ow - 1),
+                            (float)(oh - 1), false);
+  const bool valid = g.ok;
+  const int c = valid ? cls[i] : 0;
+  wh[2 * i] = g.w;
+  wh[2 * i + 1] = g.h;
+  reg[2 * i] = g.rx;
+  reg[2 * i + 1] = g.ry;
+  ind[i] = (long long)g.cy * ow + g.cx;
   reg_mask[i] = valid ? 1 : 0;
   obj_cls[i] = c;
-  obj_cx[i] = cx;
-  obj_cy[i] = cy;
-  obj_radius[i] = rad;
+  obj_cx[i] = g.cx;
+  obj_cy[i] = g.cy;
+  obj_radius[i] = g.r;
   obj_valid[i] = valid ? 1 : 0;
   if (cat_spec_wh) {
     float *sw = cat_spec_wh + i * 2 * num_classes;
     unsigned char *sm = cat_spec_mask + i * 2 * num_classes;
     for (int j = 0; j < num_classes; ++j) {
       const bool on = valid && j == c;
-      sw[2 * j] = on ? w : 0.f;
-      sw[2 * j + 1] = on ? h : 0.f;
+      sw[2 * j] = on ? g.w : 0.f;
+      sw[2 * j + 1] = on ? g.h : 0.f;
       sm[2 * j] = sm[2 * j + 1] = on ? 1 : 0;
     }
   }
 }
 
 // ---------------------------------------------------------------- multi_pose targets (multi_pose.py:104-160)
-// One thread per (image, slot), looping over the joints; the box half is k_ctdet_targets' arithmetic.  A slot gets
+// One thread per (image, slot), looping over the joints; the box half is k_ctdet_targets' map_box.  A slot gets
 // targets when (h > 0 && w > 0) || rotated; reg_mask is 1 only when it has a visible joint (num_kpts != 0: the
 // visibilities are finite and >= 0, checked on the host, so the float32 sum is 0 exactly when all are) and the
 // image is not rotated.  The centre list is "got targets": hm[cls, ct] = 0.9999 for num_kpts == 0 is overwritten
@@ -371,41 +393,12 @@ __global__ void __launch_bounds__(kThreads) k_multi_pose_targets(
   const int b = (int)(i / m), k = (int)(i % m);
   const bool rot = rotated[b] != 0, fl = flip[b] != 0;
   const float wd = (float)src_hw[2 * b + 1];
-  float w = 0.f, h = 0.f, rx = 0.f, ry = 0.f;
-  int c = 0, cx = 0, cy = 0, rad = 0;
-  bool valid = false, any_kpt = false;
-  if (k < min(num_objs[b], m)) {
-    const float *bb = boxes + i * 4;
-    float x0 = bb[0], y0 = bb[1], x1 = bb[2], y1 = bb[3];
-    if (fl) {   // bbox[[0, 2]] = width - bbox[[2, 0]] - 1 in float32
-      const float nx0 = __fsub_rn(__fsub_rn(wd, x1), 1.f), nx1 = __fsub_rn(__fsub_rn(wd, x0), 1.f);
-      x0 = nx0;
-      x1 = nx1;
-    }
-    const double *t = trans + 6 * b;
-    float p0 = affine_f32(t, x0, y0), q0 = affine_f32(t + 3, x0, y0);
-    float p1 = affine_f32(t, x1, y1), q1 = affine_f32(t + 3, x1, y1);
-    const float mx = (float)(res - 1);
-    p0 = fminf(fmaxf(p0, 0.f), mx);
-    p1 = fminf(fmaxf(p1, 0.f), mx);
-    q0 = fminf(fmaxf(q0, 0.f), mx);
-    q1 = fminf(fmaxf(q1, 0.f), mx);
-    h = __fsub_rn(q1, q0);
-    w = __fsub_rn(p1, p0);
-    if ((h > 0.f && w > 0.f) || rot) {
-      const double r = gaussian_radius_f64((long long)ceilf(h), (long long)ceilf(w));
-      rad = r > 0.0 ? (int)r : 0;   // max(0, int(radius))
-      const float ctx = __fdiv_rn(__fadd_rn(p0, p1), 2.f), cty = __fdiv_rn(__fadd_rn(q0, q1), 2.f);
-      cx = (int)ctx;
-      cy = (int)cty;
-      rx = __fsub_rn(ctx, (float)cx);
-      ry = __fsub_rn(cty, (float)cy);
-      c = cls[i];
-      valid = true;
-    } else {
-      w = h = 0.f;
-    }
-  }
+  MapBox g = {};
+  if (k < min(num_objs[b], m))
+    g = map_box<radius_f64>(boxes + i * 4, fl ? src_hw + 2 * b + 1 : nullptr, trans + 6 * b, (float)(res - 1),
+                            (float)(res - 1), rot);
+  const bool valid = g.ok;
+  bool any_kpt = false;
   const float *pk = kps + i * nj * 3;
   const double *tr = trans_rot + 6 * b;
   for (int j = 0; j < nj; ++j) {
@@ -425,8 +418,8 @@ __global__ void __launch_bounds__(kThreads) k_multi_pose_targets(
           in = true;
           jx = (int)px;
           jy = (int)py;
-          hx = __fsub_rn(px, (float)cx);
-          hy = __fsub_rn(py, (float)cy);
+          hx = __fsub_rn(px, (float)g.cx);
+          hy = __fsub_rn(py, (float)g.cy);
           ox = __fsub_rn(px, (float)jx);
           oy = __fsub_rn(py, (float)jy);
         }
@@ -441,19 +434,19 @@ __global__ void __launch_bounds__(kThreads) k_multi_pose_targets(
     hp_mask[o] = in ? 1 : 0;
     hp_cx[l] = jx;
     hp_cy[l] = jy;
-    hp_radius[l] = in ? rad : 0;
+    hp_radius[l] = in ? g.r : 0;
     hp_valid[l] = in ? 1 : 0;
   }
-  wh[2 * i] = w;
-  wh[2 * i + 1] = h;
-  reg[2 * i] = rx;
-  reg[2 * i + 1] = ry;
-  ind[i] = valid ? (long long)cy * res + cx : 0;
+  wh[2 * i] = g.w;
+  wh[2 * i + 1] = g.h;
+  reg[2 * i] = g.rx;
+  reg[2 * i + 1] = g.ry;
+  ind[i] = (long long)g.cy * res + g.cx;
   reg_mask[i] = (valid && any_kpt && !rot) ? 1 : 0;
-  obj_cls[i] = c;
-  obj_cx[i] = cx;
-  obj_cy[i] = cy;
-  obj_radius[i] = rad;
+  obj_cls[i] = valid ? cls[i] : 0;
+  obj_cx[i] = g.cx;
+  obj_cy[i] = g.cy;
+  obj_radius[i] = g.r;
   obj_valid[i] = valid ? 1 : 0;
 }
 
@@ -549,7 +542,7 @@ struct DddSlot {
   bool gauss;               // draws draw_umich_gaussian(hm[cls], ct, r)
   int cx, cy, r;            // ct_int and the radius
   int ox0, oy0, ox1, oy1;   // then hm[cls, oy0:oy1 + 1, ox0:ox1 + 1] = 0.9999 (empty when ox0 > ox1)
-  float ctx, cty, w, h;
+  float rx, ry, w, h;       // the offset ct - ct_int, and the box's size on the map
 };
 
 __device__ __forceinline__ DddSlot ddd_slot(const float *bb, int cls, const double *t, int num_classes, int oh, int ow,
@@ -563,26 +556,19 @@ __device__ __forceinline__ DddSlot ddd_slot(const float *bb, int cls, const doub
   s.ox1 = -1;
   s.oy0 = 0;
   s.oy1 = -1;
-  s.ctx = s.cty = s.w = s.h = 0.f;
+  s.rx = s.ry = s.w = s.h = 0.f;
   const bool pos = cls >= 0 && cls < num_classes;
   const bool ign = cls == -1 || (cls <= -2 && cls >= -num_classes - 1);
   if (!pos && !ign) return s;
-  float p0 = affine_f32(t, bb[0], bb[1]), q0 = affine_f32(t + 3, bb[0], bb[1]);
-  float p1 = affine_f32(t, bb[2], bb[3]), q1 = affine_f32(t + 3, bb[2], bb[3]);
-  const float xm = (float)(ow - 1), ym = (float)(oh - 1);
-  p0 = fminf(fmaxf(p0, 0.f), xm);
-  p1 = fminf(fmaxf(p1, 0.f), xm);
-  q0 = fminf(fmaxf(q0, 0.f), ym);
-  q1 = fminf(fmaxf(q1, 0.f), ym);
-  const float h = __fsub_rn(q1, q0), w = __fsub_rn(p1, p0);
-  if (!(h > 0.f && w > 0.f)) return s;
-  s.h = h;
-  s.w = w;
-  s.r = ddd_radius(h, w);
-  s.ctx = __fdiv_rn(__fadd_rn(p0, p1), 2.f);
-  s.cty = __fdiv_rn(__fadd_rn(q0, q1), 2.f);
-  s.cx = (int)s.ctx;
-  s.cy = (int)s.cty;
+  const MapBox g = map_box<ddd_radius>(bb, nullptr, t, (float)(ow - 1), (float)(oh - 1), false);
+  if (!g.ok) return s;
+  s.h = g.h;
+  s.w = g.w;
+  s.r = g.r;
+  s.rx = g.rx;
+  s.ry = g.ry;
+  s.cx = g.cx;
+  s.cy = g.cy;
   if (pos) {
     s.kind = 1;
     s.cls = cls;
@@ -591,10 +577,10 @@ __device__ __forceinline__ DddSlot ddd_slot(const float *bb, int cls, const doub
     s.kind = 2;
     s.cls = cls == -1 ? -1 : -cls - 2;
     if (rect_mask) {   // hm[ignore_id, int(y0):int(y1) + 1, int(x0):int(x1) + 1] = 0.9999
-      s.ox0 = (int)p0;
-      s.ox1 = (int)p1;
-      s.oy0 = (int)q0;
-      s.oy1 = (int)q1;
+      s.ox0 = (int)g.p0;
+      s.ox1 = (int)g.p1;
+      s.oy0 = (int)g.q0;
+      s.oy1 = (int)g.q1;
     } else {           // the Gaussian, then hm[ignore_id, ct_int.y, ct_int.x] = 0.9999
       s.gauss = true;
       s.ox0 = s.ox1 = s.cx;
@@ -637,8 +623,8 @@ __global__ void __launch_bounds__(kThreads) k_ddd_targets(
   }
   wh[2 * i] = on ? s.w : 0.f;
   wh[2 * i + 1] = on ? s.h : 0.f;
-  reg[2 * i] = on ? __fsub_rn(s.ctx, (float)s.cx) : 0.f;
-  reg[2 * i + 1] = on ? __fsub_rn(s.cty, (float)s.cy) : 0.f;
+  reg[2 * i] = on ? s.rx : 0.f;
+  reg[2 * i + 1] = on ? s.ry : 0.f;
   ind[i] = on ? (long long)s.cy * ow + s.cx : 0;
   dep[i] = on ? depth[i] : 0.f;
   dim_out[3 * i] = on ? dim[3 * i] : 0.f;
@@ -778,8 +764,7 @@ __global__ void __launch_bounds__(kThreads) k_exdet_targets(
     const float h = __fsub_rn(py[2], py[0]), w = __fsub_rn(px[3], px[1]);
     valid = h > 0.f && w > 0.f;
     if (valid) {
-      const double r = gaussian_radius_f64((long long)ceilf(h), (long long)ceilf(w));
-      rad = r > 0.0 ? (int)r : 0;   // max(0, int(radius))
+      rad = radius_f64(h, w);
       cx = (int)__fdiv_rn(__fadd_rn(px[3], px[1]), 2.f);
       cy = (int)__fdiv_rn(__fadd_rn(py[0], py[2]), 2.f);
       c = cls[i];

@@ -94,10 +94,24 @@ def crop_draws(height, width, c, s, opt):
     return s
 
 
-def color_draws(data_rng, eig_val, eig_vec):
-    """color_aug's draws (utils/image.py:221-230): random.shuffle of its three functions, one data_rng.uniform
-    per blend in the order they run, then the lighting normal.  Returns (order code, blend [6] float32 (alpha,
-    1 - alpha) of brightness, contrast, saturation, light [3] float64)."""
+def scale_shift_draws(height, width, c, s, opt):
+    """ddd's aug_ddd draws (ddd.py:47-51) and exdet's not_rand_crop draws (exdet.py:49-53): three randn in the order
+    scale, x shift, y shift, the shifts scaled by the image's width and height (not by s, as crop_draws scales
+    them).  Updates the float64 centre c in place; returns the scale."""
+    sf, cf = opt.scale, opt.shift
+    s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
+    c[0] += width * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+    c[1] += height * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+    return s
+
+
+def color_draws(split, opt, data_rng, eig_val, eig_vec):
+    """color_aug's draws (utils/image.py:221-230) in the train split without opt.no_color_aug: random.shuffle of its
+    three functions, one data_rng.uniform per blend in the order they run, then the lighting normal.  Returns
+    (order code, blend [6] float32 (alpha, 1 - alpha) of brightness, contrast, saturation, light [3] float64);
+    otherwise draws nothing and returns (-1, zeros, zeros), no colour augmentation."""
+    if split != 'train' or opt.no_color_aug:
+        return -1, np.zeros(6, F32), np.zeros(3, np.float64)
     blend = np.zeros(6, F32)
     kinds = [0, 1, 2]
     random.shuffle(kinds)
@@ -126,9 +140,7 @@ def sample_params(height, width, opt, split, data_rng, eig_val, eig_vec):
         if np.random.random() < opt.flip:
             flipped = True
             c[0] = width - c[0] - 1
-    order, blend, light = -1, np.zeros(6, F32), np.zeros(3, np.float64)
-    if split == 'train' and not opt.no_color_aug:
-        order, blend, light = color_draws(data_rng, eig_val, eig_vec)
+    order, blend, light = color_draws(split, opt, data_rng, eig_val, eig_vec)
     output_h, output_w = input_h // opt.down_ratio, input_w // opt.down_ratio
     return {'c': c, 's': s, 'flip': flipped, 'input_h': input_h, 'input_w': input_w,
             'output_h': output_h, 'output_w': output_w,
@@ -137,18 +149,21 @@ def sample_params(height, width, opt, split, data_rng, eig_val, eig_vec):
             'order': order, 'blend': blend, 'light': light}
 
 
-class CTDetTrainInput(torch.utils.data.Dataset):
-    """Wraps a reference CTDetDataset instance (duck-typed on opt, coco, images, img_dir, max_objs, cat_ids,
-    num_classes, mean, std, _data_rng, _eig_val, _eig_vec and split).  __getitem__ reads the image and the
-    annotations and draws the random parameters as the reference does, and returns them with the uint8 image and
-    the float32 box corners; it does no pixel work (collate_ctdet + build_ctdet_batch do)."""
+class _TrainInput(torch.utils.data.Dataset):
+    """Wraps a reference dataset instance, duck-typed on opt, coco, images, img_dir, max_objs, mean, std and split
+    plus what the sampler's own fields read.  __getitem__ reads the image and its first max_objs annotations (no
+    random draws), then makes the sampler's draws as the reference does and returns them with the uint8 image and
+    the sampler's annotation fields; it does no pixel work (the sampler's collate_* + build_*_batch do).  The
+    constructor rejects opt.mse_loss and the opt flags in `unsupported`, whose targets are not implemented."""
+    unsupported = ()
 
     def __init__(self, dataset):
-        opt = dataset.opt
+        opt, name = dataset.opt, type(self).__name__
         if opt.mse_loss:
-            raise NotImplementedError("CTDetTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not implemented")
-        if opt.dense_wh:
-            raise NotImplementedError("CTDetTrainInput: opt.dense_wh targets are not implemented")
+            raise NotImplementedError("%s: opt.mse_loss (draw_msra_gaussian targets) is not implemented" % name)
+        for flag in self.unsupported:
+            if getattr(opt, flag):
+                raise NotImplementedError("%s: opt.%s targets are not implemented" % (name, flag))
         self.dataset = dataset
 
     def __len__(self):
@@ -159,20 +174,35 @@ class CTDetTrainInput(torch.utils.data.Dataset):
         ds = self.dataset
         img_id = ds.images[index]
         file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
-        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
-        num_objs = min(len(anns), ds.max_objs)
+        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))[:ds.max_objs]
         img = cv2.imread(os.path.join(ds.img_dir, file_name))
-        sample = sample_params(img.shape[0], img.shape[1], ds.opt, ds.split, ds._data_rng, ds._eig_val, ds._eig_vec)
-        boxes = np.zeros((num_objs, 4), F32)
-        cls = np.zeros(num_objs, np.int32)
-        for k in range(num_objs):
-            b = anns[k]['bbox']
-            boxes[k] = np.array([b[0], b[1], b[0] + b[2], b[1] + b[3]], dtype=np.float32)
-            cls[k] = int(ds.cat_ids[anns[k]['category_id']])
-        sample.update(image=img, boxes=boxes, cls=cls, max_objs=ds.max_objs, num_classes=ds.num_classes,
-                      mean=np.asarray(ds.mean, F32).reshape(3), std=np.asarray(ds.std, F32).reshape(3),
-                      cat_spec_wh=bool(ds.opt.cat_spec_wh), reg_offset=bool(ds.opt.reg_offset))
+        sample = self._params(ds, img.shape[0], img.shape[1])
+        sample.update(self._fields(ds, anns), image=img, max_objs=ds.max_objs, mean=np.asarray(ds.mean, F32).reshape(3),
+                      std=np.asarray(ds.std, F32).reshape(3), reg_offset=bool(ds.opt.reg_offset))
         return sample
+
+
+def _boxes(anns):
+    """_coco_box_to_bbox of each annotation's bbox: [n, 4] float32 corners."""
+    boxes = np.zeros((len(anns), 4), F32)
+    for k, a in enumerate(anns):
+        b = a['bbox']
+        boxes[k] = np.array([b[0], b[1], b[0] + b[2], b[1] + b[3]], dtype=np.float32)
+    return boxes
+
+
+class CTDetTrainInput(_TrainInput):
+    """Wraps a reference CTDetDataset instance (also duck-typed on cat_ids, num_classes, _data_rng, _eig_val and
+    _eig_vec): sample_params' draws, the float32 box corners and the class cat_ids[category_id]; the batch is
+    collate_ctdet + build_ctdet_batch's.  opt.dense_wh is rejected."""
+    unsupported = ('dense_wh',)
+
+    def _params(self, ds, height, width):
+        return sample_params(height, width, ds.opt, ds.split, ds._data_rng, ds._eig_val, ds._eig_vec)
+
+    def _fields(self, ds, anns):
+        return {'boxes': _boxes(anns), 'cls': np.array([int(ds.cat_ids[a['category_id']]) for a in anns], np.int32),
+                'num_classes': ds.num_classes, 'cat_spec_wh': bool(ds.opt.cat_spec_wh)}
 
 
 class _Packer(object):
@@ -193,6 +223,10 @@ class _Packer(object):
         for off, a in self.parts:
             host[off:off + a.size] = a
         return buf
+
+    def collated(self, scalars):
+        """A collate_* result: the buffer (pinned in the main process), its layout and the scalars."""
+        return {'buffer': self.tensor(_pin()), 'layout': self.layout, 'scalars': scalars}
 
 
 def _pin():
@@ -225,6 +259,33 @@ def _pack_images(pk, images, minv, flip, order, blend, light, mean, std):
     pk.add('norm', np.concatenate([np.asarray(mean, F32).reshape(3), np.asarray(std, F32).reshape(3)]))
 
 
+def _collate(samples, what, keys, same=None, slots=True, color=True):
+    """What every collate_* (named `what` in the messages) does before it packs its slot arrays.  Raises ValueError
+    when the samples differ in `same` (default: keys), for an image that is not uint8 [H, W, 3] and, with `slots`,
+    for max_objs outside [1, 128] (FocalSplatLoss / splat_gaussian, the ddd heat map).  Packs the images -- with
+    `color` the samples' flips and colour parameters, else neither -- and trans_output.  Returns the packer and the
+    scalars: `keys` of the first sample, batch and color (any colour augmentation)."""
+    s0 = samples[0]
+    for s in samples:
+        if any(s[k] != s0[k] for k in (keys if same is None else same)):
+            raise ValueError("%s: samples with different settings cannot be batched" % what)
+    images = [s['image'] for s in samples]
+    _check_images(images)
+    b, m = len(samples), int(s0['max_objs'])
+    if slots and not 1 <= m <= 128:
+        raise ValueError("%s: 1 to 128 object slots, got %d" % (what, m))
+    if color:
+        flip, order, blend, light = ([s[k] for s in samples] for k in ('flip', 'order', 'blend', 'light'))
+    else:
+        flip, order, blend, light = np.zeros(b, np.uint8), np.full(b, -1), np.zeros((b, 6), F32), np.zeros((b, 3))
+    pk = _Packer()
+    _pack_images(pk, images, [s['minv'] for s in samples], flip, order, blend, light, s0['mean'], s0['std'])
+    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
+    scalars = {k: s0[k] for k in keys}
+    scalars.update(batch=b, color=any(o >= 0 for o in order))
+    return pk, scalars
+
+
 def _views(buf, layout):
     out = {}
     for name, (off, dt, shape) in layout.items():
@@ -253,6 +314,25 @@ def _launch_images(v, b, out_h, out_w, color, dtype, memory_format, dev):
 
 def _device(device):
     return torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+
+
+def _upload(packed, device, out_h, out_w, dtype, memory_format):
+    """A collate_* result's one non-blocking H2D copy on the current stream and the image pass at out_h x out_w:
+    returns the views of the device buffer and 'input'."""
+    dev = _device(device)
+    sc = packed['scalars']
+    v = _views(packed['buffer'].to(dev, non_blocking=True), packed['layout'])
+    return v, _launch_images(v, sc['batch'], out_h, out_w, sc['color'], dtype, memory_format, dev)
+
+
+# The FocalSplatLoss object lists, returned as obj_*, hp_* (no class) and ex_*.
+_LIST_KEYS = ('cls', 'cx', 'cy', 'radius', 'valid')
+
+
+def _lists(shape, dev, n=5):
+    """The last n of the _LIST_KEYS lists, of `shape`: int32, and uint8 for valid."""
+    return [torch.empty(shape, dtype=torch.int32, device=dev) for _ in range(n - 1)] + \
+        [torch.empty(shape, dtype=torch.uint8, device=dev)]
 
 
 def augment_images(images, matrices, out_h, out_w, mean, std, flips=None, orders=None, blends=None, lights=None,
@@ -291,8 +371,8 @@ def collate_ctdet(samples):
         if (s['input_h'], s['input_w']) != (s0['input_h'], s0['input_w']):
             raise ValueError("collate_ctdet: samples of different input sizes (%dx%d and %dx%d) cannot be batched"
                              % (s0['input_h'], s0['input_w'], s['input_h'], s['input_w']))
-    images = [s['image'] for s in samples]
-    _check_images(images)
+    pk, scalars = _collate(samples, 'collate_ctdet', ('input_h', 'input_w', 'output_h', 'output_w', 'max_objs',
+                                                      'num_classes', 'cat_spec_wh', 'reg_offset'), same=(), slots=False)
     b, m = len(samples), int(s0['max_objs'])
     boxes = np.zeros((b, m, 4), F32)
     cls = np.zeros((b, m), np.int32)
@@ -302,18 +382,10 @@ def collate_ctdet(samples):
         boxes[i, :n], cls[i, :n], nobj[i] = s['boxes'][:n], s['cls'][:n], n
         if n and (cls[i, :n].min() < 0 or cls[i, :n].max() >= s0['num_classes']):
             raise ValueError("collate_ctdet: class id outside [0, %d)" % s0['num_classes'])
-    pk = _Packer()
-    _pack_images(pk, images, [s['minv'] for s in samples], [s['flip'] for s in samples],
-                 [s['order'] for s in samples], [s['blend'] for s in samples], [s['light'] for s in samples],
-                 s0['mean'], s0['std'])
-    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
     pk.add('nobj', nobj)
     pk.add('boxes', boxes)
     pk.add('cls', cls)
-    scalars = {k: s0[k] for k in ('input_h', 'input_w', 'output_h', 'output_w', 'max_objs', 'num_classes',
-                                  'cat_spec_wh', 'reg_offset')}
-    scalars.update(batch=b, color=any(s['order'] >= 0 for s in samples))
-    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+    return pk.collated(scalars)
 
 
 def build_ctdet_batch(packed, device=None, dtype=torch.float32, memory_format=torch.contiguous_format,
@@ -323,20 +395,17 @@ def build_ctdet_batch(packed, device=None, dtype=torch.float32, memory_format=to
     plus splat_gaussian with dense_hm.  Keys, shapes and dtypes as ctdet.py:128-140 returns them; 'hm' only with
     dense_hm; always the FocalSplatLoss lists obj_cls, obj_cx, obj_cy, obj_radius (int32) and obj_valid (uint8).
     The packed host buffer is not modified."""
-    dev = _device(device)
     sc = packed['scalars']
     b, m, nc, oh, ow = sc['batch'], sc['max_objs'], sc['num_classes'], sc['output_h'], sc['output_w']
-    buf = packed['buffer'].to(dev, non_blocking=True)
-    v = _views(buf, packed['layout'])
-    inp = _launch_images(v, b, sc['input_h'], sc['input_w'], sc['color'], dtype, memory_format, dev)
+    v, inp = _upload(packed, device, sc['input_h'], sc['input_w'], dtype, memory_format)
+    dev = inp.device
     f32 = dict(dtype=torch.float32, device=dev)
     u8 = dict(dtype=torch.uint8, device=dev)
-    i32 = dict(dtype=torch.int32, device=dev)
     wh, reg = torch.empty((b, m, 2), **f32), torch.empty((b, m, 2), **f32)
     ind, reg_mask = torch.empty((b, m), dtype=torch.int64, device=dev), torch.empty((b, m), **u8)
     csw = torch.empty((b, m, 2 * nc), **f32) if sc['cat_spec_wh'] else None
     csm = torch.empty((b, m, 2 * nc), **u8) if sc['cat_spec_wh'] else None
-    lists = [torch.empty((b, m), **i32) for _ in range(4)] + [torch.empty((b, m), **u8)]
+    lists = _lists((b, m), dev)
     C.ctdet_targets(ptr(v['boxes']), ptr(v['cls']), ptr(v['nobj']), ptr(v['flip']), ptr(v['src_hw']),
                     ptr(v['trans_output']), b, m, nc, oh, ow, ptr(wh), ptr(ind), ptr(reg), ptr(reg_mask), ptr(csw),
                     ptr(csm), *[ptr(t) for t in lists], stream_ptr(wh))
@@ -349,7 +418,7 @@ def build_ctdet_batch(packed, device=None, dtype=torch.float32, memory_format=to
         ret['wh'] = wh
     if sc['reg_offset']:
         ret['reg'] = reg
-    ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
+    ret.update(('obj_' + k, t) for k, t in zip(_LIST_KEYS, lists))
     return ret
 
 
@@ -372,9 +441,7 @@ def multi_pose_params(height, width, opt, split, data_rng, eig_val, eig_vec):
         if np.random.random() < opt.flip:
             flipped = True
             c[0] = width - c[0] - 1
-    order, blend, light = -1, np.zeros(6, F32), np.zeros(3, np.float64)
-    if split == 'train' and not opt.no_color_aug:
-        order, blend, light = color_draws(data_rng, eig_val, eig_vec)
+    order, blend, light = color_draws(split, opt, data_rng, eig_val, eig_vec)
     res, out_res = int(opt.input_res), int(opt.output_res)
     return {'c': c, 's': s, 'rot': rot, 'flip': flipped, 'input_res': res, 'output_res': out_res,
             'minv': np.array(_invert(affine_transform(c, s, [res, res], rot)), np.float64),
@@ -383,49 +450,23 @@ def multi_pose_params(height, width, opt, split, data_rng, eig_val, eig_vec):
             'order': order, 'blend': blend, 'light': light}
 
 
-class MultiPoseTrainInput(torch.utils.data.Dataset):
-    """Wraps a reference MultiPoseDataset instance (duck-typed on opt, coco, images, img_dir, max_objs,
-    num_classes, num_joints, flip_idx, mean, std, _data_rng, _eig_val, _eig_vec and split).  __getitem__ reads the
-    image, the annotations and their keypoints and draws the random parameters as the reference does; it does no
-    pixel work (collate_multi_pose + build_multi_pose_batch do).  The class is int(category_id) - 1, as there."""
+class MultiPoseTrainInput(_TrainInput):
+    """Wraps a reference MultiPoseDataset instance (also duck-typed on num_classes, num_joints, flip_idx, _data_rng,
+    _eig_val and _eig_vec): multi_pose_params' draws, the float32 box corners, the keypoints and the class
+    int(category_id) - 1, as there; the batch is collate_multi_pose + build_multi_pose_batch's.  opt.dense_hp is
+    rejected."""
+    unsupported = ('dense_hp',)
 
-    def __init__(self, dataset):
-        opt = dataset.opt
-        if opt.mse_loss:
-            raise NotImplementedError("MultiPoseTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not "
-                                      "implemented")
-        if opt.dense_hp:
-            raise NotImplementedError("MultiPoseTrainInput: opt.dense_hp targets are not implemented")
-        self.dataset = dataset
+    def _params(self, ds, height, width):
+        return multi_pose_params(height, width, ds.opt, ds.split, ds._data_rng, ds._eig_val, ds._eig_vec)
 
-    def __len__(self):
-        return len(self.dataset)
-
-    def __getitem__(self, index):
-        import cv2
-        ds = self.dataset
-        img_id = ds.images[index]
-        file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
-        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
-        num_objs = min(len(anns), ds.max_objs)
-        img = cv2.imread(os.path.join(ds.img_dir, file_name))
-        sample = multi_pose_params(img.shape[0], img.shape[1], ds.opt, ds.split, ds._data_rng, ds._eig_val,
-                                   ds._eig_vec)
-        boxes = np.zeros((num_objs, 4), F32)
-        cls = np.zeros(num_objs, np.int64)
-        kps = []
-        for k in range(num_objs):
-            b = anns[k]['bbox']
-            boxes[k] = np.array([b[0], b[1], b[0] + b[2], b[1] + b[3]], dtype=np.float32)
-            cls[k] = int(anns[k]['category_id']) - 1
-            kps.append(np.array(anns[k]['keypoints'], np.float32).reshape(-1))
+    def _fields(self, ds, anns):
         opt = ds.opt
-        sample.update(image=img, boxes=boxes, cls=cls, keypoints=kps, max_objs=ds.max_objs,
-                      num_classes=ds.num_classes, num_joints=ds.num_joints,
-                      flip_idx=[tuple(e) for e in ds.flip_idx], mean=np.asarray(ds.mean, F32).reshape(3),
-                      std=np.asarray(ds.std, F32).reshape(3), reg_offset=bool(opt.reg_offset),
-                      hm_hp=bool(opt.hm_hp), reg_hp_offset=bool(opt.reg_hp_offset))
-        return sample
+        return {'boxes': _boxes(anns), 'cls': np.array([int(a['category_id']) - 1 for a in anns], np.int64),
+                'keypoints': [np.array(a['keypoints'], np.float32).reshape(-1) for a in anns],
+                'num_classes': ds.num_classes, 'num_joints': ds.num_joints,
+                'flip_idx': [tuple(e) for e in ds.flip_idx], 'hm_hp': bool(opt.hm_hp),
+                'reg_hp_offset': bool(opt.reg_hp_offset)}
 
 
 def flip_permutation(num_joints, flip_idx):
@@ -444,16 +485,9 @@ def collate_multi_pose(samples):
     length is not 3 J, a visibility that is negative or not finite, a class outside [0, num_classes), more than
     128 slots, a rotated sample with a box of negative width or height, or samples of different settings."""
     s0 = samples[0]
-    keys = ('input_res', 'output_res', 'max_objs', 'num_classes', 'num_joints', 'flip_idx', 'reg_offset', 'hm_hp',
-            'reg_hp_offset')
-    for s in samples:
-        if any(s[k] != s0[k] for k in keys):
-            raise ValueError("collate_multi_pose: samples with different settings cannot be batched")
-    images = [s['image'] for s in samples]
-    _check_images(images)
+    keys = ('input_res', 'output_res', 'max_objs', 'num_classes', 'num_joints', 'reg_offset', 'hm_hp', 'reg_hp_offset')
+    pk, scalars = _collate(samples, 'collate_multi_pose', keys, same=keys + ('flip_idx',))
     b, m, nj, nc = len(samples), int(s0['max_objs']), int(s0['num_joints']), int(s0['num_classes'])
-    if not 1 <= m <= 128:
-        raise ValueError("collate_multi_pose: 1 to 128 object slots (FocalSplatLoss / splat_gaussian), got %d" % m)
     if nj < 1:
         raise ValueError("collate_multi_pose: no joints")
     perm = flip_permutation(nj, s0['flip_idx'])
@@ -481,11 +515,6 @@ def collate_multi_pose(samples):
             raise ValueError("collate_multi_pose: a box with negative width or height in a rotated sample "
                              "(gaussian_radius of it is NaN in the reference)")
         boxes[i, :n], cls[i, :n] = bx, c
-    pk = _Packer()
-    _pack_images(pk, images, [s['minv'] for s in samples], [s['flip'] for s in samples],
-                 [s['order'] for s in samples], [s['blend'] for s in samples], [s['light'] for s in samples],
-                 s0['mean'], s0['std'])
-    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
     pk.add('trans_output_rot', np.array([s['trans_output_rot'] for s in samples], np.float64).reshape(b, 6))
     pk.add('nobj', nobj)
     pk.add('boxes', boxes)
@@ -493,10 +522,8 @@ def collate_multi_pose(samples):
     pk.add('kps', kps)
     pk.add('rotated', rotated)
     pk.add('perm', perm)
-    scalars = {k: s0[k] for k in ('input_res', 'output_res', 'max_objs', 'num_classes', 'num_joints', 'reg_offset',
-                                  'hm_hp', 'reg_hp_offset')}
-    scalars.update(batch=b, color=any(s['order'] >= 0 for s in samples), rotated=rotated.astype(bool).tolist())
-    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+    scalars['rotated'] = rotated.astype(bool).tolist()
+    return pk.collated(scalars)
 
 
 def build_multi_pose_batch(packed, device=None, dtype=torch.float32, memory_format=torch.contiguous_format,
@@ -515,22 +542,18 @@ def build_multi_pose_batch(packed, device=None, dtype=torch.float32, memory_form
     if not dense_hm and any(sc['rotated']):
         raise ValueError("build_multi_pose_batch: a rotated sample's hm is the constant 0.9999, which the object "
                          "lists cannot express; use dense_hm=True")
-    dev = _device(device)
     b, m, nj, nc, r = sc['batch'], sc['max_objs'], sc['num_joints'], sc['num_classes'], sc['output_res']
-    buf = packed['buffer'].to(dev, non_blocking=True)
-    v = _views(buf, packed['layout'])
-    inp = _launch_images(v, b, sc['input_res'], sc['input_res'], sc['color'], dtype, memory_format, dev)
+    v, inp = _upload(packed, device, sc['input_res'], sc['input_res'], dtype, memory_format)
+    dev = inp.device
     f32 = dict(dtype=torch.float32, device=dev)
     u8 = dict(dtype=torch.uint8, device=dev)
-    i32 = dict(dtype=torch.int32, device=dev)
     i64 = dict(dtype=torch.int64, device=dev)
     wh, reg = torch.empty((b, m, 2), **f32), torch.empty((b, m, 2), **f32)
     ind, reg_mask = torch.empty((b, m), **i64), torch.empty((b, m), **u8)
     hps, hps_mask = torch.empty((b, m, 2 * nj), **f32), torch.empty((b, m, 2 * nj), **u8)
     hp_offset, hp_ind, hp_mask = torch.empty((b, m * nj, 2), **f32), torch.empty((b, m * nj), **i64), \
         torch.empty((b, m * nj), **i64)
-    lists = [torch.empty((b, m), **i32) for _ in range(4)] + [torch.empty((b, m), **u8)]
-    hp_lists = [torch.empty((b, nj, m), **i32) for _ in range(3)] + [torch.empty((b, nj, m), **u8)]
+    lists, hp_lists = _lists((b, m), dev), _lists((b, nj, m), dev, 4)
     C.multi_pose_targets(ptr(v['boxes']), ptr(v['cls']), ptr(v['nobj']), ptr(v['kps']), ptr(v['flip']),
                          ptr(v['rotated']), ptr(v['src_hw']), ptr(v['trans_output']), ptr(v['trans_output_rot']),
                          ptr(v['perm']), b, m, nj, r, ptr(wh), ptr(ind), ptr(reg), ptr(reg_mask), ptr(hps),
@@ -550,9 +573,9 @@ def build_multi_pose_batch(packed, device=None, dtype=torch.float32, memory_form
         ret['hm_hp'] = splat_gaussian(torch.zeros_like(flat[0]), *flat, 1, r, r).view(b, nj, r, r)
     if sc['reg_hp_offset']:
         ret.update(hp_offset=hp_offset, hp_ind=hp_ind, hp_mask=hp_mask)
-    ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
+    ret.update(('obj_' + k, t) for k, t in zip(_LIST_KEYS, lists))
     if sc['hm_hp']:
-        ret.update(zip(('hp_cx', 'hp_cy', 'hp_radius', 'hp_valid'), hp_lists))
+        ret.update(('hp_' + k, t) for k, t in zip(_LIST_KEYS[1:], hp_lists))
     return ret
 
 
@@ -560,9 +583,9 @@ def build_multi_pose_batch(packed, device=None, dtype=torch.float32, memory_form
 def ddd_params(height, width, opt, split):
     """The random draws of DddDataset.__getitem__ (ddd.py:37-66) for one height x width image and the matrices they
     give.  Only np.random draws: in the train split one np.random.random() < aug_ddd (none in val: the `and`
-    short-circuits) and, when it succeeds, three randn in the order scale, x shift, y shift, the shifts scaled by
-    the image's width and height.  There is no flip and no colour augmentation.  The centre is float64 and the scale
-    an int32 pair ([input_w, input_h] under keep_res, else [width, height]), float64 once augmented."""
+    short-circuits) and, when it succeeds, scale_shift_draws.  There is no flip and no colour augmentation.  The
+    centre is float64 and the scale an int32 pair ([input_w, input_h] under keep_res, else [width, height]), float64
+    once augmented."""
     c = np.array([width / 2., height / 2.])
     if opt.keep_res:
         s = np.array([opt.input_w, opt.input_h], dtype=np.int32)
@@ -571,10 +594,7 @@ def ddd_params(height, width, opt, split):
     aug = False
     if split == 'train' and np.random.random() < opt.aug_ddd:
         aug = True
-        sf, cf = opt.scale, opt.shift
-        s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
-        c[0] += width * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
-        c[1] += height * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+        s = scale_shift_draws(height, width, c, s, opt)
     input_h, input_w = int(opt.input_h), int(opt.input_w)
     output_h, output_w = int(opt.output_h), int(opt.output_w)
     return {'c': c, 's': s, 'aug': aug, 'input_h': input_h, 'input_w': input_w, 'output_h': output_h,
@@ -586,51 +606,24 @@ def ddd_params(height, width, opt, split):
 _DDD_IGNORED = {'alpha': 0., 'depth': 0., 'dim': [0., 0., 0.]}
 
 
-class DddTrainInput(torch.utils.data.Dataset):
-    """Wraps a reference DddDataset instance (duck-typed on opt, coco, images, img_dir, max_objs, cat_ids,
-    alpha_in_degree, mean, std and split).  __getitem__ reads the image and the annotations -- box, class
-    cat_ids[category_id], _convert_alpha(alpha) as float64, depth and dim -- and draws the parameters as the
-    reference does; it does no pixel work (collate_ddd + build_ddd_batch do).  The number of classes is
-    opt.num_classes, as there."""
+class DddTrainInput(_TrainInput):
+    """Wraps a reference DddDataset instance (also duck-typed on cat_ids and alpha_in_degree): ddd_params' draws and
+    per annotation the float32 box corners, the class cat_ids[category_id], _convert_alpha(alpha) as float64, depth
+    and dim; the batch is collate_ddd + build_ddd_batch's.  The number of classes is opt.num_classes, as there."""
 
-    def __init__(self, dataset):
-        if dataset.opt.mse_loss:
-            raise NotImplementedError("DddTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not implemented")
-        self.dataset = dataset
+    def _params(self, ds, height, width):
+        return ddd_params(height, width, ds.opt, ds.split)
 
-    def __len__(self):
-        return len(self.dataset)
-
-    def __getitem__(self, index):
-        import cv2
-        ds = self.dataset
-        img_id = ds.images[index]
-        file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
-        img = cv2.imread(os.path.join(ds.img_dir, file_name))
+    def _fields(self, ds, anns):
         opt = ds.opt
-        sample = ddd_params(img.shape[0], img.shape[1], opt, ds.split)
-        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
-        num_objs = min(len(anns), ds.max_objs)
-        boxes = np.zeros((num_objs, 4), F32)
-        cls = np.zeros(num_objs, np.int64)
-        alpha = np.zeros(num_objs, np.float64)
-        depth = np.zeros(num_objs, np.float64)
-        dims = []
-        for k in range(num_objs):
-            a = anns[k]
-            b = a['bbox']
-            boxes[k] = np.array([b[0], b[1], b[0] + b[2], b[1] + b[3]], dtype=np.float32)
-            cls[k] = int(ds.cat_ids[a['category_id']])
-            # only positive classes read these in the reference; an ignore object may lack them
-            val = a if cls[k] >= 0 else dict(_DDD_IGNORED, **a)
-            alpha[k] = math.radians(val['alpha'] + 45) if ds.alpha_in_degree else val['alpha']
-            depth[k] = val['depth']
-            dims.append(np.asarray(val['dim'], np.float64).reshape(-1))
-        sample.update(image=img, boxes=boxes, cls=cls, alpha=alpha, depth=depth, dim=dims, max_objs=ds.max_objs,
-                      num_classes=int(opt.num_classes), mean=np.asarray(ds.mean, F32).reshape(3),
-                      std=np.asarray(ds.std, F32).reshape(3), rect_mask=bool(opt.rect_mask),
-                      reg_bbox=bool(opt.reg_bbox), reg_offset=bool(opt.reg_offset))
-        return sample
+        cls = np.array([int(ds.cat_ids[a['category_id']]) for a in anns], np.int64)
+        # only positive classes read these in the reference; an ignore object may lack them
+        vals = [a if c >= 0 else dict(_DDD_IGNORED, **a) for a, c in zip(anns, cls)]
+        alpha = [math.radians(v['alpha'] + 45) if ds.alpha_in_degree else v['alpha'] for v in vals]
+        return {'boxes': _boxes(anns), 'cls': cls, 'alpha': np.array(alpha, np.float64),
+                'depth': np.array([v['depth'] for v in vals], np.float64),
+                'dim': [np.asarray(v['dim'], np.float64).reshape(-1) for v in vals],
+                'num_classes': int(opt.num_classes), 'rect_mask': bool(opt.rect_mask), 'reg_bbox': bool(opt.reg_bbox)}
 
 
 def collate_ddd(samples):
@@ -641,14 +634,8 @@ def collate_ddd(samples):
     s0 = samples[0]
     keys = ('input_h', 'input_w', 'output_h', 'output_w', 'max_objs', 'num_classes', 'rect_mask', 'reg_bbox',
             'reg_offset')
-    for s in samples:
-        if any(s[k] != s0[k] for k in keys):
-            raise ValueError("collate_ddd: samples with different settings cannot be batched")
-    images = [s['image'] for s in samples]
-    _check_images(images)
+    pk, scalars = _collate(samples, 'collate_ddd', keys, color=False)
     b, m, nc = len(samples), int(s0['max_objs']), int(s0['num_classes'])
-    if not 1 <= m <= 128:
-        raise ValueError("collate_ddd: 1 to 128 object slots, got %d" % m)
     boxes = np.zeros((b, m, 4), F32)
     cls = np.zeros((b, m), np.int32)
     alpha = np.zeros((b, m), np.float64)
@@ -672,10 +659,6 @@ def collate_ddd(samples):
         cls[i, :n] = np.maximum(c, -99)
         alpha[i, :n] = np.asarray(s['alpha'][:n], np.float64)
         depth[i, :n] = np.asarray(s['depth'][:n], np.float64)
-    pk = _Packer()
-    _pack_images(pk, images, [s['minv'] for s in samples], np.zeros(b, np.uint8), np.full(b, -1),
-                 np.zeros((b, 6), F32), np.zeros((b, 3)), s0['mean'], s0['std'])
-    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
     pk.add('aug', np.array([bool(s['aug']) for s in samples], np.uint8))
     pk.add('nobj', nobj)
     pk.add('boxes', boxes)
@@ -683,9 +666,7 @@ def collate_ddd(samples):
     pk.add('alpha', alpha)
     pk.add('depth', depth)
     pk.add('dim', dim)
-    scalars = {k: s0[k] for k in keys}
-    scalars.update(batch=b)
-    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+    return pk.collated(scalars)
 
 
 def build_ddd_batch(packed, device=None, dtype=torch.float32, memory_format=torch.contiguous_format):
@@ -695,12 +676,10 @@ def build_ddd_batch(packed, device=None, dtype=torch.float32, memory_format=torc
     rotbin [B,M,2] i64, rotres [B,M,2] f32, reg_mask u8, rot_mask u8; wh with reg_bbox, reg with reg_offset.  hm is
     always dense: the ignore regions overwrite it in object order, which no object list expresses.  The packed host
     buffer is not modified."""
-    dev = _device(device)
     sc = packed['scalars']
     b, m, nc, oh, ow = sc['batch'], sc['max_objs'], sc['num_classes'], sc['output_h'], sc['output_w']
-    buf = packed['buffer'].to(dev, non_blocking=True)
-    v = _views(buf, packed['layout'])
-    inp = _launch_images(v, b, sc['input_h'], sc['input_w'], False, dtype, memory_format, dev)
+    v, inp = _upload(packed, device, sc['input_h'], sc['input_w'], dtype, memory_format)
+    dev = inp.device
     f32 = dict(dtype=torch.float32, device=dev)
     u8 = dict(dtype=torch.uint8, device=dev)
     i64 = dict(dtype=torch.int64, device=dev)
@@ -726,10 +705,10 @@ def build_ddd_batch(packed, device=None, dtype=torch.float32, memory_format=torc
 def exdet_params(height, width, opt, split, data_rng, eig_val, eig_vec):
     """The random draws of EXDetDataset.__getitem__ (exdet.py:36-65) for one height x width image, in the reference's
     order, and the matrices they give.  The centre is float64.  In the train split: the random crop's choice and two
-    randint (ctdet's crop_draws), or under not_rand_crop three randn in the order scale, x shift, y shift, the shifts
-    scaled by the image's width and height; then the flip draw.  The flip mirrors the image but leaves the centre,
-    so trans_input / trans_output are the unflipped get_affine_transform(c, s, 0, [res, res]) applied to the mirrored
-    source.  color_aug's draws follow as in ctdet.  The input is input_res square (there is no keep_res branch)."""
+    randint (ctdet's crop_draws), or under not_rand_crop scale_shift_draws; then the flip draw.  The flip mirrors the
+    image but leaves the centre, so trans_input / trans_output are the unflipped get_affine_transform(c, s, 0,
+    [res, res]) applied to the mirrored source.  color_aug's draws follow as in ctdet.  The input is input_res square
+    (there is no keep_res branch)."""
     c = np.array([width / 2., height / 2.])
     s = max(height, width) * 1.0
     flipped = False
@@ -737,15 +716,10 @@ def exdet_params(height, width, opt, split, data_rng, eig_val, eig_vec):
         if not opt.not_rand_crop:
             s = crop_draws(height, width, c, s, opt)
         else:
-            sf, cf = opt.scale, opt.shift
-            s = s * np.clip(np.random.randn() * sf + 1, 1 - sf, 1 + sf)
-            c[0] += width * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
-            c[1] += height * np.clip(np.random.randn() * cf, -2 * cf, 2 * cf)
+            s = scale_shift_draws(height, width, c, s, opt)
         if np.random.random() < opt.flip:
             flipped = True
-    order, blend, light = -1, np.zeros(6, F32), np.zeros(3, np.float64)
-    if split == 'train' and not opt.no_color_aug:
-        order, blend, light = color_draws(data_rng, eig_val, eig_vec)
+    order, blend, light = color_draws(split, opt, data_rng, eig_val, eig_vec)
     res, out_res = int(opt.input_res), int(opt.output_res)
     return {'c': c, 's': s, 'flip': flipped, 'input_res': res, 'output_res': out_res,
             'minv': np.array(_invert(affine_transform(c, s, [res, res])), np.float64),
@@ -753,36 +727,18 @@ def exdet_params(height, width, opt, split, data_rng, eig_val, eig_vec):
             'order': order, 'blend': blend, 'light': light}
 
 
-class ExdetTrainInput(torch.utils.data.Dataset):
-    """Wraps a reference EXDetDataset instance (duck-typed on opt, coco, images, img_dir, max_objs, cat_ids, mean,
-    std, _data_rng, _eig_val, _eig_vec and split).  __getitem__ reads the image and the annotations -- extreme_points
-    as float32 (t, l, b, r), class cat_ids[category_id] -- and draws the parameters as the reference does; it does no
-    pixel work (collate_exdet + build_exdet_batch do).  The number of classes is opt.num_classes, as there."""
+class ExdetTrainInput(_TrainInput):
+    """Wraps a reference EXDetDataset instance (also duck-typed on cat_ids, _data_rng, _eig_val and _eig_vec):
+    exdet_params' draws, the extreme_points as float32 (t, l, b, r) and the class cat_ids[category_id]; the batch is
+    collate_exdet + build_exdet_batch's.  The number of classes is opt.num_classes, as there."""
 
-    def __init__(self, dataset):
-        if dataset.opt.mse_loss:
-            raise NotImplementedError("ExdetTrainInput: opt.mse_loss (draw_msra_gaussian targets) is not implemented")
-        self.dataset = dataset
+    def _params(self, ds, height, width):
+        return exdet_params(height, width, ds.opt, ds.split, ds._data_rng, ds._eig_val, ds._eig_vec)
 
-    def __len__(self):
-        return len(self.dataset)
-
-    def __getitem__(self, index):
-        import cv2
-        ds = self.dataset
-        img_id = ds.images[index]
-        file_name = ds.coco.loadImgs(ids=[img_id])[0]['file_name']
-        img = cv2.imread(os.path.join(ds.img_dir, file_name))
-        opt = ds.opt
-        sample = exdet_params(img.shape[0], img.shape[1], opt, ds.split, ds._data_rng, ds._eig_val, ds._eig_vec)
-        anns = ds.coco.loadAnns(ids=ds.coco.getAnnIds(imgIds=[img_id]))
-        num_objs = min(len(anns), ds.max_objs)
-        pts = [np.array(anns[k]['extreme_points'], dtype=np.float32).reshape(-1) for k in range(num_objs)]
-        cls = np.array([int(ds.cat_ids[anns[k]['category_id']]) for k in range(num_objs)], np.int64)
-        sample.update(image=img, points=pts, cls=cls, max_objs=ds.max_objs, num_classes=int(opt.num_classes),
-                      mean=np.asarray(ds.mean, F32).reshape(3), std=np.asarray(ds.std, F32).reshape(3),
-                      agnostic_ex=bool(opt.agnostic_ex), reg_offset=bool(opt.reg_offset))
-        return sample
+    def _fields(self, ds, anns):
+        return {'points': [np.array(a['extreme_points'], dtype=np.float32).reshape(-1) for a in anns],
+                'cls': np.array([int(ds.cat_ids[a['category_id']]) for a in anns], np.int64),
+                'num_classes': int(ds.opt.num_classes), 'agnostic_ex': bool(ds.opt.agnostic_ex)}
 
 
 def collate_exdet(samples):
@@ -793,14 +749,8 @@ def collate_exdet(samples):
     coordinate that is not finite (the reference's pts.astype(np.int32) of it is undefined)."""
     s0 = samples[0]
     keys = ('input_res', 'output_res', 'max_objs', 'num_classes', 'agnostic_ex', 'reg_offset')
-    for s in samples:
-        if any(s[k] != s0[k] for k in keys):
-            raise ValueError("collate_exdet: samples with different settings cannot be batched")
-    images = [s['image'] for s in samples]
-    _check_images(images)
+    pk, scalars = _collate(samples, 'collate_exdet', keys)
     b, m, nc = len(samples), int(s0['max_objs']), int(s0['num_classes'])
-    if not 1 <= m <= 128:
-        raise ValueError("collate_exdet: 1 to 128 object slots (FocalSplatLoss / splat_gaussian), got %d" % m)
     pts = np.zeros((b, m, 4, 2), F32)
     cls = np.zeros((b, m), np.int32)
     nobj = np.zeros(b, np.int32)
@@ -817,17 +767,10 @@ def collate_exdet(samples):
                 raise ValueError("collate_exdet: extreme_points must be finite")
             pts[i, k] = p.reshape(4, 2)
         nobj[i], cls[i, :n] = n, c
-    pk = _Packer()
-    _pack_images(pk, images, [s['minv'] for s in samples], [s['flip'] for s in samples],
-                 [s['order'] for s in samples], [s['blend'] for s in samples], [s['light'] for s in samples],
-                 s0['mean'], s0['std'])
-    pk.add('trans_output', np.array([s['trans_output'] for s in samples], np.float64).reshape(b, 6))
     pk.add('nobj', nobj)
     pk.add('pts', pts)
     pk.add('cls', cls)
-    scalars = {k: s0[k] for k in keys}
-    scalars.update(batch=b, color=any(s['order'] >= 0 for s in samples))
-    return {'buffer': pk.tensor(_pin()), 'layout': pk.layout, 'scalars': scalars}
+    return pk.collated(scalars)
 
 
 EXDET_PARTS = ('t', 'l', 'b', 'r')
@@ -844,20 +787,15 @@ def build_exdet_batch(packed, device=None, dtype=torch.float32, memory_format=to
     (int32) and obj_valid (uint8) [B,M], and the extreme points ex_cls / ex_cx / ex_cy / ex_radius (int32) and
     ex_valid (uint8) [4,B,M] in the order t, l, b, r -- ex_*[p] is part p's [B,M] list set, and the [4B, M] view
     of all four gives the four extreme maps in one splat.  The packed host buffer is not modified."""
-    dev = _device(device)
     sc = packed['scalars']
     b, m, nc, r = sc['batch'], sc['max_objs'], sc['num_classes'], sc['output_res']
     num_hm = 1 if sc['agnostic_ex'] else nc
-    buf = packed['buffer'].to(dev, non_blocking=True)
-    v = _views(buf, packed['layout'])
-    inp = _launch_images(v, b, sc['input_res'], sc['input_res'], sc['color'], dtype, memory_format, dev)
-    u8 = dict(dtype=torch.uint8, device=dev)
-    i32 = dict(dtype=torch.int32, device=dev)
+    v, inp = _upload(packed, device, sc['input_res'], sc['input_res'], dtype, memory_format)
+    dev = inp.device
     reg = torch.empty((4, b, m, 2), dtype=torch.float32, device=dev)
     ind = torch.empty((4, b, m), dtype=torch.int64, device=dev)
-    reg_mask = torch.empty((b, m), **u8)
-    lists = [torch.empty((b, m), **i32) for _ in range(4)] + [torch.empty((b, m), **u8)]
-    ex_lists = [torch.empty((4, b, m), **i32) for _ in range(4)] + [torch.empty((4, b, m), **u8)]
+    reg_mask = torch.empty((b, m), dtype=torch.uint8, device=dev)
+    lists, ex_lists = _lists((b, m), dev), _lists((4, b, m), dev)
     C.exdet_targets(ptr(v['pts']), ptr(v['cls']), ptr(v['nobj']), ptr(v['flip']), ptr(v['src_hw']),
                     ptr(v['trans_output']), b, m, r, int(sc['agnostic_ex']), ptr(reg), ptr(ind), ptr(reg_mask),
                     *[ptr(t) for t in lists], *[ptr(t) for t in ex_lists], stream_ptr(reg))
@@ -870,6 +808,6 @@ def build_exdet_batch(packed, device=None, dtype=torch.float32, memory_format=to
         ret['reg_mask'] = reg_mask
         ret.update(('reg_' + p, reg[j]) for j, p in enumerate(EXDET_PARTS))
         ret.update(('ind_' + p, ind[j]) for j, p in enumerate(EXDET_PARTS))
-    ret.update(zip(('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid'), lists))
-    ret.update(zip(('ex_cls', 'ex_cx', 'ex_cy', 'ex_radius', 'ex_valid'), ex_lists))
+    ret.update(('obj_' + k, t) for k, t in zip(_LIST_KEYS, lists))
+    ret.update(('ex_' + k, t) for k, t in zip(_LIST_KEYS, ex_lists))
     return ret

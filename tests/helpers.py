@@ -1,5 +1,7 @@
-"""Shared test helpers: golden loading and tie-aware detection comparison."""
+"""Shared test helpers: golden loading, bit and tie-aware detection comparison, and the training samplers' stubs."""
 import os
+import random
+import zlib
 
 import numpy as np
 
@@ -52,6 +54,42 @@ def assert_same_bits(got, want, what=""):
         i = tuple(idx[0])
         raise AssertionError("%s: %d of %d elements differ, first at %s: got %r, want %r"
                              % (what, len(idx), bad.size, i, got[i], want[i]))
+
+
+def assert_bits(got, want, what):
+    """Same dtype, same shape and the same bytes (NaN payloads and the sign of zero included)."""
+    got, want = np.asarray(got), np.asarray(want)
+    assert got.dtype == want.dtype and got.shape == want.shape, (what, got.dtype, got.shape, want.dtype, want.shape)
+    u = np.dtype("u%d" % got.itemsize)
+    bad = np.ascontiguousarray(got).view(u) != np.ascontiguousarray(want).view(u)
+    assert not bad.any(), "%s: %d of %d values differ, first at %s" % (what, bad.sum(), bad.size,
+                                                                         np.argwhere(bad)[0])
+
+
+def state_crcs(data_rng):
+    """CRCs of the three generators a training sampler draws from: np.random, random and the dataset's data_rng."""
+    k, pos = np.random.get_state()[1:3]
+    c_np = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
+    c_py = zlib.crc32(np.asarray(random.getstate()[1], np.uint64).tobytes())
+    k, pos = data_rng.get_state()[1:3]
+    c_dr = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
+    return np.array([c_np, c_py, c_dr], np.uint32)
+
+
+class StubCOCO(object):
+    """The pycocotools calls the training datasets make, over {image id: file name} and {image id: [annotation]}."""
+
+    def __init__(self, files, anns):
+        self.files, self.anns = files, anns
+
+    def loadImgs(self, ids):
+        return [{'file_name': self.files[ids[0]]}]
+
+    def getAnnIds(self, imgIds):
+        return [(imgIds[0], k) for k in range(len(self.anns[imgIds[0]]))]
+
+    def loadAnns(self, ids):
+        return [self.anns[i][k] for i, k in ids]
 
 
 def flat_results(res, num_classes):

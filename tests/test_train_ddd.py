@@ -14,28 +14,13 @@ import pytest
 import ddd_train_cases as DC
 import train_ddd_np as DN
 import train_np as TN
-from helpers import golden
+from helpers import assert_bits, golden, state_crcs, StubCOCO
 
 from centernet_b200 import train_input as T
 from centernet_b200._lib import C
 
 SAMPLES = [(n, i) for n, c in DC.CASES.items() for i in range(len(c['sizes']))]
 TARGETS = ('hm', 'dep', 'dim', 'ind', 'rotbin', 'rotres', 'reg_mask', 'rot_mask', 'wh', 'reg')
-
-
-def _state_crcs(data_rng):
-    k, pos = np.random.get_state()[1:3]
-    c_np = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    c_py = zlib.crc32(np.asarray(random.getstate()[1], np.uint64).tobytes())
-    k, pos = data_rng.get_state()[1:3]
-    c_dr = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    return np.array([c_np, c_py, c_dr], np.uint32)
-
-
-def _bits(a, b, what):
-    a, b = np.asarray(a), np.asarray(b)
-    assert a.dtype == b.dtype and a.shape == b.shape, (what, a.dtype, a.shape, b.dtype, b.shape)
-    assert a.tobytes() == b.tobytes(), what
 
 
 @pytest.mark.parametrize("name", list(DC.CASES))
@@ -50,14 +35,14 @@ def test_wrapper_draws_and_matrices_match_reference(name):
         for i, (h, w) in enumerate(case['sizes']):
             p = "%s_%d_" % (name, i)
             d = T.ddd_params(h, w, opt, case['split'])
-            np.testing.assert_array_equal(_state_crcs(data_rng), g[p + "states"], err_msg=p)
-            _bits(d['c'], g[p + "c"], p + "c")
-            _bits(d['s'], g[p + "s"], p + "s")
+            np.testing.assert_array_equal(state_crcs(data_rng), g[p + "states"], err_msg=p)
+            assert_bits(d['c'], g[p + "c"], p + "c")
+            assert_bits(d['s'], g[p + "s"], p + "s")
             assert d['aug'] == bool(g[p + "aug"]), p
-            _bits(d['trans_output'].reshape(2, 3), g[p + "trans_output"], p + "trans_output")
-            _bits(T.affine_transform(d['c'], d['s'], [d['input_w'], d['input_h']]), g[p + "trans_input"],
+            assert_bits(d['trans_output'].reshape(2, 3), g[p + "trans_output"], p + "trans_output")
+            assert_bits(T.affine_transform(d['c'], d['s'], [d['input_w'], d['input_h']]), g[p + "trans_input"],
                   p + "trans_input")
-            _bits(d['minv'], np.array(T._invert(g[p + "trans_input"]), np.float64), p + "minv")
+            assert_bits(d['minv'], np.array(T._invert(g[p + "trans_input"]), np.float64), p + "minv")
     finally:
         np.random.set_state(saved[0]); random.setstate(saved[1])
 
@@ -80,7 +65,7 @@ def test_oracle_matches_golden(name, i):
     assert set(keys) == set(TARGETS) - ({'wh'} if not case['reg_bbox'] else set()) \
         - ({'reg'} if not case['reg_offset'] else set())
     for k in keys:
-        _bits(t[k], g[p + k], p + k)
+        assert_bits(t[k], g[p + k], p + k)
 
 
 def test_radius_restatement_matches_reference_table():
@@ -91,7 +76,7 @@ def test_radius_restatement_matches_reference_table():
     r = DN.gaussian_radius_f32(h, w)
     assert np.uint32(zlib.crc32(r.tobytes())) == g["radius_crc"]
     assert np.uint32(zlib.crc32(np.maximum(r.astype(np.int64), 0).astype(np.int16).tobytes())) == g["radius_int_crc"]
-    _bits(DN.gaussian_radius_f32(*DC.near_pairs(g["radius_near_h0"], g["radius_near_w0"])), g["radius_near"],
+    assert_bits(DN.gaussian_radius_f32(*DC.near_pairs(g["radius_near_h0"], g["radius_near_w0"])), g["radius_near"],
           "near-integer radii")
 
 
@@ -128,30 +113,16 @@ def test_centre_enters_src1_as_given():
             s = np.array([rng.integers(32, 1300), rng.integers(32, 1300)], np.float32) * rng.choice(
                 np.arange(0.6, 1.4, 0.1))
         size = [int(rng.integers(16, 1025)), int(rng.integers(16, 1025))]
-        _bits(T.affine_transform(c, s, size), f32_centre(c, s, size), "float32 centre")
+        assert_bits(T.affine_transform(c, s, size), f32_centre(c, s, size), "float32 centre")
     g = golden("train_ddd")
     differs = 0
     for name, i in SAMPLES:
         p = "%s_%d_" % (name, i)
         opt = DC.make_opt(DC.CASES[name])
         c, s, size = g[p + "c"], g[p + "s"], [opt.output_w, opt.output_h]
-        _bits(T.affine_transform(c, s, size), g[p + "trans_output"], p + "trans_output")
+        assert_bits(T.affine_transform(c, s, size), g[p + "trans_output"], p + "trans_output")
         differs += not np.array_equal(f32_centre(c, s, size), g[p + "trans_output"])
     assert differs > 0
-
-
-class _StubCOCO(object):
-    def __init__(self, files, anns):
-        self.files, self.anns = files, anns
-
-    def loadImgs(self, ids):
-        return [{'file_name': self.files[ids[0]]}]
-
-    def getAnnIds(self, imgIds):
-        return [(imgIds[0], k) for k in range(len(self.anns[imgIds[0]]))]
-
-    def loadAnns(self, ids):
-        return [self.anns[i][k] for i, k in ids]
 
 
 @pytest.mark.parametrize("name", ["kitti", "keep"])
@@ -164,7 +135,7 @@ def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path, name):
         files[i] = "%s_%d.png" % (name, i)
         cv2.imwrite(os.path.join(str(tmp_path), files[i]), DC.case_image(name, i))
         anns[i] = DC.case_anns(name, i)
-    ds = types.SimpleNamespace(**DC.case_dataset(name, _StubCOCO(files, anns), str(tmp_path),
+    ds = types.SimpleNamespace(**DC.case_dataset(name, StubCOCO(files, anns), str(tmp_path),
                                                  np.random.RandomState(case['seed'])))
     w = T.DddTrainInput(ds)
     saved = np.random.get_state(), random.getstate()
@@ -174,15 +145,15 @@ def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path, name):
             p = "%s_%d_" % (name, i)
             s = w[i]
             np.testing.assert_array_equal(s['image'], DC.case_image(name, i))
-            np.testing.assert_array_equal(_state_crcs(ds._data_rng), g[p + "states"])
-            _bits(s['c'], g[p + "c"], p + "c")
+            np.testing.assert_array_equal(state_crcs(ds._data_rng), g[p + "states"])
+            assert_bits(s['c'], g[p + "c"], p + "c")
             assert s['aug'] == bool(g[p + "aug"])
             boxes, cls, alpha, depth, dim = DC.case_objects(name, i)
-            _bits(s['boxes'], boxes, p + "boxes")
-            _bits(s['cls'], cls, p + "cls")
-            _bits(s['alpha'], alpha, p + "alpha")
-            _bits(s['depth'], depth, p + "depth")
-            _bits(np.array(s['dim']).reshape(-1, 3), dim, p + "dim")
+            assert_bits(s['boxes'], boxes, p + "boxes")
+            assert_bits(s['cls'], cls, p + "cls")
+            assert_bits(s['alpha'], alpha, p + "alpha")
+            assert_bits(s['depth'], depth, p + "depth")
+            assert_bits(np.array(s['dim']).reshape(-1, 3), dim, p + "dim")
     finally:
         np.random.set_state(saved[0]); random.setstate(saved[1])
 

@@ -14,22 +14,13 @@ import torch
 import ddd_train_cases as DC
 import train_ddd_np as DN
 import train_np as TN
-from helpers import golden
+from helpers import assert_bits, golden
 
 pytestmark = pytest.mark.gpu
 
 DTYPES = (torch.float32, torch.bfloat16, torch.float16)
 FORMATS = (torch.contiguous_format, torch.channels_last)
 TARGETS = ('hm', 'dep', 'dim', 'ind', 'rotbin', 'rotres', 'reg_mask', 'rot_mask', 'wh', 'reg')
-
-
-def _assert_bits(got, want, what):
-    got, want = np.ascontiguousarray(got), np.ascontiguousarray(want)
-    assert got.dtype == want.dtype and got.shape == want.shape, (what, got.dtype, got.shape, want.dtype, want.shape)
-    u = np.dtype("u%d" % got.itemsize)
-    bad = got.view(u) != want.view(u)
-    assert not bad.any(), "%s: %d of %d values differ, first at %s" % (what, bad.sum(), bad.size,
-                                                                         np.argwhere(bad)[0])
 
 
 def case_samples(name):
@@ -93,7 +84,7 @@ def test_ddd_batch_matches_reference(name, dtype, fmt):
     assert inp.dtype == dtype and inp.is_contiguous(memory_format=fmt)
     got = inp.float().cpu().numpy()
     want = torch.from_numpy(oracle_inputs(name)).to(dtype).float().numpy()
-    _assert_bits(got, want, "%s input %s" % (name, dtype))
+    assert_bits(got, want, "%s input %s" % (name, dtype))
     for i, s in enumerate(samples):
         p = "%s_%d_" % (name, i)
         if dtype == torch.float32:
@@ -101,8 +92,8 @@ def test_ddd_batch_matches_reference(name, dtype, fmt):
         t = restated(s)
         for k in TARGETS:
             if k in batch:
-                _assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k)
-                _assert_bits(batch[k][i].cpu().numpy(), t[k], p + k + " restated")
+                assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k)
+                assert_bits(batch[k][i].cpu().numpy(), t[k], p + k + " restated")
 
 
 def test_ddd_batch_bit_identical_run_to_run():
@@ -130,7 +121,7 @@ def test_device_radius_matches_reference_table():
         th, tw = torch.from_numpy(hh).cuda(), torch.from_numpy(ww).cuda()
         out = torch.empty(len(hh), dtype=torch.int32, device="cuda")
         C.ddd_gaussian_radius(ptr(th), ptr(tw), len(hh), ptr(out), torch.cuda.current_stream().cuda_stream)
-        _assert_bits(out.cpu().numpy(), want, "radius")
+        assert_bits(out.cpu().numpy(), want, "radius")
 
 
 def test_targets_edge_cases_against_restatement():
@@ -165,7 +156,7 @@ def test_targets_edge_cases_against_restatement():
         for i, s in enumerate(samples):
             t = restated(s)
             for k in TARGETS:
-                _assert_bits(batch[k][i].cpu().numpy(), t[k], "%s %d %s" % (rect, i, k))
+                assert_bits(batch[k][i].cpu().numpy(), t[k], "%s %d %s" % (rect, i, k))
         assert float(batch['hm'][0].abs().sum()) == 0 and int(batch['rot_mask'].sum()) > 0
 
 

@@ -14,7 +14,7 @@ import pytest
 import exdet_train_cases as EC
 import train_exdet_np as EN
 import train_np as TN
-from helpers import golden
+from helpers import assert_bits, golden, state_crcs, StubCOCO
 
 from centernet_b200 import train_input as T
 from centernet_b200._lib import C
@@ -23,21 +23,6 @@ SAMPLES = [(n, i) for n, c in EC.CASES.items() for i in range(len(c['sizes']))]
 PARTS = ('t', 'l', 'b', 'r')
 TARGETS = ('reg_mask',) + tuple('reg_' + p for p in PARTS) + tuple('ind_' + p for p in PARTS)
 MAPS = tuple('hm_' + p for p in PARTS + ('c',))
-
-
-def _state_crcs(data_rng):
-    k, pos = np.random.get_state()[1:3]
-    c_np = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    c_py = zlib.crc32(np.asarray(random.getstate()[1], np.uint64).tobytes())
-    k, pos = data_rng.get_state()[1:3]
-    c_dr = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    return np.array([c_np, c_py, c_dr], np.uint32)
-
-
-def _bits(a, b, what):
-    a, b = np.asarray(a), np.asarray(b)
-    assert a.dtype == b.dtype and a.shape == b.shape, (what, a.dtype, a.shape, b.dtype, b.shape)
-    assert a.tobytes() == b.tobytes(), what
 
 
 @pytest.mark.parametrize("name", list(EC.CASES))
@@ -52,15 +37,16 @@ def test_wrapper_draws_and_matrices_match_reference(name):
         for i, (h, w) in enumerate(case['sizes']):
             p = "%s_%d_" % (name, i)
             d = T.exdet_params(h, w, opt, case['split'], data_rng, EC.EIG_VAL, EC.EIG_VEC)
-            np.testing.assert_array_equal(_state_crcs(data_rng), g[p + "states"], err_msg=p)
-            _bits(d['c'], g[p + "c"], p + "c")
-            _bits(np.float64(d['s']), g[p + "s"], p + "s")
+            np.testing.assert_array_equal(state_crcs(data_rng), g[p + "states"], err_msg=p)
+            assert_bits(d['c'], g[p + "c"], p + "c")
+            assert_bits(np.float64(d['s']), g[p + "s"], p + "s")
             assert d['flip'] == bool(g[p + "flip"]) and d['order'] == int(g[p + "order"]), p
-            _bits(d['blend'], g[p + "blend"], p + "blend")
-            _bits(d['light'], g[p + "light"], p + "light")
-            _bits(d['trans_output'].reshape(2, 3), g[p + "trans_output"], p + "trans_output")
-            _bits(T.affine_transform(d['c'], d['s'], [d['input_res']] * 2), g[p + "trans_input"], p + "trans_input")
-            _bits(d['minv'], np.array(T._invert(g[p + "trans_input"]), np.float64), p + "minv")
+            assert_bits(d['blend'], g[p + "blend"], p + "blend")
+            assert_bits(d['light'], g[p + "light"], p + "light")
+            assert_bits(d['trans_output'].reshape(2, 3), g[p + "trans_output"], p + "trans_output")
+            assert_bits(T.affine_transform(d['c'], d['s'], [d['input_res']] * 2), g[p + "trans_input"],
+                        p + "trans_input")
+            assert_bits(d['minv'], np.array(T._invert(g[p + "trans_input"]), np.float64), p + "minv")
     finally:
         np.random.set_state(saved[0]); random.setstate(saved[1])
 
@@ -75,7 +61,7 @@ def test_float64_centre_reaches_src1_unrounded():
         c, s = g[p + "c"], g[p + "s"][()]
         assert c.dtype == np.float64
         r = EC.make_opt(EC.CASES["ex_shift"]).output_res
-        _bits(T.affine_transform(c, s, [r, r]), g[p + "trans_output"], p)
+        assert_bits(T.affine_transform(c, s, [r, r]), g[p + "trans_output"], p)
         differs += not np.array_equal(T.affine_transform(c.astype(np.float32), s, [r, r]), g[p + "trans_output"])
     assert differs > 0
 
@@ -97,26 +83,12 @@ def test_oracle_matches_golden(name, i):
     keys = [k for k in TARGETS if p + k in g]
     assert set(keys) == (set(TARGETS) if case['reg_offset'] else set())
     for k in keys:
-        _bits(t[k], g[p + k], p + k)
+        assert_bits(t[k], g[p + k], p + k)
     if i < case['hm_samples']:
         maps = EN.exdet_maps(t, case['num_classes'], r, case['agnostic_ex'])
         for k in MAPS:
-            _bits(maps[k], g[p + k], p + k)
+            assert_bits(maps[k], g[p + k], p + k)
         assert g[p + "hm_t"].shape[0] == (1 if case['agnostic_ex'] else case['num_classes'])
-
-
-class _StubCOCO(object):
-    def __init__(self, files, anns):
-        self.files, self.anns = files, anns
-
-    def loadImgs(self, ids):
-        return [{'file_name': self.files[ids[0]]}]
-
-    def getAnnIds(self, imgIds):
-        return [(imgIds[0], k) for k in range(len(self.anns[imgIds[0]]))]
-
-    def loadAnns(self, ids):
-        return [self.anns[i][k] for i, k in ids]
 
 
 @pytest.mark.parametrize("name", ["ex_flip", "ex_plain"])
@@ -129,7 +101,7 @@ def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path, name):
         files[i] = "%s_%d.png" % (name, i)
         cv2.imwrite(os.path.join(str(tmp_path), files[i]), EC.case_image(name, i))
         anns[i] = EC.case_anns(name, i)
-    ds = types.SimpleNamespace(**EC.case_dataset(name, _StubCOCO(files, anns), str(tmp_path),
+    ds = types.SimpleNamespace(**EC.case_dataset(name, StubCOCO(files, anns), str(tmp_path),
                                                  np.random.RandomState(case['seed'])))
     w = T.ExdetTrainInput(ds)
     saved = np.random.get_state(), random.getstate()
@@ -139,12 +111,12 @@ def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path, name):
             p = "%s_%d_" % (name, i)
             s = w[i]
             np.testing.assert_array_equal(s['image'], EC.case_image(name, i))
-            np.testing.assert_array_equal(_state_crcs(ds._data_rng), g[p + "states"])
-            _bits(s['c'], g[p + "c"], p + "c")
+            np.testing.assert_array_equal(state_crcs(ds._data_rng), g[p + "states"])
+            assert_bits(s['c'], g[p + "c"], p + "c")
             assert s['flip'] == bool(g[p + "flip"])
             pts, cls = EC.case_objects(name, i)
-            _bits(np.array(s['points']).reshape(-1, 4, 2), pts, p + "points")
-            _bits(s['cls'], cls, p + "cls")
+            assert_bits(np.array(s['points']).reshape(-1, 4, 2), pts, p + "points")
+            assert_bits(s['cls'], cls, p + "cls")
             assert (s['num_classes'], s['agnostic_ex'], s['reg_offset']) == \
                 (case['num_classes'], case['agnostic_ex'], case['reg_offset'])
     finally:

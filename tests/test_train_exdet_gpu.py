@@ -12,7 +12,7 @@ import torch
 import exdet_train_cases as EC
 import train_exdet_np as EN
 import train_np as TN
-from helpers import golden
+from helpers import assert_bits, golden
 
 pytestmark = pytest.mark.gpu
 
@@ -23,15 +23,6 @@ TARGETS = ('reg_mask',) + tuple('reg_' + p for p in PARTS) + tuple('ind_' + p fo
 MAPS = tuple('hm_' + p for p in PARTS + ('c',))
 LISTS = ('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid')
 EX_LISTS = ('ex_cls', 'ex_cx', 'ex_cy', 'ex_radius', 'ex_valid')
-
-
-def _assert_bits(got, want, what):
-    got, want = np.ascontiguousarray(got), np.ascontiguousarray(want)
-    assert got.dtype == want.dtype and got.shape == want.shape, (what, got.dtype, got.shape, want.dtype, want.shape)
-    u = np.dtype("u%d" % got.itemsize)
-    bad = got.view(u) != want.view(u)
-    assert not bad.any(), "%s: %d of %d values differ, first at %s" % (what, bad.sum(), bad.size,
-                                                                         np.argwhere(bad)[0])
 
 
 def case_samples(name):
@@ -95,18 +86,18 @@ def _check_batch(name, samples, batch, dense_hm):
         p = "%s_%d_" % (name, i)
         for k in TARGETS:
             if k in batch:
-                _assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k)
+                assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k)
         t = restated(s)
         for k in LISTS:
-            _assert_bits(batch[k][i].cpu().numpy(), t[k], p + k)
+            assert_bits(batch[k][i].cpu().numpy(), t[k], p + k)
         for k in EX_LISTS:
-            _assert_bits(batch[k][:, i].cpu().numpy(), t[k], p + k)
+            assert_bits(batch[k][:, i].cpu().numpy(), t[k], p + k)
         if dense_hm:
             for k in MAPS:
                 assert tuple(batch[k].shape) == (b, case['num_classes'] if k == 'hm_c' else num_hm, r, r), k
-                _assert_bits(batch[k][i].cpu().numpy(), t[k], p + k)
+                assert_bits(batch[k][i].cpu().numpy(), t[k], p + k)
                 if p + k in g:
-                    _assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k + " golden")
+                    assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k + " golden")
 
 
 @pytest.mark.parametrize("name", list(EC.CASES))
@@ -125,7 +116,7 @@ def test_exdet_batch_matches_reference(name, dtype, fmt):
     assert inp.dtype == dtype and inp.is_contiguous(memory_format=fmt)
     got = inp.float().cpu().numpy()
     want = torch.from_numpy(oracle_inputs(name)).to(dtype).float().numpy()
-    _assert_bits(got, want, "%s input %s" % (name, dtype))
+    assert_bits(got, want, "%s input %s" % (name, dtype))
     if dtype == torch.float32:
         for i in range(len(samples)):
             np.testing.assert_array_equal(EC.input_sample(got[i]), g["%s_%d_input_sample" % (name, i)])
@@ -261,8 +252,8 @@ def test_targets_edge_cases_against_restatement(agnostic_ex):
     for i, s in enumerate(samples):
         t = restated(s)
         for k in TARGETS + LISTS + MAPS:
-            _assert_bits(batch[k][i].cpu().numpy(), t[k], "%d %s" % (i, k))
+            assert_bits(batch[k][i].cpu().numpy(), t[k], "%d %s" % (i, k))
         for k in EX_LISTS:
-            _assert_bits(batch[k][:, i].cpu().numpy(), t[k], "%d %s" % (i, k))
+            assert_bits(batch[k][:, i].cpu().numpy(), t[k], "%d %s" % (i, k))
         zero_radius += int(((t['obj_radius'] == 0) & (t['obj_valid'] == 1)).sum())
     assert int(batch['obj_valid'][0].sum()) == 0 and int(batch['reg_mask'].sum()) > 0 and zero_radius > 0

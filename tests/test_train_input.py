@@ -12,7 +12,7 @@ import torch
 
 import train_cases as TC
 import train_np as TN
-from helpers import golden
+from helpers import golden, state_crcs, StubCOCO
 from oracle import image_np
 
 from centernet_b200 import train_input as T
@@ -88,15 +88,6 @@ def test_oracle_rotated_warp_matches_golden(name):
     _check_input(x, g, p)
 
 
-def _state_crcs(data_rng):
-    k, pos = np.random.get_state()[1:3]
-    c_np = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    c_py = zlib.crc32(np.asarray(random.getstate()[1], np.uint64).tobytes())
-    k, pos = data_rng.get_state()[1:3]
-    c_dr = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    return np.array([c_np, c_py, c_dr], np.uint32)
-
-
 @pytest.mark.parametrize("name", [n for n, c in TC.CASES.items() if 'rot' not in c])
 def test_wrapper_draws_match_reference(name):
     g = golden("train")
@@ -109,7 +100,7 @@ def test_wrapper_draws_match_reference(name):
         for i, (h, w) in enumerate(case['sizes']):
             p = "%s_%d_" % (name, i)
             d = T.sample_params(h, w, opt, case['split'], data_rng, TC.EIG_VAL, TC.EIG_VEC)
-            np.testing.assert_array_equal(_state_crcs(data_rng), g[p + "states"])
+            np.testing.assert_array_equal(state_crcs(data_rng), g[p + "states"])
             np.testing.assert_array_equal(d['c'], g[p + "c"])
             s = d['s'] if isinstance(d['s'], np.ndarray) else [d['s'], d['s']]
             np.testing.assert_array_equal(np.asarray(s, np.float64), g[p + "s"])
@@ -120,20 +111,6 @@ def test_wrapper_draws_match_reference(name):
             assert (d['input_h'], d['input_w']) == _input_size(case, h, w)
     finally:
         np.random.set_state(saved[0]); random.setstate(saved[1])
-
-
-class _StubCOCO(object):
-    def __init__(self, files, anns):
-        self.files, self.anns = files, anns
-
-    def loadImgs(self, ids):
-        return [{'file_name': self.files[ids[0]]}]
-
-    def getAnnIds(self, imgIds):
-        return [(imgIds[0], k) for k in range(len(self.anns[imgIds[0]]))]
-
-    def loadAnns(self, ids):
-        return [self.anns[i][k] for i, k in ids]
 
 
 def make_dataset(name, tmpdir):
@@ -147,7 +124,7 @@ def make_dataset(name, tmpdir):
         cv2.imwrite(os.path.join(str(tmpdir), files[i]), TC.case_image(name, i))
         anns[i] = TC.case_anns(name, i)
     return types.SimpleNamespace(
-        opt=TC.make_opt(case), coco=_StubCOCO(files, anns), images=list(range(len(files))), img_dir=str(tmpdir),
+        opt=TC.make_opt(case), coco=StubCOCO(files, anns), images=list(range(len(files))), img_dir=str(tmpdir),
         max_objs=case['max_objs'], cat_ids=TC.cat_ids(case), num_classes=case['num_classes'],
         mean=TC.MEAN.reshape(1, 1, 3), std=TC.STD.reshape(1, 1, 3), _data_rng=np.random.RandomState(case['seed']),
         _eig_val=TC.EIG_VAL, _eig_vec=TC.EIG_VEC, split=case["split"])
@@ -166,7 +143,7 @@ def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path):
             p = "%s_%d_" % (name, i)
             s = w[i]
             np.testing.assert_array_equal(s['image'], TC.case_image(name, i))
-            np.testing.assert_array_equal(_state_crcs(ds._data_rng), g[p + "states"])
+            np.testing.assert_array_equal(state_crcs(ds._data_rng), g[p + "states"])
             np.testing.assert_array_equal(s['c'], g[p + "c"])
             boxes, cls = _boxes(name, i, TC.CASES[name])
             np.testing.assert_array_equal(s['boxes'], boxes)

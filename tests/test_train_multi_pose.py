@@ -14,28 +14,13 @@ import pytest
 import multi_pose_train_cases as MC
 import train_multi_pose_np as MN
 import train_np as TN
-from helpers import golden
+from helpers import assert_bits, golden, state_crcs, StubCOCO
 
 from centernet_b200 import train_input as T
 from centernet_b200._lib import C
 
 SAMPLES = [(n, i) for n, c in MC.CASES.items() for i in range(len(c['sizes']))]
 TARGETS = ('reg_mask', 'ind', 'wh', 'hps', 'hps_mask', 'reg', 'hp_offset', 'hp_ind', 'hp_mask')
-
-
-def _state_crcs(data_rng):
-    k, pos = np.random.get_state()[1:3]
-    c_np = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    c_py = zlib.crc32(np.asarray(random.getstate()[1], np.uint64).tobytes())
-    k, pos = data_rng.get_state()[1:3]
-    c_dr = zlib.crc32(np.asarray(k, np.uint32).tobytes() + np.int64(pos).tobytes())
-    return np.array([c_np, c_py, c_dr], np.uint32)
-
-
-def _bits(a, b, what):
-    a, b = np.asarray(a), np.asarray(b)
-    assert a.dtype == b.dtype and a.shape == b.shape, (what, a.dtype, a.shape, b.dtype, b.shape)
-    assert a.tobytes() == b.tobytes(), what
 
 
 @pytest.mark.parametrize("name", list(MC.CASES))
@@ -50,17 +35,17 @@ def test_wrapper_draws_and_matrices_match_reference(name):
         for i, (h, w) in enumerate(case['sizes']):
             p = "%s_%d_" % (name, i)
             d = T.multi_pose_params(h, w, opt, case['split'], data_rng, MC.EIG_VAL, MC.EIG_VEC)
-            np.testing.assert_array_equal(_state_crcs(data_rng), g[p + "states"], err_msg=p)
-            _bits(d['c'], g[p + "c"], p + "c")
-            _bits(np.float64(d['s']), g[p + "s"], p + "s")
-            _bits(np.float64(d['rot']), g[p + "rot"], p + "rot")
+            np.testing.assert_array_equal(state_crcs(data_rng), g[p + "states"], err_msg=p)
+            assert_bits(d['c'], g[p + "c"], p + "c")
+            assert_bits(np.float64(d['s']), g[p + "s"], p + "s")
+            assert_bits(np.float64(d['rot']), g[p + "rot"], p + "rot")
             assert d['flip'] == bool(g[p + "flip"]) and d['order'] == int(g[p + "order"]), p
-            _bits(d['blend'], g[p + "blend"], p + "blend")
-            _bits(d['light'], g[p + "light"], p + "light")
-            _bits(d['trans_output_rot'].reshape(2, 3), g[p + "trans_output_rot"], p + "trans_output_rot")
-            _bits(d['trans_output'].reshape(2, 3), g[p + "trans_output"], p + "trans_output")
-            _bits(d['minv'], np.array(T._invert(g[p + "trans_input"]), np.float64), p + "minv")
-            _bits(T.affine_transform(d['c'], d['s'], [d['input_res']] * 2, d['rot']), g[p + "trans_input"],
+            assert_bits(d['blend'], g[p + "blend"], p + "blend")
+            assert_bits(d['light'], g[p + "light"], p + "light")
+            assert_bits(d['trans_output_rot'].reshape(2, 3), g[p + "trans_output_rot"], p + "trans_output_rot")
+            assert_bits(d['trans_output'].reshape(2, 3), g[p + "trans_output"], p + "trans_output")
+            assert_bits(d['minv'], np.array(T._invert(g[p + "trans_input"]), np.float64), p + "minv")
+            assert_bits(T.affine_transform(d['c'], d['s'], [d['input_res']] * 2, d['rot']), g[p + "trans_input"],
                   p + "trans_input")
     finally:
         np.random.set_state(saved[0]); random.setstate(saved[1])
@@ -103,7 +88,7 @@ def test_rotated_matrices_match_train_golden_and_unrotated_are_unchanged():
         case = TC.CASES[name]
         h, w = case['sizes'][0]
         c = np.array([w / 2., h / 2.], np.float32)
-        _bits(T.affine_transform(c, max(h, w) * case['scale'], [case['out']] * 2, case['rot']),
+        assert_bits(T.affine_transform(c, max(h, w) * case['scale'], [case['out']] * 2, case['rot']),
               g[name + "_0_matrix"], name)
     from centernet_b200.post_process import _affine_points, cv_affine_transform
 
@@ -124,7 +109,7 @@ def test_rotated_matrices_match_train_golden_and_unrotated_are_unchanged():
             s = np.array([rng.integers(32, 1300), rng.integers(32, 1300)], np.float32) * rng.choice(
                 np.arange(0.6, 1.4, 0.1))
         size = [int(rng.integers(16, 1025)), int(rng.integers(16, 1025))]
-        _bits(T.affine_transform(c, s, size), unrotated(c, s, size), "rot 0")
+        assert_bits(T.affine_transform(c, s, size), unrotated(c, s, size), "rot 0")
 
 
 @pytest.mark.parametrize("name,i", SAMPLES)
@@ -148,26 +133,12 @@ def test_oracle_matches_golden(name, i):
     assert set(keys) == set(TARGETS) - ({'reg'} if not case['reg_offset'] else set()) \
         - ({'hp_offset', 'hp_ind', 'hp_mask'} if not case['reg_hp_offset'] else set())
     for k in keys:
-        _bits(t[k], g[p + k], p + k)
+        assert_bits(t[k], g[p + k], p + k)
     if p + "hm" in g:
         hm, hm_hp = MN.multi_pose_maps(t, case['num_classes'], r, rotated)
-        _bits(hm, g[p + "hm"], p + "hm")
+        assert_bits(hm, g[p + "hm"], p + "hm")
         if p + "hm_hp" in g:
-            _bits(hm_hp, g[p + "hm_hp"], p + "hm_hp")
-
-
-class _StubCOCO(object):
-    def __init__(self, files, anns):
-        self.files, self.anns = files, anns
-
-    def loadImgs(self, ids):
-        return [{'file_name': self.files[ids[0]]}]
-
-    def getAnnIds(self, imgIds):
-        return [(imgIds[0], k) for k in range(len(self.anns[imgIds[0]]))]
-
-    def loadAnns(self, ids):
-        return [self.anns[i][k] for i, k in ids]
+            assert_bits(hm_hp, g[p + "hm_hp"], p + "hm_hp")
 
 
 def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path):
@@ -180,7 +151,7 @@ def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path):
         files[i] = "%s_%d.png" % (name, i)
         cv2.imwrite(os.path.join(str(tmp_path), files[i]), MC.case_image(name, i))
         anns[i] = MC.case_anns(name, i)
-    ds = types.SimpleNamespace(**MC.case_dataset(name, _StubCOCO(files, anns), str(tmp_path),
+    ds = types.SimpleNamespace(**MC.case_dataset(name, StubCOCO(files, anns), str(tmp_path),
                                                  np.random.RandomState(case['seed'])))
     w = T.MultiPoseTrainInput(ds)
     saved = np.random.get_state(), random.getstate()
@@ -190,13 +161,13 @@ def test_dataset_wrapper_reads_and_draws_like_reference(tmp_path):
             p = "%s_%d_" % (name, i)
             s = w[i]
             np.testing.assert_array_equal(s['image'], MC.case_image(name, i))
-            np.testing.assert_array_equal(_state_crcs(ds._data_rng), g[p + "states"])
-            _bits(s['c'], g[p + "c"], p + "c")
+            np.testing.assert_array_equal(state_crcs(ds._data_rng), g[p + "states"])
+            assert_bits(s['c'], g[p + "c"], p + "c")
             boxes, cls, kps = MC.case_objects(name, i)
-            _bits(s['boxes'], boxes, p + "boxes")
-            _bits(s['cls'], cls, p + "cls")
+            assert_bits(s['boxes'], boxes, p + "boxes")
+            assert_bits(s['cls'], cls, p + "cls")
             for a, b in zip(s['keypoints'], kps):
-                _bits(a, b, p + "keypoints")
+                assert_bits(a, b, p + "keypoints")
     finally:
         np.random.set_state(saved[0]); random.setstate(saved[1])
 

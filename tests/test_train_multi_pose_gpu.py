@@ -12,7 +12,7 @@ import torch
 import multi_pose_train_cases as MC
 import train_multi_pose_np as MN
 import train_np as TN
-from helpers import golden
+from helpers import assert_bits, golden
 
 pytestmark = pytest.mark.gpu
 
@@ -21,15 +21,6 @@ FORMATS = (torch.contiguous_format, torch.channels_last)
 TARGETS = ('reg_mask', 'ind', 'wh', 'hps', 'hps_mask', 'reg', 'hp_offset', 'hp_ind', 'hp_mask')
 LISTS = ('obj_cls', 'obj_cx', 'obj_cy', 'obj_radius', 'obj_valid')
 HP_LISTS = ('hp_cx', 'hp_cy', 'hp_radius', 'hp_valid')
-
-
-def _assert_bits(got, want, what):
-    got, want = np.ascontiguousarray(got), np.ascontiguousarray(want)
-    assert got.dtype == want.dtype and got.shape == want.shape, (what, got.dtype, got.shape, want.dtype, want.shape)
-    u = np.dtype("u%d" % got.itemsize)
-    bad = got.view(u) != want.view(u)
-    assert not bad.any(), "%s: %d of %d values differ, first at %s" % (what, bad.sum(), bad.size,
-                                                                         np.argwhere(bad)[0])
 
 
 def case_samples(name):
@@ -103,7 +94,7 @@ def test_multi_pose_batch_matches_reference(name, dtype, fmt):
     assert inp.dtype == dtype and inp.is_contiguous(memory_format=fmt)
     got = inp.float().cpu().numpy()
     want = torch.from_numpy(oracle_inputs(name)).to(dtype).float().numpy()
-    _assert_bits(got, want, "%s input %s" % (name, dtype))
+    assert_bits(got, want, "%s input %s" % (name, dtype))
     r = case['input_res'] // case['down_ratio']
     for i, s in enumerate(samples):
         p = "%s_%d_" % (name, i)
@@ -111,18 +102,18 @@ def test_multi_pose_batch_matches_reference(name, dtype, fmt):
             np.testing.assert_array_equal(got[i][:, ::17, ::13], g[p + "input_sample"])
         for k in TARGETS:
             if k in batch:
-                _assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k)
+                assert_bits(batch[k][i].cpu().numpy(), g[p + k], p + k)
         t = restated(s)
         for k in LISTS + (HP_LISTS if case['hm_hp'] else ()):
-            _assert_bits(batch[k][i].cpu().numpy(), t[k], p + k)
-        _assert_bits(batch['hm'][i].cpu().numpy(), t['hm'], p + "hm")
+            assert_bits(batch[k][i].cpu().numpy(), t[k], p + k)
+        assert_bits(batch['hm'][i].cpu().numpy(), t['hm'], p + "hm")
         assert tuple(batch['hm'].shape[1:]) == (case['num_classes'], r, r)
         if case['hm_hp']:
-            _assert_bits(batch['hm_hp'][i].cpu().numpy(), t['hm_hp'], p + "hm_hp")
+            assert_bits(batch['hm_hp'][i].cpu().numpy(), t['hm_hp'], p + "hm_hp")
         if p + "hm" in g:
-            _assert_bits(batch['hm'][i].cpu().numpy(), g[p + "hm"], p + "hm golden")
+            assert_bits(batch['hm'][i].cpu().numpy(), g[p + "hm"], p + "hm golden")
         if p + "hm_hp" in g:
-            _assert_bits(batch['hm_hp'][i].cpu().numpy(), g[p + "hm_hp"], p + "hm_hp golden")
+            assert_bits(batch['hm_hp'][i].cpu().numpy(), g[p + "hm_hp"], p + "hm_hp golden")
         if s['rot'] != 0:
             assert (batch['hm'][i] == np.float32(0.9999).item()).all()
 
@@ -254,5 +245,5 @@ def test_targets_edge_cases_against_restatement():
     for i, s in enumerate(samples):
         t = restated(s)
         for k in TARGETS + LISTS + HP_LISTS + ('hm', 'hm_hp'):
-            _assert_bits(batch[k][i].cpu().numpy(), t[k], "%d %s" % (i, k))
+            assert_bits(batch[k][i].cpu().numpy(), t[k], "%d %s" % (i, k))
     assert int(batch['obj_valid'][0].sum()) == 0 and int(batch['hp_mask'].sum()) > 0
