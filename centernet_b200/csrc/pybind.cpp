@@ -525,6 +525,22 @@ PYBIND11_MODULE(_C, m) {
                                        ptr<void>(ws), wsb, ptr<void>(stream)),
           "cnb_dcnv2_forward_fused_bf16");
   });
+  m.def("head_w1t_bytes", &cnb_head_w1t_bytes);
+  m.def("head_w2t_bytes", &cnb_head_w2t_bytes);
+  m.def("head_prepare_weights_bf16", [](P w1, P w2, int cin, int cmid, int cout, P w1t, size_t w1tb, P w2t,
+                                        size_t w2tb, P stream) {
+    check(cnb_head_prepare_weights_bf16(ptr<const float>(w1), ptr<const float>(w2), cin, cmid, cout, ptr<void>(w1t),
+                                        w1tb, ptr<void>(w2t), w2tb, ptr<void>(stream)),
+          "cnb_head_prepare_weights_bf16");
+  });
+  m.def("head_workspace_bytes", &cnb_head_workspace_bytes);
+  m.def("head_forward_bf16", [](P input, int in_dt, int nhwc, P w1t, P b1, P w2t, P b2, P out, int b, int cin, int h,
+                                int w, int cmid, int cout, P ws, size_t wsb, P stream) {
+    check(cnb_head_forward_bf16(ptr<const void>(input), in_dt, nhwc, ptr<const void>(w1t), ptr<const float>(b1),
+                                ptr<const void>(w2t), ptr<const float>(b2), ptr<void>(out), b, cin, h, w, cmid, cout,
+                                ptr<void>(ws), wsb, ptr<void>(stream)),
+          "cnb_head_forward_bf16");
+  });
   m.def("dcnv2_backward", [](P input, P offset, P mask, P weight, P gout, P gin, P goff, P gmask, P gw, P gb, int b,
                              int cin, int h, int w, int cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh,
                              int dw, int dg, P ws, size_t wsb, P stream) {

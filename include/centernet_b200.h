@@ -44,7 +44,7 @@ extern "C" {
 
 /* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16, cnb_ctdet_decode_ex,
  * cnb_flip_merge_ex, cnb_ddd_decode_ex, cnb_multi_pose_decode_ex, cnb_edge_aggregate_ex, cnb_exct_decode_ex,
- * cnb_gather_feat_ex and the loss calls cnb_focal_*_ex / cnb_reg_loss_*ex). */
+ * cnb_gather_feat_ex, the loss calls cnb_focal_*_ex / cnb_reg_loss_*ex and cnb_head_forward_bf16). */
 #define CNB_DTYPE_F32 0
 #define CNB_DTYPE_BF16 1
 #define CNB_DTYPE_F16 2
@@ -542,6 +542,35 @@ int cnb_dcnv2_backward_bf16(const void *input, int input_dtype, int input_channe
                             int b, int cin, int h, int w, int cout, int kh, int kw,
                             int stride, int pad, int dil, int deformable_groups,
                             void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------- output heads: 3x3 conv, ReLU and 1x1 conv in one bf16 kernel (inference)
+ * Every DLASeg / PoseResNet head is nn.Sequential(Conv2d(cin, cmid, 3, padding=1), ReLU, Conv2d(cmid, cout, 1))
+ * (pose_dla_dcn.py:448-459, resnet_dcn.py:157-165, msra_resnet.py:135-143).  cnb_head_forward_bf16 runs all three in
+ * one kernel on bf16 wgmma; the cmid-channel intermediate stays on chip.  Numeric contract: the result is that of
+ *   1. rounding the input, w1 and w2 once to bf16 (RN);
+ *   2. an exact-product, fp32-accumulated 3x3 conv (zero padding 1) plus b1;
+ *   3. ReLU (NaN stays NaN, as torch.relu), then one rounding to bf16 (RN);
+ *   4. a fp32-accumulated 1x1 conv plus b2;
+ *   5. rounding to the input's dtype (fp32: none; bf16: RN).
+ * Only the order of the fp32 sums is free; it is fixed, so the output is bit-identical run to run (no atomics).
+ * Weights: w1 [cmid][cin][3][3] and w2 [cout][cmid] fp32, rounded and tiled once by cnb_head_prepare_weights_bf16 into
+ * w1t (cnb_head_w1t_bytes) and w2t (cnb_head_w2t_bytes), both 16-byte aligned, reused while the weights do not change.
+ * input: [b,cin,h,w] of input_dtype (CNB_DTYPE_F32 or CNB_DTYPE_BF16), NCHW, or [b][h][w][cin] (torch channels_last)
+ * when input_channels_last != 0; 16-byte aligned.  A bf16 channels-last input is read in place, any other is first
+ * copied to bf16 channels-last into the workspace (cnb_head_workspace_bytes; 0 when none is needed).  b1 [cmid] and
+ * b2 [cout] are fp32.  out: [b,cout,h,w] of input_dtype, in the input's layout.
+ * Range: cin and cmid multiples of 32, cmid <= 256, 1 <= cout <= 256, any b, h, w >= 1 within 32-bit indexing; else
+ * CNB_EUNSUPPORTED (and the size queries return 0).  Errors, checked before any CUDA call: CNB_EINVAL for a null
+ * pointer, an unknown dtype code, a bad shape or a misaligned buffer; CNB_EWORKSPACE for too small a buffer. */
+size_t cnb_head_w1t_bytes(int cin, int cmid);
+size_t cnb_head_w2t_bytes(int cmid, int cout);
+int cnb_head_prepare_weights_bf16(const float *w1, const float *w2, int cin, int cmid, int cout,
+                                  void *w1t, size_t w1t_bytes, void *w2t, size_t w2t_bytes, void *stream);
+size_t cnb_head_workspace_bytes(int b, int cin, int h, int w, int input_dtype, int input_channels_last);
+int cnb_head_forward_bf16(const void *input, int input_dtype, int input_channels_last,
+                          const void *w1t, const float *b1, const void *w2t, const float *b2, void *out,
+                          int b, int cin, int h, int w, int cmid, int cout,
+                          void *ws, size_t ws_bytes, void *stream);
 
 /* ------------------------------------------------- A10/A11: DCNv2, float64
  * The reference's second build, _ext.dcn_v2_double (dcn_v2_cuda_double.c, dcn_v2_im2col_cuda_double.cu): the
