@@ -81,20 +81,24 @@ __global__ void __launch_bounds__(1024) k_pose_assemble(const PoseArgs a) {
       d[D - 1] = (float)a.c_clses[o];
     }
     if (has_hp) {
+      // :548-551: first minimum of the L2 distance over the non-NaN distances (candidate 0 when all are NaN)
       float best = 0.0f, bx = 0.0f, by = 0.0f, bs = 0.0f;
-      for (int m = 0; m < K; ++m) {  // :548-551: first minimum of the L2 distance
+      for (int m = 0; m < K; ++m) {
         const float dx = kx - cx[m], dy = ky - cy[m];
         const float dist = sqrtf(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)));
-        if (m == 0 || dist < best) {
+        if (m == 0 || dist < best || (isnan(best) && !isnan(dist))) {
           best = dist; bx = cx[m]; by = cy[m]; bs = cs[m];
         }
       }
-      const float lim = fmaxf(bt - t, r - l) * 0.3f;  // :558-565
+      // :558-565; torch.max propagates NaN (fmaxf would drop it), and a NaN limit rejects nothing
+      const float bh = bt - t, bw = r - l;
+      const float lim = ((isnan(bh) || isnan(bw)) ? bh + bw : fmaxf(bh, bw)) * 0.3f;
       const bool reject = (bx < l) || (bx > r) || (by < t) || (by > bt) || (bs < 0.1f) || (best > lim);
-      if (!reject) {
-        kx = bx;
-        ky = by;
-      }
+      // :566-567: the reference's blend (1 - mask) * hm_kps + mask * kps, not a select, so that a NaN or infinite
+      // keypoint regression gives what the reference gives (0 * inf is NaN)
+      const float m = reject ? 1.0f : 0.0f;
+      kx = __fadd_rn(__fmul_rn(1.0f - m, bx), __fmul_rn(m, kx));
+      ky = __fadd_rn(__fmul_rn(1.0f - m, by), __fmul_rn(m, ky));
     }
     d[5 + 2 * j] = kx;
     d[5 + 2 * j + 1] = ky;

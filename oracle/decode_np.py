@@ -123,8 +123,32 @@ def ddd_decode(heat, rot, depth, dim, wh=None, reg=None, K=40):
 
 
 # --------------------------------------------------------------------------- A6
-def multi_pose_decode(heat, wh, kps, reg=None, hm_hp=None, hp_offset=None, K=100):
-    """models/decode.py:497-571."""
+def multi_pose_decode(heat, wh, kps, reg=None, hm_hp=None, hp_offset=None, K=100, nonfinite="reference"):
+    """models/decode.py:497-571.
+
+    ``nonfinite="reference"`` is the reference's arithmetic, NaN and inf included.  ``"library"`` is the keypoint
+    assembly's defined rule (DESIGN.md, "Non-finite scores"): the same arithmetic with two deviations, both where one
+    non-finite value would otherwise reach every detection of the image:
+    (a) a joint candidate at or below the threshold is exactly (score -1, x -10000, y -10000), whatever its offset
+        (the reference's ``-10000 + 0 * off`` is NaN for a non-finite offset);
+    (b) the nearest candidate is the first minimum over the non-NaN distances, candidate 0 when all are NaN (the
+        reference's ``torch.min`` picks the first NaN).
+    Heat-map scores are assumed finite (their rule is the selection's, ``oracle/select_torch.py``)."""
+    if nonfinite not in ("reference", "library"):
+        raise ValueError("nonfinite must be 'reference' or 'library'")
+    with np.errstate(invalid="ignore", over="ignore"):
+        return _multi_pose_decode(heat, wh, kps, reg, hm_hp, hp_offset, K, nonfinite == "library")
+
+
+def _first_min_skip_nan(dist):
+    """Index of the first minimum along the last axis, NaN skipped; 0 where every entry is NaN."""
+    nan = np.isnan(dist)
+    key = np.where(nan, F32(np.inf), dist)
+    hit = (key == key.min(axis=-1, keepdims=True)) & ~nan
+    return hit.argmax(axis=-1)
+
+
+def _multi_pose_decode(heat, wh, kps, reg, hm_hp, hp_offset, K, library):
     heat = np.asarray(heat, F32); wh = np.asarray(wh, F32); kps = np.asarray(kps, F32)
     B, C, H, W = heat.shape
     J = kps.shape[1] // 2
@@ -156,14 +180,21 @@ def multi_pose_decode(heat, wh, kps, reg=None, hm_hp=None, hp_offset=None, K=100
         else:
             hxs = hxs + F32(0.5)
             hys = hys + F32(0.5)
-        m = (hs > thresh).astype(F32)
-        hs = (F32(1) - m) * F32(-1) + m * hs
-        hys = (F32(1) - m) * F32(-10000) + m * hys
-        hxs = (F32(1) - m) * F32(-10000) + m * hxs
+        keep = hs > thresh
+        if library:                                                        # rule (a)
+            hs = np.where(keep, hs, F32(-1))
+            hys = np.where(keep, hys, F32(-10000))
+            hxs = np.where(keep, hxs, F32(-10000))
+        else:
+            m = keep.astype(F32)
+            hs = (F32(1) - m) * F32(-1) + m * hs
+            hys = (F32(1) - m) * F32(-10000) + m * hys
+            hxs = (F32(1) - m) * F32(-10000) + m * hxs
         hm_kps = np.stack([hxs, hys], axis=-1)                             # B,J,K,2
         d = reg_kps[:, :, :, None, :] - hm_kps[:, :, None, :, :]           # B,J,K(det),K(cand),2
         dist = np.sqrt((d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]).astype(F32)).astype(F32)
-        min_ind = dist.argmin(axis=3)                                      # first minimum
+        # first minimum; np.argmin, like torch.min, takes the first NaN if there is one; rule (b) skips NaN
+        min_ind = _first_min_skip_nan(dist) if library else dist.argmin(axis=3)
         min_dist = np.take_along_axis(dist, min_ind[..., None], axis=3)    # B,J,K,1
         sel_s = np.take_along_axis(hs, min_ind, axis=2)[..., None]
         sel_kp = np.take_along_axis(hm_kps, min_ind[..., None].repeat(2, axis=-1), axis=2)
@@ -171,9 +202,9 @@ def multi_pose_decode(heat, wh, kps, reg=None, hm_hp=None, hp_offset=None, K=100
         r_ = boxes[:, None, :, 2:3]; b_ = boxes[:, None, :, 3:4]
         bad = ((sel_kp[..., 0:1] < l) | (sel_kp[..., 0:1] > r_) |
                (sel_kp[..., 1:2] < t) | (sel_kp[..., 1:2] > b_) |
-               (sel_s < thresh) | (min_dist > np.maximum(b_ - t, r_ - l) * F32(0.3)))
-        bad = np.broadcast_to(bad, sel_kp.shape)
-        out_kp = np.where(bad, reg_kps, sel_kp)
+               (sel_s < thresh) | (min_dist > np.maximum(b_ - t, r_ - l) * F32(0.3)))   # np.maximum keeps NaN
+        m = np.broadcast_to(bad, sel_kp.shape).astype(F32)
+        out_kp = (F32(1) - m) * sel_kp + m * reg_kps                       # the reference's blend (:566)
         kp = out_kp.transpose(0, 2, 1, 3).reshape(B, K, J * 2)
     return np.concatenate([boxes, scores[..., None], kp, clses.astype(F32)[..., None]],
                           axis=2).astype(F32)

@@ -42,6 +42,38 @@ def assert_dets_equal(ref, got, score_col=4, atol=0.0, positive_only=False, what
             k = e + 1
 
 
+def canonical_bits(a):
+    """float32 -> its uint32 bits, with every NaN (any sign, any payload) mapped to the one NaN 0x7fc00000."""
+    a = np.asarray(a, np.float32)
+    u = np.ascontiguousarray(a).view(np.uint32).copy()
+    u[np.isnan(a)] = 0x7fc00000
+    return u
+
+
+def assert_dets_bits(ref, got, score_col=4, what=""):
+    """assert_dets_equal without any tolerance at the bit level: every float equal as canonical_bits (so -0 differs
+    from +0 and NaN matches NaN); rows compared as multisets inside every run of equal scores."""
+    ref, got = canonical_bits(ref), canonical_bits(got)
+    assert ref.shape == got.shape, (what, ref.shape, got.shape)
+    for b in range(ref.shape[0]):
+        rs = ref[b, :, score_col]
+        np.testing.assert_array_equal(got[b, :, score_col], rs, err_msg="%s: scores differ (image %d)" % (what, b))
+        k, K = 0, ref.shape[1]
+        while k < K:
+            e = k
+            while e + 1 < K and rs[e + 1] == rs[k]:
+                e += 1
+            a, c = ref[b, k:e + 1], got[b, k:e + 1]
+            if e > k:
+                a = a[np.lexsort(a.T[::-1])]; c = c[np.lexsort(c.T[::-1])]
+            if not np.array_equal(a, c):
+                i = np.argwhere(a != c)[0]
+                raise AssertionError("%s: image %d rows %d..%d differ, first at row %d column %d: got %r, want %r"
+                                     % (what, b, k, e, k + i[0], i[1], c[tuple(i)].view(np.float32),
+                                        a[tuple(i)].view(np.float32)))
+            k = e + 1
+
+
 def assert_same_bits(got, want, what=""):
     """float32 arrays equal bit for bit (the sign of zero included); NaN matches NaN of any sign or payload (the
     device's canonical NaN and x86's default NaN differ in their bits, not in what they mean)."""

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import big_inputs as BI
-from helpers import assert_dets_equal, golden
+from helpers import assert_dets_bits, assert_dets_equal, golden
 from oracle import decode_np as O
 
 TOL = 1e-4
@@ -94,7 +94,7 @@ def test_gpu_multi_pose_big():
     g, ins = _multi_pose()
     heat, wh, kps, reg, hm_hp, hp_off = dev(*ins)
     got = D.multi_pose_decode(heat, wh, kps, reg=reg, hm_hp=hm_hp, hp_offset=hp_off, K=100).cpu().numpy()
-    assert_dets_equal(g["dets"], got, atol=TOL, what="big multi_pose")
+    assert_dets_bits(g["dets"], got, what="big multi_pose")
 
 
 @pytest.mark.gpu

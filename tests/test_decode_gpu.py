@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import assert_dets_equal, golden
+from helpers import assert_dets_bits, assert_dets_equal, golden
 from oracle import decode_np as O
 
 pytestmark = pytest.mark.gpu
@@ -66,10 +66,10 @@ def test_golden_ddd():
     g = golden("ddd")
     K = int(g["K"])
     heat, rot, depth, dim, wh, reg = dev(g["heat"], g["rot"], g["depth"], g["dim"], g["wh"], g["reg"])
-    assert_dets_equal(g["dets"], D.ddd_decode(heat, rot, depth, dim, wh=wh, reg=reg, K=K).cpu().numpy(),
-                      score_col=2, atol=TOL, what="ddd")
-    assert_dets_equal(g["dets_min"], D.ddd_decode(heat, rot, depth, dim, K=K).cpu().numpy(), score_col=2, atol=TOL,
-                      what="ddd_min")
+    assert_dets_bits(g["dets"], D.ddd_decode(heat, rot, depth, dim, wh=wh, reg=reg, K=K).cpu().numpy(),
+                     score_col=2, what="ddd")
+    assert_dets_bits(g["dets_min"], D.ddd_decode(heat, rot, depth, dim, K=K).cpu().numpy(), score_col=2,
+                     what="ddd_min")
 
 
 # ------------------------------------------------------------------ oracle sweeps

@@ -4,12 +4,11 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import assert_dets_equal, golden
+from helpers import assert_dets_bits, golden
 from oracle import decode_np as O
 from oracle import image_np, losses_np
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-4
 
 
 def dev(*arrs):
@@ -34,11 +33,11 @@ def test_golden_multi_pose():
     K = int(g["K"])
     heat, wh, kps, reg, hm_hp, off = dev(g["heat"], g["wh"], g["kps"], g["reg"], g["hm_hp"], g["hp_offset"])
     got = D.multi_pose_decode(heat, wh, kps, reg=reg, hm_hp=hm_hp, hp_offset=off, K=K).cpu().numpy()
-    assert_dets_equal(g["dets"], got, atol=TOL, what="multi_pose")
+    assert_dets_bits(g["dets"], got, what="multi_pose")
     got = D.multi_pose_decode(heat, wh, kps, reg=None, hm_hp=hm_hp, hp_offset=None, K=K).cpu().numpy()
-    assert_dets_equal(g["dets_nooff"], got, atol=TOL, what="multi_pose_nooff")
+    assert_dets_bits(g["dets_nooff"], got, what="multi_pose_nooff")
     got = D.multi_pose_decode(heat, wh, kps, reg=reg, K=K).cpu().numpy()
-    assert_dets_equal(g["dets_nohp"], got, atol=TOL, what="multi_pose_nohp")
+    assert_dets_bits(g["dets_nohp"], got, what="multi_pose_nohp")
 
 
 @pytest.mark.parametrize("B,H,W,K", [(2, 128, 128, 100), (3, 40, 56, 32)])
@@ -51,9 +50,7 @@ def test_multi_pose_vs_oracle(B, H, W, K):
     want = O.multi_pose_decode(heat, wh, kps, reg, hm_hp, off, K=K)
     got = D.multi_pose_decode(*dev(heat, wh, kps, reg, hm_hp, off), K=K).cpu().numpy()
     assert got.shape == (B, K, 40)
-    np.testing.assert_array_equal(got[..., 4], want[..., 4])
-    np.testing.assert_array_equal(got[..., -1], want[..., -1])
-    np.testing.assert_allclose(got, want, rtol=0, atol=TOL)
+    assert_dets_bits(want, got, what="multi_pose B=%d %dx%d K=%d" % (B, H, W, K))
 
 
 # ------------------------------------------------------------------ edge aggregation (bit-exact: sequential fp32 sums)

@@ -4,8 +4,8 @@ Contract 1: multi_pose_decode_from_logits(hm, ..., hm_hp) == multi_pose_decode(t
 torch.sigmoid(hm_hp)), and ddd_decode_from_logits(hm, rot, dep, ...) == ddd_decode(torch.sigmoid(hm), rot,
 1. / (torch.sigmoid(dep) + 1e-6) - 1., ...), bit for bit, with torch's own CUDA ops on the right.
 Contract 2: every one of the four functions returns for half heads (any mix of dtypes) what it returns for their
-.float() upcast.  The fp32 decodes on the right are pinned against the reference elsewhere (test_pose_aggr_loss_gpu.py,
-test_decode_gpu.py, test_big_golden.py)."""
+.float() upcast.  The fp32 decodes on the right are pinned bit for bit against the reference and the oracle elsewhere
+(test_pose_ddd_edges_gpu.py, test_pose_aggr_loss_gpu.py, test_decode_gpu.py, test_big_golden.py)."""
 import numpy as np
 import pytest
 import torch
