@@ -1,5 +1,5 @@
-"""CPU: the C-ABI library loads and exports every symbol include/centernet_b200.h declares;
-argument validation works without a GPU (no compute calls here)."""
+"""CPU: the C-ABI library loads and exports every symbol include/centernet_b200.h declares and _C binds
+each of them with the header's parameters; argument validation works without a GPU (no compute calls here)."""
 import ctypes
 import os
 import re
@@ -10,9 +10,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _declared():
+    """{name: [parameter declarations]} of every function the header declares ((void) is no parameter)."""
     src = open(os.path.join(ROOT, "include", "centernet_b200.h")).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(cnb_[a-z0-9_]+)\s*\(", src)))
+    return {name: [p.strip() for p in params.split(",") if p.strip() != "void"]
+            for name, params in re.findall(r"\b(cnb_[a-z0-9_]+)\s*\(([^)]*)\)", src)}
 
 
 def test_every_declared_symbol_is_exported():
@@ -23,6 +25,24 @@ def test_every_declared_symbol_is_exported():
         assert hasattr(lib, n), "missing export " + n
     lib.cnb_version.restype = ctypes.c_int
     assert lib.cnb_version() >= 100
+
+
+def test_every_declared_function_is_bound_with_its_parameters():
+    """_C binds exactly the header's functions, each positionally with the header's parameters in order: a float
+    where the header has float or double, an int for a pointer or an integer type.  Reads __doc__ only; a call with
+    made-up pointers could reach the GPU."""
+    from centernet_b200._lib import _C   # the extension itself; centernet_b200._C is its device-guarding proxy
+    decls = _declared()
+    bound = {n for n in dir(_C) if not n.startswith("_") and callable(getattr(_C, n))}
+    assert bound == {n[4:] for n in decls}
+    for name, params in decls.items():
+        if name in ("cnb_last_error", "cnb_select_plan_info"):   # bound by hand: return a str / a dict
+            continue
+        want = ["float" if "*" not in p and re.search(r"\b(float|double)\b", p) else "int" for p in params]
+        sig = getattr(_C, name[4:]).__doc__.splitlines()[0]
+        got = [(int(i), "float" if "float" in t.lower() else "int" if "int" in t.lower() else t)
+               for i, t in re.findall(r"\barg(\d+): ([\w. |]+)", sig)]
+        assert got == list(enumerate(want)), "%s: header (%s), bound %s" % (name, ", ".join(params), sig)
 
 
 def test_pybind_layer_and_validation():
