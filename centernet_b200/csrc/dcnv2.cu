@@ -798,6 +798,71 @@ int cnb_dcnv2_forward_fused_bf16(const void *input, int input_dtype, int input_c
                        stride, pad, dil, deformable_groups, workspace, workspace_bytes, stream, 1);
 }
 
+// ------------------------------------------------------------------ DCN block (opt-in; dcnv2_tc.cu)
+// The range of the block kernel: the DCN of dla_34 and resnet_dcn
+static int dcn_block_range(const char *fn, int cin, int kh, int kw, int stride, int pad, int dil, int dg) {
+  CNB_REQUIRE(kh == 3 && kw == 3 && stride == 1 && pad == 1 && dil == 1 && dg == 1 && cin % TC_CB == 0,
+              CNB_EUNSUPPORTED,
+              "%s: needs a 3x3 kernel, stride 1, padding 1, dilation 1, one deformable group and cin %% 32 == 0 "
+              "(got %dx%d, stride %d, padding %d, dilation %d, %d groups, cin %d)", fn, kh, kw, stride, pad, dil, dg, cin);
+  return CNB_OK;
+}
+
+size_t cnb_dcnv2_om_tiles_bytes(int cin, int kh, int kw, int dg) {
+  const char *fn = "cnb_dcnv2_om_tiles_bytes";
+  if (cin <= 0 || dcn_block_range(fn, cin, kh, kw, 1, 1, 1, dg) != CNB_OK) return 0;
+  return dcn_om_tiles_bytes(cin);
+}
+
+int cnb_dcnv2_prepare_om_weights_bf16(const float *w_om, int cin, int kh, int kw, int dg, void *om_tiles,
+                                      size_t om_tiles_bytes, void *stream) {
+  const char *fn = "cnb_dcnv2_prepare_om_weights_bf16";
+  CNB_REQUIRE(w_om && om_tiles, CNB_EINVAL, "%s: null pointer", fn);
+  CNB_REQUIRE(cin > 0 && kh > 0 && kw > 0 && dg > 0, CNB_EINVAL, "%s: bad shape", fn);
+  const int rc = dcn_block_range(fn, cin, kh, kw, 1, 1, 1, dg);
+  if (rc != CNB_OK) return rc;
+  CNB_REQUIRE(om_tiles_bytes >= dcn_om_tiles_bytes(cin), CNB_EWORKSPACE, "%s: buffer %zu < %zu", fn, om_tiles_bytes,
+              dcn_om_tiles_bytes(cin));
+  CNB_REQUIRE((reinterpret_cast<uintptr_t>(om_tiles) & 15u) == 0, CNB_EINVAL, "%s: buffer must be 16-byte aligned", fn);
+  return dcn_prepare_om_weights_bf16(w_om, cin, om_tiles, (cudaStream_t)stream);
+}
+
+size_t cnb_dcnv2_block_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw, int stride, int pad,
+                                       int dil, int dg) {
+  const char *fn = "cnb_dcnv2_block_workspace_bytes";
+  DcnPlan p;
+  if (dcn_plan(fn, b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg, false, false, false, &p) !=
+          CNB_OK ||
+      dcn_block_range(fn, cin, kh, kw, stride, pad, dil, dg) != CNB_OK)
+    return 0;
+  return p.bf16.bytes;
+}
+
+int cnb_dcnv2_forward_block_bf16(const void *input, int input_dtype, int input_channels_last, const void *om_tiles,
+                                 const float *om_bias, const void *wtiles, const float *bias, const float *bn_scale,
+                                 const float *bn_shift, int relu, void *output, int b, int cin, int h, int w, int cout,
+                                 int kh, int kw, int stride, int pad, int dil, int deformable_groups, void *workspace,
+                                 size_t workspace_bytes, void *stream) {
+  const char *fn = "cnb_dcnv2_forward_block_bf16";
+  CNB_REQUIRE(input && om_tiles && wtiles && output && workspace, CNB_EINVAL, "%s: null pointer", fn);
+  CNB_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), CNB_EINVAL, "%s: bn_scale and bn_shift go together", fn);
+  CNB_REQUIRE(input_dtype == CNB_DTYPE_F32 || input_dtype == CNB_DTYPE_BF16, CNB_EINVAL,
+              "%s: input dtype must be CNB_DTYPE_F32 or CNB_DTYPE_BF16 (got %d)", fn, input_dtype);
+  DcnPlan p;
+  int rc = dcn_plan(fn, b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, deformable_groups, false,
+                    input_channels_last != 0, false, &p);
+  if (rc != CNB_OK) return rc;
+  rc = dcn_block_range(fn, cin, kh, kw, stride, pad, dil, deformable_groups);
+  if (rc != CNB_OK) return rc;
+  CNB_REQUIRE(workspace_bytes >= p.bf16.bytes, CNB_EWORKSPACE, "%s: workspace too small (%zu < %zu)", fn,
+              workspace_bytes, p.bf16.bytes);
+  CNB_REQUIRE(((reinterpret_cast<uintptr_t>(workspace) | reinterpret_cast<uintptr_t>(wtiles) |
+                reinterpret_cast<uintptr_t>(om_tiles) | reinterpret_cast<uintptr_t>(input)) & 15u) == 0,
+              CNB_EINVAL, "%s: buffers must be 16-byte aligned", fn);
+  return dcn_forward_block_bf16(p, input, input_dtype == CNB_DTYPE_BF16, om_tiles, om_bias, wtiles, bias, output,
+                                workspace, (cudaStream_t)stream, bn_scale, bn_shift, relu);
+}
+
 int cnb_dcnv2_forward(const float *input, const float *offset, const float *mask, const float *weight,
                       const float *bias, float *output, int b, int cin, int h, int w, int cout, int kh, int kw,
                       int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int deformable_groups,

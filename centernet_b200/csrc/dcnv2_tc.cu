@@ -33,9 +33,10 @@
 // cnb_dcnv2_forward_prepared (what the Python module does).
 //
 // k_dcn_forward_bf16 (further down) is the opt-in bf16 form of the forward: bf16 tiles, wgmma k16 bf16 -> fp32.
+// Its OM variant (the DCN block) also computes the 3x3 conv_offset_mask inside the kernel.
 #include <cuda_bf16.h>
 
-#include "dcnv2_tc.cuh"
+#include "halo.cuh"
 
 namespace cnb {
 
@@ -134,11 +135,12 @@ __device__ __forceinline__ ItemTc tc_item(const DcnShapeTc &s, int item) {
 }
 
 // Bilinear geometry of every (tap, pixel) of item `it` in deformable group g, the mask folded into the corner weights
-// (dcn_v2_im2col_cuda.cu:18-47, :165); st = this thread's index among the sampler threads.  Shared by the fp32 and the
-// bf16 forward, so both sample at bit-identical fp32 weights.
-__device__ __forceinline__ void tc_build_meta(const DcnShapeTc &s, const float *__restrict__ offset,
-                                              const float *__restrict__ mask, const ItemTc &it, int g, int st,
-                                              int KT, long long HWo, TapMetaTc *meta) {
+// (dcn_v2_im2col_cuda.cu:18-47, :165); st = this thread's index among the sampler threads.  load(t, pp, p, dy, dx, m)
+// fetches the offsets and the mask (a logit when s.mask_logit) of tap t at tile pixel pp, image pixel p.  Shared by the
+// fp32, the bf16 and the block forward, so all of them sample at bit-identical fp32 weights for the same offsets.
+template <typename Load>
+__device__ __forceinline__ void tc_build_meta_from(const DcnShapeTc &s, const ItemTc &it, int st, int KT,
+                                                   TapMetaTc *meta, Load load) {
   for (int idx = st; idx < TC_NT * TC_TP; idx += TC_SAMPLERS * 32) {
     const int t = idx / TC_TP, pp = idx - t * TC_TP;
     const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
@@ -148,9 +150,8 @@ __device__ __forceinline__ void tc_build_meta(const DcnShapeTc &s, const float *
     if (ho < s.Ho && wo < s.Wo && t < KT) {
       const long long p = (long long)ho * s.Wo + wo;
       const int i = t / s.kw, j = t - i * s.kw;
-      const float *op = offset + (long long)it.b * s.off_bs + (long long)g * 2 * KT * HWo;
-      const float dy = __ldg(op + (2 * t) * HWo + p), dx = __ldg(op + (2 * t + 1) * HWo + p);
-      float m = __ldg(mask + (long long)it.b * s.mask_bs + ((long long)g * KT + t) * HWo + p);
+      float dy, dx, m;
+      load(t, pp, p, dy, dx, m);
       if (s.mask_logit) m = 1.0f / (1.0f + expf(-m));        // torch.sigmoid(mask), dcn_v2.py:68
       const float h_im = (float)(ho * s.sh - s.ph + i * s.dh) + dy;
       const float w_im = (float)(wo * s.sw - s.pw + j * s.dw) + dx;
@@ -167,6 +168,19 @@ __device__ __forceinline__ void tc_build_meta(const DcnShapeTc &s, const float *
     }
     meta[idx] = mt;
   }
+}
+
+// ... with the offsets and the mask read from global memory
+__device__ __forceinline__ void tc_build_meta(const DcnShapeTc &s, const float *__restrict__ offset,
+                                              const float *__restrict__ mask, const ItemTc &it, int g, int st,
+                                              int KT, long long HWo, TapMetaTc *meta) {
+  const float *op = offset + (long long)it.b * s.off_bs + (long long)g * 2 * KT * HWo;
+  const float *mp = mask + (long long)it.b * s.mask_bs + (long long)g * KT * HWo;
+  tc_build_meta_from(s, it, st, KT, meta, [&](int t, int, long long p, float &dy, float &dx, float &m) {
+    dy = __ldg(op + (2 * t) * HWo + p);
+    dx = __ldg(op + (2 * t + 1) * HWo + p);
+    m = __ldg(mp + t * HWo + p);
+  });
 }
 
 template <int CO_T, int STAGES>
@@ -473,22 +487,51 @@ __global__ void __launch_bounds__(256) k_dcn_reduce_bf16(const float *__restrict
   }
 }
 
+// DCN block variant (OM = true, cnb_dcnv2_forward_block_bf16): the 3x3 conv_offset_mask runs inside the kernel.
+// For every item the TMA warp streams, per 32-channel block, the (tw + 2) x (th + 2) halo of the tile as four 8-channel
+// slabs (4-D tensor-map loads; the out-of-bounds fill is the conv's zero padding, halo.cuh) and the nine [32][32] W_om
+// tiles of the block into a ring of its own.  The consumer warpgroups compute om[128 px][27 -> 32] with wgmma m64n32k16
+// straight from the halo (shifted descriptors, no im2col), add b_om in fp32 and leave the 27 fp32 values of every pixel
+// in one of two shared buffers; the samplers build the item's tap geometry from that buffer (tc_build_meta_from, the
+// mask logit through the same sigmoid).  The consumers compute the offsets of the CTA's NEXT item before the main loop
+// of the current one, so the samplers find them ready when they reach the item boundary.  Every item computes its own
+// offsets (Cout tiles and K splits of one pixel tile recompute them).  Warpgroup wg's 64 GEMM rows are the tile's
+// column half wg (8 x 16 tiles: 8 rows of 8 pixels, one halo row apart) or row half wg (16 x 8 tiles).
+constexpr int OM_N = 32;                             // 27 offset / mask channels, padded to the wgmma N
+constexpr int OM_C = 27;                             // dg * 3 * 9 with dg = 1
+constexpr int OM_PITCH = TC_TP + 4;                  // fp32 om of one channel: 128 pixels (+4: conflict-free stores)
+constexpr uint32_t OM_SLAB = 180 * 16;               // one 8-channel slab of a 10 x 18 (or 18 x 10) halo
+constexpr uint32_t OM_SLAB_PITCH = 2944;             // slabs 128-byte aligned (TMA destination)
+constexpr uint32_t OM_HALO_BYTES = 4 * OM_SLAB_PITCH;
+constexpr uint32_t OM_W_BYTES = TC_NT * OM_N * TC_K * 2;   // the nine W_om tiles of one channel block
+constexpr uint32_t OM_STAGE_BYTES = OM_HALO_BYTES + OM_W_BYTES;
+constexpr int OM_STAGES = 2;
+constexpr uint32_t OM_BUF_BYTES = (OM_C * OM_PITCH * 4 + 127) / 128 * 128;
+constexpr uint32_t OM_SMEM_BYTES = OM_STAGES * OM_STAGE_BYTES + 2 * OM_BUF_BYTES + 128;   // + 128: alignment slack
+
 // Warp roles, items and mbarrier hand-over as k_dcn_forward_tc.  Sampler warp item = one 8-row group of the A tile
 // (8 pixels): lane = pixel * 4 + k-chunk, every lane gathers the 4 corners of its pixel as 16-byte pieces (8 bf16
 // channels), interpolates in fp32 and stores one rounded 16-byte k-chunk; each warp fills two row groups a chunk, both
 // gathered before either is reduced.
-template <int CO_T, int STAGES, typename TOut>
+template <int CO_T, int STAGES, typename TOut, bool OM>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict__ offset,
                    const float *__restrict__ mask, const __nv_bfloat16 *__restrict__ wtiles,
-                   const float *__restrict__ bias, TOut *__restrict__ y, float *__restrict__ part, const DcnShapeTc s) {
-  extern __shared__ __align__(128) unsigned char tc_smem[];
+                   const float *__restrict__ bias, TOut *__restrict__ y, float *__restrict__ part, const DcnShapeTc s,
+                   const __grid_constant__ CUtensorMap xmap, const __nv_bfloat16 *__restrict__ womt,
+                   const float *__restrict__ bom) {
+  extern __shared__ __align__(128) unsigned char tc_smem_raw[];
+  // the block variant's TMA halo needs a 128-byte aligned destination
+  unsigned char *tc_smem = OM ? tc_smem_raw + ((128u - (smem_u32(tc_smem_raw) & 127u)) & 127u) : tc_smem_raw;
   constexpr int B_BYTES = CO_T * TC_K * 2;
   constexpr int STAGE_BYTES = BF_A_BYTES + B_BYTES;
   constexpr int ROWGROUPS = TC_TP / 8 / TC_SAMPLERS;   // 2 row groups a sampler warp
   static_assert(ROWGROUPS == 2, "k_dcn_forward_bf16: two row groups a sampler warp");
   TapMetaTc *meta = reinterpret_cast<TapMetaTc *>(tc_smem + (size_t)STAGES * STAGE_BYTES);     // [9][128]
+  unsigned char *om_ring = tc_smem + (size_t)STAGES * STAGE_BYTES + sizeof(TapMetaTc) * TC_NT * TC_TP;
+  float *om_buf = reinterpret_cast<float *>(om_ring + OM_STAGES * OM_STAGE_BYTES);   // [2][27][OM_PITCH]
   __shared__ __align__(8) uint64_t a_full[STAGES], b_full[STAGES], empty[STAGES];
+  __shared__ __align__(8) uint64_t om_full[OM ? OM_STAGES : 1], om_empty[OM ? OM_STAGES : 1], om_ready[2], om_free[2];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int KT = s.kh * s.kw;
@@ -501,6 +544,16 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
       mbar_init(&b_full[i], 1);
       mbar_init(&empty[i], TC_MMA_WGS);
     }
+    if (OM) {
+      for (int i = 0; i < OM_STAGES; ++i) {
+        mbar_init(&om_full[i], 1);
+        mbar_init(&om_empty[i], TC_MMA_WGS);
+      }
+      for (int i = 0; i < 2; ++i) {
+        mbar_init(&om_ready[i], TC_MMA_WGS * 128);
+        mbar_init(&om_free[i], 1);
+      }
+    }
     mbar_fence_init();
   }
   __syncthreads();
@@ -510,8 +563,8 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
     const int sw = warp - TC_WARP_S0, st = tid - TC_WARP_S0 * 32;
     const int sp = lane >> 2, sq = lane & 3;
     const int rg0 = sw * ROWGROUPS, rg1 = rg0 + 1;
-    int stage = 0, ph = 0;
-    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
+    int stage = 0, ph = 0, n = 0;
+    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x, ++n) {
       const ItemTc it = tc_item(s, item);
       const __nv_bfloat16 *xbat = xt + (long long)it.b * HW * Cp + sq * 8;
       int cur_g = -1;
@@ -520,8 +573,20 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
         if (g != cur_g) {
           cur_g = g;
           named_bar_sync(1, TC_SAMPLERS * 32);   // everybody is done reading the previous geometry
-          tc_build_meta(s, offset, mask, it, g, st, KT, HWo, meta);
+          if constexpr (OM) {
+            // dg == 1: one geometry an item, from the offsets the consumers left in buffer n % 2
+            mbar_wait(&om_ready[n & 1], (uint32_t)((n >> 1) & 1));
+            const float *ob = om_buf + (n & 1) * (OM_BUF_BYTES / 4);
+            tc_build_meta_from(s, it, st, KT, meta, [&](int t, int pp, long long, float &dy, float &dx, float &m) {
+              dy = ob[(2 * t) * OM_PITCH + pp];
+              dx = ob[(2 * t + 1) * OM_PITCH + pp];
+              m = ob[(2 * TC_NT + t) * OM_PITCH + pp];
+            });
+          } else {
+            tc_build_meta(s, offset, mask, it, g, st, KT, HWo, meta);
+          }
           named_bar_sync(1, TC_SAMPLERS * 32);
+          if (OM && st == 0) mbar_arrive_tc(&om_free[n & 1]);   // the buffer may take the offsets of item n + 2
         }
         const __nv_bfloat16 *xb = xbat + (long long)bi * TC_CB;
         for (int tap = 0; tap < TC_NT; ++tap) {
@@ -567,8 +632,28 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
   } else if (warp == TC_WARP_TMA) {
     // =========================================================== B operand: one bf16 weight tile by TMA bulk copy
     if (lane == 0) {
-      int stage = 0, ph = 0;
+      int stage = 0, ph = 0, os = 0, oph = 0;
+      // block variant: the halo slabs and W_om tiles of every channel block of item `item`, in consumer order
+      auto put_om = [&](int item) {
+        const ItemTc it = tc_item(s, item);
+        for (int cb = 0; cb < s.nb; ++cb) {
+          mbar_wait(&om_empty[os], (uint32_t)(oph ^ 1));
+          unsigned char *h = om_ring + (size_t)os * OM_STAGE_BYTES;
+          mbar_expect_tx(&om_full[os], 4u * OM_SLAB + OM_W_BYTES);
+#pragma unroll
+          for (int kc = 0; kc < 4; ++kc)
+            tma_load_4d(h + kc * OM_SLAB_PITCH, &xmap, cb * TC_CB + kc * 8, it.tx0 - 1, it.ty0 - 1, it.b, &om_full[os]);
+          bulk_g2s(h + OM_HALO_BYTES, womt + (size_t)cb * (OM_W_BYTES / 2), OM_W_BYTES, &om_full[os]);
+          if (++os == OM_STAGES) { os = 0; oph ^= 1; }
+        }
+      };
+      if constexpr (OM) {
+        if ((int)blockIdx.x < s.n_items) put_om(blockIdx.x);
+      }
       for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
+        if constexpr (OM) {
+          if (item + (int)gridDim.x < s.n_items) put_om(item + gridDim.x);
+        }
         const ItemTc it = tc_item(s, item);
         for (int bi = it.b0; bi < it.b1; ++bi) {
           for (int tap = 0; tap < TC_NT; ++tap) {
@@ -585,8 +670,59 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
   } else {
     // =========================================================== consumers: wgmma over the ring, epilogue from registers
     const int wgi = warp >> 2, wq = warp & 3;
-    int stage = 0, ph = 0;
-    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
+    int stage = 0, ph = 0, n = 0;
+    // block variant: om of the CTA's k-th item into buffer k % 2 -- fp32 sums of exact bf16 products, + b_om.  The
+    // k-th item takes offset-ring slots k * nb .. k * nb + nb - 1 (no ring state stays live across the main loop)
+    auto om_gemm = [&](int k) {
+      const uint32_t hx16 = (uint32_t)(s.tw + 2) * 16u;               // one halo row
+      const uint32_t half = s.tw == 16 ? (uint32_t)wgi * 128u : (uint32_t)wgi * 8u * hx16;
+      float q[OM_N / 2];
+#pragma unroll
+      for (int i = 0; i < OM_N / 2; ++i) q[i] = 0.f;
+      for (int cb = 0; cb < s.nb; ++cb) {
+        const int slot = k * s.nb + cb, os = slot % OM_STAGES;
+        mbar_wait(&om_full[os], (uint32_t)((slot / OM_STAGES) & 1));
+        const uint32_t h = smem_u32(om_ring + (size_t)os * OM_STAGE_BYTES) + half;
+        const uint32_t wb = smem_u32(om_ring + (size_t)os * OM_STAGE_BYTES + OM_HALO_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < TC_NT; ++tap) {
+          const uint32_t a = h + (uint32_t)((tap / 3) * (int)hx16 + (tap % 3) * 16);
+#pragma unroll
+          for (int ks = 0; ks < 2; ++ks)   // one k16 step = two 8-channel slabs
+            wgmma_ss<OM_N>(q, wg_desc(a + (uint32_t)ks * 2u * OM_SLAB_PITCH, OM_SLAB_PITCH, hx16),
+                           wg_desc(wb + (uint32_t)tap * (OM_N * TC_K * 2) + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO,
+                                   BF_B_SBO),
+                           (cb > 0 || tap > 0 || ks > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        if ((tid & 127) == 0) mbar_arrive_tc(&om_empty[os]);
+      }
+      mbar_wait(&om_free[k & 1], (uint32_t)(((k >> 1) & 1) ^ 1));   // the samplers are done with item k - 2
+      float *ob = om_buf + (k & 1) * (OM_BUF_BYTES / 4);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = wq * 16 + (lane >> 2) + 8 * hh;                 // GEMM row: pixel (m / 8, m % 8) of the half
+        const int pp = s.tw == 16 ? (m >> 3) * 16 + wgi * 8 + (m & 7) : wgi * 64 + m;
+#pragma unroll
+        for (int j = 0; j < OM_N / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * j + 2 * (lane & 3) + e;
+            if (c < OM_C) ob[c * OM_PITCH + pp] = bom ? q[4 * j + 2 * hh + e] + __ldg(bom + c) : q[4 * j + 2 * hh + e];
+          }
+        }
+      }
+      mbar_arrive_tc(&om_ready[k & 1]);
+    };
+    if constexpr (OM) {
+      if ((int)blockIdx.x < s.n_items) om_gemm(0);
+    }
+    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x, ++n) {
+      if constexpr (OM) {
+        if (item + (int)gridDim.x < s.n_items) om_gemm(n + 1);
+      }
       const ItemTc it = tc_item(s, item);
       float d[CO_T / 2];
 #pragma unroll
@@ -652,47 +788,61 @@ int dcn_prepare_weights_bf16(const float *weight, int cin, int cout, int kh, int
   return CNB_OK;
 }
 
-template <int CO_T, typename TOut>
-static int launch_fwd_bf16(const __nv_bfloat16 *xt, const float *offset, const float *mask, const void *wtiles,
-                           const float *bias, void *output, float *part, const DcnShapeTc &s, cudaStream_t stream) {
-  constexpr int STAGES = BF_STAGES;
-  const size_t smem = (size_t)STAGES * (BF_A_BYTES + CO_T * TC_K * 2) + sizeof(TapMetaTc) * TC_NT * TC_TP;
-  static thread_local int dev_done = -1;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev_done != dev) {
-    CNB_CUDA(cudaFuncSetAttribute(k_dcn_forward_bf16<CO_T, STAGES, TOut>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)smem));
-    dev_done = dev;
-  }
-  const int grid = s.n_items < num_sms() ? s.n_items : num_sms();
-  k_dcn_forward_bf16<CO_T, STAGES, TOut><<<grid, TC_THREADS, smem, stream>>>(
-      xt, offset, mask, reinterpret_cast<const __nv_bfloat16 *>(wtiles), bias, reinterpret_cast<TOut *>(output), part,
-      s);
-  CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 (wgmma)");
+// W_om [27][Cin][3][3] (fp32) -> per channel block nine bf16 tiles [32][32] (rows 27..31 zero), tile index bi * 9 + tap:
+// k_dcn_prep_weights_bf16 with one Cout tile of 32 rows
+int dcn_prepare_om_weights_bf16(const float *w_om, int cin, void *om_tiles, cudaStream_t stream) {
+  DcnShapeTc s;
+  fill_shape(&s, 1, cin, 8, 8, OM_C, 3, 3, 1, 1, 1, 1, 1, 1, 1);
+  s.co_t = OM_N;
+  s.n_cot = 1;
+  k_dcn_prep_weights_bf16<<<s.nb * TC_NT, 256, 0, stream>>>(w_om, s, reinterpret_cast<unsigned char *>(om_tiles));
+  CNB_CHECK_LAUNCH("cnb_dcnv2 bf16 offset-conv weight tiles");
   count_launch();
   return CNB_OK;
 }
 
-int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
-                     const void *wtiles, const float *bias, void *output, bool out_bf16, void *workspace,
-                     cudaStream_t stream, int fused_offset_mask, const float *epi_scale, const float *epi_shift,
-                     int relu) {
-  DcnShapeTc s = p.s;
-  if (fused_offset_mask) {   // `offset` is the raw [b, 3*kt*dg, ho, wo] output of conv_offset_mask; mask = its last third
-    s.off_bs = s.mask_bs = (long long)s.dg * 3 * s.kh * s.kw * s.Ho * s.Wo;
-    s.mask_logit = 1;
-    mask = offset + (long long)s.dg * 2 * s.kh * s.kw * s.Ho * s.Wo;
+size_t dcn_om_tiles_bytes(int cin) { return (size_t)(cin / TC_CB) * OM_W_BYTES; }
+
+// The operands of the block variant (OM); the plain bf16 forward passes none
+struct OmArgs {
+  CUtensorMap xmap;
+  const __nv_bfloat16 *womt;
+  const float *bom;
+};
+
+template <int CO_T, typename TOut, bool OM>
+static int launch_fwd_bf16(const __nv_bfloat16 *xt, const float *offset, const float *mask, const void *wtiles,
+                           const float *bias, void *output, float *part, const DcnShapeTc &s, const OmArgs &om,
+                           cudaStream_t stream) {
+  constexpr int STAGES = BF_STAGES;
+  const size_t smem = (size_t)STAGES * (BF_A_BYTES + CO_T * TC_K * 2) + sizeof(TapMetaTc) * TC_NT * TC_TP +
+                      (OM ? OM_SMEM_BYTES : 0);
+  static thread_local int dev_done = -1;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev_done != dev) {
+    CNB_CUDA(cudaFuncSetAttribute(k_dcn_forward_bf16<CO_T, STAGES, TOut, OM>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dev_done = dev;
   }
-  s.epi_scale = epi_scale;
-  s.epi_shift = epi_scale ? epi_shift : nullptr;
-  s.relu = relu;
+  const int grid = s.n_items < num_sms() ? s.n_items : num_sms();
+  k_dcn_forward_bf16<CO_T, STAGES, TOut, OM><<<grid, TC_THREADS, smem, stream>>>(
+      xt, offset, mask, reinterpret_cast<const __nv_bfloat16 *>(wtiles), bias, reinterpret_cast<TOut *>(output), part,
+      s, om.xmap, om.womt, om.bom);
+  CNB_CHECK_LAUNCH(OM ? "cnb_dcnv2_forward_block_bf16 (wgmma)" : "cnb_dcnv2_forward_bf16 (wgmma)");
+  count_launch();
+  return CNB_OK;
+}
+
+// The bf16 channels-last source [B][HW][nb][32] the kernel samples: a bf16 channels-last input in place, else a copy
+// into the workspace (p.bf16.xt)
+static int bf16_source(const DcnPlan &p, const DcnShapeTc &s, const void *input, bool in_bf16, void *workspace,
+                       cudaStream_t stream, const __nv_bfloat16 **xsrc) {
   __nv_bfloat16 *xt = reinterpret_cast<__nv_bfloat16 *>(reinterpret_cast<char *>(workspace) + p.bf16.xt);
-  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
   const long long HW = (long long)s.H * s.W;
-  const __nv_bfloat16 *xsrc = xt;
+  *xsrc = xt;
   if (p.x_cl && in_bf16) {
-    xsrc = reinterpret_cast<const __nv_bfloat16 *>(input);   // sampled in place
+    *xsrc = reinterpret_cast<const __nv_bfloat16 *>(input);   // sampled in place
   } else if (p.x_cl) {
     const long long n8 = (long long)s.B * HW * s.Cin / 8;
     const int grid = (int)((n8 + 255) / 256 < 4096 ? (n8 + 255) / 256 : 4096);
@@ -710,13 +860,21 @@ int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const fl
     CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 channels-last copy");
     count_launch();
   }
+  return CNB_OK;
+}
+
+// The kernel for the Cout tile and output dtype, then the split-K reduce on small maps
+template <bool OM>
+static int run_fwd_bf16(const __nv_bfloat16 *xsrc, const float *offset, const float *mask, const void *wtiles,
+                        const float *bias, void *output, bool out_bf16, float *part, const DcnShapeTc &s,
+                        const OmArgs &om, cudaStream_t stream) {
   int rc;
   if (s.co_t == 64)
-    rc = out_bf16 ? launch_fwd_bf16<64, __nv_bfloat16>(xsrc, offset, mask, wtiles, bias, output, part, s, stream)
-                  : launch_fwd_bf16<64, float>(xsrc, offset, mask, wtiles, bias, output, part, s, stream);
+    rc = out_bf16 ? launch_fwd_bf16<64, __nv_bfloat16, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream)
+                  : launch_fwd_bf16<64, float, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream);
   else
-    rc = out_bf16 ? launch_fwd_bf16<128, __nv_bfloat16>(xsrc, offset, mask, wtiles, bias, output, part, s, stream)
-                  : launch_fwd_bf16<128, float>(xsrc, offset, mask, wtiles, bias, output, part, s, stream);
+    rc = out_bf16 ? launch_fwd_bf16<128, __nv_bfloat16, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream)
+                  : launch_fwd_bf16<128, float, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream);
   if (rc != CNB_OK) return rc;
   if (s.splits > 1) {
     const long long total = (long long)s.B * s.Cout * s.Ho * s.Wo;
@@ -732,6 +890,50 @@ int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const fl
     count_launch();
   }
   return CNB_OK;
+}
+
+int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
+                     const void *wtiles, const float *bias, void *output, bool out_bf16, void *workspace,
+                     cudaStream_t stream, int fused_offset_mask, const float *epi_scale, const float *epi_shift,
+                     int relu) {
+  DcnShapeTc s = p.s;
+  if (fused_offset_mask) {   // `offset` is the raw [b, 3*kt*dg, ho, wo] output of conv_offset_mask; mask = its last third
+    s.off_bs = s.mask_bs = (long long)s.dg * 3 * s.kh * s.kw * s.Ho * s.Wo;
+    s.mask_logit = 1;
+    mask = offset + (long long)s.dg * 2 * s.kh * s.kw * s.Ho * s.Wo;
+  }
+  s.epi_scale = epi_scale;
+  s.epi_shift = epi_scale ? epi_shift : nullptr;
+  s.relu = relu;
+  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
+  const __nv_bfloat16 *xsrc;
+  const int rc = bf16_source(p, s, input, in_bf16, workspace, stream, &xsrc);
+  if (rc != CNB_OK) return rc;
+  OmArgs none;
+  memset(&none, 0, sizeof(none));
+  return run_fwd_bf16<false>(xsrc, offset, mask, wtiles, bias, output, out_bf16, part, s, none, stream);
+}
+
+int dcn_forward_block_bf16(const DcnPlan &p, const void *input, bool in_bf16, const void *om_tiles,
+                           const float *om_bias, const void *wtiles, const float *bias, void *output,
+                           void *workspace, cudaStream_t stream, const float *epi_scale, const float *epi_shift,
+                           int relu) {
+  DcnShapeTc s = p.s;
+  s.mask_logit = 1;   // the last 9 of the 27 offset-conv channels are mask logits
+  s.epi_scale = epi_scale;
+  s.epi_shift = epi_scale ? epi_shift : nullptr;
+  s.relu = relu;
+  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
+  const __nv_bfloat16 *xsrc;
+  int rc = bf16_source(p, s, input, in_bf16, workspace, stream, &xsrc);
+  if (rc != CNB_OK) return rc;
+  OmArgs om;
+  const CUresult cr = encode_halo_map(&om.xmap, xsrc, s.B, s.Cin, s.H, s.W, s.tw + 2, s.th + 2);
+  CNB_REQUIRE(cr == CUDA_SUCCESS, CNB_ECUDA, "cnb_dcnv2_forward_block_bf16: cuTensorMapEncodeTiled failed (%d)",
+              (int)cr);
+  om.womt = reinterpret_cast<const __nv_bfloat16 *>(om_tiles);
+  om.bom = om_bias;
+  return run_fwd_bf16<true>(xsrc, nullptr, nullptr, wtiles, bias, output, in_bf16, part, s, om, stream);
 }
 
 // Workspace of the prepared forward: channels-last copy of the input (+ split-K partial sums); the plain forward puts

@@ -263,6 +263,15 @@ int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const fl
                      const void *wtiles, const float *bias, void *output, bool out_bf16, void *workspace,
                      cudaStream_t stream, int fused_offset_mask, const float *epi_scale, const float *epi_shift,
                      int relu);
+// DCN block (dcnv2_tc.cu): the 3x3 conv_offset_mask inside the bf16 forward.  Offset-conv weight tiles of a
+// [27][cin][3][3] W_om (dcn_om_tiles_bytes), then the forward into the workspace of p.bf16 with the input's dtype out;
+// the caller has checked the range (3x3, stride 1, pad 1, dilation 1, dg 1, cin % 32 == 0)
+size_t dcn_om_tiles_bytes(int cin);
+int dcn_prepare_om_weights_bf16(const float *w_om, int cin, void *om_tiles, cudaStream_t stream);
+int dcn_forward_block_bf16(const DcnPlan &p, const void *input, bool in_bf16, const void *om_tiles,
+                           const float *om_bias, const void *wtiles, const float *bias, void *output,
+                           void *workspace, cudaStream_t stream, const float *epi_scale, const float *epi_shift,
+                           int relu);
 // Tensor-core backward (dcnv2_bwd_tc.cu) into the workspace of p.bwd: dX, dOffset, dMask; then dW and dBias
 int dcn_backward_data_tc(const DcnPlan &p, const float *input, const float *offset, const float *mask,
                          const float *weight, const float *grad_output, float *grad_input, float *grad_offset,

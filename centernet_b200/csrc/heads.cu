@@ -22,11 +22,9 @@
 // Cmid is padded to CMID in {64, 128, 256} and C to N2 in {8, ..., 256}: padded weight rows are zero and the padded
 // intermediate channels are forced to zero, so they add exact zeros (no Inf * 0) and are never stored.
 // Every sum is in a fixed order and there are no atomics: the output is bit-identical run to run.
-#include <cuda.h>
-#include <cudaTypedefs.h>
 #include <cuda_bf16.h>
 
-#include "dcnv2_tc.cuh"
+#include "halo.cuh"
 
 namespace cnb {
 namespace {
@@ -55,83 +53,6 @@ inline int head_n2_pad(int cout) {
   int n = 8;
   while (n < cout) n *= 2;
   return n;
-}
-
-__device__ __forceinline__ void wgmma_bf16_n8(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3}"
-      ", %4, %5, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-__device__ __forceinline__ void wgmma_bf16_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7}"
-      ", %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}"
-      ", %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-__device__ __forceinline__ void wgmma_bf16_n256(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,"
-      "%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
-      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,"
-      "%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
-      "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,"
-      "%120,%121,%122,%123,%124,%125,%126,%127}"
-      ", %128, %129, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-
-template <int N>
-__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
-  if constexpr (N == 8) wgmma_bf16_n8(d, da, db, scale_d);
-  else if constexpr (N == 16) wgmma_bf16_n16(d, da, db, scale_d);
-  else if constexpr (N == 32) wgmma_bf16_n32(d, da, db, scale_d);
-  else if constexpr (N == 64) wgmma_bf16_n64(d, da, db, scale_d);
-  else if constexpr (N == 128) wgmma_bf16_n128(d, da, db, scale_d);
-  else wgmma_bf16_n256(d, da, db, scale_d);
-}
-
-__device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, int c0, int c1, int c2, int c3,
-                                            uint64_t *bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
-      "r"(smem_u32(bar))
-      : "memory");
 }
 
 __device__ __forceinline__ uint32_t pack2_bf16(float lo, float hi) {   // lo -> lower address
@@ -388,20 +309,6 @@ int launch_head_n2(const CUtensorMap &map, const void *w1t, const float *b1, con
   }
 }
 
-PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = [] {
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess) {
-      (void)cudaGetLastError();
-      p = nullptr;
-    }
-    return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
-  }();
-  return fn;
-}
-
 // The checks every entry shares: CNB_EINVAL for a bad shape, CNB_EUNSUPPORTED outside the kernel's range
 int head_check(const char *fn, int b, int cin, int h, int w, int cmid, int cout) {
   CNB_REQUIRE(b > 0 && cin > 0 && h > 0 && w > 0 && cmid > 0 && cout > 0, CNB_EINVAL, "%s: bad shape", fn);
@@ -473,8 +380,7 @@ int cnb_head_forward_bf16(const void *input, int input_dtype, int input_channels
   CNB_REQUIRE(((reinterpret_cast<uintptr_t>(input) | reinterpret_cast<uintptr_t>(w1t) |
                 reinterpret_cast<uintptr_t>(w2t) | reinterpret_cast<uintptr_t>(ws)) & 15u) == 0,
               CNB_EINVAL, "%s: input, tile buffers and workspace must be 16-byte aligned", fn);
-  PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
-  CNB_REQUIRE(encode != nullptr, CNB_ECUDA, "%s: the driver has no cuTensorMapEncodeTiled", fn);
+  CNB_REQUIRE(tensor_map_encoder() != nullptr, CNB_ECUDA, "%s: the driver has no cuTensorMapEncodeTiled", fn);
 
   cudaStream_t st = (cudaStream_t)stream;
   const long long HW = (long long)h * w;
@@ -499,13 +405,7 @@ int cnb_head_forward_bf16(const void *input, int input_dtype, int input_channels
   }
 
   CUtensorMap map;
-  cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)b};
-  cuuint64_t strides[3] = {(cuuint64_t)cin * 2, (cuuint64_t)w * cin * 2, (cuuint64_t)HW * cin * 2};
-  cuuint32_t box[4] = {8, HD_HX, HD_HY, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  const CUresult cr = encode(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(xt), dims, strides, box,
-                             estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult cr = encode_halo_map(&map, xt, b, cin, h, w, HD_HX, HD_HY);
   CNB_REQUIRE(cr == CUDA_SUCCESS, CNB_ECUDA, "%s: cuTensorMapEncodeTiled failed (%d)", fn, (int)cr);
 
   HeadShape s;

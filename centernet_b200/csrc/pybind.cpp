@@ -135,6 +135,10 @@ PYBIND11_MODULE(_C, m) {
   VALUE(dcnv2_bf16_workspace_bytes);
   STATUS(dcnv2_forward_bf16);
   STATUS(dcnv2_forward_fused_bf16);
+  VALUE(dcnv2_om_tiles_bytes);
+  STATUS(dcnv2_prepare_om_weights_bf16);
+  VALUE(dcnv2_block_workspace_bytes);
+  STATUS(dcnv2_forward_block_bf16);
   VALUE(dcnv2_backward_workspace_bytes);
   STATUS(dcnv2_backward_ex);
   VALUE(dcnv2_set_deterministic);

@@ -8,7 +8,7 @@ from torch import nn
 from torch.nn.modules.utils import _pair
 
 from .dcn_v2_func import (DCNv2Function, DCNv2PoolingFunction, _check_backward_dtype, _check_compute_dtype,
-                          dcn_fused_inference)
+                          dcn_block_inference, dcn_fused_inference)
 
 
 class DCNv2(nn.Module):
@@ -63,6 +63,9 @@ class DCN(DCNv2):
         self.conv_offset_mask.bias.data.zero_()
 
     def forward(self, input):
+        y = _block_forward(self, input)
+        if y is not None:
+            return y
         out = self.conv_offset_mask(input)
         # inference in fp32 uses the fused kernel; float64 (no fused form) takes the path below
         if input.is_cuda and not torch.is_grad_enabled() and self.kernel_size[0] * self.kernel_size[1] <= 9 and \
@@ -133,6 +136,32 @@ class DCNPooling(DCNv2Pooling):
         return self.func(data, rois, offset) * mask
 
 
+def _block_forward(dcn, x, bn_scale=None, bn_shift=None, relu=False):
+    """The DCN block kernel for a module flagged by fuse_offset_conv, or None where the module runs its usual path:
+    not flagged, compute_dtype not bf16, training, grad mode, autocast, not a CUDA float32 / bfloat16 input, or outside
+    the kernel's range (dcn_block_inference)."""
+    if not getattr(dcn, "offset_conv_fused", False) or getattr(dcn, "compute_dtype", None) != torch.bfloat16 or \
+            dcn.training or torch.is_grad_enabled() or not x.is_cuda or torch.is_autocast_enabled("cuda"):
+        return None
+    om = dcn.conv_offset_mask
+    return dcn_block_inference(x, om.weight, om.bias, dcn.weight, dcn.bias, dcn.stride, dcn.padding, dcn.dilation,
+                               dcn.deformable_groups, bn_scale, bn_shift, relu)
+
+
+def fuse_offset_conv(model):
+    """Flags every DCN of `model` to run its conv_offset_mask inside the bf16 DCN kernel (cnb_dcnv2_forward_block_bf16)
+    and returns how many it flagged.  A flagged DCN whose compute_dtype is torch.bfloat16 takes the block kernel in
+    eval mode under no_grad on CUDA, inside the kernel's range, in DCN.forward and in the forward fuse_dcn_bn_relu
+    installs; everything else runs as before.  The flag is read at call time, so this composes with set_compute_dtype
+    and fuse_dcn_bn_relu in any order; it is a plain attribute, so state-dict keys do not change."""
+    n = 0
+    for m in model.modules():
+        if isinstance(m, DCN):
+            m.offset_conv_fused = True
+            n += 1
+    return n
+
+
 # ------------------------------------------------------------------ N3: DCN + BatchNorm + ReLU (pose_dla_dcn.py:345-357)
 def fold_bn(bn):
     """Inference BatchNorm as y = scale * x + shift (float64 fold, fp32 result)."""
@@ -161,6 +190,9 @@ def fuse_dcn_bn_relu(model):
                     x.dtype == torch.float64:
                 return _orig(x)
             scale, shift = fold_bn(bn)
+            y = _block_forward(c, x, scale, shift, True)
+            if y is not None:
+                return y
             om = c.conv_offset_mask(x)
             return dcn_fused_inference(x, om, c.weight, c.bias, c.stride, c.padding, c.dilation, c.deformable_groups,
                                        bn_scale=scale, bn_shift=shift, relu=True,

@@ -386,6 +386,61 @@ def dcn_fused_inference(input, offset_mask, weight, bias, stride, padding, dilat
     return out
 
 
+# ------------------------------------------------------------------ DCN block (opt-in: dcn_v2.fuse_offset_conv)
+def _om_tiles(w_om):
+    """bf16 tiles of a conv_offset_mask weight (cnb_dcnv2_prepare_om_weights_bf16), cached per weight version next to
+    the tiles of _weight_tiles: rebuilt when torch bumps `_version` (optimizer step, load_state_dict), tied to the
+    tensor object by a weak reference."""
+    key = (id(w_om), "om")
+    hit = _WT_CACHE.get(key)
+    if hit is not None and hit[0]() is w_om and hit[1] == w_om._version and hit[2].device == w_om.device:
+        return hit[2]
+    ver = w_om._version
+    w = f32c(w_om)
+    cin = int(w.shape[1])
+    t = workspace(C.dcnv2_om_tiles_bytes(cin, 3, 3, 1), w.device)
+    C.dcnv2_prepare_om_weights_bf16(ptr(w), cin, 3, 3, 1, ptr(t), t.numel(), stream_ptr(w))
+    try:
+        _WT_CACHE[key] = (weakref.ref(w_om, lambda _r, k=key: _WT_CACHE.pop(k, None)), ver, t)
+    except TypeError:          # not weak-referenceable: do not cache
+        pass
+    return t
+
+
+def dcn_block_inference(input, w_om, b_om, weight, bias, stride, padding, dilation, deformable_groups,
+                        bn_scale=None, bn_shift=None, relu=False):
+    """Inference form of a whole DCN module in ONE kernel (cnb_dcnv2_forward_block_bf16): conv_offset_mask (w_om,
+    b_om), the chunk / cat / sigmoid and the bf16 deformable conv, plus the optional folded BatchNorm + ReLU.  The
+    offsets are computed in fp32 from bf16 operands and never leave the chip; from them on the result is
+    dcn_fused_inference(..., compute_dtype=torch.bfloat16) fed those offsets.  Output in the input's dtype.  Returns
+    None where the kernel does not run (not a CUDA float32 / bfloat16 input, outside its range -- 3x3, stride 1,
+    padding 1, dilation 1, one deformable group, input channels a multiple of 32); the caller then runs
+    conv_offset_mask and dcn_fused_inference.  No autograd."""
+    if not input.is_cuda or input.dtype not in (torch.float32, torch.bfloat16) or input.dim() != 4:
+        return None
+    n, cin, h, wd = [int(v) for v in input.shape]
+    cout, cin_w, kh, kw = [int(v) for v in weight.shape]
+    if cin_w != cin or tuple(w_om.shape) != (3 * kh * kw * deformable_groups, cin, kh, kw):
+        return None
+    wsb = C.dcnv2_block_workspace_bytes(n, cin, cout, h, wd, kh, kw, stride, padding, dilation, deformable_groups)
+    if wsb == 0:
+        return None
+    cl = input.is_contiguous(memory_format=torch.channels_last) and not input.is_contiguous()
+    x = input if cl else input.contiguous()
+    if x.data_ptr() % 16:
+        x = x.clone()               # the kernel reads 16-byte pieces (clone keeps the memory format)
+    dt = C.DTYPE_BF16 if x.dtype == torch.bfloat16 else C.DTYPE_F32
+    wt = _weight_tiles(weight, deformable_groups, bf16=True)
+    omt = _om_tiles(w_om)
+    out = torch.empty((n, cout, h, wd), dtype=input.dtype, device=input.device)
+    ws = workspace(wsb, input.device)
+    bom, b, sc, sh = f32c(b_om), f32c(bias), f32c(bn_scale), f32c(bn_shift)
+    C.dcnv2_forward_block_bf16(ptr(x), dt, int(cl), ptr(omt), ptr(bom), ptr(wt), ptr(b), ptr(sc), ptr(sh),
+                               int(bool(relu)), ptr(out), n, cin, h, wd, cout, kh, kw, stride, padding, dilation,
+                               deformable_groups, ptr(ws), ws.numel(), stream_ptr(x))
+    return out
+
+
 class DCNv2Function(object):
     """Callable instance, same constructor as the reference's old-style Function.  compute_dtype=torch.bfloat16
     selects the bf16 forward (float32 or bfloat16 input, output in the input's dtype); None keeps the default.

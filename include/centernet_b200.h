@@ -44,7 +44,8 @@ extern "C" {
 
 /* Element type codes of the entry points that take more than one (cnb_dcnv2_forward_bf16, cnb_ctdet_decode_ex,
  * cnb_flip_merge_ex, cnb_ddd_decode_ex, cnb_multi_pose_decode_ex, cnb_edge_aggregate_ex, cnb_exct_decode_ex,
- * cnb_gather_feat_ex, the loss calls cnb_focal_*_ex / cnb_reg_loss_*ex and cnb_head_forward_bf16). */
+ * cnb_gather_feat_ex, the loss calls cnb_focal_*_ex / cnb_reg_loss_*ex, cnb_head_forward_bf16 and
+ * cnb_dcnv2_forward_block_bf16). */
 #define CNB_DTYPE_F32 0
 #define CNB_DTYPE_BF16 1
 #define CNB_DTYPE_F16 2
@@ -471,6 +472,39 @@ int cnb_dcnv2_forward_fused_bf16(const void *input, int input_dtype, int input_c
                                  const float *offset_mask, const void *wtiles, const float *bias,
                                  const float *bn_scale, const float *bn_shift, int relu,
                                  void *output, int output_dtype,
+                                 int b, int cin, int h, int w, int cout, int kh, int kw,
+                                 int stride, int pad, int dil, int deformable_groups,
+                                 void *workspace, size_t workspace_bytes, void *stream);
+/* DCN block, bf16 inference (opt-in): the whole DCN module -- its 3x3 conv_offset_mask, the chunk / cat / sigmoid of
+ * dcn_v2.py and the deformable conv -- plus the optional folded BatchNorm + ReLU of DeformConv, in ONE kernel.  The
+ * 27 offset / mask values of every pixel are computed on the bf16 tensor cores inside the kernel and never reach
+ * global memory.  Numeric contract:
+ *   - x and w_om are rounded once to bf16 (RN); om = the exact-product, fp32-accumulated 3x3 conv (zero padding 1)
+ *     of them plus om_bias in fp32, kept in fp32 (never rounded to bf16);
+ *   - from om on, the result is exactly cnb_dcnv2_forward_fused_bf16 fed that fp32 om as offset_mask: sigmoid,
+ *     geometry, bf16 column rounding, bf16 contraction with fp32 accumulate, fp32 epilogue, output rounded to the
+ *     input's dtype;
+ *   - only the order of the fp32 sums of the two contractions is free; it is fixed (no atomics), so the output is
+ *     bit-identical run to run.
+ * Range: kh = kw = 3, stride 1, pad 1, dilation 1, deformable_groups 1, cin % 32 == 0, any cout, b, h, w that
+ * cnb_dcnv2_forward_bf16 takes.  Outside it every call returns CNB_EUNSUPPORTED and the two size queries return 0;
+ * the caller then runs conv_offset_mask itself and cnb_dcnv2_forward_fused_bf16.
+ * w_om: [27][cin][3][3] fp32, rounded and tiled once by cnb_dcnv2_prepare_om_weights_bf16 into om_tiles
+ * (cnb_dcnv2_om_tiles_bytes, 16-byte aligned), reused while the weight does not change.  om_bias [27] fp32 (NULL: no
+ * bias).  wtiles / bias / bn_scale / bn_shift / relu as cnb_dcnv2_forward_fused_bf16.  input: [b,cin,h,w] of
+ * input_dtype (CNB_DTYPE_F32 or CNB_DTYPE_BF16), [b][h*w][cin] when input_channels_last != 0 (a bf16 one is read in
+ * place); 16-byte aligned.  output: [b,cout,h,w] NCHW of input_dtype.  workspace: cnb_dcnv2_block_workspace_bytes
+ * (16-byte aligned).  Errors, checked before any CUDA call: CNB_EINVAL for a null pointer, an unknown dtype code, a
+ * bad shape or a misaligned buffer; CNB_EUNSUPPORTED outside the range; CNB_EWORKSPACE for too small a buffer. */
+size_t cnb_dcnv2_om_tiles_bytes(int cin, int kh, int kw, int dg);
+int cnb_dcnv2_prepare_om_weights_bf16(const float *w_om, int cin, int kh, int kw, int dg,
+                                      void *om_tiles, size_t om_tiles_bytes, void *stream);
+size_t cnb_dcnv2_block_workspace_bytes(int b, int cin, int cout, int h, int w, int kh, int kw,
+                                       int stride, int pad, int dil, int dg);
+int cnb_dcnv2_forward_block_bf16(const void *input, int input_dtype, int input_channels_last,
+                                 const void *om_tiles, const float *om_bias,
+                                 const void *wtiles, const float *bias,
+                                 const float *bn_scale, const float *bn_shift, int relu, void *output,
                                  int b, int cin, int h, int w, int cout, int kh, int kw,
                                  int stride, int pad, int dil, int deformable_groups,
                                  void *workspace, size_t workspace_bytes, void *stream);
