@@ -13,4 +13,4 @@ calling with non-CUDA tensors, raises.
 """
 from ._lib import C as _C, version  # noqa: F401  (fails loudly if the extension is missing)
 
-__all__ = ["decode", "utils", "losses", "dcn_v2", "dcn_v2_func", "heads", "version"]
+__all__ = ["decode", "utils", "losses", "dcn_v2", "dcn_v2_func", "heads", "ida", "version"]

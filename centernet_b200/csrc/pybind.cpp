@@ -153,6 +153,8 @@ PYBIND11_MODULE(_C, m) {
   VALUE(head_workspace_bytes);
   STATUS(head_forward_bf16);
 
+  STATUS(ida_up_add);
+
   VALUE(dcnv2_f64_workspace_bytes);
   STATUS(dcnv2_forward_f64);
   STATUS(dcnv2_backward_f64);

@@ -606,6 +606,30 @@ int cnb_head_forward_bf16(const void *input, int input_dtype, int input_channels
                           int b, int cin, int h, int w, int cmid, int cout,
                           void *ws, size_t ws_bytes, void *stream);
 
+/* ------------------------------------- IDA up-sampling step of DLASeg: depthwise transposed conv + skip add (inference)
+ * Every step of pose_dla_dcn's IDAUp is node(up(proj(x)) + skip), with up = ConvTranspose2d(C, C, 2f, stride f,
+ * padding f/2, groups C, no bias).  cnb_ida_up_add computes
+ *   out = conv_transpose2d(p, w, stride=f, padding=f/2, groups=c) + skip
+ * in one pass; the up-sampled map never reaches HBM.  Numeric contract:
+ *   1. p and w are widened exactly to fp32;
+ *   2. the up value of an output element is an fp32 FMA chain over its valid taps (at most 2 x 2), starting from 0,
+ *      in the fixed order (row q-1, column q-1), (q-1, q), (q, q-1), (q, q), q = (y + f/2) / f per axis;
+ *   3. skip, widened exactly, is added to it in fp32;
+ *   4. the sum is rounded once (RN) to the output dtype.
+ * Out-of-range taps are not computed (never multiplied by anything); Inf / NaN propagate through valid taps as in
+ * IEEE arithmetic.  The unfused bf16 module rounds twice (after the up and after the add) and cuDNN runs an fp32
+ * conv in TF32 by default, so the two differ slightly; this result is the more accurate one.  There are no atomics
+ * and no workspace: the output is bit-identical run to run.
+ * p: [b,c,hp,wp] and skip: [b,c,f*hp,f*wp], both of dtype (CNB_DTYPE_F32 or CNB_DTYPE_BF16), each NCHW or, when its
+ * *_channels_last is 1, [b][h][w][c] (torch channels_last).  w: [c][2f][2f] fp32.  out: [b,c,f*hp,f*wp] of dtype, in
+ * the layout out_channels_last picks; it must not overlap p or skip.  skip and out 16-byte aligned.
+ * Range: f in {2, 4, 8}, any c >= 1 and b, hp, wp >= 1 within 32-bit indexing; else CNB_EUNSUPPORTED.  Errors,
+ * checked before any CUDA call: CNB_EINVAL for a null or misaligned pointer, an unknown dtype code, a channels_last
+ * flag other than 0 / 1 or a bad shape. */
+int cnb_ida_up_add(const void *p, int dtype, int p_channels_last, const float *w, int f, const void *skip,
+                   int skip_channels_last, void *out, int out_channels_last, int b, int c, int hp, int wp,
+                   void *stream);
+
 /* ------------------------------------------------- A10/A11: DCNv2, float64
  * The reference's second build, _ext.dcn_v2_double (dcn_v2_cuda_double.c, dcn_v2_im2col_cuda_double.cu): the
  * same layouts and arguments as the fp32 calls above with double tensors, any kernel size, stride, padding,
