@@ -520,7 +520,6 @@ static int dcn_plan(const char *fn, int b, int cin, int h, int w, int cout, int 
   p->fp32_dw_splits = fp32_weight_splits(b, cin, cout, dg, ((long long)ho * wo + DCN_TP - 1) / DCN_TP);
   plan_forward_tc(p);
   plan_backward_tc(p);
-  plan_backward_bf16(p);
   return CNB_OK;
 }
 
@@ -750,7 +749,7 @@ size_t cnb_dcnv2_bf16_workspace_bytes(int b, int cin, int cout, int h, int w, in
   if (dcn_plan("cnb_dcnv2_bf16_workspace_bytes", b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg,
                false, false, false, &p) != CNB_OK)
     return 0;
-  return p.bf16.bytes;
+  return p.bf16.prepared_bytes;
 }
 
 // The checks of both bf16 entry points, in order: pointers, dtype codes, shape (dcn_plan), workspace, alignment.
@@ -768,8 +767,8 @@ static int dcn_bf16_call(const char *fn, const void *input, int input_dtype, int
   int rc = dcn_plan(fn, b, cin, h, w, cout, kh, kw, stride, stride, pad, pad, dil, dil, dg, false,
                     input_channels_last != 0, false, &p);
   if (rc != CNB_OK) return rc;
-  CNB_REQUIRE(workspace_bytes >= p.bf16.bytes, CNB_EWORKSPACE, "%s: workspace too small (%zu < %zu)", fn,
-              workspace_bytes, p.bf16.bytes);
+  CNB_REQUIRE(workspace_bytes >= p.bf16.prepared_bytes, CNB_EWORKSPACE, "%s: workspace too small (%zu < %zu)", fn,
+              workspace_bytes, p.bf16.prepared_bytes);
   CNB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 15u) == 0 && (reinterpret_cast<uintptr_t>(wtiles) & 15u) == 0 &&
                   (reinterpret_cast<uintptr_t>(input) & 15u) == 0,
               CNB_EINVAL, "%s: buffers must be 16-byte aligned", fn);
@@ -835,7 +834,7 @@ size_t cnb_dcnv2_block_workspace_bytes(int b, int cin, int cout, int h, int w, i
           CNB_OK ||
       dcn_block_range(fn, cin, kh, kw, stride, pad, dil, dg) != CNB_OK)
     return 0;
-  return p.bf16.bytes;
+  return p.bf16.prepared_bytes;
 }
 
 int cnb_dcnv2_forward_block_bf16(const void *input, int input_dtype, int input_channels_last, const void *om_tiles,
@@ -854,8 +853,8 @@ int cnb_dcnv2_forward_block_bf16(const void *input, int input_dtype, int input_c
   if (rc != CNB_OK) return rc;
   rc = dcn_block_range(fn, cin, kh, kw, stride, pad, dil, deformable_groups);
   if (rc != CNB_OK) return rc;
-  CNB_REQUIRE(workspace_bytes >= p.bf16.bytes, CNB_EWORKSPACE, "%s: workspace too small (%zu < %zu)", fn,
-              workspace_bytes, p.bf16.bytes);
+  CNB_REQUIRE(workspace_bytes >= p.bf16.prepared_bytes, CNB_EWORKSPACE, "%s: workspace too small (%zu < %zu)", fn,
+              workspace_bytes, p.bf16.prepared_bytes);
   CNB_REQUIRE(((reinterpret_cast<uintptr_t>(workspace) | reinterpret_cast<uintptr_t>(wtiles) |
                 reinterpret_cast<uintptr_t>(om_tiles) | reinterpret_cast<uintptr_t>(input)) & 15u) == 0,
               CNB_EINVAL, "%s: buffers must be 16-byte aligned", fn);

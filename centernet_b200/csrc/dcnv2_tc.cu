@@ -32,43 +32,55 @@
 // cnb_dcnv2_forward, or once per weight version through cnb_dcnv2_prepare_weights +
 // cnb_dcnv2_forward_prepared (what the Python module does).
 //
-// k_dcn_forward_bf16 (further down) is the opt-in bf16 form of the forward: bf16 tiles, wgmma k16 bf16 -> fp32.
-// Its OM variant (the DCN block) also computes the 3x3 conv_offset_mask inside the kernel.
+// k_dcn_forward is templated on the operand format (Tf32x3 / Bf16, dcnv2_tc.cuh).  Its Bf16 form is the opt-in bf16
+// forward: one bf16 tile per operand, wgmma k16 bf16 -> fp32, samplers with 8-channel lanes.  Its OM variant (the DCN
+// block, bf16 only) also computes the 3x3 conv_offset_mask inside the kernel.
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "halo.cuh"
 
 namespace cnb {
 
-// W[Cout][Cin][KT] -> per (cout tile, channel block bi, tap): hi tile then lo tile, each [co_t][32] in the K-major
-// layout; k = channel within the block.  Tile index = (cot * nb + bi) * 9 + tap.
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {   // lo -> lower address (smaller k)
+  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t *>(&v);
+}
+__device__ __forceinline__ void store_out(float *p, float v) { *p = v; }
+__device__ __forceinline__ void store_out(__nv_bfloat16 *p, float v) { *p = __float2bfloat16_rn(v); }
+__device__ __forceinline__ float load_in(const float *p) { return __ldg(p); }
+__device__ __forceinline__ float load_in(const __nv_bfloat16 *p) { return __bfloat162float(p[0]); }
+
+// W[Cout][Cin][KT] (fp32) -> per (cout tile, channel block bi, tap) one operand tile [co_t][32] (k = channel within
+// the block; TF32: hi tile then lo tile).  Tile index = (cot * nb + bi) * 9 + tap.
+template <typename F>
 __global__ void __launch_bounds__(256) k_dcn_prep_weights(const float *__restrict__ w, const DcnShapeTc s,
-                                                          float *__restrict__ ws) {
+                                                          unsigned char *__restrict__ ws) {
   const int KT = s.kh * s.kw;
   const int cpg = s.Cin / s.dg;
   const int tile = blockIdx.x;
   const int tap = tile % TC_NT, r = tile / TC_NT;
   const int bi = r % s.nb, cot = r / s.nb;
   const int g = bi / s.cbs_pg, cbi = bi - g * s.cbs_pg;
-  const size_t tile_floats = (size_t)s.co_t * TC_K;
-  unsigned char *hi = reinterpret_cast<unsigned char *>(ws + (size_t)tile * 2 * tile_floats);
-  unsigned char *lo = hi + tile_floats * 4;
+  const size_t tile_elems = (size_t)s.co_t * TC_K;
+  unsigned char *dst = ws + (size_t)tile * tile_elems * F::ELEM;
   for (int i = threadIdx.x; i < s.co_t * TC_K; i += blockDim.x) {
     const int o = i / TC_K, k = i - o * TC_K;
     const int cw = cbi * TC_CB + k;                    // channel within the group
     float v = 0.f;
     const int oc = cot * s.co_t + o;
     if (oc < s.Cout && cw < cpg && tap < KT) v = w[((size_t)oc * s.Cin + g * cpg + cw) * KT + tap];
-    const float h = tf32_hi(v);
-    *reinterpret_cast<float *>(hi + tc_tile_off(o, k)) = h;
-    *reinterpret_cast<float *>(lo + tc_tile_off(o, k)) = v - h;
+    F::put(dst, tile_elems * 4, o, k, v);
   }
 }
 
-// x [B][Cin][HW] -> xt [B][HW][nb][32]; channel ch of group g sits in block g*cbs_pg + (ch - g*cpg)/32,
-// slot (ch - g*cpg) % 32 (identity when Cin/dg is a multiple of 32; pad slots are zero-filled by the caller).
-// grid (pixel blocks of 32, channel blocks of 64, B), 256 threads.
-__global__ void __launch_bounds__(256) k_dcn_nhwc(const float *__restrict__ x, float *__restrict__ xt,
+// x [B][Cin][HW] -> xt [B][HW][nb][32] (fp32 or bf16 either side; bf16 out is rounded RN, bf16 in widens exactly);
+// channel ch of group g sits in block g*cbs_pg + (ch - g*cpg)/32, slot (ch - g*cpg) % 32 (identity when Cin/dg is a
+// multiple of 32; pad slots are zero-filled by the caller).  grid (pixel blocks of 32, channel blocks of 64, B), 256
+// threads.
+template <typename TIn, typename TOut>
+__global__ void __launch_bounds__(256) k_dcn_nhwc(const TIn *__restrict__ x, TOut *__restrict__ xt,
                                                   const DcnShapeTc s) {
   __shared__ float tile[64][33];
   const long long HW = (long long)s.H * s.W;
@@ -80,7 +92,7 @@ __global__ void __launch_bounds__(256) k_dcn_nhwc(const float *__restrict__ x, f
     const int px = threadIdx.x & 31, cr = threadIdx.x >> 5;
     for (int c = cr; c < 64; c += 8) {
       float v = 0.f;
-      if (c0 + c < s.Cin && p0 + px < HW) v = __ldg(x + ((long long)b * s.Cin + c0 + c) * HW + p0 + px);
+      if (c0 + c < s.Cin && p0 + px < HW) v = load_in(x + ((long long)b * s.Cin + c0 + c) * HW + p0 + px);
       tile[c][px] = v;
     }
   }
@@ -92,14 +104,16 @@ __global__ void __launch_bounds__(256) k_dcn_nhwc(const float *__restrict__ x, f
       const int g = ch / cpg, within = ch - g * cpg;
       const int slot = (g * s.cbs_pg + within / TC_CB) * TC_CB + within % TC_CB;
       for (int px = pr; px < 32; px += 4)
-        if (p0 + px < HW) xt[((long long)b * HW + p0 + px) * Cp + slot] = tile[c][px];
+        if (p0 + px < HW) store_out(xt + ((long long)b * HW + p0 + px) * Cp + slot, tile[c][px]);
     }
   }
 }
 
-// y[b][o][p] = bias[o] + sum_s part[s][b][o][p], s ascending (deterministic split-K epilogue)
+// y[b][o][p] = epilogue(bias[o] + sum_s part[s][b][o][p]), s ascending (deterministic split-K epilogue), stored as
+// fp32 or rounded (RN) to bf16
+template <typename TOut>
 __global__ void __launch_bounds__(256) k_dcn_reduce(const float *__restrict__ part, const float *__restrict__ bias,
-                                                    float *__restrict__ y, int splits, int cout, long long hwo,
+                                                    TOut *__restrict__ y, int splits, int cout, long long hwo,
                                                     long long total, const float *__restrict__ epi_scale,
                                                     const float *__restrict__ epi_shift, int relu) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
@@ -110,7 +124,27 @@ __global__ void __launch_bounds__(256) k_dcn_reduce(const float *__restrict__ pa
     if (bias) v += __ldg(bias + o);
     if (epi_scale) v = fmaf(v, __ldg(epi_scale + o), __ldg(epi_shift + o));
     if (relu) v = fmaxf(v, 0.f);
-    y[i] = v;
+    store_out(y + i, v);
+  }
+}
+
+// fp32 channels-last [B][HW][Cin] with whole 32-channel blocks (so slot == channel) -> bf16 xt, 8 values a thread
+__global__ void __launch_bounds__(256) k_dcn_cl_to_bf16(const float4 *__restrict__ x, uint4 *__restrict__ xt,
+                                                        long long n8) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const float4 a = __ldg(x + 2 * i), b = __ldg(x + 2 * i + 1);
+    xt[i] = make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(b.x, b.y), pack_bf16x2(b.z, b.w));
+  }
+}
+
+// bf16 channels-last [B][HW][Cin] with whole 32-channel blocks (slot == channel) -> fp32 xt, 8 values a thread
+__global__ void __launch_bounds__(256) k_dcn_cl_widen(const uint4 *__restrict__ x, float4 *__restrict__ xt, long long n8) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 u = __ldg(x + i);
+    xt[2 * i] = make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                            __uint_as_float(u.y & 0xffff0000u));
+    xt[2 * i + 1] = make_float4(__uint_as_float(u.z << 16), __uint_as_float(u.z & 0xffff0000u),
+                                __uint_as_float(u.w << 16), __uint_as_float(u.w & 0xffff0000u));
   }
 }
 
@@ -183,21 +217,52 @@ __device__ __forceinline__ void tc_build_meta(const DcnShapeTc &s, const float *
   });
 }
 
-template <int CO_T, int STAGES>
+// DCN block variant (OM = true, cnb_dcnv2_forward_block_bf16): the 3x3 conv_offset_mask runs inside the kernel.
+// For every item the TMA warp streams, per 32-channel block, the (tw + 2) x (th + 2) halo of the tile as four 8-channel
+// slabs (4-D tensor-map loads; the out-of-bounds fill is the conv's zero padding, halo.cuh) and the nine [32][32] W_om
+// tiles of the block into a ring of its own.  The consumer warpgroups compute om[128 px][27 -> 32] with wgmma m64n32k16
+// straight from the halo (shifted descriptors, no im2col), add b_om in fp32 and leave the 27 fp32 values of every pixel
+// in one of two shared buffers; the samplers build the item's tap geometry from that buffer (tc_build_meta_from, the
+// mask logit through the same sigmoid).  The consumers compute the offsets of the CTA's NEXT item before the main loop
+// of the current one, so the samplers find them ready when they reach the item boundary.  Every item computes its own
+// offsets (Cout tiles and K splits of one pixel tile recompute them).  Warpgroup wg's 64 GEMM rows are the tile's
+// column half wg (8 x 16 tiles: 8 rows of 8 pixels, one halo row apart) or row half wg (16 x 8 tiles).
+constexpr int OM_N = 32;                             // 27 offset / mask channels, padded to the wgmma N
+constexpr int OM_C = 27;                             // dg * 3 * 9 with dg = 1
+constexpr int OM_PITCH = TC_TP + 4;                  // fp32 om of one channel: 128 pixels (+4: conflict-free stores)
+constexpr uint32_t OM_SLAB = 180 * 16;               // one 8-channel slab of a 10 x 18 (or 18 x 10) halo
+constexpr uint32_t OM_SLAB_PITCH = 2944;             // slabs 128-byte aligned (TMA destination)
+constexpr uint32_t OM_HALO_BYTES = 4 * OM_SLAB_PITCH;
+constexpr uint32_t OM_W_BYTES = TC_NT * OM_N * TC_K * 2;   // the nine W_om tiles of one channel block
+constexpr uint32_t OM_STAGE_BYTES = OM_HALO_BYTES + OM_W_BYTES;
+constexpr int OM_STAGES = 2;
+constexpr uint32_t OM_BUF_BYTES = (OM_C * OM_PITCH * 4 + 127) / 128 * 128;
+constexpr uint32_t OM_SMEM_BYTES = OM_STAGES * OM_STAGE_BYTES + 2 * OM_BUF_BYTES + 128;   // + 128: alignment slack
+
+template <typename F, int CO_T, typename TOut, bool OM>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset, const float *__restrict__ mask,
-                 const float *__restrict__ wtiles, const float *__restrict__ bias, float *__restrict__ y,
-                 float *__restrict__ part, const DcnShapeTc s) {
-  extern __shared__ __align__(128) unsigned char tc_smem[];
-  constexpr int B_BYTES = CO_T * TC_K * 4;                  // one hi or lo weight tile
-  constexpr int STAGE_BYTES = 2 * FW_A_BYTES + 2 * B_BYTES;
+k_dcn_forward(const typename F::X *__restrict__ xt, const float *__restrict__ offset, const float *__restrict__ mask,
+              const unsigned char *__restrict__ wtiles, const float *__restrict__ bias, TOut *__restrict__ y,
+              float *__restrict__ part, const DcnShapeTc s, const __grid_constant__ CUtensorMap xmap,
+              const __nv_bfloat16 *__restrict__ womt, const float *__restrict__ bom) {
+  static_assert(!OM || F::KE == 8, "k_dcn_forward: the DCN block variant is bf16 only");
+  extern __shared__ __align__(128) unsigned char tc_smem_raw[];
+  // the block variant's TMA halo needs a 128-byte aligned destination
+  unsigned char *tc_smem = OM ? tc_smem_raw + ((128u - (smem_u32(tc_smem_raw) & 127u)) & 127u) : tc_smem_raw;
+  constexpr int STAGES = F::fw_stages(CO_T);
+  constexpr int B_BYTES = CO_T * TC_K * F::ELEM;          // one weight operand tile
+  constexpr int STAGE_BYTES = F::FW_A + B_BYTES;
+  static_assert(TC_SAMPLER_ROUNDS == 2, "k_dcn_forward: two row groups a sampler warp");
   TapMetaTc *meta = reinterpret_cast<TapMetaTc *>(tc_smem + (size_t)STAGES * STAGE_BYTES);     // [9][128]
+  unsigned char *om_ring = tc_smem + (size_t)STAGES * STAGE_BYTES + sizeof(TapMetaTc) * TC_NT * TC_TP;
+  float *om_buf = reinterpret_cast<float *>(om_ring + OM_STAGES * OM_STAGE_BYTES);   // [2][27][OM_PITCH]
   __shared__ __align__(8) uint64_t a_full[STAGES], b_full[STAGES], empty[STAGES];
+  __shared__ __align__(8) uint64_t om_full[OM ? OM_STAGES : 1], om_empty[OM ? OM_STAGES : 1], om_ready[2], om_free[2];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int KT = s.kh * s.kw;
   const long long HWo = (long long)s.Ho * s.Wo, HW = (long long)s.H * s.W;
-  const int Cp = s.nb * TC_CB;       // channel pitch of the channels-last copy
+  const int Cp = s.nb * TC_CB;
 
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
@@ -205,31 +270,55 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
       mbar_init(&b_full[i], 1);
       mbar_init(&empty[i], TC_MMA_WGS);
     }
+    if (OM) {
+      for (int i = 0; i < OM_STAGES; ++i) {
+        mbar_init(&om_full[i], 1);
+        mbar_init(&om_empty[i], TC_MMA_WGS);
+      }
+      for (int i = 0; i < 2; ++i) {
+        mbar_init(&om_ready[i], TC_MMA_WGS * 128);
+        mbar_init(&om_free[i], 1);
+      }
+    }
     mbar_fence_init();
   }
   __syncthreads();
 
   if (warp >= TC_WARP_S0) {
     // =========================================================== samplers: A operand of every chunk
+    // lane = (pixel sp, k-chunk sq): TF32 4 pixels x 8 k-chunks of 4 channels, bf16 8 pixels x 4 k-chunks of 8
+    constexpr int KC = TC_K / F::KE;
     const int sw = warp - TC_WARP_S0, st = tid - TC_WARP_S0 * 32;
-    const int sp = lane >> 3, sq = lane & 7;
-    int stage = 0, ph = 0;
-    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
+    const int sp = lane / KC, sq = lane % KC;
+    int stage = 0, ph = 0, n = 0;
+    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x, ++n) {
       const ItemTc it = tc_item(s, item);
-      const float *xbat = xt + (long long)it.b * HW * Cp + sq * 4;
+      const typename F::X *xbat = xt + (long long)it.b * HW * Cp + sq * F::KE;
       int cur_g = -1;
       for (int bi = it.b0; bi < it.b1; ++bi) {
         const int g = bi / s.cbs_pg;
         if (g != cur_g) {
-          // ---- bilinear geometry of every (tap, pixel) of this deformable group (mask folded into the weights)
           cur_g = g;
           named_bar_sync(1, TC_SAMPLERS * 32);   // everybody is done reading the previous geometry
-          tc_build_meta(s, offset, mask, it, g, st, KT, HWo, meta);
+          if constexpr (OM) {
+            // dg == 1: one geometry an item, from the offsets the consumers left in buffer n % 2
+            mbar_wait(&om_ready[n & 1], (uint32_t)((n >> 1) & 1));
+            const float *ob = om_buf + (n & 1) * (OM_BUF_BYTES / 4);
+            tc_build_meta_from(s, it, st, KT, meta, [&](int t, int pp, long long, float &dy, float &dx, float &m) {
+              dy = ob[(2 * t) * OM_PITCH + pp];
+              dx = ob[(2 * t + 1) * OM_PITCH + pp];
+              m = ob[(2 * TC_NT + t) * OM_PITCH + pp];
+            });
+          } else {
+            tc_build_meta(s, offset, mask, it, g, st, KT, HWo, meta);
+          }
           named_bar_sync(1, TC_SAMPLERS * 32);
+          if (OM && st == 0) mbar_arrive_tc(&om_free[n & 1]);   // the buffer may take the offsets of item n + 2
         }
-        const float *xb = xbat + (long long)bi * TC_CB;
+        const typename F::X *xb = xbat + (long long)bi * TC_CB;
         for (int tap = 0; tap < TC_NT; ++tap) {
-          // warp item = 4 pixels: every lane gathers the 4 corners of its pixel as 16-byte pieces (4 channels);
+          if constexpr (F::KE == 4) {
+          // TF32: warp item = 4 pixels: every lane gathers the 4 corners of its pixel as 16-byte pieces (4 channels);
           // a warp fills TC_SAMPLER_ROUNDS 8-pixel row groups, one after the other; both items of a group (pixels
           // 8r..8r+3 and 8r+4..8r+7) are gathered before either is reduced
 #pragma unroll 1
@@ -268,328 +357,11 @@ k_dcn_forward_tc(const float *__restrict__ xt, const float *__restrict__ offset,
             *reinterpret_cast<float4 *>(a_lo + off1) = make_float4(v1.x - h1.x, v1.y - h1.y, v1.z - h1.z, v1.w - h1.w);
           }
           }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> async proxy (wgmma reads)
-          __syncwarp();
-          if (lane == 0) mbar_arrive_tc(&a_full[stage]);
-          if (++stage == STAGES) { stage = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == TC_WARP_TMA) {
-    // =========================================================== B operand: weight tiles by TMA bulk copy
-    if (lane == 0) {
-      int stage = 0, ph = 0;
-      for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
-        const ItemTc it = tc_item(s, item);
-        for (int bi = it.b0; bi < it.b1; ++bi) {
-          for (int tap = 0; tap < TC_NT; ++tap) {
-            mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
-            unsigned char *b_hi = tc_smem + (size_t)stage * STAGE_BYTES + 2 * FW_A_BYTES;
-            const float *src = wtiles + (((size_t)it.cot * s.nb + bi) * TC_NT + tap) * 2 * (size_t)CO_T * TC_K;
-            mbar_expect_tx(&b_full[stage], 2u * B_BYTES);
-            for (uint32_t off = 0; off < 2u * B_BYTES; off += 8192u)
-              bulk_g2s(b_hi + off, reinterpret_cast<const unsigned char *>(src) + off, 8192u, &b_full[stage]);
-            if (++stage == STAGES) { stage = 0; ph ^= 1; }
-          }
-        }
-      }
-    }
-  } else {
-    // =========================================================== consumers: wgmma over the ring, epilogue from registers
-    const int wgi = warp >> 2, wq = warp & 3;
-    int stage = 0, ph = 0;
-    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x) {
-      const ItemTc it = tc_item(s, item);
-      float d[CO_T / 2];
-#pragma unroll
-      for (int i = 0; i < CO_T / 2; ++i) d[i] = 0.f;
-      const int n_ch = (it.b1 - it.b0) * TC_NT;
-      for (int ch = 0; ch < n_ch; ++ch) {
-        mbar_wait(&a_full[stage], (uint32_t)ph);
-        mbar_wait(&b_full[stage], (uint32_t)ph);
-        const uint32_t base = smem_u32(tc_smem + (size_t)stage * STAGE_BYTES);
-        const uint32_t ah = base + (uint32_t)wgi * 8u * FW_SBO, al = ah + FW_A_BYTES;   // this warpgroup's 64 rows
-        const uint32_t bh = base + 2u * FW_A_BYTES, bl = bh + B_BYTES;
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < TC_K / 8; ++ks) {   // one k8 step = two 16-byte k-chunks
-          const uint32_t koff = (uint32_t)ks * 2u * TC_LBO, koff_a = (uint32_t)ks * 2u * FW_LBO;
-          wgmma_3xtf32<CO_T>(d, fw_desc_a(ah + koff_a), fw_desc_a(al + koff_a), tc_desc(bh + koff), tc_desc(bl + koff),
-                             (ch > 0 || ks > 0) ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait_all();          // the slot is read: hand it back to the samplers and the TMA warp
-        if ((tid & 127) == 0) mbar_arrive_tc(&empty[stage]);
-        if (++stage == STAGES) { stage = 0; ph ^= 1; }
-      }
-      // epilogue: d[4j + r] = (row wq*16 + lane/4 + 8*(r/2), column 8j + 2*(lane%4) + r%2) of this warpgroup's 64 rows
-      float *dst = (s.splits > 1 ? part + (long long)it.split * s.B * s.Cout * HWo : y) + (long long)it.b * s.Cout * HWo;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int pp = wgi * 64 + wq * 16 + (lane >> 2) + 8 * h;
-        const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
-        if (ho >= s.Ho || wo >= s.Wo) continue;
-        float *dp = dst + (long long)ho * s.Wo + wo;
-#pragma unroll
-        for (int j = 0; j < CO_T / 8; ++j) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int o = it.cot * CO_T + 8 * j + 2 * (lane & 3) + e;
-            if (o < s.Cout) {
-              float r = d[4 * j + 2 * h + e];
-              if (s.splits == 1) {
-                if (bias) r += __ldg(bias + o);
-                if (s.epi_scale) r = fmaf(r, __ldg(s.epi_scale + o), __ldg(s.epi_shift + o));
-                if (s.relu) r = fmaxf(r, 0.f);
-              }
-              dp[(long long)o * HWo] = r;
-            }
-          }
-        }
-      }
-    }
-  }
-}
-
-// =====================================================================================================================
-// bf16 forward: the same pipeline with one bf16 A tile and one bf16 B tile a chunk and wgmma k16 bf16 -> fp32.
-// Numeric contract (include/centernet_b200.h): the geometry and the 4-corner interpolation are the fp32 kernel's
-// (tc_build_meta, the same fmaf chain), the masked column value is rounded once to bf16 (RN); the weights were
-// rounded once (RN) by k_dcn_prep_weights_bf16; the contraction accumulates in fp32, split-K partials are added in
-// split order, bias / BN / ReLU are applied in fp32 and the result is stored as fp32 or rounded (RN) to bf16.
-
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {   // lo -> lower address (smaller k)
-  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t *>(&v);
-}
-__device__ __forceinline__ void store_out(float *p, float v) { *p = v; }
-__device__ __forceinline__ void store_out(__nv_bfloat16 *p, float v) { *p = __float2bfloat16_rn(v); }
-__device__ __forceinline__ float load_in(const float *p) { return __ldg(p); }
-__device__ __forceinline__ float load_in(const __nv_bfloat16 *p) { return __bfloat162float(p[0]); }
-
-// W[Cout][Cin][KT] (fp32) -> per (cout tile, channel block, tap) one bf16 tile [co_t][32] (k = channel within the
-// block), the layout of bf_tile_off; tile index = (cot * nb + bi) * 9 + tap, as k_dcn_prep_weights
-__global__ void __launch_bounds__(256) k_dcn_prep_weights_bf16(const float *__restrict__ w, const DcnShapeTc s,
-                                                               unsigned char *__restrict__ ws) {
-  const int KT = s.kh * s.kw;
-  const int cpg = s.Cin / s.dg;
-  const int tile = blockIdx.x;
-  const int tap = tile % TC_NT, r = tile / TC_NT;
-  const int bi = r % s.nb, cot = r / s.nb;
-  const int g = bi / s.cbs_pg, cbi = bi - g * s.cbs_pg;
-  unsigned char *dst = ws + (size_t)tile * s.co_t * TC_K * 2;
-  for (int i = threadIdx.x; i < s.co_t * TC_K; i += blockDim.x) {
-    const int o = i / TC_K, k = i - o * TC_K;
-    const int cw = cbi * TC_CB + k;
-    const int oc = cot * s.co_t + o;
-    float v = 0.f;
-    if (oc < s.Cout && cw < cpg && tap < KT) v = w[((size_t)oc * s.Cin + g * cpg + cw) * KT + tap];
-    *reinterpret_cast<__nv_bfloat16 *>(dst + bf_tile_off(o, k)) = __float2bfloat16_rn(v);
-  }
-}
-
-// x [B][Cin][HW] (fp32 or bf16) -> bf16 xt [B][HW][nb][32], the slot mapping of k_dcn_nhwc
-template <typename T>
-__global__ void __launch_bounds__(256) k_dcn_nhwc_bf16(const T *__restrict__ x, __nv_bfloat16 *__restrict__ xt,
-                                                       const DcnShapeTc s) {
-  __shared__ float tile[64][33];
-  const long long HW = (long long)s.H * s.W;
-  const long long p0 = (long long)blockIdx.x * 32;
-  const int c0 = blockIdx.y * 64, b = blockIdx.z;
-  const int Cp = s.nb * TC_CB;
-  const int cpg = s.Cin / s.dg;
-  {
-    const int px = threadIdx.x & 31, cr = threadIdx.x >> 5;
-    for (int c = cr; c < 64; c += 8) {
-      float v = 0.f;
-      if (c0 + c < s.Cin && p0 + px < HW) v = load_in(x + ((long long)b * s.Cin + c0 + c) * HW + p0 + px);
-      tile[c][px] = v;
-    }
-  }
-  __syncthreads();
-  {
-    const int c = threadIdx.x & 63, pr = threadIdx.x >> 6;
-    const int ch = c0 + c;
-    if (ch < s.Cin) {
-      const int g = ch / cpg, within = ch - g * cpg;
-      const int slot = (g * s.cbs_pg + within / TC_CB) * TC_CB + within % TC_CB;
-      for (int px = pr; px < 32; px += 4)
-        if (p0 + px < HW) xt[((long long)b * HW + p0 + px) * Cp + slot] = __float2bfloat16_rn(tile[c][px]);
-    }
-  }
-}
-
-// fp32 channels-last [B][HW][Cin] with whole 32-channel blocks (so slot == channel) -> bf16 xt, 8 values a thread
-__global__ void __launch_bounds__(256) k_dcn_cl_to_bf16(const float4 *__restrict__ x, uint4 *__restrict__ xt,
-                                                        long long n8) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
-    const float4 a = __ldg(x + 2 * i), b = __ldg(x + 2 * i + 1);
-    xt[i] = make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(b.x, b.y), pack_bf16x2(b.z, b.w));
-  }
-}
-
-// bf16 x [B][Cin][HW] -> fp32 xt [B][HW][nb][32] (exact widening): k_dcn_nhwc reading bf16, for the bf16 backward
-__global__ void __launch_bounds__(256) k_dcn_nhwc_widen(const __nv_bfloat16 *__restrict__ x, float *__restrict__ xt,
-                                                        const DcnShapeTc s) {
-  __shared__ float tile[64][33];
-  const long long HW = (long long)s.H * s.W;
-  const long long p0 = (long long)blockIdx.x * 32;
-  const int c0 = blockIdx.y * 64, b = blockIdx.z;
-  const int Cp = s.nb * TC_CB;
-  const int cpg = s.Cin / s.dg;
-  {
-    const int px = threadIdx.x & 31, cr = threadIdx.x >> 5;
-    for (int c = cr; c < 64; c += 8) {
-      float v = 0.f;
-      if (c0 + c < s.Cin && p0 + px < HW) v = load_in(x + ((long long)b * s.Cin + c0 + c) * HW + p0 + px);
-      tile[c][px] = v;
-    }
-  }
-  __syncthreads();
-  {
-    const int c = threadIdx.x & 63, pr = threadIdx.x >> 6;
-    const int ch = c0 + c;
-    if (ch < s.Cin) {
-      const int g = ch / cpg, within = ch - g * cpg;
-      const int slot = (g * s.cbs_pg + within / TC_CB) * TC_CB + within % TC_CB;
-      for (int px = pr; px < 32; px += 4)
-        if (p0 + px < HW) xt[((long long)b * HW + p0 + px) * Cp + slot] = tile[c][px];
-    }
-  }
-}
-
-// bf16 channels-last [B][HW][Cin] with whole 32-channel blocks (slot == channel) -> fp32 xt, 8 values a thread
-__global__ void __launch_bounds__(256) k_dcn_cl_widen(const uint4 *__restrict__ x, float4 *__restrict__ xt, long long n8) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
-    const uint4 u = __ldg(x + i);
-    xt[2 * i] = make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
-                            __uint_as_float(u.y & 0xffff0000u));
-    xt[2 * i + 1] = make_float4(__uint_as_float(u.z << 16), __uint_as_float(u.z & 0xffff0000u),
-                                __uint_as_float(u.w << 16), __uint_as_float(u.w & 0xffff0000u));
-  }
-}
-
-// y[b][o][p] = epilogue(bias[o] + sum_s part[s][b][o][p]), s ascending, stored as bf16 (k_dcn_reduce writes fp32)
-__global__ void __launch_bounds__(256) k_dcn_reduce_bf16(const float *__restrict__ part, const float *__restrict__ bias,
-                                                         __nv_bfloat16 *__restrict__ y, int splits, int cout,
-                                                         long long hwo, long long total,
-                                                         const float *__restrict__ epi_scale,
-                                                         const float *__restrict__ epi_shift, int relu) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int o = (int)((i / hwo) % cout);
-    float v = 0.f;
-    for (int s = 0; s < splits; ++s) v += __ldg(part + (long long)s * total + i);
-    if (bias) v += __ldg(bias + o);
-    if (epi_scale) v = fmaf(v, __ldg(epi_scale + o), __ldg(epi_shift + o));
-    if (relu) v = fmaxf(v, 0.f);
-    y[i] = __float2bfloat16_rn(v);
-  }
-}
-
-// DCN block variant (OM = true, cnb_dcnv2_forward_block_bf16): the 3x3 conv_offset_mask runs inside the kernel.
-// For every item the TMA warp streams, per 32-channel block, the (tw + 2) x (th + 2) halo of the tile as four 8-channel
-// slabs (4-D tensor-map loads; the out-of-bounds fill is the conv's zero padding, halo.cuh) and the nine [32][32] W_om
-// tiles of the block into a ring of its own.  The consumer warpgroups compute om[128 px][27 -> 32] with wgmma m64n32k16
-// straight from the halo (shifted descriptors, no im2col), add b_om in fp32 and leave the 27 fp32 values of every pixel
-// in one of two shared buffers; the samplers build the item's tap geometry from that buffer (tc_build_meta_from, the
-// mask logit through the same sigmoid).  The consumers compute the offsets of the CTA's NEXT item before the main loop
-// of the current one, so the samplers find them ready when they reach the item boundary.  Every item computes its own
-// offsets (Cout tiles and K splits of one pixel tile recompute them).  Warpgroup wg's 64 GEMM rows are the tile's
-// column half wg (8 x 16 tiles: 8 rows of 8 pixels, one halo row apart) or row half wg (16 x 8 tiles).
-constexpr int OM_N = 32;                             // 27 offset / mask channels, padded to the wgmma N
-constexpr int OM_C = 27;                             // dg * 3 * 9 with dg = 1
-constexpr int OM_PITCH = TC_TP + 4;                  // fp32 om of one channel: 128 pixels (+4: conflict-free stores)
-constexpr uint32_t OM_SLAB = 180 * 16;               // one 8-channel slab of a 10 x 18 (or 18 x 10) halo
-constexpr uint32_t OM_SLAB_PITCH = 2944;             // slabs 128-byte aligned (TMA destination)
-constexpr uint32_t OM_HALO_BYTES = 4 * OM_SLAB_PITCH;
-constexpr uint32_t OM_W_BYTES = TC_NT * OM_N * TC_K * 2;   // the nine W_om tiles of one channel block
-constexpr uint32_t OM_STAGE_BYTES = OM_HALO_BYTES + OM_W_BYTES;
-constexpr int OM_STAGES = 2;
-constexpr uint32_t OM_BUF_BYTES = (OM_C * OM_PITCH * 4 + 127) / 128 * 128;
-constexpr uint32_t OM_SMEM_BYTES = OM_STAGES * OM_STAGE_BYTES + 2 * OM_BUF_BYTES + 128;   // + 128: alignment slack
-
-// Warp roles, items and mbarrier hand-over as k_dcn_forward_tc.  Sampler warp item = one 8-row group of the A tile
-// (8 pixels): lane = pixel * 4 + k-chunk, every lane gathers the 4 corners of its pixel as 16-byte pieces (8 bf16
-// channels), interpolates in fp32 and stores one rounded 16-byte k-chunk; each warp fills two row groups a chunk, both
-// gathered before either is reduced.
-template <int CO_T, int STAGES, typename TOut, bool OM>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict__ offset,
-                   const float *__restrict__ mask, const __nv_bfloat16 *__restrict__ wtiles,
-                   const float *__restrict__ bias, TOut *__restrict__ y, float *__restrict__ part, const DcnShapeTc s,
-                   const __grid_constant__ CUtensorMap xmap, const __nv_bfloat16 *__restrict__ womt,
-                   const float *__restrict__ bom) {
-  extern __shared__ __align__(128) unsigned char tc_smem_raw[];
-  // the block variant's TMA halo needs a 128-byte aligned destination
-  unsigned char *tc_smem = OM ? tc_smem_raw + ((128u - (smem_u32(tc_smem_raw) & 127u)) & 127u) : tc_smem_raw;
-  constexpr int B_BYTES = CO_T * TC_K * 2;
-  constexpr int STAGE_BYTES = BF_A_BYTES + B_BYTES;
-  constexpr int ROWGROUPS = TC_TP / 8 / TC_SAMPLERS;   // 2 row groups a sampler warp
-  static_assert(ROWGROUPS == 2, "k_dcn_forward_bf16: two row groups a sampler warp");
-  TapMetaTc *meta = reinterpret_cast<TapMetaTc *>(tc_smem + (size_t)STAGES * STAGE_BYTES);     // [9][128]
-  unsigned char *om_ring = tc_smem + (size_t)STAGES * STAGE_BYTES + sizeof(TapMetaTc) * TC_NT * TC_TP;
-  float *om_buf = reinterpret_cast<float *>(om_ring + OM_STAGES * OM_STAGE_BYTES);   // [2][27][OM_PITCH]
-  __shared__ __align__(8) uint64_t a_full[STAGES], b_full[STAGES], empty[STAGES];
-  __shared__ __align__(8) uint64_t om_full[OM ? OM_STAGES : 1], om_empty[OM ? OM_STAGES : 1], om_ready[2], om_free[2];
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int KT = s.kh * s.kw;
-  const long long HWo = (long long)s.Ho * s.Wo, HW = (long long)s.H * s.W;
-  const int Cp = s.nb * TC_CB;
-
-  if (tid == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&a_full[i], TC_SAMPLERS);
-      mbar_init(&b_full[i], 1);
-      mbar_init(&empty[i], TC_MMA_WGS);
-    }
-    if (OM) {
-      for (int i = 0; i < OM_STAGES; ++i) {
-        mbar_init(&om_full[i], 1);
-        mbar_init(&om_empty[i], TC_MMA_WGS);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&om_ready[i], TC_MMA_WGS * 128);
-        mbar_init(&om_free[i], 1);
-      }
-    }
-    mbar_fence_init();
-  }
-  __syncthreads();
-
-  if (warp >= TC_WARP_S0) {
-    // =========================================================== samplers: A operand of every chunk
-    const int sw = warp - TC_WARP_S0, st = tid - TC_WARP_S0 * 32;
-    const int sp = lane >> 2, sq = lane & 3;
-    const int rg0 = sw * ROWGROUPS, rg1 = rg0 + 1;
-    int stage = 0, ph = 0, n = 0;
-    for (int item = blockIdx.x; item < s.n_items; item += gridDim.x, ++n) {
-      const ItemTc it = tc_item(s, item);
-      const __nv_bfloat16 *xbat = xt + (long long)it.b * HW * Cp + sq * 8;
-      int cur_g = -1;
-      for (int bi = it.b0; bi < it.b1; ++bi) {
-        const int g = bi / s.cbs_pg;
-        if (g != cur_g) {
-          cur_g = g;
-          named_bar_sync(1, TC_SAMPLERS * 32);   // everybody is done reading the previous geometry
-          if constexpr (OM) {
-            // dg == 1: one geometry an item, from the offsets the consumers left in buffer n % 2
-            mbar_wait(&om_ready[n & 1], (uint32_t)((n >> 1) & 1));
-            const float *ob = om_buf + (n & 1) * (OM_BUF_BYTES / 4);
-            tc_build_meta_from(s, it, st, KT, meta, [&](int t, int pp, long long, float &dy, float &dx, float &m) {
-              dy = ob[(2 * t) * OM_PITCH + pp];
-              dx = ob[(2 * t + 1) * OM_PITCH + pp];
-              m = ob[(2 * TC_NT + t) * OM_PITCH + pp];
-            });
           } else {
-            tc_build_meta(s, offset, mask, it, g, st, KT, HWo, meta);
-          }
-          named_bar_sync(1, TC_SAMPLERS * 32);
-          if (OM && st == 0) mbar_arrive_tc(&om_free[n & 1]);   // the buffer may take the offsets of item n + 2
-        }
-        const __nv_bfloat16 *xb = xbat + (long long)bi * TC_CB;
-        for (int tap = 0; tap < TC_NT; ++tap) {
+          // bf16: warp item = one 8-row group of the A tile (8 pixels): every lane gathers the 4 corners of its pixel as
+          // 16-byte pieces (8 bf16 channels), interpolates in fp32 and stores one rounded 16-byte k-chunk; each warp
+          // fills two row groups a chunk, both gathered before either is reduced
+          const int rg0 = sw * TC_SAMPLER_ROUNDS, rg1 = rg0 + 1;
           const TapMetaTc m0 = meta[tap * TC_TP + rg0 * 8 + sp], m1 = meta[tap * TC_TP + rg1 * 8 + sp];
           uint4 u0[4], u1[4];
 #pragma unroll
@@ -622,6 +394,7 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
           const uint32_t off = (uint32_t)sq * BF_LBO + (uint32_t)sp * 16u;
           *reinterpret_cast<uint4 *>(a + (uint32_t)rg0 * BF_SBO + off) = v0;
           *reinterpret_cast<uint4 *>(a + (uint32_t)rg1 * BF_SBO + off) = v1;
+          }
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> async proxy (wgmma reads)
           __syncwarp();
           if (lane == 0) mbar_arrive_tc(&a_full[stage]);
@@ -630,7 +403,7 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
       }
     }
   } else if (warp == TC_WARP_TMA) {
-    // =========================================================== B operand: one bf16 weight tile by TMA bulk copy
+    // =========================================================== B operand: weight tiles by TMA bulk copy
     if (lane == 0) {
       int stage = 0, ph = 0, os = 0, oph = 0;
       // block variant: the halo slabs and W_om tiles of every channel block of item `item`, in consumer order
@@ -658,10 +431,10 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
         for (int bi = it.b0; bi < it.b1; ++bi) {
           for (int tap = 0; tap < TC_NT; ++tap) {
             mbar_wait(&empty[stage], (uint32_t)(ph ^ 1));
-            unsigned char *b = tc_smem + (size_t)stage * STAGE_BYTES + BF_A_BYTES;
-            const __nv_bfloat16 *src = wtiles + (((size_t)it.cot * s.nb + bi) * TC_NT + tap) * (size_t)CO_T * TC_K;
+            unsigned char *b = tc_smem + (size_t)stage * STAGE_BYTES + F::FW_A;
+            const unsigned char *src = wtiles + (((size_t)it.cot * s.nb + bi) * TC_NT + tap) * (size_t)B_BYTES;
             mbar_expect_tx(&b_full[stage], (uint32_t)B_BYTES);
-            bulk_g2s(b, src, (uint32_t)B_BYTES, &b_full[stage]);
+            F::fetch(b, src, (uint32_t)B_BYTES, &b_full[stage]);
             if (++stage == STAGES) { stage = 0; ph ^= 1; }
           }
         }
@@ -690,7 +463,7 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
           const uint32_t a = h + (uint32_t)((tap / 3) * (int)hx16 + (tap % 3) * 16);
 #pragma unroll
           for (int ks = 0; ks < 2; ++ks)   // one k16 step = two 8-channel slabs
-            wgmma_ss<OM_N>(q, wg_desc(a + (uint32_t)ks * 2u * OM_SLAB_PITCH, OM_SLAB_PITCH, hx16),
+            wgmma_bf16<OM_N>(q, wg_desc(a + (uint32_t)ks * 2u * OM_SLAB_PITCH, OM_SLAB_PITCH, hx16),
                            wg_desc(wb + (uint32_t)tap * (OM_N * TC_K * 2) + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO,
                                    BF_B_SBO),
                            (cb > 0 || tap > 0 || ks > 0) ? 1u : 0u);
@@ -732,19 +505,16 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
         mbar_wait(&a_full[stage], (uint32_t)ph);
         mbar_wait(&b_full[stage], (uint32_t)ph);
         const uint32_t base = smem_u32(tc_smem + (size_t)stage * STAGE_BYTES);
-        const uint32_t a = base + (uint32_t)wgi * 8u * BF_SBO;   // this warpgroup's 64 rows
-        const uint32_t b = base + (uint32_t)BF_A_BYTES;
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < TC_K / 16; ++ks)   // one k16 step = two 16-byte k-chunks
-          wgmma_bf16<CO_T>(d, wg_desc(a + (uint32_t)ks * 2u * BF_LBO, BF_LBO, BF_SBO),
-                           wg_desc(b + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO, BF_B_SBO), (ch > 0 || ks > 0) ? 1u : 0u);
+        wgmma_fence();   // A: this warpgroup's 64 rows
+        F::template mma_k32<CO_T>(d, base + (uint32_t)wgi * 8u * F::FW_A_SBO, F::FW_A / 2, F::FW_A_LBO, F::FW_A_SBO,
+                                  base + F::FW_A, B_BYTES / 2, ch > 0);
         wgmma_commit();
         wgmma_wait_all();
         if ((tid & 127) == 0) mbar_arrive_tc(&empty[stage]);
         if (++stage == STAGES) { stage = 0; ph ^= 1; }
       }
-      // epilogue: the accumulator fragment of k_dcn_forward_tc; split-K partials stay fp32
+      // epilogue: d[4j + r] = (row wq*16 + lane/4 + 8*(r/2), column 8j + 2*(lane%4) + r%2) of this warpgroup's 64
+      // rows; split-K partials stay fp32
       const long long img = (long long)it.b * s.Cout * HWo;
       float *pdst = s.splits > 1 ? part + (long long)it.split * s.B * s.Cout * HWo + img : nullptr;
       TOut *ydst = y + img;
@@ -777,239 +547,153 @@ k_dcn_forward_bf16(const __nv_bfloat16 *__restrict__ xt, const float *__restrict
   }
 }
 
-int dcn_prepare_weights_bf16(const float *weight, int cin, int cout, int kh, int kw, int dg, void *wtiles,
-                             cudaStream_t stream) {
-  DcnShapeTc s;
-  fill_shape(&s, 1, cin, 8, 8, cout, kh, kw, 1, 1, 1, 1, 1, 1, dg);
-  k_dcn_prep_weights_bf16<<<s.n_cot * s.nb * TC_NT, 256, 0, stream>>>(weight, s,
-                                                                       reinterpret_cast<unsigned char *>(wtiles));
-  CNB_CHECK_LAUNCH("cnb_dcnv2 bf16 weight tiles");
+
+// ------------------------------------------------------------------ host
+// Weight tiles of one format, one tile a (cout tile, channel block, tap) of the shape s
+template <typename F>
+static int prep_weights(const float *weight, const DcnShapeTc &s, void *wtiles, cudaStream_t stream) {
+  k_dcn_prep_weights<F><<<s.n_cot * s.nb * TC_NT, 256, 0, stream>>>(weight, s, reinterpret_cast<unsigned char *>(wtiles));
+  CNB_CHECK_LAUNCH("cnb_dcnv2 weight tiles");
   count_launch();
   return CNB_OK;
-}
-
-// W_om [27][Cin][3][3] (fp32) -> per channel block nine bf16 tiles [32][32] (rows 27..31 zero), tile index bi * 9 + tap:
-// k_dcn_prep_weights_bf16 with one Cout tile of 32 rows
-int dcn_prepare_om_weights_bf16(const float *w_om, int cin, void *om_tiles, cudaStream_t stream) {
-  DcnShapeTc s;
-  fill_shape(&s, 1, cin, 8, 8, OM_C, 3, 3, 1, 1, 1, 1, 1, 1, 1);
-  s.co_t = OM_N;
-  s.n_cot = 1;
-  k_dcn_prep_weights_bf16<<<s.nb * TC_NT, 256, 0, stream>>>(w_om, s, reinterpret_cast<unsigned char *>(om_tiles));
-  CNB_CHECK_LAUNCH("cnb_dcnv2 bf16 offset-conv weight tiles");
-  count_launch();
-  return CNB_OK;
-}
-
-size_t dcn_om_tiles_bytes(int cin) { return (size_t)(cin / TC_CB) * OM_W_BYTES; }
-
-// The operands of the block variant (OM); the plain bf16 forward passes none
-struct OmArgs {
-  CUtensorMap xmap;
-  const __nv_bfloat16 *womt;
-  const float *bom;
-};
-
-template <int CO_T, typename TOut, bool OM>
-static int launch_fwd_bf16(const __nv_bfloat16 *xt, const float *offset, const float *mask, const void *wtiles,
-                           const float *bias, void *output, float *part, const DcnShapeTc &s, const OmArgs &om,
-                           cudaStream_t stream) {
-  constexpr int STAGES = BF_STAGES;
-  const size_t smem = (size_t)STAGES * (BF_A_BYTES + CO_T * TC_K * 2) + sizeof(TapMetaTc) * TC_NT * TC_TP +
-                      (OM ? OM_SMEM_BYTES : 0);
-  static thread_local int dev_done = -1;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev_done != dev) {
-    CNB_CUDA(cudaFuncSetAttribute(k_dcn_forward_bf16<CO_T, STAGES, TOut, OM>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dev_done = dev;
-  }
-  const int grid = s.n_items < num_sms() ? s.n_items : num_sms();
-  k_dcn_forward_bf16<CO_T, STAGES, TOut, OM><<<grid, TC_THREADS, smem, stream>>>(
-      xt, offset, mask, reinterpret_cast<const __nv_bfloat16 *>(wtiles), bias, reinterpret_cast<TOut *>(output), part,
-      s, om.xmap, om.womt, om.bom);
-  CNB_CHECK_LAUNCH(OM ? "cnb_dcnv2_forward_block_bf16 (wgmma)" : "cnb_dcnv2_forward_bf16 (wgmma)");
-  count_launch();
-  return CNB_OK;
-}
-
-// The bf16 channels-last source [B][HW][nb][32] the kernel samples: a bf16 channels-last input in place, else a copy
-// into the workspace (p.bf16.xt)
-static int bf16_source(const DcnPlan &p, const DcnShapeTc &s, const void *input, bool in_bf16, void *workspace,
-                       cudaStream_t stream, const __nv_bfloat16 **xsrc) {
-  __nv_bfloat16 *xt = reinterpret_cast<__nv_bfloat16 *>(reinterpret_cast<char *>(workspace) + p.bf16.xt);
-  const long long HW = (long long)s.H * s.W;
-  *xsrc = xt;
-  if (p.x_cl && in_bf16) {
-    *xsrc = reinterpret_cast<const __nv_bfloat16 *>(input);   // sampled in place
-  } else if (p.x_cl) {
-    const long long n8 = (long long)s.B * HW * s.Cin / 8;
-    const int grid = (int)((n8 + 255) / 256 < 4096 ? (n8 + 255) / 256 : 4096);
-    k_dcn_cl_to_bf16<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4 *>(input), reinterpret_cast<uint4 *>(xt), n8);
-    CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 bf16 copy");
-    count_launch();
-  } else {
-    if ((s.Cin / s.dg) % TC_CB != 0)   // pad slots of the last channel block of every group must read as zero
-      CNB_CUDA(cudaMemsetAsync(xt, 0, (size_t)s.B * HW * s.nb * TC_CB * 2, stream));
-    dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((s.Cin + 63) / 64), (unsigned)s.B);
-    if (in_bf16)
-      k_dcn_nhwc_bf16<__nv_bfloat16><<<tgrid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16 *>(input), xt, s);
-    else
-      k_dcn_nhwc_bf16<float><<<tgrid, 256, 0, stream>>>(reinterpret_cast<const float *>(input), xt, s);
-    CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 channels-last copy");
-    count_launch();
-  }
-  return CNB_OK;
-}
-
-// The kernel for the Cout tile and output dtype, then the split-K reduce on small maps
-template <bool OM>
-static int run_fwd_bf16(const __nv_bfloat16 *xsrc, const float *offset, const float *mask, const void *wtiles,
-                        const float *bias, void *output, bool out_bf16, float *part, const DcnShapeTc &s,
-                        const OmArgs &om, cudaStream_t stream) {
-  int rc;
-  if (s.co_t == 64)
-    rc = out_bf16 ? launch_fwd_bf16<64, __nv_bfloat16, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream)
-                  : launch_fwd_bf16<64, float, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream);
-  else
-    rc = out_bf16 ? launch_fwd_bf16<128, __nv_bfloat16, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream)
-                  : launch_fwd_bf16<128, float, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream);
-  if (rc != CNB_OK) return rc;
-  if (s.splits > 1) {
-    const long long total = (long long)s.B * s.Cout * s.Ho * s.Wo;
-    const int grid = (int)((total + 255) / 256 < 1184 ? (total + 255) / 256 : 1184);
-    if (out_bf16)
-      k_dcn_reduce_bf16<<<grid, 256, 0, stream>>>(part, bias, reinterpret_cast<__nv_bfloat16 *>(output), s.splits,
-                                                  s.Cout, (long long)s.Ho * s.Wo, total, s.epi_scale, s.epi_shift,
-                                                  s.relu);
-    else
-      k_dcn_reduce<<<grid, 256, 0, stream>>>(part, bias, reinterpret_cast<float *>(output), s.splits, s.Cout,
-                                             (long long)s.Ho * s.Wo, total, s.epi_scale, s.epi_shift, s.relu);
-    CNB_CHECK_LAUNCH("cnb_dcnv2_forward_bf16 split-K reduce");
-    count_launch();
-  }
-  return CNB_OK;
-}
-
-int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
-                     const void *wtiles, const float *bias, void *output, bool out_bf16, void *workspace,
-                     cudaStream_t stream, int fused_offset_mask, const float *epi_scale, const float *epi_shift,
-                     int relu) {
-  DcnShapeTc s = p.s;
-  if (fused_offset_mask) {   // `offset` is the raw [b, 3*kt*dg, ho, wo] output of conv_offset_mask; mask = its last third
-    s.off_bs = s.mask_bs = (long long)s.dg * 3 * s.kh * s.kw * s.Ho * s.Wo;
-    s.mask_logit = 1;
-    mask = offset + (long long)s.dg * 2 * s.kh * s.kw * s.Ho * s.Wo;
-  }
-  s.epi_scale = epi_scale;
-  s.epi_shift = epi_scale ? epi_shift : nullptr;
-  s.relu = relu;
-  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
-  const __nv_bfloat16 *xsrc;
-  const int rc = bf16_source(p, s, input, in_bf16, workspace, stream, &xsrc);
-  if (rc != CNB_OK) return rc;
-  OmArgs none;
-  memset(&none, 0, sizeof(none));
-  return run_fwd_bf16<false>(xsrc, offset, mask, wtiles, bias, output, out_bf16, part, s, none, stream);
-}
-
-int dcn_forward_block_bf16(const DcnPlan &p, const void *input, bool in_bf16, const void *om_tiles,
-                           const float *om_bias, const void *wtiles, const float *bias, void *output,
-                           void *workspace, cudaStream_t stream, const float *epi_scale, const float *epi_shift,
-                           int relu) {
-  DcnShapeTc s = p.s;
-  s.mask_logit = 1;   // the last 9 of the 27 offset-conv channels are mask logits
-  s.epi_scale = epi_scale;
-  s.epi_shift = epi_scale ? epi_shift : nullptr;
-  s.relu = relu;
-  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
-  const __nv_bfloat16 *xsrc;
-  int rc = bf16_source(p, s, input, in_bf16, workspace, stream, &xsrc);
-  if (rc != CNB_OK) return rc;
-  OmArgs om;
-  const CUresult cr = encode_halo_map(&om.xmap, xsrc, s.B, s.Cin, s.H, s.W, s.tw + 2, s.th + 2);
-  CNB_REQUIRE(cr == CUDA_SUCCESS, CNB_ECUDA, "cnb_dcnv2_forward_block_bf16: cuTensorMapEncodeTiled failed (%d)",
-              (int)cr);
-  om.womt = reinterpret_cast<const __nv_bfloat16 *>(om_tiles);
-  om.bom = om_bias;
-  return run_fwd_bf16<true>(xsrc, nullptr, nullptr, wtiles, bias, output, in_bf16, part, s, om, stream);
-}
-
-// Workspace of the prepared forward: channels-last copy of the input (+ split-K partial sums); the plain forward puts
-// the weight tiles in front of it.  The bf16 forward's workspace has the same regions with a bf16 copy.
-void plan_forward_tc(DcnPlan *p) {
-  const DcnShapeTc &s = p->s;
-  const size_t part_bytes = s.splits > 1 ? align_up((size_t)s.splits * s.B * s.Cout * s.Ho * s.Wo * 4, 256) : 0;
-  p->xt_bytes = align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * 4, 256);
-  p->fwd.xt = 0;
-  p->fwd.part = p->fwd.xt + p->xt_bytes;
-  p->fwd.prepared_bytes = p->fwd.part + part_bytes;
-  p->fwd.wtiles_bytes = align_up((size_t)s.n_cot * s.nb * TC_NT * 2 * s.co_t * TC_K * 4, 256);
-  p->fwd.bytes = p->fwd.wtiles_bytes + p->fwd.prepared_bytes;
-  p->bf16.xt = 0;
-  p->bf16.xt_bytes = align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * 2, 256);
-  p->bf16.part = p->bf16.xt + p->bf16.xt_bytes;
-  p->bf16.bytes = p->bf16.part + part_bytes;
-  p->bf16.wtiles_bytes = align_up((size_t)s.n_cot * s.nb * TC_NT * s.co_t * TC_K * 2, 256);
 }
 
 int dcn_prepare_weights_tc(const float *weight, int cin, int cout, int kh, int kw, int dg, float *wtiles,
                            cudaStream_t stream) {
   DcnShapeTc s;
   fill_shape(&s, 1, cin, 8, 8, cout, kh, kw, 1, 1, 1, 1, 1, 1, dg);
-  k_dcn_prep_weights<<<s.n_cot * s.nb * TC_NT, 256, 0, stream>>>(weight, s, wtiles);
-  CNB_CHECK_LAUNCH("cnb_dcnv2 weight tiles");
-  count_launch();
-  return CNB_OK;
+  return prep_weights<Tf32x3>(weight, s, wtiles, stream);
 }
 
-int dcn_to_channels_last(const float *x, float *xt, const DcnShapeTc &s, cudaStream_t stream) {
+int dcn_prepare_weights_bf16(const float *weight, int cin, int cout, int kh, int kw, int dg, void *wtiles,
+                             cudaStream_t stream) {
+  DcnShapeTc s;
+  fill_shape(&s, 1, cin, 8, 8, cout, kh, kw, 1, 1, 1, 1, 1, 1, dg);
+  return prep_weights<Bf16>(weight, s, wtiles, stream);
+}
+
+// W_om [27][Cin][3][3] (fp32) -> per channel block nine bf16 tiles [32][32] (rows 27..31 zero), tile index bi * 9 + tap:
+// the bf16 weight tiles of one Cout tile of 32 rows
+int dcn_prepare_om_weights_bf16(const float *w_om, int cin, void *om_tiles, cudaStream_t stream) {
+  DcnShapeTc s;
+  fill_shape(&s, 1, cin, 8, 8, OM_C, 3, 3, 1, 1, 1, 1, 1, 1, 1);
+  s.co_t = OM_N;
+  s.n_cot = 1;
+  return prep_weights<Bf16>(w_om, s, om_tiles, stream);
+}
+
+size_t dcn_om_tiles_bytes(int cin) { return (size_t)(cin / TC_CB) * OM_W_BYTES; }
+
+// x -> channels-last copy xt [B][HW][nb][32] in xt's element type.  x_cl: x is [B][HW][Cin] with whole 32-channel
+// blocks (slot == channel) in the other element type, converted flat; else x is NCHW
+template <typename TIn, typename TOut>
+static int to_channels_last(const TIn *x, bool x_cl, TOut *xt, const DcnShapeTc &s, cudaStream_t stream) {
   const long long HW = (long long)s.H * s.W;
-  if ((s.Cin / s.dg) % TC_CB != 0)   // pad slots of the last channel block of every group must read as zero
-    CNB_CUDA(cudaMemsetAsync(xt, 0, (size_t)s.B * HW * s.nb * TC_CB * 4, stream));
-  dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((s.Cin + 63) / 64), (unsigned)s.B);
-  k_dcn_nhwc<<<tgrid, 256, 0, stream>>>(x, xt, s);
+  if (x_cl) {
+    const long long n8 = (long long)s.B * HW * s.Cin / 8;
+    const int grid = (int)((n8 + 255) / 256 < 4096 ? (n8 + 255) / 256 : 4096);
+    if constexpr (std::is_same_v<TOut, float>)
+      k_dcn_cl_widen<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint4 *>(x), reinterpret_cast<float4 *>(xt), n8);
+    else
+      k_dcn_cl_to_bf16<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4 *>(x), reinterpret_cast<uint4 *>(xt), n8);
+  } else {
+    if ((s.Cin / s.dg) % TC_CB != 0)   // pad slots of the last channel block of every group must read as zero
+      CNB_CUDA(cudaMemsetAsync(xt, 0, (size_t)s.B * HW * s.nb * TC_CB * sizeof(TOut), stream));
+    dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((s.Cin + 63) / 64), (unsigned)s.B);
+    k_dcn_nhwc<TIn, TOut><<<tgrid, 256, 0, stream>>>(x, xt, s);
+  }
   CNB_CHECK_LAUNCH("cnb_dcnv2 channels-last copy");
   count_launch();
   return CNB_OK;
 }
 
-int dcn_to_channels_last(const __nv_bfloat16 *x, bool x_cl, float *xt, const DcnShapeTc &s, cudaStream_t stream) {
-  const long long HW = (long long)s.H * s.W;
-  if (x_cl) {
-    const long long n8 = (long long)s.B * HW * s.Cin / 8;
-    const int grid = (int)((n8 + 255) / 256 < 4096 ? (n8 + 255) / 256 : 4096);
-    k_dcn_cl_widen<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint4 *>(x), reinterpret_cast<float4 *>(xt), n8);
-    CNB_CHECK_LAUNCH("cnb_dcnv2 channels-last fp32 copy of a bf16 input");
-    count_launch();
-    return CNB_OK;
-  }
-  if ((s.Cin / s.dg) % TC_CB != 0)
-    CNB_CUDA(cudaMemsetAsync(xt, 0, (size_t)s.B * HW * s.nb * TC_CB * 4, stream));
-  dim3 tgrid((unsigned)((HW + 31) / 32), (unsigned)((s.Cin + 63) / 64), (unsigned)s.B);
-  k_dcn_nhwc_widen<<<tgrid, 256, 0, stream>>>(x, xt, s);
-  CNB_CHECK_LAUNCH("cnb_dcnv2 channels-last fp32 copy of a bf16 input");
-  count_launch();
-  return CNB_OK;
+int dcn_to_channels_last(const float *x, float *xt, const DcnShapeTc &s, cudaStream_t stream) {
+  return to_channels_last(x, false, xt, s, stream);
 }
 
-template <int CO_T, int STAGES>
-static int launch_fwd(const float *xt, const float *offset, const float *mask, const float *wtiles, const float *bias,
-                      float *output, float *part, const DcnShapeTc &s, cudaStream_t stream) {
-  const size_t smem = (size_t)STAGES * (2 * FW_A_BYTES + 2 * CO_T * TC_K * 4) + sizeof(TapMetaTc) * TC_NT * TC_TP;
+int dcn_to_channels_last(const __nv_bfloat16 *x, bool x_cl, float *xt, const DcnShapeTc &s, cudaStream_t stream) {
+  return to_channels_last(x, x_cl, xt, s, stream);
+}
+
+// The channels-last source [B][HW][nb][32] the forward of format F samples: a channels-last input of F's element type
+// in place, else a copy into the workspace region xt (l.xt)
+template <typename F>
+static int fwd_source(const DcnPlan &p, const DcnFwdLayout &l, const DcnShapeTc &s, const void *input, bool in_bf16,
+                      void *workspace, cudaStream_t stream, const typename F::X **xsrc) {
+  using X = typename F::X;
+  X *xt = reinterpret_cast<X *>(reinterpret_cast<char *>(workspace) + l.xt);
+  *xsrc = xt;
+  if (p.x_cl && in_bf16 == std::is_same_v<X, __nv_bfloat16>) {
+    *xsrc = reinterpret_cast<const X *>(input);   // sampled in place
+    return CNB_OK;
+  }
+  if (in_bf16) return to_channels_last(reinterpret_cast<const __nv_bfloat16 *>(input), p.x_cl, xt, s, stream);
+  return to_channels_last(reinterpret_cast<const float *>(input), p.x_cl, xt, s, stream);
+}
+
+// The operands of the block variant (OM); the other forwards pass none
+struct OmArgs {
+  CUtensorMap xmap;
+  const __nv_bfloat16 *womt;
+  const float *bom;
+};
+
+template <typename F, int CO_T, typename TOut, bool OM>
+static int launch_fwd(const typename F::X *xt, const float *offset, const float *mask, const void *wtiles,
+                      const float *bias, void *output, float *part, const DcnShapeTc &s, const OmArgs &om,
+                      cudaStream_t stream) {
+  const size_t smem = (size_t)F::fw_stages(CO_T) * (F::FW_A + CO_T * TC_K * F::ELEM) +
+                      sizeof(TapMetaTc) * TC_NT * TC_TP + (OM ? OM_SMEM_BYTES : 0);
   static thread_local int dev_done = -1;
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev_done != dev) {
-    CNB_CUDA(cudaFuncSetAttribute(k_dcn_forward_tc<CO_T, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CNB_CUDA(cudaFuncSetAttribute(k_dcn_forward<F, CO_T, TOut, OM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
     dev_done = dev;
   }
   const int grid = s.n_items < num_sms() ? s.n_items : num_sms();
-  k_dcn_forward_tc<CO_T, STAGES><<<grid, TC_THREADS, smem, stream>>>(xt, offset, mask, wtiles, bias, output, part, s);
-  CNB_CHECK_LAUNCH("cnb_dcnv2_forward (wgmma)");
+  k_dcn_forward<F, CO_T, TOut, OM><<<grid, TC_THREADS, smem, stream>>>(
+      xt, offset, mask, reinterpret_cast<const unsigned char *>(wtiles), bias, reinterpret_cast<TOut *>(output), part,
+      s, om.xmap, om.womt, om.bom);
+  CNB_CHECK_LAUNCH("cnb_dcnv2 forward (wgmma)");
   count_launch();
   return CNB_OK;
+}
+
+// The kernel for the Cout tile, then the split-K reduce on small maps
+template <typename F, typename TOut, bool OM>
+static int run_fwd(const typename F::X *xsrc, const float *offset, const float *mask, const void *wtiles,
+                   const float *bias, void *output, float *part, const DcnShapeTc &s, const OmArgs &om,
+                   cudaStream_t stream) {
+  const int rc = s.co_t == 64 ? launch_fwd<F, 64, TOut, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream)
+                              : launch_fwd<F, 128, TOut, OM>(xsrc, offset, mask, wtiles, bias, output, part, s, om, stream);
+  if (rc != CNB_OK) return rc;
+  if (s.splits > 1) {
+    const long long total = (long long)s.B * s.Cout * s.Ho * s.Wo;
+    const int grid = (int)((total + 255) / 256 < 1184 ? (total + 255) / 256 : 1184);
+    k_dcn_reduce<TOut><<<grid, 256, 0, stream>>>(part, bias, reinterpret_cast<TOut *>(output), s.splits, s.Cout,
+                                                 (long long)s.Ho * s.Wo, total, s.epi_scale, s.epi_shift, s.relu);
+    CNB_CHECK_LAUNCH("cnb_dcnv2 forward split-K reduce");
+    count_launch();
+  }
+  return CNB_OK;
+}
+
+// The call's shape: fused_offset_mask: `offset` is the raw [b, 3*kt*dg, ho, wo] output of conv_offset_mask and *mask
+// becomes its last third (mask logits); epi_scale / epi_shift / relu: the folded BatchNorm + ReLU epilogue
+static DcnShapeTc call_shape(const DcnPlan &p, int fused_offset_mask, const float *offset, const float **mask,
+                             const float *epi_scale, const float *epi_shift, int relu) {
+  DcnShapeTc s = p.s;
+  if (fused_offset_mask) {
+    s.off_bs = s.mask_bs = (long long)s.dg * 3 * s.kh * s.kw * s.Ho * s.Wo;
+    s.mask_logit = 1;
+    *mask = offset + (long long)s.dg * 2 * s.kh * s.kw * s.Ho * s.Wo;
+  }
+  s.epi_scale = epi_scale;
+  s.epi_shift = epi_scale ? epi_shift : nullptr;
+  s.relu = relu;
+  return s;
 }
 
 // Tensor-core forward from pre-tiled weights.  p.x_cl: `input` already is [B][H*W][Cin] (torch channels_last) with
@@ -1017,37 +701,65 @@ static int launch_fwd(const float *xt, const float *offset, const float *mask, c
 int dcn_forward_tc_prepared(const DcnPlan &p, const float *input, const float *offset, const float *mask,
                             const float *wtiles, const float *bias, float *output, void *workspace, cudaStream_t stream,
                             int fused_offset_mask, const float *epi_scale, const float *epi_shift, int relu) {
-  DcnShapeTc s = p.s;
-  if (fused_offset_mask) {   // `offset` is the raw [b, 3*kt*dg, ho, wo] output of conv_offset_mask; mask = its last third
-    s.off_bs = s.mask_bs = (long long)s.dg * 3 * s.kh * s.kw * s.Ho * s.Wo;
-    s.mask_logit = 1;
-    mask = offset + (long long)s.dg * 2 * s.kh * s.kw * s.Ho * s.Wo;
-  }
-  s.epi_scale = epi_scale;
-  s.epi_shift = epi_scale ? epi_shift : nullptr;
-  s.relu = relu;
-  float *xt = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.fwd.xt);
-  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.fwd.part);
-  const float *xsrc = xt;
-  if (p.x_cl) {
-    xsrc = input;
-  } else {
-    const int rc_t = dcn_to_channels_last(input, xt, s, stream);
-    if (rc_t != CNB_OK) return rc_t;
-  }
-  int rc;
-  if (s.co_t == 64) rc = launch_fwd<64, 3>(xsrc, offset, mask, wtiles, bias, output, part, s, stream);
-  else rc = launch_fwd<128, 2>(xsrc, offset, mask, wtiles, bias, output, part, s, stream);
+  const DcnShapeTc s = call_shape(p, fused_offset_mask, offset, &mask, epi_scale, epi_shift, relu);
+  const float *xsrc;
+  const int rc = fwd_source<Tf32x3>(p, p.fwd, s, input, false, workspace, stream, &xsrc);
   if (rc != CNB_OK) return rc;
-  if (s.splits > 1) {
-    const long long total = (long long)s.B * s.Cout * s.Ho * s.Wo;
-    const int grid = (int)((total + 255) / 256 < 1184 ? (total + 255) / 256 : 1184);
-    k_dcn_reduce<<<grid, 256, 0, stream>>>(part, bias, output, s.splits, s.Cout, (long long)s.Ho * s.Wo, total,
-                                           s.epi_scale, s.epi_shift, s.relu);
-    CNB_CHECK_LAUNCH("cnb_dcnv2_forward split-K reduce");
-    count_launch();
-  }
-  return CNB_OK;
+  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.fwd.part);
+  return run_fwd<Tf32x3, float, false>(xsrc, offset, mask, wtiles, bias, output, part, s, OmArgs{}, stream);
+}
+
+int dcn_forward_bf16(const DcnPlan &p, const void *input, bool in_bf16, const float *offset, const float *mask,
+                     const void *wtiles, const float *bias, void *output, bool out_bf16, void *workspace,
+                     cudaStream_t stream, int fused_offset_mask, const float *epi_scale, const float *epi_shift,
+                     int relu) {
+  const DcnShapeTc s = call_shape(p, fused_offset_mask, offset, &mask, epi_scale, epi_shift, relu);
+  const __nv_bfloat16 *xsrc;
+  const int rc = fwd_source<Bf16>(p, p.bf16, s, input, in_bf16, workspace, stream, &xsrc);
+  if (rc != CNB_OK) return rc;
+  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
+  return out_bf16 ? run_fwd<Bf16, __nv_bfloat16, false>(xsrc, offset, mask, wtiles, bias, output, part, s, OmArgs{},
+                                                        stream)
+                  : run_fwd<Bf16, float, false>(xsrc, offset, mask, wtiles, bias, output, part, s, OmArgs{}, stream);
+}
+
+int dcn_forward_block_bf16(const DcnPlan &p, const void *input, bool in_bf16, const void *om_tiles,
+                           const float *om_bias, const void *wtiles, const float *bias, void *output,
+                           void *workspace, cudaStream_t stream, const float *epi_scale, const float *epi_shift,
+                           int relu) {
+  const float *mask = nullptr;
+  DcnShapeTc s = call_shape(p, 0, nullptr, &mask, epi_scale, epi_shift, relu);
+  s.mask_logit = 1;   // the last 9 of the 27 offset-conv channels are mask logits
+  const __nv_bfloat16 *xsrc;
+  const int rc = fwd_source<Bf16>(p, p.bf16, s, input, in_bf16, workspace, stream, &xsrc);
+  if (rc != CNB_OK) return rc;
+  float *part = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + p.bf16.part);
+  OmArgs om;
+  const CUresult cr = encode_halo_map(&om.xmap, xsrc, s.B, s.Cin, s.H, s.W, s.tw + 2, s.th + 2);
+  CNB_REQUIRE(cr == CUDA_SUCCESS, CNB_ECUDA, "cnb_dcnv2_forward_block_bf16: cuTensorMapEncodeTiled failed (%d)",
+              (int)cr);
+  om.womt = reinterpret_cast<const __nv_bfloat16 *>(om_tiles);
+  om.bom = om_bias;
+  return in_bf16 ? run_fwd<Bf16, __nv_bfloat16, true>(xsrc, nullptr, nullptr, wtiles, bias, output, part, s, om, stream)
+                 : run_fwd<Bf16, float, true>(xsrc, nullptr, nullptr, wtiles, bias, output, part, s, om, stream);
+}
+
+// Workspace of one forward format: channels-last copy of the input (+ split-K partial sums); the plain fp32 forward
+// puts the weight tiles in front of it
+template <typename F>
+static void plan_fwd(const DcnShapeTc &s, DcnFwdLayout &l) {
+  const size_t part_bytes = s.splits > 1 ? align_up((size_t)s.splits * s.B * s.Cout * s.Ho * s.Wo * 4, 256) : 0;
+  l.xt = 0;
+  l.xt_bytes = align_up((size_t)s.B * s.H * s.W * s.nb * TC_CB * sizeof(typename F::X), 256);
+  l.part = l.xt + l.xt_bytes;
+  l.prepared_bytes = l.part + part_bytes;
+  l.wtiles_bytes = align_up((size_t)s.n_cot * s.nb * TC_NT * s.co_t * TC_K * F::ELEM, 256);
+  l.bytes = l.wtiles_bytes + l.prepared_bytes;
+}
+
+void plan_forward_tc(DcnPlan *p) {
+  plan_fwd<Tf32x3>(p->s, p->fwd);
+  plan_fwd<Bf16>(p->s, p->bf16);
 }
 
 }  // namespace cnb

@@ -205,9 +205,9 @@ k_head_fwd_bf16(const __grid_constant__ CUtensorMap xmap, const __nv_bfloat16 *_
           wgmma_fence();
 #pragma unroll
           for (int ks = 0; ks < 2; ++ks)   // one k16 step = two 8-channel slabs
-            wgmma_ss<L::NT1>(d, wg_desc(a + (uint32_t)ks * 2u * HD_SLAB_PITCH, HD_SLAB_PITCH, HD_HX * 16),
-                           wg_desc(bw + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO, BF_B_SBO),
-                           (cb > 0 || tap > 0 || ks > 0) ? 1u : 0u);
+            wgmma_bf16<L::NT1>(d, wg_desc(a + (uint32_t)ks * 2u * HD_SLAB_PITCH, HD_SLAB_PITCH, HD_HX * 16),
+                               wg_desc(bw + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO, BF_B_SBO),
+                               (cb > 0 || tap > 0 || ks > 0) ? 1u : 0u);
           wgmma_commit();
           wgmma_wait_all();
           if ((tid & 127) == 0) mbar_arrive_tc(&w_empty[ws]);
@@ -246,8 +246,8 @@ k_head_fwd_bf16(const __grid_constant__ CUtensorMap xmap, const __nv_bfloat16 *_
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks)
-        wgmma_ss<N2>(e, wg_desc(a + (uint32_t)ks * 256u, 128, CMID * 16),
-                     wg_desc(bw + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO, BF_B_SBO), (kc > 0 || ks > 0) ? 1u : 0u);
+        wgmma_bf16<N2>(e, wg_desc(a + (uint32_t)ks * 256u, 128, CMID * 16),
+                       wg_desc(bw + (uint32_t)ks * 2u * BF_B_LBO, BF_B_LBO, BF_B_SBO), (kc > 0 || ks > 0) ? 1u : 0u);
       wgmma_commit();
       wgmma_wait_all();
       if ((tid & 127) == 0) mbar_arrive_tc(&w_empty[ws]);
