@@ -35,7 +35,7 @@ struct DcnShape {
   int B, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, Ho, Wo;
 };
 
-struct TapMeta {   // one (tap, pixel): clamped corner offsets into an input plane + weights (0 when out of range)
+struct TapMeta {   // one (tap, pixel): corner offsets into an input plane (-1: out of range, never read) + weights
   int o[4];
   float w[4];
 };
@@ -76,6 +76,12 @@ __device__ __forceinline__ void sample_point(const DcnShape &s, const float *__r
   *w_im = (float)(wo * s.sw - s.pw + j * s.dw) + dx;
 }
 
+// x at corner offset o of plane xp: an out-of-range corner (o < 0) is not read and counts 0, as in the reference
+// (dcn_v2_im2col_cuda.cu:31-41), so a NaN / Inf elsewhere in the plane never meets its zero weight
+__device__ __forceinline__ float corner_value(const float *__restrict__ xp, int o) {
+  return o >= 0 ? __ldg(xp + o) : 0.0f;
+}
+
 // Fill meta[t][pp] for the pixel tile (deformable group g).  fold_mask: weights *= mask.
 __device__ __forceinline__ void build_meta(const DcnShape &s, const float *offset, const float *mask, int b, int g,
                                            long long p_base, long long HWo, TapMeta *meta, float *mask_out,
@@ -87,7 +93,7 @@ __device__ __forceinline__ void build_meta(const DcnShape &s, const float *offse
     TapMeta mt;
     float mval = 0.0f;
 #pragma unroll
-    for (int q = 0; q < 4; ++q) { mt.o[q] = 0; mt.w[q] = 0.0f; }
+    for (int q = 0; q < 4; ++q) { mt.o[q] = -1; mt.w[q] = 0.0f; }
     if (p < HWo) {
       float h_im, w_im;
       sample_point(s, offset, mask, b, g, t, (int)p, &h_im, &w_im, &mval);
@@ -95,6 +101,7 @@ __device__ __forceinline__ void build_meta(const DcnShape &s, const float *offse
       const float hh = 1.0f - bl.lh, hw = 1.0f - bl.lw;
       const float f = fold_mask ? mval : 1.0f;
       const int base = bl.h_low * s.W + bl.w_low;
+      if (!bl.inside) mt.w[0] = 0.0f * f;   // outside: the column value is 0 * mask (:174), NaN for a NaN mask
       if (bl.v1) { mt.o[0] = base; mt.w[0] = hh * hw * f; }
       if (bl.v2) { mt.o[1] = base + 1; mt.w[1] = hh * bl.lw * f; }
       if (bl.v3) { mt.o[2] = base + s.W; mt.w[2] = bl.lh * hw * f; }
@@ -155,10 +162,10 @@ k_dcn_forward(const float *__restrict__ x, const float *__restrict__ offset, con
         const int cl = r / KT, t = r - cl * KT;
         const TapMeta mt = meta[t * DCN_TP + pp];
         const float *xp = x + ((long long)b * s.Cin + c0 + cl) * HW;
-        float v = mt.w[0] * __ldg(xp + mt.o[0]);
-        v = fmaf(mt.w[1], __ldg(xp + mt.o[1]), v);
-        v = fmaf(mt.w[2], __ldg(xp + mt.o[2]), v);
-        v = fmaf(mt.w[3], __ldg(xp + mt.o[3]), v);
+        float v = mt.w[0] * corner_value(xp, mt.o[0]);
+        v = fmaf(mt.w[1], corner_value(xp, mt.o[1]), v);
+        v = fmaf(mt.w[2], corner_value(xp, mt.o[2]), v);
+        v = fmaf(mt.w[3], corner_value(xp, mt.o[3]), v);
         col[r * DCN_TP + pp] = v;
       }
       __syncthreads();
@@ -418,10 +425,10 @@ k_dcn_bwd_weight(const float *__restrict__ x, const float *__restrict__ offset, 
       const int cl = r / KT, t = r - cl * KT;
       const TapMeta mt = meta[t * DCN_TP + pp];
       const float *xp = x + ((long long)b * s.Cin + c0 + cl) * HW;
-      float v = mt.w[0] * __ldg(xp + mt.o[0]);
-      v = fmaf(mt.w[1], __ldg(xp + mt.o[1]), v);
-      v = fmaf(mt.w[2], __ldg(xp + mt.o[2]), v);
-      v = fmaf(mt.w[3], __ldg(xp + mt.o[3]), v);
+      float v = mt.w[0] * corner_value(xp, mt.o[0]);
+      v = fmaf(mt.w[1], corner_value(xp, mt.o[1]), v);
+      v = fmaf(mt.w[2], corner_value(xp, mt.o[2]), v);
+      v = fmaf(mt.w[3], corner_value(xp, mt.o[3]), v);
       col[r * DCN_TP + pp] = v;
     }
     __syncthreads();

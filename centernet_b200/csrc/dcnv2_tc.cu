@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(256) k_dcn_reduce(const float *__restrict__ pa
     for (int s = 0; s < splits; ++s) v += __ldg(part + (long long)s * total + i);
     if (bias) v += __ldg(bias + o);
     if (epi_scale) v = fmaf(v, __ldg(epi_scale + o), __ldg(epi_shift + o));
-    if (relu) v = fmaxf(v, 0.f);
+    if (relu) v = v < 0.f ? 0.f : v;   // keeps NaN, as torch.relu (fmaxf would make it 0)
     store_out(y + i, v);
   }
 }
@@ -178,9 +178,9 @@ __device__ __forceinline__ void tc_build_meta_from(const DcnShapeTc &s, const It
   for (int idx = st; idx < TC_NT * TC_TP; idx += TC_SAMPLERS * 32) {
     const int t = idx / TC_TP, pp = idx - t * TC_TP;
     const int ho = it.ty0 + pp / s.tw, wo = it.tx0 + pp % s.tw;
-    TapMetaTc mt;
+    TapMetaTc mt;   // o = -1: corner out of range, not read (the samplers select 0)
 #pragma unroll
-    for (int q = 0; q < 4; ++q) { mt.o[q] = 0; mt.w[q] = 0.f; }
+    for (int q = 0; q < 4; ++q) { mt.o[q] = -1; mt.w[q] = 0.f; }
     if (ho < s.Ho && wo < s.Wo && t < KT) {
       const long long p = (long long)ho * s.Wo + wo;
       const int i = t / s.kw, j = t - i * s.kw;
@@ -198,6 +198,8 @@ __device__ __forceinline__ void tc_build_meta_from(const DcnShapeTc &s, const It
         if (hl >= 0 && wl + 1 <= s.W - 1) { mt.o[1] = base + 1; mt.w[1] = hh * lw * m; }
         if (hl + 1 <= s.H - 1 && wl >= 0) { mt.o[2] = base + s.W; mt.w[2] = lh * hw * m; }
         if (hl + 1 <= s.H - 1 && wl + 1 <= s.W - 1) { mt.o[3] = base + s.W + 1; mt.w[3] = lh * lw * m; }
+      } else {
+        mt.w[0] = 0.f * m;   // outside: the column value is 0 * mask (:174), NaN for a NaN mask
       }
     }
     meta[idx] = mt;
@@ -328,9 +330,9 @@ k_dcn_forward(const typename F::X *__restrict__ xt, const float *__restrict__ of
           const TapMetaTc m0 = meta[tap * TC_TP + pp0], m1 = meta[tap * TC_TP + pp1];
           float4 u0[4], u1[4];
 #pragma unroll
-          for (int q = 0; q < 4; ++q) u0[q] = __ldg(reinterpret_cast<const float4 *>(xb + (long long)m0.o[q] * Cp));
+          for (int q = 0; q < 4; ++q) u0[q] = m0.o[q] >= 0 ? __ldg(reinterpret_cast<const float4 *>(xb + (long long)m0.o[q] * Cp)) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-          for (int q = 0; q < 4; ++q) u1[q] = __ldg(reinterpret_cast<const float4 *>(xb + (long long)m1.o[q] * Cp));
+          for (int q = 0; q < 4; ++q) u1[q] = m1.o[q] >= 0 ? __ldg(reinterpret_cast<const float4 *>(xb + (long long)m1.o[q] * Cp)) : make_float4(0.f, 0.f, 0.f, 0.f);
           auto reduce = [&](const TapMetaTc &mt, const float4 (&u)[4]) {
             float4 v;
             v.x = fmaf(mt.w[3], u[3].x, fmaf(mt.w[2], u[2].x, fmaf(mt.w[1], u[1].x, mt.w[0] * u[0].x)));
@@ -365,9 +367,9 @@ k_dcn_forward(const typename F::X *__restrict__ xt, const float *__restrict__ of
           const TapMetaTc m0 = meta[tap * TC_TP + rg0 * 8 + sp], m1 = meta[tap * TC_TP + rg1 * 8 + sp];
           uint4 u0[4], u1[4];
 #pragma unroll
-          for (int q = 0; q < 4; ++q) u0[q] = __ldg(reinterpret_cast<const uint4 *>(xb + (long long)m0.o[q] * Cp));
+          for (int q = 0; q < 4; ++q) u0[q] = m0.o[q] >= 0 ? __ldg(reinterpret_cast<const uint4 *>(xb + (long long)m0.o[q] * Cp)) : make_uint4(0, 0, 0, 0);
 #pragma unroll
-          for (int q = 0; q < 4; ++q) u1[q] = __ldg(reinterpret_cast<const uint4 *>(xb + (long long)m1.o[q] * Cp));
+          for (int q = 0; q < 4; ++q) u1[q] = m1.o[q] >= 0 ? __ldg(reinterpret_cast<const uint4 *>(xb + (long long)m1.o[q] * Cp)) : make_uint4(0, 0, 0, 0);
           // fp32 value of channel 2e (lower half) / 2e + 1 (upper half) of a 4 x 32-bit piece: exact widening
           auto reduce = [&](const TapMetaTc &mt, const uint4 (&u)[4]) {
             uint32_t r[4];
@@ -536,7 +538,7 @@ k_dcn_forward(const typename F::X *__restrict__ xt, const float *__restrict__ of
               } else {
                 if (bias) r += __ldg(bias + o);
                 if (s.epi_scale) r = fmaf(r, __ldg(s.epi_scale + o), __ldg(s.epi_shift + o));
-                if (s.relu) r = fmaxf(r, 0.f);
+                if (s.relu) r = r < 0.f ? 0.f : r;   // keeps NaN, as torch.relu
                 store_out(ydst + (long long)o * HWo + p, r);
               }
             }

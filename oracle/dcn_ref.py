@@ -47,10 +47,12 @@ def dcn_v2_forward(x, offset, mask, weight, bias, stride=1, padding=1, dilation=
             h_low = h_low.long(); w_low = w_low.long(); h_high = h_low + 1; w_high = w_low + 1
 
             def corner(hi, wi, ok):
+                # an out-of-range corner is never read (v = 0): a select, so a NaN / Inf that the clamped index
+                # happens to hit stays out of the sum (v * ok would give NaN * 0 = NaN)
                 ok = ok & inside
                 idx = (hi.clamp(0, H - 1) * W + wi.clamp(0, W - 1)).view(B, 1, Ho * Wo).expand(B, cpg, Ho * Wo)
                 v = xg.gather(2, idx).view(B, cpg, Ho, Wo)
-                return v * ok.unsqueeze(1)
+                return torch.where(ok.unsqueeze(1), v, 0.0)
 
             v1 = corner(h_low, w_low, (h_low >= 0) & (w_low >= 0))            # :31-41
             v2 = corner(h_low, w_high, (h_low >= 0) & (w_high <= W - 1))
@@ -58,6 +60,9 @@ def dcn_v2_forward(x, offset, mask, weight, bias, stride=1, padding=1, dilation=
             v4 = corner(h_high, w_high, (h_high <= H - 1) & (w_high <= W - 1))
             val = (hh * hw).unsqueeze(1) * v1 + (hh * lw).unsqueeze(1) * v2 + \
                   (lh * hw).unsqueeze(1) * v3 + (lh * lw).unsqueeze(1) * v4   # :43-46
+            # outside samples: val stays 0 (:160-168) even where a NaN / Inf offset made the corner weights NaN;
+            # val * m is stored for them too (:174), so a NaN mask gives NaN there
+            val = torch.where(inside.unsqueeze(1), val, 0.0)
             cols.append((val * m.unsqueeze(1), g, t))                          # :174
     # col[b, c, t, p] ordered as the weight's (c, kh, kw) axes
     col = torch.zeros(B, Cin, KT, Ho, Wo, dtype=torch.float64)

@@ -127,3 +127,89 @@ def test_anisotropic_geometry():
         _, _, Ho, Wo = want.shape
         got = dcn_v2_forward(x, torch.zeros(2, 12, Ho, Wo), torch.ones(2, 6, Ho, Wo), w, b, stride, pad, dil)
         assert got.shape == want.shape and (got - want).abs().max().item() < 1e-12
+
+
+# ---------------------------------------------------------------- non-finite inputs: the reference's rule
+# The reference never reads an out-of-range corner (v = 0, :31-41) and never samples outside the open box (val = 0,
+# :160-168), but it multiplies every in-range corner by its weight, 0 included, and stores val * mask for every sample
+# (:174).  One output pixel per sample: a 1x1 tap of weight 1, stride 1, pad 0, so y[p] = bias + mask[p] * val[p].
+NH, NW = 4, 5
+NPOS = (-1.5, -1.0, -0.5, 0.0, 0.5, 1.0, 2.0, NH - 1.0, NH - 0.5, float(NH))
+
+
+def _one_tap(x, pos, m=None):
+    """y[k] = the oracle's sample of x [NH, NW] at pos[k] = (h, w) times m[k]: a 1x1 tap of weight 1 at stride 1, pad 0,
+    each sample on an output pixel of its own (the rest sample at -40, outside)."""
+    n = len(pos)
+    m = torch.ones(n, dtype=torch.float64) if m is None else m
+    ys = []
+    for k0 in range(0, n, NH * NW):
+        chunk = pos[k0:k0 + NH * NW]
+        off = torch.full((1, 2, NH, NW), -40.0, dtype=torch.float64)
+        mk = torch.ones(1, 1, NH, NW, dtype=torch.float64)
+        for k, (h, w) in enumerate(chunk):
+            ho, wo = divmod(k, NW)
+            off[0, 0, ho, wo], off[0, 1, ho, wo], mk[0, 0, ho, wo] = h - ho, w - wo, m[k0 + k]
+        y = dcn_v2_forward(x.view(1, 1, NH, NW), off, mk, torch.ones(1, 1, 1, 1), None, stride=1, padding=0)
+        ys.append(y.view(-1)[:len(chunk)])
+    return torch.cat(ys)
+
+
+def _touches_origin(h, w):
+    """Whether the sample at (h, w) reads corner (0, 0) with a zero / non-zero weight: (reads, weight)."""
+    if not (-1 < h < NH and -1 < w < NW):
+        return False, 0.0
+    hl, wl = math.floor(h), math.floor(w)
+    if hl not in (-1, 0) or wl not in (-1, 0):
+        return False, 0.0
+    lh, lw = h - hl, w - wl
+    return True, (lh if hl == -1 else 1 - lh) * (lw if wl == -1 else 1 - lw)
+
+
+def test_nonfinite_at_the_origin_reaches_only_the_samples_that_read_it():
+    pos = [(h, w) for h in NPOS for w in (-1.5, -1.0, -0.5, 0.0, 0.5, 1.0, 2.0, NW - 1.5)]
+    for v in (float("nan"), float("inf"), -float("inf")):
+        x = XB[:NH, :NW].clone()
+        x[0, 0] = v
+        y = _one_tap(x, pos)
+        for k, (h, w) in enumerate(pos):
+            reads, wt = _touches_origin(h, w)
+            if not reads:
+                assert math.isfinite(y[k].item()), (v, h, w)        # v * ok would give NaN here
+            elif wt == 0.0 or math.isnan(v):
+                assert math.isnan(y[k].item()), (v, h, w)           # in range with weight 0: 0 * Inf = NaN
+            else:
+                assert y[k].item() == v, (v, h, w)
+
+
+def test_nonfinite_mask_and_offsets():
+    x = XB[:NH, :NW].clone()
+    pos = [(-40.0, 1.0), (float(NH), 1.0), (1.0, -1.0), (1.5, 1.5), (0.0, 0.0)]   # three outside, two inside
+    y = _one_tap(x, pos, torch.full((len(pos),), float("nan"), dtype=torch.float64))
+    assert torch.isnan(y).all()                       # val * NaN for the outside samples too (val = 0 there)
+    # NaN / Inf offsets: never inside the open box, so val = 0 and the output is 0 * mask
+    for bad in (float("nan"), float("inf"), -float("inf")):
+        y = _one_tap(x, [(bad, 1.0), (1.0, bad), (bad, bad)], torch.full((3,), 0.5, dtype=torch.float64))
+        assert torch.equal(y, torch.zeros(3, dtype=torch.float64)), bad
+        y = _one_tap(x, [(bad, 1.0)], torch.full((1,), float("nan"), dtype=torch.float64))
+        assert torch.isnan(y).all(), bad
+
+
+def test_nonfinite_x_gradients():
+    """An Inf at (0, 0) that a sample does not read leaves that sample's dOffset and dMask finite; dX never depends
+    on x."""
+    x = XB[:NH, :NW].clone()
+    x[0, 0] = float("inf")
+    x = x.view(1, 1, NH, NW).requires_grad_(True)
+    off = torch.full((1, 2, NH, NW), -40.0, dtype=torch.float64)
+    pos = [(2.0, 2.5), (-0.5, -0.5), (1.5, 3.0)]             # pixel 1 reads (0, 0), pixels 0 and 2 do not
+    for k, (h, w) in enumerate(pos):
+        off[0, 0, 0, k], off[0, 1, 0, k] = h, w - k
+    off.requires_grad_(True)
+    m = torch.full((1, 1, NH, NW), 0.5, dtype=torch.float64, requires_grad=True)
+    dcn_v2_forward(x, off, m, torch.ones(1, 1, 1, 1), None, stride=1, padding=0).sum().backward()
+    assert torch.isfinite(x.grad).all()
+    assert x.grad[0, 0, 0, 0].item() == 0.125                 # the corner weight 1/4 times the mask
+    assert torch.isfinite(off.grad[0, :, 0, 0]).all() and torch.isfinite(off.grad[0, :, 0, 2]).all()
+    assert math.isfinite(m.grad[0, 0, 0, 0].item()) and math.isfinite(m.grad[0, 0, 0, 2].item())
+    assert torch.isinf(off.grad[0, :, 0, 1]).all() and m.grad[0, 0, 0, 1].item() == float("inf")
