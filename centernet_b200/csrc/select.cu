@@ -31,6 +31,10 @@
 // .float() upcast (DESIGN 4.1).  Other stage-1 kernels read fp32 only.
 #include "select.cuh"
 #include <stdlib.h>
+#include <algorithm>
+#include <map>
+#include <mutex>
+#include <utility>
 
 namespace cnb {
 
@@ -826,6 +830,15 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
 // tuning build only (tools/select_stats.py rebuilds the library with -DCNB_SELECT_STATS): per CTA
 // [total, wait, bootstrap, flush, finalize] cycles and [units, bootstraps, flushes, finalizes] counts
 __device__ unsigned long long g_select_stats[SEL_MAX_CTA][10];
+// per call (ring of SEL_TIME_CALLS launches, indexed by SelectPlan::stat_call) and CTA: %globaltimer (ns) at
+// [entry, first stage ready, last plane swept, exit]; tools/decode_junction_time.py reads it
+constexpr int SEL_TIME_CALLS = 64;
+__device__ unsigned long long g_select_times[SEL_TIME_CALLS][SEL_MAX_CTA][4];
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 #define CNB_STAT(x) x
 #else
 #define CNB_STAT(x)
@@ -1075,6 +1088,7 @@ k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ c
   static_assert(SEL_MASK_WORDS >= SEL_MAX_CTA, "s_fcnt must hold one count per candidate segment");
   static_assert(SEL_HIST_FINE == 64 * SEL_WARPS, "bootstrap derives one coarse bin per warp");
 
+  CNB_STAT(unsigned long long tm[4]; tm[0] = global_ns(); tm[1] = tm[2] = tm[3] = 0ull;)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int K = pl.K, C = pl.C;
   constexpr int HW = 128 * 128;
@@ -1112,6 +1126,13 @@ k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ c
     }
   };
 
+  // Programmatic dependent launch (launch_hot): the next launch on the stream may start as soon as every CTA of this
+  // one is resident; each of its CTAs then takes an SM as one of ours leaves it.  Before griddepcontrol.wait (in
+  // flush) a CTA only issues TMA loads of its map and sweeps them in shared memory: the map is never written by this
+  // kernel, and any other kernel between two hot launches does not trigger early, so plain stream order holds across
+  // it.  Segments, counts, thresholds, tickets and dets are touched only after the wait, i.e. after the previous
+  // launch has completed and its writes (its ticket resets included) are visible.
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (tid == 0) {
     s_flag[0] = s_flag[1] = s_flag[2] = s_flag[3] = 0;
     for (int s = 0; s < SEL_STAGES; ++s) {
@@ -1210,6 +1231,9 @@ k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ c
 
   // ---- CTA-wide flush of image `img` (all threads; called at image boundaries only)
   auto flush = [&](int img) {
+    // before the CTA's first global write or workspace read (see the launch note above); returns at once after the
+    // first flush
+    asm volatile("griddepcontrol.wait;" ::: "memory");
     __syncthreads();
     int n_out;
     if (s_cnt[1]) {
@@ -1274,7 +1298,11 @@ k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ c
     int ticket = 0;
     if (tid == 0) ticket = atomicAdd(&img_done[img], 1);   // in flight while the histogram is cleared
     clear_hist();
-    if (tid == 0) s_cnt[2] = (ticket == i1 - i0) ? 1 : 0;
+    if (tid == 0) {
+      s_cnt[2] = (ticket == i1 - i0) ? 1 : 0;
+      // last ticket: every other CTA of this image has drawn its own, so the ticket is free again for the next launch
+      if (s_cnt[2]) img_done[img] = 0;
+    }
     __syncthreads();
     if (s_cnt[2]) {  // every segment of this image is in global memory: merge + emit here
       __threadfence();
@@ -1373,7 +1401,7 @@ k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ c
     const T *st = stages + (size_t)stage * (128 * 128);
     CNB_STAT(st_q = clock64();)
     mbar_wait(&full[stage], (uint32_t)par);
-    CNB_STAT(st_wait += clock64() - st_q; st_q = clock64();)
+    CNB_STAT(st_wait += clock64() - st_q; st_q = clock64(); if (u == 0) tm[1] = global_ns();)
     if (*(volatile int *)&s_flag[u & 3]) compact(u & 3);   // set 3 units ago, before this plane's TMA was issued
     if (fresh) {
       // bootstrap (see header): histogram-only pass, K-th best of the plane, key pass
@@ -1410,7 +1438,7 @@ k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ c
       }
     }
     // next unit
-    CNB_STAT(st_q = clock64();)
+    CNB_STAT(st_q = clock64(); if (u == total_units - 1) tm[2] = global_ns();)
     if (++c == C) {
       flush(img);
       c = 0;
@@ -1432,6 +1460,9 @@ k_select_hot(const T *__restrict__ src, const SelectPlan pl, u64 *__restrict__ c
     unsigned int smid;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
     d[9] = smid;
+    tm[3] = global_ns();
+    unsigned long long *t = g_select_times[pl.stat_call % SEL_TIME_CALLS][me];
+    t[0] = tm[0]; t[1] = tm[1]; t[2] = tm[2]; t[3] = tm[3];
   }
 #endif
 }
@@ -1575,8 +1606,43 @@ static int launch_stage1(const float *src, const SelectPlan &pl, const FinalizeO
   return CNB_OK;
 }
 
+// Tickets of the hot kernel: one int per image, owned by the library per (device, stream) and zero between launches.
+// The CTA that draws an image's last ticket puts it back to 0, so every launch leaves the array as it found it and
+// the next launch on the stream needs no memset.  The array is made (and zeroed) on first use and replaced by a
+// larger zeroed one when a launch has more images; the old one is freed in stream order, so a launch still in flight
+// keeps its tickets.  Keyed by cudaStreamGetId, not the handle: the legacy and per-thread default streams have
+// fixed handles.
+static std::mutex g_ticket_mu;
+static std::map<std::pair<int, unsigned long long>, std::pair<int *, int>> g_tickets;   // -> (array, images)
+
+static int hot_tickets(int n_img, cudaStream_t stream, int **out) {
+  int dev = 0;
+  unsigned long long sid = 0;
+  CNB_CUDA(cudaGetDevice(&dev));
+  CNB_CUDA(cudaStreamGetId(stream, &sid));
+  std::lock_guard<std::mutex> lock(g_ticket_mu);
+  std::pair<int *, int> &t = g_tickets[std::make_pair(dev, sid)];
+  if (t.second < n_img) {
+    const int n = std::max(n_img, std::max(2 * t.second, 256));
+    int *p = nullptr;
+    CNB_CUDA(cudaMallocAsync(reinterpret_cast<void **>(&p), (size_t)n * 4, stream));
+    CNB_CUDA(cudaMemsetAsync(p, 0, (size_t)n * 4, stream));
+    if (t.first) CNB_CUDA(cudaFreeAsync(t.first, stream));
+    t = std::make_pair(p, n);
+  }
+  *out = t.first;
+  return CNB_OK;
+}
+
+#ifdef CNB_SELECT_STATS
+static std::atomic<int> g_hot_calls{0};   // hot launches so far (slot of the next one's timestamps)
+#endif
+
+// Launched with programmatic stream serialization: the kernel triggers its dependents at entry and waits for its
+// predecessor grid before its first global write or workspace read (k_select_hot), so the next call's CTAs take
+// each SM as this call's CTA leaves it and stream their planes under this call's tail.
 template <typename T>
-static int launch_hot(const void *src, const SelectPlan &pl, const FinalizeOut &out, u64 *cand, int *cnt, int *done,
+static int launch_hot(const void *src, const SelectPlan &pl, const FinalizeOut &out, u64 *cand, int *cnt,
                       uint32_t *thr, cudaStream_t stream) {
   constexpr size_t smem1 = hot_smem_bytes<T>();
   static thread_local int hot_dev = -1;
@@ -1587,9 +1653,30 @@ static int launch_hot(const void *src, const SelectPlan &pl, const FinalizeOut &
     CNB_CUDA(cudaFuncSetAttribute(k_select_hot<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
     hot_dev = dev;
   }
+  int *tickets = nullptr;
+  const int rc = hot_tickets(pl.n_img, stream, &tickets);
+  if (rc != CNB_OK) return rc;
   const T *s = reinterpret_cast<const T *>(src);
-  if (pl.logits) k_select_hot<T, true><<<pl.n_cta, SEL_THREADS, smem1, stream>>>(s, pl, cand, cnt, done, thr, out);
-  else k_select_hot<T, false><<<pl.n_cta, SEL_THREADS, smem1, stream>>>(s, pl, cand, cnt, done, thr, out);
+#ifdef CNB_SELECT_STATS
+  SelectPlan pl_ = pl;
+  pl_.stat_call = g_hot_calls.fetch_add(1);
+  const SelectPlan &plx = pl_;
+#else
+  const SelectPlan &plx = pl;
+#endif
+  void (*kern)(const T *, SelectPlan, u64 *, int *, int *, uint32_t *, FinalizeOut) =
+      pl.logits ? k_select_hot<T, true> : k_select_hot<T, false>;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(pl.n_cta);
+  cfg.blockDim = dim3(SEL_THREADS);
+  cfg.dynamicSmemBytes = smem1;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  CNB_CUDA(cudaLaunchKernelEx(&cfg, kern, s, plx, cand, cnt, tickets, thr, out));
   CNB_CHECK_LAUNCH("select stage 1 (hot)");
   count_launch();
   return CNB_OK;
@@ -1599,12 +1686,13 @@ template <bool NMS>
 static int launch_select(const void *src_v, int src_dtype, const SelectPlan &pl, const FinalizeOut &out, u64 *cand,
                          int *cnt, int *done, uint32_t *thr, cudaStream_t stream) {
   const float *src = reinterpret_cast<const float *>(src_v);   // every path but the hot one reads fp32
-  if (pl.fused_finalize) CNB_CUDA(cudaMemsetAsync(done, 0, (size_t)pl.n_img * 4, stream));
+  const bool hot = NMS && pl.hot;
+  if (pl.fused_finalize && !hot) CNB_CUDA(cudaMemsetAsync(done, 0, (size_t)pl.n_img * 4, stream));
   int rc;
-  if (NMS && pl.hot) {
-    if (src_dtype == CNB_DTYPE_BF16) rc = launch_hot<__nv_bfloat16>(src_v, pl, out, cand, cnt, done, thr, stream);
-    else if (src_dtype == CNB_DTYPE_F16) rc = launch_hot<__half>(src_v, pl, out, cand, cnt, done, thr, stream);
-    else rc = launch_hot<float>(src_v, pl, out, cand, cnt, done, thr, stream);
+  if (hot) {
+    if (src_dtype == CNB_DTYPE_BF16) rc = launch_hot<__nv_bfloat16>(src_v, pl, out, cand, cnt, thr, stream);
+    else if (src_dtype == CNB_DTYPE_F16) rc = launch_hot<__half>(src_v, pl, out, cand, cnt, thr, stream);
+    else rc = launch_hot<float>(src_v, pl, out, cand, cnt, thr, stream);
   } else if (NMS && pl.use_tma && pl.W == 128 && pl.H == 128 && pl.rb == 128)
     rc = launch_stage1<NMS, true, 2>(src, pl, out, cand, cnt, done, stream);
   else if (pl.use_tma && pl.ncb == 1)
@@ -1643,6 +1731,14 @@ int run_select(const void *src, const SelectPlan &pl, const FinalizeOut &out, vo
 #ifdef CNB_SELECT_STATS
 extern "C" int cnb_debug_select_stats(unsigned long long *out, int n_cta) {
   return cudaMemcpyFromSymbol(out, g_select_stats, sizeof(unsigned long long) * 10 * n_cta) == cudaSuccess ? 0 : 1;
+}
+// the whole timestamp ring, [SEL_TIME_CALLS][SEL_MAX_CTA][4]; returns the number of launches so far in *n_calls
+extern "C" int cnb_debug_select_times(unsigned long long *out, int *n_calls, int *ring, int *max_cta) {
+  *ring = SEL_TIME_CALLS;
+  *max_cta = SEL_MAX_CTA;
+  *n_calls = g_hot_calls.load();
+  if (out == nullptr) return 0;
+  return cudaMemcpyFromSymbol(out, g_select_times, sizeof(g_select_times)) == cudaSuccess ? 0 : 1;
 }
 #endif
 

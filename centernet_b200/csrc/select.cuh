@@ -40,6 +40,9 @@ struct SelectPlan {
   int wb;         // partition weight of an image boundary, in planes (flush + bootstrap + finalize cost)
   long long P;    // planes = n_img * C
   int cta_start[SEL_MAX_CTA + 1];  // first plane of every CTA's contiguous range (host-computed partition)
+#ifdef CNB_SELECT_STATS
+  int stat_call;  // tuning build: launch number of the hot kernel (slot of its per-CTA timestamps)
+#endif
 };
 
 // Raw top-K outputs ([n_img, K] each, any pointer may be null) plus the fused ctdet epilogue.

@@ -17,11 +17,24 @@
  *     contiguous, resident on the current device;
  *     index outputs use the reference's dtypes (int64 indices, int32 classes);
  *   - the caller owns every buffer, including the scratch `workspace`
- *     (size from the matching cnb_*_workspace_bytes); the library never calls
- *     cudaMalloc and keeps no global mutable state, so it may be called from
- *     one thread per GPU concurrently (torch DataParallel style);
+ *     (size from the matching cnb_*_workspace_bytes).  One exception: the hot
+ *     selection kernel (hot = 1 in cnb_select_plan_info; every decode of
+ *     128x128 maps with k <= 256 runs it) keeps per-stream ticket state, one
+ *     int per image in library-owned device memory for each (device, stream).
+ *     That array is allocated and zeroed in stream order on first use
+ *     (cudaMallocAsync), replaced by a larger one when a call has more images
+ *     (the old one freed in stream order), and every launch leaves it zero.
+ *     The library may be called from one thread per GPU concurrently (torch
+ *     DataParallel style), each thread on its own streams;
  *   - all work is enqueued on `stream` (a cudaStream_t passed as void*);
  *     nothing synchronises the host;
+ *   - the hot selection kernel is a programmatic dependent launch: it may start
+ *     while the previous hot selection on the same stream is still finishing.
+ *     Until that launch has completed it only reads its score map; its
+ *     outputs, workspace and tickets are touched after.  Work of any other
+ *     kernel enqueued before the call (a map written in place, say) completes
+ *     before it starts, as in plain stream order, since no other kernel lets
+ *     its dependents start early;
  *   - return value: CNB_OK or an error code; cnb_last_error() gives a
  *     thread-local description.  The reference's THArgCheck/THError
  *     (dcn_v2_cuda.c:20-38) map to CNB_EINVAL.
